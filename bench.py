@@ -1,6 +1,7 @@
-"""bench.py — throughput of the NaviLLM per-step hot path on synthetic batches, Vicuna-7B, bf16, on N B200s (one process per GPU).
+"""bench.py — throughput of the NaviLLM per-step hot path on synthetic batches, Vicuna-7B, bf16, on N H100s (one process per GPU).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload c2|c5|c3]   # this repo (sm_100a kernels)
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload c2|c5|c3]   # this repo (sm_90a kernels)
+    python bench.py ... --dump-outputs DIR                                      # + what the last timed step computed
     python bench.py --impl reference [...]                                      # the reference path on the host cores
 
 Workloads (BASELINE.json `configs`, SURVEY.md §8d):
@@ -21,9 +22,15 @@ result.  Multi-GPU: weak scaling, one batch per rank; the model is wrapped in na
 the timed region.
 
 The `--impl reference` arm and `cpu_baseline` time the CPU oracle port of the reference algorithm (oracle/navillm_oracle.py;
-kind "port": the reference is Python and /root/reference does not exist on the GPU box) on the host cores over a BOUNDED
+kind "port": the reference is Python and is not part of this repository) on the host cores over a BOUNDED
 sample: full-width Vicuna-7B layers, B=1, one prompt of the workload's mean length, 2 of the 32 layers, at most 3 timed
 passes and a hard wall-clock cap, whatever --steps says.
+
+`--dump-outputs DIR` writes, after the timed steps, what the timed path computed in its last step as DIR/<name>.npy
+(float32 / float64, finite): the loss and the navigation logits (training workloads; per micro-batch losses for c4) or the generated
+token ids (c3), plus a fixed, seeded sample of every parameter gradient.  The inputs depend only on the arguments (seeded
+synthetic batches, seeded initialisation) and every reduction of the path sums in a fixed order (no float atomics), so
+two runs of one build write identical files and two builds can be compared output for output.
 
 Progress goes to stderr, one line per phase, so a lost box is attributable; stdout carries exactly one JSON line.
 """
@@ -79,49 +86,62 @@ def log(msg: str) -> None:
     print(f"[bench +{time.time() - T0:6.1f}s rank{os.environ.get('RANK', '0')}] {msg}", file=sys.stderr, flush=True)
 
 
-def gemm_traffic():
-    """Average DRAM bytes per launch of the dominant kernel from the newest committed `ncu --set full` capture
-    (profiles/r0N_gemm2cta*_ncu_summary.json: dram__bytes_read.sum + dram__bytes_write.sum of GEMM launches inside a step)."""
-    cands = sorted((ROOT / "profiles").glob("r0*_gemm2cta*_ncu_summary.json"))
-    if not cands:
-        return None, None
-    p = cands[-1]
-    unit = {"Gbyte": 1e9, "Mbyte": 1e6, "Kbyte": 1e3, "byte": 1.0}
-    tot, n = 0.0, 0
-    for k in json.loads(p.read_text())["kernels"]:
-        b = 0.0
-        for key in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-            v, u = k[key].split()
-            b += float(v) * unit[u]
-        tot += b
-        n += 1
-    return (tot / n if n else None), f"mean over {n} captured launches, {p.name}"
-
-
-def decode_traffic(n_layers: int):
-    """DRAM bytes of one decode step from the committed `ncu --set full` capture of the decode kernels
-    (profiles/r0N_decode_ncu_summary.json): the first five captured launches are one layer's set in stream order (o_proj,
-    gate|up + SwiGLU, down_proj, next layer's qkv, decode attention; the row kernels move < 1 MB); lm_head is added at its
-    algorithmic size."""
-    cands = sorted((ROOT / "profiles").glob("r0*_decode_ncu_summary.json"))
-    if not cands:
-        return None, None
-    unit = {"Gbyte": 1e9, "Mbyte": 1e6, "Kbyte": 1e3, "byte": 1.0}
-    ks = json.loads(cands[-1].read_text())["kernels"][:5]
-    per_layer = 0.0
-    for k in ks:
-        for key in ("dram_read", "dram_write"):
-            v, u = k[key].split()
-            per_layer += float(v) * unit[u]
-    return per_layer * n_layers + 2.0 * (VOCAB + 6) * D_MODEL, f"{cands[-1].name}: 5 launches = one layer, x{n_layers} + lm_head"
-
-
 def peaks():
     p = ROOT / "MEASURED_PEAKS.json"
     if p.exists():
         j = json.loads(p.read_text())
         return {"bf16_tflops": j.get("bf16_tflops_sustained", j.get("bf16_tflops")), "hbm_gbs": j.get("hbm_gbs"), "src": "measured"}
-    return {"bf16_tflops": 1400.0, "hbm_gbs": 6650.0, "src": "fallback"}
+    # NVIDIA H100 SXM data sheet (dense bf16, HBM3), for a card allowed 700 W: an upper bound, not a measured rate
+    return {"bf16_tflops": 989.0, "hbm_gbs": 3350.0, "src": "H100 SXM data sheet"}
+
+
+def gpu_info(index: int) -> dict:
+    """Which card the numbers of this run were measured on, and its power limit."""
+    info = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", str(index)],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+        info["power_limit_w"] = float(out.splitlines()[0])
+    except Exception:
+        pass
+    return info
+
+
+DUMP_GRAD_SAMPLE = 4096      # gradient elements sampled per parameter tensor by --dump-outputs
+
+
+def dump_outputs(out_dir, arrays: dict, model=None) -> None:
+    """--dump-outputs: arrays (name -> tensor / ndarray) as DIR/<name>.npy in float32 (float64 stays float64), plus
+    `grad_sample.npy`: DUMP_GRAD_SAMPLE elements of every parameter gradient at indices drawn from a generator seeded
+    with the parameter's position (the same elements in every run), concatenated in parameter order.  Every file holds
+    finite numbers: an array with non-finite entries (the -inf of masked navigation slots) is written with those entries
+    set to 0, next to `<name>_finite.npy` (1 where the value was finite, 0 where not)."""
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    total = 0
+    if model is not None:
+        parts = []
+        for i, p in enumerate(model.parameters()):
+            if p.grad is None:
+                continue
+            flat = p.grad.detach().reshape(-1)
+            idx = torch.randint(flat.numel(), (min(DUMP_GRAD_SAMPLE, flat.numel()),), generator=torch.Generator().manual_seed(i))
+            parts.append(flat[idx.to(flat.device)].float().cpu())
+        if parts:
+            arrays = dict(arrays, grad_sample=torch.cat(parts))
+    for name, v in arrays.items():
+        a = v.detach().cpu().numpy() if torch.is_tensor(v) and v.dtype != torch.bfloat16 else (
+            v.detach().float().cpu().numpy() if torch.is_tensor(v) else np.asarray(v))
+        a = a.astype(np.float64 if a.dtype == np.float64 else np.float32)
+        fin = np.isfinite(a)
+        if not fin.all():
+            np.save(d / f"{name}_finite.npy", fin.astype(np.float32))
+            total += fin.size * 4
+            a = np.where(fin, a, 0).astype(a.dtype)
+        total += a.nbytes
+        np.save(d / f"{name}.npy", a)
+    assert total <= 64 << 20, f"--dump-outputs wrote {total} bytes (> 64 MB)"
+    log(f"outputs of the last timed step written to {d} ({total} bytes)")
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -193,8 +213,9 @@ def build_model(dev, seed=0):
     return model
 
 
-def nav_step(model, dev_in, meta, dev, text=None):
-    """One batch of navigation steps through the public API; returns the loss tensor (on device)."""
+def nav_step(model, dev_in, meta, dev, text=None, outputs=None):
+    """One batch of navigation steps through the public API; returns the loss tensor (on device).  With `outputs` (a dict)
+    the navigation logits are kept there as well."""
     B = dev_in["view_img_fts"].shape[0]
     n_hist = dev_in["hist_vis"].shape[1]
     pano = model("panorama", {"view_img_fts": dev_in["view_img_fts"], "view_lens": meta["view_lens"], "loc_fts": dev_in["loc_fts"],
@@ -214,6 +235,8 @@ def nav_step(model, dev_in, meta, dev, text=None):
     out = model("navigation", batch)
     loss = torch.nn.functional.cross_entropy(out["fuse_logits"].float(), dev_in["target_cols"], reduction="sum",
                                              ignore_index=-100) / B                               # mp3d_agent.py:750
+    if outputs is not None:
+        outputs["fuse_logits"] = out["fuse_logits"]
     return loss
 
 
@@ -512,14 +535,18 @@ def run_train(a, rank, local_rank, world, dev):
     if fwd_only:
         core_model.eval()
 
+    last = {}                                              # outputs of the latest resident step (--dump-outputs)
+
     def step_resident():
         if fwd_only:
             with torch.no_grad():
-                return nav_step(model, resident, meta, dev, text=text)
+                last["loss"] = nav_step(model, resident, meta, dev, text=text, outputs=last)
+                return last["loss"]
         core_model.zero_grad(lazy=True)
         with sync_ctx():
-            loss = nav_step(model, resident, meta, dev, text=text)
+            loss = nav_step(model, resident, meta, dev, text=text, outputs=last)
             loss.backward()                                # N > 1: the flat-gradient exchange fires from this backward
+        last["loss"] = loss
         return loss
 
     def step_e2e():
@@ -552,6 +579,9 @@ def run_train(a, rank, local_rank, world, dev):
     gemm_bytes = sum(t[3] for t in timer)
     n_gemm = len(timer)
     log(f"timed region done: {ms / a.steps:.1f} ms/step")
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, {"loss": last["loss"].double(), "fuse_logits": last["fuse_logits"]},
+                     None if fwd_only else core_model)
 
     if a.profile:
         if rank == 0:
@@ -570,7 +600,6 @@ def run_train(a, rank, local_rank, world, dev):
         # algorithmic FLOPs of the whole step on REAL (non-pad) tokens (SURVEY.md §8d): 3 x (12.952 GF/token + attention)
         lens = np.asarray(text["attention_mask"].sum(1), dtype=np.float64)
         algo_step = (1.0 if fwd_only else 3.0) * (float((lens * 12.952e9 + 0.262144e6 * lens * lens).sum()) + 2.229e9 * B)
-        traffic, traffic_src = gemm_traffic()
         st = core_model.grad_sync.stats
         line = {
             "metric": "nav_steps_per_sec", "value": value, "unit": "nav-steps/s", "n_gpus": world, "steps": a.steps, "warmup": a.warmup,
@@ -585,11 +614,11 @@ def run_train(a, rank, local_rank, world, dev):
                        "zero_grad": "lazy (first wgrad of a step overwrites: beta=0)", "optimizer_step": "outside the boundary (train.py:86-89), not timed"},
             "e2e": {"value": e2e, "unit": "nav-steps/s", "h2d_bytes_per_step": int(h2d_bytes), "d2h_bytes_per_step": 4,
                     "ms_per_step": ms_e2e / a.steps},
-            "gpu_launches": int(launches),
-            "roofline": {"bound": "tensor", "kernel": "gemm_bf16_tcgen05_2cta (cta_group::2; skinny launches use gemm_bf16_tcgen05)", "achieved": achieved, "peak": pk["bf16_tflops"], "unit": "TFLOP/s",
-                         "frac": (achieved / pk["bf16_tflops"]) if achieved else None, "peak_src": pk["src"] + " (sustained cuBLAS bf16)",
+            "gpu_launches": int(launches), "gpu": gpu_info(local_rank),
+            "roofline": {"bound": "tensor", "kernel": "gemm_bf16_wgmma (128 x 256 and 128 x 128 tiles)", "achieved": achieved, "peak": pk["bf16_tflops"], "unit": "TFLOP/s",
+                         "frac": (achieved / pk["bf16_tflops"]) if achieved else None, "peak_src": pk["src"],
                          "launches_per_step": n_gemm // max(a.steps, 1), "share_of_step": gemm_ms / ms,
-                         "traffic": traffic, "traffic_unit": "bytes/launch (DRAM read+write)", "traffic_src": traffic_src,
+                         "traffic": None, "traffic_unit": "bytes/launch (DRAM read+write)", "traffic_src": "not measured",
                          "algorithmic_bytes_per_launch_mean": gemm_bytes / max(n_gemm, 1),
                          "step_algorithmic_tflop": algo_step / 1e12,
                          "step_frac_of_peak": algo_step / 1e12 / (ms / a.steps / 1e3) / pk["bf16_tflops"]},
@@ -674,16 +703,20 @@ def run_mixed(a, rank, local_rank, world, dev):
             return out.loss.float()
         yield qa
 
+    losses = []                                         # micro-batch losses of the latest step (--dump-outputs)
+
     def step(up, read):
         core_model.zero_grad(lazy=True)
         mbs = list(micro_batches(up))
         total = 0.0
+        losses.clear()
         for i, mb in enumerate(mbs):
             last = i == len(mbs) - 1
             ctx = contextlib.nullcontext() if ((last and do_sync) or world == 1) else model.no_sync()
             with ctx:                                   # tasks/agents/mp3d_agent.py:661-667: only the last backward exchanges
                 loss = mb()
                 loss.backward()
+            losses.append(loss.detach())
             if read:
                 total += float(loss.detach())
         return total
@@ -707,6 +740,8 @@ def run_mixed(a, rank, local_rank, world, dev):
         ms = timed(lambda: step(up_resident, False), a.steps, world, dev)
     launches = (_lib.launch_count - launches0) // max(a.steps, 1)
     log(f"timed region done: {ms / a.steps:.1f} ms/step")
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, {"micro_batch_losses": torch.stack([x.double() for x in losses])}, core_model)
     if a.profile:
         if rank == 0:
             print(json.dumps({"profile_run": True, "ms_per_step": ms / a.steps, "launches": int(launches)}))
@@ -730,10 +765,10 @@ def run_mixed(a, rank, local_rank, world, dev):
                                              + ("NVLS in-switch all-reduce" if getattr(model, "nvls", False) else "NCCL")) if world > 1 else "n/a"},
                 "e2e": {"value": world * B * a.steps / (ms_e2e / 1e3), "unit": "samples/s", "h2d_bytes_per_step": int(h2d_bytes),
                         "d2h_bytes_per_step": 4 * 4, "ms_per_step": ms_e2e / a.steps},
-                "gpu_launches": int(launches),
+                "gpu_launches": int(launches), "gpu": gpu_info(local_rank),
                 "roofline": {"bound": "tensor", "kernel": "whole step (algorithmic FLOPs of the four micro-batches on real tokens)",
                              "achieved": algo_step / 1e12 / (ms / a.steps / 1e3), "peak": pk["bf16_tflops"], "unit": "TFLOP/s",
-                             "frac": algo_step / 1e12 / (ms / a.steps / 1e3) / pk["bf16_tflops"], "peak_src": pk["src"] + " (sustained cuBLAS bf16)",
+                             "frac": algo_step / 1e12 / (ms / a.steps / 1e3) / pk["bf16_tflops"], "peak_src": pk["src"],
                              "step_algorithmic_tflop": algo_step / 1e12, "traffic": None},
                 "clocks": clk.summary()}
         if not a.no_cpu_baseline and world == 1:
@@ -790,15 +825,17 @@ def run_generate(a, rank, local_rank, world, dev):
     torch.cuda.synchronize()
     launches0 = _lib.launch_count
     log(f"timed region: {a.steps} generations")
-    per = []
+    per, last = [], {}
     with ClockSampler(local_rank) as clk:
         def one():
             s = {}
-            step_resident(s)
+            last["out"] = step_resident(s)
             per.append(s)
         ms = timed(one, a.steps, world, dev)
     launches = (_lib.launch_count - launches0) // max(a.steps, 1)
     log(f"timed region done: {ms / a.steps:.1f} ms per generation")
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, {"token_ids": last["out"].double()})      # [B, S0 + new] ids
     if a.profile:
         if rank == 0:
             print(json.dumps({"profile_run": True, "ms_per_step": ms / a.steps, "launches": int(launches)}))
@@ -828,11 +865,11 @@ def run_generate(a, rank, local_rank, world, dev):
                        "step_includes": "prefill + first token + 127 CUDA-graph replays (graph captured once per shape, in the warm-up)"},
             "e2e": {"value": e2e, "unit": "tokens/s", "h2d_bytes_per_step": int(h2d), "d2h_bytes_per_step": int(B * (S0 + NEW) * 8),
                     "ms_per_step": ms_e2e / a.steps, "path": "model('3dqa', batch, training=False): panorama encoder + tokenisation + generate + batch_decode"},
-            "gpu_launches": int(launches),
-            "roofline": {"bound": "hbm", "kernel": "decode step (CUDA graph: gemm_skinny_tcgen05 x4/layer + rmsnorm/rope-kv/decode_attn)", "achieved": achieved,
+            "gpu_launches": int(launches), "gpu": gpu_info(local_rank),
+            "roofline": {"bound": "hbm", "kernel": "decode step (CUDA graph: gemm_skinny_wgmma x4/layer + rmsnorm/rope-kv/decode_attn)", "achieved": achieved,
                          "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": (achieved / pk["hbm_gbs"]) if achieved else None, "peak_src": pk["src"],
-                         "algorithmic_bytes_per_token_step": bytes_tok, "traffic": decode_traffic(a.layers)[0],
-                         "traffic_unit": "bytes per decode step (DRAM read+write)", "traffic_src": decode_traffic(a.layers)[1]},
+                         "algorithmic_bytes_per_token_step": bytes_tok, "traffic": None,
+                         "traffic_unit": "bytes per decode step (DRAM read+write)", "traffic_src": "not measured"},
             "clocks": clk.summary(),
         }
         if not a.no_cpu_baseline and world == 1:
@@ -858,6 +895,8 @@ def main():
     ap.add_argument("--grad-sync", default="overlap", choices=["overlap", "end", "none"],
                     help="debug only (N>1): 'end' = exchange at the end of the backward only, 'none' = no exchange => number is INVALID")
     ap.add_argument("--profile", action="store_true", help="for runs under ncu: no e2e / cpu arms, any warm-up count; the printed number is not a bench value")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed as DIR/<name>.npy (see the module docstring)")
     a = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))

@@ -1,4 +1,4 @@
-/* navillm_b200 — C ABI of the B200-native NaviLLM hot path (libnavillm_b200.so, sm_100a only).
+/* navillm_b200 — C ABI of the native NaviLLM hot path (libnavillm_b200.so, sm_90a / H100 only).
  *
  * The reference (zd11024/NaviLLM) is pure Python/PyTorch and has NO native interface of its own: its
  * "operator API" for this path is the set of torch calls made inside NavModel.forward() and below
@@ -11,7 +11,7 @@
  *   - the library allocates nothing on the device: outputs and workspaces are caller-owned;
  *   - return value: 0 = ok; negative = argument / environment error (NV_ERR_*); positive = cudaError_t.
  *     nv_last_error() returns a thread-local message for the last failure;
- *   - there is NO CPU fallback: without an sm_100 device every compute entry fails (NV_ERR_NO_DEVICE or a
+ *   - there is NO CPU fallback: without an sm_90 device every compute entry fails (NV_ERR_NO_DEVICE or a
  *     CUDA error), it never computes on the host;
  *   - bf16 tensors are row-major with 16-byte aligned rows (leading dimensions multiples of 8 elements).
  */
@@ -41,24 +41,24 @@ int nv_abi_version(void);
  * cudaLaunchAttributeProgrammaticStreamSerialization so a kernel's prologue (and the skinny GEMM's first weight tiles)
  * overlaps the tail of its predecessor.  Returns the previous setting.  Process-wide; default off. */
 int nv_set_pdl(int on);
-int nv_device_check(void); /* NV_OK iff the current device is sm_100-class */
+int nv_device_check(void); /* NV_OK iff the current device is sm_90 (Hopper) */
 int nv_sm_count(void);
 
-/* ---- tcgen05 bf16 GEMM (csrc/gemm_bf16.cu) -----------------------------------------------------------
+/* ---- wgmma bf16 GEMM (csrc/gemm_bf16.cu) -------------------------------------------------------------
  * C[M,N] = A·B (+addend).  a_mn=0: A is [M,K]; a_mn=1: A is [K,M].  b_mn=0: B is [N,K] (nn.Linear weight);
  * b_mn=1: B is [K,N].  Replaces every nn.Linear of the LLaMA block and lm_head and their autograd dgrad /
  * wgrad: models/modified_lm.py:112-116 (HF LlamaDecoderLayer q/k/v/o/gate/up/down_proj) and :120 (lm_head).
- * block_n: 0 (auto), 128 or 256. */
+ * block_n: 0 (auto), 32 (M <= 128, K-major B), 128 or 256 (output tile 128 x block_n). */
 int nv_gemm_bf16(const void* A, int64_t lda, int a_mn, const void* B, int64_t ldb, int b_mn, void* C, int64_t ldc,
                  const void* addend, int64_t ld_add, int M, int N, int K, unsigned flags, int block_n, void* stream);
 
-/* Fused-epilogue forms on the CTA-pair kernel (csrc/gemm_bf16_2cta.cu), bit-identical to the unfused sequences:
+/* Fused-epilogue forms on the 128 x 256 tile (csrc/gemm_bf16.cu), bit-identical to the unfused sequences:
  *   nv_gemm_swiglu_bf16   gu = x Wgu^T and h = silu(gate)*up        (HF LlamaMLP: act_fn(gate_proj(x)) * up_proj(x))
  *   nv_gemm_dswiglu_bf16  dgu = swiglu'(gu) o (dx Wd)               (autograd of the above through down_proj)
  *   nv_gemm_rope_bf16     qkv = x Wqkv^T with rotate-half RoPE on the q,k columns (HF apply_rotary_pos_emb)
  *   nv_gemm_attnd_bf16    dO = dY Wo (o_proj dgrad) and D[h,t] = sum_d dO O of the attention backward (same values as
  *                         the separate row-sum kernel up to fp32 summation order) */
-/* Decode-step GEMM (M <= 16 rows, reference: HF generate through models/modified_lm.py:184-199): swap-AB tcgen05
+/* Decode-step GEMM (M <= 16 rows, reference: HF generate through models/modified_lm.py:184-199): swap-AB wgmma
  * kernel with the K range split over a thread-block cluster and reduced through distributed shared memory
  * (csrc/gemm_skinny.cu).  C = bf16(bf16(X W^T) + addend), X [M,K], W [N,K] (nn.Linear layout). */
 int nv_gemm_skinny_bf16(const void* X, int64_t ldx, const void* W, int64_t ldw, void* C, int64_t ldc, const void* addend,
@@ -93,9 +93,8 @@ int nv_attn_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const vo
                 int64_t ldo, const void* dout, int64_t lddo, const float* lse, float* dvec, void* dq, int64_t lddq,
                 void* dk, int64_t lddk, void* dv, int64_t lddv, const int* cu_seqlens, int B, int T, int H, int head_dim,
                 int total_blocks, float scale, const int* rope_pos, const void* cos_t, const void* sin_t, void* stream);
-/* Developer hook (no reference counterpart): per-CTA SM-clock phase trace of the last nv_attn_bwd (kernel 0 = dk/dv
- * pass, 1 = dq pass) or nv_attn_fwd (kernel 2).  Returns the number of 64-bit words copied, 0 unless built with -DNV_ATTN_TRACE
- * (tools/attn_trace.py). */
+/* Developer hook (no reference counterpart) for an in-kernel phase trace of the attention kernels.  The sm_90a kernels
+ * record none: returns 0 (words copied). */
 int nv_debug_attn_trace(int kernel, unsigned long long* out, int max_words);
 
 /* ---- row-wise LM kernels (csrc/lm_ops.cu) ---------------------------------------------------------------
@@ -136,7 +135,7 @@ int nv_ce_fwd_bwd(const void* logits, int64_t ld, const int* labels, const int* 
  * scatter glue of NavModel.forward_navigation (models/nav_model.py:146-224), forward and backward. */
 int nv_sgemm(const float* A, int64_t lda, int ta, const float* B, int64_t ldb, int tb, float* C, int64_t ldc,
              const float* bias, int M, int N, int K, int accumulate, void* stream);
-/* Same contract on the tensor cores (tcgen05 kind::tf32, fp32 accumulate; csrc/gemm_tf32.cu): the numerical mode the
+/* Same contract on the tensor cores (wgmma tf32, fp32 accumulate; csrc/gemm_tf32.cu): the numerical mode the
  * reference's pinned torch 1.10 (allow_tf32 = True by default, requirements.txt:19) used for these fp32 nn.Linear
  * layers.  Needs 16-byte aligned bases and lda/ldb % 4 == 0; other shapes go to nv_sgemm. */
 int nv_gemm_tf32(const float* A, int64_t lda, int ta, const float* B, int64_t ldb, int tb, float* C, int64_t ldc,

@@ -1,4 +1,4 @@
-"""Build the navillm_b200 C-ABI shared library (sm_100a only) with nvcc, in-tree.
+"""Build the navillm_b200 C-ABI shared library (sm_90a only) with nvcc, in-tree.
 
     python -m navillm_b200.build [--force] [--verbose]
 
@@ -23,12 +23,12 @@ LIBDIR = PKG / "lib"
 OBJDIR = PKG / "lib" / "obj"
 LIB = LIBDIR / "libnavillm_b200.so"
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [
     "-O3", "-std=c++17", "-lineinfo", "--use_fast_math", "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr", "-Xptxas", "-v", "-DNDEBUG",
 ]
-# developer-only extra flags (e.g. NV_NVCC_EXTRA="-DNV_ATTN_TRACE" for the in-kernel phase trace of tools/attn_trace.py)
+# developer-only extra flags (e.g. NV_NVCC_EXTRA="-DNV_MBAR_TIMEOUT_CYCLES=1000000000")
 NVCC_FLAGS += os.environ.get("NV_NVCC_EXTRA", "").split()
 
 
@@ -36,7 +36,7 @@ def _nvcc() -> str:
     for cand in (os.environ.get("NVCC"), shutil.which("nvcc"), "/usr/local/cuda/bin/nvcc"):
         if cand and Path(cand).exists():
             return cand
-    raise RuntimeError("nvcc not found (needed to build navillm_b200 for sm_100a)")
+    raise RuntimeError("nvcc not found (needed to build navillm_b200 for sm_90a)")
 
 
 def _sources() -> list[Path]:

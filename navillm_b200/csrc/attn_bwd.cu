@@ -1,4 +1,4 @@
-// navillm_b200 — causal self-attention backward on tcgen05 (packed variable-length rows), pipelined.
+// navillm_b200 — causal self-attention backward on Hopper wgmma (packed variable-length rows), pipelined.
 //
 // Hand-written twin of attn_fwd.cu; replaces the autograd backward of HF LLaMA's eager attention
 // (reference: loss.backward() call sites tasks/agents/mp3d_agent.py:750-757, tasks/agents/llava.py:38-40
@@ -6,43 +6,31 @@
 //
 // With P = exp(S*scale - LSE), D_i = sum_d dO_id O_id, dS = P o (dP - D) * scale:
 //     dV = P^T dO      dK = dS^T Q      dQ = dS K
-// Two deterministic passes (no atomics).  Both walk the partner dimension in 64-wide SUB-blocks so that the
-// score tiles are only 64 TMEM columns and can be double-buffered: the tensor pipe computes the scores of
-// sub-block n+1 while the compute warps turn sub-block n into P / dS and the accumulate MMAs of n run.
+// Two deterministic passes (no atomics).  Both walk the partner dimension in 64-wide sub-blocks streamed by TMA
+// through a 4-stage ring; two warpgroups own 64 rows each of the CTA's 128-row block, keep
+// their accumulators in registers and feed P / dS back into the tensor cores from registers (the wgmma
+// A-from-registers form: a score accumulator is laid out like an A fragment).
 //
-//   dq pass   CTA = (128-query block, head).  Q,dO resident; K_n,V_n [64 keys x 128] streamed (3 stages).
-//             S = Q K_n^T, dP = dO V_n^T  [128 q x 64 keys] -> dS (bf16, K-major A operand) -> dQ += dS K_n.
-//             TMEM: S[2] dP[2] (4 x 64 columns) + dQ (128).
-//   dkdv pass CTA = (128-key block, head).  K,V resident; Q_n,dO_n [64 queries x 128] streamed (2 stages).
-//             TRANSPOSED scores so that TMEM lanes are keys: S^T = K Q_n^T, dP^T = V dO_n^T [128 keys x 64 q]
-//             -> P^T, dS^T (bf16, K-major A operands) -> dV += P^T dO_n, dK += dS^T Q_n.
-//             TMEM: S^T[2] dP^T[2] (4 x 64) + dV (128) + dK (128) = 512 columns.
-// Roles: warp 0 TMA producer, warp 1 MMA issuer, warps 2..9 compute (two warps per TMEM lane quarter, each owning
-// 32 of the 64 score columns; no row reductions are needed in the backward: LSE and D are precomputed).
-// The inverse rotary embedding of dQ / dK is applied in the epilogue (optional).
+//   dq pass   CTA = (128-query block, head).  Q,dO resident; K_n,V_n [64 keys x 128] streamed.
+//             S = Q K_n^T, dP = dO V_n^T  [64 q x 64 keys per warpgroup] -> dS (bf16, registers) -> dQ += dS K_n.
+//   dkdv pass CTA = (128-key block, head).  K,V resident; Q_n,dO_n [64 queries x 128] streamed.
+//             TRANSPOSED scores so that accumulator rows are keys: S^T = K Q_n^T, dP^T = V dO_n^T [64 keys x 64 q]
+//             -> P^T, dS^T (bf16, registers) -> dV += P^T dO_n, dK += dS^T Q_n.
+// Threads: warps 0..7 (warpgroups 0, 1); thread 0 also issues the TMA loads (a producer warp as a ninth warp would put
+// three warps on one SM sub-partition and cap the dk/dv pass below the registers its two accumulators need).  No row
+// reductions are needed in the backward: LSE and D are precomputed.  The inverse rotary embedding of dQ / dK is applied in the epilogue (optional).
 #include "nv_common.cuh"
 #include "nv_host.h"
 
 namespace nv {
 
-constexpr uint32_t AB_THREADS = 320;
+constexpr uint32_t AB_THREADS = 256;
 constexpr uint32_t AB_T128 = 128 * 128 * 2;  // [128 rows x 128 hd] bf16 = two 16 KB swizzle atoms (hd halves)
 constexpr uint32_t AB_A128 = 128 * 128;      // one atom of a 128-row tile
 constexpr uint32_t AB_T64 = 64 * 128 * 2;    // [64 rows x 128 hd] bf16 = two 8 KB atoms
 constexpr uint32_t AB_A64 = 64 * 128;        // one atom of a 64-row tile
-constexpr uint32_t AB_PS = 128 * 64 * 2;     // [128 rows x 64 cols] bf16 = one 16 KB atom (P / dS operands)
+constexpr uint32_t AB_NST = 4;               // streamed sub-block stages
 constexpr float LOG2E = 1.4426950408889634f;
-
-// Developer phase trace (compiled in only with -DNV_ATTN_TRACE, see tools/attn_trace.py): SM-clock stamps of the
-// pipeline events of the CTAs of one head, read back through nv_debug_attn_trace().
-#ifdef NV_ATTN_TRACE
-__device__ unsigned long long g_attn_trace[2][256 * 64];
-#define AB_TR(k, slot) do { if (blockIdx.y == 5 && blockIdx.x < 256) g_attn_trace[k][blockIdx.x * 64 + (slot)] = clock64(); } while (0)
-#define AB_TRV(k, slot, v) do { if (blockIdx.y == 5 && blockIdx.x < 256) g_attn_trace[k][blockIdx.x * 64 + (slot)] = (v); } while (0)
-#else
-#define AB_TR(k, slot) do {} while (0)
-#define AB_TRV(k, slot, v) do {} while (0)
-#endif
 
 __device__ __forceinline__ bool locate_block_bwd(const int* __restrict__ cu, int B, uint32_t blk, int& seq_start,
                                                  int& seq_len, uint32_t& idx) {
@@ -84,35 +72,28 @@ __device__ __forceinline__ void load_tile(uint8_t* dst, const CUtensorMap* m, ui
       tma_load_2d(dst + a * ATOM + r * (64 * 128), m, bar, col + a * 64, row + r * 64);
 }
 
-// Epilogue shared by both passes, in two phases so that HBM sees full 256-byte rows (a row-per-thread store - what the
-// TMEM lane mapping suggests - touches 32 different rows per instruction and, with the per-row cos/sin loads of the fused
-// inverse RoPE, cost 7.5k of a dk/dv CTA's ~28k cycles in the in-kernel trace):
-//   stage_acc_tile   thread = accumulator row: tcgen05.ld its 2 x 32 columns (chunks c0 and c0 + 64), round to bf16,
-//                    write them into a padded row-major smem tile (272-byte rows: conflict-free 16-byte stores);
+// Epilogue shared by both passes, in two phases so that HBM sees full 256-byte rows (a row-per-thread store would touch
+// many rows per instruction, with per-row cos/sin loads for the fused inverse RoPE on top):
+//   stage_acc_tile   the warpgroup's 64 x 128 fp32 accumulator, rounded to bf16, into a padded row-major smem tile
+//                    (272-byte rows);
 //   flush_acc_tile   warp = row: lane l owns columns 4l..4l+3, its rotate-half partner sits in lane l^16; optional
 //                    rotation by -theta[pos] with the rounding points of rope_kernel(sign = -1); 8-byte coalesced stores.
-// The 8 compute warps synchronise on named barrier 1 between the phases; the staging buffers are operand stages that
-// are free once the `done` barrier has fired.
+// The 8 compute warps synchronise on named barrier 1 before staging (every operand stage is then free) and between
+// the phases.
 constexpr uint32_t AB_STAGE_LD = 272;                        // bytes per staged row (256 + 16 padding)
 constexpr uint32_t AB_STAGE_BYTES = 128 * AB_STAGE_LD;       // 34 816 B per accumulator
 
-__device__ __forceinline__ void compute_warps_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+__device__ __forceinline__ void compute_warps_sync() { named_bar_sync(1, 256); }
 
-__device__ __forceinline__ void stage_acc_tile(uint32_t tm, uint32_t lane_off, uint32_t c0, uint32_t r, uint8_t* stage) {
-  uint32_t a[32], b[32];
-  tmem_ld_32x32b_x32(tm + lane_off + c0, a);
-  tmem_ld_32x32b_x32(tm + lane_off + c0 + 64, b);
-  tmem_ld_wait();
-  uint8_t* row = stage + r * AB_STAGE_LD;
+// wg: warpgroup (rows 64 wg ..), acc: its accumulator fragment (rows r, r + 8; columns 8 i + 2 (lane % 4) + {0, 1})
+__device__ __forceinline__ void stage_acc_tile(const float (&acc)[64], uint32_t wg, uint8_t* stage) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t r = wg * 64 + ((threadIdx.x & 127) >> 5) * 16 + (lane >> 2);
 #pragma unroll
-  for (uint32_t i = 0; i < 32; i += 8) {
-    uint4 o1, o2;
-    o1.x = pack_bf16x2(__uint_as_float(a[i]), __uint_as_float(a[i + 1]));     o1.y = pack_bf16x2(__uint_as_float(a[i + 2]), __uint_as_float(a[i + 3]));
-    o1.z = pack_bf16x2(__uint_as_float(a[i + 4]), __uint_as_float(a[i + 5])); o1.w = pack_bf16x2(__uint_as_float(a[i + 6]), __uint_as_float(a[i + 7]));
-    o2.x = pack_bf16x2(__uint_as_float(b[i]), __uint_as_float(b[i + 1]));     o2.y = pack_bf16x2(__uint_as_float(b[i + 2]), __uint_as_float(b[i + 3]));
-    o2.z = pack_bf16x2(__uint_as_float(b[i + 4]), __uint_as_float(b[i + 5])); o2.w = pack_bf16x2(__uint_as_float(b[i + 6]), __uint_as_float(b[i + 7]));
-    *reinterpret_cast<uint4*>(row + (c0 + i) * 2) = o1;
-    *reinterpret_cast<uint4*>(row + (c0 + 64 + i) * 2) = o2;
+  for (uint32_t i = 0; i < 16; ++i) {
+    const uint32_t c = 8 * i + 2 * (lane & 3);
+    *reinterpret_cast<uint32_t*>(stage + r * AB_STAGE_LD + c * 2) = pack_bf16x2(acc[4 * i], acc[4 * i + 1]);
+    *reinterpret_cast<uint32_t*>(stage + (r + 8) * AB_STAGE_LD + c * 2) = pack_bf16x2(acc[4 * i + 2], acc[4 * i + 3]);
   }
 }
 
@@ -142,34 +123,67 @@ __device__ __forceinline__ void flush_acc_tile(const uint8_t* stage, uint32_t cw
   }
 }
 
-// ======================================================================================================
-// dq pass -- A operands in TENSOR MEMORY (tcgen05.mma ".ts" form)
-// ======================================================================================================
-// Round 1 ran this pass with every operand in shared memory and measured it smem-bandwidth-bound: 176 KB of shared-memory
-// traffic per 64-key sub-block (1375 cycles at 128 B/clk) against 768 tensor cycles, ~1550 measured (in-kernel trace).
-// Q and dO are the A operands of EVERY score MMA of the CTA, and dS is produced by the compute warps from TMEM data:
-//   * Q, dO  are written once into TMEM as bf16 (2 x 64 columns): TMA stages the two tiles in shared memory, each compute
-//            thread copies half of its own row (a row-per-thread load straight from HBM cost 5300 cycles of prologue)
-//   * dS(n)  is written with tcgen05.st straight over the S(n) columns it was computed from (no smem store, no
-//            fence.proxy.async), laid out so that every warp overwrites only columns it has already read
-// so per sub-block only the B operands (K_n, V_n: 48 KB) and the TMA fills (32 KB) touch shared memory, and the N = 64 score
-// MMAs run at their 32-cycle tensor floor instead of 48.
-//   TMEM: S[2] [0,128)  dP[2] [128,256)  dQ [256,384)  Q [384,448)  dO [448,512);  dS(n) aliases S[n & 1].
-//   smem: Q | dO staging (64 KB, once; the epilogue stages dQ there) + 5 stages of (K_n 16 KB | V_n 16 KB).  With the
-//   sub-block time down to ~800 cycles a 3-stage ring left only two sub-blocks (< the ~2000-cycle TMA latency) between a
-//   stage being freed by dQ(n) and S(n+3) needing its successor (in-kernel trace: the issuer waited for kv_full).
-struct DqSmem {
-  static constexpr uint32_t NST = 5;
-  static constexpr uint32_t QDO_OFF = 0;                          // Q 32K | dO 32K
-  static constexpr uint32_t KV_OFF = 2 * AB_T128;                 // NST x (K 16K | V 16K)
-  static constexpr uint32_t BAR_OFF = KV_OFF + NST * 2 * AB_T64;
-  // kv_full[5], kv_empty[5], sdp_full[2], sdp_empty[2], ds_full[2], res_full, qdo_ready, done
-  static constexpr uint32_t NUM_BARS = 19;
-  static constexpr uint32_t DYN_BYTES = BAR_OFF + NUM_BARS * 8 + 16 + 1024;
-};
-static_assert(AB_STAGE_BYTES <= 2 * AB_T128, "dQ staging reuses the Q/dO staging area");
-static_assert(DqSmem::DYN_BYTES <= 232448, "dq pass shared memory");
+// P / dS fragment for wgmma A operand chunk kk (16 partner columns) from fp32 pairs of a 64-column accumulator
+__device__ __forceinline__ void a_frag(const float (&x)[32], uint32_t kk, uint32_t (&a)[4]) {
+  a[0] = pack_bf16x2(x[8 * kk], x[8 * kk + 1]);
+  a[1] = pack_bf16x2(x[8 * kk + 2], x[8 * kk + 3]);
+  a[2] = pack_bf16x2(x[8 * kk + 4], x[8 * kk + 5]);
+  a[3] = pack_bf16x2(x[8 * kk + 6], x[8 * kk + 7]);
+}
 
+// S (+)= A_rows · B_n^T over hd = 128: A = 64 resident rows (atoms AB_A128 apart, at `a_off` inside them), B = a streamed
+// [64 x 128] tile (atoms AB_A64 apart); both K-major over hd.
+__device__ __forceinline__ void scores_64x64(float (&acc)[32], uint32_t a_base, uint32_t b_base) {
+  const uint64_t ad = gmma_desc_sw128(a_base, 0, 1024), bd = gmma_desc_sw128(b_base, 0, 1024);
+#pragma unroll
+  for (uint32_t ks = 0; ks < 8; ++ks)
+    wgmma_ss_bf16<64, 0, 0>(acc, ad + (ks >> 2) * (AB_A128 >> 4) + (ks & 3) * 2, bd + (ks >> 2) * (AB_A64 >> 4) + (ks & 3) * 2,
+                            ks ? 1u : 0u);
+}
+
+struct BwdSmem {
+  static constexpr uint32_t RES_OFF = 0;                          // two resident [128 x 128] tiles
+  static constexpr uint32_t ST_OFF = 2 * AB_T128;                 // AB_NST x two [64 x 128] tiles
+  static constexpr uint32_t BAR_OFF = ST_OFF + AB_NST * 2 * AB_T64;
+  // res_full, st_full[NST], st_empty[NST]
+  static constexpr uint32_t NUM_BARS = 1 + 2 * AB_NST;
+  static constexpr uint32_t DYN_BYTES = BAR_OFF + NUM_BARS * 8 + 1024;
+};
+static_assert(AB_STAGE_BYTES <= 2 * AB_T128, "accumulator staging reuses the resident tiles");
+static_assert(BwdSmem::DYN_BYTES <= 232448, "attention backward shared memory");
+
+// TMA issue of both passes, by thread 0: the two resident tiles and the first AB_NST sub-blocks up front ...
+__device__ __forceinline__ void bwd_load_prologue(uint8_t* smem, uint64_t* res_full, uint64_t* st_full, const CUtensorMap* r0,
+                                                  const CUtensorMap* r1, const CUtensorMap* s0, const CUtensorMap* s1,
+                                                  int32_t col, int32_t res_row, int32_t st_row0, uint32_t n_it) {
+  using L = BwdSmem;
+  mbar_arrive_expect_tx(res_full, 2 * AB_T128);
+  load_tile<128>(smem + L::RES_OFF, r0, res_full, col, res_row);
+  load_tile<128>(smem + L::RES_OFF + AB_T128, r1, res_full, col, res_row);
+  for (uint32_t n = 0; n < min(n_it, AB_NST); ++n) {
+    uint8_t* dst = smem + L::ST_OFF + n * 2 * AB_T64;
+    mbar_arrive_expect_tx(&st_full[n], 2 * AB_T64);
+    load_tile<64>(dst, s0, &st_full[n], col, st_row0 + n * 64);
+    load_tile<64>(dst + AB_T64, s1, &st_full[n], col, st_row0 + n * 64);
+  }
+}
+// ... then sub-block n + AB_NST into stage n % AB_NST once both warpgroups have released sub-block n.
+__device__ __forceinline__ void bwd_load_refill(uint8_t* smem, uint64_t* st_full, uint64_t* st_empty, const CUtensorMap* s0,
+                                                const CUtensorMap* s1, int32_t col, int32_t st_row0, uint32_t n, uint32_t n_it) {
+  using L = BwdSmem;
+  if (n + AB_NST >= n_it) return;
+  const uint32_t st = n % AB_NST;
+  mbar_wait(&st_empty[st], (n / AB_NST) & 1);
+  uint8_t* dst = smem + L::ST_OFF + st * 2 * AB_T64;
+  const int32_t row = st_row0 + (n + AB_NST) * 64;
+  mbar_arrive_expect_tx(&st_full[st], 2 * AB_T64);
+  load_tile<64>(dst, s0, &st_full[st], col, row);
+  load_tile<64>(dst + AB_T64, s1, &st_full[st], col, row);
+}
+
+// ======================================================================================================
+// dq pass
+// ======================================================================================================
 __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_do,
                    const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v,
@@ -177,21 +191,13 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_cons
                    int64_t lddq, const int* __restrict__ cu_seqlens, int B, int T, float scale,
                    const int* __restrict__ rope_pos, const __nv_bfloat16* __restrict__ cos_t,
                    const __nv_bfloat16* __restrict__ sin_t) {
-  using L = DqSmem;
+  using L = BwdSmem;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQdO = smem + L::QDO_OFF;
-  uint8_t* sKV = smem + L::KV_OFF;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
-  uint64_t* kv_full = bars + 0;     // [5]
-  uint64_t* kv_empty = bars + 5;    // [5]
-  uint64_t* sdp_full = bars + 10;   // [2]
-  uint64_t* sdp_empty = bars + 12;  // [2]
-  uint64_t* ds_full = bars + 14;    // [2]
-  uint64_t* res_full = bars + 16;
-  uint64_t* qdo_ready = bars + 17;
-  uint64_t* done = bars + 18;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + L::NUM_BARS);
+  uint64_t* res_full = bars;
+  uint64_t* st_full = bars + 1;
+  uint64_t* st_empty = bars + 1 + AB_NST;
 
   const uint32_t warp = warp_id_uniform(), lane = threadIdx.x & 31;
   const uint32_t head = blockIdx.y;
@@ -200,207 +206,86 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_cons
   if (!locate_block_bwd(cu_seqlens, B, gridDim.x - 1 - blockIdx.x, seq_start, seq_len, own)) return;  // heavy first
   // 64-key sub-blocks 0 .. n_sub-1 cover keys [0, min((own+1)*128, len))
   const uint32_t n_sub = min(2 * own + 2, (uint32_t)(seq_len + 63) / 64);
-  if (threadIdx.x == 0) {
-    AB_TR(1, 0); AB_TRV(1, 3, n_sub);
-#ifdef NV_ATTN_TRACE
-    unsigned sm; asm volatile("mov.u32 %0, %%smid;" : "=r"(sm)); AB_TRV(1, 4, sm);
-    unsigned long long gt; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt)); AB_TRV(1, 5, gt);
-#endif
-  }
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmap_q); tma_prefetch_desc(&tmap_do); tma_prefetch_desc(&tmap_k); tma_prefetch_desc(&tmap_v);
-    for (uint32_t i = 0; i < L::NST; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&sdp_full[i], 1); mbar_init(&sdp_empty[i], 8); mbar_init(&ds_full[i], 8); }
+  if (threadIdx.x == 0) {
     mbar_init(res_full, 1);
-    mbar_init(qdo_ready, 8);
-    mbar_init(done, 1);
+    for (uint32_t i = 0; i < AB_NST; ++i) { mbar_init(&st_full[i], 1); mbar_init(&st_empty[i], 2); }
     fence_mbar_init();
   }
-  if (warp == 1) { tmem_alloc(tmem_ptr_smem, 512); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  const uint32_t tmem_dQ = tmem_base + 256, tmem_Qa = tmem_base + 384, tmem_dOa = tmem_base + 448;
-  if (threadIdx.x == 0) AB_TR(1, 1);
 
-  if (warp == 0) {
-    const int32_t col = head * 128;
-    if (elect_one()) {
-      mbar_arrive_expect_tx(res_full, 2 * AB_T128);
-      load_tile<128>(sQdO, &tmap_q, res_full, col, seq_start + own * 128);
-      load_tile<128>(sQdO + AB_T128, &tmap_do, res_full, col, seq_start + own * 128);
-    }
-    __syncwarp();
-    for (uint32_t n = 0; n < n_sub; ++n) {
-      const uint32_t st = n % L::NST, use = n / L::NST;
-      mbar_wait(&kv_empty[st], (use & 1) ^ 1);
-      if (elect_one()) {
-        mbar_arrive_expect_tx(&kv_full[st], 2 * AB_T64);
-        load_tile<64>(sKV + st * 2 * AB_T64, &tmap_k, &kv_full[st], col, seq_start + n * 64);
-        load_tile<64>(sKV + st * 2 * AB_T64 + AB_T64, &tmap_v, &kv_full[st], col, seq_start + n * 64);
-      }
-      __syncwarp();
-    }
-  } else if (warp == 1) {
-    // whole warp runs the issue loop (uniform registers, see elect_one()); one elected lane issues
-    constexpr uint32_t idesc_s = umma_idesc_bf16(128, 64, 0, 0);    // [128 q] x [64 keys], both K-major over hd
-    constexpr uint32_t idesc_dq = umma_idesc_bf16(128, 128, 0, 1);  // dS (K-major over keys) x K_n (MN-major: hd contiguous)
-    auto issue_sdp = [&](uint32_t n) {
-      const uint32_t st = n % L::NST, b = n & 1;
-      mbar_wait(&kv_full[st], (n / L::NST) & 1);
-      mbar_wait(&sdp_empty[b], ((n >> 1) & 1) ^ 1);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint64_t kd = umma_smem_desc_sw128(smem_u32(sKV + st * 2 * AB_T64), 0, 1024);
-        const uint64_t vd = kd + (AB_T64 >> 4);
+  if (threadIdx.x == 0)
+    bwd_load_prologue(smem, res_full, st_full, &tmap_q, &tmap_do, &tmap_k, &tmap_v, head * 128, seq_start + own * 128,
+                      seq_start, n_sub);
+
+  const uint32_t wg = warp >> 2;
+  const uint32_t ra = wg * 64 + (warp & 3) * 16 + (lane >> 2);    // rows ra, ra + 8 of the block
+  const uint32_t qa = own * 128 + ra, qb = qa + 8;
+  const uint32_t cq = 2 * (lane & 3);
+  const float sl2 = scale * LOG2E;
+  // an invalid row gets LSE = +inf -> p = exp2(-inf) = 0 without a branch
+  const float la = qa < (uint32_t)seq_len ? lse[(int64_t)head * T + seq_start + qa] * LOG2E : INFINITY;
+  const float lb = qb < (uint32_t)seq_len ? lse[(int64_t)head * T + seq_start + qb] * LOG2E : INFINITY;
+  const float da = qa < (uint32_t)seq_len ? Dvec[(int64_t)head * T + seq_start + qa] : 0.f;
+  const float db = qb < (uint32_t)seq_len ? Dvec[(int64_t)head * T + seq_start + qb] : 0.f;
+  const uint32_t sQ = smem_u32(smem + L::RES_OFF) + wg * 8192, sdO = sQ + AB_T128;
+  float dqacc[64];
 #pragma unroll
-        for (uint32_t ka = 0; ka < 2; ++ka)
+  for (uint32_t i = 0; i < 64; ++i) dqacc[i] = 0.f;
+  mbar_wait(res_full, 0);
+  for (uint32_t n = 0; n < n_sub; ++n) {
+    const uint32_t st = n % AB_NST;
+    const uint32_t sKn = smem_u32(smem + L::ST_OFF + st * 2 * AB_T64), sVn = sKn + AB_T64;
+    mbar_wait(&st_full[st], (n / AB_NST) & 1);
+    float sacc[32], dpacc[32];
+    wgmma_fence();
+    scores_64x64(sacc, sQ, sKn);
+    scores_64x64(dpacc, sdO, sVn);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(sacc);
+    reg_fence(dpacc);
+    const bool diag = (n >= 2 * own);                     // sub-blocks that touch the diagonal 128x128 block
 #pragma unroll
-          for (uint32_t ks = 0; ks < 4; ++ks)      // hd step ka*64 + ks*16 -> A columns (ka*32 + ks*8), B bytes as before
-            umma_f16_ts(tmem_base + b * 64, tmem_Qa + ka * 32 + ks * 8, kd + ka * (AB_A64 >> 4) + ks * 2, idesc_s,
-                        (ka | ks) ? 1u : 0u);
+    for (uint32_t i = 0; i < 8; ++i) {
 #pragma unroll
-        for (uint32_t ka = 0; ka < 2; ++ka)
-#pragma unroll
-          for (uint32_t ks = 0; ks < 4; ++ks)
-            umma_f16_ts(tmem_base + 128 + b * 64, tmem_dOa + ka * 32 + ks * 8, vd + ka * (AB_A64 >> 4) + ks * 2, idesc_s,
-                        (ka | ks) ? 1u : 0u);
-        umma_commit(&sdp_full[b]);
-        if (n < 8) AB_TR(1, 10 + 2 * n);
-      }
-      __syncwarp();
-    };
-    mbar_wait(qdo_ready, 0);
-    tc_fence_after();
-    if (lane == 0) AB_TR(1, 2);
-    issue_sdp(0);
-    for (uint32_t n = 0; n < n_sub; ++n) {
-      if (n + 1 < n_sub) issue_sdp(n + 1);
-      const uint32_t st = n % L::NST, b = n & 1;
-      mbar_wait(&ds_full[b], (n >> 1) & 1);
-      tc_fence_after();
-      if (elect_one()) {
-        if (n < 8) AB_TR(1, 11 + 2 * n);
-        // dQ += dS K_n : contraction over the 64 keys (4 k-steps).  A = dS(n) in the S[b] columns: keys 0..31 at columns
-        // 0..15, keys 32..63 at columns 32..47 (each compute warp overwrote only what it had read).  B rows = keys, 64-wide
-        // hd atoms AB_A64 apart.
-        const uint64_t km = umma_smem_desc_sw128(smem_u32(sKV + st * 2 * AB_T64), AB_A64, 1024);
-#pragma unroll
-        for (uint32_t ks = 0; ks < 4; ++ks)
-          umma_f16_ts(tmem_dQ, tmem_base + b * 64 + (ks >> 1) * 32 + (ks & 1) * 8, km + ks * 128, idesc_dq, (n | ks) ? 1u : 0u);
-        umma_commit(&kv_empty[st]);
-        if (n + 1 == n_sub) umma_commit(done);
-      }
-      __syncwarp();
-    }
-  } else {
-    const uint32_t quarter = warp & 3, half = (warp - 2) >> 2;
-    const uint32_t r = quarter * 32 + lane;
-    const uint32_t lane_off = (quarter * 32) << 16;
-    const float sl2 = scale * LOG2E;
-    const uint32_t qi = own * 128 + r;
-    const bool row_valid = qi < (uint32_t)seq_len;
-    const int64_t tok = (int64_t)seq_start + qi;
-    // ---- Q, dO -> TMEM (bf16 A-operand layout): this thread owns hd [half*64, half*64+64) of its row = atom `half` of
-    // the TMA-staged tile (two 64-row boxes per atom, 128-byte rows, 16-byte chunks XOR-swizzled by the row) ----
-    {
-      uint32_t a[32], d[32];
-      mbar_wait(res_full, 0);
-      const uint32_t rowoff = half * AB_A128 + (r >> 6) * (64 * 128);
-      const uint32_t qb = smem_u32(sQdO) + rowoff, ob = qb + AB_T128;
-#pragma unroll
-      for (uint32_t i = 0; i < 8; ++i) {
-        const uint32_t o = sw128_offset(r & 63, i);
-        uint4 x, y;
-        asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(x.x), "=r"(x.y), "=r"(x.z), "=r"(x.w) : "r"(qb + o));
-        asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(y.x), "=r"(y.y), "=r"(y.z), "=r"(y.w) : "r"(ob + o));
-        if (!row_valid) { x = make_uint4(0, 0, 0, 0); y = make_uint4(0, 0, 0, 0); }   // rows past the sequence: next sequence's data
-        a[4 * i] = x.x; a[4 * i + 1] = x.y; a[4 * i + 2] = x.z; a[4 * i + 3] = x.w;
-        d[4 * i] = y.x; d[4 * i + 1] = y.y; d[4 * i + 2] = y.z; d[4 * i + 3] = y.w;
-      }
-      tmem_st_32x32b_x32(tmem_Qa + lane_off + half * 32, a);
-      tmem_st_32x32b_x32(tmem_dOa + lane_off + half * 32, d);
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(qdo_ready);
-    }
-    // an invalid row gets LSE = +inf -> p = exp2(-inf) = 0 without a branch
-    const float lse_r = row_valid ? lse[(int64_t)head * T + tok] * LOG2E : INFINITY;
-    const float d_r = row_valid ? Dvec[(int64_t)head * T + tok] : 0.f;
-    const float2 sl2v = make_float2(sl2, sl2), nl = make_float2(-lse_r, -lse_r);
-    const float2 scv = make_float2(scale, scale), nds = make_float2(-d_r * scale, -d_r * scale);
-    for (uint32_t n = 0; n < n_sub; ++n) {
-      const uint32_t b = n & 1;
-      mbar_wait(&sdp_full[b], (n >> 1) & 1);
-      if (warp == 2 && lane == 0 && n < 8) AB_TR(1, 30 + 2 * n);
-      tc_fence_after();
-      uint32_t sv[32], dv[32];
-      tmem_ld_32x32b_x32(tmem_base + b * 64 + lane_off + half * 32, sv);
-      tmem_ld_32x32b_x32(tmem_base + 128 + b * 64 + lane_off + half * 32, dv);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&sdp_empty[b]);           // (kept for symmetry; program order already protects S[b])
-      const bool diag = (n >= 2 * own);                     // sub-blocks that touch the diagonal 128x128 block
-      const uint32_t key0 = n * 64 + half * 32;             // first key of this thread's 32 columns
-      uint32_t dd[16];
-#pragma unroll
-      for (uint32_t i = 0; i < 32; i += 2) {
-        float2 e = __ffma2_rn(make_float2(__uint_as_float(sv[i]), __uint_as_float(sv[i + 1])), sl2v, nl);
-        float p0 = exp2f(e.x), p1 = exp2f(e.y);
-        if (diag) {
-          if (key0 + i > qi) p0 = 0.f;
-          if (key0 + i + 1 > qi) p1 = 0.f;
-        }
+      for (uint32_t e = 0; e < 4; ++e) {
+        const uint32_t key = n * 64 + 8 * i + cq + (e & 1);
+        const uint32_t q = (e & 2) ? qb : qa;
+        float p = exp2f(fmaf(sacc[4 * i + e], sl2, -((e & 2) ? lb : la)));
+        if (diag && key > q) p = 0.f;
         // dS = P o (dP - D) * scale
-        const float2 t = __ffma2_rn(make_float2(__uint_as_float(dv[i]), __uint_as_float(dv[i + 1])), scv, nds);
-        const float2 ds = __fmul2_rn(make_float2(p0, p1), t);
-        dd[i >> 1] = pack_bf16x2(ds.x, ds.y);
+        sacc[4 * i + e] = p * ((dpacc[4 * i + e] - ((e & 2) ? db : da)) * scale);
       }
-      // dS(n) over the S columns this warp has just consumed: keys half*32.. -> 16 packed columns at half*32
-      tmem_st_32x32b_x16(tmem_base + b * 64 + lane_off + half * 32, dd);
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&ds_full[b]);
-      if (warp == 2 && lane == 0 && n < 8) AB_TR(1, 31 + 2 * n);
     }
-    mbar_wait(done, 0);
-    if (warp == 2 && lane == 0) AB_TR(1, 50);
-    tc_fence_after();
-    uint8_t* stage = sQdO;                                  // Q/dO staging is free since qdo_ready
-    stage_acc_tile(tmem_dQ, lane_off, half * 32, r, stage);
-    compute_warps_sync();
-    const uint32_t rows_valid = min(128u, (uint32_t)seq_len - own * 128);
-    const int64_t tok0 = (int64_t)seq_start + own * 128;
-    flush_acc_tile(stage, warp - 2, lane, rows_valid, dq + tok0 * lddq + head * 128, lddq,
-                   rope_pos != nullptr ? rope_pos + tok0 : nullptr, cos_t, sin_t);
-    if (warp == 2 && lane == 0) AB_TR(1, 51);
+    // dQ += dS K_n : contraction over the 64 keys; B = K_n rows = keys (K dim), hd contiguous (MN-major)
+    const uint64_t kd = gmma_desc_sw128(sKn, AB_A64, 1024);
+    wgmma_fence();
+#pragma unroll
+    for (uint32_t kk = 0; kk < 4; ++kk) {
+      uint32_t a[4];
+      a_frag(sacc, kk, a);
+      wgmma_rs_bf16<128, 1>(dqacc, a, kd + kk * ((16 * 128) >> 4), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(dqacc);
+    if ((threadIdx.x & 127) == 0) mbar_arrive(&st_empty[st]);
+    if (threadIdx.x == 0) bwd_load_refill(smem, st_full, st_empty, &tmap_k, &tmap_v, head * 128, seq_start, n, n_sub);
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, 512); }
-  if (threadIdx.x == 32) AB_TR(1, 52);
+  compute_warps_sync();                                     // every operand stage is free
+  uint8_t* stage = smem + L::RES_OFF;
+  stage_acc_tile(dqacc, wg, stage);
+  compute_warps_sync();
+  const uint32_t rows_valid = min(128u, (uint32_t)seq_len - own * 128);
+  const int64_t tok0 = (int64_t)seq_start + own * 128;
+  flush_acc_tile(stage, warp, lane, rows_valid, dq + tok0 * lddq + head * 128, lddq,
+                 rope_pos != nullptr ? rope_pos + tok0 : nullptr, cos_t, sin_t);
 }
 
 // ======================================================================================================
-// dk/dv pass (transposed scores: TMEM lanes = keys)
+// dk/dv pass (transposed scores: accumulator rows = keys)
 // ======================================================================================================
-struct DkvSmem {
-  static constexpr uint32_t NST = 4;                              // 3 stages left 2 sub-blocks of slack < TMA latency (trace); 5 do not fit next to the 2 KB of static smem
-  static constexpr uint32_t K_OFF = 0, V_OFF = AB_T128;
-  static constexpr uint32_t QO_OFF = 2 * AB_T128;                 // NST x (Q 16K | dO 16K)
-  static constexpr uint32_t BAR_OFF = QO_OFF + NST * 2 * AB_T64;
-  // res_full, qo_full[NST], qo_empty[NST] (slots for 5), sdp_full[2], sdp_empty[2], pds_full[2], done
-  static constexpr uint32_t NUM_BARS = 18;
-  static constexpr uint32_t DYN_BYTES = BAR_OFF + NUM_BARS * 8 + 16 + 1024;
-};
-static_assert(DkvSmem::DYN_BYTES + 2048 <= 232448, "dk/dv pass shared memory (dynamic + s_stats)");
-
 __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                     const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_do,
@@ -408,22 +293,13 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
                     int64_t lddk, __nv_bfloat16* __restrict__ dv, int64_t lddv, const int* __restrict__ cu_seqlens,
                     int B, int T, float scale, const int* __restrict__ rope_pos,
                     const __nv_bfloat16* __restrict__ cos_t, const __nv_bfloat16* __restrict__ sin_t) {
-  using L = DkvSmem;
+  using L = BwdSmem;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sK = smem + L::K_OFF;
-  uint8_t* sV = smem + L::V_OFF;
-  uint8_t* sQO = smem + L::QO_OFF;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
-  uint64_t* res_full = bars + 0;
-  uint64_t* qo_full = bars + 1;     // [5]
-  uint64_t* qo_empty = bars + 6;    // [5]
-  uint64_t* sdp_full = bars + 11;   // [2]
-  uint64_t* sdp_empty = bars + 13;  // [2]
-  uint64_t* pds_full = bars + 15;   // [2] P^T(n) / dS^T(n) are in TMEM (over S^T[b] / dP^T[b])
-  uint64_t* done = bars + 17;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + L::NUM_BARS);
-  __shared__ float s_stats[8][2][32];   // per compute warp: LSE*log2e and D of its 32 query columns
+  uint64_t* res_full = bars;
+  uint64_t* st_full = bars + 1;
+  uint64_t* st_empty = bars + 1 + AB_NST;
 
   const uint32_t warp = warp_id_uniform(), lane = threadIdx.x & 31;
   const uint32_t head = blockIdx.y;
@@ -433,211 +309,109 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
   // 64-query sub-blocks first .. n_qsub-1 can see keys of this block (causal): q >= own*128
   const uint32_t first = 2 * own, n_qsub = (uint32_t)(seq_len + 63) / 64;
   const uint32_t n_it = n_qsub - first;
-  if (threadIdx.x == 0) {
-    AB_TR(0, 0); AB_TRV(0, 3, n_it);
-#ifdef NV_ATTN_TRACE
-    unsigned sm; asm volatile("mov.u32 %0, %%smid;" : "=r"(sm)); AB_TRV(0, 4, sm);
-    unsigned long long gt; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt)); AB_TRV(0, 5, gt);
-#endif
-  }
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmap_q); tma_prefetch_desc(&tmap_k); tma_prefetch_desc(&tmap_v); tma_prefetch_desc(&tmap_do);
+  if (threadIdx.x == 0) {
     mbar_init(res_full, 1);
-    for (uint32_t i = 0; i < L::NST; ++i) { mbar_init(&qo_full[i], 1); mbar_init(&qo_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&sdp_full[i], 1); mbar_init(&sdp_empty[i], 8); }
-    mbar_init(&pds_full[0], 8); mbar_init(&pds_full[1], 8);
-    mbar_init(done, 1);
+    for (uint32_t i = 0; i < AB_NST; ++i) { mbar_init(&st_full[i], 1); mbar_init(&st_empty[i], 2); }
     fence_mbar_init();
   }
-  if (warp == 1) { tmem_alloc(tmem_ptr_smem, 512); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  const uint32_t tmem_dV = tmem_base + 256, tmem_dK = tmem_base + 384;
-  if (threadIdx.x == 0) AB_TR(0, 1);
 
-  if (warp == 0) {
-    const int32_t col = head * 128;
-    if (elect_one()) {
-      mbar_arrive_expect_tx(res_full, 2 * AB_T128);
-      load_tile<128>(sK, &tmap_k, res_full, col, seq_start + own * 128);
-      load_tile<128>(sV, &tmap_v, res_full, col, seq_start + own * 128);
-    }
-    __syncwarp();
-    for (uint32_t n = 0; n < n_it; ++n) {
-      const uint32_t st = n % L::NST, use = n / L::NST;
-      mbar_wait(&qo_empty[st], (use & 1) ^ 1);
-      if (elect_one()) {
-        mbar_arrive_expect_tx(&qo_full[st], 2 * AB_T64);
-        load_tile<64>(sQO + st * 2 * AB_T64, &tmap_q, &qo_full[st], col, seq_start + (first + n) * 64);
-        load_tile<64>(sQO + st * 2 * AB_T64 + AB_T64, &tmap_do, &qo_full[st], col, seq_start + (first + n) * 64);
+  if (threadIdx.x == 0)
+    bwd_load_prologue(smem, res_full, st_full, &tmap_k, &tmap_v, &tmap_q, &tmap_do, head * 128, seq_start + own * 128,
+                      seq_start + first * 64, n_it);
+
+  const uint32_t wg = warp >> 2;
+  const uint32_t ra = wg * 64 + (warp & 3) * 16 + (lane >> 2);    // key rows ra, ra + 8 of the block
+  const uint32_t ka = own * 128 + ra, kb = ka + 8;
+  const uint32_t cq = 2 * (lane & 3);
+  const float sl2 = scale * LOG2E;
+  const uint32_t sK = smem_u32(smem + L::RES_OFF) + wg * 8192, sV = sK + AB_T128;
+  float dvacc[64], dkacc[64];
+#pragma unroll
+  for (uint32_t i = 0; i < 64; ++i) { dvacc[i] = 0.f; dkacc[i] = 0.f; }
+  mbar_wait(res_full, 0);
+  for (uint32_t n = 0; n < n_it; ++n) {
+    const uint32_t st = n % AB_NST;
+    const uint32_t sQn = smem_u32(smem + L::ST_OFF + st * 2 * AB_T64), sdOn = sQn + AB_T64;
+    const uint32_t q0 = (first + n) * 64;
+    // -LSE * log2e and -D * scale of the thread's 16 query columns (stored negated: -inf -> p = 0 past the sequence);
+    // loaded before the wait so that their latency hides under it
+    float nl[16], nd[16];
+#pragma unroll
+    for (uint32_t i = 0; i < 8; ++i)
+#pragma unroll
+      for (uint32_t e = 0; e < 2; ++e) {
+        const uint32_t q = q0 + 8 * i + cq + e;
+        const bool ok = q < (uint32_t)seq_len;
+        const int64_t idx = (int64_t)head * T + seq_start + q;
+        nl[2 * i + e] = ok ? -lse[idx] * LOG2E : -INFINITY;
+        nd[2 * i + e] = ok ? -Dvec[idx] * scale : 0.f;
       }
-      __syncwarp();
-    }
-  } else if (warp == 1) {
-    // whole warp runs the issue loop (uniform registers, see elect_one()); one elected lane issues
-    constexpr uint32_t idesc_s = umma_idesc_bf16(128, 64, 0, 0);     // [128 keys] x [64 q], both K-major over hd
-    constexpr uint32_t idesc_acc = umma_idesc_bf16(128, 128, 0, 1);  // P^T/dS^T (K-major over q) x dO_n/Q_n (MN-major)
-    const uint64_t k_k = umma_smem_desc_sw128(smem_u32(sK), 0, 1024);
-    const uint64_t v_k = umma_smem_desc_sw128(smem_u32(sV), 0, 1024);
-    auto issue_sdp = [&](uint32_t n) {
-      const uint32_t st = n % L::NST, b = n & 1;
-      mbar_wait(&qo_full[st], (n / L::NST) & 1);
-      mbar_wait(&sdp_empty[b], ((n >> 1) & 1) ^ 1);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint64_t qd = umma_smem_desc_sw128(smem_u32(sQO + st * 2 * AB_T64), 0, 1024);
-        const uint64_t od = qd + (AB_T64 >> 4);
+    mbar_wait(&st_full[st], (n / AB_NST) & 1);
+    float sacc[32], dpacc[32];
+    wgmma_fence();
+    scores_64x64(sacc, sK, sQn);
+    scores_64x64(dpacc, sV, sdOn);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(sacc);
+    reg_fence(dpacc);
+    const bool diag = (first + n) < 2 * own + 2;            // query sub-blocks inside the diagonal 128x128 block
 #pragma unroll
-        for (uint32_t ka = 0; ka < 2; ++ka)
+    for (uint32_t i = 0; i < 8; ++i) {
 #pragma unroll
-          for (uint32_t ks = 0; ks < 4; ++ks)
-            umma_f16_ss(tmem_base + b * 64, k_k + ka * (AB_A128 >> 4) + ks * 2, qd + ka * (AB_A64 >> 4) + ks * 2, idesc_s,
-                        (ka | ks) ? 1u : 0u);
-#pragma unroll
-        for (uint32_t ka = 0; ka < 2; ++ka)
-#pragma unroll
-          for (uint32_t ks = 0; ks < 4; ++ks)
-            umma_f16_ss(tmem_base + 128 + b * 64, v_k + ka * (AB_A128 >> 4) + ks * 2, od + ka * (AB_A64 >> 4) + ks * 2,
-                        idesc_s, (ka | ks) ? 1u : 0u);
-        umma_commit(&sdp_full[b]);
-        if (n < 8) AB_TR(0, 10 + 2 * n);
+      for (uint32_t e = 0; e < 4; ++e) {
+        const uint32_t c = 2 * i + (e & 1);
+        const uint32_t q = q0 + 8 * i + cq + (e & 1);
+        float p = exp2f(fmaf(sacc[4 * i + e], sl2, nl[c]));
+        if (diag && q < ((e & 2) ? kb : ka)) p = 0.f;     // causal: a query sees keys <= itself
+        sacc[4 * i + e] = p;
+        dpacc[4 * i + e] = p * fmaf(dpacc[4 * i + e], scale, nd[c]);   // dS^T = P^T o (dP^T - D) * scale
       }
-      __syncwarp();
-    };
-    mbar_wait(res_full, 0);
-    if (lane == 0) AB_TR(0, 2);
-    issue_sdp(0);
-    for (uint32_t n = 0; n < n_it; ++n) {
-      if (n + 1 < n_it) issue_sdp(n + 1);
-      const uint32_t st = n % L::NST, b = n & 1;
-      mbar_wait(&pds_full[b], (n >> 1) & 1);
-      tc_fence_after();
-      if (elect_one()) {
-        if (n < 8) AB_TR(0, 11 + 2 * n);
-        // contraction over the 64 queries (4 k-steps).  A operands in TENSOR MEMORY (.ts form): P^T(n) lies over the
-        // S^T[b] columns it was computed from, dS^T(n) over dP^T[b] (queries 0..31 at columns 0..15, 32..63 at 32..47: each
-        // compute warp overwrote only what it had read) - no smem store, no proxy fence, no A-operand smem bandwidth.
-        // B rows = queries, 64-wide hd atoms AB_A64 apart.
-        const uint64_t qm = umma_smem_desc_sw128(smem_u32(sQO + st * 2 * AB_T64), AB_A64, 1024);
-        const uint64_t om = qm + (AB_T64 >> 4);
-#pragma unroll
-        for (uint32_t ks = 0; ks < 4; ++ks)
-          umma_f16_ts(tmem_dV, tmem_base + b * 64 + (ks >> 1) * 32 + (ks & 1) * 8, om + ks * 128, idesc_acc, (n | ks) ? 1u : 0u);
-#pragma unroll
-        for (uint32_t ks = 0; ks < 4; ++ks)
-          umma_f16_ts(tmem_dK, tmem_base + 128 + b * 64 + (ks >> 1) * 32 + (ks & 1) * 8, qm + ks * 128, idesc_acc, (n | ks) ? 1u : 0u);
-        umma_commit(&qo_empty[st]);
-        if (n + 1 == n_it) umma_commit(done);
-      }
-      __syncwarp();
     }
-  } else {
-    const uint32_t cw = warp - 2;
-    const uint32_t quarter = warp & 3, half = cw >> 2;
-    const uint32_t r = quarter * 32 + lane;                 // key row of this thread
-    const uint32_t lane_off = (quarter * 32) << 16;
-    const float sl2 = scale * LOG2E;
-    const uint32_t kj = own * 128 + r;                      // key index inside the sequence
-    float* st_l = s_stats[cw][0];
-    float* st_d = s_stats[cw][1];
-    // LSE / D of the 32 query columns a warp handles in sub-block n: one coalesced load per lane, shared inside the warp
-    // through smem.  The loads for sub-block n+1 are issued before sub-block n is processed - on the critical path they
-    // cost ~900 cycles of global-load latency per sub-block (in-kernel trace: gap between P^T/dS^T of n and S^T of n+1).
-    auto load_stats = [&](uint32_t n, float& l_out, float& d_out) {
-      const uint32_t qi = (first + n) * 64 + half * 32 + lane;
-      const bool ok = qi < (uint32_t)seq_len;
-      const int64_t tq = (int64_t)seq_start + qi;
-      // stored NEGATED / pre-scaled so that the loop is two packed FMAs: -inf -> p = exp2(-inf) = 0 for rows past the sequence
-      l_out = ok ? -lse[(int64_t)head * T + tq] * LOG2E : -INFINITY;
-      d_out = ok ? -Dvec[(int64_t)head * T + tq] * scale : 0.f;
-    };
-    float cur_l = -INFINITY, cur_d = 0.f;
-    const float2 sl2v = make_float2(sl2, sl2), scv = make_float2(scale, scale);
-    if (n_it > 0) load_stats(0, cur_l, cur_d);
-    for (uint32_t n = 0; n < n_it; ++n) {
-      const uint32_t b = n & 1;
-      const uint32_t q0 = (first + n) * 64 + half * 32;     // first query of the 32 columns
-      __syncwarp();
-      st_l[lane] = cur_l;
-      st_d[lane] = cur_d;
-      __syncwarp();
-      if (n + 1 < n_it) load_stats(n + 1, cur_l, cur_d);   // in flight while this sub-block is processed
-      mbar_wait(&sdp_full[b], (n >> 1) & 1);
-      if (warp == 2 && lane == 0 && n < 8) AB_TR(0, 30 + 2 * n);
-      tc_fence_after();
-      uint32_t sv[32], dv[32];
-      tmem_ld_32x32b_x32(tmem_base + b * 64 + lane_off + half * 32, sv);
-      tmem_ld_32x32b_x32(tmem_base + 128 + b * 64 + lane_off + half * 32, dv);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&sdp_empty[b]);
-      const bool diag = (first + n) < 2 * own + 2;          // query sub-blocks inside the diagonal 128x128 block
-      uint32_t pp[16], dd[16];
+    // dV += P^T dO_n, dK += dS^T Q_n: contraction over the 64 queries; B rows = queries, hd contiguous (MN-major)
+    const uint64_t qd = gmma_desc_sw128(sQn, AB_A64, 1024), od = gmma_desc_sw128(sdOn, AB_A64, 1024);
+    wgmma_fence();
 #pragma unroll
-      for (uint32_t i = 0; i < 32; i += 2) {
-        const float2 l2 = *reinterpret_cast<const float2*>(st_l + i);       // -LSE * log2e of queries i, i+1
-        const float2 d2 = *reinterpret_cast<const float2*>(st_d + i);       // -D * scale
-        const float2 e = __ffma2_rn(make_float2(__uint_as_float(sv[i]), __uint_as_float(sv[i + 1])), sl2v, l2);
-        float p0 = exp2f(e.x), p1 = exp2f(e.y);
-        if (diag) {                                         // causal: a query sees keys <= itself
-          if (q0 + i < kj) p0 = 0.f;
-          if (q0 + i + 1 < kj) p1 = 0.f;
-        }
-        pp[i >> 1] = pack_bf16x2(p0, p1);
-        const float2 t = __ffma2_rn(make_float2(__uint_as_float(dv[i]), __uint_as_float(dv[i + 1])), scv, d2);   // (dP - D) * scale
-        const float2 ds = __fmul2_rn(make_float2(p0, p1), t);
-        dd[i >> 1] = pack_bf16x2(ds.x, ds.y);
-      }
-      // P^T(n) / dS^T(n) straight into TMEM, over the score columns this warp has just consumed (queries half*32..)
-      tmem_st_32x32b_x16(tmem_base + b * 64 + lane_off + half * 32, pp);
-      tmem_st_32x32b_x16(tmem_base + 128 + b * 64 + lane_off + half * 32, dd);
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&pds_full[b]);
-      if (warp == 2 && lane == 0 && n < 8) AB_TR(0, 31 + 2 * n);
+    for (uint32_t kk = 0; kk < 4; ++kk) {
+      uint32_t a[4];
+      a_frag(sacc, kk, a);
+      wgmma_rs_bf16<128, 1>(dvacc, a, od + kk * ((16 * 128) >> 4), 1u);
     }
-    mbar_wait(done, 0);
-    if (warp == 2 && lane == 0) AB_TR(0, 50);
-    tc_fence_after();
-    uint8_t* stage_v = sK;                                  // resident K/V and the Q/dO stages are free now
-    uint8_t* stage_k = sQO;
-    stage_acc_tile(tmem_dV, lane_off, half * 32, r, stage_v);
-    stage_acc_tile(tmem_dK, lane_off, half * 32, r, stage_k);
-    compute_warps_sync();
-    const uint32_t rows_valid = min(128u, (uint32_t)seq_len - own * 128);
-    const int64_t tok0 = (int64_t)seq_start + own * 128;
-    flush_acc_tile(stage_v, cw, lane, rows_valid, dv + tok0 * lddv + head * 128, lddv, nullptr, cos_t, sin_t);
-    flush_acc_tile(stage_k, cw, lane, rows_valid, dk + tok0 * lddk + head * 128, lddk,
-                   rope_pos != nullptr ? rope_pos + tok0 : nullptr, cos_t, sin_t);
-    if (warp == 2 && lane == 0) AB_TR(0, 51);
+#pragma unroll
+    for (uint32_t kk = 0; kk < 4; ++kk) {
+      uint32_t a[4];
+      a_frag(dpacc, kk, a);
+      wgmma_rs_bf16<128, 1>(dkacc, a, qd + kk * ((16 * 128) >> 4), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(dvacc);
+    reg_fence(dkacc);
+    if ((threadIdx.x & 127) == 0) mbar_arrive(&st_empty[st]);
+    if (threadIdx.x == 0)
+      bwd_load_refill(smem, st_full, st_empty, &tmap_q, &tmap_do, head * 128, seq_start + first * 64, n, n_it);
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, 512); }
-  if (threadIdx.x == 32) AB_TR(0, 52);
+  compute_warps_sync();                                     // every operand stage is free
+  uint8_t* stage_v = smem + L::RES_OFF;                     // resident K/V and the Q/dO stages are free now
+  uint8_t* stage_k = smem + L::ST_OFF;
+  stage_acc_tile(dvacc, wg, stage_v);
+  stage_acc_tile(dkacc, wg, stage_k);
+  compute_warps_sync();
+  const uint32_t rows_valid = min(128u, (uint32_t)seq_len - own * 128);
+  const int64_t tok0 = (int64_t)seq_start + own * 128;
+  flush_acc_tile(stage_v, warp, lane, rows_valid, dv + tok0 * lddv + head * 128, lddv, nullptr, cos_t, sin_t);
+  flush_acc_tile(stage_k, warp, lane, rows_valid, dk + tok0 * lddk + head * 128, lddk,
+                 rope_pos != nullptr ? rope_pos + tok0 : nullptr, cos_t, sin_t);
 }
 
 }  // namespace nv
 
-// Developer hook: copy the phase trace of the last nv_attn_bwd (kernel 0 = dk/dv pass, 1 = dq pass) to the host.
-// Returns the number of 64-bit words written, 0 when the library was built without -DNV_ATTN_TRACE.
+// Developer hook of the in-kernel phase trace.  The sm_90a kernels carry no trace: returns 0 words.
 extern "C" int nv_debug_attn_trace(int kernel, unsigned long long* out, int max_words) {
-  if (kernel == 2 && out) return nv::attn_fwd_trace_copy(out, max_words);      // forward kernel (attn_fwd.cu)
-#ifdef NV_ATTN_TRACE
-  if (kernel < 0 || kernel > 1 || !out) return 0;
-  const int n = max_words < 256 * 64 ? max_words : 256 * 64;
-  if (cudaMemcpyFromSymbol(out, nv::g_attn_trace, (size_t)n * 8, (size_t)kernel * 256 * 64 * 8) != cudaSuccess) return 0;
-  return n;
-#else
   (void)kernel; (void)out; (void)max_words;
   return 0;
-#endif
 }
 
 // Inputs: q,k,v (post-RoPE) and o, do as bf16 [T, H*128]-column views; lse [H,T] from the forward.
@@ -664,8 +438,8 @@ extern "C" int nv_attn_bwd(const void* q, int64_t ldq, const void* k, int64_t ld
   if ((rc = make_tmap_2d(&tdo, dout, 2, (uint64_t)H * 128, (uint64_t)T, (uint64_t)lddo * 2, 64, 64))) return rc;
   static bool attr_set = false;
   if (!attr_set) {
-    NV_CUDA(cudaFuncSetAttribute(attn_bwd_dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DqSmem::DYN_BYTES));
-    NV_CUDA(cudaFuncSetAttribute(attn_bwd_dkv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DkvSmem::DYN_BYTES));
+    NV_CUDA(cudaFuncSetAttribute(attn_bwd_dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BwdSmem::DYN_BYTES));
+    NV_CUDA(cudaFuncSetAttribute(attn_bwd_dkv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BwdSmem::DYN_BYTES));
     attr_set = true;
   }
   if (o != nullptr) {     // o == nullptr: dvec already holds D (written by the o_proj dgrad epilogue, nv_gemm_attnd_bf16)
@@ -677,11 +451,11 @@ extern "C" int nv_attn_bwd(const void* q, int64_t ldq, const void* k, int64_t ld
   const __nv_bfloat16* c = reinterpret_cast<const __nv_bfloat16*>(cos_t);
   const __nv_bfloat16* s = reinterpret_cast<const __nv_bfloat16*>(sin_t);
   dim3 grid(total_blocks, H);
-  attn_bwd_dkv_kernel<<<grid, AB_THREADS, DkvSmem::DYN_BYTES, stream>>>(
+  attn_bwd_dkv_kernel<<<grid, AB_THREADS, BwdSmem::DYN_BYTES, stream>>>(
       tq, tk, tv, tdo, lse, dvec, reinterpret_cast<__nv_bfloat16*>(dk), lddk, reinterpret_cast<__nv_bfloat16*>(dv), lddv,
       cu_seqlens, B, T, scale, rope_pos, c, s);
   NV_LAUNCH_CHECK();
-  attn_bwd_dq_kernel<<<grid, AB_THREADS, DqSmem::DYN_BYTES, stream>>>(
+  attn_bwd_dq_kernel<<<grid, AB_THREADS, BwdSmem::DYN_BYTES, stream>>>(
       tq, tdo, tk, tv, lse, dvec, reinterpret_cast<__nv_bfloat16*>(dq), lddq, cu_seqlens, B, T, scale, rope_pos, c, s);
   NV_LAUNCH_CHECK();
   return NV_OK;

@@ -1,4 +1,4 @@
-// navillm_b200 — causal self-attention forward on tcgen05 (flash-style, packed variable-length rows).
+// navillm_b200 — causal self-attention forward on Hopper wgmma (flash-style, packed variable-length rows).
 //
 // Replaces HF LLaMA's eager attention (reference call site models/modified_lm.py:112-116 ->
 // LlamaAttention: scores = QK^T/sqrt(hd) + causal/left-pad mask, fp32 softmax, P·V; SURVEY.md §2b K9),
@@ -7,24 +7,16 @@
 // cu_seqlens[b+1]; the reference's left padding is reproduced by the explicit position ids given to
 // the rotary kernel, so results at real tokens are identical (pad positions do not exist here).
 //
-// One CTA = one (256-query block = two 128-row tiles, head).  head_dim = 128.
-//   warp 0            TMA producer: Q0,Q1 once; K_j through a 2-slot ring, V_j through ONE slot.  S(j+1) is issued at the
-//                     START of iteration j, so K is prefetched two blocks ahead (K_{j+2} loads during iteration j-1: the
-//                     ~2000-cycle TMA latency is off the critical path); V_{j+1} is requested when PV(j) has completed
-//                     and is not needed before the end of iteration j+1 (in-kernel trace: with a K0 V0 K1 V1 ring of three
-//                     slots K_{j+2} could only start after PV(j) and S(j+2) waited ~1300 cycles per block for it)
-//   warp 1            tcgen05.mma issuer.  S_t(j+1) = Q_t K_{j+1}^T is issued as soon as the softmax warps of tile t have
-//                     pulled S_t(j) out of TMEM into registers (`s_free`), i.e. it runs on the tensor pipe UNDER the
-//                     softmax of block j; PV_t(j) follows when P_t(j) is in shared memory (`p_ready`).  The softmax
-//                     warps therefore never wait for the tensor pipe in steady state: the loop is bound by
-//                     max(softmax, MMA), not by their sum (round 1 issued S_t(j+1) only after P_t(j): a serial chain).
-//   warps 2..5 / 6..9 softmax of tile 0 / tile 1, one thread per query row: tcgen05.ld S (128 columns) -> running max
-//                     (FMNMX3) -> exp2 (FFMA2 + MUFU) -> fp32 row sum (FADD2) -> P (bf16) into 128B-swizzled smem.
-//                     LAZY rescale: the exponent reference m only moves when the block maximum exceeds it by more than
-//                     2^8 (p <= 256 stays exact enough in bf16/fp32), so the TMEM round trip that rescales O is rare
-//                     after the first blocks instead of happening whenever any row's maximum moved.
-// TMEM: S0 [0,128) S1 [128,256) O0 [256,384) O1 [384,512).
-// smem: Q 2x32K + K 2x32K + V 32K + P 2x32K = 224 KB.
+// One CTA = one (128-query block, head).  head_dim = 128.  288 threads:
+//   warp 8            TMA producer: Q once; K_j and V_j through a 2-slot ring (separate full barriers, so that the
+//                     scores of block j can start while V_j is still in flight)
+//   warpgroups 0, 1   query rows 0..63 / 64..127 of the block.  Per key block: S = Q K_j^T with m64n128k16 wgmmas from
+//                     shared memory (fp32 in registers), online softmax in registers (row max / sum over the four
+//                     threads of a row), P rounded to bf16 and fed to O += P V_j straight from registers (the wgmma
+//                     A-from-registers form: the S accumulator layout is the A-fragment layout), V read MN-major.
+// The exponent reference is the running row maximum (log2 units); the row sum is taken over the fp32 p before their
+// bf16 rounding, and O is normalised once at the end.
+// smem: Q 32K + K 2x32K + V 2x32K = 160 KB.
 #include "nv_common.cuh"
 #include "nv_host.h"
 
@@ -32,59 +24,20 @@ namespace nv {
 
 constexpr uint32_t ATT_TILE_BYTES = 128 * 128 * 2;  // one 128x128 bf16 tile = two 64-wide swizzle atoms
 constexpr uint32_t ATT_ATOM_BYTES = 128 * 128;      // 128 rows x 128 B
-constexpr uint32_t ATT_THREADS = 320;
-constexpr uint32_t ATT_QROWS = 256;
-constexpr uint32_t ATT_RING = 3;                    // smem slots: 0,1 = K ring, 2 = V
-constexpr float ATT_LAZY_LOG2 = 8.f;                // rescale threshold in log2 units
+constexpr uint32_t ATT_THREADS = 288;
+constexpr uint32_t ATT_QROWS = 128;
 
 struct AttnFwdSmem {
-  static constexpr uint32_t Q_OFF = 0;                                  // 2 tiles
-  static constexpr uint32_t KV_OFF = Q_OFF + 2 * ATT_TILE_BYTES;         // 3-slot ring
-  static constexpr uint32_t P_OFF = KV_OFF + ATT_RING * ATT_TILE_BYTES;  // 2 tiles
-  static constexpr uint32_t BAR_OFF = P_OFF + 2 * ATT_TILE_BYTES;
-  // q_full, kv_full[3], kv_empty[3] (slots 0,1: K ring, slot 2: V), s_full[2], s_free[2], p_ready[2], pv_done[2]
-  static constexpr uint32_t NUM_BARS = 15;
-  static constexpr uint32_t TOTAL = BAR_OFF + NUM_BARS * 8 + 16;
-  static constexpr uint32_t DYN_BYTES = TOTAL + 1024;
+  static constexpr uint32_t Q_OFF = 0;
+  static constexpr uint32_t K_OFF = Q_OFF + ATT_TILE_BYTES;        // 2 slots
+  static constexpr uint32_t V_OFF = K_OFF + 2 * ATT_TILE_BYTES;    // 2 slots
+  static constexpr uint32_t BAR_OFF = V_OFF + 2 * ATT_TILE_BYTES;
+  // q_full, k_full[2], v_full[2], kv_empty[2]
+  static constexpr uint32_t NUM_BARS = 7;
+  static constexpr uint32_t DYN_BYTES = BAR_OFF + NUM_BARS * 8 + 1024;
 };
 
-// Developer phase trace (compiled in only with -DNV_ATTN_TRACE, see tools/attn_trace.py): SM-clock stamps of the CTAs of
-// one head, read back through nv_debug_attn_trace(2, ...).
-#ifdef NV_ATTN_TRACE
-__device__ unsigned long long g_attn_fwd_trace[256 * 64];
-#define AF_TR(slot) do { if (blockIdx.y == 5 && blockIdx.x < 256) g_attn_fwd_trace[blockIdx.x * 64 + (slot)] = clock64(); } while (0)
-#define AF_TRV(slot, v) do { if (blockIdx.y == 5 && blockIdx.x < 256) g_attn_fwd_trace[blockIdx.x * 64 + (slot)] = (v); } while (0)
-#else
-#define AF_TR(slot) do {} while (0)
-#define AF_TRV(slot, v) do {} while (0)
-#endif
-
-// exp2 on the FMA pipe (Cody-Waite range reduction + degree-3 minimax polynomial on [-0.5, 0.5], max relative error
-// 7.5e-5: far below the bf16 rounding of P).  MUFU.EX2 runs at 16 results/clk/SM, exactly the rate at which a 128x128
-// score tile is consumed by the tensor pipe, so the softmax is MUFU-bound; moving a quarter of the exponentials to the
-// (otherwise mostly idle) FMA pipe shortens it.  x <= ~8 by construction (lazy rescale), clamped below at -125.
-__device__ __forceinline__ float2 exp2_fma2(float2 x) {
-  const float2 magic = make_float2(12582912.f, 12582912.f);               // 1.5 * 2^23: integer part lands in the low mantissa bits
-  x.x = fmaxf(x.x, -125.f);
-  x.y = fmaxf(x.y, -125.f);
-  const float2 r = __fadd2_rn(x, magic);
-  const float2 xi = __fadd2_rn(r, make_float2(-12582912.f, -12582912.f));
-  const float2 f = __fadd2_rn(x, make_float2(-xi.x, -xi.y));
-  float2 p = __ffma2_rn(make_float2(0.05517146f, 0.05517146f), f, make_float2(0.24261086f, 0.24261086f));
-  p = __ffma2_rn(p, f, make_float2(0.69326099f, 0.69326099f));
-  p = __ffma2_rn(p, f, make_float2(0.99992809f, 0.99992809f));
-  p.x = __int_as_float(__float_as_int(p.x) + (__float_as_int(r.x) << 23));
-  p.y = __int_as_float(__float_as_int(p.y) + (__float_as_int(r.y) << 23));
-  return p;
-}
-
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
-
-// Map a flat block id to (sequence, 256-row query block); heavy (late) blocks are launched first.
+// Map a flat block id to (sequence, 128-row query block); heavy (late) blocks are launched first.
 __device__ __forceinline__ bool locate_qblock(const int* __restrict__ cu, int B, uint32_t blk, int& seq_start,
                                               int& seq_len, uint32_t& qblk, int& seq_idx) {
   for (int b = 0; b < B; ++b) {
@@ -105,17 +58,13 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem + L::Q_OFF;
-  uint8_t* sKV = smem + L::KV_OFF;
-  uint8_t* sP = smem + L::P_OFF;
+  uint8_t* sK = smem + L::K_OFF;
+  uint8_t* sV = smem + L::V_OFF;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
   uint64_t* q_full = bars + 0;
-  uint64_t* kv_full = bars + 1;    // [3]
-  uint64_t* kv_empty = bars + 4;   // [3]
-  uint64_t* s_full = bars + 7;     // [2] per tile: S_t(j) is in TMEM
-  uint64_t* s_free = bars + 9;     // [2] per tile: S_t(j) has been read into registers
-  uint64_t* p_ready = bars + 11;   // [2] per tile: P_t(j) is in smem (and O_t rescaled if needed)
-  uint64_t* pv_done = bars + 13;   // [2] per tile: PV_t(j) has completed
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + L::NUM_BARS);
+  uint64_t* k_full = bars + 1;     // [2]
+  uint64_t* v_full = bars + 3;     // [2]
+  uint64_t* kv_empty = bars + 5;   // [2] both warpgroups are done with K_j and V_j of the slot
 
   const uint32_t warp = warp_id_uniform(), lane = threadIdx.x & 31;
   const uint32_t head = blockIdx.y;
@@ -129,298 +78,172 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   // dk = kv_len - seq_len.
   const int kv0 = kv_start ? kv_start[seq_idx] : seq_start;
   const uint32_t dk = kv_len ? (uint32_t)(kv_len[seq_idx] - seq_len) : 0u;
-  const uint32_t q0 = qblk * ATT_QROWS;                         // first query row (inside the sequence)
-  const bool tile1_on = (q0 + 128) < (uint32_t)seq_len;         // second tile has at least one real row
-  // key blocks seen by a tile: 0 .. ceil((dk + last real row + 1) / 128) - 1   (dk = 0: 2*qblk+1 and 2*qblk+2)
-  const uint32_t nb0 = (dk + min(q0 + 128, (uint32_t)seq_len) + 127) / 128;
-  const uint32_t nb1 = tile1_on ? (dk + min(q0 + 256, (uint32_t)seq_len) + 127) / 128 : 0u;
-  const uint32_t n_blocks = max(nb0, nb1);
-  auto tile_on = [&](uint32_t t, uint32_t j) -> bool { return j < (t == 0 ? nb0 : nb1); };
-  auto last_tile = [&](uint32_t j) -> uint32_t { return tile_on(1, j) ? 1u : 0u; };
-  if (threadIdx.x == 0) {
-    AF_TR(0); AF_TRV(3, n_blocks);
-#ifdef NV_ATTN_TRACE
-    unsigned sm; asm volatile("mov.u32 %0, %%smid;" : "=r"(sm)); AF_TRV(4, sm);
-    unsigned long long gt; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt)); AF_TRV(5, gt);
-#endif
-  }
+  const uint32_t q0 = qblk * ATT_QROWS;                                       // first query row (inside the sequence)
+  const uint32_t n_blocks = (dk + min(q0 + ATT_QROWS, (uint32_t)seq_len) + 127) / 128;   // key blocks the block sees
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmap_q); tma_prefetch_desc(&tmap_k); tma_prefetch_desc(&tmap_v);
+  if (threadIdx.x == 0) {
     mbar_init(q_full, 1);
-    for (int i = 0; i < 3; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&s_full[i], 1); mbar_init(&s_free[i], 4); mbar_init(&p_ready[i], 4); mbar_init(&pv_done[i], 1);
-    }
+    for (int i = 0; i < 2; ++i) { mbar_init(&k_full[i], 1); mbar_init(&v_full[i], 1); mbar_init(&kv_empty[i], 2); }
     fence_mbar_init();
   }
-  if (warp == 1) { tmem_alloc(tmem_ptr_smem, 512); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  if (threadIdx.x == 0) AF_TR(1);
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ================================ TMA producer ================================
-    // (whole warp runs the loop, one elected lane issues: see elect_one() in nv_common.cuh)
-    const int32_t qcol = head * 128;
-    const int32_t qrow0 = seq_start + q0;
+    tma_prefetch_desc(&tmap_q); tma_prefetch_desc(&tmap_k); tma_prefetch_desc(&tmap_v);
+    const int32_t col = head * 128;
     if (elect_one()) {
-      mbar_arrive_expect_tx(q_full, 2 * ATT_TILE_BYTES);
-#pragma unroll
-      for (int t = 0; t < 2; ++t) {
-        tma_load_2d(sQ + t * ATT_TILE_BYTES, &tmap_q, q_full, qcol, qrow0 + t * 128);
-        tma_load_2d(sQ + t * ATT_TILE_BYTES + ATT_ATOM_BYTES, &tmap_q, q_full, qcol + 64, qrow0 + t * 128);
-      }
+      mbar_arrive_expect_tx(q_full, ATT_TILE_BYTES);
+      tma_load_2d(sQ, &tmap_q, q_full, col, seq_start + q0);
+      tma_load_2d(sQ + ATT_ATOM_BYTES, &tmap_q, q_full, col + 64, seq_start + q0);
     }
     __syncwarp();
-    auto load_block = [&](uint32_t slot, uint32_t parity, const CUtensorMap* tm, uint32_t j) {
-      mbar_wait(&kv_empty[slot], parity);
+    for (uint32_t j = 0; j < n_blocks; ++j) {
+      const uint32_t slot = j & 1;
+      mbar_wait(&kv_empty[slot], ((j >> 1) & 1) ^ 1);
       if (elect_one()) {
-        uint8_t* dst = sKV + slot * ATT_TILE_BYTES;
         const int32_t krow0 = kv0 + j * 128;
-        mbar_arrive_expect_tx(&kv_full[slot], ATT_TILE_BYTES);
-        tma_load_2d(dst, tm, &kv_full[slot], qcol, krow0);
-        tma_load_2d(dst + ATT_ATOM_BYTES, tm, &kv_full[slot], qcol + 64, krow0);
+        mbar_arrive_expect_tx(&k_full[slot], ATT_TILE_BYTES);
+        tma_load_2d(sK + slot * ATT_TILE_BYTES, &tmap_k, &k_full[slot], col, krow0);
+        tma_load_2d(sK + slot * ATT_TILE_BYTES + ATT_ATOM_BYTES, &tmap_k, &k_full[slot], col + 64, krow0);
+        mbar_arrive_expect_tx(&v_full[slot], ATT_TILE_BYTES);
+        tma_load_2d(sV + slot * ATT_TILE_BYTES, &tmap_v, &v_full[slot], col, krow0);
+        tma_load_2d(sV + slot * ATT_TILE_BYTES + ATT_ATOM_BYTES, &tmap_v, &v_full[slot], col + 64, krow0);
       }
       __syncwarp();
-    };
-    // request order K0 K1 V0 K2 V1 K3 V2 ...: each wait is for the buffer that frees EARLIEST among what is still needed
-    load_block(0, 1, &tmap_k, 0);
-    if (n_blocks > 1) load_block(1, 1, &tmap_k, 1);
-    for (uint32_t j = 0; j < n_blocks; ++j) {
-      load_block(2, (j & 1) ^ 1, &tmap_v, j);                                   // V_j: slot 2, use j
-      if (j + 2 < n_blocks) load_block(j & 1, (((j + 2) >> 1) & 1) ^ 1, &tmap_k, j + 2);   // K_{j+2}: slot (j+2)&1, use (j+2)>>1
     }
-  } else if (warp == 1) {
-    // ================================ MMA issuer ================================
-    // The whole warp walks the (uniform) schedule; each group of tcgen05.mma + commit is issued by the elected lane,
-    // with every operand in uniform registers so that the MMAs go out back to back.
-    constexpr uint32_t idesc_s = umma_idesc_bf16(128, 128, 0, 0);   // Q (K-major) x K (K-major)
-    constexpr uint32_t idesc_pv = umma_idesc_bf16(128, 128, 0, 1);  // P (K-major) x V (MN-major: hd contiguous)
-    const uint64_t qd0 = umma_smem_desc_sw128(smem_u32(sQ), 0, 1024);
-    const uint64_t pd0 = umma_smem_desc_sw128(smem_u32(sP), 0, 1024);
-    const uint64_t kd0 = umma_smem_desc_sw128(smem_u32(sKV), 0, 1024);
-    // V tile: rows = keys (K dim), 128 B of hd per row per atom; atoms (hd halves) ATT_ATOM_BYTES apart
-    const uint64_t vd0 = umma_smem_desc_sw128(smem_u32(sKV), ATT_ATOM_BYTES, 1024);
-    auto wait_k = [&](uint32_t j) { mbar_wait(&kv_full[j & 1], (j >> 1) & 1); tc_fence_after(); };
-    auto wait_v = [&](uint32_t j) { mbar_wait(&kv_full[2], j & 1); tc_fence_after(); };
-    auto issue_s = [&](uint32_t t, uint32_t slot, uint64_t* extra_commit) {
-      if (elect_one()) {
-        const uint32_t d_tmem = tmem_base + t * 128;
-#pragma unroll
-        for (uint32_t ka = 0; ka < 2; ++ka)
-#pragma unroll
-          for (uint32_t ks = 0; ks < 4; ++ks)
-            umma_f16_ss(d_tmem, qd0 + ((t * ATT_TILE_BYTES + ka * ATT_ATOM_BYTES) >> 4) + ks * 2,
-                        kd0 + ((slot * ATT_TILE_BYTES + ka * ATT_ATOM_BYTES) >> 4) + ks * 2, idesc_s, (ka | ks) ? 1u : 0u);
-        umma_commit(&s_full[t]);
-        if (extra_commit) umma_commit(extra_commit);
-      }
-      __syncwarp();
-    };
-    auto issue_pv = [&](uint32_t t, uint32_t slot, bool accumulate, uint64_t* extra_commit) {
-      if (elect_one()) {
-        const uint32_t d_tmem = tmem_base + 256 + t * 128;
-#pragma unroll
-        for (uint32_t ka = 0; ka < 2; ++ka)
-#pragma unroll
-          for (uint32_t ks = 0; ks < 4; ++ks)   // key rows ka*64 + ks*16 -> byte offset * 128 >> 4
-            umma_f16_ss(d_tmem, pd0 + ((t * ATT_TILE_BYTES + ka * ATT_ATOM_BYTES) >> 4) + ks * 2,
-                        vd0 + ((slot * ATT_TILE_BYTES) >> 4) + ((ka * 64 + ks * 16) * 128 >> 4), idesc_pv,
-                        (accumulate || (ka | ks)) ? 1u : 0u);
-        umma_commit(&pv_done[t]);
-        if (extra_commit) umma_commit(extra_commit);
-      }
-      __syncwarp();
-    };
-    mbar_wait(q_full, 0);
-    wait_k(0);
-    if (lane == 0) AF_TR(2);
-    for (uint32_t t = 0; t < 2; ++t)
-      if (tile_on(t, 0)) issue_s(t, 0, t == last_tile(0) ? &kv_empty[0] : nullptr);
-    for (uint32_t j = 0; j < n_blocks; ++j) {
-      if (j + 1 < n_blocks) {                      // S(j+1): needs only the S registers of block j and K(j+1)
-        const uint32_t slot = (j + 1) & 1;
-        bool waited = false;
-        for (uint32_t t = 0; t < 2; ++t) {
-          if (!tile_on(t, j + 1)) continue;        // (implies tile_on(t, j))
-          mbar_wait(&s_free[t], j & 1);
-          tc_fence_after();
-          if (!waited) { wait_k(j + 1); waited = true; }
-          issue_s(t, slot, t == last_tile(j + 1) ? &kv_empty[slot] : nullptr);
-        }
-        if (lane == 0 && j < 8) AF_TR(10 + 3 * j);
-      }
-      const uint32_t vslot = 2;
-      bool vwaited = false;
-      for (uint32_t t = 0; t < 2; ++t) {
-        if (!tile_on(t, j)) continue;
-        mbar_wait(&p_ready[t], j & 1);             // tile t processes every block 0..its last, so its phase index is j
-        tc_fence_after();
-        if (!vwaited) { wait_v(j); vwaited = true; }
-        issue_pv(t, vslot, j > 0, t == last_tile(j) ? &kv_empty[vslot] : nullptr);
-        if (lane == 0 && j < 8) AF_TR(11 + 3 * j + t);
-      }
-    }
-  } else {
-    // ================================ softmax groups ================================
-    const uint32_t t = (warp - 2) >> 2;                   // tile of this group
-    const uint32_t quarter = warp & 3;
-    const uint32_t r = quarter * 32 + lane;               // row inside the tile
-    const uint32_t lane_off = (quarter * 32) << 16;       // TMEM lane field
-    const uint32_t tmem_S = tmem_base + t * 128, tmem_O = tmem_base + 256 + t * 128;
-    const uint32_t sPt_u32 = smem_u32(sP + t * ATT_TILE_BYTES);
-    const float sl2 = scale * 1.4426950408889634f;
-    const float2 sl2v = make_float2(sl2, sl2);
-    const uint32_t my_blocks = (t == 0) ? nb0 : nb1;
-    const uint32_t vis0 = dk + q0 + t * 128;               // last key visible to the tile's first row
-    float m_used = -INFINITY, l_run = 0.f;                 // exponent reference (log2 domain) and running row sum
-    for (uint32_t j = 0; j < my_blocks; ++j) {
-      mbar_wait(&s_full[t], j & 1);
-      if (warp == 2 && lane == 0 && j < 6) AF_TR(34 + 4 * j);
-      tc_fence_after();
-      // whole S row -> registers (4 x 32 columns), one wait; then the tensor pipe may overwrite S_t with block j+1
-      uint32_t s[128];
-      tmem_ld_32x32b_x32(tmem_S + lane_off + 0, *reinterpret_cast<uint32_t(*)[32]>(&s[0]));
-      tmem_ld_32x32b_x32(tmem_S + lane_off + 32, *reinterpret_cast<uint32_t(*)[32]>(&s[32]));
-      tmem_ld_32x32b_x32(tmem_S + lane_off + 64, *reinterpret_cast<uint32_t(*)[32]>(&s[64]));
-      tmem_ld_32x32b_x32(tmem_S + lane_off + 96, *reinterpret_cast<uint32_t(*)[32]>(&s[96]));
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&s_free[t]);
-      const bool diag = (j * 128 + 127 > vis0);             // block holds keys that some row of the tile must not see
-      const int lim = (int)(vis0 + r) - (int)(j * 128);     // this row sees columns 0 .. lim of the block
-      if (diag) {
-#pragma unroll
-        for (uint32_t i = 0; i < 128; ++i)
-          if ((int)i > lim) s[i] = 0xff800000u;             // -inf: exp2 -> 0, never the maximum
-      }
-      // four independent running maxima (3-input FMNMX3): a single dependent chain would cost its latency 64 times
-      float mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-      for (uint32_t i = 0; i < 128; i += 8) {
-        mx[0] = fmax3(mx[0], __uint_as_float(s[i + 0]), __uint_as_float(s[i + 1]));
-        mx[1] = fmax3(mx[1], __uint_as_float(s[i + 2]), __uint_as_float(s[i + 3]));
-        mx[2] = fmax3(mx[2], __uint_as_float(s[i + 4]), __uint_as_float(s[i + 5]));
-        mx[3] = fmax3(mx[3], __uint_as_float(s[i + 6]), __uint_as_float(s[i + 7]));
-      }
-      const float mb2 = fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3])) * sl2;
-      const bool need = mb2 > m_used + ATT_LAZY_LOG2;       // (first block: m_used = -inf)
-      const float m_new = need ? mb2 : m_used;
-      const float alpha = need ? exp2f(m_used - m_new) : 1.f;
-      const float2 nm = make_float2(-m_new, -m_new);
-      float2 rs0 = make_float2(0.f, 0.f), rs1 = make_float2(0.f, 0.f);
-#pragma unroll
-      for (uint32_t i = 0; i < 128; i += 4) {
-        float2 a = __ffma2_rn(make_float2(__uint_as_float(s[i]), __uint_as_float(s[i + 1])), sl2v, nm);
-        float2 b = __ffma2_rn(make_float2(__uint_as_float(s[i + 2]), __uint_as_float(s[i + 3])), sl2v, nm);
-        a.x = exp2f(a.x); a.y = exp2f(a.y);
-        if ((i & 4) != 0) {                                 // one pair in four on the FMA pipe (see exp2_fma2)
-          b = exp2_fma2(b);
-        } else {
-          b.x = exp2f(b.x); b.y = exp2f(b.y);
-        }
-        rs0 = __fadd2_rn(rs0, a);
-        rs1 = __fadd2_rn(rs1, b);
-        s[i >> 1] = pack_bf16x2(a.x, a.y);
-        s[(i >> 1) + 1] = pack_bf16x2(b.x, b.y);
-      }
-      const float rs = (rs0.x + rs0.y) + (rs1.x + rs1.y);
-      if (warp == 2 && lane == 0 && j < 6) AF_TR(35 + 4 * j);
-      if (j > 0) { mbar_wait(&pv_done[t], (j - 1) & 1); tc_fence_after(); }   // P_t buffer and O_t accumulator free again
-#pragma unroll
-      for (uint32_t c = 0; c < 16; ++c)                  // 16 chunks of 8 bf16 (16 B)
-        sts128(sPt_u32 + (c >> 3) * ATT_ATOM_BYTES + sw128_offset(r, c & 7), s[c * 4], s[c * 4 + 1], s[c * 4 + 2], s[c * 4 + 3]);
-      if (warp == 2 && lane == 0 && j < 6) AF_TR(36 + 4 * j);
-      l_run = l_run * alpha + rs;
-      m_used = m_new;
-      if (j > 0 && __any_sync(0xffffffffu, need)) {       // warp-uniform: the TMEM round trip is .sync.aligned
-#pragma unroll 1
-        for (uint32_t c = 0; c < 128; c += 32) {
-          uint32_t v[32];
-          tmem_ld_32x32b_x32(tmem_O + lane_off + c, v);
-          tmem_ld_wait();
-#pragma unroll
-          for (uint32_t i = 0; i < 32; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) * alpha);
-          tmem_st_32x32b_x32(tmem_O + lane_off + c, v);
-        }
-        tmem_st_wait();
-      }
-      fence_proxy_async_smem();  // P stores (generic proxy) -> visible to tcgen05.mma (async proxy)
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&p_ready[t]);
-      if (warp == 2 && lane == 0 && j < 6) AF_TR(37 + 4 * j);
-    }
-    // ---- epilogue ----
-    // Two phases so that HBM sees full 256-byte rows: each thread (= query row) rounds its normalised O row to bf16 into
-    // the group's P tile (free after the last PV; 16-byte chunks XOR-swizzled by the row: conflict-free for the row-per-
-    // thread writes and the row-per-warp reads), then each warp streams whole rows out with 8-byte coalesced stores.
-    if (my_blocks > 0) {
-      mbar_wait(&pv_done[t], (my_blocks - 1) & 1);
-      if (warp == 2 && lane == 0) AF_TR(58);
-      tc_fence_after();
-      const uint32_t qi = q0 + t * 128 + r;
-      const bool valid = qi < (uint32_t)seq_len;
-      const float inv_l = 1.f / l_run;
-      const int64_t tok = (int64_t)seq_start + qi;
-      const uint32_t srow = sPt_u32 + r * 256;
-#pragma unroll 1
-      for (uint32_t c = 0; c < 128; c += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(tmem_O + lane_off + c, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (uint32_t i = 0; i < 32; i += 8) {
-          uint4 o;
-          o.x = pack_bf16x2(__uint_as_float(v[i + 0]) * inv_l, __uint_as_float(v[i + 1]) * inv_l);
-          o.y = pack_bf16x2(__uint_as_float(v[i + 2]) * inv_l, __uint_as_float(v[i + 3]) * inv_l);
-          o.z = pack_bf16x2(__uint_as_float(v[i + 4]) * inv_l, __uint_as_float(v[i + 5]) * inv_l);
-          o.w = pack_bf16x2(__uint_as_float(v[i + 6]) * inv_l, __uint_as_float(v[i + 7]) * inv_l);
-          sts128(srow + ((((c + i) >> 3) ^ (r & 15)) << 4), o.x, o.y, o.z, o.w);
-        }
-      }
-      // natural-log LSE of the scaled scores: m_used is in log2 units
-      if (valid && lse) lse[(int64_t)head * T + tok] = m_used * 0.6931471805599453f + __logf(l_run);
-      asm volatile("bar.sync %0, 128;" ::"r"(1 + t) : "memory");        // the tile's four softmax warps
-      const uint32_t rows_valid = min(128u, (uint32_t)seq_len - (q0 + t * 128));
-      const uint32_t wq = warp & 3;
-      __nv_bfloat16* obase = O + ((int64_t)seq_start + q0 + t * 128) * ldo + head * 128;
-      for (uint32_t rr = wq; rr < rows_valid; rr += 4) {
-        const uint32_t chunk = (lane >> 1) ^ (rr & 15);
-        const uint2 x = lds64(sPt_u32 + rr * 256 + (chunk << 4) + ((lane & 1) << 3));
-        *reinterpret_cast<uint2*>(obase + (int64_t)rr * ldo + lane * 4) = x;
-      }
-      if (warp == 2 && lane == 0) AF_TR(59);
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, 512); }
-  if (threadIdx.x == 32) AF_TR(60);
-}
+  // ================================ consumers ================================
+  const uint32_t wg = warp >> 2;
+  const uint32_t ra = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's rows ra, ra + 8 (inside the block)
+  const uint32_t qa = q0 + ra, qb = qa + 8;                       // query index inside the sequence
+  const uint32_t cq = 2 * (lane & 3);                             // column offset of the thread's pairs
+  const float sl2 = scale * 1.4426950408889634f;
+  const uint32_t vis_first = dk + q0 + wg * 64;                   // last key visible to the warpgroup's first row
+  float oacc[64];
+#pragma unroll
+  for (uint32_t i = 0; i < 64; ++i) oacc[i] = 0.f;
+  float m_a = -INFINITY, m_b = -INFINITY, l_a = 0.f, l_b = 0.f;   // running max (log2 units) and partial row sums
+  const uint64_t qdesc = gmma_desc_sw128(smem_u32(sQ + wg * 8192), 0, 1024);
+  mbar_wait(q_full, 0);
+  for (uint32_t j = 0; j < n_blocks; ++j) {
+    const uint32_t slot = j & 1, par = (j >> 1) & 1;
+    float sacc[64];
+    mbar_wait(&k_full[slot], par);
+    {
+      const uint64_t kdesc = gmma_desc_sw128(smem_u32(sK + slot * ATT_TILE_BYTES), 0, 1024);
+      wgmma_fence();
+#pragma unroll
+      for (uint32_t ks = 0; ks < 8; ++ks)   // hd step 16 ks: atom ks / 4, +32 B per step inside it
+        wgmma_ss_bf16<128, 0, 0>(sacc, qdesc + (ks >> 2) * (ATT_ATOM_BYTES >> 4) + (ks & 3) * 2,
+                                 kdesc + (ks >> 2) * (ATT_ATOM_BYTES >> 4) + (ks & 3) * 2, ks ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(sacc);
+    }
+    if (j * 128 + 127 > vis_first) {                               // block holds keys some row must not see
+      const int lim_a = (int)(dk + qa) - (int)(j * 128), lim_b = lim_a + 8;
+#pragma unroll
+      for (uint32_t i = 0; i < 16; ++i) {
+        const int c = (int)(8 * i + cq);
+        if (c > lim_a) sacc[4 * i] = -INFINITY;
+        if (c + 1 > lim_a) sacc[4 * i + 1] = -INFINITY;
+        if (c > lim_b) sacc[4 * i + 2] = -INFINITY;
+        if (c + 1 > lim_b) sacc[4 * i + 3] = -INFINITY;
+      }
+    }
+    float mxa = -INFINITY, mxb = -INFINITY;
+#pragma unroll
+    for (uint32_t i = 0; i < 16; ++i) {
+      mxa = fmaxf(mxa, fmaxf(sacc[4 * i], sacc[4 * i + 1]));
+      mxb = fmaxf(mxb, fmaxf(sacc[4 * i + 2], sacc[4 * i + 3]));
+    }
+    mxa = fmaxf(mxa, __shfl_xor_sync(0xffffffffu, mxa, 1));
+    mxa = fmaxf(mxa, __shfl_xor_sync(0xffffffffu, mxa, 2));
+    mxb = fmaxf(mxb, __shfl_xor_sync(0xffffffffu, mxb, 1));
+    mxb = fmaxf(mxb, __shfl_xor_sync(0xffffffffu, mxb, 2));
+    // key 0 is visible to every row, so the maximum is finite from the first block on
+    const float mna = fmaxf(m_a, mxa * sl2), mnb = fmaxf(m_b, mxb * sl2);
+    const float alpha_a = exp2f(m_a - mna), alpha_b = exp2f(m_b - mnb);
+    m_a = mna; m_b = mnb;
+    float rsa = 0.f, rsb = 0.f;
+#pragma unroll
+    for (uint32_t i = 0; i < 16; ++i) {
+      sacc[4 * i] = exp2f(fmaf(sacc[4 * i], sl2, -mna));
+      sacc[4 * i + 1] = exp2f(fmaf(sacc[4 * i + 1], sl2, -mna));
+      sacc[4 * i + 2] = exp2f(fmaf(sacc[4 * i + 2], sl2, -mnb));
+      sacc[4 * i + 3] = exp2f(fmaf(sacc[4 * i + 3], sl2, -mnb));
+      rsa += sacc[4 * i] + sacc[4 * i + 1];
+      rsb += sacc[4 * i + 2] + sacc[4 * i + 3];
+    }
+    l_a = l_a * alpha_a + rsa;
+    l_b = l_b * alpha_b + rsb;
+#pragma unroll
+    for (uint32_t i = 0; i < 16; ++i) {
+      oacc[4 * i] *= alpha_a; oacc[4 * i + 1] *= alpha_a;
+      oacc[4 * i + 2] *= alpha_b; oacc[4 * i + 3] *= alpha_b;
+    }
+    // O += P V_j: P (bf16) from registers, 16 keys per wgmma; V rows = keys (K dim), hd contiguous (MN-major B)
+    mbar_wait(&v_full[slot], par);
+    {
+      const uint64_t vdesc = gmma_desc_sw128(smem_u32(sV + slot * ATT_TILE_BYTES), ATT_ATOM_BYTES, 1024);
+      wgmma_fence();
+#pragma unroll
+      for (uint32_t kk = 0; kk < 8; ++kk) {
+        const uint32_t a[4] = {pack_bf16x2(sacc[8 * kk], sacc[8 * kk + 1]), pack_bf16x2(sacc[8 * kk + 2], sacc[8 * kk + 3]),
+                               pack_bf16x2(sacc[8 * kk + 4], sacc[8 * kk + 5]), pack_bf16x2(sacc[8 * kk + 6], sacc[8 * kk + 7])};
+        wgmma_rs_bf16<128, 1>(oacc, a, vdesc + kk * ((16 * 128) >> 4), 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(oacc);
+    }
+    if ((threadIdx.x & 127) == 0) mbar_arrive(&kv_empty[slot]);
+  }
 
-int attn_fwd_trace_copy(unsigned long long* out, int max_words) {
-#ifdef NV_ATTN_TRACE
-  const int n = max_words < 256 * 64 ? max_words : 256 * 64;
-  if (cudaMemcpyFromSymbol(out, g_attn_fwd_trace, (size_t)n * 8, 0) != cudaSuccess) return 0;
-  return n;
-#else
-  (void)out; (void)max_words;
-  return 0;
-#endif
+  // ---- epilogue ----
+  l_a += __shfl_xor_sync(0xffffffffu, l_a, 1);
+  l_a += __shfl_xor_sync(0xffffffffu, l_a, 2);
+  l_b += __shfl_xor_sync(0xffffffffu, l_b, 1);
+  l_b += __shfl_xor_sync(0xffffffffu, l_b, 2);
+  // natural-log LSE of the scaled scores: m is in log2 units
+  if (lse && (lane & 3) == 0) {
+    if (qa < (uint32_t)seq_len) lse[(int64_t)head * T + seq_start + qa] = m_a * 0.6931471805599453f + __logf(l_a);
+    if (qb < (uint32_t)seq_len) lse[(int64_t)head * T + seq_start + qb] = m_b * 0.6931471805599453f + __logf(l_b);
+  }
+  // Two phases so that HBM sees full 256-byte rows: the normalised bf16 O rows of the warpgroup go into its own 16 KB
+  // of the K ring (free once both warpgroups are past the last block; 16-byte chunks XOR-swizzled by the row), then each
+  // warp streams whole rows out with 8-byte coalesced stores.
+  named_bar_sync(1, 256);
+  const uint32_t stg = smem_u32(sK + wg * 64 * 256);
+  const float inv_a = 1.f / l_a, inv_b = 1.f / l_b;
+  const uint32_t rl = ra - wg * 64;
+#pragma unroll
+  for (uint32_t i = 0; i < 16; ++i) {
+    const uint32_t c = 8 * i + cq;
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(stg + rl * 256 + ((((c >> 3) ^ (rl & 15))) << 4) + (c & 7) * 2),
+                 "r"(pack_bf16x2(oacc[4 * i] * inv_a, oacc[4 * i + 1] * inv_a)) : "memory");
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(stg + (rl + 8) * 256 + ((((c >> 3) ^ ((rl + 8) & 15))) << 4) + (c & 7) * 2),
+                 "r"(pack_bf16x2(oacc[4 * i + 2] * inv_b, oacc[4 * i + 3] * inv_b)) : "memory");
+  }
+  named_bar_sync(2 + wg, 128);
+  const uint32_t r0 = q0 + wg * 64;
+  const uint32_t rows_valid = (uint32_t)seq_len > r0 ? min(64u, (uint32_t)seq_len - r0) : 0u;
+  __nv_bfloat16* obase = O + ((int64_t)seq_start + r0) * ldo + head * 128;
+  for (uint32_t rr = warp & 3; rr < rows_valid; rr += 4) {
+    const uint32_t chunk = (lane >> 1) ^ (rr & 15);
+    const uint2 x = lds64(stg + rr * 256 + (chunk << 4) + ((lane & 1) << 3));
+    *reinterpret_cast<uint2*>(obase + (int64_t)rr * ldo + lane * 4) = x;
+  }
 }
 
 }  // namespace nv
 
 // q, k, v: bf16 row-major [T, *] views with leading dimensions ldq/ldk/ldv (elements); head h occupies
 // columns [h*128, (h+1)*128).  o: [T, H*128] bf16 (ldo).  lse: [H, T] fp32 or null.
-// cu_seqlens: device int32 [B+1]; total_qblocks = sum_b ceil(len_b / 128) (the host knows the lengths);
-// the kernel itself works on 256-row blocks: the grid is sized from an upper bound and surplus CTAs exit.
+// cu_seqlens: device int32 [B+1]; total_qblocks = sum_b ceil(len_b / 128) (the host knows the lengths): one CTA each.
 static int attn_fwd_launch(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* o,
                            int64_t ldo, float* lse, const int* cu_seqlens, const int* kv_start, const int* kv_len, int B, int T,
                            int Tkv, int H, int head_dim, int total_qblocks, float scale, void* stream) {
@@ -438,9 +261,7 @@ static int attn_fwd_launch(const void* q, int64_t ldq, const void* k, int64_t ld
     NV_CUDA(cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnFwdSmem::DYN_BYTES));
     attr_set = true;
   }
-  // sum_b ceil(len_b/256) <= ceil((total_qblocks + B) / 2): launch that many, CTAs beyond the real count return
-  const int grid_x = (total_qblocks + B + 1) / 2;
-  dim3 grid(grid_x, H);
+  dim3 grid(total_qblocks, H);
   attn_fwd_kernel<<<grid, ATT_THREADS, AttnFwdSmem::DYN_BYTES, reinterpret_cast<cudaStream_t>(stream)>>>(
       tq, tk, tv, reinterpret_cast<__nv_bfloat16*>(o), ldo, lse, cu_seqlens, B, T, scale, kv_start, kv_len);
   NV_LAUNCH_CHECK();

@@ -1,18 +1,19 @@
-// navillm_b200 — skinny bf16 GEMM for the decode step (M <= 16 activation rows), swap-AB on tcgen05.
+// navillm_b200 — skinny bf16 GEMM for the decode step (M <= 16 activation rows), swap-AB on wgmma.
 //
 // The per-token GEMMs of greedy/sampled generation (reference: HF GenerationMixin.generate through
 // models/modified_lm.py:184-199; SURVEY.md §8 a10, K13) multiply a handful of activation rows by every weight of
-// the model: pure HBM weight streaming.  The general kernel (gemm_bf16.cu) puts the activations on the UMMA M side,
+// the model: pure HBM weight streaming.  The general kernel (gemm_bf16.cu) puts the activations on the MMA M side,
 // so each CTA re-stages a mostly-zero 128-row activation tile per k-block and the N/128 output tiles of a 4096-wide
-// projection occupy 32 of 148 SMs.  Here the roles are swapped:
+// projection occupy 32 of 132 SMs.  Here the roles are swapped:
 //
-//   C^T[n, m] = sum_k W[n, k] * X[m, k]        UMMA M = 128 weight rows (A operand), UMMA N = 16 activation rows (B)
+//   C^T[n, m] = sum_k W[n, k] * X[m, k]        MMA M = 128 weight rows (A operand), MMA N = 16 activation rows (B)
 //
 // so a k-block moves 16 KB of weights + 2 KB of activations, and the K range of one weight tile is split over the
 // CTAs of a thread-block cluster (S = 1, 2, 4 or 8) whose partial accumulators are reduced through distributed
 // shared memory in the leader CTA - no atomics, no workspace, no second kernel.  4-stage rings of 18 KB let three
 // CTAs share an SM, so a 4096-column projection runs as 256 CTAs (S = 8) instead of 32.
-//   warp 0  TMA producer   warp 1  tcgen05.mma issuer   warps 2..5  epilogue (TMEM -> DSMEM reduce -> bf16 (+addend))
+//   warps 0..7  two consumer warpgroups, m64n16k16 wgmmas over weight rows 0..63 / 64..127 of the tile
+//   warp 8      TMA producer
 #include <stdlib.h>
 
 #include "nv_common.cuh"
@@ -20,17 +21,17 @@
 
 namespace nv {
 
-constexpr uint32_t SK_BN = 128;      // weight rows per tile (UMMA M)
-constexpr uint32_t SK_BM = 16;       // activation rows (UMMA N)
+constexpr uint32_t SK_BN = 128;      // weight rows per tile (MMA M)
+constexpr uint32_t SK_BM = 16;       // activation rows (MMA N)
 constexpr uint32_t SK_BK = 64;
 constexpr uint32_t SK_STAGES = 4;
-constexpr uint32_t SK_THREADS = 192;
+constexpr uint32_t SK_THREADS = 288;
 constexpr uint32_t SK_W_BYTES = SK_BN * SK_BK * 2, SK_X_BYTES = SK_BM * SK_BK * 2;
 constexpr uint32_t SK_STAGE_BYTES = SK_W_BYTES + SK_X_BYTES;
 constexpr uint32_t SK_BAR_OFF = SK_STAGES * SK_STAGE_BYTES;
-constexpr uint32_t SK_DYN_BYTES = SK_BAR_OFF + (2 * SK_STAGES + 1) * 8 + 16 + 1024;
+constexpr uint32_t SK_DYN_BYTES = SK_BAR_OFF + 2 * SK_STAGES * 8 + 1024;
 constexpr uint32_t SK_RED_BYTES = SK_BM * SK_BN * 4;   // one partner's partial tile [16 m][128 n] fp32 (8 KB)
-static_assert(7 * SK_RED_BYTES <= SK_STAGES * SK_W_BYTES, "reduction buffers reuse the weight stages");
+static_assert(8 * SK_RED_BYTES <= SK_STAGES * SK_W_BYTES, "reduction buffers and the output tile reuse the weight stages");
 
 __device__ __forceinline__ uint32_t sk_cluster_rank() {
   uint32_t r;
@@ -53,19 +54,17 @@ __device__ __forceinline__ void sk_st_remote_f32(float* p, uint32_t cta, float v
 // rows F + n_blk*64.. (two 64-row TMA boxes), the leader pairs them and writes h[m, n] = bf16(bf16(silu(g)) * u), the
 // same rounding points as swiglu_fwd_kernel on the bf16 gate|up buffer (which is not materialised here).
 __global__ void __launch_bounds__(SK_THREADS)
-gemm_skinny_tcgen05(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_x,
-                    __nv_bfloat16* __restrict__ C, int64_t ldc, const __nv_bfloat16* __restrict__ addend, int64_t ld_add,
-                    uint32_t M, uint32_t N, uint32_t K, uint32_t splits, uint32_t swiglu_f) {
+gemm_skinny_wgmma(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_x,
+                  __nv_bfloat16* __restrict__ C, int64_t ldc, const __nv_bfloat16* __restrict__ addend, int64_t ld_add,
+                  uint32_t M, uint32_t N, uint32_t K, uint32_t splits, uint32_t swiglu_f) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_w = smem;
   uint8_t* smem_x = smem + SK_STAGES * SK_W_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SK_BAR_OFF);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + SK_STAGES;
-  uint64_t* acc_full = bars + 2 * SK_STAGES;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 2 * SK_STAGES + 1);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + SK_BAR_OFF);
+  uint64_t* empty_bar = full_bar + SK_STAGES;
   float* red = reinterpret_cast<float*>(smem_w);          // leader: [splits-1][16][128] fp32, valid after the main loop
+  float* ex = red + 7 * SK_BM * SK_BN;                    // leader: the reduced tile [16 m][128 n]
 
   const uint32_t warp = warp_id_uniform(), lane = threadIdx.x & 31;
   const uint32_t rank = splits > 1 ? sk_cluster_rank() : 0u;
@@ -75,21 +74,20 @@ gemm_skinny_tcgen05(const __grid_constant__ CUtensorMap tmap_w, const __grid_con
   const uint32_t kb0 = min(rank * kb_per, total_kb);
   const uint32_t nkb = min(kb_per, total_kb - kb0);        // may be 0 for a trailing split: contributes zeros
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmap_w);
-    tma_prefetch_desc(&tmap_x);
-    for (uint32_t i = 0; i < SK_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    mbar_init(acc_full, 1);
+  if (threadIdx.x == 0) {
+    for (uint32_t i = 0; i < SK_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 2); }
     fence_mbar_init();
   }
-  if (warp == 1) { tmem_alloc(tmem_ptr_smem, 32); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
   griddep_launch();                                        // the next kernel of the stream may start its own prologue
-  if (warp == 0) {
+  float acc[8];
+#pragma unroll
+  for (uint32_t i = 0; i < 8; ++i) acc[i] = 0.f;
+  const uint32_t wg = warp >> 2;
+  if (warp == 8) {
+    tma_prefetch_desc(&tmap_w);
+    tma_prefetch_desc(&tmap_x);
     const int32_t n0 = swiglu_f ? n_blk * 64 : n_blk * SK_BN;
     auto load_w = [&](uint32_t stage, int32_t k0) {
       if (swiglu_f) {                                                                   // box {64 k, 64 n}: gate half, up half
@@ -127,69 +125,68 @@ gemm_skinny_tcgen05(const __grid_constant__ CUtensorMap tmap_w, const __grid_con
       }
       __syncwarp();
     }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = umma_idesc_bf16(SK_BN, SK_BM, 0, 0);
+  } else {
     for (uint32_t i = 0; i < nkb; ++i) {
       const uint32_t stage = i % SK_STAGES, phase = (i / SK_STAGES) & 1;
       mbar_wait(&full_bar[stage], phase);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint64_t wdesc = umma_smem_desc_sw128(smem_u32(smem_w + stage * SK_W_BYTES), 0, 1024);
-        const uint64_t xdesc = umma_smem_desc_sw128(smem_u32(smem_x + stage * SK_X_BYTES), 0, 1024);
+      const uint64_t wdesc = gmma_desc_sw128(smem_u32(smem_w + stage * SK_W_BYTES + wg * 8192), 0, 1024);
+      const uint64_t xdesc = gmma_desc_sw128(smem_u32(smem_x + stage * SK_X_BYTES), 0, 1024);
+      wgmma_fence();
 #pragma unroll
-        for (uint32_t k = 0; k < SK_BK / 16; ++k)
-          umma_f16_ss(tmem_base, wdesc + k * 2, xdesc + k * 2, idesc, (i | k) != 0 ? 1u : 0u);
-        umma_commit(&empty_bar[stage]);
-        if (i + 1 == nkb) umma_commit(acc_full);
-      }
-      __syncwarp();
+      for (uint32_t k = 0; k < SK_BK / 16; ++k) wgmma_ss_bf16<16, 0, 0>(acc, wdesc + k * 2, xdesc + k * 2, 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[stage]);
     }
+    reg_fence(acc);
+    griddep_wait();                                        // before the first read of `addend` / write of C
   }
 
-  // ---- epilogue: this CTA's partial C^T tile [128 n (TMEM lanes) x 16 m (columns)] -------------------------------
-  float acc[SK_BM];
-  const uint32_t quarter = warp & 3;
-  const uint32_t nl = quarter * 32 + lane;               // weight row inside the tile (epilogue warps only)
-  if (warp >= 2) {
-    griddep_wait();                                        // before the first read of `addend` / write of C
-    if (nkb > 0) {
-      mbar_wait(acc_full, 0);
-      tc_fence_after();
-      uint32_t v[16];
-      tmem_ld_32x32b_x16(tmem_base + ((quarter * 32) << 16), v);
-      tmem_ld_wait();
-#pragma unroll
-      for (uint32_t m = 0; m < SK_BM; ++m) acc[m] = __uint_as_float(v[m]);
-    } else {
-#pragma unroll
-      for (uint32_t m = 0; m < SK_BM; ++m) acc[m] = 0.f;
-    }
-  }
+  // ---- this CTA's partial C^T tile: thread holds weight rows nr, nr + 8 and activation rows mc, mc + 1, mc + 8, mc + 9 ----
+  const uint32_t nr = wg * 64 + ((threadIdx.x & 127) >> 5) * 16 + (lane >> 2), mc = 2 * (lane & 3);
+  auto frag = [&](uint32_t j, uint32_t& m, uint32_t& n) {  // element j of acc[8] -> (m, n) in the tile
+    n = nr + ((j >> 1) & 1) * 8;
+    m = mc + (j & 1) + (j >> 2) * 8;
+  };
   if (splits > 1) {
     sk_cluster_sync();                                     // every CTA of the cluster is past its main loop: stages are free
-    if (warp >= 2 && rank != 0) {
+    if (warp < 8 && rank != 0) {
 #pragma unroll
-      for (uint32_t m = 0; m < SK_BM; ++m)
-        if (m < M) sk_st_remote_f32(red + ((rank - 1) * SK_BM + m) * SK_BN + nl, 0, acc[m]);
+      for (uint32_t j = 0; j < 8; ++j) {
+        uint32_t m, n;
+        frag(j, m, n);
+        if (m < M) sk_st_remote_f32(red + ((rank - 1) * SK_BM + m) * SK_BN + n, 0, acc[j]);
+      }
     }
     sk_cluster_sync();                                     // partials visible in the leader
-    if (warp >= 2 && rank == 0) {
+    if (warp < 8 && rank == 0) {
       for (uint32_t r = 0; r + 1 < splits; ++r)
 #pragma unroll
-        for (uint32_t m = 0; m < SK_BM; ++m)
-          if (m < M) acc[m] += red[(r * SK_BM + m) * SK_BN + nl];
+        for (uint32_t j = 0; j < 8; ++j) {
+          uint32_t m, n;
+          frag(j, m, n);
+          if (m < M) acc[j] += red[(r * SK_BM + m) * SK_BN + n];
+        }
+    }
+  } else {
+    __syncthreads();                                       // both warpgroups are done with the weight stages
+  }
+  if (rank != 0) return;
+  // the reduced tile -> ex[16 m][128 n] (bf16-rounded: every output below rounds the projection first)
+  if (warp < 8) {
+#pragma unroll
+    for (uint32_t j = 0; j < 8; ++j) {
+      uint32_t m, n;
+      frag(j, m, n);
+      ex[m * SK_BN + n] = bf16_round(acc[j]);
     }
   }
+  __syncthreads();
+  const uint32_t nl = threadIdx.x;                         // weight row inside the tile
+  if (nl >= SK_BN) return;
   if (swiglu_f) {
-    // pair lane nl < 64 (gate column) with lane nl + 64 (up column) through the last 8 KB of the weight stages
-    float* ex = red + 7 * SK_BM * SK_BN;
-    if (splits == 1) __syncthreads();                      // (with a cluster the two cluster syncs already ordered the stages)
-    if (warp >= 2 && rank == 0) {
-#pragma unroll
-      for (uint32_t m = 0; m < SK_BM; ++m) ex[m * SK_BN + nl] = bf16_round(acc[m]);
-    }
-    __syncthreads();
-    if (warp >= 2 && rank == 0 && nl < 64) {
+    // pair gate row nl < 64 with up row nl + 64
+    if (nl < 64) {
       const uint32_t n = n_blk * 64 + nl;
       if (n < N) {
 #pragma unroll
@@ -201,23 +198,19 @@ gemm_skinny_tcgen05(const __grid_constant__ CUtensorMap tmap_w, const __grid_con
         }
       }
     }
-  } else if (warp >= 2 && rank == 0) {
+  } else {
     const uint32_t n = n_blk * SK_BN + nl;
     if (n < N) {
 #pragma unroll
       for (uint32_t m = 0; m < SK_BM; ++m) {
         if (m < M) {
-          float x = bf16_round(acc[m]);
+          float x = ex[m * SK_BN + nl];
           if (addend) x += __bfloat162float(addend[(int64_t)m * ld_add + n]);
           C[(int64_t)m * ldc + n] = __float2bfloat16_rn(x);
         }
       }
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, 32); }
 }
 
 }  // namespace nv
@@ -232,7 +225,7 @@ static int skinny_launch(const void* X, int64_t ldx, const void* W, int64_t ldw,
   if ((rc = make_tmap_2d(&tx, X, 2, (uint64_t)K, (uint64_t)M, (uint64_t)ldx * 2, 64, SK_BM))) return rc;
   static bool attr_set = false;
   if (!attr_set) {
-    NV_CUDA(cudaFuncSetAttribute(gemm_skinny_tcgen05, cudaFuncAttributeMaxDynamicSharedMemorySize, SK_DYN_BYTES));
+    NV_CUDA(cudaFuncSetAttribute(gemm_skinny_wgmma, cudaFuncAttributeMaxDynamicSharedMemorySize, SK_DYN_BYTES));
     attr_set = true;
   }
   const uint32_t tiles = ceil_div_u32(N, swiglu_f ? 64 : SK_BN), total_kb = ceil_div_u32(K, SK_BK);
@@ -264,7 +257,7 @@ static int skinny_launch(const void* X, int64_t ldx, const void* W, int64_t ldw,
     attr[1].val.programmaticStreamSerializationAllowed = 1;
     cfg.numAttrs = 2;
   }
-  NV_CUDA(cudaLaunchKernelEx(&cfg, gemm_skinny_tcgen05, tw, tx, reinterpret_cast<__nv_bfloat16*>(C), ldc,
+  NV_CUDA(cudaLaunchKernelEx(&cfg, gemm_skinny_wgmma, tw, tx, reinterpret_cast<__nv_bfloat16*>(C), ldc,
                              reinterpret_cast<const __nv_bfloat16*>(addend), ld_add, (uint32_t)M, (uint32_t)N, (uint32_t)K,
                              splits, swiglu_f));
   return NV_OK;

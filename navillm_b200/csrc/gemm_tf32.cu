@@ -1,4 +1,4 @@
-// navillm_b200 — fp32-in / fp32-out GEMM on tcgen05 tensor cores (kind::tf32) for the panorama encoder.
+// navillm_b200 — fp32-in / fp32-out GEMM on Hopper tensor cores (wgmma .tf32) for the panorama encoder.
 //
 // Replaces the cuBLAS GEMMs behind the fp32 nn.Linear / nn.MultiheadAttention projections of the reference's
 // image-embedding stack (models/image_embedding.py:51-121, models/detr_transformer.py:170-182; SURVEY.md §8 a2/a3).
@@ -7,186 +7,187 @@
 // kernel makes the same numerical choice.  The exact-fp32 CUDA-core kernel (nv_sgemm) stays available
 // (ops.set_pano_precision("fp32")) and is what the tight-tolerance parity tests use.
 //
-//   C[M,N] (+)= op(A) · op(B) (+ bias[N])      fp32 operands read as TF32 (10-bit mantissa), fp32 accumulate in TMEM
+//   C[M,N] (+)= op(A) · op(B) (+ bias[N])      fp32 operands read as TF32 (10-bit mantissa), fp32 accumulate
 //   ta = 0 : A stored [M,K]   ta = 1 : A stored [K,M]      tb = 0 : B stored [N,K]   tb = 1 : B stored [K,N]
 //
 // The encoder's problems are small (M = B*36 rows): one 128 x 128 tile per CTA, the K range split over blockIdx.y
-// so that a few hundred CTAs are in flight; splits add their partial sums with fp32 reductions (red.global.add).
-//   warp 0  TMA producer (32-float = 128-byte swizzled rows, 6-stage ring)   warp 1  tcgen05.mma issuer (K = 8 / MMA)
-//   warps 2..5  epilogue: tcgen05.ld -> (+bias) -> store / red.add
+// so that a few hundred CTAs are in flight.  The splits of a tile form one thread-block cluster and add their partial
+// tiles in rank order in the leader's shared memory (distributed shared memory): the result does not depend on timing,
+// and no atomics, workspace or memset are needed.
+// The tf32 form of wgmma reads both operands K-major from shared memory only, so the two warpgroups stage every
+// 32-wide k-block themselves: global -> registers (the next k-block's loads are in flight while the current one is
+// multiplied) -> 128-byte-swizzled K-major rows in one of two shared-memory buffers, whatever the HBM layout
+// (an MN-major operand is transposed on the way).  Each warpgroup then issues m64n128k8 wgmmas for its 64 rows.
 #include "nv_common.cuh"
 #include "nv_host.h"
 
 namespace nv {
 
-constexpr uint32_t T32_BM = 128, T32_BN = 128, T32_BK = 32, T32_UK = 8, T32_STAGES = 6, T32_THREADS = 192;
-constexpr uint32_t T32_A_BYTES = T32_BM * T32_BK * 4, T32_B_BYTES = T32_BN * T32_BK * 4;
-constexpr uint32_t T32_BAR_OFF = T32_STAGES * (T32_A_BYTES + T32_B_BYTES);
-constexpr uint32_t T32_DYN_BYTES = T32_BAR_OFF + (2 * T32_STAGES + 1) * 8 + 16 + 1024;
+constexpr uint32_t T32_BM = 128, T32_BN = 128, T32_BK = 32, T32_THREADS = 256;
+constexpr uint32_t T32_TILE_BYTES = 128 * T32_BK * 4;            // one operand tile: 128 rows x 128 B
+constexpr uint32_t T32_DYN_BYTES = 2 * 2 * T32_TILE_BYTES + 1024;  // two buffers of (A, B)
 
-__host__ __device__ constexpr uint32_t umma_idesc_tf32(uint32_t M, uint32_t N, uint32_t a_mn, uint32_t b_mn) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | (a_mn << 15) | (b_mn << 16) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-// MN-major 32-bit operands must use the 128B_BASE32B layout (layout type 1: 32-byte chunks swizzled over groups of
-// FOUR 128-byte k-rows; TMA CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B writes it): SBO = 4 k-rows = 512 B, LBO = distance
-// between 32-float MN atoms.
-__device__ __forceinline__ uint64_t umma_smem_desc_mn32(uint32_t smem_addr, uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= static_cast<uint64_t>((512u >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(1) << 61;
-  return d;
-}
-__device__ __forceinline__ void umma_tf32_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
+// One 128-row x 32-k operand tile: 4 x 16 B per thread.  K-major source X[row][k]: a thread loads 4 consecutive k of
+// one row.  MN-major source X[k][row]: a thread loads 4 consecutive rows of one k (lanes walk k, so that the transposed
+// shared-memory writes of a warp hit 32 different banks).
+template <bool MN>
+struct T32Tile {
+  float4 v[4];
+  __device__ __forceinline__ void load(const float* __restrict__ X, int64_t ld, uint32_t row0, uint32_t rows, uint32_t k0,
+                                       uint32_t K) {
+#pragma unroll
+    for (uint32_t i = 0; i < 4; ++i) {
+      const uint32_t idx = threadIdx.x + i * T32_THREADS;
+      float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
+      if constexpr (!MN) {
+        const uint32_t r = row0 + (idx >> 3), k = k0 + (idx & 7) * 4;
+        if (r < rows) {
+          const float* p = X + (int64_t)r * ld + k;
+          if (k + 4 <= K) x = *reinterpret_cast<const float4*>(p);
+          else {
+            if (k < K) x.x = p[0];
+            if (k + 1 < K) x.y = p[1];
+            if (k + 2 < K) x.z = p[2];
+          }
+        }
+      } else {
+        const uint32_t k = k0 + (idx & 31), r = row0 + (idx >> 5) * 4;
+        if (k < K) {
+          const float* p = X + (int64_t)k * ld + r;
+          if (r + 4 <= rows) x = *reinterpret_cast<const float4*>(p);
+          else {
+            if (r < rows) x.x = p[0];
+            if (r + 1 < rows) x.y = p[1];
+            if (r + 2 < rows) x.z = p[2];
+          }
+        }
+      }
+      v[i] = x;
+    }
+  }
+  // -> K-major 128-byte-swizzled rows (32 k = 128 B per row) at shared address `dst`
+  __device__ __forceinline__ void store(uint32_t dst) const {
+#pragma unroll
+    for (uint32_t i = 0; i < 4; ++i) {
+      const uint32_t idx = threadIdx.x + i * T32_THREADS;
+      if constexpr (!MN) {
+        const uint32_t r = idx >> 3, c = idx & 7;
+        sts128(dst + sw128_offset(r, c), __float_as_uint(v[i].x), __float_as_uint(v[i].y), __float_as_uint(v[i].z),
+               __float_as_uint(v[i].w));
+      } else {
+        const uint32_t k = idx & 31, r = (idx >> 5) * 4;
+        const float e[4] = {v[i].x, v[i].y, v[i].z, v[i].w};
+#pragma unroll
+        for (uint32_t j = 0; j < 4; ++j)
+          asm volatile("st.shared.f32 [%0], %1;" ::"r"(dst + sw128_offset(r + j, k >> 2) + (k & 3) * 4), "f"(e[j]) : "memory");
+      }
+    }
+  }
+};
 
 template <bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(T32_THREADS, 1)
-gemm_tf32_tcgen05(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                  float* __restrict__ C, int64_t ldc, const float* __restrict__ bias, uint32_t M, uint32_t N, uint32_t K,
-                  uint32_t num_n, uint32_t kb_per_split, uint32_t reduce) {
+gemm_tf32_wgmma(const float* __restrict__ A, int64_t lda, const float* __restrict__ B, int64_t ldb, float* __restrict__ C,
+                int64_t ldc, const float* __restrict__ bias, uint32_t M, uint32_t N, uint32_t K, uint32_t num_n,
+                uint32_t kb_per_split, uint32_t accumulate) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + T32_STAGES * T32_A_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + T32_BAR_OFF);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + T32_STAGES;
-  uint64_t* acc_full = bars + 2 * T32_STAGES;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 2 * T32_STAGES + 1);
+  const uint32_t sbase = (smem_u32(smem_raw) + 1023) & ~1023u;
+  auto sA = [&](uint32_t buf) { return sbase + buf * 2 * T32_TILE_BYTES; };
+  auto sB = [&](uint32_t buf) { return sbase + buf * 2 * T32_TILE_BYTES + T32_TILE_BYTES; };
 
-  const uint32_t warp = warp_id_uniform(), lane = threadIdx.x & 31;
   const uint32_t m_blk = blockIdx.x / num_n, n_blk = blockIdx.x % num_n;
+  const uint32_t m0 = m_blk * T32_BM, n0 = n_blk * T32_BN;
   const uint32_t total_kb = ceil_div_u32(K, T32_BK);
   const uint32_t kb0 = blockIdx.y * kb_per_split;
   const uint32_t nkb = min(kb_per_split, total_kb - kb0);   // host guarantees kb0 < total_kb
+  const uint32_t wg = threadIdx.x >> 7;
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmap_a);
-    tma_prefetch_desc(&tmap_b);
-    for (uint32_t i = 0; i < T32_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    mbar_init(acc_full, 1);
-    fence_mbar_init();
-  }
-  if (warp == 1) { tmem_alloc(tmem_ptr_smem, T32_BN); tmem_relinquish(); }
-  tc_fence_before();
+  T32Tile<A_MN> ta;
+  T32Tile<B_MN> tb;
+  ta.load(A, lda, m0, M, kb0 * T32_BK, K);
+  tb.load(B, ldb, n0, N, kb0 * T32_BK, K);
+  ta.store(sA(0));
+  tb.store(sB(0));
+  fence_proxy_async_smem();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    const int32_t m0 = m_blk * T32_BM, n0 = n_blk * T32_BN;
-    for (uint32_t i = 0; i < nkb; ++i) {
-      const uint32_t stage = i % T32_STAGES, phase = (i / T32_STAGES) & 1;
-      mbar_wait(&empty_bar[stage], phase ^ 1);
-      if (elect_one()) {
-        mbar_arrive_expect_tx(&full_bar[stage], T32_A_BYTES + T32_B_BYTES);
-        const int32_t k0 = (kb0 + i) * T32_BK;
-        uint8_t* sa = smem_a + stage * T32_A_BYTES;
-        uint8_t* sb = smem_b + stage * T32_B_BYTES;
-        if constexpr (!A_MN) {
-          tma_load_2d(sa, &tmap_a, &full_bar[stage], k0, m0);          // box {32 k, 128 m}
-        } else {
+  float acc[64];
 #pragma unroll
-          for (uint32_t a = 0; a < T32_BM / 32; ++a)                    // box {32 m, 32 k} per 32-wide MN atom
-            tma_load_2d(sa + a * (T32_BK * 128), &tmap_a, &full_bar[stage], m0 + a * 32, k0);
-        }
-        if constexpr (!B_MN) {
-          tma_load_2d(sb, &tmap_b, &full_bar[stage], k0, n0);
-        } else {
-#pragma unroll
-          for (uint32_t a = 0; a < T32_BN / 32; ++a)
-            tma_load_2d(sb + a * (T32_BK * 128), &tmap_b, &full_bar[stage], n0 + a * 32, k0);
-        }
-      }
-      __syncwarp();
+  for (uint32_t i = 0; i < 64; ++i) acc[i] = 0.f;
+  for (uint32_t i = 0; i < nkb; ++i) {
+    const uint32_t buf = i & 1;
+    const bool more = i + 1 < nkb;
+    if (more) {                                            // next k-block's loads in flight under this one's wgmmas
+      ta.load(A, lda, m0, M, (kb0 + i + 1) * T32_BK, K);
+      tb.load(B, ldb, n0, N, (kb0 + i + 1) * T32_BK, K);
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    constexpr uint32_t idesc = umma_idesc_tf32(T32_BM, T32_BN, A_MN ? 1u : 0u, B_MN ? 1u : 0u);
-    // K-major: 8 floats = 32 B per MMA inside the 128-byte swizzle span.  MN-major (128B_BASE32B): LBO = one 32-wide
-    // MN atom (BK rows x 128 B), SBO = 4 k-rows; an MMA advances 8 k-rows = 1024 B.
-    constexpr uint32_t A_LBO = A_MN ? T32_BK * 128 : 0, B_LBO = B_MN ? T32_BK * 128 : 0;
-    constexpr uint32_t A_KADV = A_MN ? (T32_UK * 128) >> 4 : (T32_UK * 4) >> 4;
-    constexpr uint32_t B_KADV = B_MN ? (T32_UK * 128) >> 4 : (T32_UK * 4) >> 4;
-    for (uint32_t i = 0; i < nkb; ++i) {
-      const uint32_t stage = i % T32_STAGES, phase = (i / T32_STAGES) & 1;
-      mbar_wait(&full_bar[stage], phase);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t sa = smem_u32(smem_a + stage * T32_A_BYTES), sb = smem_u32(smem_b + stage * T32_B_BYTES);
-        const uint64_t adesc = A_MN ? umma_smem_desc_mn32(sa, A_LBO) : umma_smem_desc_sw128(sa, 0, 1024);
-        const uint64_t bdesc = B_MN ? umma_smem_desc_mn32(sb, B_LBO) : umma_smem_desc_sw128(sb, 0, 1024);
+    const uint64_t adesc = gmma_desc_sw128(sA(buf) + wg * 8192, 0, 1024);
+    const uint64_t bdesc = gmma_desc_sw128(sB(buf), 0, 1024);
+    wgmma_fence();
 #pragma unroll
-        for (uint32_t k = 0; k < T32_BK / T32_UK; ++k)
-          umma_tf32_ss(tmem_base, adesc + k * A_KADV, bdesc + k * B_KADV, idesc, (i | k) != 0 ? 1u : 0u);
-        umma_commit(&empty_bar[stage]);
-        if (i + 1 == nkb) umma_commit(acc_full);
-      }
-      __syncwarp();
+    for (uint32_t k = 0; k < T32_BK / 8; ++k) wgmma_ss_tf32_n128(acc, adesc + k * 2, bdesc + k * 2, 1u);
+    wgmma_commit();
+    if (more) {                                            // the other buffer was released by the previous wait
+      ta.store(sA(buf ^ 1));
+      tb.store(sB(buf ^ 1));
+      fence_proxy_async_smem();
     }
-  } else {
-    // ===================== epilogue (warps 2..5) =====================
-    const uint32_t quarter = warp & 3;
-    mbar_wait(acc_full, 0);
-    tc_fence_after();
-    const uint32_t row = m_blk * T32_BM + quarter * 32 + lane;
-    const uint32_t col0 = n_blk * T32_BN;
-    const uint32_t taddr = tmem_base + ((quarter * 32) << 16);
-    const bool add_bias = bias != nullptr && blockIdx.y == 0;
-#pragma unroll 1
-    for (uint32_t c = 0; c < T32_BN; c += 32) {
-      uint32_t v[32];
-      tmem_ld_32x32b_x32(taddr + c, v);
-      tmem_ld_wait();
-      const uint32_t col = col0 + c;
-      if (row < M && col < N) {
-        float* dst = C + static_cast<int64_t>(row) * ldc + col;
-        if (!reduce && col + 32 <= N && (ldc & 3) == 0) {
+    wgmma_wait<0>();
+    __syncthreads();
+  }
+  reg_fence(acc);
+
+  // ---- split-K: running sum in the leader's operand buffers (64 KB = 64 floats x 256 threads), ranks in order ----
+  if (gridDim.y > 1) {
+    const uint32_t rank = blockIdx.y;                      // cluster (1, splits, 1): the rank is the split index
+    if (rank == 0) {
 #pragma unroll
-          for (uint32_t j = 0; j < 32; j += 4) {
-            float4 o = make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]),
-                                   __uint_as_float(v[j + 3]));
-            if (add_bias) {
-              const float4 b = *reinterpret_cast<const float4*>(bias + col + j);
-              o.x += b.x; o.y += b.y; o.z += b.z; o.w += b.w;
-            }
-            *reinterpret_cast<float4*>(dst + j) = o;
-          }
-        } else {
+      for (uint32_t i = 0; i < 64; ++i)
+        asm volatile("st.shared.f32 [%0], %1;" ::"r"(sbase + (i * T32_THREADS + threadIdx.x) * 4), "f"(acc[i]) : "memory");
+    }
+    cluster_sync_all();
+    for (uint32_t r = 1; r < gridDim.y; ++r) {
+      if (rank == r) {
 #pragma unroll
-          for (uint32_t j = 0; j < 32; ++j) {
-            if (col + j < N) {
-              float x = __uint_as_float(v[j]);
-              if (add_bias) x += bias[col + j];
-              if (reduce) atomicAdd(dst + j, x);
-              else dst[j] = x;
-            }
-          }
+        for (uint32_t i = 0; i < 64; ++i) dsmem_add_f32(sbase + (i * T32_THREADS + threadIdx.x) * 4, 0, acc[i]);
+      }
+      cluster_sync_all();
+    }
+    if (rank != 0) return;
+#pragma unroll
+    for (uint32_t i = 0; i < 64; ++i)
+      asm volatile("ld.shared.f32 %0, [%1];" : "=f"(acc[i]) : "r"(sbase + (i * T32_THREADS + threadIdx.x) * 4) : "memory");
+  }
+
+  // ---- epilogue straight from the accumulator fragment: rows r, r + 8; columns 8 i + 2 (lane % 4) + {0, 1} ----
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t r = m0 + wg * 64 + ((threadIdx.x & 127) >> 5) * 16 + (lane >> 2);
+  const bool add_bias = bias != nullptr;
+#pragma unroll
+  for (uint32_t i = 0; i < 16; ++i) {
+    const uint32_t c = n0 + i * 8 + 2 * (lane & 3);
+#pragma unroll
+    for (uint32_t h = 0; h < 2; ++h) {
+      const uint32_t row = r + h * 8;
+      if (row >= M) continue;
+      float* dst = C + (int64_t)row * ldc + c;
+#pragma unroll
+      for (uint32_t e = 0; e < 2; ++e) {
+        if (c + e < N) {
+          float x = acc[4 * i + 2 * h + e];
+          if (add_bias) x += bias[c + e];
+          if (accumulate) x += dst[e];                     // one writer per element
+          dst[e] = x;
         }
       }
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, T32_BN); }
 }
 
 template <bool A_MN, bool B_MN>
-static int launch_tf32(const CUtensorMap& ta, const CUtensorMap& tb, float* C, int64_t ldc, const float* bias, int M, int N,
-                       int K, int accumulate, cudaStream_t stream) {
-  auto kern = gemm_tf32_tcgen05<A_MN, B_MN>;
+static int launch_tf32(const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc, const float* bias, int M,
+                       int N, int K, int accumulate, cudaStream_t stream) {
+  auto kern = gemm_tf32_wgmma<A_MN, B_MN>;
   static bool attr_set = false;
   if (!attr_set) {
     NV_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, T32_DYN_BYTES));
@@ -194,23 +195,33 @@ static int launch_tf32(const CUtensorMap& ta, const CUtensorMap& tb, float* C, i
   }
   const uint32_t num_m = ceil_div_u32(M, T32_BM), num_n = ceil_div_u32(N, T32_BN);
   const uint32_t tiles = num_m * num_n, total_kb = ceil_div_u32(K, T32_BK);
-  // split K until about two CTAs per SM are in flight, keeping at least 8 k-blocks (256 k) per split
+  // split K until about two CTAs per SM are in flight, keeping at least 8 k-blocks (256 k) per split; the splits of
+  // a tile are one cluster (at most 8 CTAs)
   uint32_t splits = 1;
-  while (splits < 16 && tiles * splits * 2 <= 2u * (uint32_t)sm_count() && total_kb / (splits * 2) >= 8) splits *= 2;
+  while (splits < 8 && tiles * splits * 2 <= 2u * (uint32_t)sm_count() && total_kb / (splits * 2) >= 8) splits *= 2;
   const uint32_t kb_per_split = ceil_div_u32(total_kb, splits);
   splits = ceil_div_u32(total_kb, kb_per_split);
-  const uint32_t reduce = (splits > 1 || accumulate) ? 1u : 0u;
-  if (splits > 1 && !accumulate)
-    NV_CUDA(cudaMemset2DAsync(C, ldc * sizeof(float), 0, (size_t)N * sizeof(float), (size_t)M, stream));
-  kern<<<dim3(tiles, splits), T32_THREADS, T32_DYN_BYTES, stream>>>(ta, tb, C, ldc, bias, M, N, K, num_n, kb_per_split, reduce);
-  NV_LAUNCH_CHECK();
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(tiles, splits);
+  cfg.blockDim = dim3(T32_THREADS);
+  cfg.dynamicSmemBytes = T32_DYN_BYTES;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = 1;
+  attr[0].val.clusterDim.y = splits;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  NV_CUDA(cudaLaunchKernelEx(&cfg, kern, A, lda, B, ldb, C, ldc, bias, (uint32_t)M, (uint32_t)N, (uint32_t)K, num_n,
+                             kb_per_split, (uint32_t)(accumulate ? 1 : 0)));
   return NV_OK;
 }
 
 }  // namespace nv
 
 // Same contract as nv_sgemm (csrc/pano_ops.cu) with TF32 operand rounding.  Requirements beyond nv_sgemm's: base
-// pointers 16-byte aligned and lda/ldb multiples of 4 floats (TMA); returns NV_ERR_BAD_ARG otherwise so that the
+// pointers 16-byte aligned and lda/ldb multiples of 4 floats (16-byte loads); returns NV_ERR_BAD_ARG otherwise so that the
 // caller can route odd shapes (e.g. the K = 7 location-feature projections) to nv_sgemm.
 extern "C" int nv_gemm_tf32(const float* A, int64_t lda, int ta, const float* B, int64_t ldb, int tb, float* C, int64_t ldc,
                             const float* bias, int M, int N, int K, int accumulate, void* stream_) {
@@ -220,16 +231,10 @@ extern "C" int nv_gemm_tf32(const float* A, int64_t lda, int ta, const float* B,
   NV_REQUIRE(M > 0 && N > 0 && K > 0 && A && B && C, "nv_gemm_tf32: bad arguments M=%d N=%d K=%d", M, N, K);
   NV_REQUIRE((lda & 3) == 0 && (ldb & 3) == 0, "nv_gemm_tf32: lda/ldb must be multiples of 4 (got %lld, %lld)",
              (long long)lda, (long long)ldb);
-  CUtensorMap tma_a, tma_b;
-  int rc;
-  if (!ta) rc = make_tmap_2d(&tma_a, A, 4, (uint64_t)K, (uint64_t)M, (uint64_t)lda * 4, 32, T32_BM);
-  else     rc = make_tmap_2d(&tma_a, A, 4, (uint64_t)M, (uint64_t)K, (uint64_t)lda * 4, 32, T32_BK, true);
-  if (rc) return rc;
-  if (!tb) rc = make_tmap_2d(&tma_b, B, 4, (uint64_t)K, (uint64_t)N, (uint64_t)ldb * 4, 32, T32_BN);
-  else     rc = make_tmap_2d(&tma_b, B, 4, (uint64_t)N, (uint64_t)K, (uint64_t)ldb * 4, 32, T32_BK, true);
-  if (rc) return rc;
-  if (!ta && !tb) return launch_tf32<false, false>(tma_a, tma_b, C, ldc, bias, M, N, K, accumulate, stream);
-  if (!ta && tb) return launch_tf32<false, true>(tma_a, tma_b, C, ldc, bias, M, N, K, accumulate, stream);
-  if (ta && tb) return launch_tf32<true, true>(tma_a, tma_b, C, ldc, bias, M, N, K, accumulate, stream);
-  return launch_tf32<true, false>(tma_a, tma_b, C, ldc, bias, M, N, K, accumulate, stream);
+  NV_REQUIRE(((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(B)) & 15) == 0,
+             "nv_gemm_tf32: A and B must be 16-byte aligned");
+  if (!ta && !tb) return launch_tf32<false, false>(A, lda, B, ldb, C, ldc, bias, M, N, K, accumulate, stream);
+  if (!ta && tb) return launch_tf32<false, true>(A, lda, B, ldb, C, ldc, bias, M, N, K, accumulate, stream);
+  if (ta && tb) return launch_tf32<true, true>(A, lda, B, ldb, C, ldc, bias, M, N, K, accumulate, stream);
+  return launch_tf32<true, false>(A, lda, B, ldb, C, ldc, bias, M, N, K, accumulate, stream);
 }

@@ -2,7 +2,7 @@
 //
 // The library allocates no device memory of its own: every buffer (inputs, outputs, workspaces) is
 // owned by the caller (the PyTorch caching allocator in the Python host).  There is deliberately NO
-// CPU fallback anywhere in this library: with no sm_100 device every compute entry point fails with
+// CPU fallback anywhere in this library: with no sm_90 device every compute entry point fails with
 // NV_ERR_NO_DEVICE (north star: "no CPU fallback").
 #include "nv_host.h"
 
@@ -61,7 +61,7 @@ static EncodeTiledFn get_encode_fn() {
 }
 
 int make_tmap_2d(CUtensorMap* out, const void* base, int elem_bytes, uint64_t inner, uint64_t outer,
-                 uint64_t outer_stride_bytes, uint32_t box_inner, uint32_t box_outer, bool swizzle_atom_32b) {
+                 uint64_t outer_stride_bytes, uint32_t box_inner, uint32_t box_outer) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) {
     set_error("cuTensorMapEncodeTiled unavailable (no CUDA driver / no GPU)");
@@ -79,7 +79,7 @@ int make_tmap_2d(CUtensorMap* out, const void* base, int elem_bytes, uint64_t in
   cuuint32_t box[2] = {box_inner, box_outer};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = fn(out, dt, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  swizzle_atom_32b ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B,
+                  CU_TENSOR_MAP_SWIZZLE_128B,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("cuTensorMapEncodeTiled failed: CUresult %d (inner=%llu outer=%llu stride=%llu box=%ux%u)", (int)r,
@@ -104,7 +104,7 @@ int nv_set_pdl(int on) {
   return prev;
 }
 
-// 0 when an sm_100-class device is current, NV_ERR_NO_DEVICE otherwise.
+// 0 when an sm_90 (Hopper) device is current, NV_ERR_NO_DEVICE otherwise.
 int nv_device_check(void) {
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
@@ -120,8 +120,8 @@ int nv_device_check(void) {
     nv::set_error("cudaGetDeviceProperties: %s", cudaGetErrorString(e));
     return NV_ERR_NO_DEVICE;
   }
-  if (p.major != 10) {
-    nv::set_error("device %d is sm_%d%d; this library is built for sm_100a only", dev, p.major, p.minor);
+  if (p.major != 9 || p.minor != 0) {
+    nv::set_error("device %d is sm_%d%d; this library is built for sm_90a only", dev, p.major, p.minor);
     return NV_ERR_NO_DEVICE;
   }
   return NV_OK;

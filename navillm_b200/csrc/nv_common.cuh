@@ -1,9 +1,9 @@
-// navillm_b200 — shared device-side primitives for the sm_100a kernels.
+// navillm_b200 — shared device-side primitives for the sm_90a kernels.
 //
-// Thin inline-PTX wrappers for the Blackwell async machinery used by every hot
-// kernel in this package: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA,
-// TMEM alloc/ld/st, commit, fences) and the UMMA shared-memory / instruction
-// descriptors.  Nothing here is a port of reference code: the reference
+// Thin inline-PTX wrappers for the Hopper async machinery used by every hot
+// kernel in this package: mbarrier, TMA (cp.async.bulk.tensor), warpgroup MMA
+// (wgmma ordering and shared-memory descriptors; the MMA wrappers themselves are
+// in nv_wgmma.cuh).  Nothing here is a port of reference code: the reference
 // (zd11024/NaviLLM) ships no native sources (SURVEY.md §2a).
 #pragma once
 
@@ -12,6 +12,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+
+#include "nv_wgmma.cuh"
 
 namespace nv {
 
@@ -100,7 +102,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
-// generic-proxy smem writes -> visible to the async proxy (TMA / tcgen05.mma operand reads)
+// generic-proxy smem writes -> visible to the async proxy (TMA stores / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -142,36 +144,25 @@ __device__ __forceinline__ void tma_store_wait_all() {
 }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// warpgroup MMA (wgmma): ordering and shared-memory matrix descriptors
 // ----------------------------------------------------------------------------------------------
-// All three must be executed by one full warp (.sync.aligned).
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
+// wgmma_fence before the first wgmma that reads accumulator / A registers written by ordinary instructions;
+// wgmma_commit closes the group of wgmmas issued so far; wgmma_wait<N> returns when at most N groups are pending
+// (their accumulators are then readable and their shared-memory operands may be overwritten).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// tcgen05.commit: arrive on `bar` once all MMAs previously issued by this thread have completed.
-// Implicitly performs tcgen05.fence::before_thread_sync.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+// The accumulator registers are not visible to the compiler as wgmma operands between issue and wait: this pins them.
+template <int R>
+__device__ __forceinline__ void reg_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// One lane of a converged warp.  tcgen05.mma / commit sequences are issued as
-//     if (elect_one()) { ...MMAs...; umma_commit(bar); }  __syncwarp();
-// from code that the WHOLE warp executes (warp index taken from warp_id_uniform()): descriptors and TMEM addresses
-// then live in uniform registers and consecutive UTCHMMA issue back to back.  Issuing from an `if (lane == 0)`
-// branch instead makes ptxas wrap every MMA in an ELECT / R2UR / BRA.U.ANY waterfall (~100 cycles per MMA, measured
-// with the in-kernel trace of tools/attn_trace.py), which starves the tensor pipe whenever an MMA is shorter than that.
+// One lane of a converged warp (TMA issue from code the whole warp runs keeps the operands in uniform registers).
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile("{\n\t.reg .pred e;\n\telect.sync _|e, 0xffffffff;\n\tselp.u32 %0, 1, 0, e;\n\t}" : "=r"(pred));
@@ -179,110 +170,47 @@ __device__ __forceinline__ bool elect_one() {
 }
 __device__ __forceinline__ uint32_t warp_id_uniform() { return __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0); }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16/f16 inputs, fp32 accumulate. One thread issues.
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+// Named barrier over `count` threads (multiple of 32); id 0 is __syncthreads.
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
-
-// D[tmem] (+)= A[TMEM] * B[smem desc]: the ".ts" form.  A is a bf16 [128 x K] tile in tensor memory: row m = TMEM lane m,
-// 32-bit column c holds elements k = 2c, 2c+1 (what tcgen05.st.32x32b of packed bf16 pairs writes; verified by the one-hot
-// probes of tools/mma_ts_check.cu), so a K = 16 step advances the A address by 8 columns.  The A operand then costs no
-// shared-memory bandwidth: a 128xNx16 MMA runs at the N/2-cycle tensor floor (N = 64: 32 cycles, where the SS form needs
-// 48 because it reads 128 B/clk of smem operands).
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// TMEM -> registers: the warp reads its own 32-lane quarter, 32 consecutive fp32 columns per thread
-// (thread t <-> TMEM lane 32*(warp%4)+t).
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%32], "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31};"
-      ::"r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-        "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-        "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31]), "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%16], "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15};"
-      ::"r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // ----------------------------------------------------------------------------------------------
-// UMMA descriptors (bit layouts: PTX ISA "tcgen05 matrix descriptor" / "instruction descriptor")
+// thread-block clusters: barrier over every thread of every CTA, and a read-modify-write of a float in the
+// shared memory of another CTA (distributed shared memory)
 // ----------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor, 128-byte swizzle, descriptor version 1 (sm_100).
-//   bits [0,14)  start address >> 4      bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4 bits [46,48) version = 1
-//   bits [61,64) layout type (2 = SWIZZLE_128B)
-// K-major tile (rows of 64 bf16 = 128 B, 8-row swizzle atoms): SBO = 1024, LBO unused.
-// MN-major tile (rows = K index, 64 MN elements = 128 B per row, one 64-wide MN atom after the
-// other): SBO = 1024 (next 8 K rows), LBO = bytes between consecutive 64-wide MN atoms.
-__device__ __forceinline__ uint64_t umma_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes,
-                                                         uint32_t sbo_bytes) {
+__device__ __forceinline__ void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// *(float at shared address `saddr` in CTA `cta` of the cluster) += v   (the caller guarantees a single writer)
+__device__ __forceinline__ void dsmem_add_f32(uint32_t saddr, uint32_t cta, float v) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\t.reg .f32 x;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "ld.shared::cluster.f32 x, [ra];\n\t"
+      "add.f32 x, x, %2;\n\t"
+      "st.shared::cluster.f32 [ra], x;\n\t}"
+      ::"r"(saddr), "r"(cta), "f"(v)
+      : "memory");
+}
+
+// sm_90 shared-memory matrix descriptor, 128-byte swizzle (PTX ISA "Matrix Descriptor Format" of wgmma):
+//   bits [0,14) start address >> 4   [16,30) leading byte offset >> 4   [32,46) stride byte offset >> 4
+//   [62,64) layout type (1 = SWIZZLE_128B)
+// K-major tile (rows of 64 bf16 / 32 fp32 = 128 B, 8-row swizzle atoms): SBO = 1024, LBO unused; a 32-byte K step is +2.
+// MN-major tile (rows = K index, 64 MN elements = 128 B per row, one 64-wide MN atom after the other): SBO = 1024
+// (next 8 K rows), LBO = bytes between consecutive 64-wide MN atoms; a 16-row K step is +128.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
 
-// Instruction descriptor for kind::f16 with bf16 A/B and fp32 D.
-//   [4,6) D format (1 = f32)   [7,10) A format (1 = bf16)   [10,13) B format (1 = bf16)
-//   [15] A major (0 = K, 1 = MN)   [16] B major   [17,23) N >> 3   [24,29) M >> 4
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(uint32_t M, uint32_t N, uint32_t a_mn_major,
-                                                       uint32_t b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((N >> 3) << 17) |
-         ((M >> 4) << 24);
-}
-
 // Byte offset of 16-byte chunk `chunk` (0..7) in row `row` of a 128-byte-swizzled tile whose rows are
-// 128 B and whose base is 1024-byte aligned (the layout TMA SWIZZLE_128B writes and UMMA reads).
+// 128 B and whose base is 1024-byte aligned (the layout TMA SWIZZLE_128B writes and wgmma reads).
 __device__ __forceinline__ uint32_t sw128_offset(uint32_t row, uint32_t chunk) {
   return row * 128u + ((chunk ^ (row & 7u)) << 4);
 }

@@ -60,18 +60,8 @@ inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, siz
 }
 
 // 2-D bf16/fp32 tiled tensor map with 128-byte swizzle. `inner` is the contiguous dimension.
-// Out-of-bounds box elements read as zero (and are clipped on store).  swizzle_atom_32b selects
-// CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B (32-byte chunks permuted inside the 128-byte span), the only layout tcgen05
-// accepts for MN-major 32-bit (tf32) operands.
+// Out-of-bounds box elements read as zero (and are clipped on store).
 int make_tmap_2d(CUtensorMap* out, const void* base, int elem_bytes, uint64_t inner, uint64_t outer,
-                 uint64_t outer_stride_bytes, uint32_t box_inner, uint32_t box_outer, bool swizzle_atom_32b = false);
-
-// attn_fwd.cu: developer phase trace of the forward attention kernel (0 words unless built with -DNV_ATTN_TRACE)
-int attn_fwd_trace_copy(unsigned long long* out, int max_words);
-
-// gemm_bf16_2cta.cu: cta_group::2 variant (256x256 tile per SM pair), selected with block_n == 512
-int gemm_bf16_2cta_dispatch(const void* A, int64_t lda, int a_mn, const void* B, int64_t ldb, int b_mn, void* C,
-                            int64_t ldc, const void* addend, int64_t ld_add, int M, int N, int K, unsigned flags,
-                            cudaStream_t stream);
+                 uint64_t outer_stride_bytes, uint32_t box_inner, uint32_t box_outer);
 
 }  // namespace nv

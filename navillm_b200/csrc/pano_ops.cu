@@ -22,21 +22,21 @@ namespace nv {
 constexpr int SG_BM = 64, SG_BN = 64, SG_BK = 16;
 enum { SG_ACCUM = 1 };
 
-// blockIdx.z = K split: each split handles a contiguous k range and (when there are several) adds its partial
-// with fp32 atomics into a C that already holds the accumulate-into value (or zeros).
+// blockIdx.z = K split: each split handles a contiguous k range.  The splits of a tile form one thread-block cluster
+// and add their partial tiles in rank order in the leader's shared memory, so the sum does not depend on timing.
 __global__ void __launch_bounds__(256) sgemm_kernel(const float* __restrict__ A, int64_t lda, int ta,
                                                     const float* __restrict__ B, int64_t ldb, int tb,
                                                     float* __restrict__ C, int64_t ldc, const float* __restrict__ bias,
                                                     int M, int N, int K, int flags, int k_per_split) {
   __shared__ float As[SG_BK][SG_BM + 4];
   __shared__ float Bs[SG_BK][SG_BN + 4];
+  __shared__ float red[16 * 256];                // split-K: the leader's running sum of the splits' partial tiles
   const int tid = threadIdx.x;
   const int m0 = blockIdx.y * SG_BM, n0 = blockIdx.x * SG_BN;
   const int tx = tid & 15, ty = tid >> 4;  // 16 x 16 threads, each 4x4 outputs
   float acc[4][4] = {};
   const int k_begin = blockIdx.z * k_per_split;
   const int k_end = min(K, k_begin + k_per_split);
-  const bool split = gridDim.z > 1;
   for (int k0 = k_begin; k0 < k_end; k0 += SG_BK) {
     // load A tile (64 x 16) and B tile (16 x 64): 1024 elements each, 4 per thread
 #pragma unroll
@@ -73,6 +73,24 @@ __global__ void __launch_bounds__(256) sgemm_kernel(const float* __restrict__ A,
     }
     __syncthreads();
   }
+  if (gridDim.z > 1) {                           // cluster (1, 1, splits): the rank is the split index
+    const uint32_t rank = blockIdx.z, base = smem_u32(red) + tid * 4;
+    if (rank == 0) {
+#pragma unroll
+      for (int i = 0; i < 16; ++i) red[i * 256 + tid] = acc[i >> 2][i & 3];
+    }
+    cluster_sync_all();
+    for (uint32_t r = 1; r < gridDim.z; ++r) {
+      if (rank == r) {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) dsmem_add_f32(base + i * 256 * 4, 0, acc[i >> 2][i & 3]);
+      }
+      cluster_sync_all();
+    }
+    if (rank != 0) return;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) acc[i >> 2][i & 3] = red[i * 256 + tid];
+  }
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const int gm = m0 + ty * 4 + i;
@@ -82,14 +100,10 @@ __global__ void __launch_bounds__(256) sgemm_kernel(const float* __restrict__ A,
       const int gn = n0 + tx * 4 + j;
       if (gn >= N) continue;
       float v = acc[i][j];
-      if (bias && blockIdx.z == 0) v += bias[gn];
+      if (bias) v += bias[gn];
       float* c = C + (int64_t)gm * ldc + gn;
-      if (split) {
-        atomicAdd(c, v);                 // C was zeroed (or holds the accumulate-into value) by the host wrapper
-      } else {
-        if (flags & SG_ACCUM) v += *c;
-        *c = v;
-      }
+      if (flags & SG_ACCUM) v += *c;
+      *c = v;
     }
   }
 }
@@ -381,7 +395,8 @@ __global__ void __launch_bounds__(128) mha_bwd_b_kernel(const float* __restrict_
 // Row combine:  out[r] = (accumulate ? out[r] : 0) + alpha * A[ia[r]] + beta * Bm[ib[r]]
 // An index < 0 contributes nothing; ia == null means identity (row r).  Covers embedding lookups,
 // masked fills (index -1), candidate fusion and permuted gathers (models/nav_model.py:146-224).
-// rows_scatter_add is its transpose for gradients (fp32 atomics: tables have <= 100 rows).
+// rows_scatter_add is its transpose for gradients: a thread owns one column and walks the source rows in order, so
+// rows landing on the same destination row are summed in a fixed order (no atomics).
 // ------------------------------------------------------------------------------------------------
 __global__ void rows_combine_kernel(float* __restrict__ out, int64_t ldo, const float* __restrict__ A, int64_t lda,
                                     const int* __restrict__ ia, float alpha, const float* __restrict__ Bm, int64_t ldb,
@@ -397,11 +412,21 @@ __global__ void rows_combine_kernel(float* __restrict__ out, int64_t ldo, const 
 }
 __global__ void rows_scatter_add_kernel(float* __restrict__ dst, int64_t ldd, const int* __restrict__ idx,
                                         const float* __restrict__ src, int64_t lds, float alpha, int R, int D) {
-  for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < (int64_t)R * D;
-       e += (int64_t)gridDim.x * blockDim.x) {
-    const int r = e / D, c = e % D;
-    const int s = idx ? idx[r] : r;
-    if (s >= 0) atomicAdd(dst + (int64_t)s * ldd + c, alpha * src[(int64_t)r * lds + c]);
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= D) return;
+  constexpr int U = 8;                           // source rows whose loads are in flight together
+  for (int r0 = 0; r0 < R; r0 += U) {
+    int s[U];
+    float v[U];
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const int r = r0 + u;
+      s[u] = r < R ? (idx ? idx[r] : r) : -1;
+      v[u] = s[u] >= 0 ? src[(int64_t)r * lds + c] : 0.f;
+    }
+#pragma unroll
+    for (int u = 0; u < U; ++u)
+      if (s[u] >= 0) dst[(int64_t)s[u] * ldd + c] += alpha * v[u];
   }
 }
 
@@ -429,11 +454,19 @@ int nv_sgemm(const float* A, int64_t lda, int ta, const float* B, int64_t ldb, i
   while (splits < 8 && tiles * splits < 3 * sm_count() && K / (splits * 2) >= 256) splits *= 2;
   int k_per_split = ((K + splits - 1) / splits + SG_BK - 1) / SG_BK * SG_BK;
   grid.z = (K + k_per_split - 1) / k_per_split;
-  if (grid.z > 1 && !accumulate)
-    NV_CUDA(cudaMemset2DAsync(C, ldc * sizeof(float), 0, (size_t)N * sizeof(float), (size_t)M, S_(stream)));
-  sgemm_kernel<<<grid, 256, 0, S_(stream)>>>(A, lda, ta, B, ldb, tb, C, ldc, bias, M, N, K, accumulate ? SG_ACCUM : 0,
-                                             k_per_split);
-  NV_LAUNCH_CHECK();
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid;
+  cfg.blockDim = dim3(256);
+  cfg.stream = S_(stream);
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;   // the K splits of a tile are one cluster (<= 8 CTAs)
+  attr[0].val.clusterDim.x = 1;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = grid.z;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  NV_CUDA(cudaLaunchKernelEx(&cfg, sgemm_kernel, A, lda, ta, B, ldb, tb, C, ldc, bias, M, N, K,
+                             accumulate ? (int)SG_ACCUM : 0, k_per_split));
   return NV_OK;
 }
 
@@ -567,7 +600,7 @@ int nv_rows_combine(float* out, int64_t ldo, const float* A, int64_t lda, const 
 int nv_rows_scatter_add(float* dst, int64_t ldd, const int* idx, const float* src, int64_t lds, float alpha, int R, int D,
                         void* stream) {
   if (R == 0 || D == 0) return NV_OK;
-  rows_scatter_add_kernel<<<grid_1d((int64_t)R * D, 256), 256, 0, S_(stream)>>>(dst, ldd, idx, src, lds, alpha, R, D);
+  rows_scatter_add_kernel<<<(D + 127) / 128, 128, 0, S_(stream)>>>(dst, ldd, idx, src, lds, alpha, R, D);
   NV_LAUNCH_CHECK();
   return NV_OK;
 }

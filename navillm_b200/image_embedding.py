@@ -1,4 +1,4 @@
-"""Panorama scene encoder on the fp32 sm_100a kernels (csrc/pano_ops.cu), forward + hand-written backward.
+"""Panorama scene encoder on the fp32 sm_90a kernels (csrc/pano_ops.cu), forward + hand-written backward.
 
 Mirror of the reference's ``ImageEmbeddings`` (models/image_embedding.py:11-121) with the DETR pre-LN encoder
 (models/detr_transformer.py:62-89,170-182; built by models/ops.py:6-18): same constructor arguments, same

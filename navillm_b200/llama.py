@@ -1,4 +1,4 @@
-"""Packed LLaMA decoder stack over the sm_100a kernels: hand-written forward AND backward.
+"""Packed LLaMA decoder stack over the sm_90a kernels: hand-written forward AND backward.
 
 Host-side mirror of what the reference reaches through ``ModifiedLlamaForCausalLM`` ->
 ``transformers.models.llama.LlamaModel`` (reference call site models/modified_lm.py:112-116; HF names kept
@@ -316,7 +316,7 @@ class LlamaCore:
         H = d.n_heads
         saved: List[_Saved] = []
         last = d.n_layers - 1
-        # fused-epilogue kernels (CTA-pair GEMM) need head_dim 128, F % 128 == 0 and at least one wave of tiles
+        # fused-epilogue kernels (128 x 256-tile GEMM) need head_dim 128, F % 128 == 0 and at least one wave of tiles
         fused = self.fused_epilogues and x.shape[0] >= 1024 and d.inter % 128 == 0 and d.hidden % 256 == 0
         if kv_store is not None and kv_sink is None:                  # (kc list, vc list): post-RoPE K, V of every layer go to the caches
             B_, T_ = len(seqlens), x.shape[0]
@@ -420,9 +420,8 @@ class LlamaCore:
             return g if acc else None
 
         # Weight-gradient GEMMs on a SIDE stream (NAVILLM_WGRAD_STREAM=1): nothing downstream in the backward reads a weight
-        # gradient, so they can trail the dgrad chain.  Both streams run persistent CTA-pair GEMMs with dynamic tile claims:
-        # when one kernel's last, partially filled wave leaves CTA pairs idle (o_proj wgrad: 256 pair tiles on 74 pairs = 3.46
-        # waves), the other stream's kernel takes them.
+        # gradient, so they can trail the dgrad chain: when one GEMM's last, partially filled wave of tiles leaves SMs idle, the
+        # other stream's kernel takes them.
         side = WGRAD_STREAM and dx.shape[0] >= 1024
         main = torch.cuda.current_stream() if side else None
         ws = self._wgrad_stream() if side else None

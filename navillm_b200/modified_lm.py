@@ -1,4 +1,4 @@
-"""Modified LLaMA causal LM on the sm_100a kernels -- host mirror of the reference's
+"""Modified LLaMA causal LM on the sm_90a kernels -- host mirror of the reference's
 ``ModifiedLlamaForCausalLM`` (models/modified_lm.py:33-146,176-199).
 
 Same surface: ``init_tokenizer``, ``tokenize``, ``forward(input_ids, attention_mask, labels, cand_vis, hist_vis,

@@ -1,4 +1,4 @@
-"""``NavModel`` -- the drop-in boundary of the reference (models/nav_model.py:32-451) on sm_100a kernels.
+"""``NavModel`` -- the drop-in boundary of the reference (models/nav_model.py:32-451) on sm_90a kernels.
 
 Same constructor ``NavModel(args, logger, model_config)``, same ``forward(mode, batch, **kwargs)`` modes and
 return keys, same child-module / parameter names (``lang_model, img_embeddings, token_type_embeddings,

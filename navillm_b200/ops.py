@@ -1,4 +1,4 @@
-"""Python-side launchers for the sm_100a kernels (thin: argument checking + C-ABI call).
+"""Python-side launchers for the sm_90a kernels (thin: argument checking + C-ABI call).
 
 Every function here writes into caller-provided or freshly ``torch.empty``-allocated CUDA tensors and
 launches on the current stream.  Nothing falls back to torch math.
@@ -27,7 +27,7 @@ def _rowmajor(t: torch.Tensor, name: str) -> None:
 
 def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = False, out: torch.Tensor | None = None,
          addend: torch.Tensor | None = None, out_f32: bool = False, block_n: int = 0) -> torch.Tensor:
-    """C[M,N] = A·B (+ addend) on tcgen05 (csrc/gemm_bf16.cu).
+    """C[M,N] = A·B (+ addend) on wgmma (csrc/gemm_bf16.cu).
 
     a: [M,K] (a_mn=False) or [K,M] (a_mn=True);  b: [N,K] (b_mn=False) or [K,N] (b_mn=True); bf16.
     """
@@ -273,7 +273,7 @@ def ce_fwd_bwd(logits, labels, special_ids, *, grad_scale=None):
     """Per-row masked CE on bf16 logits; returns (row_loss fp32 [N], dlogits bf16 [N,V] or None)."""
     N, V = logits.shape
     row_loss = torch.empty((N,), dtype=torch.float32, device=logits.device)
-    # rows padded to a multiple of 64 elements so dlogits can feed the tcgen05 GEMMs (16-byte aligned rows)
+    # rows padded to a multiple of 64 elements so dlogits can feed the wgmma GEMMs (16-byte aligned rows)
     dlogits = torch.empty((N, (V + 63) // 64 * 64), dtype=bf16, device=logits.device)[:, :V] if grad_scale is not None else None
     check(_lib.load().nv_ce_fwd_bwd(ptr(logits), i64(logits.stride(0)), ptr(labels), ptr(special_ids),
                                     i32(special_ids.numel()), ptr(row_loss), ptr(dlogits),
@@ -324,7 +324,7 @@ def _f32_2d(t: torch.Tensor, name: str) -> None:
         raise ValueError(f"{name}: expected a 2-D fp32 CUDA tensor with unit inner stride, got {t.dtype} {tuple(t.shape)} {t.stride()}")
 
 
-# Numerical mode of the fp32 panorama-encoder GEMMs: "tf32" = tcgen05 kind::tf32 (what the reference's pinned
+# Numerical mode of the fp32 panorama-encoder GEMMs: "tf32" = wgmma tf32 (what the reference's pinned
 # torch 1.10 did by default on Ampere+: torch.backends.cuda.matmul.allow_tf32 = True), "fp32" = exact CUDA-core sgemm.
 _PANO_PRECISION = os.environ.get("NAVILLM_PANO_PRECISION", "tf32")
 
@@ -626,7 +626,7 @@ def add_int_(x, delta):
 
 
 # ---------------------------------------------------------------------------------------------------
-# fused-epilogue GEMMs on the CTA-pair kernel (csrc/gemm_bf16_2cta.cu)
+# fused-epilogue GEMMs on the 128 x 256 tile (csrc/gemm_bf16.cu)
 # ---------------------------------------------------------------------------------------------------
 def _timed(fn, flops, nbytes):
     timer = gemm_timer

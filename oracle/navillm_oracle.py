@@ -9,7 +9,7 @@ no CPU path at all.
 
 Pinning (SURVEY.md §8c): the reference ships NO tests or golden vectors for this path ("parity
 unpinned" at the source).  The oracle is therefore pinned against outputs of the reference code itself,
-imported unmodified from /root/reference in the authoring container with three stubs (bert-large
+imported unmodified from a checkout of the reference with three stubs (bert-large
 config, AutoConfig, tokenizer): ``tests/golden/make_golden.py`` generates the fixtures in
 ``tests/golden/*.pt`` and ``tests/test_oracle_golden.py`` checks every function below against them
 (forward outputs, loss and gradients).  The LLaMA block arithmetic is not in the reference tree: it is
@@ -20,7 +20,7 @@ reference's own generation branch run with a keyword-argument adapter for prepar
 (tests/golden/make_generate_golden.py -> generate_*.pt; the positional call of models/modified_lm.py:187-194 is the
 only thing that does not run under transformers 5.x, SURVEY.md §8c).
 
-Each function cites the reference file:line it follows (paths relative to /root/reference).
+Each function cites the reference file:line it follows (paths relative to the reference repository root).
 """
 from __future__ import annotations
 

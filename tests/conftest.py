@@ -10,7 +10,7 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with -m gpu on a machine that has one)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -30,7 +30,7 @@ def cuda_dev():
 @pytest.fixture(params=["fp32", "tf32"])
 def pano_precision(request):
     """Runs a GPU test in both numerical modes of the fp32 panorama-encoder GEMMs (navillm_b200.ops.set_pano_precision):
-    exact CUDA-core fp32 and the product default, tcgen05 kind::tf32."""
+    exact CUDA-core fp32 and the product default, wgmma tf32."""
     from navillm_b200 import ops
     prev = ops.set_pano_precision(request.param)
     yield request.param

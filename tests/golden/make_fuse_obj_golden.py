@@ -1,19 +1,20 @@
 """Golden vectors for the `fuse_obj` branch of the panorama encoder (models/image_embedding.py:78-94; `--fuse_obj`,
 tools/parser.py:95: "whether fuse object features for REVERIE and SOON"), from the UNMODIFIED reference's
-ImageEmbeddings run on CPU in eval() mode at tiny dimensions.  Authoring container only (/root/reference does not
-exist on the GPU box).
+ImageEmbeddings run on CPU in eval() mode at tiny dimensions.  Needs a checkout of the reference, named by the
+NAVILLM_REFERENCE environment variable (nothing under tests/ reads it at test time).
 
     python tests/golden/make_fuse_obj_golden.py     # writes tests/golden/pano_fuse_obj.pt
 
 Recorded: the module's state_dict, the inputs, `pano_embeds / pano_masks / obj_embeds / obj_masks`, and the gradients
 of every parameter for the scalar  sum(pano_embeds * wp) + sum(obj_embeds * wo)  with recorded random weights."""
+import os
 import sys
 import types
 from pathlib import Path
 
 import torch
 
-REF = "/root/reference"
+REF = os.environ["NAVILLM_REFERENCE"]
 OUT = Path(__file__).resolve().parent / "pano_fuse_obj.pt"
 DIMS = dict(pano_hidden=128, pano_heads=2, pano_inter=256, image_feat_size=64, obj_feat_size=48, output_size=256, num_pano_layers=2)
 

@@ -8,6 +8,7 @@ nav_gmap_variable (tasks/agents/mp3d_agent.py:143-212, 264-371) with torch.Tenso
 The observations and every returned tensor / list are stored; tests/test_step_glue_cpu.py replays the observations through
 navillm_b200.step_glue and compares.
 """
+import os
 import sys
 import types
 from pathlib import Path
@@ -15,7 +16,7 @@ from pathlib import Path
 import numpy as np
 import torch
 
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.environ["NAVILLM_REFERENCE"])   # a checkout of the reference
 torch.Tensor.cuda = lambda self, *a, **k: self          # the reference calls .cuda() on everything it builds
 
 from models.graph_utils import GraphMap  # noqa: E402

@@ -1,7 +1,7 @@
 """Generate golden vectors from the UNMODIFIED reference (zd11024/NaviLLM) at tiny dimensions.
 
-Runs only in the authoring container, where the reference is mounted read-only at /root/reference
-(it does not exist on the GPU box; nothing under tests/ reads it at test time).  The reference's model
+Needs a checkout of the reference, named by the NAVILLM_REFERENCE environment variable (nothing under tests/ reads
+it at test time).  The reference's model
 code is imported as-is; three things it would fetch from the network are stubbed (SURVEY.md §8c):
   (i)   PretrainedConfig.from_pretrained('bert-large-uncased')   -> tiny pano-encoder config
   (ii)  AutoConfig.from_pretrained(vicuna)                        -> tiny LlamaConfig (eager attention)
@@ -15,6 +15,7 @@ and in 'fp32'.
 Recorded: transformers.__version__, torch.__version__, the state_dict, all inputs, forward outputs of
 every mode, the action-CE / LM losses and a selection of gradients.
 """
+import os
 import sys
 import types
 from pathlib import Path
@@ -23,7 +24,7 @@ import torch
 
 ROOT = Path(__file__).resolve().parents[2]
 sys.path.insert(0, str(ROOT))
-REF = "/root/reference"
+REF = os.environ["NAVILLM_REFERENCE"]
 
 DIMS = dict(hidden=256, n_layers=2, n_heads=2, inter=256, base_vocab=256,
             pano_hidden=128, pano_heads=2, pano_inter=256, image_feat_size=64, obj_feat_size=48)
@@ -140,7 +141,7 @@ def run(precision: str):
     model, tf_version = build_reference_model(precision)
     pano_in, nav_in, targets = make_inputs()
     out = {"meta": {"transformers": tf_version, "torch": torch.__version__, "precision": precision, "dims": DIMS,
-                    "reference": "zd11024/NaviLLM @ /root/reference (unmodified; 3 stubs, see make_golden.py)"},
+                    "reference": "zd11024/NaviLLM (unmodified; 3 stubs, see make_golden.py)"},
            "state_dict": {k: v.detach().clone() for k, v in model.state_dict().items()},
            "pano_in": pano_in, "nav_in": nav_in, "targets": targets}
     model.zero_grad()

@@ -1,4 +1,4 @@
-"""tcgen05 flash attention (csrc/attn_fwd.cu, attn_bwd.cu) against a plain PyTorch fp32 reference.
+"""wgmma flash attention (csrc/attn_fwd.cu, attn_bwd.cu) against a plain PyTorch fp32 reference.
 
 Tolerance (forward): q,k,v are bf16; the kernel keeps S and the running softmax in fp32 and rounds P to
 bf16 before the PV product and O to bf16 at the end, like the reference's eager path (fp32 softmax cast
@@ -103,7 +103,7 @@ def test_o_proj_dgrad_with_fused_attention_D(cuda_dev):
     cu = torch.tensor([0] + list(np.cumsum(seqlens)), dtype=torch.int32, device=cuda_dev)
     o, lse = ops.attn_fwd(qkv, cu, seqlens, H)
     dout, dvec = ops.gemm_attnd(dy, wo, o)
-    ref = ops.gemm(dy, wo, b_mn=True, block_n=512)
+    ref = ops.gemm(dy, wo, b_mn=True, block_n=256)
     torch.cuda.synchronize()
     assert torch.equal(dout, ref)
     want = (dout.float() * o.float()).view(T, H, HD).sum(-1).t().contiguous()          # [H, T]

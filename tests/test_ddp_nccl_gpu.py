@@ -1,8 +1,8 @@
 """The real NavModel under navillm_b200.parallel.DistributedDataParallel over NCCL (2 GPUs): the rollout pattern of
 tasks/agents/mp3d_agent.py:661-667 (no_sync around all steps but the last, different rollout lengths per rank, a second
 backward in the synced step) must leave every rank with the rank-MEAN of the locally accumulated gradients -- with the
-overlapped layer-slice reductions and without.  Skipped on a 1-GPU box (the driver's `-m gpu` run); run it with
-`gpurun --gpus 2 -- python -m pytest tests/test_ddp_nccl_gpu.py -m gpu -q`."""
+overlapped layer-slice reductions and without.  Skipped on a machine with one GPU; run it on two or more with
+`python -m pytest tests/test_ddp_nccl_gpu.py -m gpu -q`."""
 import os
 import socket
 import sys
@@ -138,7 +138,7 @@ def _worker(rank, world, port, q):
 
 def test_navmodel_ddp_two_ranks_nccl():
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2); the gloo twin tests/test_parallel_cpu.py covers the logic on CPU")
+        pytest.skip("needs 2 GPUs; the gloo twin tests/test_parallel_cpu.py covers the logic on CPU")
     import torch.multiprocessing as mp
     s = socket.socket()
     s.bind(("127.0.0.1", 0))

@@ -2,7 +2,7 @@
 
 The golden fixtures pin the boundary at toy widths (hidden 256, T <= 367), where ``LlamaCore`` takes the unfused
 single-CTA kernels.  The tests here run Vicuna-7B widths (hidden 4096 / 32 heads / F 11008, 36 x 1408 views, panorama
-hidden 1024 / 16 heads, vocab 32006) on 2 decoder layers with T >= 1024 packed rows, so the CTA-pair GEMM and its fused
+hidden 1024 / 16 heads, vocab 32006) on 2 decoder layers with T >= 1024 packed rows, so the 128 x 256-tile GEMM and its fused
 epilogues (``nv_gemm_rope / swiglu / dswiglu / attnd_bf16``), the 128-wide attention kernels and -- for generate -- the
 swap-AB skinny GEMMs at N = 4096 / 11008 / 32006 execute inside the stack, and compare with the CPU oracle (which
 finishes 2 full-width layers in seconds):
@@ -332,7 +332,7 @@ def test_generate_c3_shape_vs_oracle(cuda_dev):
                                             cand_vis=cand.to(cuda_dev), max_new_tokens=N_NEW, stop_on_eos=False,
                                             use_cuda_graph=graph).cpu()
         assert ids.shape == ref_ids.shape and torch.equal(ids[:, :S0], text["input_ids"])
-        assert spy.n["gemm_rope"] == LAYERS, spy.n                         # prefill took the fused CTA-pair path (T >= 1024)
+        assert spy.n["gemm_rope"] == LAYERS, spy.n                         # prefill took the fused-epilogue path (T >= 1024)
         assert spy.n["gemm_skinny"] > 0 and spy.n["gemm_skinny_swiglu"] > 0, spy.n   # decode took the swap-AB kernels
         matched, cut = compare_greedy_rows(ids, ref_ids, ref_logits, S0, N_NEW, tag=f"graph={graph}")
         print(f"\n[c3 generate, graph={graph}] matched tokens per row {matched} of {N_NEW}; "

@@ -1,4 +1,4 @@
-"""tcgen05 bf16 GEMM (csrc/gemm_bf16.cu) against a plain PyTorch fp32 reference of the same op.
+"""wgmma bf16 GEMM (csrc/gemm_bf16.cu) against a plain PyTorch fp32 reference of the same op.
 
 Tolerance: inputs are bf16, accumulation fp32, output rounded once to bf16 -> the only admissible
 difference from an fp32 reference rounded to bf16 is accumulation order: |diff| <= 2 bf16 ulp of the
@@ -34,7 +34,7 @@ def test_gemm_matches_fp32_reference(cuda_dev, M, N, K, a_mn, b_mn):
     g = torch.Generator(device="cpu").manual_seed(M * 7 + N * 3 + K)
     a = torch.randn((K, M) if a_mn else (M, K), generator=g).to(cuda_dev, torch.bfloat16)
     b = torch.randn((K, N) if b_mn else (N, K), generator=g).to(cuda_dev, torch.bfloat16)
-    for bn in (128, 256, 512):                         # 512 = CTA-pair (cta_group::2) kernel
+    for bn in (128, 256):
         out = ops.gemm(a, b, a_mn=a_mn, b_mn=b_mn, block_n=bn)
         torch.cuda.synchronize()
         ref = _ref(a, b, a_mn, b_mn)
@@ -93,7 +93,7 @@ def test_gemm_skinny_m_weight_streaming(cuda_dev):
 
 
 def test_fused_epilogues_are_bit_identical_to_unfused(cuda_dev):
-    """SwiGLU / SwiGLU-backward / RoPE epilogues of the CTA-pair GEMM vs GEMM followed by the row kernels."""
+    """SwiGLU / SwiGLU-backward / RoPE epilogues of the fused GEMM vs GEMM followed by the row kernels."""
     from navillm_b200 import ops
     from navillm_b200.llama import LlamaDims, rope_tables
     g = torch.Generator(device="cpu").manual_seed(21)
@@ -205,7 +205,7 @@ def test_decode_attn_rope_fused_matches_two_kernels(cuda_dev):
 @pytest.mark.parametrize("N,K", [(4096, 4096), (12288, 4096), (22016, 4096), (4096, 11008)])
 def test_mid_m_auto_dispatch_is_bit_identical_to_every_tile_variant(cuda_dev, M, N, K):
     """16 < M < 512 (one forward of a small batch, evaluation rollouts, prefix-reuse suffixes): nv_gemm_bf16's auto rule
-    picks the tile variant per (M, N) from a measured table (tools/midm_bench.py).  Every variant accumulates the k-blocks in
+    picks the tile variant per (M, N).  Every variant accumulates the k-blocks in
     the same order, so the choice must not change one output bit - with and without the residual add - and the result
     matches the fp32 reference."""
     from navillm_b200 import ops
@@ -215,7 +215,7 @@ def test_mid_m_auto_dispatch_is_bit_identical_to_every_tile_variant(cuda_dev, M,
     add = torch.randn((M, N), generator=g).to(cuda_dev, torch.bfloat16)
     for addend in (None, add):
         auto = ops.gemm(a, b, addend=addend)
-        for bn in (32, 128, 256, 512):
+        for bn in (32, 128, 256):
             if bn == 32 and M > 128:
                 continue
             assert torch.equal(ops.gemm(a, b, addend=addend, block_n=bn), auto), (bn, addend is not None)

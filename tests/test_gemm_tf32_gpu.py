@@ -1,4 +1,4 @@
-"""tcgen05 kind::tf32 GEMM (csrc/gemm_tf32.cu) against PyTorch references of the same op.
+"""wgmma tf32 GEMM (csrc/gemm_tf32.cu) against PyTorch references of the same op.
 
 Two checks, tolerances stated:
   * exactness of the TF32 model: the tensor core reads fp32 operands with a 10-bit mantissa.  Against an fp64 product

@@ -1,4 +1,4 @@
-"""Packed LLaMA stack (navillm_b200/llama.py: tcgen05 GEMMs + flash attention + row kernels, hand-written
+"""Packed LLaMA stack (navillm_b200/llama.py: wgmma GEMMs + flash attention + row kernels, hand-written
 backward) against the CPU oracle's restatement of HF LLaMA (oracle/navillm_oracle.py::llama_model).
 
 "bf16 tolerance", stated: let `truth` be the oracle run in fp32 with the same (bf16-valued) weights.  The

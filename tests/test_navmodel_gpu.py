@@ -1,4 +1,4 @@
-"""End-to-end parity of navillm_b200.NavModel (the drop-in boundary) on a B200 against
+"""End-to-end parity of navillm_b200.NavModel (the drop-in boundary) on an H100 against
 (a) golden vectors produced by the UNMODIFIED reference (tests/golden/nav_amp_bf16.pt) and
 (b) the CPU oracle, forward outputs, losses and gradients, for every mode of NavModel.forward.
 
@@ -6,7 +6,7 @@ bf16 tolerance, stated: `truth` = golden fp32 run of the reference (nav_fp32.pt;
 bf16 rounding); the reference's own bf16 run deviates from it by e_ref.  The CUDA path, loaded with the bf16
 golden weights, must satisfy |cuda - ref_bf16| <= 3 * |ref_bf16 - truth|_max + 2e-2 * scale  for logits/losses
 and gradient tensors (scale = max|ref|).  fp32 parts (pano encoder outputs, fuse_embeds) must agree to 1e-4 with the
-exact-fp32 panorama GEMMs and to 4e-3 with the default tcgen05 kind::tf32 GEMMs (10-bit-mantissa operands, the mode
+exact-fp32 panorama GEMMs and to 4e-3 with the default wgmma tf32 GEMMs (10-bit-mantissa operands, the mode
 the reference's pinned torch 1.10 used on Ampere+; see tests/test_pano_gpu.py).
 """
 import sys

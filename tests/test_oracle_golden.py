@@ -1,6 +1,5 @@
 """Pin the CPU oracle (oracle/navillm_oracle.py) against golden vectors produced by the UNMODIFIED
-reference code (tests/golden/make_golden.py, run in the authoring container where /root/reference is
-mounted).  CPU only: runs under `-m "not gpu"`.
+reference code (tests/golden/make_golden.py, run against a checkout of the reference).  CPU only: runs under `-m "not gpu"`.
 
 Tolerances: the oracle restates the same torch arithmetic in the same dtypes, so fp32 results agree to
 accumulation-order noise (1e-5 relative) and the bf16 LM path to 1 bf16 ulp on logits / hidden states.

@@ -4,7 +4,7 @@ the reference's ImageEmbeddings (oracle.forward_panorama), forward and parameter
 Two numerical modes (ops.set_pano_precision):
   fp32  exact CUDA-core GEMMs: both sides fp32, only summation order differs -> 1e-4 (forward) / 2e-4 (gradients)
         relative to the tensor's max.
-  tf32  tcgen05 kind::tf32 GEMMs (the product default; what the reference's pinned torch 1.10 did on Ampere+ with its
+  tf32  wgmma tf32 GEMMs (the product default; what the reference's pinned torch 1.10 did on Ampere+ with its
         default allow_tf32 = True): operands carry a 10-bit mantissa (unit roundoff 2^-10 under truncation), errors
         accumulate over 2 encoder layers + projections -> 4e-3 (forward) / 1e-2 (gradients) relative to the max.
 """

@@ -9,7 +9,7 @@ The oracle cannot run these sizes in seconds, so parity here is structural:
                            padded column index), checked against an explicitly shifted run;
   * gradient linearity  -- backward(2*g) == 2*backward(g) up to bf16 rounding, and weight gradients accumulate;
   * GEMM identities at full size -- (A B^T) via the K-major path equals the MN-major path on transposed storage;
-                           dgrad/wgrad shapes of the 7B model run through the CTA-pair kernel.
+                           dgrad/wgrad shapes of the 7B model run through the 128 x 256-tile kernel.
 """
 import sys
 from pathlib import Path
@@ -117,7 +117,7 @@ def test_gemm_major_forms_agree_at_7b_shapes(cuda_dev):
     T, D, F = 4096, 4096, 11008
     x = torch.randn(T, D, generator=g, device=cuda_dev).to(bf16)
     w = (torch.randn(2 * F, D, generator=g, device=cuda_dev) * 0.02).to(bf16)
-    y_k = ops.gemm(x, w)                                     # K-major A, K-major B (forward form), CTA-pair kernel
+    y_k = ops.gemm(x, w)                                     # K-major A, K-major B (forward form), 128 x 256-tile kernel
     y_mn = ops.gemm(x.t().contiguous(), w.t().contiguous(), a_mn=True, b_mn=True)   # same product, MN-major storage
     y_1 = ops.gemm(x, w, block_n=256)                        # single-CTA kernel
     assert torch.equal(y_k, y_mn) and torch.equal(y_k, y_1)  # same k order, same fp32 accumulation -> bit-exact

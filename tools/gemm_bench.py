@@ -1,7 +1,7 @@
-"""Time the tcgen05 bf16 GEMM on the LLaMA-7B shapes of the path and print TFLOP/s next to cuBLAS
+"""Time the wgmma bf16 GEMM on the LLaMA-7B shapes of the path and print TFLOP/s next to cuBLAS
 (torch.matmul; comparison bar only, never used by the product).  Run on the GPU box:
 
-    python tools/gemm_bench.py [--tokens 16384] [--json gpurun_out/gemm_bench.json]
+    python tools/gemm_bench.py [--tokens 16384] [--json gemm_bench.json]
 """
 import argparse
 import json
@@ -34,7 +34,6 @@ def main():
     ap.add_argument("--no-cublas", action="store_true")
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--only-512", action="store_true", help="time only the CTA-pair kernel")
     a = ap.parse_args()
     T = a.tokens
     dev = torch.device("cuda:0")
@@ -59,7 +58,7 @@ def main():
         C = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
         flops = 2.0 * M * N * K
         res = {"name": name, "M": M, "N": N, "K": K}
-        for bn in ((512,) if a.only_512 else (256, 512)):
+        for bn in (128, 256):
             ms = timeit(lambda: ops.gemm(A, B, a_mn=a_mn, b_mn=b_mn, out=C, block_n=bn), iters=a.iters, warmup=a.warmup)
             res[f"nv_bn{bn}_ms"] = ms
             res[f"nv_bn{bn}_tflops"] = flops / ms / 1e9

@@ -26,7 +26,7 @@ def timeit(fn, iters=24, warmup=4):
 def main():
     dev = torch.device("cuda:0")
     Ms = [int(a) for a in sys.argv[1:]] or [48, 128, 192, 256, 384, 640]
-    variants = [("bn32", 32), ("bn128", 128), ("bn256", 256), ("pair", 512), ("auto", 0)]
+    variants = [("bn32", 32), ("bn128", 128), ("bn256", 256), ("auto", 0)]
     if hasattr(ops, "gemm_stream"):
         variants.append(("stream", -1))
     for name, N, K in (("qkv", 12288, 4096), ("o", 4096, 4096), ("gateup", 22016, 4096), ("down", 4096, 11008)):
