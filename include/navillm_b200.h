@@ -66,6 +66,18 @@ int nv_gemm_skinny_bf16(const void* X, int64_t ldx, const void* W, int64_t ldw, 
 /* ... with the SwiGLU of HF LlamaMLP fused: h[M,F] = bf16(bf16(silu(g)) * u), [g|u] = bf16(X Wgu^T), Wgu [2F,K] */
 int nv_gemm_skinny_swiglu_bf16(const void* X, int64_t ldx, const void* Wgu, int64_t ldw, void* H, int64_t ldh, int M, int F,
                                int K, void* stream);
+/* Opt-in fp8 weight streaming of the same decode-step GEMMs (HF generate through models/modified_lm.py:184-199; no
+ * reference counterpart for the number format).  nv_quantize_fp8_rows (csrc/quant.cu) rounds a bf16 weight W [N,K] to
+ * e4m3 with one power-of-two scale per row: exps[n] = e_n (int8, the smallest e with max|W[n,:]| / 2^e <= 448, clamped
+ * below at -117; 0 for an all-zero row), Q [N,K] = e4m3(W / 2^e_n) (round to nearest even, subnormals kept), and W is
+ * overwritten in place with W' = Q * 2^e_n, which bf16 holds exactly.  K % 8 == 0, ldq (bytes) % 16 == 0.
+ * nv_gemm_skinny_fp8 / nv_gemm_skinny_swiglu_fp8 are nv_gemm_skinny_bf16 / nv_gemm_skinny_swiglu_bf16 with the weight
+ * given as (Q, exps): they stream half the bytes and return bit for bit what the bf16 kernels return on W'.  ldw in bytes. */
+int nv_quantize_fp8_rows(void* W, int64_t ldw, void* Q, int64_t ldq, void* exps, int N, int K, void* stream);
+int nv_gemm_skinny_fp8(const void* X, int64_t ldx, const void* Wq, int64_t ldw, const void* exps, void* C, int64_t ldc,
+                       const void* addend, int64_t ld_add, int M, int N, int K, void* stream);
+int nv_gemm_skinny_swiglu_fp8(const void* X, int64_t ldx, const void* Wgu_q, int64_t ldw, const void* exps, void* H,
+                              int64_t ldh, int M, int F, int K, void* stream);
 int nv_gemm_swiglu_bf16(const void* x, int64_t ldx, const void* Wgu, int64_t ldw, void* gu, int64_t ldgu, void* h,
                         int64_t ldh, int M, int F, int K, int keep_gu, void* stream);
 int nv_gemm_dswiglu_bf16(const void* dx, int64_t lddx, const void* Wd, int64_t ldw, const void* gu, int64_t ldgu, void* dgu,

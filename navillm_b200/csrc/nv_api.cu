@@ -61,7 +61,7 @@ static EncodeTiledFn get_encode_fn() {
 }
 
 int make_tmap_2d(CUtensorMap* out, const void* base, int elem_bytes, uint64_t inner, uint64_t outer,
-                 uint64_t outer_stride_bytes, uint32_t box_inner, uint32_t box_outer) {
+                 uint64_t outer_stride_bytes, uint32_t box_inner, uint32_t box_outer, bool swizzle128) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) {
     set_error("cuTensorMapEncodeTiled unavailable (no CUDA driver / no GPU)");
@@ -70,16 +70,22 @@ int make_tmap_2d(CUtensorMap* out, const void* base, int elem_bytes, uint64_t in
   NV_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0, "TMA base pointer %p not 16-byte aligned", base);
   NV_REQUIRE((outer_stride_bytes & 15) == 0, "TMA row stride %llu B not a multiple of 16",
              (unsigned long long)outer_stride_bytes);
-  NV_REQUIRE(box_inner * elem_bytes == 128, "TMA box inner extent must be 128 bytes (got %u)",
-             box_inner * elem_bytes);
+  NV_REQUIRE(elem_bytes == 1 || elem_bytes == 2 || elem_bytes == 4, "TMA element size %d not supported", elem_bytes);
+  if (swizzle128)
+    NV_REQUIRE(box_inner * elem_bytes == 128, "TMA box inner extent must be 128 bytes (got %u)", box_inner * elem_bytes);
+  else
+    NV_REQUIRE((box_inner * elem_bytes) % 16 == 0 && box_inner <= 256, "TMA box inner extent %u B not a multiple of 16",
+               box_inner * elem_bytes);
   NV_REQUIRE(box_outer >= 1 && box_outer <= 256, "TMA box outer extent %u out of range", box_outer);
-  CUtensorMapDataType dt = elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  const CUtensorMapDataType dt = elem_bytes == 1   ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                                 : elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                                   : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
   cuuint64_t dims[2] = {inner, outer};
   cuuint64_t strides[1] = {outer_stride_bytes};
   cuuint32_t box[2] = {box_inner, box_outer};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = fn(out, dt, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  CU_TENSOR_MAP_SWIZZLE_128B,
+                  swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("cuTensorMapEncodeTiled failed: CUresult %d (inner=%llu outer=%llu stride=%llu box=%ux%u)", (int)r,

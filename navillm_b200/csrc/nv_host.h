@@ -59,9 +59,10 @@ inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, siz
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
 
-// 2-D bf16/fp32 tiled tensor map with 128-byte swizzle. `inner` is the contiguous dimension.
+// 2-D tiled tensor map of bf16 (elem_bytes 2), fp32 (4) or raw bytes such as e4m3 (1). `inner` is the contiguous dimension.
+// swizzle128: 128-byte swizzle, the box row must be exactly 128 bytes; otherwise unswizzled, box rows a multiple of 16 bytes.
 // Out-of-bounds box elements read as zero (and are clipped on store).
 int make_tmap_2d(CUtensorMap* out, const void* base, int elem_bytes, uint64_t inner, uint64_t outer,
-                 uint64_t outer_stride_bytes, uint32_t box_inner, uint32_t box_outer);
+                 uint64_t outer_stride_bytes, uint32_t box_inner, uint32_t box_outer, bool swizzle128 = true);
 
 }  // namespace nv

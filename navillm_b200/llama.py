@@ -17,6 +17,7 @@ from __future__ import annotations
 
 import os
 from dataclasses import dataclass
+from types import SimpleNamespace
 from typing import List, Optional
 
 import torch
@@ -158,6 +159,8 @@ class FlatParams:
                 p.data = view
                 p.grad = self.flat_grad[o:o + p.numel()].view(p.shape)
         self._ptr0 = params[0].data_ptr()
+        # bumped by writers that bypass torch's version counters (the fused AdamW of optim.py writes through raw pointers)
+        self.generation = 0
 
     def intact(self) -> bool:
         return self.params[0].data_ptr() == self._ptr0 and self.params[0].grad is not None and \
@@ -206,6 +209,69 @@ class FlatParams:
     def grad_view(self, members, shape) -> torch.Tensor:
         o, numel = self._fused_span(members, shape)
         return self.flat_grad[o:o + numel].view(shape)
+
+
+class Fp8Weights:
+    """e4m3 copy of linear weights of a ``FlatParams`` buffer for the decode-step GEMMs (csrc/gemm_skinny.cu).
+
+    Building it rounds every listed weight IN PLACE to W' = e4m3(W / 2^e_n) * 2^e_n (one power-of-two exponent per output
+    row, csrc/quant.cu), so the bf16 buffer and the fp8 copy describe the same model.  The copy keeps the flat buffer's
+    parameter order and 64-element alignment (non-listed parameters are skipped), so members that are adjacent there --
+    q|k|v, gate|up -- are adjacent here too and the fused weights are plain views.  ``stale_reason`` reports any write to
+    the weights since: a torch in-place op on a parameter or on the buffer (version counters), or a bump of
+    ``FlatParams.generation`` by a raw-pointer writer."""
+
+    def __init__(self, flat: FlatParams, params: List[nn.Parameter]):
+        want = {id(p) for p in params}
+        align = 64
+        self.flat = flat
+        self.params = [p for p in flat.params if id(p) in want]
+        if len(self.params) != len(want):
+            raise RuntimeError("Fp8Weights: every weight must live in the flat buffer")
+        self._off, self._row, total, rows = {}, {}, 0, 0
+        for p in self.params:
+            if p.dim() != 2:
+                raise RuntimeError(f"Fp8Weights: 2-D weights only, got {tuple(p.shape)}")
+            self._off[id(p)], self._row[id(p)] = total, rows
+            total += (p.numel() + align - 1) // align * align
+            rows += p.shape[0]
+        dev = flat.flat.device
+        self.q = torch.empty(total, dtype=ops.fp8, device=dev)
+        self.exps = torch.empty(rows, dtype=torch.int8, device=dev)
+        for p in self.params:
+            q, e = self.view([p], tuple(p.shape))
+            ops.quantize_fp8_(p.data, q, e)
+        self._versions = self._version_state()
+        self._generation = flat.generation
+
+    @property
+    def nbytes(self) -> int:
+        return self.q.numel() + self.exps.numel()
+
+    def view(self, members, shape):
+        """(e4m3 [N, K], int8 exponents [N]) of the weight formed by ``members`` stacked in order (``FlatParams.view``)."""
+        o, r = self._off[id(members[0])], self._row[id(members[0])]
+        end_o, end_r = o, r
+        for m in members:
+            if self._off.get(id(m)) != end_o or self._row[id(m)] != end_r:
+                raise RuntimeError("Fp8Weights.view: the members are not adjacent, in order and unpadded")
+            end_o += m.numel()
+            end_r += m.shape[0]
+        if end_o - o != shape[0] * shape[1] or end_r - r != shape[0]:
+            raise RuntimeError(f"Fp8Weights.view: members hold {end_o - o} elements, shape {tuple(shape)} needs {shape[0] * shape[1]}")
+        return self.q[o:end_o].view(shape), self.exps[r:end_r]
+
+    def _version_state(self):
+        return self.flat.flat._version, sum(p._version for p in self.params)
+
+    def stale_reason(self, flat: FlatParams) -> Optional[str]:
+        if flat is not self.flat or flat.params[0].data_ptr() != flat._ptr0:
+            return "the weights were moved to new storage"
+        if flat.generation != self._generation:
+            return "an optimizer step updated the weights"
+        if self._version_state() != self._versions:
+            return "the weights were modified in place (optimizer step, load_state_dict or another write)"
+        return None
 
 
 def allreduce_flat_grads(flats, average: bool = True) -> int:
@@ -265,6 +331,22 @@ class LlamaCore:
             self.gd.append(m.down_proj.weight.grad)
         self.cos, self.sin = rope_tables(dims, flat.flat.device)
         self.fused_epilogues = True
+        self.fp8 = None
+
+    def set_fp8(self, fp8: Optional[Fp8Weights]) -> None:
+        """Stream ``fp8``'s copy of the linear weights in the skinny decode GEMMs (None: the bf16 weights)."""
+        self.fp8 = None
+        if fp8 is None:
+            return
+        D, F = self.d.hidden, self.d.inter
+        w = SimpleNamespace(wqkv=[], wo=[], wgu=[], wd=[])
+        for lyr in self.model.layers:
+            a, m = lyr.self_attn, lyr.mlp
+            w.wqkv.append(fp8.view([a.q_proj.weight, a.k_proj.weight, a.v_proj.weight], (3 * D, D)))
+            w.wo.append(fp8.view([a.o_proj.weight], (D, D)))
+            w.wgu.append(fp8.view([m.gate_proj.weight, m.up_proj.weight], (2 * F, D)))
+            w.wd.append(fp8.view([m.down_proj.weight], (D, F)))
+        self.fp8 = w
 
     def refresh_grad_views(self) -> None:
         """Re-derive the fused gradient views after ``FlatParams.rebind_grads``."""
@@ -511,27 +593,36 @@ class LlamaCore:
         # The step is HBM-bound weight streaming.  Batches <= 16 use the swap-AB cluster-split-K kernel with the SwiGLU fused
         # (gemm_skinny.cu); larger batches go through nv_gemm_bf16's auto dispatch, which picks the tile variant per (M, N)
         # from a measured table (32-column tiles for the 4096-wide projections, 256 for gate|up: tools/midm_bench.py).
+        # With an fp8 copy of the weights (set_fp8), the skinny GEMMs stream it instead: same bits as bf16 on W'.
         bn = DECODE_BLOCK_N
         skinny = bn == 0 and x.shape[0] <= 16
         fuse_mlp = skinny and d.inter % 64 == 0
-        if skinny:
-            lin = lambda a, w, addend=None: ops.gemm_skinny(a, w, addend=addend)
+        f8 = self.fp8 if skinny else None
+        if f8 is not None:
+            lin = lambda a, w, addend=None: ops.gemm_skinny_fp8(a, *w, addend=addend)
+            wqkv, wo, wgu, wd = f8.wqkv, f8.wo, f8.wgu, f8.wd
         else:
-            lin = lambda a, w, addend=None: ops.gemm(a, w, addend=addend, block_n=bn)
+            wqkv, wo, wgu, wd = self.wqkv, self.wo, self.wgu, self.wd
+            if skinny:
+                lin = lambda a, w, addend=None: ops.gemm_skinny(a, w, addend=addend)
+            else:
+                lin = lambda a, w, addend=None: ops.gemm(a, w, addend=addend, block_n=bn)
         for l, lyr in enumerate(self.model.layers):
             xn, _ = ops.rmsnorm_fwd(x, lyr.input_layernorm.weight.data, d.rms_eps)
-            qkv = lin(xn, self.wqkv[l])
+            qkv = lin(xn, wqkv[l])
             if d.head_dim == 128:
                 ao = ops.decode_attn_rope(qkv, lens, self.cos, self.sin, kc[l], vc[l], H)   # RoPE + cache append + attention
             else:
                 ops.rope_(qkv, lens, self.cos, self.sin, 2 * H, d.head_dim)
                 ops.kv_append(qkv, lens, kc[l], vc[l])
                 ao = ops.decode_attn(qkv, kc[l], vc[l], lens, H)
-            xm = lin(ao, self.wo[l], x)
+            xm = lin(ao, wo[l], x)
             xn2, _ = ops.rmsnorm_fwd(xm, lyr.post_attention_layernorm.weight.data, d.rms_eps)
-            if fuse_mlp:
-                h = ops.gemm_skinny_swiglu(xn2, self.wgu[l])                            # gate|up projection + SwiGLU
+            if fuse_mlp and f8 is not None:
+                h = ops.gemm_skinny_swiglu_fp8(xn2, *wgu[l])
+            elif fuse_mlp:
+                h = ops.gemm_skinny_swiglu(xn2, wgu[l])                                 # gate|up projection + SwiGLU
             else:
-                h = ops.swiglu_fwd(lin(xn2, self.wgu[l]))
-            x = lin(h, self.wd[l], xm)
+                h = ops.swiglu_fwd(lin(xn2, wgu[l]))
+            x = lin(h, wd[l], xm)
         return x

@@ -25,7 +25,7 @@ import torch.nn as nn
 
 from . import llama as llama_mod
 from . import ops
-from .llama import FlatParams, LlamaCore, LlamaDims, LlamaModelParams, _Linear
+from .llama import FlatParams, Fp8Weights, LlamaCore, LlamaDims, LlamaModelParams, _Linear
 from .parallel import GradSync
 from .tokenizer import HFTokenizerAdapter, SyntheticTokenizer
 
@@ -487,6 +487,54 @@ class ModifiedLlamaForCausalLM(nn.Module):
         return LMOutput(loss=loss, logits=logits, past_key_values=None, hidden_states=hidden, attentions=None)
 
 
+    # ---- opt-in fp8 (e4m3) weight streaming in the decode step ----
+    def fp8_linear_weights(self) -> List[nn.Parameter]:
+        """The weights ``quantize_weights_fp8`` rounds: q/k/v/o and gate/up/down of every layer, and lm_head."""
+        ps: List[nn.Parameter] = []
+        for lyr in self.model.layers:
+            a, m = lyr.self_attn, lyr.mlp
+            ps += [a.q_proj.weight, a.k_proj.weight, a.v_proj.weight, a.o_proj.weight, m.gate_proj.weight, m.up_proj.weight,
+                   m.down_proj.weight]
+        return ps + [self.lm_head.weight]
+
+    @torch.no_grad()
+    def quantize_weights_fp8(self) -> int:
+        """Round every LM linear weight IN PLACE to W' = e4m3(W / 2^e_n) * 2^e_n (one power-of-two exponent per output row,
+        include/navillm_b200.h) and keep an fp8 copy of them (about 6.6 GB at Vicuna-7B).  W' is exact in bf16, so the
+        model afterwards IS the model with weights W': prefill, navigation, training and ``state_dict()`` all see W'.
+        ``generate`` then streams the fp8 copy in every decode-step GEMM of batches <= 16 (half the bytes; the same bits as
+        the bf16 kernels on W') and keeps the bf16 path on W' above that.  Irreversible: reload the checkpoint to get W
+        back.  Any later write to the weights (an optimizer step, ``load_state_dict``) makes ``generate`` raise until this
+        is called again (or ``drop_fp8_weights``).  Returns the size of the copy in bytes."""
+        self._ensure()
+        self.drop_fp8_weights()
+        self._fp8 = Fp8Weights(self.flat, self.fp8_linear_weights())
+        self.core.set_fp8(self._fp8)
+        return self._fp8.nbytes
+
+    def drop_fp8_weights(self) -> None:
+        """Free the fp8 copy; ``generate`` goes back to the bf16 kernels (on the weights as they are, W' if quantized)."""
+        self._fp8 = None
+        if self.core is not None:
+            self.core.set_fp8(None)
+        self.__dict__.pop("_decode_states", None)     # captured decode graphs hold the pointers of the other kernels
+
+    @property
+    def fp8_weights(self) -> Optional[Fp8Weights]:
+        return self.__dict__.get("_fp8")
+
+    def _check_fp8_fresh(self) -> None:
+        fp8 = self.fp8_weights
+        if fp8 is None:
+            return
+        why = fp8.stale_reason(self.flat)
+        if why is not None:
+            raise RuntimeError(f"generate(): the fp8 copy of the weights is stale ({why} after quantize_weights_fp8()); call "
+                               f"quantize_weights_fp8() again to re-quantize the current weights, or drop_fp8_weights() to "
+                               f"decode with them in bf16")
+        if self.core.fp8 is None:                    # the decoder stack was rebuilt around the same buffer
+            self.core.set_fp8(fp8)
+
     # ---- generation (models/nav_model.py:324-338,388-399; HF GenerationMixin greedy / sampling) ----
     decode_pdl = os.environ.get("NAVILLM_DECODE_PDL", "1") != "0"   # developer knob: 0 = plain stream-ordered launches
     max_decode_states = 2        # cached (KV buffers + captured decode graph) sets, least recently used evicted
@@ -538,6 +586,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
         if do_sample and not temperature > 0:
             raise ValueError("generate(do_sample=True) needs temperature > 0")
         self._ensure()
+        self._check_fp8_fresh()
         dev = self._device()
         core, d = self.core, self.dims
         eos = self.tokenizer.eos_token_id if eos_token_id is None else eos_token_id
@@ -563,9 +612,15 @@ class ModifiedLlamaForCausalLM(nn.Module):
         hid_last, _ = core.forward(x, pp.pos, pp.cu, pp.seqlens, save=False, kv_store=(kc, vc), out_rows=pp.last_rows)
         special = self.special_ids_dev
 
+        fp8_head = None
+        if core.fp8 is not None:
+            fp8_head = self._fp8.view([self.lm_head.weight], tuple(self.lm_head.weight.shape))
+
         def head(h_rows):
             hn, _ = ops.rmsnorm_fwd(h_rows, self.model.norm.weight.data, d.rms_eps)
-            if B <= 16 and llama_mod.DECODE_BLOCK_N == 0:
+            if B <= 16 and llama_mod.DECODE_BLOCK_N == 0 and fp8_head is not None:
+                ops.gemm_skinny_fp8(hn, *fp8_head, out=logits)
+            elif B <= 16 and llama_mod.DECODE_BLOCK_N == 0:
                 ops.gemm_skinny(hn, self.lm_head.weight.data, out=logits)
             else:
                 ops.gemm(hn, self.lm_head.weight.data, out=logits, block_n=llama_mod.DECODE_BLOCK_N)

@@ -243,6 +243,16 @@ class NavModel(nn.Module):
         elif f.params[0].grad is None or f.params[0].grad.data_ptr() != f.flat_grad.data_ptr():
             f.reattach_grads()
 
+    def quantize_weights_fp8(self) -> int:
+        """Opt-in fp8 (e4m3) weight streaming for text generation: ``ModifiedLlamaForCausalLM.quantize_weights_fp8`` on the
+        language model.  Rounds its linear weights (and lm_head) in place; the embeddings, norms, ``out_head`` / ``og_head``
+        and the fp32 panorama encoder are not touched.  Returns the size of the fp8 copy in bytes."""
+        self._ensure()
+        return self.lang_model.quantize_weights_fp8()
+
+    def drop_fp8_weights(self) -> None:
+        self.lang_model.drop_fp8_weights()
+
     def _flat_buffers_ready(self) -> bool:
         return self.lang_model.core is not None and self._flat32 is not None
 

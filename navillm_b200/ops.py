@@ -675,6 +675,73 @@ def gemm_skinny_swiglu(x: torch.Tensor, wgu: torch.Tensor, *, out: torch.Tensor 
     return out
 
 
+fp8 = torch.float8_e4m3fn
+
+
+def quantize_fp8_(w: torch.Tensor, q: torch.Tensor, exps: torch.Tensor) -> torch.Tensor:
+    """Round the bf16 weight w [N, K] in place to W' = e4m3(w / 2^e_n) * 2^e_n with one power-of-two exponent per row
+    (csrc/quant.cu, format in include/navillm_b200.h): q [N, K] float8_e4m3fn receives the e4m3 values, exps [N] int8 the
+    exponents.  Returns w."""
+    _rowmajor(w, "w"); _rowmajor(q, "q")
+    if w.dtype != bf16 or q.dtype != fp8 or exps.dtype != torch.int8:
+        raise ValueError(f"quantize_fp8_: w bf16, q float8_e4m3fn, exps int8 expected (got {w.dtype}, {q.dtype}, {exps.dtype})")
+    N, K = w.shape
+    if tuple(q.shape) != (N, K) or exps.shape != (N,) or not exps.is_contiguous():
+        raise ValueError(f"quantize_fp8_: w {tuple(w.shape)} q {tuple(q.shape)} exps {tuple(exps.shape)}")
+    check(_lib.load().nv_quantize_fp8_rows(ptr(w), i64(w.stride(0)), ptr(q), i64(q.stride(0)), ptr(exps), i32(N), i32(K),
+                                           stream_ptr()), "nv_quantize_fp8_rows")
+    return w
+
+
+def _fp8_weight(wq: torch.Tensor, exps: torch.Tensor, name: str) -> None:
+    _rowmajor(wq, name)
+    if wq.dtype != fp8 or exps.dtype != torch.int8 or exps.shape != (wq.shape[0],) or not exps.is_contiguous():
+        raise ValueError(f"{name}: float8_e4m3fn [N, K] weight with int8 [N] row exponents expected "
+                         f"(got {wq.dtype} {tuple(wq.shape)}, {exps.dtype} {tuple(exps.shape)})")
+
+
+def gemm_skinny_fp8(x: torch.Tensor, wq: torch.Tensor, exps: torch.Tensor, *, addend: torch.Tensor | None = None,
+                    out: torch.Tensor | None = None) -> torch.Tensor:
+    """``gemm_skinny`` with the weight in the fp8 format of ``quantize_fp8_`` (wq e4m3 [N, K], exps int8 [N]): bit for
+    bit ``gemm_skinny(x, W')`` while reading half the weight bytes."""
+    _rowmajor(x, "x"); _fp8_weight(wq, exps, "wq")
+    assert x.dtype == bf16
+    M, K = x.shape
+    N = wq.shape[0]
+    if wq.shape[1] != K or M > 16:
+        raise ValueError(f"gemm_skinny_fp8: x {tuple(x.shape)} wq {tuple(wq.shape)} (needs M <= 16 and matching K)")
+    if out is None:
+        out = torch.empty((M, N), dtype=bf16, device=x.device)
+    _rowmajor(out, "out")
+    assert out.shape == (M, N) and out.dtype == bf16
+    if addend is not None:
+        _rowmajor(addend, "addend")
+        assert addend.shape == (M, N) and addend.dtype == bf16
+    check(_lib.load().nv_gemm_skinny_fp8(ptr(x), i64(x.stride(0)), ptr(wq), i64(wq.stride(0)), ptr(exps), ptr(out),
+                                         i64(out.stride(0)), ptr(addend), i64(addend.stride(0) if addend is not None else 0),
+                                         i32(M), i32(N), i32(K), stream_ptr()), "nv_gemm_skinny_fp8")
+    return out
+
+
+def gemm_skinny_swiglu_fp8(x: torch.Tensor, wgu_q: torch.Tensor, exps: torch.Tensor, *,
+                           out: torch.Tensor | None = None) -> torch.Tensor:
+    """``gemm_skinny_swiglu`` with the fused gate|up weight in fp8 (wgu_q e4m3 [2F, K], exps int8 [2F])."""
+    _rowmajor(x, "x"); _fp8_weight(wgu_q, exps, "wgu_q")
+    assert x.dtype == bf16
+    M, K = x.shape
+    F = wgu_q.shape[0] // 2
+    if wgu_q.shape[1] != K or M > 16 or F % 64 or wgu_q.shape[0] != 2 * F:
+        raise ValueError(f"gemm_skinny_swiglu_fp8: x {tuple(x.shape)} wgu_q {tuple(wgu_q.shape)} (needs M <= 16, F % 64 == 0)")
+    if out is None:
+        out = torch.empty((M, F), dtype=bf16, device=x.device)
+    _rowmajor(out, "out")
+    assert out.shape == (M, F) and out.dtype == bf16
+    check(_lib.load().nv_gemm_skinny_swiglu_fp8(ptr(x), i64(x.stride(0)), ptr(wgu_q), i64(wgu_q.stride(0)), ptr(exps), ptr(out),
+                                                i64(out.stride(0)), i32(M), i32(F), i32(K), stream_ptr()),
+          "nv_gemm_skinny_swiglu_fp8")
+    return out
+
+
 def decode_rope_kv_(qkv, lens, cos_t, sin_t, kc, vc, n_heads):
     """In-place RoPE of the new token's q,k at position lens[b] + append of the rotated K and V to the caches."""
     B, Smax, HD = kc.shape

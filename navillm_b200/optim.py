@@ -52,6 +52,7 @@ class FlatAdamW:
                                     i32(f.dtype == torch.bfloat16), f32(lr), f32(self.betas[0]), f32(self.betas[1]), f32(self.eps),
                                     f32(self.weight_decay), i32(self.step_count), ptr(state), i32(write_clipped_grad),
                                     stream_ptr()), "nv_adamw_flat")
+            f.generation += 1                          # raw-pointer write: invalidates an fp8 copy of the weights
 
     def grad_norm(self) -> torch.Tensor:
         """Total gradient norm measured by the last ``step(max_grad_norm=...)`` (device scalar, no sync)."""
