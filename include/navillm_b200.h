@@ -78,6 +78,12 @@ int nv_gemm_skinny_fp8(const void* X, int64_t ldx, const void* Wq, int64_t ldw, 
                        const void* addend, int64_t ld_add, int M, int N, int K, void* stream);
 int nv_gemm_skinny_swiglu_fp8(const void* X, int64_t ldx, const void* Wgu_q, int64_t ldw, const void* exps, void* H,
                               int64_t ldh, int M, int F, int K, void* stream);
+/* nv_gemm_fp8w_bf16 is nv_gemm_bf16 with K-major operands (a_mn = b_mn = 0) and the weight given as (Wq, exps) in the same
+ * format, for the inference GEMMs above 16 rows (prefix-cached navigation suffixes, pruned last layers, decode batches
+ * 17..256): C = bf16(bf16(A Wq'^T) + addend) with addend optional, bit for bit nv_gemm_bf16's result on W' at every M, N, K
+ * and tile width.  block_n: 0 (auto), 32 or 128.  lda % 8 == 0, ldw (bytes) % 16 == 0. */
+int nv_gemm_fp8w_bf16(const void* A, int64_t lda, const void* Wq, int64_t ldw, const void* exps, void* C, int64_t ldc,
+                      const void* addend, int64_t ld_add, int M, int N, int K, int block_n, void* stream);
 int nv_gemm_swiglu_bf16(const void* x, int64_t ldx, const void* Wgu, int64_t ldw, void* gu, int64_t ldgu, void* h,
                         int64_t ldh, int M, int F, int K, int keep_gu, void* stream);
 int nv_gemm_dswiglu_bf16(const void* dx, int64_t lddx, const void* Wd, int64_t ldw, const void* gu, int64_t ldgu, void* dgu,
@@ -238,6 +244,11 @@ typedef struct nv_layer_args {
   void* ws; int64_t ws_bytes;
   int B, T, total_qblocks, Smax, Tkv, kv_mode, R, D, F, H;
   float eps, scale;
+  /* optional fp8 copies of the four weights (e4m3 rows, int8 row exponents: nv_quantize_fp8_rows); a GEMM whose weight
+   * pair is set and whose row count (T for qkv, R or T for the others) is <= fp8_max_rows runs nv_gemm_fp8w_bf16 */
+  const void* wqkv_q; const void* wqkv_e; const void* wo_q; const void* wo_e;
+  const void* wgu_q; const void* wgu_e; const void* wd_q; const void* wd_e;
+  int fp8_max_rows;
 } nv_layer_args;
 int nv_layer_args_size(void);                           /* sizeof(nv_layer_args): bindings check their mirror against it */
 int64_t nv_llama_layer_ws_bytes(int T, int R, int D, int F);

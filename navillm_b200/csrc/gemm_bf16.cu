@@ -23,7 +23,16 @@
 // rows (rotate-half pairs, the gate and up halves of SwiGLU, the per-head row sums of the attention backward).
 // HBM layout assumptions: base pointers 16-byte aligned, leading dimensions multiples of 8 elements.
 // Ragged M/N/K are handled by TMA zero-fill on loads and predicated stores.
+//
+// fp8 weights (WT = uint8_t; EPI_PLAIN, K-major operands, BLOCK_N 32 / 128): B is the e4m3 copy of an nn.Linear weight with
+// one power-of-two exponent per row (nv_fp8.cuh).  The producer TMA-loads the e4m3 tile unswizzled (64-byte rows, half the
+// bytes of a bf16 stage) next to the bf16 A tile.  A fourth warpgroup (warps 9..12) expands each raw tile with
+// fp8x4_to_bf16x4 into a bf16 buffer of its own stage, 128-byte swizzled exactly as the TMA writes a bf16 B tile, and signals
+// a third mbarrier per stage; the consumers wait for it and run the unchanged SS wgmmas.  The expansion of stage s + 1
+// overlaps the MMAs of stage s.  The k-blocks, the wgmma sequence and the epilogue are those of the bf16 kernel, and the
+// expanded operand is bit for bit the W' the quantizer wrote back, so C equals nv_gemm_bf16's C on W'.
 #include "nv_common.cuh"
+#include "nv_fp8.cuh"
 #include "nv_host.h"
 
 namespace nv {
@@ -62,15 +71,22 @@ struct EpiAux {
   const __nv_bfloat16* cos_t;
   const __nv_bfloat16* sin_t;
   uint32_t rope_cols;   // ROPE: q and k columns (2 * H * 128)
+  const int8_t* w_exp;  // fp8 weights: w_exp[n] = exponent of weight row n (W' = e4m3 * 2^w_exp)
 };
 
-template <uint32_t BLOCK_N, uint32_t STAGES>
+// Shared memory: [A stages][B stages][fp8 only: expanded bf16 B stages][full | empty | fp8 only: expanded barriers]
+template <uint32_t BLOCK_N, uint32_t STAGES, typename WT = __nv_bfloat16>
 struct GemmSmem {
+  static constexpr bool kFp8 = sizeof(WT) == 1;
+  static constexpr uint32_t THREADS = kFp8 ? GEMM_THREADS + 128 : GEMM_THREADS;   // + the expansion warpgroup
   static constexpr uint32_t A_BYTES = GEMM_BLOCK_M * GEMM_BLOCK_K * 2;
-  static constexpr uint32_t B_BYTES = BLOCK_N * GEMM_BLOCK_K * 2;
-  static constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr uint32_t BAR_OFF = STAGES * STAGE_BYTES;
-  static constexpr uint32_t DYN_BYTES = BAR_OFF + 2 * STAGES * 8 + 1024;  // + slack for manual 1024-byte alignment
+  static constexpr uint32_t B_BYTES = BLOCK_N * GEMM_BLOCK_K * sizeof(WT);
+  static constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;                      // TMA bytes per stage
+  static constexpr uint32_t CVT_BYTES = kFp8 ? BLOCK_N * GEMM_BLOCK_K * 2 : 0;
+  static constexpr uint32_t CVT_OFF = STAGES * STAGE_BYTES;
+  static constexpr uint32_t BAR_OFF = CVT_OFF + STAGES * CVT_BYTES;
+  static constexpr uint32_t DYN_BYTES = BAR_OFF + (kFp8 ? 3 : 2) * STAGES * 8 + 1024;  // + slack for 1024-byte alignment
+  static_assert(CVT_OFF % 1024 == 0, "the expanded stages are 128-byte-swizzle atoms");
   static constexpr uint32_t ACC_LD = BLOCK_N + 4;                         // staged fp32 row (+16 B: conflict-free)
   static_assert(GEMM_BLOCK_M * ACC_LD * 4 <= BAR_OFF, "accumulator staging reuses the stage ring");
   static_assert(DYN_BYTES <= 232448, "shared memory per block");
@@ -98,19 +114,23 @@ __device__ __forceinline__ void ld_acc32(const float* p, uint32_t (&v)[32]) {
   }
 }
 
-template <uint32_t BLOCK_N, uint32_t STAGES, bool A_MN, bool B_MN, int EPI>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
+template <uint32_t BLOCK_N, uint32_t STAGES, bool A_MN, bool B_MN, int EPI, typename WT = __nv_bfloat16>
+__global__ void __launch_bounds__(GemmSmem<BLOCK_N, STAGES, WT>::THREADS, 1)
 gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                 void* __restrict__ Cout, int64_t ldc, const __nv_bfloat16* __restrict__ addend, int64_t ld_add,
                 uint32_t M, uint32_t N, uint32_t K, uint32_t flags, EpiAux ea) {
-  using L = GemmSmem<BLOCK_N, STAGES>;
+  using L = GemmSmem<BLOCK_N, STAGES, WT>;
   static_assert(EPI == EPI_PLAIN || BLOCK_N == 256, "fused epilogues use the 128 x 256 tile");
+  static_assert(!L::kFp8 || (EPI == EPI_PLAIN && !A_MN && !B_MN && BLOCK_N <= 128),
+                "fp8 weights: plain epilogue, K-major operands, 32- or 128-wide tiles");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + STAGES * L::A_BYTES;
+  uint8_t* smem_cvt = smem + L::CVT_OFF;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
   uint64_t* empty_bar = full_bar + STAGES;
+  uint64_t* cvt_bar = empty_bar + STAGES;                 // fp8: the expanded bf16 B tile of the stage is complete
 
   const uint32_t warp = warp_id_uniform();
   // logical output columns per tile: BLOCK_N, except SWIGLU where the 256 accumulator columns are 128 gate + 128 up
@@ -124,7 +144,9 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
   if (threadIdx.x == 0) {
     for (uint32_t i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 2);  // one arrive per consumer warpgroup
+      // one arrive per consumer warpgroup (fp8: + one per expansion thread, after its reads of the raw tile)
+      mbar_init(&empty_bar[i], L::kFp8 ? 2 + 128 : 2);
+      if constexpr (L::kFp8) mbar_init(&cvt_bar[i], 128);
     }
     fence_mbar_init();
   }
@@ -150,7 +172,9 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
           for (uint32_t i = 0; i < GEMM_BLOCK_M / 64; ++i)  // box {64 m, 64 k} per 64-wide MN atom
             tma_load_2d(sa + i * (GEMM_BLOCK_K * 128), &tmap_a, &full_bar[stage], m0 + i * 64, k0);
         }
-        if constexpr (!B_MN) {
+        if constexpr (L::kFp8) {
+          tma_load_2d(sb, &tmap_b, &full_bar[stage], k0, n_blk * BLOCK_N);   // box {64 k, BLOCK_N n}, unswizzled e4m3
+        } else if constexpr (!B_MN) {
           constexpr uint32_t BOX = BLOCK_N < 128 ? BLOCK_N : 128;  // box {64 k, BOX n}
 #pragma unroll
           for (uint32_t i = 0; i < BLOCK_N / BOX; ++i) {
@@ -169,6 +193,47 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
     return;  // the producer takes no part in the epilogue (named barrier 1 counts the 256 consumer threads only)
   }
 
+  if constexpr (L::kFp8) {
+    if (warp >= 9) {
+      // ===================== fp8 expansion (warps 9..12) =====================
+      // thread t owns the 16-byte e4m3 chunks q = t + 128 j of the tile (row q / 4, k 16 (q % 4) ..+15) and writes them as
+      // bf16 chunks 2 (q % 4), 2 (q % 4) + 1 of the swizzled row.  Rows >= N are TMA zero fill (scale 1).
+      constexpr uint32_t J = BLOCK_N * GEMM_BLOCK_K / 16 / 128;
+      const uint32_t t = threadIdx.x - GEMM_THREADS;
+      float scale[J];
+#pragma unroll
+      for (uint32_t j = 0; j < J; ++j) {
+        const uint32_t n = n_blk * BLOCK_N + ((t + 128 * j) >> 2);
+        scale[j] = n < N ? fp8_pow2(ea.w_exp[n]) : 1.f;
+      }
+      uint32_t stage = 0, phase = 0;
+      for (uint32_t kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        // the consumers released this stage's expanded buffer (empty_bar) before the producer refilled it
+        const uint32_t src = smem_u32(smem_b + stage * L::B_BYTES);
+        const uint32_t dst = smem_u32(smem_cvt + stage * L::CVT_BYTES);
+#pragma unroll
+        for (uint32_t j = 0; j < J; ++j) {
+          const uint32_t q = t + 128 * j, row = q >> 2, c = q & 3;
+          uint4 v;
+          asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(src + q * 16));
+          uint32_t o[8];
+          fp8x4_to_bf16x4(v.x, scale[j], o[0], o[1]);
+          fp8x4_to_bf16x4(v.y, scale[j], o[2], o[3]);
+          fp8x4_to_bf16x4(v.z, scale[j], o[4], o[5]);
+          fp8x4_to_bf16x4(v.w, scale[j], o[6], o[7]);
+          sts128(dst + sw128_offset(row, 2 * c), o[0], o[1], o[2], o[3]);
+          sts128(dst + sw128_offset(row, 2 * c + 1), o[4], o[5], o[6], o[7]);
+        }
+        fence_proxy_async_smem();                          // generic-proxy writes -> wgmma operand reads
+        mbar_arrive(&cvt_bar[stage]);
+        mbar_arrive(&empty_bar[stage]);                    // this thread's part of the raw e4m3 tile has been read
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      return;
+    }
+  }
+
   // ===================== consumers (warpgroups 0, 1) =====================
   const uint32_t wg = warp >> 2;
   float acc[BLOCK_N / 2];
@@ -183,8 +248,10 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
     uint32_t stage = 0, phase = 0, prev = 0;
     for (uint32_t kb = 0; kb < num_kb; ++kb) {
       mbar_wait(&full_bar[stage], phase);
+      if constexpr (L::kFp8) mbar_wait(&cvt_bar[stage], phase);
       const uint64_t adesc = gmma_desc_sw128(smem_u32(smem_a + stage * L::A_BYTES + wg * 8192), A_LBO, 1024);
-      const uint64_t bdesc = gmma_desc_sw128(smem_u32(smem_b + stage * L::B_BYTES), B_LBO, 1024);
+      const uint64_t bdesc = gmma_desc_sw128(smem_u32(L::kFp8 ? smem_cvt + stage * L::CVT_BYTES : smem_b + stage * L::B_BYTES),
+                                             B_LBO, 1024);
       wgmma_fence();
 #pragma unroll
       for (uint32_t k = 0; k < GEMM_BLOCK_K / 16; ++k)
@@ -412,19 +479,19 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
   }
 }
 
-template <uint32_t BN, uint32_t ST, bool A_MN, bool B_MN, int EPI = EPI_PLAIN>
+template <uint32_t BN, uint32_t ST, bool A_MN, bool B_MN, int EPI = EPI_PLAIN, typename WT = __nv_bfloat16>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int64_t ldc, const void* addend,
                        int64_t ld_add, uint32_t M, uint32_t N, uint32_t K, uint32_t flags, cudaStream_t stream,
                        EpiAux ea = EpiAux{}) {
-  using L = GemmSmem<BN, ST>;
-  auto kern = gemm_bf16_wgmma<BN, ST, A_MN, B_MN, EPI>;
+  using L = GemmSmem<BN, ST, WT>;
+  auto kern = gemm_bf16_wgmma<BN, ST, A_MN, B_MN, EPI, WT>;
   static bool attr_set = false;
   if (!attr_set) {
     NV_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::DYN_BYTES));
     attr_set = true;
   }
   const uint32_t tiles = ceil_div_u32(M, GEMM_BLOCK_M) * ceil_div_u32(N, EPI == EPI_SWIGLU ? 128u : BN);
-  kern<<<tiles, GEMM_THREADS, L::DYN_BYTES, stream>>>(ta, tb, C, ldc, reinterpret_cast<const __nv_bfloat16*>(addend), ld_add,
+  kern<<<tiles, L::THREADS, L::DYN_BYTES, stream>>>(ta, tb, C, ldc, reinterpret_cast<const __nv_bfloat16*>(addend), ld_add,
                                                       M, N, K, flags, ea);
   NV_LAUNCH_CHECK();
   return NV_OK;
@@ -487,6 +554,33 @@ extern "C" int nv_gemm_bf16(const void* A, int64_t lda, int a_mn, const void* B,
   }
   NV_GEMM_CASE(128, 6);
 #undef NV_GEMM_CASE
+}
+
+// C[M,N] = A[M,K] · W'[N,K]^T (+ addend) with W' = Wq * 2^exps given in the fp8 weight format (e4m3 rows, one int8
+// exponent per row; ldw in bytes): bit for bit nv_gemm_bf16(A, W', block_n) for every M, N, K, reading half the weight bytes.
+extern "C" int nv_gemm_fp8w_bf16(const void* A, int64_t lda, const void* Wq, int64_t ldw, const void* exps, void* C, int64_t ldc,
+                                 const void* addend, int64_t ld_add, int M, int N, int K, int block_n, void* stream_) {
+  using namespace nv;
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  NV_REQUIRE(M > 0 && N > 0 && K > 0, "nv_gemm_fp8w_bf16: empty problem M=%d N=%d K=%d", M, N, K);
+  NV_REQUIRE(A && Wq && exps && C, "nv_gemm_fp8w_bf16: null operand");
+  NV_REQUIRE((lda & 7) == 0 && (ldw & 15) == 0,
+             "nv_gemm_fp8w_bf16: lda must be a multiple of 8 and ldw (bytes) of 16 (got %lld, %lld)", (long long)lda, (long long)ldw);
+  // auto: nv_gemm_bf16's choice for K-major operands below M = 512 (the 256-wide tile is not built for fp8 weights)
+  if (block_n == 0) block_n = (M <= 128 && N <= 4096) ? 32 : 128;
+  NV_REQUIRE(block_n == 32 || block_n == 128, "nv_gemm_fp8w_bf16: block_n must be 0, 32 or 128 (got %d)", block_n);
+  CUtensorMap ta, tb;
+  int rc = make_tmap_2d(&ta, A, 2, (uint64_t)K, (uint64_t)M, (uint64_t)lda * 2, 64, GEMM_BLOCK_M);
+  if (rc) return rc;
+  if ((rc = make_tmap_2d(&tb, Wq, 1, (uint64_t)K, (uint64_t)N, (uint64_t)ldw, 64, (uint32_t)block_n, /*swizzle128=*/false)))
+    return rc;
+  EpiAux ea{};
+  ea.w_exp = reinterpret_cast<const int8_t*>(exps);
+  const uint32_t flags = addend ? GEMM_ADD : 0u;
+  // stages: the bf16 kernel's 10 at BLOCK_N = 32; 5 of 40 KB (A, e4m3 B, expanded B) fit at 128
+  if (block_n == 32)
+    return launch_gemm<32, 10, false, false, EPI_PLAIN, uint8_t>(ta, tb, C, ldc, addend, ld_add, M, N, K, flags, stream, ea);
+  return launch_gemm<128, 5, false, false, EPI_PLAIN, uint8_t>(ta, tb, C, ldc, addend, ld_add, M, N, K, flags, stream, ea);
 }
 
 // ---- fused-epilogue entry points (K-major activations x nn.Linear weights) -------------------------------------

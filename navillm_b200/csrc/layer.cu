@@ -63,10 +63,17 @@ extern "C" int nv_llama_layer_infer(const nv_layer_args* a, void* stream) {
   void* h = c.take((int64_t)Tm * F * 2);
   NV_REQUIRE(h != nullptr, "nv_llama_layer_infer: workspace carve failed");
   int rc;
+  // y[rows, N] = x[rows, K] W^T (+ addend): the fp8 copy of W when it is given and the GEMM has at most fp8_max_rows rows
+  auto linear = [&](const void* x, const void* w, const void* wq, const void* we, void* y, const void* addend, int rows, int N,
+                    int K) {
+    if (wq && we && rows <= a->fp8_max_rows)
+      return nv_gemm_fp8w_bf16(x, K, wq, K, we, y, N, addend, D, rows, N, K, 0, stream);
+    return nv_gemm_bf16(x, K, 0, w, K, 0, y, N, addend, addend ? D : 0, rows, N, K, addend ? 1u : 0u, 0, stream);
+  };
 #define STEP(call) do { rc = (call); if (rc != NV_OK) return rc; } while (0)
   // ---- attention block:  xm = x + o_proj(attn(rope(qkv(rmsnorm1(x))))) ----
   STEP(nv_rmsnorm_fwd(a->x, D, a->ln1, xn, D, rstd, T, D, a->eps, stream));
-  STEP(nv_gemm_bf16(xn, D, 0, a->wqkv, D, 0, qkv, 3 * (int64_t)D, nullptr, 0, T, 3 * D, D, 0u, 0, stream));
+  STEP(linear(xn, a->wqkv, a->wqkv_q, a->wqkv_e, qkv, nullptr, T, 3 * D, D));
   STEP(nv_rope_inplace(qkv, 3 * (int64_t)D, a->pos, a->cos_t, a->sin_t, T, 2 * H, 128, 0, stream));
   if (a->kv_mode == 2) {            // new rows appended to a cache that already holds a prefix; attention over the cache
     STEP(nv_kv_store_suffix(qkv, 3 * (int64_t)D, a->cu_seqlens, a->cached, a->kcache, a->vcache, a->B, T, a->Smax, D, stream));
@@ -82,12 +89,12 @@ extern "C" int nv_llama_layer_infer(const nv_layer_args* a, void* stream) {
     STEP(nv_gather_rows(ao, D, a->out_rows, aor, D, R, D, stream));
     STEP(nv_gather_rows(a->x, D, a->out_rows, xr, D, R, D, stream));
   }
-  STEP(nv_gemm_bf16(aor, D, 0, a->wo, D, 0, xm, D, xr, D, Tm, D, D, 1u /* + addend */, 0, stream));
+  STEP(linear(aor, a->wo, a->wo_q, a->wo_e, xm, xr, Tm, D, D));
   // ---- MLP:  y = xm + down(silu(gate(xn2)) * up(xn2)) ----
   STEP(nv_rmsnorm_fwd(xm, D, a->ln2, xn2, D, rstd2, Tm, D, a->eps, stream));
-  STEP(nv_gemm_bf16(xn2, D, 0, a->wgu, D, 0, gu, 2 * (int64_t)F, nullptr, 0, Tm, 2 * F, D, 0u, 0, stream));
+  STEP(linear(xn2, a->wgu, a->wgu_q, a->wgu_e, gu, nullptr, Tm, 2 * F, D));
   STEP(nv_swiglu_fwd(gu, 2 * (int64_t)F, h, F, Tm, F, stream));
-  STEP(nv_gemm_bf16(h, F, 0, a->wd, F, 0, a->y, D, xm, D, Tm, D, F, 1u, 0, stream));
+  STEP(linear(h, a->wd, a->wd_q, a->wd_e, a->y, xm, Tm, D, F));
 #undef STEP
   return NV_OK;
 }

@@ -6,8 +6,8 @@
 // 448 = 0.875 * 2^9.  e_n is clamped below at NV_FP8_EXP_MIN so that every non-zero W' (>= 2^-9 * 2^e_n) is an fp32 / bf16
 // normal number: then the scale is an exact power of two in both directions, W' is exactly representable in bf16, and
 // flush-to-zero arithmetic cannot change it.  Only rows with max|W| < 2^-108 are affected by the clamp.
-// The quantizer (quant.cu) and the fp8 skinny GEMM (gemm_skinny.cu) expand e4m3 to bf16 with the same function below, so the
-// GEMM's bf16 operand is bit for bit the W' the quantizer wrote back.
+// The quantizer (quant.cu) and the fp8 GEMMs (gemm_skinny.cu, gemm_bf16.cu) expand e4m3 to bf16 with the same function below,
+// so a GEMM's bf16 operand is bit for bit the W' the quantizer wrote back.
 #pragma once
 
 #include <cuda_bf16.h>

@@ -28,6 +28,12 @@ from . import ops
 # decode GEMMs: 0 (default) = swap-AB skinny kernel for batches <= 16 (csrc/gemm_skinny.cu), nv_gemm_bf16's measured tile
 # table above that; 128 / 32 = force that column-tile width of the general kernel (A/B measurements)
 DECODE_BLOCK_N = int(os.environ.get("NAVILLM_DECODE_BLOCK_N", "0"))
+# Largest GEMM row count at which an inference GEMM above 16 rows streams the fp8 copy of its weight (Fp8Weights,
+# nv_gemm_fp8w_bf16) instead of the bf16 weights.  Measured (tools/midm_bench.py --fp8, H100 80GB HBM3 at 700 W, fp8 vs bf16):
+# qkv 1.04-1.10x and down 1.10x at M = 17..64, o_proj 0.95-1.03x; from M = 96 qkv is slower (0.96x), from M = 128 down (0.90x),
+# and at M >= 192 every shape is (0.64-0.94x).  The fused gate|up weight (N = 2F) is slower at every M (0.90-0.95x up to 128),
+# so it keeps its bf16 weight above 16 rows (_fp8_layer).  lm_head: 0.94x at 17, 0.99x at 32, 1.06x at 64.
+FP8_MAX_ROWS = 64
 # weight-gradient GEMMs on a side stream (see LlamaCore.backward)
 WGRAD_STREAM = os.environ.get("NAVILLM_WGRAD_STREAM", "0") != "0"
 
@@ -212,7 +218,8 @@ class FlatParams:
 
 
 class Fp8Weights:
-    """e4m3 copy of linear weights of a ``FlatParams`` buffer for the decode-step GEMMs (csrc/gemm_skinny.cu).
+    """e4m3 copy of linear weights of a ``FlatParams`` buffer for the inference GEMMs: the decode-step skinny GEMMs
+    (csrc/gemm_skinny.cu) and, up to ``FP8_MAX_ROWS`` rows, nv_gemm_fp8w_bf16 (csrc/gemm_bf16.cu).
 
     Building it rounds every listed weight IN PLACE to W' = e4m3(W / 2^e_n) * 2^e_n (one power-of-two exponent per output
     row, csrc/quant.cu), so the bf16 buffer and the fp8 copy describe the same model.  The copy keeps the flat buffer's
@@ -332,10 +339,13 @@ class LlamaCore:
         self.cos, self.sin = rope_tables(dims, flat.flat.device)
         self.fused_epilogues = True
         self.fp8 = None
+        self.fp8_src = None
 
     def set_fp8(self, fp8: Optional[Fp8Weights]) -> None:
-        """Stream ``fp8``'s copy of the linear weights in the skinny decode GEMMs (None: the bf16 weights)."""
+        """Stream ``fp8``'s copy of the linear weights in the inference GEMMs (None: the bf16 weights): the decode step, and
+        the no-grad forwards while the copy is fresh (``fp8_for_inference``)."""
         self.fp8 = None
+        self.fp8_src = fp8
         if fp8 is None:
             return
         D, F = self.d.hidden, self.d.inter
@@ -347,6 +357,25 @@ class LlamaCore:
             w.wgu.append(fp8.view([m.gate_proj.weight, m.up_proj.weight], (2 * F, D)))
             w.wd.append(fp8.view([m.down_proj.weight], (D, F)))
         self.fp8 = w
+
+    def fp8_for_inference(self):
+        """The per-layer fp8 weight pairs when the copy still describes the current weights, else None.  The inference
+        forwards (navigation, grounding, prefix-cached steps, prefill) then run bf16 on the current weights: a weight write
+        after ``quantize_weights_fp8`` must not change what they compute, and must not make them fail either."""
+        if self.fp8 is None or self.fp8_src.stale_reason(self.flat) is not None:
+            return None
+        return self.fp8
+
+    @staticmethod
+    def _linear(a, w, wq, addend=None):
+        """a · w^T (+ addend) from the fp8 pair ``wq`` when it is given and a has at most FP8_MAX_ROWS rows."""
+        if wq[0] is not None and a.shape[0] <= FP8_MAX_ROWS:
+            return ops.gemm_fp8w(a, *wq, addend=addend)
+        return ops.gemm(a, w, addend=addend)
+
+    def _fp8_layer(self, f8, l):
+        """(qkv, o, gate|up, down) fp8 pairs of layer l for the GEMMs above 16 rows: gate|up stays bf16 (see FP8_MAX_ROWS)."""
+        return None if f8 is None else (f8.wqkv[l], f8.wo[l], (None, None), f8.wd[l])
 
     def refresh_grad_views(self) -> None:
         """Re-derive the fused gradient views after ``FlatParams.rebind_grads``."""
@@ -374,12 +403,13 @@ class LlamaCore:
             run.set_cache_mode(1, kv_store[0][0].shape[1])
         bufs = [torch.empty_like(x), torch.empty_like(x)]
         last = d.n_layers - 1
+        f8 = self.fp8_for_inference()
         for l, lyr in enumerate(self.model.layers):
             pruned = out_rows is not None and l == last
             y = torch.empty((R, d.hidden), dtype=bf16, device=x.device) if pruned else bufs[l & 1]
             run.run(x, y, lyr.input_layernorm.weight.data, self.wqkv[l], self.wo[l], lyr.post_attention_layernorm.weight.data, self.wgu[l],
                     self.wd[l], kc=kv_store[0][l] if kv_store is not None else None, vc=kv_store[1][l] if kv_store is not None else None,
-                    out_rows=out_rows if pruned else None)
+                    out_rows=out_rows if pruned else None, fp8=self._fp8_layer(f8, l), fp8_max_rows=FP8_MAX_ROWS)
             x = y
         return x
 
@@ -405,14 +435,16 @@ class LlamaCore:
             kv_sink = lambda l, qkv: ops.kv_store_prefill(qkv, cu, kv_store[0][l], kv_store[1][l], B_, T_)
         if self.LAYER_CALL and not save and not fused and d.head_dim == 128 and (kv_store is not None or kv_sink is None):
             return self._forward_layer_calls(x, pos, cu, seqlens, kv_store, out_rows), None
+        f8 = None if save else self.fp8_for_inference()     # training forwards never read the fp8 copy
         for l, lyr in enumerate(self.model.layers):
+            w8 = self._fp8_layer(f8, l) or ((None, None),) * 4
             s = _Saved()
             s.x = x
             s.xn, s.rstd1 = ops.rmsnorm_fwd(x, lyr.input_layernorm.weight.data, d.rms_eps)
             if fused:
                 s.qkv = ops.gemm_rope(s.xn, self.wqkv[l], pos, self.cos, self.sin, 2 * d.hidden)   # RoPE in the epilogue
             else:
-                s.qkv = ops.gemm(s.xn, self.wqkv[l])
+                s.qkv = self._linear(s.xn, self.wqkv[l], w8[0])
                 ops.rope_(s.qkv, pos, self.cos, self.sin, 2 * H, d.head_dim)
             if kv_sink is not None:
                 kv_sink(l, s.qkv)                      # prefill of generate(): post-RoPE K,V go to the cache
@@ -423,14 +455,14 @@ class LlamaCore:
                 s.rows = out_rows
                 ao = s.ao_r = ops.gather_rows(s.ao, out_rows)
                 xin = ops.gather_rows(x, out_rows)
-            s.xm = ops.gemm(ao, self.wo[l], addend=xin)
+            s.xm = self._linear(ao, self.wo[l], w8[1], addend=xin)
             s.xn2, s.rstd2 = ops.rmsnorm_fwd(s.xm, lyr.post_attention_layernorm.weight.data, d.rms_eps)
             if fused and s.rows is None:
                 s.gu, s.h = ops.gemm_swiglu(s.xn2, self.wgu[l])                                    # SwiGLU in the epilogue
             else:
-                s.gu = ops.gemm(s.xn2, self.wgu[l])
+                s.gu = self._linear(s.xn2, self.wgu[l], w8[2])
                 s.h = ops.swiglu_fwd(s.gu)
-            x = ops.gemm(s.h, self.wd[l], addend=s.xm)
+            x = self._linear(s.h, self.wd[l], w8[3], addend=s.xm)
             if save:
                 saved.append(s)
         return x, ((saved, (pos, cu, list(seqlens))) if save else None)
@@ -450,6 +482,7 @@ class LlamaCore:
         B, T = len(q_lens), x.shape[0]
         last = d.n_layers - 1
         fused = self.fused_epilogues and T >= 1024 and d.inter % 128 == 0 and d.hidden % 256 == 0
+        f8 = self.fp8_for_inference()
         if self.LAYER_CALL and not fused and d.head_dim == 128:
             R = 0 if out_rows is None else out_rows.numel()
             run = ops.LayerRunner(T, D, d.inter, H, d.rms_eps, pos, self.cos, self.sin, cu, B, ops._qblocks(q_lens), R=R, device=x.device)
@@ -459,15 +492,17 @@ class LlamaCore:
                 pruned = out_rows is not None and l == last
                 y = torch.empty((R, D), dtype=bf16, device=x.device) if pruned else bufs[l & 1]
                 run.run(x, y, lyr.input_layernorm.weight.data, self.wqkv[l], self.wo[l], lyr.post_attention_layernorm.weight.data,
-                        self.wgu[l], self.wd[l], kc=kc[l], vc=vc[l], out_rows=out_rows if pruned else None)
+                        self.wgu[l], self.wd[l], kc=kc[l], vc=vc[l], out_rows=out_rows if pruned else None,
+                        fp8=self._fp8_layer(f8, l), fp8_max_rows=FP8_MAX_ROWS)
                 x = y
             return x
         for l, lyr in enumerate(self.model.layers):
+            w8 = self._fp8_layer(f8, l) or ((None, None),) * 4
             xn, _ = ops.rmsnorm_fwd(x, lyr.input_layernorm.weight.data, d.rms_eps)
             if fused:
                 qkv = ops.gemm_rope(xn, self.wqkv[l], pos, self.cos, self.sin, 2 * D)
             else:
-                qkv = ops.gemm(xn, self.wqkv[l])
+                qkv = self._linear(xn, self.wqkv[l], w8[0])
                 ops.rope_(qkv, pos, self.cos, self.sin, 2 * H, d.head_dim)
             ops.kv_store_suffix(qkv, cu, cached, kc[l], vc[l], B, T)
             ao = ops.attn_fwd_kv(qkv[:, :D], kc[l], vc[l], cu, q_lens, kv_start, kv_len, H)
@@ -475,13 +510,13 @@ class LlamaCore:
             if out_rows is not None and l == last:
                 ao = ops.gather_rows(ao, out_rows)
                 xin = ops.gather_rows(x, out_rows)
-            xm = ops.gemm(ao, self.wo[l], addend=xin)
+            xm = self._linear(ao, self.wo[l], w8[1], addend=xin)
             xn2, _ = ops.rmsnorm_fwd(xm, lyr.post_attention_layernorm.weight.data, d.rms_eps)
             if fused and xm.shape[0] >= 1024:
                 _, h = ops.gemm_swiglu(xn2, self.wgu[l], keep_gu=False)
             else:
-                h = ops.swiglu_fwd(ops.gemm(xn2, self.wgu[l]))
-            x = ops.gemm(h, self.wd[l], addend=xm)
+                h = ops.swiglu_fwd(self._linear(xn2, self.wgu[l], w8[2]))
+            x = self._linear(h, self.wd[l], w8[3], addend=xm)
         return x
 
     # -------------------------------------------------------------------------------------------------
@@ -593,14 +628,19 @@ class LlamaCore:
         # The step is HBM-bound weight streaming.  Batches <= 16 use the swap-AB cluster-split-K kernel with the SwiGLU fused
         # (gemm_skinny.cu); larger batches go through nv_gemm_bf16's auto dispatch, which picks the tile variant per (M, N)
         # from a measured table (32-column tiles for the 4096-wide projections, 256 for gate|up: tools/midm_bench.py).
-        # With an fp8 copy of the weights (set_fp8), the skinny GEMMs stream it instead: same bits as bf16 on W'.
+        # With an fp8 copy of the weights (set_fp8), the skinny GEMMs and, up to FP8_MAX_ROWS rows, nv_gemm_fp8w_bf16 stream
+        # it instead: same bits as bf16 on W'.  generate() refuses a stale copy before it gets here.
         bn = DECODE_BLOCK_N
         skinny = bn == 0 and x.shape[0] <= 16
         fuse_mlp = skinny and d.inter % 64 == 0
-        f8 = self.fp8 if skinny else None
+        f8 = self.fp8 if bn == 0 and x.shape[0] <= FP8_MAX_ROWS else None
         if f8 is not None:
-            lin = lambda a, w, addend=None: ops.gemm_skinny_fp8(a, *w, addend=addend)
-            wqkv, wo, wgu, wd = f8.wqkv, f8.wo, f8.wgu, f8.wd
+            if skinny:
+                lin = lambda a, w, addend=None: ops.gemm_skinny_fp8(a, *w, addend=addend)
+            else:
+                lin = lambda a, w, addend=None: ops.gemm_fp8w(a, *w, addend=addend) if w[0] is not None else ops.gemm(a, w[1], addend=addend)
+            wqkv, wo, wd = f8.wqkv, f8.wo, f8.wd
+            wgu = f8.wgu if skinny else [(None, w) for w in self.wgu]        # gate|up: bf16 above 16 rows (FP8_MAX_ROWS)
         else:
             wqkv, wo, wgu, wd = self.wqkv, self.wo, self.wgu, self.wd
             if skinny:

@@ -502,10 +502,13 @@ class ModifiedLlamaForCausalLM(nn.Module):
         """Round every LM linear weight IN PLACE to W' = e4m3(W / 2^e_n) * 2^e_n (one power-of-two exponent per output row,
         include/navillm_b200.h) and keep an fp8 copy of them (about 6.6 GB at Vicuna-7B).  W' is exact in bf16, so the
         model afterwards IS the model with weights W': prefill, navigation, training and ``state_dict()`` all see W'.
-        ``generate`` then streams the fp8 copy in every decode-step GEMM of batches <= 16 (half the bytes; the same bits as
-        the bf16 kernels on W') and keeps the bf16 path on W' above that.  Irreversible: reload the checkpoint to get W
-        back.  Any later write to the weights (an optimizer step, ``load_state_dict``) makes ``generate`` raise until this
-        is called again (or ``drop_fp8_weights``).  Returns the size of the copy in bytes."""
+        The inference GEMMs then stream the fp8 copy (half the bytes; the same bits as the bf16 kernels on W'): every
+        decode-step GEMM of ``generate`` and its lm_head at batches up to ``llama.FP8_MAX_ROWS``, and the GEMMs of at most
+        that many rows in no-grad forwards (navigation and grounding steps, prefix-cached suffixes, prefills, the pruned
+        last layer).  Training forwards and the LM-loss lm_head keep the bf16 weights.  Irreversible: reload the checkpoint
+        to get W back.  Any later write to the weights (an optimizer step, ``load_state_dict``) makes ``generate`` raise
+        until this is called again (or ``drop_fp8_weights``); the no-grad forwards then run bf16 on the current weights.
+        Returns the size of the copy in bytes."""
         self._ensure()
         self.drop_fp8_weights()
         self._fp8 = Fp8Weights(self.flat, self.fp8_linear_weights())
@@ -620,6 +623,8 @@ class ModifiedLlamaForCausalLM(nn.Module):
             hn, _ = ops.rmsnorm_fwd(h_rows, self.model.norm.weight.data, d.rms_eps)
             if B <= 16 and llama_mod.DECODE_BLOCK_N == 0 and fp8_head is not None:
                 ops.gemm_skinny_fp8(hn, *fp8_head, out=logits)
+            elif B <= llama_mod.FP8_MAX_ROWS and llama_mod.DECODE_BLOCK_N == 0 and fp8_head is not None:
+                ops.gemm_fp8w(hn, *fp8_head, out=logits)
             elif B <= 16 and llama_mod.DECODE_BLOCK_N == 0:
                 ops.gemm_skinny(hn, self.lm_head.weight.data, out=logits)
             else:

@@ -244,7 +244,7 @@ class NavModel(nn.Module):
             f.reattach_grads()
 
     def quantize_weights_fp8(self) -> int:
-        """Opt-in fp8 (e4m3) weight streaming for text generation: ``ModifiedLlamaForCausalLM.quantize_weights_fp8`` on the
+        """Opt-in fp8 (e4m3) weight streaming for inference: ``ModifiedLlamaForCausalLM.quantize_weights_fp8`` on the
         language model.  Rounds its linear weights (and lm_head) in place; the embeddings, norms, ``out_head`` / ``og_head``
         and the fp32 panorama encoder are not touched.  Returns the size of the fp8 copy in bytes."""
         self._ensure()

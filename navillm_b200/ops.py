@@ -592,8 +592,14 @@ class LayerRunner:
         a.kv_len = kv_len.data_ptr() if kv_len is not None else None
         self._keep += (cached, kv_start, kv_len)
 
-    def run(self, x, y, ln1, wqkv, wo, ln2, wgu, wd, *, kc=None, vc=None, out_rows=None):
+    def run(self, x, y, ln1, wqkv, wo, ln2, wgu, wd, *, kc=None, vc=None, out_rows=None, fp8=None, fp8_max_rows=0):
+        """``fp8``: None, or the (e4m3, exponents) pairs of wqkv, wo, wgu, wd (``Fp8Weights.view``); each GEMM with at most
+        ``fp8_max_rows`` rows then streams its pair through nv_gemm_fp8w_bf16 (same bits as the bf16 weights W')."""
         a = self.args
+        pairs = fp8 if fp8 is not None else ((None, None),) * 4
+        (a.wqkv_q, a.wqkv_e), (a.wo_q, a.wo_e), (a.wgu_q, a.wgu_e), (a.wd_q, a.wd_e) = \
+            [(q.data_ptr(), e.data_ptr()) if q is not None else (None, None) for q, e in pairs]
+        a.fp8_max_rows = fp8_max_rows if fp8 is not None else 0
         a.x, a.y = x.data_ptr(), y.data_ptr()
         a.ln1, a.wqkv, a.wo, a.ln2, a.wgu, a.wd = ln1.data_ptr(), wqkv.data_ptr(), wo.data_ptr(), ln2.data_ptr(), wgu.data_ptr(), wd.data_ptr()
         a.kcache = kc.data_ptr() if kc is not None else None
@@ -739,6 +745,30 @@ def gemm_skinny_swiglu_fp8(x: torch.Tensor, wgu_q: torch.Tensor, exps: torch.Ten
     check(_lib.load().nv_gemm_skinny_swiglu_fp8(ptr(x), i64(x.stride(0)), ptr(wgu_q), i64(wgu_q.stride(0)), ptr(exps), ptr(out),
                                                 i64(out.stride(0)), i32(M), i32(F), i32(K), stream_ptr()),
           "nv_gemm_skinny_swiglu_fp8")
+    return out
+
+
+def gemm_fp8w(a: torch.Tensor, q: torch.Tensor, e: torch.Tensor, *, addend: torch.Tensor | None = None,
+              out: torch.Tensor | None = None, block_n: int = 0) -> torch.Tensor:
+    """``gemm(a, W', addend=addend, block_n=block_n)`` with the weight in the fp8 format of ``quantize_fp8_`` (q e4m3 [N, K],
+    e int8 [N]; W' = q * 2^e): bit for bit the same result at any M while reading half the weight bytes (csrc/gemm_bf16.cu).
+    block_n: 0 (auto), 32 or 128."""
+    _rowmajor(a, "a"); _fp8_weight(q, e, "q")
+    assert a.dtype == bf16
+    M, K = a.shape
+    N = q.shape[0]
+    if q.shape[1] != K:
+        raise ValueError(f"gemm_fp8w: contraction mismatch a {tuple(a.shape)} q {tuple(q.shape)}")
+    if out is None:
+        out = torch.empty((M, N), dtype=bf16, device=a.device)
+    _rowmajor(out, "out")
+    assert out.shape == (M, N) and out.dtype == bf16
+    if addend is not None:
+        _rowmajor(addend, "addend")
+        assert addend.shape == (M, N) and addend.dtype == bf16
+    check(_lib.load().nv_gemm_fp8w_bf16(ptr(a), i64(a.stride(0)), ptr(q), i64(q.stride(0)), ptr(e), ptr(out), i64(out.stride(0)),
+                                        ptr(addend), i64(addend.stride(0) if addend is not None else 0), i32(M), i32(N), i32(K),
+                                        i32(block_n), stream_ptr()), "nv_gemm_fp8w_bf16")
     return out
 
 

@@ -11,6 +11,7 @@
 (v)   the GPU name and power limit, read in the same run.
 """
 import argparse
+import gc
 import json
 import sys
 from pathlib import Path
@@ -79,9 +80,9 @@ def gemm_table(dev, iters):
     return rows
 
 
-def c3_generate(dev, layers, gens):
+def c3_generate(dev, layers, gens, batch=None):
     wl = bench.WORKLOADS["c3"]
-    B, NV, NT, NEW = wl["B"], wl["n_cand_tok"], wl["n_text"], wl["n_new"]
+    B, NV, NT, NEW = batch or wl["B"], wl["n_cand_tok"], wl["n_text"], wl["n_new"]
     if layers != bench.N_LAYERS:
         import navillm_b200.nav_model as nm
         nm.VICUNA_7B["num_hidden_layers"] = layers
@@ -127,6 +128,7 @@ def main():
     ap.add_argument("--iters", type=int, default=50)
     ap.add_argument("--gens", type=int, default=3)
     ap.add_argument("--skip-gemm", action="store_true")
+    ap.add_argument("--batch", type=int, nargs="*", default=[], help="decode batch sizes of the generate comparison (default: C3's)")
     ap.add_argument("--out", default=None, help="also write the result as JSON here")
     a = ap.parse_args()
     if not torch.cuda.is_available():
@@ -135,8 +137,12 @@ def main():
     res = {"gpu": bench.gpu_info(0)}
     print(json.dumps(res["gpu"]), flush=True)
     res["gemm"] = [] if a.skip_gemm else gemm_table(dev, a.iters)
-    res["c3_generate"] = c3_generate(dev, a.layers, a.gens)
-    print(json.dumps(res["c3_generate"]), flush=True)
+    res["c3_generate"] = []
+    for b in a.batch or [None]:
+        res["c3_generate"].append(c3_generate(dev, a.layers, a.gens, b))
+        print(json.dumps(res["c3_generate"][-1]), flush=True)
+        gc.collect()                                                          # one 7B model (+ copy, + KV caches) at a time
+        torch.cuda.empty_cache()
     if a.out:
         Path(a.out).parent.mkdir(parents=True, exist_ok=True)
         Path(a.out).write_text(json.dumps(res, indent=1))

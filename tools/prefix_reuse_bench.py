@@ -53,10 +53,14 @@ def main():
     ap.add_argument("--steps", type=int, default=16)
     ap.add_argument("--hist0", type=int, default=0, help="history length at the first step (C5: 40 with --steps 1..)")
     ap.add_argument("--json", type=str, default="")
+    ap.add_argument("--fp8", action="store_true", help="quantize the weights and time the prefix-cached rollout with the fp8 copy "
+                                                       "against bf16 on the same weights (bitwise-equal fuse_logits required)")
     a = ap.parse_args()
     from navillm_b200.modified_lm import PrefixKVCache
     dev = torch.device("cuda:0")
     model = bench.build_model(dev).eval()
+    if a.fp8:
+        return fp8_rollout(model, a, dev)
     rng = np.random.RandomState(0)
     g = torch.Generator().manual_seed(0)
     B, D, G, n_cand = a.batch, 4096, 64, 12
@@ -99,6 +103,55 @@ def main():
     print(json.dumps(out), flush=True)
     if a.json:
         Path(a.json).write_text(json.dumps({"summary": out, "steps": rows}, indent=1))
+
+
+def fp8_rollout(model, a, dev):
+    """The same rollout twice in lock-step, each with its own prefix cache: with the fp8 copy of the weights and with bf16 on
+    the same (quantized) weights, alternating per step."""
+    from navillm_b200.modified_lm import PrefixKVCache
+    lm = model.lang_model
+    model.quantize_weights_fp8()
+    copy = lm.fp8_weights
+    rng = np.random.RandomState(0)
+    g = torch.Generator().manual_seed(0)
+    B, D, G, n_cand = a.batch, 4096, 64, 12
+    words = [f"w{i}" for i in range(5000)]
+    instr = [" ".join(words[i] for i in rng.randint(0, 5000, size=rng.randint(60, 100))) for _ in range(B)]
+    hist = [[torch.randn(D, generator=g).to(dev) for _ in range(a.hist0)] for _ in range(B)]
+    caches = {"fp8": PrefixKVCache(lm, batch_size=B, max_len=2048), "bf16": PrefixKVCache(lm, batch_size=B, max_len=2048)}
+    to_dev = lambda b: {k: (v.to(dev) if torch.is_tensor(v) else v) for k, v in b.items()}
+    ev = lambda: torch.cuda.Event(enable_timing=True)
+    rows, equal = [], True
+    with torch.no_grad():
+        for t in range(a.hist0, a.hist0 + a.steps):
+            batch = to_dev(make_step(rng, g, B, t, instr, n_cand, D, G))
+            batch["hist_vis"] = [list(h) for h in hist]
+            out, ms, enc = {}, {}, 0
+            for mode in (("fp8", "bf16") if t % 2 == 0 else ("bf16", "fp8")):
+                lm.core.set_fp8(copy if mode == "fp8" else None)
+                e0, e1 = ev(), ev()
+                enc0 = caches[mode].stats["tokens_encoded"]
+                torch.manual_seed(t); e0.record()
+                out[mode] = model("navigation", dict(batch), prefix_cache=caches[mode])
+                e1.record(); torch.cuda.synchronize()
+                ms[mode], enc = e0.elapsed_time(e1), caches[mode].stats["tokens_encoded"] - enc0
+            equal &= torch.equal(out["fp8"]["fuse_logits"], out["bf16"]["fuse_logits"])
+            rows.append({"hist": t, "encoded_tokens": enc, "bf16_ms": ms["bf16"], "fp8_ms": ms["fp8"]})
+            for b in range(B):
+                hist[b].append(out["bf16"]["fuse_embeds"][b, 1 + (t % 3)].float())
+    timed = rows[1:] or rows                                   # the first step encodes whole prompts (and warms up)
+    n = len(timed)
+    res = {"config": f"eval rollout with PrefixKVCache, B={B}, hist {a.hist0}..{a.hist0 + a.steps - 1}, 12 candidates, "
+                     f"Vicuna-7B random init, quantized, no_grad", "gpu": bench.gpu_info(0),
+           "encoded_tokens_per_step": sum(r["encoded_tokens"] for r in timed) / n,
+           "bf16_ms_per_step": sum(r["bf16_ms"] for r in timed) / n, "fp8_ms_per_step": sum(r["fp8_ms"] for r in timed) / n,
+           "fuse_logits_bitwise_equal": bool(equal)}
+    res["speedup"] = res["bf16_ms_per_step"] / res["fp8_ms_per_step"]
+    print(json.dumps(res), flush=True)
+    if a.json:
+        Path(a.json).write_text(json.dumps({"summary": res, "steps": rows}, indent=1))
+    if not equal:
+        raise SystemExit("prefix_reuse_bench --fp8: fuse_logits differ between the fp8 copy and bf16")
 
 
 if __name__ == "__main__":
