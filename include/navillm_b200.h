@@ -206,6 +206,7 @@ int nv_decode_attn(const void* q, int64_t ldq, const void* kcache, const void* v
 /* nv_decode_rope_kv + nv_decode_attn in one launch (qkv pre-RoPE, not modified; k / v appended at row lens[b]). */
 int nv_decode_attn_rope(const void* qkv, int64_t ld, const int* lens, const void* cos_t, const void* sin_t, void* kcache,
                         void* vcache, void* out, int64_t ldo, int B, int Smax, int H, int head_dim, float scale, void* stream);
+/* at most 64 special ids (n_special), here and in nv_sample_topk; longer lists return NV_ERR_BAD_ARG */
 int nv_argmax_masked(const void* logits, int64_t ld, int V, const int* special, int n_special, int* finished, int eos_id,
                      int pad_id, int stop_on_eos, int* next, int B, void* stream);
 int nv_add_int(int* x, int n, int delta, void* stream);

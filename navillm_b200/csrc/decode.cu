@@ -267,6 +267,10 @@ __global__ void __launch_bounds__(DA_WARPS * 32) decode_attn_kernel(const __nv_b
   }
 }
 
+// Special ids masked by argmax_kernel and sample_topk_kernel: they are staged in shared memory, so the host entry points
+// reject longer lists.
+constexpr int MAX_SPECIAL = 64;
+
 // next[b] = finished[b] ? pad_id : argmax_c logits[b,c] over non-special columns (first index wins ties, like
 // torch.argmax); finished[b] |= next == eos (when stop_on_eos).  One CTA per row.
 __global__ void __launch_bounds__(1024) argmax_kernel(const __nv_bfloat16* __restrict__ logits, int64_t ld, int V,
@@ -275,11 +279,11 @@ __global__ void __launch_bounds__(1024) argmax_kernel(const __nv_bfloat16* __res
                                                       int* __restrict__ next) {
   __shared__ float sv[32];
   __shared__ int si[32];
-  __shared__ int s_special[64];
+  __shared__ int s_special[MAX_SPECIAL];
   griddep_launch();
   griddep_wait();
   const int b = blockIdx.x;
-  const int ns = min(n_special, 64);
+  const int ns = n_special;
   if (threadIdx.x < ns) s_special[threadIdx.x] = special[threadIdx.x];
   __syncthreads();
   float best = -INFINITY;
@@ -383,10 +387,10 @@ __global__ void __launch_bounds__(SMP_THREADS) sample_topk_kernel(const __nv_bfl
   extern __shared__ float sc[];                              // [V] scores, then probabilities
   __shared__ int hist[256];
   __shared__ float red[32];
-  __shared__ int s_special[64];
+  __shared__ int s_special[MAX_SPECIAL];
   __shared__ int s_idx, s_last;
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-  const int ns = min(n_special, 64);
+  const int ns = n_special;
   if (tid < ns) s_special[tid] = special[tid];
   if (tid < 256) hist[tid] = 0;
   if (tid == 0) { s_idx = V; s_last = -1; }
@@ -569,6 +573,8 @@ int nv_decode_attn_rope(const void* qkv, int64_t ld, const int* lens, const void
 
 int nv_argmax_masked(const void* logits, int64_t ld, int V, const int* special, int n_special, int* finished, int eos_id,
                      int pad_id, int stop_on_eos, int* next, int B, void* stream) {
+  NV_REQUIRE(n_special >= 0 && n_special <= MAX_SPECIAL, "nv_argmax_masked: n_special=%d out of range (max %d)", n_special,
+             MAX_SPECIAL);
   if (B == 0) return NV_OK;
   NV_CUDA(launch_pdl(argmax_kernel, dim3(B), dim3(1024), 0, S_(stream), CBF(logits), ld, V, special, n_special, finished, eos_id, pad_id,
                      stop_on_eos, next));
@@ -580,6 +586,8 @@ int nv_argmax_masked(const void* logits, int64_t ld, int V, const int* special, 
 int nv_sample_topk(const void* logits, int64_t ld, int V, const int* special, int n_special, int* finished, int eos_id, int pad_id,
                    int stop_on_eos, float temperature, int top_k, const float* u, int* next, float* probs_out, int B, void* stream) {
   NV_REQUIRE(logits && u && next && finished && V > 0 && temperature > 0.f, "nv_sample_topk: bad arguments (temperature must be > 0)");
+  NV_REQUIRE(n_special >= 0 && n_special <= MAX_SPECIAL, "nv_sample_topk: n_special=%d out of range (max %d)", n_special,
+             MAX_SPECIAL);
   NV_REQUIRE((int64_t)V * 4 <= 200 * 1024, "nv_sample_topk: vocabulary of %d does not fit the shared-memory score row", V);
   if (B == 0) return NV_OK;
   static bool attr_set = false;
