@@ -37,7 +37,7 @@ const char* nv_last_error(void);
 int nv_abi_version(void);
 /* Programmatic dependent launch for the decode chain (generate(): HF GenerationMixin greedy loop reached from
  * models/nav_model.py:324-338,388-399): when on, nv_embed_fwd / nv_rmsnorm_fwd / nv_gemm_skinny[_swiglu]_bf16 /
- * nv_decode_rope_kv / nv_decode_attn / nv_add_int / nv_argmax_masked are launched with
+ * nv_decode_rope_kv / nv_decode_attn / nv_add_int / nv_argmax_masked / nv_trie_mask are launched with
  * cudaLaunchAttributeProgrammaticStreamSerialization so a kernel's prologue (and the skinny GEMM's first weight tiles)
  * overlaps the tail of its predecessor.  Returns the previous setting.  Process-wide; default off. */
 int nv_set_pdl(int on);
@@ -216,6 +216,19 @@ int nv_add_int(int* x, int n, int delta, void* stream);
  * finished / eos / pad handling as nv_argmax_masked.  probs_out: optional fp32 [B, V] copy of the distribution drawn from. */
 int nv_sample_topk(const void* logits, int64_t ld, int V, const int* special, int n_special, int* finished, int eos_id, int pad_id,
                    int stop_on_eos, float temperature, int top_k, const float* u, int* next, float* probs_out, int B, void* stream);
+/* Trie-constrained decoding (TrieLogitsProcessor, models/modified_lm.py:10-30, reached from EQA validation,
+ * tasks/agents/mp3d_agent.py:545-584), on the device.  The trie is flattened to CSR: node_ptr [n_nodes + 2], child_tok [E]
+ * (ascending within a node, every id in [0, V)), child_node [E]; node 0 is the root, node n_nodes an extra childless dead node.
+ * One CTA per row b: when last != NULL, state[b] advances by last[b] like tools/trie.py's get_next_node (a node without
+ * children stays; a token that is not a child sets *miss = 1 and moves to the dead node).  Then out[b, 0:V) = -inf except
+ * the allowed tokens - the node's children, or leaf_tok (the trie's eos) at a node without any - which carry their logit.
+ * A row whose allowed non-special values are all -inf, or with an allowed NaN, sets *miss = 1 and gets 0.0 at its first
+ * allowed non-special token (or its first non-special column), so a pick from out stays inside [0, V).  *miss is never
+ * cleared here.  nv_argmax_masked / nv_sample_topk then pick from out.  ldo % 8 == 0, out 16-byte aligned,
+ * n_special <= 64; launched with PDL like the rest of the decode chain. */
+int nv_trie_mask(const void* logits, int64_t ld, void* out, int64_t ldo, int V, const int* node_ptr, const int* child_tok,
+                 const int* child_node, int n_nodes, int leaf_tok, const int* special, int n_special, int* state, const int* last,
+                 int* miss, int B, void* stream);
 
 /* ---- fused clip + AdamW over flat buffers (csrc/optim.cu) ------------------------------------------------------
  * torch.nn.utils.clip_grad_norm_(model.parameters(), 40.) + torch.optim.AdamW.step() of the reference

@@ -337,6 +337,92 @@ __global__ void __launch_bounds__(1024) argmax_kernel(const __nv_bfloat16* __res
   }
 }
 
+// ---- trie-constrained decoding (TrieLogitsProcessor, models/modified_lm.py:10-30; caller tasks/agents/mp3d_agent.py:545-584)
+// The trie is in CSR form: the children of node n are edges node_ptr[n] .. node_ptr[n+1], with child_tok ascending and
+// child_node the node each edge leads to; node 0 is the root and node n_nodes an extra childless "dead" node.  One CTA per
+// row: (1) advance state[b] by last[b] with the semantics of tools/trie.py (a node without children stays; otherwise move to
+// the child, and a token that is not a child sets *miss and moves to the dead node); (2) out[b, :] = -inf except the allowed
+// tokens (the node's children, or leaf_tok when it has none), which carry their logit; (3) a row whose allowed non-special
+// values are all -inf, or with an allowed NaN, sets *miss and gets 0.0 at its first allowed non-special token (else at its
+// first non-special column), so the argmax / draw that follows stays inside [0, V).
+constexpr int TM_THREADS = 512;
+
+__device__ __forceinline__ bool tm_is_special(const int* s_special, int ns, int c) {
+  bool sp = false;
+  for (int s = 0; s < ns; ++s) sp |= (s_special[s] == c);
+  return sp;
+}
+
+__global__ void __launch_bounds__(TM_THREADS) trie_mask_kernel(const __nv_bfloat16* __restrict__ logits, int64_t ld,
+                                                               __nv_bfloat16* __restrict__ out, int64_t ldo, int V,
+                                                               const int* __restrict__ node_ptr, const int* __restrict__ child_tok,
+                                                               const int* __restrict__ child_node, int n_nodes, int leaf_tok,
+                                                               const int* __restrict__ special, int n_special,
+                                                               int* __restrict__ state, const int* __restrict__ last,
+                                                               int* __restrict__ miss) {
+  __shared__ int s_special[MAX_SPECIAL];
+  __shared__ int s_node;
+  griddep_launch();
+  griddep_wait();
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int ns = n_special;
+  if (tid < ns) s_special[tid] = special[tid];
+  if (tid == 0) {
+    int node = state[b];
+    const int e0 = node_ptr[node], e1 = node_ptr[node + 1];
+    if (last != nullptr && e1 > e0) {
+      const int tok = last[b];
+      int lo = e0, hi = e1;                                   // first edge with child_tok >= tok
+      while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (child_tok[mid] < tok) lo = mid + 1;
+        else hi = mid;
+      }
+      if (lo < e1 && child_tok[lo] == tok) {
+        node = child_node[lo];
+      } else {
+        node = n_nodes;
+        *miss = 1;
+      }
+      state[b] = node;
+    }
+    s_node = node;
+  }
+  __nv_bfloat16* orow = out + (int64_t)b * ldo;
+  const uint4 ninf = make_uint4(0xFF80FF80u, 0xFF80FF80u, 0xFF80FF80u, 0xFF80FF80u);   // bf16 -inf x 8
+  const int nvec = V >> 3;
+  for (int v = tid; v < nvec; v += TM_THREADS) reinterpret_cast<uint4*>(orow)[v] = ninf;
+  for (int c = nvec * 8 + tid; c < V; c += TM_THREADS) orow[c] = __ushort_as_bfloat16((unsigned short)0xFF80u);
+  __syncthreads();
+  const int node = s_node;
+  const int e0 = node_ptr[node], e1 = node_ptr[node + 1];
+  const bool leaf = e1 == e0;
+  const int n_allowed = leaf ? 1 : e1 - e0;
+  const __nv_bfloat16* lrow = logits + (int64_t)b * ld;
+  int live = 0, nan = 0;
+  for (int i = tid; i < n_allowed; i += TM_THREADS) {       // fan-outs of any size: looped, not capped
+    const int c = leaf ? leaf_tok : child_tok[e0 + i];
+    const __nv_bfloat16 x = lrow[c];
+    orow[c] = x;
+    const float f = __bfloat162float(x);
+    nan |= (f != f);
+    live |= (f > -INFINITY && !tm_is_special(s_special, ns, c));
+  }
+  const int any_nan = __syncthreads_or(nan), any_live = __syncthreads_or(live);
+  if (tid == 0 && (any_nan || !any_live)) {
+    *miss = 1;
+    int c = -1;
+    for (int i = 0; i < n_allowed && c < 0; ++i) {           // children are distinct: at most ns + 1 iterations
+      const int t = leaf ? leaf_tok : child_tok[e0 + i];
+      if (!tm_is_special(s_special, ns, t)) c = t;
+    }
+    if (c < 0)
+      for (c = 0; c < V && tm_is_special(s_special, ns, c); ++c) {
+      }
+    if (c < V) orow[c] = __float2bfloat16_rn(0.f);
+  }
+}
+
 __global__ void add_int_kernel(int* __restrict__ x, int n, int delta) {
   griddep_launch();
   griddep_wait();
@@ -598,6 +684,24 @@ int nv_sample_topk(const void* logits, int64_t ld, int V, const int* special, in
   sample_topk_kernel<<<B, SMP_THREADS, (size_t)V * 4, S_(stream)>>>(CBF(logits), ld, V, special, n_special, finished, eos_id, pad_id,
                                                                      stop_on_eos, temperature, top_k, u, next, probs_out);
   NV_LAUNCH_CHECK();
+  return NV_OK;
+}
+
+// Trie mask of the next-token logits (see trie_mask_kernel).  logits [B, V] bf16 (ld), out [B, V] bf16 (ldo % 8 == 0, 16-byte
+// aligned base), state int32 [B] node per row, last int32 [B] or null (no advance), miss int32 [1] (set, never cleared).
+int nv_trie_mask(const void* logits, int64_t ld, void* out, int64_t ldo, int V, const int* node_ptr, const int* child_tok,
+                 const int* child_node, int n_nodes, int leaf_tok, const int* special, int n_special, int* state, const int* last,
+                 int* miss, int B, void* stream) {
+  NV_REQUIRE(logits && out && node_ptr && child_tok && child_node && state && miss && B >= 0, "nv_trie_mask: null argument");
+  NV_REQUIRE(V > 0 && n_nodes >= 1 && ld >= V && ldo >= V && (ldo & 7) == 0 && ((uintptr_t)out & 15) == 0,
+             "nv_trie_mask: bad shape (V=%d, n_nodes=%d, ld=%lld, ldo=%lld; ldo %% 8 == 0 and a 16-byte aligned out needed)", V,
+             n_nodes, (long long)ld, (long long)ldo);
+  NV_REQUIRE(leaf_tok >= 0 && leaf_tok < V, "nv_trie_mask: leaf_tok=%d outside [0, %d)", leaf_tok, V);
+  NV_REQUIRE(n_special >= 0 && n_special <= MAX_SPECIAL && (n_special == 0 || special),
+             "nv_trie_mask: n_special=%d out of range (max %d)", n_special, MAX_SPECIAL);
+  if (B == 0) return NV_OK;
+  NV_CUDA(launch_pdl(trie_mask_kernel, dim3(B), dim3(TM_THREADS), 0, S_(stream), CBF(logits), ld, BF(out), ldo, V, node_ptr,
+                     child_tok, child_node, n_nodes, leaf_tok, special, n_special, state, last, miss));
   return NV_OK;
 }
 

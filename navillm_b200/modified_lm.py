@@ -16,6 +16,7 @@ from __future__ import annotations
 
 import collections
 import os
+import time
 from types import SimpleNamespace
 from typing import List, Optional
 
@@ -25,6 +26,7 @@ import torch.nn as nn
 
 from . import llama as llama_mod
 from . import ops
+from . import trie as trie_mod
 from .llama import FlatParams, Fp8Weights, LlamaCore, LlamaDims, LlamaModelParams, _Linear
 from .parallel import GradSync
 from .tokenizer import HFTokenizerAdapter, SyntheticTokenizer
@@ -544,9 +546,11 @@ class ModifiedLlamaForCausalLM(nn.Module):
 
     def _decode_state(self, B: int, Smax: int, key_extra: tuple, want_graph: bool):
         """Persistent per-shape decode state: the contiguous KV cache [B, Smax, D] per layer, the step's I/O buffers and --
-        once captured -- the CUDA graph of ONE greedy decode step.  Capturing and instantiating the ~260-node graph costs
-        more than the 127 replays of a C3 generation save, so it is done once per (batch, cache length, stop rule) and
-        reused by every later ``generate`` call (evaluation loops call generate with the same shapes over and over)."""
+        once captured -- the CUDA graph of ONE decode step.  Capturing and instantiating the ~260-node graph costs more than
+        the 127 replays of a C3 generation save, so it is done once per (batch, cache length, stop rule, decoding mode and
+        the scalars the step bakes in) and reused by every later ``generate`` call (evaluation loops call generate with the
+        same shapes over and over).  The trie-constrained modes keep their flattened trie in ``trie_buf`` (see
+        ``_load_trie``), sampled modes their uniform numbers in ``u``."""
         states = self.__dict__.setdefault("_decode_states", collections.OrderedDict())
         key = (B, Smax) + key_extra
         st = states.get(key) if want_graph else None
@@ -561,12 +565,29 @@ class ModifiedLlamaForCausalLM(nn.Module):
             logits=torch.empty((B, (V + 63) // 64 * 64), dtype=bf16, device=dev)[:, :V],
             next_ids=torch.empty((B,), dtype=torch.int32, device=dev),
             finished=torch.zeros((B,), dtype=torch.int32, device=dev),
-            lens=torch.zeros((B,), dtype=torch.int32, device=dev), graph=None)
+            lens=torch.zeros((B,), dtype=torch.int32, device=dev), graph=None,
+            u=None, masked=None, node=None, miss=None, trie_buf=None, trie_cap=(0, 0))
         if want_graph:
             states[key] = st
             while len(states) > self.max_decode_states:
                 states.popitem(last=False)
         return st
+
+    @staticmethod
+    def _load_trie(st, table) -> tuple:
+        """Copy a flattened trie into the state's persistent device buffers (a captured graph keeps their pointers) in one
+        host-to-device copy.  Capacities grow in powers of two; growing drops the state's graph.  Returns the kernel's
+        (node_ptr, child_tok, child_node, n_nodes) views."""
+        ncap, ecap = st.trie_cap
+        if table.n_nodes > ncap or table.n_edges > ecap:
+            pow2 = lambda n: 1 << max(0, int(n) - 1).bit_length()
+            ncap, ecap = max(ncap, pow2(table.n_nodes)), max(ecap, pow2(max(table.n_edges, 1)))
+            st.trie_buf = torch.empty(ncap + 2 + 2 * ecap, dtype=torch.int32, device=st.next_ids.device)
+            st.trie_cap = (ncap, ecap)
+            st.graph = None
+        st.trie_buf.copy_(torch.from_numpy(table.pack(ncap, ecap)))
+        o = ncap + 2
+        return st.trie_buf[:o], st.trie_buf[o:o + ecap], st.trie_buf[o + ecap:], ncap
 
     @torch.no_grad()
     def generate(self, input_ids, attention_mask, cand_vis=None, hist_vis=None, obj_vis=None, max_new_tokens: int = 20,
@@ -576,14 +597,23 @@ class ModifiedLlamaForCausalLM(nn.Module):
                  top_p: float = 1.0, **unused) -> torch.Tensor:
         """Prefill on the packed kernels (positions = cumsum(mask)-1 like HF generate; visual tokens injected only
         here, as in models/modified_lm.py:195-197), then one token per step over a pre-allocated KV cache.  The
-        greedy step has static shapes and is replayed as a CUDA graph (captured once per shape, see ``_decode_state``).
+        decode step of the greedy, sampled and trie-constrained modes has static shapes and is replayed as a CUDA graph
+        (captured once per shape and mode, see ``_decode_state``); generic ``logits_processor=`` calls run eagerly.
         Returns [B, S0 + n_new] int64 ids (prompt part copied from the input; finished rows continue with pad_token_id
         like HF greedy search).
 
         ``do_sample=True`` follows HF ``sample`` as the reference reaches it (tasks/agents/llava.py:58-62): logits
         processors, then temperature and top-k (``top_k=50`` is transformers' generation default, which the reference
         never overrides), bf16 softmax, one multinomial draw per row - all in ``nv_sample_topk``; the uniform numbers
-        come from ``torch.rand`` on the device, so ``torch.manual_seed`` makes a run reproducible."""
+        are one [B] draw per token from the default CUDA generator, so ``torch.manual_seed`` makes a run reproducible,
+        and the graph replays draw the same numbers as ``use_cuda_graph=False``.
+
+        ``trie=`` (TrieLogitsProcessor, models/modified_lm.py:10-30) walks the trie on the device (``nv_trie_mask``
+        between the lm_head and the pick) and replays as a CUDA graph too; the stop check stays per token, as on the host.
+        A trie ``navillm_b200.trie.flatten_trie`` cannot represent faithfully, ``trie=`` together with
+        ``logits_processor=``, and a call whose device walk reports a miss (a picked token outside the allowed set, which
+        only a degenerate row can produce) run the host ``TrieLogitsProcessor`` instead - the miss case reruns the whole
+        call, with the CUDA RNG state restored, and discards the device result."""
         if top_p is not None and top_p < 1.0:
             raise NotImplementedError("generate(top_p < 1) is not built: the reference never sets it (HF default 1.0)")
         if do_sample and not temperature > 0:
@@ -591,9 +621,39 @@ class ModifiedLlamaForCausalLM(nn.Module):
         self._ensure()
         self._check_fp8_fresh()
         dev = self._device()
-        core, d = self.core, self.dims
         eos = self.tokenizer.eos_token_id if eos_token_id is None else eos_token_id
         pad = self.tokenizer.unk_token_id if pad_token_id is None else pad_token_id
+        procs = list(logits_processor or [])
+        args = (input_ids, attention_mask, cand_vis, hist_vis, obj_vis, max_new_tokens, do_sample, temperature, eos, pad,
+                stop_on_eos, use_cuda_graph, stats, top_k)
+        table, path = None, None
+        if trie is not None and not procs:
+            t0 = time.perf_counter()
+            table = trie_mod.flatten_trie(trie, self.lm_head.weight.shape[0])
+            flatten_ms = 1e3 * (time.perf_counter() - t0)
+        if table is not None:
+            rng = torch.cuda.get_rng_state(dev) if do_sample else None
+            out = self._generate(*args, procs=[], table=table)
+            path = "device" if out is not None else "device_miss_host"
+            if out is None:
+                if rng is not None:
+                    torch.cuda.set_rng_state(rng, dev)
+                out = self._generate(*args, procs=[trie_mod.TrieLogitsProcessor(trie)], table=None)
+        else:
+            if trie is not None:
+                procs = [trie_mod.TrieLogitsProcessor(trie)] + procs
+                path = "host"
+            out = self._generate(*args, procs=procs, table=None)
+        if stats is not None and trie is not None:
+            stats.update({"trie_path": path, "trie_flatten_ms": flatten_ms if table is not None else None})
+        return out
+
+    def _generate(self, input_ids, attention_mask, cand_vis, hist_vis, obj_vis, max_new_tokens, do_sample, temperature, eos, pad,
+                  stop_on_eos, use_cuda_graph, stats, top_k, *, procs, table):
+        """``generate`` with the host processors ``procs`` (the host path when not empty) or the flattened trie ``table``
+        walked on the device; returns None when the device walk reported a miss."""
+        dev = self._device()
+        core, d = self.core, self.dims
         ev = None
         if stats is not None:                                     # bench.py: device-side phase times (forces one sync at the end)
             ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
@@ -601,12 +661,23 @@ class ModifiedLlamaForCausalLM(nn.Module):
         pp = PackedPrompt(input_ids, attention_mask, self, dev, generate_positions=True)
         vis = self.cat_vis(cand_vis, hist_vis, obj_vis, pp)
         B = pp.B
-        greedy = (not do_sample) and trie is None and not logits_processor
-        need_host = trie is not None or bool(logits_processor)    # processors walk the generated ids on the host
-        graphed = greedy and use_cuda_graph
+        need_host = bool(procs)                                   # processors walk the generated ids on the host
+        graphed = use_cuda_graph and not need_host
+        mode = ("trie+sample" if do_sample else "trie") if table is not None else ("sample" if do_sample else "greedy")
         Smax = (max(pp.seqlens) + max_new_tokens + 127) // 128 * 128          # bucketed: more reuse of the cached state
-        st = self._decode_state(B, Smax, (int(eos), int(pad), bool(stop_on_eos)), graphed)
+        key = (int(eos), int(pad), bool(stop_on_eos), mode, float(temperature) if do_sample else None,
+               int(top_k) if do_sample else None, table.eos if table is not None else None)
+        st = self._decode_state(B, Smax, key, graphed)
         kc, vc, logits, next_ids, finished, lens = st.kc, st.vc, st.logits, st.next_ids, st.finished, st.lens
+        if do_sample and not need_host and st.u is None:
+            st.u = torch.empty((B,), dtype=torch.float32, device=dev)
+        if table is not None:
+            if st.masked is None:
+                V = logits.shape[1]
+                st.masked = torch.empty((B, (V + 63) // 64 * 64), dtype=bf16, device=dev)[:, :V]
+                st.node = torch.zeros((B,), dtype=torch.int32, device=dev)
+                st.miss = torch.zeros((1,), dtype=torch.int32, device=dev)
+            trie_csr = self._load_trie(st, table)
         finished.zero_()
         lens.copy_(torch.tensor(pp.seqlens, dtype=torch.int32), non_blocking=True)
 
@@ -630,30 +701,11 @@ class ModifiedLlamaForCausalLM(nn.Module):
             else:
                 ops.gemm(hn, self.lm_head.weight.data, out=logits, block_n=llama_mod.DECODE_BLOCK_N)
 
-        trie_state = [None]
-
-        def pick(all_ids_host):
-            """next token from `logits` -> next_ids (device)."""
-            if greedy:
-                ops.argmax_masked(logits, special, finished, eos, pad, stop_on_eos, next_ids)
-                return
-            if not need_host:                                     # plain sampling: straight from the bf16 logits
-                ops.sample_topk(logits, special, finished, eos, pad, stop_on_eos, temperature, top_k,
-                                torch.rand(B, device=dev, dtype=torch.float32), next_ids)
-                return
+        def pick_host(all_ids_host):
+            """next token from `logits` -> next_ids (device), through the host processors."""
             lg = logits.float()
             lg[:, self.special_token_ids] = float("-inf")
-            if trie is not None:                                  # TrieLogitsProcessor (models/modified_lm.py:10-30)
-                if trie_state[0] is None:
-                    trie_state[0] = [trie.root for _ in range(B)]
-                else:
-                    for bn in range(B):
-                        trie_state[0][bn] = trie.get_next_node(trie_state[0][bn], int(all_ids_host[bn][-1]))
-                allow = torch.zeros_like(lg, dtype=torch.bool)
-                for bn in range(B):
-                    allow[bn, trie.get_child_index(trie_state[0][bn])] = True
-                lg = lg.masked_fill(~allow, float("-inf"))
-            for proc in (logits_processor or []):
+            for proc in procs:
                 lg = proc(torch.tensor(all_ids_host, device=dev), lg)
             if do_sample:
                 ops.sample_topk(lg.to(torch.bfloat16), special, finished, eos, pad, stop_on_eos, temperature, top_k,
@@ -666,9 +718,28 @@ class ModifiedLlamaForCausalLM(nn.Module):
                 finished.copy_((fin | (nxt == eos)).to(torch.int32))
             next_ids.copy_(nxt.to(torch.int32))
 
+        def pick(advance):
+            """next token from `logits` -> next_ids (device) without host work; with a trie, the row's node first advances by
+            the token in next_ids (``advance``) and the pick reads the trie-masked copy of the logits."""
+            src = logits
+            if table is not None:
+                ops.trie_mask(logits, st.masked, *trie_csr, table.eos, special, st.node, next_ids if advance else None, st.miss)
+                src = st.masked
+            if do_sample:
+                st.u.uniform_()                                   # = torch.rand(B): the same numbers, into a static buffer
+                ops.sample_topk(src, special, finished, eos, pad, stop_on_eos, temperature, top_k, st.u, next_ids)
+            else:
+                ops.argmax_masked(src, special, finished, eos, pad, stop_on_eos, next_ids)
+
         head(hid_last)
         host_ids = [row.tolist() for row in input_ids.cpu()] if need_host else None
-        pick(host_ids)
+        if need_host:
+            pick_host(host_ids)
+        else:
+            if table is not None:                                 # every row starts at the root, in stream order
+                st.node.zero_()
+                st.miss.zero_()
+            pick(advance=False)
         out_tokens = [next_ids.clone()]
         if ev is not None:
             ev[1].record()
@@ -679,13 +750,14 @@ class ModifiedLlamaForCausalLM(nn.Module):
                 h = core.decode_step(xt, lens, kc, vc)
                 head(h)
                 ops.add_int_(lens, 1)
-                if greedy:
-                    ops.argmax_masked(logits, special, finished, eos, pad, stop_on_eos, next_ids)
+                if not need_host:
+                    pick(advance=True)
 
         # HF stops when every sequence has finished.  Asking the device after EVERY token would serialise host and device
-        # (one blocking read per token); finished rows only emit pad tokens, so the greedy loop looks every `check_every`
-        # tokens and the surplus pad columns are trimmed below -- same ids as a per-token check.
-        check_every = 1 if need_host else 8
+        # (one blocking read per token); finished rows only emit pad tokens, so the greedy and sampled loops look every
+        # `check_every` tokens and the surplus pad columns are trimmed below -- same ids as a per-token check.  Trie-constrained
+        # answers are a handful of tokens: there the check stays per token, as on the host path.
+        check_every = 1 if need_host or table is not None else 8
         replays = 0
         for it in range(1, max_new_tokens):
             if stop_on_eos and it % check_every == 0 and bool(finished.all()):
@@ -707,17 +779,24 @@ class ModifiedLlamaForCausalLM(nn.Module):
                 replays += 1
             else:
                 step()
-                if not greedy:
-                    pick(host_ids)
+                if need_host:
+                    pick_host(host_ids)
             out_tokens.append(next_ids.clone())
+        miss = False
+        if table is not None:
+            # one more advance, outside the graph: a token picked at the last step that is not a child is a miss as well
+            ops.trie_mask(logits, st.masked, *trie_csr, table.eos, special, st.node, next_ids, st.miss)
+            miss = bool(st.miss.item())
         if ev is not None:
             ev[2].record()
             torch.cuda.synchronize()
             n_dec = len(out_tokens) - 1
             stats.update({"prefill_ms": ev[0].elapsed_time(ev[1]), "decode_ms": ev[1].elapsed_time(ev[2]) if n_dec else None,
                           "decode_steps": n_dec, "graph_replays": replays, "kv_rows": Smax, "prompt_lens": list(pp.seqlens)})
+        if miss:
+            return None
         new = torch.stack(out_tokens, dim=1).to(torch.int64)
-        if stop_on_eos and not need_host and new.shape[1] > 1:
+        if stop_on_eos and check_every > 1 and new.shape[1] > 1:
             # trim the columns generated after the step at which the last row emitted EOS (see check_every above)
             is_eos = (new == eos)
             if bool(is_eos.any(dim=1).all()):

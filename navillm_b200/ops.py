@@ -564,6 +564,20 @@ def sample_topk(logits, special, finished, eos_id, pad_id, stop_on_eos, temperat
     return next_ids
 
 
+def trie_mask(logits, out, node_ptr, child_tok, child_node, n_nodes, leaf_tok, special, state, last, miss):
+    """out = logits masked to the tokens the trie allows per row (nv_trie_mask); advances ``state`` by ``last`` first
+    unless ``last`` is None.  logits / out [B, V] bf16, state / last int32 [B], miss int32 [1] (set on a miss, never
+    cleared); node_ptr / child_tok / child_node: the CSR trie with n_nodes real nodes plus the dead node n_nodes."""
+    B, V = logits.shape
+    assert out.shape == (B, V) and out.dtype == bf16 and logits.dtype == bf16 and logits.stride(1) == 1 and out.stride(1) == 1
+    assert state.dtype == torch.int32 and miss.dtype == torch.int32 and (last is None or last.dtype == torch.int32)
+    check(_lib.load().nv_trie_mask(ptr(logits), i64(logits.stride(0)), ptr(out), i64(out.stride(0)), i32(V), ptr(node_ptr),
+                                   ptr(child_tok), ptr(child_node), i32(n_nodes), i32(leaf_tok), ptr(special),
+                                   i32(0 if special is None else special.numel()), ptr(state), ptr(last), ptr(miss), i32(B),
+                                   stream_ptr()), "nv_trie_mask")
+    return out
+
+
 class LayerRunner:
     """Inference forward of decoder layers through nv_llama_layer_infer (csrc/layer.cu): ONE C-ABI call per layer instead of
     ten.  Holds the argument block and a workspace for a given packing; ``run`` fills in what changes per layer."""
