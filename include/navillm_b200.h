@@ -37,7 +37,7 @@ const char* nv_last_error(void);
 int nv_abi_version(void);
 /* Programmatic dependent launch for the decode chain (generate(): HF GenerationMixin greedy loop reached from
  * models/nav_model.py:324-338,388-399): when on, nv_embed_fwd / nv_rmsnorm_fwd / nv_gemm_skinny[_swiglu]_bf16 /
- * nv_decode_rope_kv / nv_decode_attn / nv_add_int / nv_argmax_masked / nv_trie_mask are launched with
+ * nv_decode_rope_kv / nv_decode_attn[_rope[_fp8]] / nv_add_int / nv_argmax_masked / nv_trie_mask are launched with
  * cudaLaunchAttributeProgrammaticStreamSerialization so a kernel's prologue (and the skinny GEMM's first weight tiles)
  * overlaps the tail of its predecessor.  Returns the previous setting.  Process-wide; default off. */
 int nv_set_pdl(int on);
@@ -206,6 +206,21 @@ int nv_decode_attn(const void* q, int64_t ldq, const void* kcache, const void* v
 /* nv_decode_rope_kv + nv_decode_attn in one launch (qkv pre-RoPE, not modified; k / v appended at row lens[b]). */
 int nv_decode_attn_rope(const void* qkv, int64_t ld, const int* lens, const void* cos_t, const void* sin_t, void* kcache,
                         void* vcache, void* out, int64_t ldo, int B, int Smax, int H, int head_dim, float scale, void* stream);
+/* Opt-in fp8 (e4m3) KV cache of generate()'s decode step (no reference counterpart for the number format).  Per layer,
+ * kq / vq [B, Smax, H*128] e4m3 bytes and kexp / vexp [B, Smax, H] int8: every cached (sequence b, position p, head h) row of
+ * 128 elements is stored in the weight format of nv_quantize_fp8_rows above,
+ *     K'[b,p,h,:] = e4m3(K[b,p,h,:] / 2^e) * 2^e,   e = kexp[b,p,h] = the row exponent of max|K[b,p,h,:]|   (V' alike),
+ * i.e. exactly the bytes and exponents nv_quantize_fp8_rows produces on a [B*Smax*H, 128] view of the bf16 cache (amax on the
+ * bf16 bit patterns, round to nearest even, saturating).  Half the bytes of the bf16 cache plus 1/256 for the exponents.
+ * nv_kv_store_prefill_fp8 is nv_kv_store_prefill (same packing, rows at p >= Smax dropped) into that cache.
+ * nv_decode_attn_rope_fp8 is nv_decode_attn_rope over it: the rotated k and the v of the new token are quantized as they are
+ * appended at row lens[b], and the attention returns bit for bit what nv_decode_attn_rope returns on a bf16 cache holding
+ * K' / V' (scores and P.V in fp32).  head_dim 128, ld % 8 == 0, 16-byte aligned qkv, 8-byte aligned kq / vq. */
+int nv_kv_store_prefill_fp8(const void* qkv, int64_t ld, const int* cu_seqlens, void* kq, void* vq, void* kexp, void* vexp, int B,
+                            int T, int Smax, int H, void* stream);
+int nv_decode_attn_rope_fp8(const void* qkv, int64_t ld, const int* lens, const void* cos_t, const void* sin_t, void* kq, void* vq,
+                            void* kexp, void* vexp, void* out, int64_t ldo, int B, int Smax, int H, int head_dim, float scale,
+                            void* stream);
 /* at most 64 special ids (n_special), here and in nv_sample_topk; longer lists return NV_ERR_BAD_ARG */
 int nv_argmax_masked(const void* logits, int64_t ld, int V, const int* special, int n_special, int* finished, int eos_id,
                      int pad_id, int stop_on_eos, int* next, int B, void* stream);
@@ -247,7 +262,9 @@ int nv_adamw_flat(void* p, void* g, void* m, void* v, int64_t n, int is_bf16, fl
  * kept: this is the forward of evaluation / prefill at small packed batches, where one ctypes call per kernel is the
  * bottleneck.  kv_mode 0: plain self-attention over the packed rows; 1: also store post-RoPE K/V of the rows in the caches
  * (prefill of generate); 2: the rows are suffixes of sequences whose prefixes are cached (cached / kv_start / kv_len as in
- * nv_kv_store_suffix / nv_attn_fwd_kv).  out_rows (nullable, R rows): only these rows are produced (last layer). */
+ * nv_kv_store_suffix / nv_attn_fwd_kv); 3: prefill of generate() into an fp8 cache (nv_kv_store_prefill_fp8: kcache / vcache
+ * hold e4m3 bytes, kexp / vexp the row exponents; the layer's own attention reads the unrounded K, V).  out_rows (nullable,
+ * R rows): only these rows are produced (last layer). */
 typedef struct nv_layer_args {
   const void* x;            /* [T, D] bf16 residual stream in */
   void* y;                  /* [R or T, D] bf16 residual stream out */
@@ -263,6 +280,7 @@ typedef struct nv_layer_args {
   const void* wqkv_q; const void* wqkv_e; const void* wo_q; const void* wo_e;
   const void* wgu_q; const void* wgu_e; const void* wd_q; const void* wd_e;
   int fp8_max_rows;
+  void* kexp; void* vexp;   /* kv_mode 3: int8 row exponents [B, Smax, H] of the fp8 caches */
 } nv_layer_args;
 int nv_layer_args_size(void);                           /* sizeof(nv_layer_args): bindings check their mirror against it */
 int64_t nv_llama_layer_ws_bytes(int T, int R, int D, int F);

@@ -49,7 +49,8 @@ class LayerArgs(ctypes.Structure):
                 + [(n, ctypes.c_int) for n in ("B", "T", "total_qblocks", "Smax", "Tkv", "kv_mode", "R", "D", "F", "H")]
                 + [("eps", ctypes.c_float), ("scale", ctypes.c_float)]
                 + [(n, ctypes.c_void_p) for n in ("wqkv_q", "wqkv_e", "wo_q", "wo_e", "wgu_q", "wgu_e", "wd_q", "wd_e")]
-                + [("fp8_max_rows", ctypes.c_int)])
+                + [("fp8_max_rows", ctypes.c_int)]
+                + [(n, ctypes.c_void_p) for n in ("kexp", "vexp")])
 
 
 launch_count = 0          # kernels launched through the C ABI since import (bench.py reports the per-step delta)

@@ -6,7 +6,13 @@
 // ([B, Smax, H*128] per layer for K and for V, bf16, real tokens only), one new token per sequence attends
 // over it with 128-bit coalesced loads, and the step has static shapes so the host can replay it as a CUDA
 // graph (sequence lengths live in device memory).
+//
+// Opt-in fp8 cache (nv_kv_store_prefill_fp8, nv_decode_attn_rope_fp8): the same layout in e4m3 bytes plus one int8 exponent
+// per (sequence, position, head) row of 128 elements, quantized with the weight format of nv_fp8.cuh as rows are stored.
+#include <type_traits>
+
 #include "nv_common.cuh"
+#include "nv_fp8.cuh"
 #include "nv_host.h"
 
 namespace nv {
@@ -14,6 +20,55 @@ namespace nv {
 __device__ __forceinline__ void unpack8d(const uint4& u, float (&f)[8]) {
   f[0] = bf16_lo(u.x); f[1] = bf16_hi(u.x); f[2] = bf16_lo(u.y); f[3] = bf16_hi(u.y);
   f[4] = bf16_lo(u.z); f[5] = bf16_hi(u.z); f[6] = bf16_lo(u.w); f[7] = bf16_hi(u.w);
+}
+
+// eight e4m3 bytes of a cache row with exponent e -> the fp32 values unpack8d gives for the same row rounded to bf16 (K', V')
+__device__ __forceinline__ void unpack8q(const uint2& u, int e, float (&f)[8]) {
+  const float s = fp8_pow2(e);
+  fp8x4_to_f32x4(u.x, s, f);
+  fp8x4_to_f32x4(u.y, s, f + 4);
+}
+
+// fp8 twin of kv_store_prefill_kernel (offs = 0): a half-warp owns one (token, head) row of K and of V; 16 lanes x 8 elements.
+// Same packing and the same drop of rows at p >= Smax.  Each row's amax, exponent and bytes follow quantize_fp8_rows_kernel.
+__global__ void __launch_bounds__(256) kv_store_prefill_fp8_kernel(const __nv_bfloat16* __restrict__ qkv, int64_t ld,
+                                                                   const int* __restrict__ cu, uint8_t* __restrict__ kq,
+                                                                   uint8_t* __restrict__ vq, int8_t* __restrict__ ke,
+                                                                   int8_t* __restrict__ ve, int B, int Smax, int H) {
+  const int HD = H * 128;
+  const int hl = threadIdx.x & 15, half = (threadIdx.x >> 4) & 1;
+  const int64_t rows = (int64_t)cu[B] * H;
+  const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  // the loop bound is uniform over the warp, so both halves reach every shuffle
+  for (int64_t r0 = 2 * ((int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)); r0 < rows; r0 += 2 * warps) {
+    const int64_t r = r0 + half;
+    const bool live = r < rows;
+    const int t = live ? (int)(r / H) : 0, h = live ? (int)(r % H) : 0;
+    int b = 0;
+    while (b + 1 < B && cu[b + 1] <= t) ++b;
+    const int p = t - cu[b];
+    uint4 k = make_uint4(0, 0, 0, 0), v = k;
+    if (live) {
+      k = *reinterpret_cast<const uint4*>(qkv + (int64_t)t * ld + HD + h * 128 + hl * 8);
+      v = *reinterpret_cast<const uint4*>(qkv + (int64_t)t * ld + 2 * HD + h * 128 + hl * 8);
+    }
+    uint32_t mk = bf16x8_amax_bits(k), mv = bf16x8_amax_bits(v);
+#pragma unroll
+    for (int o = 8; o > 0; o >>= 1) {                             // reduce inside the half-warp
+      mk = max(mk, __shfl_xor_sync(0xffffffffu, mk, o));
+      mv = max(mv, __shfl_xor_sync(0xffffffffu, mv, o));
+    }
+    if (live && p < Smax) {
+      const int ek = fp8_row_exponent(__uint_as_float(mk << 16)), ev = fp8_row_exponent(__uint_as_float(mv << 16));
+      const int64_t row = (int64_t)b * Smax + p;
+      *reinterpret_cast<uint2*>(kq + row * HD + h * 128 + hl * 8) = fp8x8_from_bf16x8(k, fp8_pow2(-ek));
+      *reinterpret_cast<uint2*>(vq + row * HD + h * 128 + hl * 8) = fp8x8_from_bf16x8(v, fp8_pow2(-ev));
+      if (hl == 0) {
+        ke[row * H + h] = (int8_t)ek;
+        ve[row * H + h] = (int8_t)ev;
+      }
+    }
+  }
 }
 
 // Copy the K and V column blocks of packed prefill rows into the cache: row t of sequence b at local
@@ -108,13 +163,20 @@ constexpr int DA_WARPS = 8;
 // ROPE = true fuses decode_rope_kv_kernel: q points at the PRE-RoPE fused qkv row block [B, 3*H*128]; warp 0 rotates this
 // head's q and k at position lens[b] (same rounding points as rope_kernel), appends the rotated k and the v to the caches
 // and hands the rotated q to the CTA through shared memory - one launch less per decoder layer and token.
-template <bool ROPE>
+// FP8 = true reads an fp8 cache (kc / vc e4m3 bytes, ke / ve the row exponents [B, Smax, H]; with ROPE the new k and v rows are
+// quantized as they are appended).  Keys are expanded to the fp32 values of the bf16-rounded rows K' / V', and the key
+// assignment and every reduction order are those of the bf16 kernel, so the output is bit for bit the bf16 kernel's on K' / V'.
+template <bool FP8>
+using kv_elem_t = typename std::conditional<FP8, uint8_t, __nv_bfloat16>::type;
+
+template <bool ROPE, bool FP8 = false>
 __global__ void __launch_bounds__(DA_WARPS * 32) decode_attn_kernel(const __nv_bfloat16* __restrict__ q, int64_t ldq,
-                                                          __nv_bfloat16* __restrict__ kc, __nv_bfloat16* __restrict__ vc,
+                                                          kv_elem_t<FP8>* __restrict__ kc, kv_elem_t<FP8>* __restrict__ vc,
                                                           const int* __restrict__ lens, __nv_bfloat16* __restrict__ out,
                                                           int64_t ldo, int Smax, int H, float scale,
                                                           const __nv_bfloat16* __restrict__ cos_t,
-                                                          const __nv_bfloat16* __restrict__ sin_t) {
+                                                          const __nv_bfloat16* __restrict__ sin_t,
+                                                          int8_t* __restrict__ ke, int8_t* __restrict__ ve) {
   __shared__ float s_m[DA_WARPS], s_l[DA_WARPS];
   __shared__ float s_acc[DA_WARPS][128];
   __shared__ uint4 s_q[16];                            // rotated q of this head (bf16 x 128)
@@ -128,6 +190,7 @@ __global__ void __launch_bounds__(DA_WARPS * 32) decode_attn_kernel(const __nv_b
   if (ROPE) {
     const int p = n - 1;
     if (w == 0) {
+      uint4 r0 = make_uint4(0, 0, 0, 0), r1 = r0;       // FP8: this lane's chunks of the new k row (lanes 8..15) or v row (16..31)
       if (lane < 16) {                                  // lanes 0..7: q chunk c, lanes 8..15: k chunk c
         const int c = lane & 7, is_k = lane >> 3;
         const __nv_bfloat16* base = q + (int64_t)b * ldq + (is_k ? HD : 0) + h * 128;
@@ -151,15 +214,42 @@ __global__ void __launch_bounds__(DA_WARPS * 32) decode_attn_kernel(const __nv_b
         }
         if (!is_k) {
           s_q[c] = o1; s_q[8 + c] = o2;
+        } else if constexpr (FP8) {
+          r0 = o1; r1 = o2;
         } else if (p < Smax) {
           __nv_bfloat16* dst = kc + ((int64_t)b * Smax + p) * HD + h * 128;
           *reinterpret_cast<uint4*>(dst + c * 8) = o1;
           *reinterpret_cast<uint4*>(dst + 64 + c * 8) = o2;
         }
+      } else if constexpr (FP8) {
+        r0 = *reinterpret_cast<const uint4*>(q + (int64_t)b * ldq + 2 * HD + h * 128 + (lane - 16) * 8);
       } else if (p < Smax) {                            // lanes 16..31: this head's v (16 x 16 bytes)
         const int v = lane - 16;
         *reinterpret_cast<uint4*>(vc + ((int64_t)b * Smax + p) * HD + h * 128 + v * 8) =
             *reinterpret_cast<const uint4*>(q + (int64_t)b * ldq + 2 * HD + h * 128 + v * 8);
+      }
+      if constexpr (FP8) {
+        // row amax: the k row over lanes 8..15 (xor 1, 2, 4), the v row over lanes 16..31 (and xor 8); lanes 0..7 reduce
+        // a value nobody uses
+        uint32_t m = max(bf16x8_amax_bits(r0), bf16x8_amax_bits(r1));
+#pragma unroll
+        for (int o = 1; o < 8; o <<= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+        const uint32_t m8 = __shfl_xor_sync(0xffffffffu, m, 8);
+        if (lane >= 16) m = max(m, m8);
+        const int e = fp8_row_exponent(__uint_as_float(m << 16));
+        const float inv = fp8_pow2(-e);
+        if (lane >= 8 && p < Smax) {
+          const int64_t row = (int64_t)b * Smax + p;
+          if (lane < 16) {
+            uint8_t* dst = kc + row * HD + h * 128 + (lane & 7) * 8;
+            *reinterpret_cast<uint2*>(dst) = fp8x8_from_bf16x8(r0, inv);
+            *reinterpret_cast<uint2*>(dst + 64) = fp8x8_from_bf16x8(r1, inv);
+            if (lane == 8) ke[row * H + h] = (int8_t)e;
+          } else {
+            *reinterpret_cast<uint2*>(vc + row * HD + h * 128 + (lane - 16) * 8) = fp8x8_from_bf16x8(r0, inv);
+            if (lane == 16) ve[row * H + h] = (int8_t)e;
+          }
+        }
       }
     }
     __syncthreads();                                    // rotated q in smem, new k / v rows visible to the whole CTA
@@ -172,34 +262,53 @@ __global__ void __launch_bounds__(DA_WARPS * 32) decode_attn_kernel(const __nv_b
   // before the first use, which is what a latency-bound streaming loop needs (one key per half-warp and
   // iteration kept ~1 MB in flight chip-wide and ran at 35 us for 52 MB of cache).
   constexpr int KPI = 4;
-  auto load_keys = [&](int jb, uint4 (&kr)[KPI], uint4 (&vr)[KPI]) {
+  // one key's 8 elements of this lane: 16 bytes of bf16, or 8 e4m3 bytes and (ke / ve) the row's exponent
+  using raw_t = typename std::conditional<FP8, uint2, uint4>::type;
+  auto load_keys = [&](int jb, raw_t (&kr)[KPI], raw_t (&vr)[KPI], int (&kx)[KPI], int (&vx)[KPI]) {
 #pragma unroll
     for (int u = 0; u < KPI; ++u) {
       if (jb + u < n) {
         const int64_t off = ((int64_t)b * Smax + jb + u) * HD + h * 128 + hl * 8;
-        kr[u] = *reinterpret_cast<const uint4*>(kc + off);
-        vr[u] = *reinterpret_cast<const uint4*>(vc + off);
+        kr[u] = *reinterpret_cast<const raw_t*>(kc + off);
+        vr[u] = *reinterpret_cast<const raw_t*>(vc + off);
+        if constexpr (FP8) {
+          const int64_t row = ((int64_t)b * Smax + jb + u) * H + h;
+          kx[u] = ke[row];
+          vx[u] = ve[row];
+        }
       } else {
-        kr[u] = make_uint4(0, 0, 0, 0);
-        vr[u] = make_uint4(0, 0, 0, 0);
+        if constexpr (FP8) {
+          kr[u] = make_uint2(0, 0);
+          vr[u] = make_uint2(0, 0);
+          kx[u] = vx[u] = 0;
+        } else {
+          kr[u] = make_uint4(0, 0, 0, 0);
+          vr[u] = make_uint4(0, 0, 0, 0);
+        }
       }
     }
   };
+  auto unpack = [&](const raw_t& r, int x, float (&f)[8]) {
+    if constexpr (FP8) unpack8q(r, x, f);
+    else unpack8d(r, f);
+  };
   // software pipeline: the loads of the NEXT 8 keys are in flight while the current ones are reduced (the loop is a chain
   // of DRAM-latency-long iterations otherwise)
-  uint4 knext[KPI], vnext[KPI];
-  load_keys(w * 2 * KPI + half * KPI, knext, vnext);
+  raw_t knext[KPI], vnext[KPI];
+  int kxnext[KPI], vxnext[KPI];
+  load_keys(w * 2 * KPI + half * KPI, knext, vnext, kxnext, vxnext);
   for (int j0 = w * 2 * KPI; j0 < n; j0 += DA_WARPS * 2 * KPI) {
     const int jb = j0 + half * KPI;
-    uint4 kraw[KPI], vraw[KPI];
+    raw_t kraw[KPI], vraw[KPI];
+    int kx[KPI], vx[KPI];
 #pragma unroll
-    for (int u = 0; u < KPI; ++u) { kraw[u] = knext[u]; vraw[u] = vnext[u]; }
-    if (j0 + DA_WARPS * 2 * KPI < n) load_keys(jb + DA_WARPS * 2 * KPI, knext, vnext);
+    for (int u = 0; u < KPI; ++u) { kraw[u] = knext[u]; vraw[u] = vnext[u]; kx[u] = kxnext[u]; vx[u] = vxnext[u]; }
+    if (j0 + DA_WARPS * 2 * KPI < n) load_keys(jb + DA_WARPS * 2 * KPI, knext, vnext, kxnext, vxnext);
     float sc[KPI];
 #pragma unroll
     for (int u = 0; u < KPI; ++u) {
       float kf[8];
-      unpack8d(kraw[u], kf);
+      unpack(kraw[u], kx[u], kf);
       float s = 0.f;
 #pragma unroll
       for (int i = 0; i < 8; ++i) s += qf[i] * kf[i];
@@ -223,7 +332,7 @@ __global__ void __launch_bounds__(DA_WARPS * 32) decode_attn_kernel(const __nv_b
         if (jb + u < n) {
           const float p = exp2f((sc[u] - mn) * sl2);
           float vf[8];
-          unpack8d(vraw[u], vf);
+          unpack(vraw[u], vx[u], vf);
           l += p;
 #pragma unroll
           for (int i = 0; i < 8; ++i) acc[i] += p * vf[i];
@@ -641,7 +750,7 @@ int nv_decode_attn(const void* q, int64_t ldq, const void* kcache, const void* v
   if (B == 0) return NV_OK;
   NV_CUDA(launch_pdl(decode_attn_kernel<false>, dim3(B * H), dim3(DA_WARPS * 32), 0, S_(stream), CBF(q), ldq,
                      const_cast<__nv_bfloat16*>(CBF(kcache)), const_cast<__nv_bfloat16*>(CBF(vcache)), lens, BF(out), ldo, Smax, H, scale,
-                     (const __nv_bfloat16*)nullptr, (const __nv_bfloat16*)nullptr));
+                     (const __nv_bfloat16*)nullptr, (const __nv_bfloat16*)nullptr, (int8_t*)nullptr, (int8_t*)nullptr));
   return NV_OK;
 }
 
@@ -653,7 +762,42 @@ int nv_decode_attn_rope(const void* qkv, int64_t ld, const int* lens, const void
   NV_REQUIRE(head_dim == 128 && (ld & 7) == 0, "nv_decode_attn_rope: head_dim must be 128, ld %% 8 == 0");
   if (B == 0) return NV_OK;
   NV_CUDA(launch_pdl(decode_attn_kernel<true>, dim3(B * H), dim3(DA_WARPS * 32), 0, S_(stream), CBF(qkv), ld, BF(kcache), BF(vcache), lens,
-                     BF(out), ldo, Smax, H, scale, CBF(cos_t), CBF(sin_t)));
+                     BF(out), ldo, Smax, H, scale, CBF(cos_t), CBF(sin_t), (int8_t*)nullptr, (int8_t*)nullptr));
+  return NV_OK;
+}
+
+// fp8 cache (format: include/navillm_b200.h): nv_kv_store_prefill with every stored (token, head) row quantized.
+int nv_kv_store_prefill_fp8(const void* qkv, int64_t ld, const int* cu_seqlens, void* kq, void* vq, void* kexp, void* vexp, int B,
+                            int T, int Smax, int H, void* stream) {
+  NV_REQUIRE(B >= 0 && T >= 0 && Smax > 0 && H > 0, "nv_kv_store_prefill_fp8: bad sizes (B=%d T=%d Smax=%d H=%d)", B, T, Smax, H);
+  if (T == 0 || B == 0) return NV_OK;
+  NV_REQUIRE(qkv && cu_seqlens && kq && vq && kexp && vexp, "nv_kv_store_prefill_fp8: null argument");
+  NV_REQUIRE((ld & 7) == 0 && ((uintptr_t)qkv & 15) == 0 && ((uintptr_t)kq & 7) == 0 && ((uintptr_t)vq & 7) == 0,
+             "nv_kv_store_prefill_fp8: alignment (ld %% 8 == 0, 16-byte qkv, 8-byte caches)");
+  const int64_t warps = ((int64_t)T * H + 1) / 2;
+  int grid = (int)((warps + 7) / 8);
+  const int cap = sm_count() * 16;
+  if (grid > cap) grid = cap;
+  kv_store_prefill_fp8_kernel<<<grid, 256, 0, S_(stream)>>>(CBF(qkv), ld, cu_seqlens, reinterpret_cast<uint8_t*>(kq),
+                                                            reinterpret_cast<uint8_t*>(vq), reinterpret_cast<int8_t*>(kexp),
+                                                            reinterpret_cast<int8_t*>(vexp), B, Smax, H);
+  NV_LAUNCH_CHECK();
+  return NV_OK;
+}
+
+// nv_decode_attn_rope over an fp8 cache: the new k / v rows are quantized as they are appended.
+int nv_decode_attn_rope_fp8(const void* qkv, int64_t ld, const int* lens, const void* cos_t, const void* sin_t, void* kq, void* vq,
+                            void* kexp, void* vexp, void* out, int64_t ldo, int B, int Smax, int H, int head_dim, float scale,
+                            void* stream) {
+  NV_REQUIRE(head_dim == 128 && (ld & 7) == 0, "nv_decode_attn_rope_fp8: head_dim must be 128, ld %% 8 == 0");
+  NV_REQUIRE(B >= 0 && Smax > 0 && H > 0, "nv_decode_attn_rope_fp8: bad sizes (B=%d Smax=%d H=%d)", B, Smax, H);
+  if (B == 0) return NV_OK;
+  NV_REQUIRE(qkv && lens && cos_t && sin_t && kq && vq && kexp && vexp && out, "nv_decode_attn_rope_fp8: null argument");
+  NV_REQUIRE(((uintptr_t)qkv & 15) == 0 && ((uintptr_t)kq & 7) == 0 && ((uintptr_t)vq & 7) == 0,
+             "nv_decode_attn_rope_fp8: alignment (16-byte qkv, 8-byte caches)");
+  NV_CUDA(launch_pdl(decode_attn_kernel<true, true>, dim3(B * H), dim3(DA_WARPS * 32), 0, S_(stream), CBF(qkv), ld,
+                     reinterpret_cast<uint8_t*>(kq), reinterpret_cast<uint8_t*>(vq), lens, BF(out), ldo, Smax, H, scale, CBF(cos_t),
+                     CBF(sin_t), reinterpret_cast<int8_t*>(kexp), reinterpret_cast<int8_t*>(vexp)));
   return NV_OK;
 }
 

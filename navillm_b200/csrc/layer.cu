@@ -82,6 +82,9 @@ extern "C" int nv_llama_layer_infer(const nv_layer_args* a, void* stream) {
   } else {
     if (a->kv_mode == 1)            // prefill of generate(): post-RoPE K, V also go to the cache
       STEP(nv_kv_store_prefill(qkv, 3 * (int64_t)D, a->cu_seqlens, a->kcache, a->vcache, a->B, T, a->Smax, D, stream));
+    else if (a->kv_mode == 3)       // ... into an fp8 cache
+      STEP(nv_kv_store_prefill_fp8(qkv, 3 * (int64_t)D, a->cu_seqlens, a->kcache, a->vcache, a->kexp, a->vexp, a->B, T, a->Smax, H,
+                                   stream));
     STEP(nv_attn_fwd(qkv, 3 * (int64_t)D, qkv + (int64_t)D * 2, 3 * (int64_t)D, qkv + (int64_t)D * 4, 3 * (int64_t)D, ao, D, nullptr,
                      a->cu_seqlens, a->B, T, H, 128, a->total_qblocks, a->scale, stream));
   }

@@ -60,4 +60,42 @@ __device__ __forceinline__ void fp8x4_to_bf16x4(uint32_t q, float scale, uint32_
   hi = *reinterpret_cast<uint32_t*>(&v1);
 }
 
+// The row-quantize step shared by the weight quantizer (quant.cu) and the fp8 KV cache (decode.cu).
+// |x| of eight bf16 values as 15-bit patterns (|x| orders like them): the per-lane part of a row's amax.  The row's amax is
+// the max over its lanes, and its exponent is fp8_row_exponent(__uint_as_float(amax_bits << 16)).
+__device__ __forceinline__ uint32_t bf16x8_amax_bits(const uint4& v) {
+  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+  uint32_t m = 0;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) m = max(m, max(w[j] & 0x7FFFu, (w[j] >> 16) & 0x7FFFu));
+  return m;
+}
+
+// eight bf16 values of a row with exponent e (inv = 2^-e) -> eight e4m3 bytes (lowest element in the lowest byte)
+__device__ __forceinline__ uint2 fp8x8_from_bf16x8(const uint4& v, float inv) {
+  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+  uint32_t q[2];
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const uint32_t a = w[2 * j], b = w[2 * j + 1];
+    q[j] = fp8x4_from_f32(__uint_as_float(a << 16) * inv, __uint_as_float(a & 0xffff0000u) * inv, __uint_as_float(b << 16) * inv,
+                          __uint_as_float(b & 0xffff0000u) * inv);
+  }
+  return make_uint2(q[0], q[1]);
+}
+
+// four e4m3 bytes -> the four fp32 values of e4m3 * scale (scale = 2^e): the values fp8x4_to_bf16x4 rounds to bf16, which
+// that rounding keeps exactly (see above), so they equal the fp32 widening of the bf16 W'.
+__device__ __forceinline__ void fp8x4_to_f32x4(uint32_t q, float scale, float* f) {
+  uint32_t h0, h1;
+  asm("{\n\t.reg .b16 a, b;\n\t"
+      "mov.b32 {a, b}, %2;\n\t"
+      "cvt.rn.f16x2.e4m3x2 %0, a;\n\t"
+      "cvt.rn.f16x2.e4m3x2 %1, b;\n\t}"
+      : "=r"(h0), "=r"(h1) : "r"(q));
+  const float2 f0 = __half22float2(*reinterpret_cast<const __half2*>(&h0));
+  const float2 f1 = __half22float2(*reinterpret_cast<const __half2*>(&h1));
+  f[0] = f0.x * scale; f[1] = f0.y * scale; f[2] = f1.x * scale; f[3] = f1.y * scale;
+}
+
 }  // namespace nv

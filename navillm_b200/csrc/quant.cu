@@ -19,12 +19,7 @@ quantize_fp8_rows_kernel(__nv_bfloat16* __restrict__ W, int64_t ldw, uint8_t* __
   uint4* wrow = reinterpret_cast<uint4*>(W + n * ldw);
   const int nvec = K >> 3;                                   // 8 bf16 per 16-byte vector
   uint32_t m = 0;
-  for (int i = threadIdx.x; i < nvec; i += QZ_THREADS) {
-    const uint4 v = wrow[i];
-    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-    for (int j = 0; j < 4; ++j) m = max(m, max(w[j] & 0x7FFFu, (w[j] >> 16) & 0x7FFFu));
-  }
+  for (int i = threadIdx.x; i < nvec; i += QZ_THREADS) m = max(m, bf16x8_amax_bits(wrow[i]));
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
@@ -37,16 +32,11 @@ quantize_fp8_rows_kernel(__nv_bfloat16* __restrict__ W, int64_t ldw, uint8_t* __
   if (threadIdx.x == 0) exps[n] = (int8_t)e;
   uint2* qrow = reinterpret_cast<uint2*>(Q + n * ldq);
   for (int i = threadIdx.x; i < nvec; i += QZ_THREADS) {
-    const uint4 v = wrow[i];
-    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-    uint32_t q[2], o[4];
-#pragma unroll
-    for (int j = 0; j < 2; ++j) {
-      const uint32_t a = w[2 * j], b = w[2 * j + 1];
-      q[j] = fp8x4_from_f32(bf16_lo(a) * inv, bf16_hi(a) * inv, bf16_lo(b) * inv, bf16_hi(b) * inv);
-      fp8x4_to_bf16x4(q[j], scale, o[2 * j], o[2 * j + 1]);
-    }
-    qrow[i] = make_uint2(q[0], q[1]);
+    const uint2 q = fp8x8_from_bf16x8(wrow[i], inv);
+    uint32_t o[4];
+    fp8x4_to_bf16x4(q.x, scale, o[0], o[1]);
+    fp8x4_to_bf16x4(q.y, scale, o[2], o[3]);
+    qrow[i] = q;
     wrow[i] = make_uint4(o[0], o[1], o[2], o[3]);
   }
 }

@@ -314,6 +314,12 @@ class _Saved:
     __slots__ = ("x", "rstd1", "xn", "qkv", "ao", "lse", "xm", "rstd2", "xn2", "gu", "h", "rows", "ao_r")
 
 
+def is_fp8_kv(caches) -> bool:
+    """True for the per-layer list of an fp8 KV cache: ``(e4m3 [B, Smax, H*128], int8 exponents [B, Smax, H])`` pairs
+    (include/navillm_b200.h); False for bf16 tensors [B, Smax, H*128]."""
+    return isinstance(caches[0], tuple)
+
+
 class LlamaCore:
     """Forward/backward driver of the decoder stack on packed rows.  Not an nn.Module: parameters live in
     ``LlamaModelParams`` (HF-named) and are accessed through fused views of a ``FlatParams`` buffer."""
@@ -399,17 +405,23 @@ class LlamaCore:
         R = 0 if out_rows is None else out_rows.numel()
         run = ops.LayerRunner(T, d.hidden, d.inter, d.n_heads, d.rms_eps, pos, self.cos, self.sin, cu, len(seqlens), ops._qblocks(seqlens),
                               R=R, device=x.device)
+        fp8_kv = kv_store is not None and is_fp8_kv(kv_store[0])
         if kv_store is not None:
-            run.set_cache_mode(1, kv_store[0][0].shape[1])
+            run.set_cache_mode(3 if fp8_kv else 1, kv_store[0][0][0].shape[1] if fp8_kv else kv_store[0][0].shape[1])
         bufs = [torch.empty_like(x), torch.empty_like(x)]
         last = d.n_layers - 1
         f8 = self.fp8_for_inference()
         for l, lyr in enumerate(self.model.layers):
             pruned = out_rows is not None and l == last
             y = torch.empty((R, d.hidden), dtype=bf16, device=x.device) if pruned else bufs[l & 1]
+            kc = vc = ke = ve = None
+            if fp8_kv:
+                (kc, ke), (vc, ve) = kv_store[0][l], kv_store[1][l]
+            elif kv_store is not None:
+                kc, vc = kv_store[0][l], kv_store[1][l]
             run.run(x, y, lyr.input_layernorm.weight.data, self.wqkv[l], self.wo[l], lyr.post_attention_layernorm.weight.data, self.wgu[l],
-                    self.wd[l], kc=kv_store[0][l] if kv_store is not None else None, vc=kv_store[1][l] if kv_store is not None else None,
-                    out_rows=out_rows if pruned else None, fp8=self._fp8_layer(f8, l), fp8_max_rows=FP8_MAX_ROWS)
+                    self.wd[l], kc=kc, vc=vc, ke=ke, ve=ve, out_rows=out_rows if pruned else None, fp8=self._fp8_layer(f8, l),
+                    fp8_max_rows=FP8_MAX_ROWS)
             x = y
         return x
 
@@ -423,7 +435,10 @@ class LlamaCore:
         ``out_rows`` (int32 [R], device): only these rows of the output are needed (the <cls_1> rows in the
         navigation / grounding modes, the label rows in the LM-loss modes, the last rows in prefill).  The last
         layer then runs o_proj / MLP on R rows instead of T (its K,V still come from all rows) and the return
-        value is [R, D].  The reference computes all positions and reads only these (SURVEY.md Appendix A.10)."""
+        value is [R, D].  The reference computes all positions and reads only these (SURVEY.md Appendix A.10).
+
+        ``kv_store`` (prefill of generate): (kc, vc) per-layer caches, bf16 [B, Smax, D] or fp8 ``(e4m3 [B, Smax, D], int8
+        exponents [B, Smax, H])`` pairs (``is_fp8_kv``); the prompt's own attention reads the unrounded K, V either way."""
         d = self.d
         H = d.n_heads
         saved: List[_Saved] = []
@@ -432,7 +447,11 @@ class LlamaCore:
         fused = self.fused_epilogues and x.shape[0] >= 1024 and d.inter % 128 == 0 and d.hidden % 256 == 0
         if kv_store is not None and kv_sink is None:                  # (kc list, vc list): post-RoPE K, V of every layer go to the caches
             B_, T_ = len(seqlens), x.shape[0]
-            kv_sink = lambda l, qkv: ops.kv_store_prefill(qkv, cu, kv_store[0][l], kv_store[1][l], B_, T_)
+            if is_fp8_kv(kv_store[0]):                                # fp8 cache: (e4m3 bytes, exponents) per layer
+                kv_sink = lambda l, qkv: ops.kv_store_prefill_fp8(qkv, cu, kv_store[0][l][0], kv_store[1][l][0], kv_store[0][l][1],
+                                                                  kv_store[1][l][1], B_, T_)
+            else:
+                kv_sink = lambda l, qkv: ops.kv_store_prefill(qkv, cu, kv_store[0][l], kv_store[1][l], B_, T_)
         if self.LAYER_CALL and not save and not fused and d.head_dim == 128 and (kv_store is not None or kv_sink is None):
             return self._forward_layer_calls(x, pos, cu, seqlens, kv_store, out_rows), None
         f8 = None if save else self.fp8_for_inference()     # training forwards never read the fp8 copy
@@ -620,7 +639,8 @@ class LlamaCore:
     # -------------------------------------------------------------------------------------------------
     def decode_step(self, x: torch.Tensor, lens: torch.Tensor, kc: List[torch.Tensor], vc: List[torch.Tensor]) -> torch.Tensor:
         """One new token per sequence.  x: [B, D] bf16 embeddings of the new tokens; lens: int32 [B] (device) =
-        number of cached tokens = position of the new token; caches [B, Smax, D] per layer.  Static shapes and
+        number of cached tokens = position of the new token; caches [B, Smax, D] bf16 per layer, or fp8 ``(e4m3, exponents)``
+        pairs per layer (``is_fp8_kv``; the new rows are rounded as they are appended).  Static shapes and
         device-resident lengths: the whole step can be captured in a CUDA graph.  Returns the residual stream
         [B, D] before the final RMSNorm."""
         d = self.d
@@ -647,10 +667,15 @@ class LlamaCore:
                 lin = lambda a, w, addend=None: ops.gemm_skinny(a, w, addend=addend)
             else:
                 lin = lambda a, w, addend=None: ops.gemm(a, w, addend=addend, block_n=bn)
+        fp8_kv = is_fp8_kv(kc)
+        if fp8_kv and d.head_dim != 128:
+            raise NotImplementedError("the fp8 KV cache is built for head_dim = 128")
         for l, lyr in enumerate(self.model.layers):
             xn, _ = ops.rmsnorm_fwd(x, lyr.input_layernorm.weight.data, d.rms_eps)
             qkv = lin(xn, wqkv[l])
-            if d.head_dim == 128:
+            if fp8_kv:                                                                   # same, quantizing the appended rows
+                ao = ops.decode_attn_rope_fp8(qkv, lens, self.cos, self.sin, kc[l][0], vc[l][0], kc[l][1], vc[l][1], H)
+            elif d.head_dim == 128:
                 ao = ops.decode_attn_rope(qkv, lens, self.cos, self.sin, kc[l], vc[l], H)   # RoPE + cache append + attention
             else:
                 ops.rope_(qkv, lens, self.cos, self.sin, 2 * H, d.head_dim)

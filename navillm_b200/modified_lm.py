@@ -540,12 +540,31 @@ class ModifiedLlamaForCausalLM(nn.Module):
         if self.core.fp8 is None:                    # the decoder stack was rebuilt around the same buffer
             self.core.set_fp8(fp8)
 
+    # ---- opt-in fp8 (e4m3) KV cache in generate() ----
+    kv_cache_dtype = "bf16"
+
+    def set_kv_cache_dtype(self, dtype: str) -> str:
+        """Storage format of ``generate()``'s KV cache: ``"bf16"`` (default) or ``"fp8"``.  Returns the previous format.
+
+        ``"fp8"`` stores every cached (sequence, position, head) row of K and V as e4m3 with one power-of-two exponent per
+        row (include/navillm_b200.h): half the cache memory, and half the bytes each decode step's attention reads.  The
+        prefill's attention over the prompt reads the unrounded K/V, so the first generated token is the bf16 one; every
+        later step attends over the rounded K'/V' (exactly, as bf16 attention over K'/V' would).  This covers greedy,
+        sampled and trie-constrained decoding, graphed or eager, with or without ``quantize_weights_fp8()``, at any batch
+        size.  The choice is always the caller's: a rule that depended on the batch size would make one prompt's tokens
+        depend on the batch it came in.  Its effect on task metrics has not been measured."""
+        if dtype not in ("bf16", "fp8"):
+            raise ValueError(f"set_kv_cache_dtype: 'bf16' or 'fp8' expected, got {dtype!r}")
+        prev, self.kv_cache_dtype = self.kv_cache_dtype, dtype
+        return prev
+
     # ---- generation (models/nav_model.py:324-338,388-399; HF GenerationMixin greedy / sampling) ----
     decode_pdl = os.environ.get("NAVILLM_DECODE_PDL", "1") != "0"   # developer knob: 0 = plain stream-ordered launches
     max_decode_states = 2        # cached (KV buffers + captured decode graph) sets, least recently used evicted
 
     def _decode_state(self, B: int, Smax: int, key_extra: tuple, want_graph: bool):
-        """Persistent per-shape decode state: the contiguous KV cache [B, Smax, D] per layer, the step's I/O buffers and --
+        """Persistent per-shape decode state: the contiguous KV cache [B, Smax, D] per layer (in ``kv_cache_dtype``; the caller
+        puts that format in ``key_extra``, so a graph is never replayed over the other one), the step's I/O buffers and --
         once captured -- the CUDA graph of ONE decode step.  Capturing and instantiating the ~260-node graph costs more than
         the 127 replays of a C3 generation save, so it is done once per (batch, cache length, stop rule, decoding mode and
         the scalars the step bakes in) and reused by every later ``generate`` call (evaluation loops call generate with the
@@ -559,9 +578,13 @@ class ModifiedLlamaForCausalLM(nn.Module):
             return st
         dev, d = self._device(), self.dims
         V = self.lm_head.weight.shape[0]
+        if self.kv_cache_dtype == "fp8":                          # (e4m3 bytes, int8 row exponents) per layer
+            cache = lambda: [(torch.empty((B, Smax, d.hidden), dtype=ops.fp8, device=dev),
+                              torch.empty((B, Smax, d.n_heads), dtype=torch.int8, device=dev)) for _ in range(d.n_layers)]
+        else:
+            cache = lambda: [torch.empty((B, Smax, d.hidden), dtype=bf16, device=dev) for _ in range(d.n_layers)]
         st = SimpleNamespace(
-            kc=[torch.empty((B, Smax, d.hidden), dtype=bf16, device=dev) for _ in range(d.n_layers)],
-            vc=[torch.empty((B, Smax, d.hidden), dtype=bf16, device=dev) for _ in range(d.n_layers)],
+            kc=cache(), vc=cache(),
             logits=torch.empty((B, (V + 63) // 64 * 64), dtype=bf16, device=dev)[:, :V],
             next_ids=torch.empty((B,), dtype=torch.int32, device=dev),
             finished=torch.zeros((B,), dtype=torch.int32, device=dev),
@@ -666,7 +689,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
         mode = ("trie+sample" if do_sample else "trie") if table is not None else ("sample" if do_sample else "greedy")
         Smax = (max(pp.seqlens) + max_new_tokens + 127) // 128 * 128          # bucketed: more reuse of the cached state
         key = (int(eos), int(pad), bool(stop_on_eos), mode, float(temperature) if do_sample else None,
-               int(top_k) if do_sample else None, table.eos if table is not None else None)
+               int(top_k) if do_sample else None, table.eos if table is not None else None, self.kv_cache_dtype)
         st = self._decode_state(B, Smax, key, graphed)
         kc, vc, logits, next_ids, finished, lens = st.kc, st.vc, st.logits, st.next_ids, st.finished, st.lens
         if do_sample and not need_host and st.u is None:

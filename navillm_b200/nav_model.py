@@ -253,6 +253,11 @@ class NavModel(nn.Module):
     def drop_fp8_weights(self) -> None:
         self.lang_model.drop_fp8_weights()
 
+    def set_kv_cache_dtype(self, dtype: str) -> str:
+        """KV-cache format of the language model's ``generate()`` (the 3dqa, summarization and embodied_qa modes): ``"bf16"``
+        (default) or ``"fp8"``; see ``ModifiedLlamaForCausalLM.set_kv_cache_dtype``.  Returns the previous format."""
+        return self.lang_model.set_kv_cache_dtype(dtype)
+
     def _flat_buffers_ready(self) -> bool:
         return self.lang_model.core is not None and self._flat32 is not None
 

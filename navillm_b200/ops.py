@@ -543,6 +543,54 @@ def decode_attn_rope(qkv, lens, cos_t, sin_t, kc, vc, n_heads, *, out=None, scal
     return out
 
 
+def _fp8_cache(kq, ke, name):
+    """kq: float8_e4m3fn [B, Smax, H*128] contiguous, ke: int8 [B, Smax, H] contiguous (the fp8 KV cache of one layer)."""
+    if kq.dtype != torch.float8_e4m3fn or ke.dtype != torch.int8 or kq.dim() != 3 or not kq.is_contiguous() \
+            or not ke.is_contiguous() or kq.shape[2] % 128 or tuple(ke.shape) != (kq.shape[0], kq.shape[1], kq.shape[2] // 128):
+        raise ValueError(f"{name}: float8_e4m3fn [B, Smax, H*128] cache with int8 [B, Smax, H] exponents expected "
+                         f"(got {kq.dtype} {tuple(kq.shape)}, {ke.dtype} {tuple(ke.shape)})")
+
+
+def _fp8_kv(kq, vq, ke, ve, name):
+    _fp8_cache(kq, ke, name)
+    _fp8_cache(vq, ve, name)
+    if kq.shape != vq.shape:
+        raise ValueError(f"{name}: K cache {tuple(kq.shape)} and V cache {tuple(vq.shape)} differ")
+    return kq.shape
+
+
+def kv_store_prefill_fp8(qkv, cu, kq, vq, ke, ve, B, T):
+    """``kv_store_prefill`` into an fp8 cache (include/navillm_b200.h): every stored (token, head) row of K and V is rounded
+    to e4m3 with its own power-of-two exponent, the bytes ``quantize_fp8_`` writes for that row."""
+    _, Smax, HD = _fp8_kv(kq, vq, ke, ve, "kv_store_prefill_fp8")
+    if qkv.dtype != bf16 or qkv.stride(1) != 1 or qkv.shape[1] < 3 * HD:
+        raise ValueError(f"kv_store_prefill_fp8: qkv bf16 [T, >= {3 * HD}] rows expected (got {qkv.dtype} {tuple(qkv.shape)})")
+    check(_lib.load().nv_kv_store_prefill_fp8(ptr(qkv), i64(qkv.stride(0)), ptr(cu), ptr(kq), ptr(vq), ptr(ke), ptr(ve), i32(B), i32(T),
+                                              i32(Smax), i32(HD // 128), stream_ptr()), "nv_kv_store_prefill_fp8")
+
+
+def decode_attn_rope_fp8(qkv, lens, cos_t, sin_t, kq, vq, ke, ve, n_heads, *, out=None, scale=None):
+    """``decode_attn_rope`` over an fp8 cache: the rotated k and the v of the new token are rounded to e4m3 (one exponent per
+    head row) as they are appended at row lens[b]; the output equals ``decode_attn_rope`` on a bf16 cache holding the rounded
+    rows K' / V', bit for bit.  Returns [B, H*128] bf16."""
+    B, Smax, HD = _fp8_kv(kq, vq, ke, ve, "decode_attn_rope_fp8")
+    if HD != n_heads * 128 or qkv.dtype != bf16 or qkv.stride(1) != 1 or tuple(qkv.shape) != (B, 3 * HD):
+        raise ValueError(f"decode_attn_rope_fp8: qkv bf16 [{B}, {3 * HD}] and {HD // 128} heads expected "
+                         f"(got {qkv.dtype} {tuple(qkv.shape)}, {n_heads} heads)")
+    if lens.dtype != torch.int32 or lens.numel() != B:
+        raise ValueError(f"decode_attn_rope_fp8: lens int32 [{B}] expected (got {lens.dtype} {tuple(lens.shape)})")
+    if out is None:
+        out = torch.empty((B, HD), dtype=bf16, device=qkv.device)
+    if out.dtype != bf16 or out.stride(1) != 1 or tuple(out.shape) != (B, HD):
+        raise ValueError(f"decode_attn_rope_fp8: out bf16 [{B}, {HD}] expected (got {out.dtype} {tuple(out.shape)})")
+    if scale is None:
+        scale = 128 ** -0.5
+    check(_lib.load().nv_decode_attn_rope_fp8(ptr(qkv), i64(qkv.stride(0)), ptr(lens), ptr(cos_t), ptr(sin_t), ptr(kq), ptr(vq), ptr(ke),
+                                              ptr(ve), ptr(out), i64(out.stride(0)), i32(B), i32(Smax), i32(n_heads), i32(128), f32(scale),
+                                              stream_ptr()), "nv_decode_attn_rope_fp8")
+    return out
+
+
 def argmax_masked(logits, special, finished, eos_id, pad_id, stop_on_eos, next_ids):
     B, V = logits.shape
     check(_lib.load().nv_argmax_masked(ptr(logits), i64(logits.stride(0)), i32(V), ptr(special), i32(special.numel()),
@@ -606,9 +654,10 @@ class LayerRunner:
         a.kv_len = kv_len.data_ptr() if kv_len is not None else None
         self._keep += (cached, kv_start, kv_len)
 
-    def run(self, x, y, ln1, wqkv, wo, ln2, wgu, wd, *, kc=None, vc=None, out_rows=None, fp8=None, fp8_max_rows=0):
+    def run(self, x, y, ln1, wqkv, wo, ln2, wgu, wd, *, kc=None, vc=None, out_rows=None, fp8=None, fp8_max_rows=0, ke=None, ve=None):
         """``fp8``: None, or the (e4m3, exponents) pairs of wqkv, wo, wgu, wd (``Fp8Weights.view``); each GEMM with at most
-        ``fp8_max_rows`` rows then streams its pair through nv_gemm_fp8w_bf16 (same bits as the bf16 weights W')."""
+        ``fp8_max_rows`` rows then streams its pair through nv_gemm_fp8w_bf16 (same bits as the bf16 weights W').
+        ``ke`` / ``ve``: the row exponents of an fp8 cache (cache mode 3, kc / vc then hold its e4m3 bytes)."""
         a = self.args
         pairs = fp8 if fp8 is not None else ((None, None),) * 4
         (a.wqkv_q, a.wqkv_e), (a.wo_q, a.wo_e), (a.wgu_q, a.wgu_e), (a.wd_q, a.wd_e) = \
@@ -618,6 +667,10 @@ class LayerRunner:
         a.ln1, a.wqkv, a.wo, a.ln2, a.wgu, a.wd = ln1.data_ptr(), wqkv.data_ptr(), wo.data_ptr(), ln2.data_ptr(), wgu.data_ptr(), wd.data_ptr()
         a.kcache = kc.data_ptr() if kc is not None else None
         a.vcache = vc.data_ptr() if vc is not None else None
+        if a.kv_mode == 3:
+            _fp8_kv(kc, vc, ke, ve, "LayerRunner.run")
+        a.kexp = ke.data_ptr() if ke is not None else None
+        a.vexp = ve.data_ptr() if ve is not None else None
         if out_rows is not None:
             a.out_rows, a.R = out_rows.data_ptr(), out_rows.numel()
         else:
