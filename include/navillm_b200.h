@@ -107,6 +107,13 @@ int nv_attn_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const vo
 int nv_attn_fwd_kv(const void* q, int64_t ldq, const void* kcache, int64_t ldk, const void* vcache, int64_t ldv, void* o,
                    int64_t ldo, float* lse, const int* cu_seqlens, const int* kv_start, const int* kv_len, int B, int Tq,
                    int Tkv, int H, int head_dim, int total_qblocks, float scale, void* stream);
+/* nv_attn_fwd_kv over an fp8 cache in the format of nv_kv_store_prefill_fp8 below (no reference counterpart for the number
+ * format): kq / vq e4m3 [Tkv, H*128] with dense rows, kexp / vexp int8 [Tkv, H].  The same kernel with the e4m3 tiles widened
+ * to bf16 in shared memory, so the output is bit for bit nv_attn_fwd_kv's on bf16 caches holding K' / V'.  Rows past kv_len
+ * must widen to finite values (a zeroed cache or rows the store kernels wrote).  head_dim 128, 16-byte aligned kq / vq. */
+int nv_attn_fwd_kv_fp8(const void* q, int64_t ldq, const void* kq, const void* vq, const void* kexp, const void* vexp, void* o,
+                       int64_t ldo, float* lse, const int* cu_seqlens, const int* kv_start, const int* kv_len, int B, int Tq,
+                       int Tkv, int H, int head_dim, int total_qblocks, float scale, void* stream);
 int nv_attn_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, const void* o,
                 int64_t ldo, const void* dout, int64_t lddo, const float* lse, float* dvec, void* dq, int64_t lddq,
                 void* dk, int64_t lddk, void* dv, int64_t lddv, const int* cu_seqlens, int B, int T, int H, int head_dim,
@@ -201,6 +208,10 @@ int nv_decode_rope_kv(void* qkv, int64_t ld, const int* lens, const void* cos_t,
  * holds, then attend from the new rows over cached + new keys (nv_attn_fwd_kv). */
 int nv_kv_store_suffix(const void* qkv, int64_t ld, const int* cu_seqlens, const int* cached, void* kcache, void* vcache,
                        int B, int T, int Smax, int HD, void* stream);
+/* nv_kv_store_suffix into an fp8 cache (format: nv_kv_store_prefill_fp8 below): every stored (token, head) row is quantized,
+ * the bytes and exponents nv_quantize_fp8_rows gives for that row.  Rows at p >= Smax are dropped. */
+int nv_kv_store_suffix_fp8(const void* qkv, int64_t ld, const int* cu_seqlens, const int* cached, void* kq, void* vq, void* kexp,
+                           void* vexp, int B, int T, int Smax, int H, void* stream);
 int nv_decode_attn(const void* q, int64_t ldq, const void* kcache, const void* vcache, const int* lens, void* out,
                    int64_t ldo, int B, int Smax, int H, int head_dim, float scale, void* stream);
 /* nv_decode_rope_kv + nv_decode_attn in one launch (qkv pre-RoPE, not modified; k / v appended at row lens[b]). */
@@ -263,8 +274,9 @@ int nv_adamw_flat(void* p, void* g, void* m, void* v, int64_t n, int is_bf16, fl
  * bottleneck.  kv_mode 0: plain self-attention over the packed rows; 1: also store post-RoPE K/V of the rows in the caches
  * (prefill of generate); 2: the rows are suffixes of sequences whose prefixes are cached (cached / kv_start / kv_len as in
  * nv_kv_store_suffix / nv_attn_fwd_kv); 3: prefill of generate() into an fp8 cache (nv_kv_store_prefill_fp8: kcache / vcache
- * hold e4m3 bytes, kexp / vexp the row exponents; the layer's own attention reads the unrounded K, V).  out_rows (nullable,
- * R rows): only these rows are produced (last layer). */
+ * hold e4m3 bytes, kexp / vexp the row exponents; the layer's own attention reads the unrounded K, V); 4: kv_mode 2 over an
+ * fp8 prefix cache (nv_kv_store_suffix_fp8 + nv_attn_fwd_kv_fp8: the new rows attend over their own rounded K', V' too).
+ * out_rows (nullable, R rows): only these rows are produced (last layer). */
 typedef struct nv_layer_args {
   const void* x;            /* [T, D] bf16 residual stream in */
   void* y;                  /* [R or T, D] bf16 residual stream out */
@@ -280,7 +292,7 @@ typedef struct nv_layer_args {
   const void* wqkv_q; const void* wqkv_e; const void* wo_q; const void* wo_e;
   const void* wgu_q; const void* wgu_e; const void* wd_q; const void* wd_e;
   int fp8_max_rows;
-  void* kexp; void* vexp;   /* kv_mode 3: int8 row exponents [B, Smax, H] of the fp8 caches */
+  void* kexp; void* vexp;   /* kv_mode 3, 4: int8 row exponents [B, Smax, H] of the fp8 caches */
 } nv_layer_args;
 int nv_layer_args_size(void);                           /* sizeof(nv_layer_args): bindings check their mirror against it */
 int64_t nv_llama_layer_ws_bytes(int T, int R, int D, int F);

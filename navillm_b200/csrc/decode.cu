@@ -7,8 +7,9 @@
 // over it with 128-bit coalesced loads, and the step has static shapes so the host can replay it as a CUDA
 // graph (sequence lengths live in device memory).
 //
-// Opt-in fp8 cache (nv_kv_store_prefill_fp8, nv_decode_attn_rope_fp8): the same layout in e4m3 bytes plus one int8 exponent
-// per (sequence, position, head) row of 128 elements, quantized with the weight format of nv_fp8.cuh as rows are stored.
+// Opt-in fp8 cache (nv_kv_store_prefill_fp8, nv_decode_attn_rope_fp8, nv_kv_store_suffix_fp8): the same layout in e4m3 bytes
+// plus one int8 exponent per (sequence, position, head) row of 128 elements, quantized with the weight format of nv_fp8.cuh as
+// rows are stored.
 #include <type_traits>
 
 #include "nv_common.cuh"
@@ -29,10 +30,12 @@ __device__ __forceinline__ void unpack8q(const uint2& u, int e, float (&f)[8]) {
   fp8x4_to_f32x4(u.y, s, f + 4);
 }
 
-// fp8 twin of kv_store_prefill_kernel (offs = 0): a half-warp owns one (token, head) row of K and of V; 16 lanes x 8 elements.
-// Same packing and the same drop of rows at p >= Smax.  Each row's amax, exponent and bytes follow quantize_fp8_rows_kernel.
+// fp8 twin of kv_store_prefill_kernel: a half-warp owns one (token, head) row of K and of V; 16 lanes x 8 elements.
+// Same packing (offs: rows already cached per sequence, or null) and the same drop of rows at p >= Smax.  Each row's amax,
+// exponent and bytes follow quantize_fp8_rows_kernel.
 __global__ void __launch_bounds__(256) kv_store_prefill_fp8_kernel(const __nv_bfloat16* __restrict__ qkv, int64_t ld,
-                                                                   const int* __restrict__ cu, uint8_t* __restrict__ kq,
+                                                                   const int* __restrict__ cu, const int* __restrict__ offs,
+                                                                   uint8_t* __restrict__ kq,
                                                                    uint8_t* __restrict__ vq, int8_t* __restrict__ ke,
                                                                    int8_t* __restrict__ ve, int B, int Smax, int H) {
   const int HD = H * 128;
@@ -46,7 +49,7 @@ __global__ void __launch_bounds__(256) kv_store_prefill_fp8_kernel(const __nv_bf
     const int t = live ? (int)(r / H) : 0, h = live ? (int)(r % H) : 0;
     int b = 0;
     while (b + 1 < B && cu[b + 1] <= t) ++b;
-    const int p = t - cu[b];
+    const int p = t - cu[b] + (offs && live ? offs[b] : 0);
     uint4 k = make_uint4(0, 0, 0, 0), v = k;
     if (live) {
       k = *reinterpret_cast<const uint4*>(qkv + (int64_t)t * ld + HD + h * 128 + hl * 8);
@@ -778,7 +781,27 @@ int nv_kv_store_prefill_fp8(const void* qkv, int64_t ld, const int* cu_seqlens, 
   int grid = (int)((warps + 7) / 8);
   const int cap = sm_count() * 16;
   if (grid > cap) grid = cap;
-  kv_store_prefill_fp8_kernel<<<grid, 256, 0, S_(stream)>>>(CBF(qkv), ld, cu_seqlens, reinterpret_cast<uint8_t*>(kq),
+  kv_store_prefill_fp8_kernel<<<grid, 256, 0, S_(stream)>>>(CBF(qkv), ld, cu_seqlens, nullptr, reinterpret_cast<uint8_t*>(kq),
+                                                            reinterpret_cast<uint8_t*>(vq), reinterpret_cast<int8_t*>(kexp),
+                                                            reinterpret_cast<int8_t*>(vexp), B, Smax, H);
+  NV_LAUNCH_CHECK();
+  return NV_OK;
+}
+
+// nv_kv_store_suffix into an fp8 cache: the new rows of sequence b go after its cached[b] rows, each stored (token, head) row
+// quantized as nv_kv_store_prefill_fp8 quantizes it.
+int nv_kv_store_suffix_fp8(const void* qkv, int64_t ld, const int* cu_seqlens, const int* cached, void* kq, void* vq, void* kexp,
+                           void* vexp, int B, int T, int Smax, int H, void* stream) {
+  NV_REQUIRE(B >= 0 && T >= 0 && Smax > 0 && H > 0, "nv_kv_store_suffix_fp8: bad sizes (B=%d T=%d Smax=%d H=%d)", B, T, Smax, H);
+  if (T == 0 || B == 0) return NV_OK;
+  NV_REQUIRE(qkv && cu_seqlens && cached && kq && vq && kexp && vexp, "nv_kv_store_suffix_fp8: null argument");
+  NV_REQUIRE((ld & 7) == 0 && ((uintptr_t)qkv & 15) == 0 && ((uintptr_t)kq & 7) == 0 && ((uintptr_t)vq & 7) == 0,
+             "nv_kv_store_suffix_fp8: alignment (ld %% 8 == 0, 16-byte qkv, 8-byte caches)");
+  const int64_t warps = ((int64_t)T * H + 1) / 2;
+  int grid = (int)((warps + 7) / 8);
+  const int cap = sm_count() * 16;
+  if (grid > cap) grid = cap;
+  kv_store_prefill_fp8_kernel<<<grid, 256, 0, S_(stream)>>>(CBF(qkv), ld, cu_seqlens, cached, reinterpret_cast<uint8_t*>(kq),
                                                             reinterpret_cast<uint8_t*>(vq), reinterpret_cast<int8_t*>(kexp),
                                                             reinterpret_cast<int8_t*>(vexp), B, Smax, H);
   NV_LAUNCH_CHECK();

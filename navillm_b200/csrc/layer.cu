@@ -79,6 +79,11 @@ extern "C" int nv_llama_layer_infer(const nv_layer_args* a, void* stream) {
     STEP(nv_kv_store_suffix(qkv, 3 * (int64_t)D, a->cu_seqlens, a->cached, a->kcache, a->vcache, a->B, T, a->Smax, D, stream));
     STEP(nv_attn_fwd_kv(qkv, 3 * (int64_t)D, a->kcache, D, a->vcache, D, ao, D, nullptr, a->cu_seqlens, a->kv_start, a->kv_len, a->B,
                         T, a->Tkv, H, 128, a->total_qblocks, a->scale, stream));
+  } else if (a->kv_mode == 4) {     // ... over an fp8 cache: the new rows are quantized as they are stored, then read back
+    STEP(nv_kv_store_suffix_fp8(qkv, 3 * (int64_t)D, a->cu_seqlens, a->cached, a->kcache, a->vcache, a->kexp, a->vexp, a->B, T, a->Smax,
+                                H, stream));
+    STEP(nv_attn_fwd_kv_fp8(qkv, 3 * (int64_t)D, a->kcache, a->vcache, a->kexp, a->vexp, ao, D, nullptr, a->cu_seqlens, a->kv_start,
+                            a->kv_len, a->B, T, a->Tkv, H, 128, a->total_qblocks, a->scale, stream));
   } else {
     if (a->kv_mode == 1)            // prefill of generate(): post-RoPE K, V also go to the cache
       STEP(nv_kv_store_prefill(qkv, 3 * (int64_t)D, a->cu_seqlens, a->kcache, a->vcache, a->B, T, a->Smax, D, stream));

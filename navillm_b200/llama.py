@@ -495,23 +495,29 @@ class LlamaCore:
         pos: their rotary positions, cu / q_lens: packing of the new rows, caches [B, Smax, D] (zero-initialised),
         cached / kv_start / kv_len: int32 [B] on the device (rows already cached, first cache row of the sequence,
         cached + new).  The new rows' K/V are appended to the cache; returns the residual stream ([Tn, D], or
-        [R, D] with ``out_rows``) before the final RMSNorm."""
+        [R, D] with ``out_rows``) before the final RMSNorm.
+
+        The caches may also be fp8 ``(e4m3 [B, Smax, D], int8 exponents [B, Smax, H])`` pairs per layer (``is_fp8_kv``): the
+        new rows are rounded as they are stored and the attention reads the rounded rows, theirs included."""
         d = self.d
         H, D = d.n_heads, d.hidden
         B, T = len(q_lens), x.shape[0]
         last = d.n_layers - 1
         fused = self.fused_epilogues and T >= 1024 and d.inter % 128 == 0 and d.hidden % 256 == 0
         f8 = self.fp8_for_inference()
+        fp8_kv = is_fp8_kv(kc)
+        Bc, Smax = (kc[0][0] if fp8_kv else kc[0]).shape[:2]
         if self.LAYER_CALL and not fused and d.head_dim == 128:
             R = 0 if out_rows is None else out_rows.numel()
             run = ops.LayerRunner(T, D, d.inter, H, d.rms_eps, pos, self.cos, self.sin, cu, B, ops._qblocks(q_lens), R=R, device=x.device)
-            run.set_cache_mode(2, kc[0].shape[1], kc[0].shape[0] * kc[0].shape[1], cached, kv_start, kv_len)
+            run.set_cache_mode(4 if fp8_kv else 2, Smax, Bc * Smax, cached, kv_start, kv_len)
             bufs = [torch.empty_like(x), torch.empty_like(x)]
             for l, lyr in enumerate(self.model.layers):
                 pruned = out_rows is not None and l == last
                 y = torch.empty((R, D), dtype=bf16, device=x.device) if pruned else bufs[l & 1]
+                (kl, ke), (vl, ve) = (kc[l], vc[l]) if fp8_kv else ((kc[l], None), (vc[l], None))
                 run.run(x, y, lyr.input_layernorm.weight.data, self.wqkv[l], self.wo[l], lyr.post_attention_layernorm.weight.data,
-                        self.wgu[l], self.wd[l], kc=kc[l], vc=vc[l], out_rows=out_rows if pruned else None,
+                        self.wgu[l], self.wd[l], kc=kl, vc=vl, ke=ke, ve=ve, out_rows=out_rows if pruned else None,
                         fp8=self._fp8_layer(f8, l), fp8_max_rows=FP8_MAX_ROWS)
                 x = y
             return x
@@ -523,8 +529,13 @@ class LlamaCore:
             else:
                 qkv = self._linear(xn, self.wqkv[l], w8[0])
                 ops.rope_(qkv, pos, self.cos, self.sin, 2 * H, d.head_dim)
-            ops.kv_store_suffix(qkv, cu, cached, kc[l], vc[l], B, T)
-            ao = ops.attn_fwd_kv(qkv[:, :D], kc[l], vc[l], cu, q_lens, kv_start, kv_len, H)
+            if fp8_kv:
+                (kq, ke), (vq, ve) = kc[l], vc[l]
+                ops.kv_store_suffix_fp8(qkv, cu, cached, kq, vq, ke, ve, B, T)
+                ao = ops.attn_fwd_kv_fp8(qkv[:, :D], kq, vq, ke, ve, cu, q_lens, kv_start, kv_len, H)
+            else:
+                ops.kv_store_suffix(qkv, cu, cached, kc[l], vc[l], B, T)
+                ao = ops.attn_fwd_kv(qkv[:, :D], kc[l], vc[l], cu, q_lens, kv_start, kv_len, H)
             xin = x
             if out_rows is not None and l == last:
                 ao = ops.gather_rows(ao, out_rows)

@@ -121,18 +121,42 @@ class PrefixKVCache:
     the cos/sin tables at different absolute positions (tests/test_prefix_reuse_gpu.py states the tolerance).
 
     Contract: rows are identified by batch index; the <hist> vectors of a row are append-only across steps (the
-    reference's hist_vis lists are); call ``reset()`` when a new episode starts in a row."""
+    reference's hist_vis lists are); call ``reset()`` when a new episode starts in a row.
 
-    def __init__(self, lm: "ModifiedLlamaForCausalLM", batch_size: int, max_len: int = 2048):
+    ``kv_dtype="fp8"`` (opt-in; default ``"bf16"``) stores the cache in the fp8 format of ``set_kv_cache_dtype("fp8")``
+    (include/navillm_b200.h): per layer, e4m3 bytes [B, max_len, D] plus one int8 power-of-two exponent per (row, position,
+    head), half the memory of the bf16 cache plus 1/256 (``nbytes``), which lets a rollout run a larger batch at the same
+    ``max_len``.  Every suffix step attends over the cache, so the step's new rows read their own K / V rounded to e4m3 as
+    well (K' / V'); generate()'s prefill, by contrast, attends over the unrounded K / V of the prompt.  The format is the
+    caller's choice: it does not follow the model's ``kv_cache_dtype``.  Works with and without ``quantize_weights_fp8()``."""
+
+    def __init__(self, lm: "ModifiedLlamaForCausalLM", batch_size: int, max_len: int = 2048, kv_dtype: str = "bf16"):
+        if kv_dtype not in ("bf16", "fp8"):
+            raise ValueError(f"PrefixKVCache: kv_dtype must be 'bf16' or 'fp8' (got {kv_dtype!r})")
         lm._ensure()
         dev, d = lm._device(), lm.dims
-        self.B, self.max_len = batch_size, max_len
+        self.B, self.max_len, self.kv_dtype = batch_size, max_len, kv_dtype
         # zero-initialised: rows past a sequence's length are masked in the attention kernel but must stay finite
-        self.kc = [torch.zeros((batch_size, max_len, d.hidden), dtype=bf16, device=dev) for _ in range(d.n_layers)]
-        self.vc = [torch.zeros((batch_size, max_len, d.hidden), dtype=bf16, device=dev) for _ in range(d.n_layers)]
+        if kv_dtype == "fp8":
+            if d.head_dim != 128:
+                raise ValueError(f"PrefixKVCache: the fp8 cache needs head_dim 128 (got {d.head_dim})")
+
+            def layer():
+                return (torch.zeros((batch_size, max_len, d.hidden), dtype=torch.float8_e4m3fn, device=dev),
+                        torch.zeros((batch_size, max_len, d.n_heads), dtype=torch.int8, device=dev))
+        else:
+            def layer():
+                return torch.zeros((batch_size, max_len, d.hidden), dtype=bf16, device=dev)
+        self.kc = [layer() for _ in range(d.n_layers)]
+        self.vc = [layer() for _ in range(d.n_layers)]
         self.ids: List[np.ndarray] = [np.zeros(0, dtype=np.int64) for _ in range(batch_size)]
         self.off: List[Optional[int]] = [None] * batch_size
         self.stats = {"steps": 0, "tokens": 0, "tokens_encoded": 0}
+
+    @property
+    def nbytes(self) -> int:
+        """Device bytes of the K and V caches of all layers (exponents included)."""
+        return sum(t.nbytes for c in self.kc + self.vc for t in (c if isinstance(c, tuple) else (c,)))
 
     def reset(self, rows=None) -> None:
         for b in (range(self.B) if rows is None else rows):

@@ -569,6 +569,46 @@ def kv_store_prefill_fp8(qkv, cu, kq, vq, ke, ve, B, T):
                                               i32(Smax), i32(HD // 128), stream_ptr()), "nv_kv_store_prefill_fp8")
 
 
+def kv_store_suffix_fp8(qkv, cu, cached, kq, vq, ke, ve, B, T):
+    """``kv_store_suffix`` into an fp8 cache: the new rows of sequence b go after its ``cached[b]`` rows, each (token, head)
+    row of K and V rounded to e4m3 with its own power-of-two exponent, the bytes ``quantize_fp8_`` writes for that row."""
+    _, Smax, HD = _fp8_kv(kq, vq, ke, ve, "kv_store_suffix_fp8")
+    if qkv.dtype != bf16 or qkv.stride(1) != 1 or qkv.shape[1] < 3 * HD:
+        raise ValueError(f"kv_store_suffix_fp8: qkv bf16 [T, >= {3 * HD}] rows expected (got {qkv.dtype} {tuple(qkv.shape)})")
+    for name, t, n in (("cu_seqlens", cu, B + 1), ("cached", cached, B)):
+        if t.dtype != torch.int32 or t.numel() != n or not t.is_cuda:
+            raise ValueError(f"kv_store_suffix_fp8: {name} int32 [{n}] on the device expected (got {t.dtype} {tuple(t.shape)})")
+    check(_lib.load().nv_kv_store_suffix_fp8(ptr(qkv), i64(qkv.stride(0)), ptr(cu), ptr(cached), ptr(kq), ptr(vq), ptr(ke), ptr(ve),
+                                             i32(B), i32(T), i32(Smax), i32(HD // 128), stream_ptr()), "nv_kv_store_suffix_fp8")
+
+
+def attn_fwd_kv_fp8(q: torch.Tensor, kq, vq, ke, ve, cu_q: torch.Tensor, q_lens, kv_start: torch.Tensor, kv_len: torch.Tensor,
+                    n_heads: int, *, out: torch.Tensor | None = None, scale: float | None = None):
+    """``attn_fwd_kv`` over an fp8 cache (kq / vq float8_e4m3fn [B, Smax, H*128], ke / ve int8 [B, Smax, H]): bit for bit
+    ``attn_fwd_kv`` on bf16 caches holding the rounded rows K' / V'.  Rows past kv_len must widen to finite values (a zeroed
+    cache, or rows a store wrote).  Returns o [Tq, H*128] bf16."""
+    Bc, Smax, HD = _fp8_kv(kq, vq, ke, ve, "attn_fwd_kv_fp8")
+    B = len(q_lens)
+    Tq = int(sum(int(l) for l in q_lens))
+    if HD != n_heads * 128 or q.dtype != bf16 or q.dim() != 2 or q.stride(1) != 1 or q.shape[1] < HD or q.shape[0] != Tq:
+        raise ValueError(f"attn_fwd_kv_fp8: q bf16 [{Tq}, >= {HD}] and {HD // 128} heads expected "
+                         f"(got {q.dtype} {tuple(q.shape)}, {n_heads} heads)")
+    for name, t, n in (("cu_q", cu_q, B + 1), ("kv_start", kv_start, B), ("kv_len", kv_len, B)):
+        if t.dtype != torch.int32 or t.numel() != n or not t.is_cuda:
+            raise ValueError(f"attn_fwd_kv_fp8: {name} int32 [{n}] on the device expected (got {t.dtype} {tuple(t.shape)})")
+    if out is None:
+        out = torch.empty((Tq, HD), dtype=bf16, device=q.device)
+    if out.dtype != bf16 or out.stride(1) != 1 or tuple(out.shape) != (Tq, HD):
+        raise ValueError(f"attn_fwd_kv_fp8: out bf16 [{Tq}, {HD}] expected (got {out.dtype} {tuple(out.shape)})")
+    if scale is None:
+        scale = 128 ** -0.5
+    check(_lib.load().nv_attn_fwd_kv_fp8(ptr(q), i64(q.stride(0)), ptr(kq), ptr(vq), ptr(ke), ptr(ve), ptr(out), i64(out.stride(0)),
+                                         ptr(None), ptr(cu_q), ptr(kv_start), ptr(kv_len), i32(B), i32(Tq), i32(Bc * Smax),
+                                         i32(n_heads), i32(128), i32(_qblocks(q_lens)), f32(scale), stream_ptr()),
+          "nv_attn_fwd_kv_fp8")
+    return out
+
+
 def decode_attn_rope_fp8(qkv, lens, cos_t, sin_t, kq, vq, ke, ve, n_heads, *, out=None, scale=None):
     """``decode_attn_rope`` over an fp8 cache: the rotated k and the v of the new token are rounded to e4m3 (one exponent per
     head row) as they are appended at row lens[b]; the output equals ``decode_attn_rope`` on a bf16 cache holding the rounded
@@ -657,7 +697,7 @@ class LayerRunner:
     def run(self, x, y, ln1, wqkv, wo, ln2, wgu, wd, *, kc=None, vc=None, out_rows=None, fp8=None, fp8_max_rows=0, ke=None, ve=None):
         """``fp8``: None, or the (e4m3, exponents) pairs of wqkv, wo, wgu, wd (``Fp8Weights.view``); each GEMM with at most
         ``fp8_max_rows`` rows then streams its pair through nv_gemm_fp8w_bf16 (same bits as the bf16 weights W').
-        ``ke`` / ``ve``: the row exponents of an fp8 cache (cache mode 3, kc / vc then hold its e4m3 bytes)."""
+        ``ke`` / ``ve``: the row exponents of an fp8 cache (cache modes 3 and 4, kc / vc then hold its e4m3 bytes)."""
         a = self.args
         pairs = fp8 if fp8 is not None else ((None, None),) * 4
         (a.wqkv_q, a.wqkv_e), (a.wo_q, a.wo_e), (a.wgu_q, a.wgu_e), (a.wd_q, a.wd_e) = \
@@ -667,7 +707,7 @@ class LayerRunner:
         a.ln1, a.wqkv, a.wo, a.ln2, a.wgu, a.wd = ln1.data_ptr(), wqkv.data_ptr(), wo.data_ptr(), ln2.data_ptr(), wgu.data_ptr(), wd.data_ptr()
         a.kcache = kc.data_ptr() if kc is not None else None
         a.vcache = vc.data_ptr() if vc is not None else None
-        if a.kv_mode == 3:
+        if a.kv_mode in (3, 4):
             _fp8_kv(kc, vc, ke, ve, "LayerRunner.run")
         a.kexp = ke.data_ptr() if ke is not None else None
         a.vexp = ve.data_ptr() if ve is not None else None

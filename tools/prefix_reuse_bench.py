@@ -6,9 +6,19 @@ no_grad twice - from scratch (what the reference does, tasks/agents/mp3d_agent.p
 and the two fuse_logits are compared.  Prints one JSON line.
 
     python tools/prefix_reuse_bench.py [--batch 8] [--steps 16] [--hist0 0]
+
+--kv fp8 compares the bf16 PrefixKVCache with PrefixKVCache(kv_dtype="fp8") instead (max_len 2048, bf16 weights):
+(i) the suffix attention alone, nv_attn_fwd_kv against nv_attn_fwd_kv_fp8, H = 32, 128 new rows per sequence over
+512 / 1024 / 2048 cached rows, caches rotated over copies larger than L2, arms alternated, outputs checked bit for bit;
+(ii) the prefix-cached rollout in ms/step for each --kv-batches x --kv-hist0, both caches in lock-step with the arm order
+alternated per step, and the cache GiB of each; a bf16 cache that cannot be allocated is reported as such; (iii) the GPU
+name, power limit and SM clocks, read in the same run.
+
+    python tools/prefix_reuse_bench.py --kv fp8 --steps 5 [--kv-batches 8,32,64] [--kv-hist0 0,40]
 """
 import argparse
 import json
+import subprocess
 import sys
 from pathlib import Path
 
@@ -55,9 +65,15 @@ def main():
     ap.add_argument("--json", type=str, default="")
     ap.add_argument("--fp8", action="store_true", help="quantize the weights and time the prefix-cached rollout with the fp8 copy "
                                                        "against bf16 on the same weights (bitwise-equal fuse_logits required)")
+    ap.add_argument("--kv", choices=["bf16", "fp8"], default="bf16",
+                    help="fp8: time the bf16 prefix cache against PrefixKVCache(kv_dtype='fp8') (kernel and rollout)")
+    ap.add_argument("--kv-batches", type=str, default="8,32,64")
+    ap.add_argument("--kv-hist0", type=str, default="0,40")
     a = ap.parse_args()
     from navillm_b200.modified_lm import PrefixKVCache
     dev = torch.device("cuda:0")
+    if a.kv == "fp8":
+        return kv_compare(a, dev)
     model = bench.build_model(dev).eval()
     if a.fp8:
         return fp8_rollout(model, a, dev)
@@ -152,6 +168,169 @@ def fp8_rollout(model, a, dev):
         Path(a.json).write_text(json.dumps({"summary": res, "steps": rows}, indent=1))
     if not equal:
         raise SystemExit("prefix_reuse_bench --fp8: fuse_logits differ between the fp8 copy and bf16")
+
+
+def gpu_clocks() -> dict:
+    """Card name, power limit and SM clocks (maximum and current) of GPU 0."""
+    info = bench.gpu_info(0)
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=clocks.max.sm,clocks.sm", "--format=csv,noheader,nounits", "-i", "0"],
+                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
+        info["sm_clock_max_mhz"], info["sm_clock_mhz"] = (float(x) for x in out.split(","))
+    except Exception:
+        pass
+    return info
+
+
+def suffix_attn_table(dev, iters=50, B=8, H=32, q=128, cached=(512, 1024, 2048)):
+    """One layer's suffix attention: B sequences of q new rows over `cached` rows, bf16 cache (holding K' / V') against the
+    fp8 cache, launched straight through the C ABI (arguments prepared once), caches rotated over copies larger than L2."""
+    from navillm_b200 import _lib, ops
+    lib = _lib.load()
+    g = torch.Generator(device=dev).manual_seed(0)
+    HD = H * 128
+    rows = []
+    for c in cached:
+        Smax = c + q
+        per_copy = 2 * B * Smax * HD * 2
+        ncopy = max(2, -(-200 * 2 ** 20 // per_copy))
+        qkv = torch.randn(B * q, 3 * HD, device=dev, generator=g).to(torch.bfloat16)
+        cu = torch.arange(B + 1, dtype=torch.int32, device=dev) * q
+        kv_start = torch.arange(B, dtype=torch.int32, device=dev) * Smax
+        kv_len = torch.full((B,), c + q, dtype=torch.int32, device=dev)
+        out16 = torch.empty(B * q, HD, dtype=torch.bfloat16, device=dev)
+        out8 = torch.empty_like(out16)
+        c16, c8 = [], []
+        for _ in range(ncopy):
+            kc = torch.randn(B, Smax, HD, device=dev, generator=g).to(torch.bfloat16)
+            vc = torch.randn(B, Smax, HD, device=dev, generator=g).to(torch.bfloat16)
+            kq, ke = _round_cache(kc)
+            vq, ve = _round_cache(vc)
+            c16.append((kc, vc))
+            c8.append((kq, vq, ke, ve))
+        ops.attn_fwd_kv(qkv[:, :HD], *c16[0], cu, [q] * B, kv_start, kv_len, H, out=out16)
+        ops.attn_fwd_kv_fp8(qkv[:, :HD], *c8[0], cu, [q] * B, kv_start, kv_len, H, out=out8)
+        torch.cuda.synchronize()
+        bitwise = torch.equal(out16.view(torch.int16), out8.view(torch.int16))
+        P, i64, i32 = _lib.ptr, _lib.i64, _lib.i32
+        common = (P(out16), i64(HD), None, P(cu), P(kv_start), P(kv_len), i32(B), i32(B * q), i32(B * Smax), i32(H), i32(128),
+                  i32(B), _lib.f32(128 ** -0.5))
+        a16 = [(P(qkv), i64(3 * HD), P(k), i64(HD), P(v), i64(HD)) + common for k, v in c16]
+        a8 = [(P(qkv), i64(3 * HD), P(kq), P(vq), P(ke), P(ve)) + common for kq, vq, ke, ve in c8]
+        stream = _lib.stream_ptr()
+        f16 = lambda i: lib.nv_attn_fwd_kv(*a16[i % ncopy], stream)
+        f8 = lambda i: lib.nv_attn_fwd_kv_fp8(*a8[i % ncopy], stream)
+        for i in range(5):
+            f16(i); f8(i)
+        torch.cuda.synchronize()
+        t = {"bf16": [], "fp8": []}
+        for rep in range(6):
+            for kind, f in (("bf16", f16), ("fp8", f8)) if rep % 2 == 0 else (("fp8", f8), ("bf16", f16)):
+                st, en = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                st.record()
+                for i in range(iters):
+                    rc = f(i)
+                en.record()
+                torch.cuda.synchronize()
+                assert rc == 0, kind
+                t[kind].append(st.elapsed_time(en) / iters)
+        keys = B * (c + q)
+        io = B * q * HD * 2 * 2                                   # q in, o out
+        r = {"B": B, "H": H, "q_rows": q, "cached_rows": c, "fp8_bitwise_bf16_on_rounded": bool(bitwise)}
+        for kind, by in (("bf16", keys * HD * 2 * 2 + io), ("fp8", keys * HD * 2 + keys * H * 2 + io)):
+            us = 1e3 * float(np.median(t[kind]))
+            r[f"{kind}_us"] = round(us, 2)
+            r[f"{kind}_GBps"] = round(by / us / 1e3, 1)
+        r["speedup"] = round(r["bf16_us"] / r["fp8_us"], 3)
+        rows.append(r)
+        print(json.dumps(r), flush=True)
+        del c16, c8
+        torch.cuda.empty_cache()
+    return rows
+
+
+def _round_cache(c):
+    """quantize_fp8_ on the [rows, 128] view of a bf16 cache: c becomes K' in place; returns (e4m3 bytes, exponents)."""
+    from navillm_b200 import ops
+    rows = c.view(-1, 128)
+    q = torch.empty(rows.shape, dtype=ops.fp8, device=c.device)
+    e = torch.empty(rows.shape[0], dtype=torch.int8, device=c.device)
+    ops.quantize_fp8_(rows, q, e)
+    return q.view(c.shape), e.view(*c.shape[:-1], c.shape[-1] // 128)
+
+
+def kv_rollout(model, dev, B, hist0, steps):
+    """The prefix-cached rollout with a bf16 and an fp8 PrefixKVCache in lock-step (arm order alternated per step)."""
+    from navillm_b200.modified_lm import PrefixKVCache
+    lm = model.lang_model
+    rng = np.random.RandomState(0)
+    g = torch.Generator().manual_seed(0)
+    D, G, n_cand = 4096, 64, 12
+    words = [f"w{i}" for i in range(5000)]
+    instr = [" ".join(words[i] for i in rng.randint(0, 5000, size=rng.randint(60, 100))) for _ in range(B)]
+    hist = [[torch.randn(D, generator=g).to(dev) for _ in range(hist0)] for _ in range(B)]
+    caches, res = {"fp8": PrefixKVCache(lm, batch_size=B, max_len=2048, kv_dtype="fp8")}, {"B": B, "hist0": hist0}
+    try:
+        caches["bf16"] = PrefixKVCache(lm, batch_size=B, max_len=2048)
+    except torch.cuda.OutOfMemoryError:
+        res["bf16"] = "cache does not fit"
+    torch.cuda.empty_cache()
+    for k, c in caches.items():
+        res[f"{k}_cache_GiB"] = round(c.nbytes / 2 ** 30, 3)
+    to_dev = lambda b: {k: (v.to(dev) if torch.is_tensor(v) else v) for k, v in b.items()}
+    ev = lambda: torch.cuda.Event(enable_timing=True)
+    rows, max_rel = [], 0.0
+    with torch.no_grad():
+        for t in range(hist0, hist0 + steps):
+            batch = to_dev(make_step(rng, g, B, t, instr, n_cand, D, G))
+            batch["hist_vis"] = [list(h) for h in hist]
+            out, ms, enc = {}, {}, 0
+            order = [k for k in (("fp8", "bf16") if t % 2 == 0 else ("bf16", "fp8")) if k in caches]
+            for mode in order:
+                e0, e1 = ev(), ev()
+                enc0 = caches[mode].stats["tokens_encoded"]
+                torch.manual_seed(t); e0.record()
+                out[mode] = model("navigation", dict(batch), prefix_cache=caches[mode])
+                e1.record(); torch.cuda.synchronize()
+                ms[mode], enc = e0.elapsed_time(e1), caches[mode].stats["tokens_encoded"] - enc0
+            if "bf16" in out:
+                r, c = out["bf16"]["fuse_logits"].float(), out["fp8"]["fuse_logits"].float()
+                fin = torch.isfinite(r)
+                max_rel = max(max_rel, ((r[fin] - c[fin]).abs().max() / r[fin].abs().max()).item())
+            rows.append(dict({"hist": t, "encoded_tokens": enc}, **{f"{k}_ms": v for k, v in ms.items()}))
+            src = out.get("bf16", out["fp8"])
+            for b in range(B):
+                hist[b].append(src["fuse_embeds"][b, 1 + (t % 3)].float())
+    timed = rows[1:] or rows                                   # the first step encodes whole prompts (and warms up)
+    n = len(timed)
+    res["encoded_tokens_per_step"] = sum(r["encoded_tokens"] for r in timed) / n
+    res["first_step_encoded_tokens"] = rows[0]["encoded_tokens"]
+    for k in caches:
+        res[f"{k}_ms_per_step"] = round(sum(r[f"{k}_ms"] for r in timed) / n, 2)
+        res[f"{k}_first_step_ms"] = round(rows[0][f"{k}_ms"], 2)
+    if "bf16" in caches:
+        res["speedup"] = round(res["bf16_ms_per_step"] / res["fp8_ms_per_step"], 3)
+        res["max_rel_logit_diff_fp8_vs_bf16_cache"] = max_rel
+    res["peak_allocated_GiB"] = round(torch.cuda.max_memory_allocated() / 2 ** 30, 2)
+    print(json.dumps(res), flush=True)
+    del caches
+    torch.cuda.empty_cache()
+    torch.cuda.reset_peak_memory_stats()
+    return res
+
+
+def kv_compare(a, dev):
+    res = {"gpu_before": gpu_clocks(), "suffix_attention": suffix_attn_table(dev)}
+    model = bench.build_model(dev).eval()
+    res["config"] = ("eval rollout with PrefixKVCache max_len 2048, 12 candidates, Vicuna-7B random init, bf16 weights, "
+                     f"no_grad, {a.steps} steps, the first one (whole prompts) reported apart")
+    res["weights_GiB"] = round(torch.cuda.memory_allocated() / 2 ** 30, 2)
+    res["rollouts"] = [kv_rollout(model, dev, int(B), int(h), a.steps)
+                       for h in a.kv_hist0.split(",") for B in a.kv_batches.split(",")]
+    res["gpu_after"] = gpu_clocks()
+    print(json.dumps(res), flush=True)
+    if a.json:
+        Path(a.json).write_text(json.dumps(res, indent=1))
 
 
 if __name__ == "__main__":
