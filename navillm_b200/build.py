@@ -28,7 +28,7 @@ NVCC_FLAGS = [
     "-O3", "-std=c++17", "-lineinfo", "--use_fast_math", "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr", "-Xptxas", "-v", "-DNDEBUG",
 ]
-# developer-only extra flags (e.g. NV_NVCC_EXTRA="-DNV_MBAR_TIMEOUT_CYCLES=1000000000")
+# developer-only extra flags (e.g. NV_NVCC_EXTRA="-DNV_MBAR_TIMEOUT_CYCLES=1000000000 -DNV_MBAR_TIMEOUT_REPORT")
 NVCC_FLAGS += os.environ.get("NV_NVCC_EXTRA", "").split()
 
 

@@ -18,6 +18,7 @@
 //   warps 0..7 (two warpgroups)  consumers: warpgroup w computes rows 64 w .. 64 w + 63 with m64nBLOCK_Nk16 wgmmas
 //                                straight from the shared-memory stages, one wgmma group in flight
 //   warp 8 (1 lane)              TMA producer: 128-byte-swizzled tiles, STAGES-deep mbarrier ring
+// The plain (EPI_PLAIN) 128 x 256 tile is gemm_bf16_wide below: 2-CTA clusters that share the B tile by TMA multicast.
 // Epilogue: the accumulators go through shared memory (the stage ring is free by then) so that each thread then owns
 // one output row and 32 consecutive columns at a time: 16-byte global stores, and the fused epilogues below see whole
 // rows (rotate-half pairs, the gate and up halves of SwiGLU, the per-head row sums of the attention backward).
@@ -93,11 +94,11 @@ struct GemmSmem {
 };
 
 __device__ __forceinline__ void tile_coords(uint32_t tile, uint32_t num_m, uint32_t num_n, uint32_t& m_blk,
-                                            uint32_t& n_blk) {
-  const uint32_t group_size = GEMM_GROUP_M * num_n;
+                                            uint32_t& n_blk, uint32_t group_m = GEMM_GROUP_M) {
+  const uint32_t group_size = group_m * num_n;
   const uint32_t g = tile / group_size;
-  const uint32_t first_m = g * GEMM_GROUP_M;
-  const uint32_t gm = min(num_m - first_m, GEMM_GROUP_M);
+  const uint32_t first_m = g * group_m;
+  const uint32_t gm = min(num_m - first_m, group_m);
   const uint32_t r = tile - g * group_size;
   m_blk = first_m + r % gm;
   n_blk = r / gm;
@@ -246,6 +247,9 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
     constexpr uint32_t B_KADV = B_MN ? (16 * 128) >> 4 : (16 * 2) >> 4;
     constexpr uint32_t A_LBO = A_MN ? GEMM_BLOCK_K * 128 : 0, B_LBO = B_MN ? GEMM_BLOCK_K * 128 : 0;
     uint32_t stage = 0, phase = 0, prev = 0;
+    // K > 0 (host check): without this ptxas keeps a zero-trip path that writes the accumulators outside the wgmma
+    // pipeline and serializes the wgmmas (warning C7515)
+    __builtin_assume(num_kb > 0);
     for (uint32_t kb = 0; kb < num_kb; ++kb) {
       mbar_wait(&full_bar[stage], phase);
       if constexpr (L::kFp8) mbar_wait(&cvt_bar[stage], phase);
@@ -497,6 +501,241 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, void* C, in
   return NV_OK;
 }
 
+// ================================ 128 x 256 tile: 2-CTA clusters sharing B ================================
+// The two CTAs of a cluster (ranks 0, 1) compute the M-adjacent tiles (2 mp + rank, n) of one tile pair, pairs in the
+// grouped raster order.  Per 64-deep k-block each CTA TMA-loads its own A tile and one half of the shared B tile,
+// multicast into the same stage offset of both CTAs: 32 KB from L2 per CTA instead of 48 KB.  Every CTA's full
+// barrier expects the whole 48 KB stage; a stage is refilled only after the consumer warpgroups of both CTAs released
+// it (each arrives on the empty barrier of both CTAs).  The partner of the last tile of an odd m-block count lies past
+// M: it loads its half of B and zero-filled A, and stores nothing.  The accumulator is rounded to bf16 and drained
+// through a 32 KB half-tile buffer in two passes.  Each tile still accumulates its k-blocks in one chain, in order,
+// with the m64n256k16 sequence of gemm_bf16_wgmma, so C is bit for bit the same.  Plain epilogue only: the fused
+// epilogues measured slower with this staging and stay on gemm_bf16_wgmma<256> (DESIGN.md §4).
+constexpr uint32_t WIDE_N = 256;
+constexpr uint32_t WIDE_STAGES = 4;
+constexpr uint32_t WIDE_CLUSTER = 2;
+
+struct WideSmem {
+  static constexpr uint32_t A_BYTES = GEMM_BLOCK_M * GEMM_BLOCK_K * 2;
+  static constexpr uint32_t B_BYTES = WIDE_N * GEMM_BLOCK_K * 2;
+  static constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr uint32_t STG_OFF = WIDE_STAGES * STAGE_BYTES;
+  static constexpr uint32_t STG_BYTES = GEMM_BLOCK_M * 128 * 2;           // bf16 [128 rows][128 columns]
+  static constexpr uint32_t BAR_OFF = STG_OFF + STG_BYTES;
+  static constexpr uint32_t DYN_BYTES = BAR_OFF + 2 * WIDE_STAGES * 8 + 1024;   // + slack for 1024-byte alignment
+  static_assert(DYN_BYTES <= 232448, "shared memory per block");
+};
+
+// Staging buffer: 16 chunks of 16 bytes (8 columns) per 256-byte row, chunk c of row r stored at chunk c ^ (r % 8):
+// the fragment writes (8 rows x 4 lanes) and the row reads (8 threads, one row each) are both conflict-free.
+__device__ __forceinline__ uint32_t stg_offset(uint32_t row, uint32_t chunk) {
+  return row * 256u + ((chunk ^ (row & 7u)) << 4);
+}
+// Pass p stages tile columns [64 p, 64 p + 64) in chunks 0..7 and [128 + 64 p, 128 + 64 p + 64) in chunks 8..15.
+// Returns the staged chunk of the accumulator's 8-column group i (tile columns 8 i ..), or -1 when pass p does not
+// hold it.
+__device__ __forceinline__ int stg_chunk(uint32_t i, uint32_t p) {
+  return ((i >> 3) & 1) == p ? int(i < 16 ? i - 8 * p : i - 8 - 8 * p) : -1;
+}
+// 32 staged columns (4 chunks from `chunk`) of row `row` as 16 packed bf16 pairs
+__device__ __forceinline__ void ld_stg32(uint32_t stg, uint32_t row, uint32_t chunk, uint32_t (&w)[16]) {
+#pragma unroll
+  for (uint32_t q = 0; q < 4; ++q) {
+    const uint4 x = lds128(stg + stg_offset(row, chunk + q));
+    w[4 * q] = x.x; w[4 * q + 1] = x.y; w[4 * q + 2] = x.z; w[4 * q + 3] = x.w;
+  }
+}
+
+// C[row, col .. col + 31] = w (+ addend), predicated on N
+__device__ __forceinline__ void store_plain32(const uint32_t (&w)[16], void* Cout, int64_t ldc, const __nv_bfloat16* addend,
+                                              int64_t ld_add, uint32_t row, uint32_t col, uint32_t N, bool do_add) {
+  if (col >= N) return;
+  __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(Cout) + static_cast<int64_t>(row) * ldc + col;
+  const __nv_bfloat16* add = do_add ? addend + static_cast<int64_t>(row) * ld_add + col : nullptr;
+  if (col + 32 <= N && (ldc & 7) == 0 && (!do_add || (ld_add & 7) == 0)) {
+#pragma unroll
+    for (uint32_t j = 0; j < 4; ++j) {
+      uint4 o = make_uint4(w[4 * j], w[4 * j + 1], w[4 * j + 2], w[4 * j + 3]);
+      if (do_add) {
+        const uint4 a = *reinterpret_cast<const uint4*>(add + 8 * j);
+        o.x = pack_bf16x2(bf16_lo(o.x) + bf16_lo(a.x), bf16_hi(o.x) + bf16_hi(a.x));
+        o.y = pack_bf16x2(bf16_lo(o.y) + bf16_lo(a.y), bf16_hi(o.y) + bf16_hi(a.y));
+        o.z = pack_bf16x2(bf16_lo(o.z) + bf16_lo(a.z), bf16_hi(o.z) + bf16_hi(a.z));
+        o.w = pack_bf16x2(bf16_lo(o.w) + bf16_lo(a.w), bf16_hi(o.w) + bf16_hi(a.w));
+      }
+      *reinterpret_cast<uint4*>(dst + 8 * j) = o;
+    }
+  } else {
+#pragma unroll
+    for (uint32_t j = 0; j < 32; ++j) {
+      if (col + j < N) {
+        float x = (j & 1) ? bf16_hi(w[j >> 1]) : bf16_lo(w[j >> 1]);
+        if (do_add) x = x + __bfloat162float(add[j]);
+        dst[j] = __float2bfloat16_rn(x);
+      }
+    }
+  }
+}
+
+template <bool A_MN, bool B_MN>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_bf16_wide(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+               void* __restrict__ Cout, int64_t ldc, const __nv_bfloat16* __restrict__ addend, int64_t ld_add,
+               uint32_t M, uint32_t N, uint32_t K, uint32_t flags) {
+  using L = WideSmem;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem_a = smem;
+  uint8_t* smem_b = smem + WIDE_STAGES * L::A_BYTES;
+  const uint32_t stg = smem_u32(smem + L::STG_OFF);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
+  uint64_t* empty_bar = full_bar + WIDE_STAGES;
+
+  const uint32_t warp = warp_id_uniform();
+  const uint32_t rank = cluster_ctarank();
+  const uint32_t pair = blockIdx.x / WIDE_CLUSTER;
+  const uint32_t num_m = ceil_div_u32(M, GEMM_BLOCK_M);
+  const uint32_t num_mp = ceil_div_u32(num_m, WIDE_CLUSTER);
+  const uint32_t num_n = ceil_div_u32(N, WIDE_N);
+  const uint32_t num_kb = ceil_div_u32(K, GEMM_BLOCK_K);
+
+  if (threadIdx.x == 0) {
+    for (uint32_t i = 0; i < WIDE_STAGES; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 2 * WIDE_CLUSTER);      // one arrive per consumer warpgroup of every CTA of the cluster
+    }
+    fence_mbar_init();
+  }
+  cluster_sync_all();                                  // the peer's multicasts and arrivals target these barriers
+
+  uint32_t mp, n_blk;
+  tile_coords(pair, num_mp, num_n, mp, n_blk, GEMM_GROUP_M / WIDE_CLUSTER);
+  const uint32_t m_blk = mp * WIDE_CLUSTER + rank;
+
+  if (warp == 8) {
+    // ===================== TMA producer =====================
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_b);
+    uint32_t stage = 0, phase = 0;
+    {
+      const int32_t m0 = m_blk * GEMM_BLOCK_M;
+      for (uint32_t kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        if (elect_one()) {
+          mbar_arrive_expect_tx(&full_bar[stage], L::STAGE_BYTES);
+          const int32_t k0 = kb * GEMM_BLOCK_K;
+          uint8_t* sa = smem_a + stage * L::A_BYTES;
+          uint8_t* sb = smem_b + stage * L::B_BYTES;
+          if constexpr (!A_MN) {
+            tma_load_2d(sa, &tmap_a, &full_bar[stage], k0, m0);  // box {64 k, 128 m}
+          } else {
+#pragma unroll
+            for (uint32_t i = 0; i < GEMM_BLOCK_M / 64; ++i)  // box {64 m, 64 k} per 64-wide MN atom
+              tma_load_2d(sa + i * (GEMM_BLOCK_K * 128), &tmap_a, &full_bar[stage], m0 + i * 64, k0);
+          }
+          // B: K-major two boxes {64 k, 128 n}, MN-major four boxes {64 n, 64 k};
+          // this CTA loads its 1 / WIDE_CLUSTER share of them into every CTA of the cluster
+          constexpr uint32_t BOXES = B_MN ? WIDE_N / 64 : 2, BOX_BYTES = L::B_BYTES / BOXES;
+#pragma unroll
+          for (uint32_t j = 0; j < BOXES / WIDE_CLUSTER; ++j) {
+            const uint32_t i = rank * (BOXES / WIDE_CLUSTER) + j;
+            int32_t c0, c1;
+            if constexpr (B_MN) { c0 = n_blk * WIDE_N + i * 64; c1 = k0; }
+            else { c0 = k0; c1 = n_blk * WIDE_N + i * 128; }
+            tma_load_2d_multicast(sb + i * BOX_BYTES, &tmap_b, &full_bar[stage], c0, c1, (1u << WIDE_CLUSTER) - 1);
+          }
+        }
+        __syncwarp();
+        if (++stage == WIDE_STAGES) { stage = 0; phase ^= 1; }
+      }
+    }
+  } else {
+    // ===================== consumers (warpgroups 0, 1) =====================
+    const uint32_t wg = warp >> 2, t = threadIdx.x & 127, lane = threadIdx.x & 31;
+    const uint32_t r0 = wg * 64 + (t >> 5) * 16 + (lane >> 2);   // fragment rows r0, r0 + 8
+    constexpr uint32_t A_KADV = A_MN ? (16 * 128) >> 4 : (16 * 2) >> 4;
+    constexpr uint32_t B_KADV = B_MN ? (16 * 128) >> 4 : (16 * 2) >> 4;
+    constexpr uint32_t A_LBO = A_MN ? GEMM_BLOCK_K * 128 : 0, B_LBO = B_MN ? GEMM_BLOCK_K * 128 : 0;
+    const bool do_add = (flags & GEMM_ADD) != 0;
+    uint32_t stage = 0, phase = 0;
+    {
+      float acc[WIDE_N / 2];
+#pragma unroll
+      for (uint32_t i = 0; i < WIDE_N / 2; ++i) acc[i] = 0.f;
+      uint32_t prev = 0;
+      for (uint32_t kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint64_t adesc = gmma_desc_sw128(smem_u32(smem_a + stage * L::A_BYTES + wg * 8192), A_LBO, 1024);
+        const uint64_t bdesc = gmma_desc_sw128(smem_u32(smem_b + stage * L::B_BYTES), B_LBO, 1024);
+        wgmma_fence();
+#pragma unroll
+        for (uint32_t k = 0; k < GEMM_BLOCK_K / 16; ++k)
+          wgmma_ss_bf16<WIDE_N, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc + k * A_KADV, bdesc + k * B_KADV, 1u);
+        wgmma_commit();
+        wgmma_wait<1>();                                  // the previous k-block's wgmmas are done: free its stage
+        if (kb > 0 && t == 0)
+          for (uint32_t c = 0; c < WIDE_CLUSTER; ++c) mbar_arrive_cluster(&empty_bar[prev], c);
+        prev = stage;
+        if (++stage == WIDE_STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      reg_fence(acc);
+
+      // ---- epilogue: two passes of 128 bf16 columns; thread = one output row, warpgroup = half of the pass ----
+      const uint32_t row = m_blk * GEMM_BLOCK_M + t;
+      const uint32_t col0 = n_blk * WIDE_N;
+#pragma unroll
+      for (uint32_t p = 0; p < 2; ++p) {
+        named_bar_sync(1, GEMM_CONSUMERS);                // the previous pass has drained the staging buffer
+#pragma unroll
+        for (uint32_t i = 0; i < WIDE_N / 8; ++i) {
+          const int sc = stg_chunk(i, p);
+          if (sc < 0) continue;
+          sts32(stg + stg_offset(r0, sc) + 4 * (lane & 3), pack_bf16x2(acc[4 * i], acc[4 * i + 1]));
+          sts32(stg + stg_offset(r0 + 8, sc) + 4 * (lane & 3), pack_bf16x2(acc[4 * i + 2], acc[4 * i + 3]));
+        }
+        named_bar_sync(1, GEMM_CONSUMERS);
+        if (row >= M) continue;
+#pragma unroll 1
+          for (uint32_t h = 0; h < 2; ++h) {              // chunks 4 wg + 8 h.. = tile columns 128 h + 64 p + 32 wg ..
+            uint32_t v[16];
+            ld_stg32(stg, t, 8 * h + 4 * wg, v);
+            store_plain32(v, Cout, ldc, addend, ld_add, row, col0 + 128 * h + 64 * p + 32 * wg, N, do_add);
+          }
+      }
+    }
+  }
+  __syncwarp();
+  cluster_sync_all();   // no CTA exits while its peer can still multicast into it or arrive on its barriers
+}
+
+template <bool A_MN, bool B_MN>
+static int launch_wide(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int64_t ldc, const void* addend,
+                       int64_t ld_add, uint32_t M, uint32_t N, uint32_t K, uint32_t flags, cudaStream_t stream) {
+  auto kern = gemm_bf16_wide<A_MN, B_MN>;
+  cudaLaunchConfig_t cfg = {};
+  cfg.blockDim = dim3(GEMM_THREADS);
+  cfg.dynamicSmemBytes = WideSmem::DYN_BYTES;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = WIDE_CLUSTER;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  static bool attr_set = false;
+  if (!attr_set) {
+    NV_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, WideSmem::DYN_BYTES));
+    attr_set = true;
+  }
+  const uint32_t pairs = ceil_div_u32(ceil_div_u32(M, GEMM_BLOCK_M), WIDE_CLUSTER) * ceil_div_u32(N, WIDE_N);
+  cfg.gridDim = dim3(WIDE_CLUSTER * pairs);
+  NV_CUDA(cudaLaunchKernelEx(&cfg, kern, ta, tb, C, ldc, reinterpret_cast<const __nv_bfloat16*>(addend), ld_add, M, N, K,
+                             flags));
+  return NV_OK;
+}
+
 // TMA maps of the two operands for a BLOCK_N-wide tile (B boxes of at most 128 rows when K-major).
 static int gemm_tmaps(CUtensorMap* ta, CUtensorMap* tb, const void* A, int64_t lda, int a_mn, const void* B, int64_t ldb,
                       int b_mn, int M, int N, int K, uint32_t block_n, uint64_t b_rows) {
@@ -534,9 +773,18 @@ extern "C" int nv_gemm_bf16(const void* A, int64_t lda, int a_mn, const void* B,
   NV_REQUIRE(block_n == 32 || block_n == 128 || block_n == 256, "nv_gemm_bf16: block_n must be 32, 128 or 256");
   NV_REQUIRE(!(block_n == 32 && b_mn), "nv_gemm_bf16: block_n = 32 (skinny-M weight streaming) needs a K-major B");
 
+  if (block_n == 256 && (flags & GEMM_OUT_F32)) block_n = 128;   // the 256-wide plain epilogue stages bf16 only
+
   CUtensorMap ta, tb;
   int rc = gemm_tmaps(&ta, &tb, A, lda, a_mn, B, ldb, b_mn, M, N, K, (uint32_t)block_n, (uint64_t)N);
   if (rc) return rc;
+
+  if (block_n == 256) {
+    if (!a_mn && !b_mn) return launch_wide<false, false>(ta, tb, C, ldc, addend, ld_add, M, N, K, flags, stream);
+    if (!a_mn && b_mn) return launch_wide<false, true>(ta, tb, C, ldc, addend, ld_add, M, N, K, flags, stream);
+    if (a_mn && b_mn) return launch_wide<true, true>(ta, tb, C, ldc, addend, ld_add, M, N, K, flags, stream);
+    return launch_wide<true, false>(ta, tb, C, ldc, addend, ld_add, M, N, K, flags, stream);
+  }
 
 #define NV_GEMM_CASE(BN, ST)                                                                                       \
   do {                                                                                                             \
@@ -546,7 +794,6 @@ extern "C" int nv_gemm_bf16(const void* A, int64_t lda, int a_mn, const void* B,
     return launch_gemm<BN, ST, true, false>(ta, tb, C, ldc, addend, ld_add, M, N, K, flags, stream);                      \
   } while (0)
 
-  if (block_n == 256) NV_GEMM_CASE(256, 4);
   if (block_n == 32) {
     // decode / pruned-row GEMMs (M <= 128): HBM-bound weight streaming; 10 stages keep ~40 KB of weights in flight per SM
     if (!a_mn) return launch_gemm<32, 10, false, false>(ta, tb, C, ldc, addend, ld_add, M, N, K, flags, stream);

@@ -51,6 +51,14 @@ __device__ __forceinline__ void griddep_launch() { asm volatile("griddepcontrol.
 __device__ __forceinline__ void sts128(uint32_t saddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }
+__device__ __forceinline__ void sts32(uint32_t saddr, uint32_t a) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(saddr), "r"(a) : "memory");
+}
+__device__ __forceinline__ uint4 lds128(uint32_t saddr) {
+  uint4 v;
+  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(saddr) : "memory");
+  return v;
+}
 __device__ __forceinline__ uint2 lds64(uint32_t saddr) {
   uint2 v;
   asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(saddr) : "memory");
@@ -85,7 +93,9 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   return ok != 0;
 }
 // Bounded wait: a protocol bug traps after ~2 s (error surfaces on the host as a launch failure)
-// instead of hanging the GPU box.
+// instead of hanging the GPU box.  Every caller is a wgmma kernel, and a function call anywhere in such a kernel makes
+// ptxas serialize all of its wgmmas (warning C7510): the printf that names the block, thread, barrier and parity is
+// therefore compiled in only with -DNV_MBAR_TIMEOUT_REPORT (build.py: NV_NVCC_EXTRA), for debugging a protocol.
 #ifndef NV_MBAR_TIMEOUT_CYCLES
 #define NV_MBAR_TIMEOUT_CYCLES (4000000000ll)
 #endif
@@ -95,8 +105,10 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
     if ((++spins & 255u) == 0 && clock64() - t0 > NV_MBAR_TIMEOUT_CYCLES) {
+#ifdef NV_MBAR_TIMEOUT_REPORT
       printf("navillm_b200: mbarrier timeout block (%d,%d) thread %d bar@%u parity %u\n", (int)blockIdx.x,
              (int)blockIdx.y, (int)threadIdx.x, smem_u32(bar), parity);
+#endif
       __trap();
     }
   }
@@ -118,6 +130,16 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
+      : "memory");
+}
+// The same box into the shared memory of every CTA of the cluster named in cta_mask, at the same offset, signalling
+// the mbarrier at the same offset in each of them.
+__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int32_t c0,
+                                                      int32_t c1, uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
       : "memory");
 }
 __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int32_t c0,
@@ -181,6 +203,22 @@ __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
 // ----------------------------------------------------------------------------------------------
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// arrive on the mbarrier at the offset of `bar` in CTA `cta` of the cluster.  Default (CTA-scope) release: a
+// consumer releasing a stage has already retired its wgmma reads, and .release.cluster would put a GPU-scope
+// MEMBAR in front of every arrive.
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}"
+      ::"r"(smem_u32(bar)), "r"(cta)
+      : "memory");
 }
 // *(float at shared address `saddr` in CTA `cta` of the cluster) += v   (the caller guarantees a single writer)
 __device__ __forceinline__ void dsmem_add_f32(uint32_t saddr, uint32_t cta, float v) {

@@ -1,10 +1,14 @@
 """Time the wgmma bf16 GEMM on the LLaMA-7B shapes of the path and print TFLOP/s next to cuBLAS
-(torch.matmul; comparison bar only, never used by the product).  Run on the GPU box:
+(torch.matmul; comparison bar only, never used by the product), plus the four fused-epilogue GEMMs of the training
+step (gate|up + SwiGLU, q|k|v + RoPE, down dgrad + SwiGLU backward, o_proj dgrad + attention row sums).
+--tokens defaults to the 10 425 real tokens of bench.py's C2 step.  Every row records the card, its power limit and
+the SM clock read right after the timed loop, since the rates only mean something next to those.
 
-    python tools/gemm_bench.py [--tokens 16384] [--json gemm_bench.json]
+    python tools/gemm_bench.py [--tokens 10425] [--json gemm_bench.json]
 """
 import argparse
 import json
+import subprocess
 import sys
 from pathlib import Path
 
@@ -27,9 +31,18 @@ def timeit(fn, iters=10, warmup=3):
     return st.elapsed_time(en) / iters
 
 
+def smi(query):
+    try:
+        out = subprocess.run(["nvidia-smi", f"--query-gpu={query}", "--format=csv,noheader,nounits", "-i", "0"],
+                             capture_output=True, text=True, timeout=10).stdout.strip()
+        return out or None
+    except (OSError, subprocess.SubprocessError):
+        return None
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--tokens", type=int, default=16384)
+    ap.add_argument("--tokens", type=int, default=10425)
     ap.add_argument("--json", type=str, default="")
     ap.add_argument("--no-cublas", action="store_true")
     ap.add_argument("--iters", type=int, default=10)
@@ -37,6 +50,8 @@ def main():
     a = ap.parse_args()
     T = a.tokens
     dev = torch.device("cuda:0")
+    card = {"gpu": torch.cuda.get_device_name(0), "power_limit_w": smi("power.limit"), "sm_clock_max_mhz": smi("clocks.max.sm")}
+    print(json.dumps(card), flush=True)
     d, F = 4096, 11008
     cases = [
         # name, M, N, K, a_mn, b_mn
@@ -45,6 +60,7 @@ def main():
         ("gateup_fwd", T, 2 * F, d, False, False),
         ("down_fwd", T, d, F, False, False),
         ("qkv_dgrad", T, d, 3 * d, False, True),
+        ("o_dgrad", T, d, d, False, True),
         ("gateup_dgrad", T, d, 2 * F, False, True),
         ("down_dgrad", T, F, d, False, True),
         ("qkv_wgrad", 3 * d, d, T, True, True),
@@ -62,6 +78,7 @@ def main():
             ms = timeit(lambda: ops.gemm(A, B, a_mn=a_mn, b_mn=b_mn, out=C, block_n=bn), iters=a.iters, warmup=a.warmup)
             res[f"nv_bn{bn}_ms"] = ms
             res[f"nv_bn{bn}_tflops"] = flops / ms / 1e9
+            res[f"nv_bn{bn}_sm_clock_mhz"] = smi("clocks.sm")
         if not a.no_cublas:
             At = A.t() if a_mn else A
             Bt = B if b_mn else B.t()
@@ -71,9 +88,39 @@ def main():
         rows.append(res)
         print(json.dumps(res), flush=True)
         del A, B, C
+
+    # fused epilogues (128 x 256 tile only)
+    from navillm_b200.llama import LlamaDims, rope_tables
+    g = torch.Generator(device="cpu").manual_seed(0)
+    x = (torch.randn(T, d, generator=g) * 0.5).to(dev, torch.bfloat16)
+    wgu = (torch.randn(2 * F, d, generator=g) * 0.02).to(dev, torch.bfloat16)
+    wqkv = (torch.randn(3 * d, d, generator=g) * 0.02).to(dev, torch.bfloat16)
+    wd = (torch.randn(d, F, generator=g) * 0.02).to(dev, torch.bfloat16)
+    wo = (torch.randn(d, d, generator=g) * 0.02).to(dev, torch.bfloat16)
+    cos_t, sin_t = rope_tables(LlamaDims(), dev)
+    pos = (torch.arange(T, device=dev, dtype=torch.int32) % 1024)
+    gu = torch.empty(T, 2 * F, device=dev, dtype=torch.bfloat16)
+    h = torch.empty(T, F, device=dev, dtype=torch.bfloat16)
+    qkv = torch.empty(T, 3 * d, device=dev, dtype=torch.bfloat16)
+    dgu = torch.empty(T, 2 * F, device=dev, dtype=torch.bfloat16)
+    dout = torch.empty(T, d, device=dev, dtype=torch.bfloat16)
+    dvec = torch.empty(32 * T, device=dev, dtype=torch.float32)
+    ops.gemm_swiglu(x, wgu, gu=gu, h=h)
+    fused = [
+        ("gateup_fwd_swiglu", T, 2 * F, d, lambda: ops.gemm_swiglu(x, wgu, gu=gu, h=h)),
+        ("qkv_fwd_rope", T, 3 * d, d, lambda: ops.gemm_rope(x, wqkv, pos, cos_t, sin_t, 2 * d, out=qkv)),
+        ("down_dgrad_dswiglu", T, F, d, lambda: ops.gemm_dswiglu(x, wd, gu, dgu=dgu)),
+        ("o_dgrad_attnd", T, d, d, lambda: ops.gemm_attnd(x, wo, x, dout=dout, dvec=dvec)),
+    ]
+    for name, M, N, K, fn in fused:
+        ms = timeit(fn, iters=a.iters, warmup=a.warmup)
+        res = {"name": name, "M": M, "N": N, "K": K, "nv_bn256_ms": ms, "nv_bn256_tflops": 2.0 * M * N * K / ms / 1e9,
+               "nv_bn256_sm_clock_mhz": smi("clocks.sm")}
+        rows.append(res)
+        print(json.dumps(res), flush=True)
     if a.json:
         Path(a.json).parent.mkdir(parents=True, exist_ok=True)
-        Path(a.json).write_text(json.dumps(rows, indent=1))
+        Path(a.json).write_text(json.dumps({"card": card, "rows": rows}, indent=1))
 
 
 if __name__ == "__main__":
