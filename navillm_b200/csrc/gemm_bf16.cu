@@ -18,10 +18,10 @@
 //   warps 0..7 (two warpgroups)  consumers: warpgroup w computes rows 64 w .. 64 w + 63 with m64nBLOCK_Nk16 wgmmas
 //                                straight from the shared-memory stages, one wgmma group in flight
 //   warp 8 (1 lane)              TMA producer: 128-byte-swizzled tiles, STAGES-deep mbarrier ring
-// The plain (EPI_PLAIN) 128 x 256 tile is gemm_bf16_wide below: 2-CTA clusters that share the B tile by TMA multicast.
+// The 128 x 256 tile, with the plain and the fused epilogues, is gemm_bf16_wide below: 2-CTA clusters that share the B
+// tile by TMA multicast.
 // Epilogue: the accumulators go through shared memory (the stage ring is free by then) so that each thread then owns
-// one output row and 32 consecutive columns at a time: 16-byte global stores, and the fused epilogues below see whole
-// rows (rotate-half pairs, the gate and up halves of SwiGLU, the per-head row sums of the attention backward).
+// one output row and 32 consecutive columns at a time: 16-byte global stores.
 // HBM layout assumptions: base pointers 16-byte aligned, leading dimensions multiples of 8 elements.
 // Ragged M/N/K are handled by TMA zero-fill on loads and predicated stores.
 //
@@ -64,9 +64,7 @@ enum GemmFlags : uint32_t {
 enum { EPI_PLAIN = 0, EPI_SWIGLU = 1, EPI_DSWIGLU = 2, EPI_ROPE = 3, EPI_ATTND = 4 };
 
 struct EpiAux {
-  void* aux;            // SWIGLU: h out [T,F];  DSWIGLU: gu in [T,2F];  ATTND: O in [T,D]
-  int64_t ld_aux;
-  uint32_t F;           // SWIGLU / DSWIGLU: intermediate size (columns of gate and of up)
+  uint32_t F;           // SWIGLU / DSWIGLU: intermediate size (columns of gate and of up); h, g, u, dg, du are TMA maps
   float* dvec;          // ATTND: D out [H, T] fp32 (T = M rows)
   const int* pos;       // ROPE
   const __nv_bfloat16* cos_t;
@@ -115,15 +113,14 @@ __device__ __forceinline__ void ld_acc32(const float* p, uint32_t (&v)[32]) {
   }
 }
 
-template <uint32_t BLOCK_N, uint32_t STAGES, bool A_MN, bool B_MN, int EPI, typename WT = __nv_bfloat16>
+template <uint32_t BLOCK_N, uint32_t STAGES, bool A_MN, bool B_MN, typename WT = __nv_bfloat16>
 __global__ void __launch_bounds__(GemmSmem<BLOCK_N, STAGES, WT>::THREADS, 1)
 gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                 void* __restrict__ Cout, int64_t ldc, const __nv_bfloat16* __restrict__ addend, int64_t ld_add,
                 uint32_t M, uint32_t N, uint32_t K, uint32_t flags, EpiAux ea) {
   using L = GemmSmem<BLOCK_N, STAGES, WT>;
-  static_assert(EPI == EPI_PLAIN || BLOCK_N == 256, "fused epilogues use the 128 x 256 tile");
-  static_assert(!L::kFp8 || (EPI == EPI_PLAIN && !A_MN && !B_MN && BLOCK_N <= 128),
-                "fp8 weights: plain epilogue, K-major operands, 32- or 128-wide tiles");
+  static_assert(BLOCK_N <= 128, "the 128 x 256 tile is gemm_bf16_wide");
+  static_assert(!L::kFp8 || (!A_MN && !B_MN), "fp8 weights: K-major operands");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
@@ -134,10 +131,8 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
   uint64_t* cvt_bar = empty_bar + STAGES;                 // fp8: the expanded bf16 B tile of the stage is complete
 
   const uint32_t warp = warp_id_uniform();
-  // logical output columns per tile: BLOCK_N, except SWIGLU where the 256 accumulator columns are 128 gate + 128 up
-  constexpr uint32_t TILE_N = (EPI == EPI_SWIGLU) ? 128u : BLOCK_N;
   const uint32_t num_m = ceil_div_u32(M, GEMM_BLOCK_M);
-  const uint32_t num_n = ceil_div_u32(N, TILE_N);
+  const uint32_t num_n = ceil_div_u32(N, BLOCK_N);
   const uint32_t num_kb = ceil_div_u32(K, GEMM_BLOCK_K);
   uint32_t m_blk, n_blk;
   tile_coords(blockIdx.x, num_m, num_n, m_blk, n_blk);
@@ -179,8 +174,7 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
           constexpr uint32_t BOX = BLOCK_N < 128 ? BLOCK_N : 128;  // box {64 k, BOX n}
 #pragma unroll
           for (uint32_t i = 0; i < BLOCK_N / BOX; ++i) {
-            const int32_t n0 = (EPI == EPI_SWIGLU) ? (int32_t)(n_blk * 128 + i * ea.F) : (int32_t)(n_blk * BLOCK_N + i * BOX);
-            tma_load_2d(sb + i * BOX * 128, &tmap_b, &full_bar[stage], k0, n0);
+            tma_load_2d(sb + i * BOX * 128, &tmap_b, &full_bar[stage], k0, n_blk * BLOCK_N + i * BOX);
           }
         } else {
 #pragma unroll
@@ -288,131 +282,32 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
   // ---- epilogue: thread = one output row, column chunks split between the two halves of the consumers ----
   const uint32_t rl = threadIdx.x & 127, half = threadIdx.x >> 7;
   const uint32_t row = m_blk * GEMM_BLOCK_M + rl;
-  const uint32_t col0 = n_blk * TILE_N;
+  const uint32_t col0 = n_blk * BLOCK_N;
   const float* arow = acc_s + rl * L::ACC_LD;
   if (row >= M) return;
-  if constexpr (EPI == EPI_SWIGLU) {
-    __nv_bfloat16* gu = reinterpret_cast<__nv_bfloat16*>(Cout) + static_cast<int64_t>(row) * ldc;
-    __nv_bfloat16* hrow = reinterpret_cast<__nv_bfloat16*>(ea.aux) + static_cast<int64_t>(row) * ea.ld_aux;
+  const bool do_add = (flags & GEMM_ADD) != 0;
+  const bool out_f32 = (flags & GEMM_OUT_F32) != 0;
 #pragma unroll 1
-    for (uint32_t c = half * 32; c < 128; c += 64) {
-      uint32_t g[32], u[32];
-      ld_acc32(arow + c, g);
-      ld_acc32(arow + 128 + c, u);
-      const uint32_t col = col0 + c;
-      if (col < ea.F) {   // F % 128 == 0 is required by the host wrapper
+  for (uint32_t c = half * 32; c < BLOCK_N; c += 64) {
+    uint32_t v[32];
+    ld_acc32(arow + c, v);
+    const uint32_t col = col0 + c;
+    if (col >= N) break;
+    if (out_f32) {
+      float* dst = reinterpret_cast<float*>(Cout) + static_cast<int64_t>(row) * ldc + col;
+      if (col + 32 <= N && (ldc & 3) == 0) {
 #pragma unroll
-        for (uint32_t j = 0; j < 32; j += 8) {
-          uint4 og, ou, oh;
-          uint32_t* pg = &og.x; uint32_t* pu = &ou.x; uint32_t* ph = &oh.x;
+        for (uint32_t j = 0; j < 32; j += 4)
+          *reinterpret_cast<uint4*>(dst + j) = make_uint4(v[j], v[j + 1], v[j + 2], v[j + 3]);
+      } else {
 #pragma unroll
-          for (uint32_t q = 0; q < 4; ++q) {
-            pg[q] = pack_bf16x2(__uint_as_float(g[j + 2 * q]), __uint_as_float(g[j + 2 * q + 1]));
-            pu[q] = pack_bf16x2(__uint_as_float(u[j + 2 * q]), __uint_as_float(u[j + 2 * q + 1]));
-            ph[q] = pack_bf16x2(silu_bf16(bf16_lo(pg[q])) * bf16_lo(pu[q]), silu_bf16(bf16_hi(pg[q])) * bf16_hi(pu[q]));
-          }
-          if ((flags & GEMM_NO_GU) == 0) {
-            *reinterpret_cast<uint4*>(gu + col + j) = og;
-            *reinterpret_cast<uint4*>(gu + ea.F + col + j) = ou;
-          }
-          *reinterpret_cast<uint4*>(hrow + col + j) = oh;
-        }
+        for (uint32_t j = 0; j < 32; ++j)
+          if (col + j < N) dst[j] = __uint_as_float(v[j]);
       }
-    }
-  } else if constexpr (EPI == EPI_DSWIGLU) {
-    __nv_bfloat16* dgu = reinterpret_cast<__nv_bfloat16*>(Cout) + static_cast<int64_t>(row) * ldc;
-    const __nv_bfloat16* gu = reinterpret_cast<const __nv_bfloat16*>(ea.aux) + static_cast<int64_t>(row) * ea.ld_aux;
-#pragma unroll 1
-    for (uint32_t c = half * 32; c < BLOCK_N; c += 64) {
-      uint32_t v[32];
-      ld_acc32(arow + c, v);
-      const uint32_t col = col0 + c;
-      if (col < ea.F) {   // F % 32 == 0 is required by the host wrapper
-#pragma unroll
-        for (uint32_t j = 0; j < 32; j += 8) {
-          const uint4 gg = *reinterpret_cast<const uint4*>(gu + col + j);
-          const uint4 uu = *reinterpret_cast<const uint4*>(gu + ea.F + col + j);
-          const uint32_t* pg = &gg.x; const uint32_t* pu = &uu.x;
-          uint4 og, ou;
-          uint32_t* qg = &og.x; uint32_t* qu = &ou.x;
-#pragma unroll
-          for (uint32_t q = 0; q < 4; ++q) {
-            float dg[2], du[2];
-#pragma unroll
-            for (uint32_t e = 0; e < 2; ++e) {
-              const float d = bf16_round(__uint_as_float(v[j + 2 * q + e]));   // dh as the unfused path stores it
-              const float gv = e ? bf16_hi(pg[q]) : bf16_lo(pg[q]);
-              const float uv = e ? bf16_hi(pu[q]) : bf16_lo(pu[q]);
-              const float sg = 1.f / (1.f + __expf(-gv));
-              dg[e] = d * uv * (sg * (1.f + gv * (1.f - sg)));
-              du[e] = d * (gv * sg);
-            }
-            qg[q] = pack_bf16x2(dg[0], dg[1]);
-            qu[q] = pack_bf16x2(du[0], du[1]);
-          }
-          *reinterpret_cast<uint4*>(dgu + col + j) = og;
-          *reinterpret_cast<uint4*>(dgu + ea.F + col + j) = ou;
-        }
-      }
-    }
-  } else if constexpr (EPI == EPI_ROPE) {
-    __nv_bfloat16* crow = reinterpret_cast<__nv_bfloat16*>(Cout) + static_cast<int64_t>(row) * ldc;
-    const int p = ea.pos[row];
-    const __nv_bfloat16* cs = ea.cos_t + static_cast<int64_t>(p) * 128;
-    const __nv_bfloat16* sn = ea.sin_t + static_cast<int64_t>(p) * 128;
-#pragma unroll 1
-    for (uint32_t it = half; it < 4; it += 2) {            // two 128-wide heads per tile x two 32-column chunks
-      const uint32_t hh = (it >> 1) * 128, c = (it & 1) * 32;   // chunk c pairs with chunk c + 64 (rotate-half)
-      uint32_t a[32], b[32];
-      ld_acc32(arow + hh + c, a);
-      ld_acc32(arow + hh + 64 + c, b);
-      const uint32_t col = col0 + hh + c;
-      if (col < N) {
-        const bool rope = col < ea.rope_cols;
-#pragma unroll
-        for (uint32_t j = 0; j < 32; j += 8) {
-          uint4 o1, o2;
-          uint32_t* p1 = &o1.x; uint32_t* p2 = &o2.x;
-          uint4 c1 = make_uint4(0, 0, 0, 0), s1 = c1, c2 = c1, s2 = c1;
-          if (rope) {
-            c1 = *reinterpret_cast<const uint4*>(cs + c + j);      s1 = *reinterpret_cast<const uint4*>(sn + c + j);
-            c2 = *reinterpret_cast<const uint4*>(cs + 64 + c + j); s2 = *reinterpret_cast<const uint4*>(sn + 64 + c + j);
-          }
-          const uint32_t* pc1 = &c1.x; const uint32_t* ps1 = &s1.x; const uint32_t* pc2 = &c2.x; const uint32_t* ps2 = &s2.x;
-#pragma unroll
-          for (uint32_t q = 0; q < 4; ++q) {
-            // projection output rounded to bf16 first (the reference ropes the bf16 q/k)
-            const uint32_t xa = pack_bf16x2(__uint_as_float(a[j + 2 * q]), __uint_as_float(a[j + 2 * q + 1]));
-            const uint32_t xb = pack_bf16x2(__uint_as_float(b[j + 2 * q]), __uint_as_float(b[j + 2 * q + 1]));
-            if (rope) {
-              const float y1l = bf16_round(bf16_lo(xa) * bf16_lo(pc1[q])) + bf16_round(-bf16_lo(xb) * bf16_lo(ps1[q]));
-              const float y1h = bf16_round(bf16_hi(xa) * bf16_hi(pc1[q])) + bf16_round(-bf16_hi(xb) * bf16_hi(ps1[q]));
-              const float y2l = bf16_round(bf16_lo(xb) * bf16_lo(pc2[q])) + bf16_round(bf16_lo(xa) * bf16_lo(ps2[q]));
-              const float y2h = bf16_round(bf16_hi(xb) * bf16_hi(pc2[q])) + bf16_round(bf16_hi(xa) * bf16_hi(ps2[q]));
-              p1[q] = pack_bf16x2(y1l, y1h);
-              p2[q] = pack_bf16x2(y2l, y2h);
-            } else {
-              p1[q] = xa;
-              p2[q] = xb;
-            }
-          }
-          *reinterpret_cast<uint4*>(crow + col + j) = o1;
-          *reinterpret_cast<uint4*>(crow + col + 64 + j) = o2;
-        }
-      }
-    }
-  } else if constexpr (EPI == EPI_ATTND) {
-    // N % 128 == 0 and 16-byte aligned rows are required by the host wrapper; one 128-column head per half
-    __nv_bfloat16* drow = reinterpret_cast<__nv_bfloat16*>(Cout) + static_cast<int64_t>(row) * ldc;
-    const __nv_bfloat16* orow = reinterpret_cast<const __nv_bfloat16*>(ea.aux) + static_cast<int64_t>(row) * ea.ld_aux;
-    const uint32_t hc = col0 + half * 128;
-    if (hc < N) {
-      float dsum = 0.f;
-#pragma unroll 1
-      for (uint32_t c = 0; c < 128; c += 32) {
-        uint32_t v[32];
-        ld_acc32(arow + half * 128 + c, v);
-        const uint32_t col = hc + c;
+    } else {
+      __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(Cout) + static_cast<int64_t>(row) * ldc + col;
+      const __nv_bfloat16* add = do_add ? addend + static_cast<int64_t>(row) * ld_add + col : nullptr;
+      if (col + 32 <= N && (ldc & 7) == 0 && (!do_add || (ld_add & 7) == 0)) {
 #pragma unroll
         for (uint32_t j = 0; j < 32; j += 8) {
           uint4 o;
@@ -420,62 +315,22 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
           o.y = pack_bf16x2(__uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
           o.z = pack_bf16x2(__uint_as_float(v[j + 4]), __uint_as_float(v[j + 5]));
           o.w = pack_bf16x2(__uint_as_float(v[j + 6]), __uint_as_float(v[j + 7]));
-          const uint4 a = *reinterpret_cast<const uint4*>(orow + col + j);
-          dsum += bf16_lo(o.x) * bf16_lo(a.x) + bf16_hi(o.x) * bf16_hi(a.x) + bf16_lo(o.y) * bf16_lo(a.y) + bf16_hi(o.y) * bf16_hi(a.y)
-                + bf16_lo(o.z) * bf16_lo(a.z) + bf16_hi(o.z) * bf16_hi(a.z) + bf16_lo(o.w) * bf16_lo(a.w) + bf16_hi(o.w) * bf16_hi(a.w);
-          *reinterpret_cast<uint4*>(drow + col + j) = o;
-        }
-      }
-      ea.dvec[static_cast<int64_t>(hc >> 7) * M + row] = dsum;
-    }
-  } else {
-    const bool do_add = (flags & GEMM_ADD) != 0;
-    const bool out_f32 = (flags & GEMM_OUT_F32) != 0;
-#pragma unroll 1
-    for (uint32_t c = half * 32; c < BLOCK_N; c += 64) {
-      uint32_t v[32];
-      ld_acc32(arow + c, v);
-      const uint32_t col = col0 + c;
-      if (col >= N) break;
-      if (out_f32) {
-        float* dst = reinterpret_cast<float*>(Cout) + static_cast<int64_t>(row) * ldc + col;
-        if (col + 32 <= N && (ldc & 3) == 0) {
-#pragma unroll
-          for (uint32_t j = 0; j < 32; j += 4)
-            *reinterpret_cast<uint4*>(dst + j) = make_uint4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-        } else {
-#pragma unroll
-          for (uint32_t j = 0; j < 32; ++j)
-            if (col + j < N) dst[j] = __uint_as_float(v[j]);
+          if (do_add) {
+            const uint4 a = *reinterpret_cast<const uint4*>(add + j);
+            o.x = pack_bf16x2(bf16_lo(o.x) + bf16_lo(a.x), bf16_hi(o.x) + bf16_hi(a.x));
+            o.y = pack_bf16x2(bf16_lo(o.y) + bf16_lo(a.y), bf16_hi(o.y) + bf16_hi(a.y));
+            o.z = pack_bf16x2(bf16_lo(o.z) + bf16_lo(a.z), bf16_hi(o.z) + bf16_hi(a.z));
+            o.w = pack_bf16x2(bf16_lo(o.w) + bf16_lo(a.w), bf16_hi(o.w) + bf16_hi(a.w));
+          }
+          *reinterpret_cast<uint4*>(dst + j) = o;
         }
       } else {
-        __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(Cout) + static_cast<int64_t>(row) * ldc + col;
-        const __nv_bfloat16* add = do_add ? addend + static_cast<int64_t>(row) * ld_add + col : nullptr;
-        if (col + 32 <= N && (ldc & 7) == 0 && (!do_add || (ld_add & 7) == 0)) {
 #pragma unroll
-          for (uint32_t j = 0; j < 32; j += 8) {
-            uint4 o;
-            o.x = pack_bf16x2(__uint_as_float(v[j + 0]), __uint_as_float(v[j + 1]));
-            o.y = pack_bf16x2(__uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
-            o.z = pack_bf16x2(__uint_as_float(v[j + 4]), __uint_as_float(v[j + 5]));
-            o.w = pack_bf16x2(__uint_as_float(v[j + 6]), __uint_as_float(v[j + 7]));
-            if (do_add) {
-              const uint4 a = *reinterpret_cast<const uint4*>(add + j);
-              o.x = pack_bf16x2(bf16_lo(o.x) + bf16_lo(a.x), bf16_hi(o.x) + bf16_hi(a.x));
-              o.y = pack_bf16x2(bf16_lo(o.y) + bf16_lo(a.y), bf16_hi(o.y) + bf16_hi(a.y));
-              o.z = pack_bf16x2(bf16_lo(o.z) + bf16_lo(a.z), bf16_hi(o.z) + bf16_hi(a.z));
-              o.w = pack_bf16x2(bf16_lo(o.w) + bf16_lo(a.w), bf16_hi(o.w) + bf16_hi(a.w));
-            }
-            *reinterpret_cast<uint4*>(dst + j) = o;
-          }
-        } else {
-#pragma unroll
-          for (uint32_t j = 0; j < 32; ++j) {
-            if (col + j < N) {
-              float x = bf16_round(__uint_as_float(v[j]));
-              if (do_add) x = x + __bfloat162float(add[j]);
-              dst[j] = __float2bfloat16_rn(x);
-            }
+        for (uint32_t j = 0; j < 32; ++j) {
+          if (col + j < N) {
+            float x = bf16_round(__uint_as_float(v[j]));
+            if (do_add) x = x + __bfloat162float(add[j]);
+            dst[j] = __float2bfloat16_rn(x);
           }
         }
       }
@@ -483,18 +338,18 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
   }
 }
 
-template <uint32_t BN, uint32_t ST, bool A_MN, bool B_MN, int EPI = EPI_PLAIN, typename WT = __nv_bfloat16>
+template <uint32_t BN, uint32_t ST, bool A_MN, bool B_MN, typename WT = __nv_bfloat16>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int64_t ldc, const void* addend,
                        int64_t ld_add, uint32_t M, uint32_t N, uint32_t K, uint32_t flags, cudaStream_t stream,
                        EpiAux ea = EpiAux{}) {
   using L = GemmSmem<BN, ST, WT>;
-  auto kern = gemm_bf16_wgmma<BN, ST, A_MN, B_MN, EPI, WT>;
+  auto kern = gemm_bf16_wgmma<BN, ST, A_MN, B_MN, WT>;
   static bool attr_set = false;
   if (!attr_set) {
     NV_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::DYN_BYTES));
     attr_set = true;
   }
-  const uint32_t tiles = ceil_div_u32(M, GEMM_BLOCK_M) * ceil_div_u32(N, EPI == EPI_SWIGLU ? 128u : BN);
+  const uint32_t tiles = ceil_div_u32(M, GEMM_BLOCK_M) * ceil_div_u32(N, BN);
   kern<<<tiles, L::THREADS, L::DYN_BYTES, stream>>>(ta, tb, C, ldc, reinterpret_cast<const __nv_bfloat16*>(addend), ld_add,
                                                       M, N, K, flags, ea);
   NV_LAUNCH_CHECK();
@@ -509,8 +364,8 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, void* C, in
 // it (each arrives on the empty barrier of both CTAs).  The partner of the last tile of an odd m-block count lies past
 // M: it loads its half of B and zero-filled A, and stores nothing.  The accumulator is rounded to bf16 and drained
 // through a 32 KB half-tile buffer in two passes.  Each tile still accumulates its k-blocks in one chain, in order,
-// with the m64n256k16 sequence of gemm_bf16_wgmma, so C is bit for bit the same.  Plain epilogue only: the fused
-// epilogues measured slower with this staging and stay on gemm_bf16_wgmma<256> (DESIGN.md §4).
+// with the m64n256k16 sequence, so C is bit for bit that of the 128-wide gemm_bf16_wgmma.  The fused epilogues
+// (EPI != EPI_PLAIN) skip the staging buffer: see "fused epilogues of the wide tile" below.
 constexpr uint32_t WIDE_N = 256;
 constexpr uint32_t WIDE_STAGES = 4;
 constexpr uint32_t WIDE_CLUSTER = 2;
@@ -522,7 +377,7 @@ struct WideSmem {
   static constexpr uint32_t STG_OFF = WIDE_STAGES * STAGE_BYTES;
   static constexpr uint32_t STG_BYTES = GEMM_BLOCK_M * 128 * 2;           // bf16 [128 rows][128 columns]
   static constexpr uint32_t BAR_OFF = STG_OFF + STG_BYTES;
-  static constexpr uint32_t DYN_BYTES = BAR_OFF + 2 * WIDE_STAGES * 8 + 1024;   // + slack for 1024-byte alignment
+  static constexpr uint32_t DYN_BYTES = BAR_OFF + (2 * WIDE_STAGES + 1) * 8 + 1024;   // + slack for 1024-byte alignment
   static_assert(DYN_BYTES <= 232448, "shared memory per block");
 };
 
@@ -577,12 +432,50 @@ __device__ __forceinline__ void store_plain32(const uint32_t (&w)[16], void* Cou
   }
 }
 
-template <bool A_MN, bool B_MN>
+// ---- fused epilogues of the wide tile ----
+// The accumulator fragments are rounded and combined in registers (SwiGLU pairs accumulator group i with i + 16, RoPE
+// with i + 8 in the same 128-column head: the same thread holds both) and written as bf16 into 64-column x 128-row
+// boxes, 128-byte swizzled, in the idle stage ring; one thread then TMA-stores the boxes (clipped at M and at the
+// column count) and waits only for their reads to finish before the kernel ends.  dSwiGLU and ATTND read an operand
+// tile (g and u of gu, or O) that the producer TMA-loads into the ring while the last k-blocks compute.
+constexpr uint32_t EPI_BOX_BYTES = GEMM_BLOCK_M * 128;    // one box: 128 rows of 64 bf16
+
+// TMA maps of the fused epilogues: outputs in m[0], m[1], the prefetched operand in m[2], m[3], boxes {64, 128}.
+//   SWIGLU  m[0] g -> gu[:, :F]   m[1] u -> gu[:, F:]   m[2] h -> h[T, F]
+//   DSWIGLU m[0] dg -> dgu[:, :F] m[1] du -> dgu[:, F:] m[2] g <- gu[:, :F]  m[3] u <- gu[:, F:]
+//   ROPE    m[0] q|k|v
+//   ATTND   m[0] dO               m[2] O
+// The halves of gu / dgu get a map each, so that TMA zero-fills and clips them at F.
+struct EpiMaps {
+  CUtensorMap m[4];
+};
+
+// Epilogue slot v (one box) in the idle stage ring: the stages in the order the producer would refill them after the
+// last k-block, three slots per stage (its A tile, then the two halves of its B tile).  Slots 0..8 lie in the stages of
+// k-blocks num_kb - 4 .. num_kb - 2 (or stages no k-block used), which are released while the last k-block computes.
+__device__ __forceinline__ uint8_t* epi_slot(uint8_t* smem, uint32_t num_kb, uint32_t v) {
+  const uint32_t s = (num_kb + v / 3) % WIDE_STAGES, j = v % 3;
+  return j == 0 ? smem + s * WideSmem::A_BYTES
+                : smem + WIDE_STAGES * WideSmem::A_BYTES + s * WideSmem::B_BYTES + (j - 1) * EPI_BOX_BYTES;
+}
+// byte offset, inside its box, of the bf16 pair of accumulator group i (tile columns 8 i ..) in row r held by `lane`
+__device__ __forceinline__ uint32_t frag_offset(uint32_t r, uint32_t i, uint32_t lane) {
+  return sw128_offset(r, i & 7) + 4 * (lane & 3);
+}
+
+template <bool A_MN, bool B_MN, int EPI>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_wide(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-               void* __restrict__ Cout, int64_t ldc, const __nv_bfloat16* __restrict__ addend, int64_t ld_add,
-               uint32_t M, uint32_t N, uint32_t K, uint32_t flags) {
+               const __grid_constant__ EpiMaps em, void* __restrict__ Cout, int64_t ldc,
+               const __nv_bfloat16* __restrict__ addend, int64_t ld_add, uint32_t M, uint32_t N, uint32_t K,
+               uint32_t flags, EpiAux ea) {
   using L = WideSmem;
+  static_assert(EPI == EPI_PLAIN || (!A_MN && B_MN == (EPI == EPI_DSWIGLU || EPI == EPI_ATTND)),
+                "fused epilogues: the operand forms of their entry points");
+  // logical output columns per tile: WIDE_N, except SWIGLU where the 256 accumulator columns are 128 gate + 128 up
+  constexpr uint32_t TILE_N = EPI == EPI_SWIGLU ? 128u : WIDE_N;
+  // boxes the producer prefetches for the epilogue (g and u, or O)
+  constexpr uint32_t PRE_BOXES = EPI == EPI_DSWIGLU ? 8 : EPI == EPI_ATTND ? 4 : 0;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
@@ -590,13 +483,14 @@ gemm_bf16_wide(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   const uint32_t stg = smem_u32(smem + L::STG_OFF);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
   uint64_t* empty_bar = full_bar + WIDE_STAGES;
+  uint64_t* epi_full = empty_bar + WIDE_STAGES;          // the prefetched epilogue operand has landed
 
   const uint32_t warp = warp_id_uniform();
   const uint32_t rank = cluster_ctarank();
   const uint32_t pair = blockIdx.x / WIDE_CLUSTER;
   const uint32_t num_m = ceil_div_u32(M, GEMM_BLOCK_M);
   const uint32_t num_mp = ceil_div_u32(num_m, WIDE_CLUSTER);
-  const uint32_t num_n = ceil_div_u32(N, WIDE_N);
+  const uint32_t num_n = ceil_div_u32(N, TILE_N);
   const uint32_t num_kb = ceil_div_u32(K, GEMM_BLOCK_K);
 
   if (threadIdx.x == 0) {
@@ -604,6 +498,7 @@ gemm_bf16_wide(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 2 * WIDE_CLUSTER);      // one arrive per consumer warpgroup of every CTA of the cluster
     }
+    mbar_init(epi_full, 1);
     fence_mbar_init();
   }
   cluster_sync_all();                                  // the peer's multicasts and arrivals target these barriers
@@ -611,42 +506,62 @@ gemm_bf16_wide(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   uint32_t mp, n_blk;
   tile_coords(pair, num_mp, num_n, mp, n_blk, GEMM_GROUP_M / WIDE_CLUSTER);
   const uint32_t m_blk = mp * WIDE_CLUSTER + rank;
+  const int32_t m0 = m_blk * GEMM_BLOCK_M;
+  const uint32_t col0 = n_blk * TILE_N;
 
   if (warp == 8) {
     // ===================== TMA producer =====================
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
     uint32_t stage = 0, phase = 0;
-    {
-      const int32_t m0 = m_blk * GEMM_BLOCK_M;
-      for (uint32_t kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        if (elect_one()) {
-          mbar_arrive_expect_tx(&full_bar[stage], L::STAGE_BYTES);
-          const int32_t k0 = kb * GEMM_BLOCK_K;
-          uint8_t* sa = smem_a + stage * L::A_BYTES;
-          uint8_t* sb = smem_b + stage * L::B_BYTES;
-          if constexpr (!A_MN) {
-            tma_load_2d(sa, &tmap_a, &full_bar[stage], k0, m0);  // box {64 k, 128 m}
-          } else {
+    for (uint32_t kb = 0; kb < num_kb; ++kb) {
+      mbar_wait(&empty_bar[stage], phase ^ 1);
+      if (elect_one()) {
+        mbar_arrive_expect_tx(&full_bar[stage], L::STAGE_BYTES);
+        const int32_t k0 = kb * GEMM_BLOCK_K;
+        uint8_t* sa = smem_a + stage * L::A_BYTES;
+        uint8_t* sb = smem_b + stage * L::B_BYTES;
+        if constexpr (!A_MN) {
+          tma_load_2d(sa, &tmap_a, &full_bar[stage], k0, m0);  // box {64 k, 128 m}
+        } else {
 #pragma unroll
-            for (uint32_t i = 0; i < GEMM_BLOCK_M / 64; ++i)  // box {64 m, 64 k} per 64-wide MN atom
-              tma_load_2d(sa + i * (GEMM_BLOCK_K * 128), &tmap_a, &full_bar[stage], m0 + i * 64, k0);
-          }
-          // B: K-major two boxes {64 k, 128 n}, MN-major four boxes {64 n, 64 k};
-          // this CTA loads its 1 / WIDE_CLUSTER share of them into every CTA of the cluster
-          constexpr uint32_t BOXES = B_MN ? WIDE_N / 64 : 2, BOX_BYTES = L::B_BYTES / BOXES;
-#pragma unroll
-          for (uint32_t j = 0; j < BOXES / WIDE_CLUSTER; ++j) {
-            const uint32_t i = rank * (BOXES / WIDE_CLUSTER) + j;
-            int32_t c0, c1;
-            if constexpr (B_MN) { c0 = n_blk * WIDE_N + i * 64; c1 = k0; }
-            else { c0 = k0; c1 = n_blk * WIDE_N + i * 128; }
-            tma_load_2d_multicast(sb + i * BOX_BYTES, &tmap_b, &full_bar[stage], c0, c1, (1u << WIDE_CLUSTER) - 1);
-          }
+          for (uint32_t i = 0; i < GEMM_BLOCK_M / 64; ++i)  // box {64 m, 64 k} per 64-wide MN atom
+            tma_load_2d(sa + i * (GEMM_BLOCK_K * 128), &tmap_a, &full_bar[stage], m0 + i * 64, k0);
         }
+        // B: K-major two boxes {64 k, 128 n} (SWIGLU: the gate rows n.. and the up rows F + n..), MN-major four boxes
+        // {64 n, 64 k}; this CTA loads its 1 / WIDE_CLUSTER share of them into every CTA of the cluster
+        constexpr uint32_t BOXES = B_MN ? WIDE_N / 64 : 2, BOX_BYTES = L::B_BYTES / BOXES;
+#pragma unroll
+        for (uint32_t j = 0; j < BOXES / WIDE_CLUSTER; ++j) {
+          const uint32_t i = rank * (BOXES / WIDE_CLUSTER) + j;
+          int32_t c0, c1;
+          if constexpr (B_MN) { c0 = n_blk * WIDE_N + i * 64; c1 = k0; }
+          else { c0 = k0; c1 = EPI == EPI_SWIGLU ? col0 + i * ea.F : n_blk * WIDE_N + i * 128; }
+          tma_load_2d_multicast(sb + i * BOX_BYTES, &tmap_b, &full_bar[stage], c0, c1, (1u << WIDE_CLUSTER) - 1);
+        }
+      }
+      __syncwarp();
+      if (++stage == WIDE_STAGES) { stage = 0; phase ^= 1; }
+    }
+    if constexpr (PRE_BOXES > 0) {
+      // The epilogue operand goes into the slots of the stages the ring would refill next, each as soon as the empty
+      // barrier of its stage completes.  This CTA's own empty barrier is enough: it counts the release by the consumers
+      // of both CTAs, and the partner's multicast into the stage had landed before this CTA's full barrier of the
+      // stage's last k-block flipped; no later k-block writes the stage.  The loads are local, not multicast.
+      if (m_blk < num_m) {
+        if (elect_one()) mbar_arrive_expect_tx(epi_full, PRE_BOXES * EPI_BOX_BYTES);
         __syncwarp();
-        if (++stage == WIDE_STAGES) { stage = 0; phase ^= 1; }
+#pragma unroll
+        for (uint32_t v0 = 0; v0 < PRE_BOXES; v0 += 3) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          if (elect_one()) {
+#pragma unroll
+            for (uint32_t v = v0; v < v0 + 3 && v < PRE_BOXES; ++v)   // DSWIGLU: g boxes 0..3, u boxes 4..7
+              tma_load_2d(epi_slot(smem, num_kb, v), &em.m[2 + v / 4], epi_full, col0 + 64 * (v % 4), m0);
+          }
+          __syncwarp();
+          if (++stage == WIDE_STAGES) { stage = 0; phase ^= 1; }
+        }
       }
     }
   } else {
@@ -656,13 +571,14 @@ gemm_bf16_wide(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     constexpr uint32_t A_KADV = A_MN ? (16 * 128) >> 4 : (16 * 2) >> 4;
     constexpr uint32_t B_KADV = B_MN ? (16 * 128) >> 4 : (16 * 2) >> 4;
     constexpr uint32_t A_LBO = A_MN ? GEMM_BLOCK_K * 128 : 0, B_LBO = B_MN ? GEMM_BLOCK_K * 128 : 0;
-    const bool do_add = (flags & GEMM_ADD) != 0;
     uint32_t stage = 0, phase = 0;
     {
       float acc[WIDE_N / 2];
 #pragma unroll
       for (uint32_t i = 0; i < WIDE_N / 2; ++i) acc[i] = 0.f;
       uint32_t prev = 0;
+      // K > 0 (host check): see gemm_bf16_wgmma
+      __builtin_assume(num_kb > 0);
       for (uint32_t kb = 0; kb < num_kb; ++kb) {
         mbar_wait(&full_bar[stage], phase);
         const uint64_t adesc = gmma_desc_sw128(smem_u32(smem_a + stage * L::A_BYTES + wg * 8192), A_LBO, 1024);
@@ -681,27 +597,164 @@ gemm_bf16_wide(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       wgmma_wait<0>();
       reg_fence(acc);
 
-      // ---- epilogue: two passes of 128 bf16 columns; thread = one output row, warpgroup = half of the pass ----
-      const uint32_t row = m_blk * GEMM_BLOCK_M + t;
-      const uint32_t col0 = n_blk * WIDE_N;
+      if constexpr (EPI == EPI_PLAIN) {
+        // ---- epilogue: two passes of 128 bf16 columns; thread = one output row, warpgroup = half of the pass ----
+        const bool do_add = (flags & GEMM_ADD) != 0;
+        const uint32_t row = m_blk * GEMM_BLOCK_M + t;
 #pragma unroll
-      for (uint32_t p = 0; p < 2; ++p) {
-        named_bar_sync(1, GEMM_CONSUMERS);                // the previous pass has drained the staging buffer
+        for (uint32_t p = 0; p < 2; ++p) {
+          named_bar_sync(1, GEMM_CONSUMERS);              // the previous pass has drained the staging buffer
 #pragma unroll
-        for (uint32_t i = 0; i < WIDE_N / 8; ++i) {
-          const int sc = stg_chunk(i, p);
-          if (sc < 0) continue;
-          sts32(stg + stg_offset(r0, sc) + 4 * (lane & 3), pack_bf16x2(acc[4 * i], acc[4 * i + 1]));
-          sts32(stg + stg_offset(r0 + 8, sc) + 4 * (lane & 3), pack_bf16x2(acc[4 * i + 2], acc[4 * i + 3]));
-        }
-        named_bar_sync(1, GEMM_CONSUMERS);
-        if (row >= M) continue;
+          for (uint32_t i = 0; i < WIDE_N / 8; ++i) {
+            const int sc = stg_chunk(i, p);
+            if (sc < 0) continue;
+            sts32(stg + stg_offset(r0, sc) + 4 * (lane & 3), pack_bf16x2(acc[4 * i], acc[4 * i + 1]));
+            sts32(stg + stg_offset(r0 + 8, sc) + 4 * (lane & 3), pack_bf16x2(acc[4 * i + 2], acc[4 * i + 3]));
+          }
+          named_bar_sync(1, GEMM_CONSUMERS);
+          if (row >= M) continue;
 #pragma unroll 1
           for (uint32_t h = 0; h < 2; ++h) {              // chunks 4 wg + 8 h.. = tile columns 128 h + 64 p + 32 wg ..
             uint32_t v[16];
             ld_stg32(stg, t, 8 * h + 4 * wg, v);
             store_plain32(v, Cout, ldc, addend, ld_add, row, col0 + 128 * h + 64 * p + 32 * wg, N, do_add);
           }
+        }
+      } else {
+        // ---- fused epilogues: bf16 boxes in the stage ring, TMA stores ----
+        named_bar_sync(1, GEMM_CONSUMERS);                // both warpgroups are past their last wgmma
+        if (m_blk < num_m) {                              // (the partner past M stores nothing)
+          uint8_t* slot[8];
+#pragma unroll
+          for (uint32_t v = 0; v < 8; ++v) slot[v] = epi_slot(smem, num_kb, v);
+          // boxes to store: (slot, map, column); DSWIGLU stores in place over g and u
+          constexpr uint32_t OUT_BOXES = EPI == EPI_SWIGLU ? 6 : EPI == EPI_DSWIGLU ? 8 : 4;
+          constexpr uint32_t OUT_SLOT0 = EPI == EPI_ATTND ? 4 : 0;
+          if constexpr (EPI == EPI_SWIGLU) {
+            // g in slots 0, 1, u in 2, 3, h in 4, 5:  h = bf16(silu(g) * u) on the bf16 g and u
+#pragma unroll
+            for (uint32_t i = 0; i < 16; ++i) {
+#pragma unroll
+              for (uint32_t h = 0; h < 2; ++h) {
+                const uint32_t g = pack_bf16x2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+                const uint32_t u = pack_bf16x2(acc[4 * (i + 16) + 2 * h], acc[4 * (i + 16) + 2 * h + 1]);
+                const uint32_t off = frag_offset(r0 + 8 * h, i, lane);
+                sts32(smem_u32(slot[i / 8]) + off, g);
+                sts32(smem_u32(slot[2 + i / 8]) + off, u);
+                sts32(smem_u32(slot[4 + i / 8]) + off,
+                      pack_bf16x2(silu_bf16(bf16_lo(g)) * bf16_lo(u), silu_bf16(bf16_hi(g)) * bf16_hi(u)));
+              }
+            }
+          } else if constexpr (EPI == EPI_DSWIGLU) {
+            // acc = dh; g in slots 0..3 and u in 4..7 are replaced by dg = dh*u*silu'(g) and du = dh*silu(g)
+            mbar_wait(epi_full, 0);
+#pragma unroll
+            for (uint32_t i = 0; i < 32; ++i) {
+#pragma unroll
+              for (uint32_t h = 0; h < 2; ++h) {
+                const uint32_t off = frag_offset(r0 + 8 * h, i, lane);
+                const uint32_t ga = smem_u32(slot[i / 8]) + off, ua = smem_u32(slot[4 + i / 8]) + off;
+                const uint32_t gp = lds32(ga), up = lds32(ua);
+                float dg[2], du[2];
+#pragma unroll
+                for (uint32_t e = 0; e < 2; ++e) {
+                  const float d = bf16_round(acc[4 * i + 2 * h + e]);   // dh as the unfused path stores it
+                  const float gv = e ? bf16_hi(gp) : bf16_lo(gp);
+                  const float uv = e ? bf16_hi(up) : bf16_lo(up);
+                  const float sg = 1.f / (1.f + __expf(-gv));
+                  dg[e] = d * uv * (sg * (1.f + gv * (1.f - sg)));
+                  du[e] = d * (gv * sg);
+                }
+                sts32(ga, pack_bf16x2(dg[0], dg[1]));
+                sts32(ua, pack_bf16x2(du[0], du[1]));
+              }
+            }
+          } else if constexpr (EPI == EPI_ROPE) {
+            // projection output rounded to bf16 first (the reference ropes the bf16 q/k); column c < 64 of a head
+            // (group i) pairs with c + 64 (group i + 8).  Both heads of the tile share the cos / sin of a row.
+            const bool rope0 = col0 < ea.rope_cols, rope1 = col0 + 128 < ea.rope_cols;
+            int p[2];
+#pragma unroll
+            for (uint32_t h = 0; h < 2; ++h) p[h] = m0 + r0 + 8 * h < M ? ea.pos[m0 + r0 + 8 * h] : 0;
+#pragma unroll
+            for (uint32_t i = 0; i < 8; ++i) {
+#pragma unroll
+              for (uint32_t h = 0; h < 2; ++h) {
+                const uint32_t c = 8 * i + 2 * (lane & 3), off = frag_offset(r0 + 8 * h, i, lane);
+                uint32_t c1 = 0, s1 = 0, c2 = 0, s2 = 0;
+                if (rope0) {
+                  const int64_t b = static_cast<int64_t>(p[h]) * 128 + c;
+                  c1 = *reinterpret_cast<const uint32_t*>(ea.cos_t + b);
+                  s1 = *reinterpret_cast<const uint32_t*>(ea.sin_t + b);
+                  c2 = *reinterpret_cast<const uint32_t*>(ea.cos_t + b + 64);
+                  s2 = *reinterpret_cast<const uint32_t*>(ea.sin_t + b + 64);
+                }
+#pragma unroll
+                for (uint32_t hd = 0; hd < 2; ++hd) {
+                  const uint32_t ia = 16 * hd + i, ib = ia + 8;
+                  const uint32_t xa = pack_bf16x2(acc[4 * ia + 2 * h], acc[4 * ia + 2 * h + 1]);
+                  const uint32_t xb = pack_bf16x2(acc[4 * ib + 2 * h], acc[4 * ib + 2 * h + 1]);
+                  uint32_t o1 = xa, o2 = xb;
+                  if (hd ? rope1 : rope0) {
+                    const float y1l = bf16_round(bf16_lo(xa) * bf16_lo(c1)) + bf16_round(-bf16_lo(xb) * bf16_lo(s1));
+                    const float y1h = bf16_round(bf16_hi(xa) * bf16_hi(c1)) + bf16_round(-bf16_hi(xb) * bf16_hi(s1));
+                    const float y2l = bf16_round(bf16_lo(xb) * bf16_lo(c2)) + bf16_round(bf16_lo(xa) * bf16_lo(s2));
+                    const float y2h = bf16_round(bf16_hi(xb) * bf16_hi(c2)) + bf16_round(bf16_hi(xa) * bf16_hi(s2));
+                    o1 = pack_bf16x2(y1l, y1h);
+                    o2 = pack_bf16x2(y2l, y2h);
+                  }
+                  sts32(smem_u32(slot[2 * hd]) + off, o1);
+                  sts32(smem_u32(slot[2 * hd + 1]) + off, o2);
+                }
+              }
+            }
+          } else {
+            // ATTND: bf16 dO in slots 4..7 (O is prefetched into 0..3)
+#pragma unroll
+            for (uint32_t i = 0; i < 32; ++i) {
+#pragma unroll
+              for (uint32_t h = 0; h < 2; ++h)
+                sts32(smem_u32(slot[4 + i / 8]) + frag_offset(r0 + 8 * h, i, lane),
+                      pack_bf16x2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]));
+            }
+          }
+          fence_proxy_async_smem();                       // generic-proxy writes -> TMA store reads
+          named_bar_sync(1, GEMM_CONSUMERS);
+          if (threadIdx.x == 0) {
+            const uint32_t ncols = EPI == EPI_SWIGLU || EPI == EPI_DSWIGLU ? ea.F : N;
+#pragma unroll
+            for (uint32_t b = 0; b < OUT_BOXES; ++b) {
+              // SWIGLU: boxes 0, 1 g, 2, 3 u, 4, 5 h;  DSWIGLU: 0..3 dg, 4..7 du;  ROPE / ATTND: 0..3
+              const uint32_t map = EPI == EPI_SWIGLU ? b / 2 : EPI == EPI_DSWIGLU ? b / 4 : 0;
+              const uint32_t col = col0 + 64 * (EPI == EPI_SWIGLU ? b % 2 : b % 4);
+              if (EPI == EPI_SWIGLU && map < 2 && (flags & GEMM_NO_GU)) continue;
+              if (col < ncols) tma_store_2d(&em.m[map], slot[OUT_SLOT0 + b], col, m0);
+            }
+            tma_store_commit();
+          }
+          if constexpr (EPI == EPI_ATTND) {
+            // D[h, t] = sum_d dO[t, h, d] * O[t, h, d]: thread = one row of the head of its warpgroup, summed in the
+            // order of the row kernel (32-column chunks, then 8-element groups)
+            mbar_wait(epi_full, 0);
+            const uint32_t hc = col0 + wg * 128;
+            if (hc < N && m0 + t < M) {
+              float dsum = 0.f;
+#pragma unroll
+              for (uint32_t c = 0; c < 128; c += 32) {
+#pragma unroll
+                for (uint32_t j = 0; j < 32; j += 8) {
+                  const uint32_t bb = (c + j) / 64, off = sw128_offset(t, ((c + j) % 64) / 8);   // box 2 wg + bb
+                  const uint4 o = lds128(smem_u32(wg ? slot[6 + bb] : slot[4 + bb]) + off);
+                  const uint4 a = lds128(smem_u32(wg ? slot[2 + bb] : slot[bb]) + off);
+                  dsum += bf16_lo(o.x) * bf16_lo(a.x) + bf16_hi(o.x) * bf16_hi(a.x) + bf16_lo(o.y) * bf16_lo(a.y) + bf16_hi(o.y) * bf16_hi(a.y)
+                        + bf16_lo(o.z) * bf16_lo(a.z) + bf16_hi(o.z) * bf16_hi(a.z) + bf16_lo(o.w) * bf16_lo(a.w) + bf16_hi(o.w) * bf16_hi(a.w);
+                }
+              }
+              ea.dvec[static_cast<int64_t>(hc >> 7) * M + m0 + t] = dsum;
+            }
+          }
+          if (threadIdx.x == 0) tma_store_wait_read<0>();   // the boxes stay in shared memory until the TMA read them
+        }
       }
     }
   }
@@ -709,10 +762,11 @@ gemm_bf16_wide(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   cluster_sync_all();   // no CTA exits while its peer can still multicast into it or arrive on its barriers
 }
 
-template <bool A_MN, bool B_MN>
+template <bool A_MN, bool B_MN, int EPI = EPI_PLAIN>
 static int launch_wide(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int64_t ldc, const void* addend,
-                       int64_t ld_add, uint32_t M, uint32_t N, uint32_t K, uint32_t flags, cudaStream_t stream) {
-  auto kern = gemm_bf16_wide<A_MN, B_MN>;
+                       int64_t ld_add, uint32_t M, uint32_t N, uint32_t K, uint32_t flags, cudaStream_t stream,
+                       const EpiMaps& em = EpiMaps{}, EpiAux ea = EpiAux{}) {
+  auto kern = gemm_bf16_wide<A_MN, B_MN, EPI>;
   cudaLaunchConfig_t cfg = {};
   cfg.blockDim = dim3(GEMM_THREADS);
   cfg.dynamicSmemBytes = WideSmem::DYN_BYTES;
@@ -729,10 +783,11 @@ static int launch_wide(const CUtensorMap& ta, const CUtensorMap& tb, void* C, in
     NV_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, WideSmem::DYN_BYTES));
     attr_set = true;
   }
-  const uint32_t pairs = ceil_div_u32(ceil_div_u32(M, GEMM_BLOCK_M), WIDE_CLUSTER) * ceil_div_u32(N, WIDE_N);
+  const uint32_t pairs = ceil_div_u32(ceil_div_u32(M, GEMM_BLOCK_M), WIDE_CLUSTER) *
+                         ceil_div_u32(N, EPI == EPI_SWIGLU ? 128u : WIDE_N);
   cfg.gridDim = dim3(WIDE_CLUSTER * pairs);
-  NV_CUDA(cudaLaunchKernelEx(&cfg, kern, ta, tb, C, ldc, reinterpret_cast<const __nv_bfloat16*>(addend), ld_add, M, N, K,
-                             flags));
+  NV_CUDA(cudaLaunchKernelEx(&cfg, kern, ta, tb, em, C, ldc, reinterpret_cast<const __nv_bfloat16*>(addend), ld_add, M,
+                             N, K, flags, ea));
   return NV_OK;
 }
 
@@ -826,8 +881,8 @@ extern "C" int nv_gemm_fp8w_bf16(const void* A, int64_t lda, const void* Wq, int
   const uint32_t flags = addend ? GEMM_ADD : 0u;
   // stages: the bf16 kernel's 10 at BLOCK_N = 32; 5 of 40 KB (A, e4m3 B, expanded B) fit at 128
   if (block_n == 32)
-    return launch_gemm<32, 10, false, false, EPI_PLAIN, uint8_t>(ta, tb, C, ldc, addend, ld_add, M, N, K, flags, stream, ea);
-  return launch_gemm<128, 5, false, false, EPI_PLAIN, uint8_t>(ta, tb, C, ldc, addend, ld_add, M, N, K, flags, stream, ea);
+    return launch_gemm<32, 10, false, false, uint8_t>(ta, tb, C, ldc, addend, ld_add, M, N, K, flags, stream, ea);
+  return launch_gemm<128, 5, false, false, uint8_t>(ta, tb, C, ldc, addend, ld_add, M, N, K, flags, stream, ea);
 }
 
 // ---- fused-epilogue entry points (K-major activations x nn.Linear weights) -------------------------------------
@@ -842,10 +897,18 @@ int nv_gemm_swiglu_bf16(const void* x, int64_t ldx, const void* Wgu, int64_t ldw
   CUtensorMap ta, tb;
   int rc = gemm_tmaps(&ta, &tb, x, ldx, 0, Wgu, ldw, 0, M, 2 * F, K, 256, (uint64_t)2 * F);
   if (rc) return rc;
+  EpiMaps em{};
+  if (keep_gu) {
+    if ((rc = make_tmap_2d(&em.m[0], gu, 2, (uint64_t)F, (uint64_t)M, (uint64_t)ldgu * 2, 64, GEMM_BLOCK_M))) return rc;
+    if ((rc = make_tmap_2d(&em.m[1], static_cast<__nv_bfloat16*>(gu) + F, 2, (uint64_t)F, (uint64_t)M, (uint64_t)ldgu * 2, 64,
+                           GEMM_BLOCK_M)))
+      return rc;
+  }
+  if ((rc = make_tmap_2d(&em.m[2], h, 2, (uint64_t)F, (uint64_t)M, (uint64_t)ldh * 2, 64, GEMM_BLOCK_M))) return rc;
   EpiAux ea{};
-  ea.aux = h; ea.ld_aux = ldh; ea.F = (uint32_t)F;
-  return launch_gemm<256, 4, false, false, EPI_SWIGLU>(ta, tb, gu, ldgu, nullptr, 0, M, F, K, keep_gu ? 0u : GEMM_NO_GU,
-                                                       reinterpret_cast<cudaStream_t>(stream), ea);
+  ea.F = (uint32_t)F;
+  return launch_wide<false, false, EPI_SWIGLU>(ta, tb, gu, ldgu, nullptr, 0, M, F, K, keep_gu ? 0u : GEMM_NO_GU,
+                                               reinterpret_cast<cudaStream_t>(stream), em, ea);
 }
 
 // dgu[T,2F] = swiglu'(gu) applied to dh = dx[T,D] · Wd[D,F]   (Wd is the nn.Linear weight [D, F]: B stored [K=D, N=F]).
@@ -857,10 +920,17 @@ int nv_gemm_dswiglu_bf16(const void* dx, int64_t lddx, const void* Wd, int64_t l
   CUtensorMap ta, tb;
   int rc = gemm_tmaps(&ta, &tb, dx, lddx, 0, Wd, ldw, 1, M, F, D, 256, (uint64_t)F);
   if (rc) return rc;
+  EpiMaps em{};
+  const __nv_bfloat16* halves[4] = {static_cast<const __nv_bfloat16*>(dgu), static_cast<const __nv_bfloat16*>(dgu) + F,
+                                    static_cast<const __nv_bfloat16*>(gu), static_cast<const __nv_bfloat16*>(gu) + F};
+  for (int i = 0; i < 4; ++i)
+    if ((rc = make_tmap_2d(&em.m[i], halves[i], 2, (uint64_t)F, (uint64_t)M, (uint64_t)(i < 2 ? lddgu : ldgu) * 2, 64,
+                           GEMM_BLOCK_M)))
+      return rc;
   EpiAux ea{};
-  ea.aux = const_cast<void*>(gu); ea.ld_aux = ldgu; ea.F = (uint32_t)F;
-  return launch_gemm<256, 4, false, true, EPI_DSWIGLU>(ta, tb, dgu, lddgu, nullptr, 0, M, F, D, 0u,
-                                                       reinterpret_cast<cudaStream_t>(stream), ea);
+  ea.F = (uint32_t)F;
+  return launch_wide<false, true, EPI_DSWIGLU>(ta, tb, dgu, lddgu, nullptr, 0, M, F, D, 0u,
+                                               reinterpret_cast<cudaStream_t>(stream), em, ea);
 }
 
 // dO[T, D] = dY[T, Dout] · Wo[Dout, D]  (o_proj dgrad; Wo is the nn.Linear weight, B stored [K = Dout, N = D]) and, in the
@@ -873,10 +943,13 @@ int nv_gemm_attnd_bf16(const void* dy, int64_t lddy, const void* Wo, int64_t ldw
   CUtensorMap ta, tb;
   int rc = gemm_tmaps(&ta, &tb, dy, lddy, 0, Wo, ldw, 1, M, D, Dout, 256, (uint64_t)D);
   if (rc) return rc;
+  EpiMaps em{};
+  if ((rc = make_tmap_2d(&em.m[0], dout, 2, (uint64_t)D, (uint64_t)M, (uint64_t)lddo * 2, 64, GEMM_BLOCK_M))) return rc;
+  if ((rc = make_tmap_2d(&em.m[2], o, 2, (uint64_t)D, (uint64_t)M, (uint64_t)ldo * 2, 64, GEMM_BLOCK_M))) return rc;
   EpiAux ea{};
-  ea.aux = const_cast<void*>(o); ea.ld_aux = ldo; ea.dvec = dvec;
-  return launch_gemm<256, 4, false, true, EPI_ATTND>(ta, tb, dout, lddo, nullptr, 0, M, D, Dout, 0u,
-                                                     reinterpret_cast<cudaStream_t>(stream), ea);
+  ea.dvec = dvec;
+  return launch_wide<false, true, EPI_ATTND>(ta, tb, dout, lddo, nullptr, 0, M, D, Dout, 0u,
+                                             reinterpret_cast<cudaStream_t>(stream), em, ea);
 }
 
 // qkv[T, N] = x[T,K] · Wqkv[N,K]^T with rotate-half RoPE applied to the first rope_cols columns (q and k heads).
@@ -888,11 +961,13 @@ int nv_gemm_rope_bf16(const void* x, int64_t ldx, const void* W, int64_t ldw, vo
   CUtensorMap ta, tb;
   int rc = gemm_tmaps(&ta, &tb, x, ldx, 0, W, ldw, 0, M, N, K, 256, (uint64_t)N);
   if (rc) return rc;
+  EpiMaps em{};
+  if ((rc = make_tmap_2d(&em.m[0], out, 2, (uint64_t)N, (uint64_t)M, (uint64_t)ldo * 2, 64, GEMM_BLOCK_M))) return rc;
   EpiAux ea{};
   ea.pos = pos; ea.cos_t = reinterpret_cast<const __nv_bfloat16*>(cos_t); ea.sin_t = reinterpret_cast<const __nv_bfloat16*>(sin_t);
   ea.rope_cols = (uint32_t)rope_cols;
-  return launch_gemm<256, 4, false, false, EPI_ROPE>(ta, tb, out, ldo, nullptr, 0, M, N, K, 0u,
-                                                     reinterpret_cast<cudaStream_t>(stream), ea);
+  return launch_wide<false, false, EPI_ROPE>(ta, tb, out, ldo, nullptr, 0, M, N, K, 0u,
+                                             reinterpret_cast<cudaStream_t>(stream), em, ea);
 }
 
 }  // extern "C"

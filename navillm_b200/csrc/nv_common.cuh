@@ -59,6 +59,11 @@ __device__ __forceinline__ uint4 lds128(uint32_t saddr) {
   asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(saddr) : "memory");
   return v;
 }
+__device__ __forceinline__ uint32_t lds32(uint32_t saddr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(saddr) : "memory");
+  return v;
+}
 __device__ __forceinline__ uint2 lds64(uint32_t saddr) {
   uint2 v;
   asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(saddr) : "memory");

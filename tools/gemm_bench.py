@@ -89,7 +89,7 @@ def main():
         print(json.dumps(res), flush=True)
         del A, B, C
 
-    # fused epilogues (128 x 256 tile only)
+    # fused epilogues (128 x 256 tile only), each with its rate over its plain counterpart's 256-wide rate in this run
     from navillm_b200.llama import LlamaDims, rope_tables
     g = torch.Generator(device="cpu").manual_seed(0)
     x = (torch.randn(T, d, generator=g) * 0.5).to(dev, torch.bfloat16)
@@ -107,15 +107,18 @@ def main():
     dvec = torch.empty(32 * T, device=dev, dtype=torch.float32)
     ops.gemm_swiglu(x, wgu, gu=gu, h=h)
     fused = [
-        ("gateup_fwd_swiglu", T, 2 * F, d, lambda: ops.gemm_swiglu(x, wgu, gu=gu, h=h)),
-        ("qkv_fwd_rope", T, 3 * d, d, lambda: ops.gemm_rope(x, wqkv, pos, cos_t, sin_t, 2 * d, out=qkv)),
-        ("down_dgrad_dswiglu", T, F, d, lambda: ops.gemm_dswiglu(x, wd, gu, dgu=dgu)),
-        ("o_dgrad_attnd", T, d, d, lambda: ops.gemm_attnd(x, wo, x, dout=dout, dvec=dvec)),
+        ("gateup_fwd_swiglu", "gateup_fwd", T, 2 * F, d, lambda: ops.gemm_swiglu(x, wgu, gu=gu, h=h)),
+        ("qkv_fwd_rope", "qkv_fwd", T, 3 * d, d, lambda: ops.gemm_rope(x, wqkv, pos, cos_t, sin_t, 2 * d, out=qkv)),
+        ("down_dgrad_dswiglu", "down_dgrad", T, F, d, lambda: ops.gemm_dswiglu(x, wd, gu, dgu=dgu)),
+        ("o_dgrad_attnd", "o_dgrad", T, d, d, lambda: ops.gemm_attnd(x, wo, x, dout=dout, dvec=dvec)),
     ]
-    for name, M, N, K, fn in fused:
+    plain = {r["name"]: r["nv_bn256_tflops"] for r in rows}
+    for name, plain_name, M, N, K, fn in fused:
         ms = timeit(fn, iters=a.iters, warmup=a.warmup)
-        res = {"name": name, "M": M, "N": N, "K": K, "nv_bn256_ms": ms, "nv_bn256_tflops": 2.0 * M * N * K / ms / 1e9,
-               "nv_bn256_sm_clock_mhz": smi("clocks.sm")}
+        tflops = 2.0 * M * N * K / ms / 1e9
+        res = {"name": name, "M": M, "N": N, "K": K, "nv_bn256_ms": ms, "nv_bn256_tflops": tflops,
+               "nv_bn256_sm_clock_mhz": smi("clocks.sm"), "plain": plain_name,
+               "ratio_to_plain": tflops / plain[plain_name] if plain_name in plain else None}
         rows.append(res)
         print(json.dumps(res), flush=True)
     if a.json:
