@@ -118,6 +118,19 @@ int nv_attn_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const vo
                 int64_t ldo, const void* dout, int64_t lddo, const float* lse, float* dvec, void* dq, int64_t lddq,
                 void* dk, int64_t lddk, void* dv, int64_t lddv, const int* cu_seqlens, int B, int T, int H, int head_dim,
                 int total_blocks, float scale, const int* rope_pos, const void* cos_t, const void* sin_t, void* stream);
+/* Backward of nv_attn_fwd_kv (no reference counterpart: the reference re-encodes every prompt).  q, o, dout, lse, dvec,
+ * dq, dk, dv: the Tq packed suffix rows as in nv_attn_bwd; kcache / vcache: bf16 [Tkv, H*128] (leading dimension ldkv),
+ * K/V of sequence b at rows kv_start[b] .. +kv_len[b]; acc_k / acc_v: fp32 [Tkv, >= H*128] (ldacc) gradient accumulators
+ * over the cache rows.  Key row j of sequence b with c = kv_len[b] - q_len[b]: j < c -> acc[kv_start[b] + j] += (dK, dV);
+ * j >= c -> dk / dv at its packed row = bf16(dK + acc_k), bf16(dV + acc_v) (acc only read), dk then rotated back by
+ * -theta[rope_pos] when rope_pos is given (as dq).  kv_len == q_len (c = 0) adds the accumulated gradient of cached rows
+ * to a recomputed prefix's own.  Deterministic (no atomics).  total_qblocks = sum_b ceil(q_len/128), total_kblocks =
+ * sum_b ceil(kv_len/128). */
+int nv_attn_bwd_kv(const void* q, int64_t ldq, const void* kcache, const void* vcache, int64_t ldkv, const void* o, int64_t ldo,
+                   const void* dout, int64_t lddo, const float* lse, float* dvec, void* dq, int64_t lddq, void* dk, int64_t lddk,
+                   void* dv, int64_t lddv, float* acc_k, float* acc_v, int64_t ldacc, const int* cu_seqlens,
+                   const int* kv_start, const int* kv_len, int B, int Tq, int Tkv, int H, int head_dim, int total_qblocks,
+                   int total_kblocks, float scale, const int* rope_pos, const void* cos_t, const void* sin_t, void* stream);
 /* Developer hook (no reference counterpart) for an in-kernel phase trace of the attention kernels.  The sm_90a kernels
  * record none: returns 0 (words copied). */
 int nv_debug_attn_trace(int kernel, unsigned long long* out, int max_words);

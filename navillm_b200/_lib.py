@@ -56,7 +56,7 @@ class LayerArgs(ctypes.Structure):
 launch_count = 0          # kernels launched through the C ABI since import (bench.py reports the per-step delta)
 
 # entry points that launch more than one kernel per call
-_MULTI = {"nv_rmsnorm_bwd": 2, "nv_attn_bwd": 3, "nv_layernorm_bwd": 3, "nv_head_bwd": 2, "nv_mha_bwd": 2, "nv_llama_layer_infer": 10}
+_MULTI = {"nv_rmsnorm_bwd": 2, "nv_attn_bwd": 3, "nv_attn_bwd_kv": 3, "nv_layernorm_bwd": 3, "nv_head_bwd": 2, "nv_mha_bwd": 2, "nv_llama_layer_infer": 10}
 
 
 def check(status: int, what: str) -> None:

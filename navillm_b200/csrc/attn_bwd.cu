@@ -43,6 +43,19 @@ __device__ __forceinline__ bool locate_block_bwd(const int* __restrict__ cu, int
   return false;
 }
 
+// KV form: the 128-row blocks of sequence b are counted over blk_len[b] rows (kv_len for the key blocks of the dk/dv pass,
+// the suffix length for the query blocks of the dq pass); seq is the sequence index.
+__device__ __forceinline__ bool locate_block_kv(const int* __restrict__ cu, const int* __restrict__ blk_len, int B,
+                                                uint32_t blk, int& seq_start, int& seq_len, uint32_t& idx, int& seq) {
+  for (int b = 0; b < B; ++b) {
+    const int s = cu[b], len = cu[b + 1] - s;
+    const uint32_t n = ((uint32_t)(blk_len != nullptr ? blk_len[b] : len) + 127) / 128;
+    if (blk < n) { seq_start = s; seq_len = len; idx = blk; seq = b; return true; }
+    blk -= n;
+  }
+  return false;
+}
+
 // D[h, t] = sum_d dO[t, h*128+d] * O[t, h*128+d]   (one warp per (t, h))
 __global__ void attn_bwd_prep_kernel(const __nv_bfloat16* __restrict__ O, int64_t ldo,
                                      const __nv_bfloat16* __restrict__ dO, int64_t lddo, float* __restrict__ D, int T,
@@ -184,13 +197,16 @@ __device__ __forceinline__ void bwd_load_refill(uint8_t* smem, uint64_t* st_full
 // ======================================================================================================
 // dq pass
 // ======================================================================================================
+// KV = true (nv_attn_bwd_kv): the keys / values of sequence b are rows kv_start[b] .. +kv_len[b] of a cache (tmap_k /
+// tmap_v), the queries its last seq_len positions: query i sees keys <= dk + i, dk = kv_len[b] - seq_len (as attn_fwd_kv).
+template <bool KV>
 __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_do,
                    const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v,
                    const float* __restrict__ lse, const float* __restrict__ Dvec, __nv_bfloat16* __restrict__ dq,
                    int64_t lddq, const int* __restrict__ cu_seqlens, int B, int T, float scale,
                    const int* __restrict__ rope_pos, const __nv_bfloat16* __restrict__ cos_t,
-                   const __nv_bfloat16* __restrict__ sin_t) {
+                   const __nv_bfloat16* __restrict__ sin_t, const int* __restrict__ kv_start, const int* __restrict__ kv_len) {
   using L = BwdSmem;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -202,10 +218,22 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_cons
   const uint32_t warp = warp_id_uniform(), lane = threadIdx.x & 31;
   const uint32_t head = blockIdx.y;
   int seq_start = 0, seq_len = 0;
-  uint32_t own = 0;
-  if (!locate_block_bwd(cu_seqlens, B, gridDim.x - 1 - blockIdx.x, seq_start, seq_len, own)) return;  // heavy first
-  // 64-key sub-blocks 0 .. n_sub-1 cover keys [0, min((own+1)*128, len))
-  const uint32_t n_sub = min(2 * own + 2, (uint32_t)(seq_len + 63) / 64);
+  uint32_t own = 0, dk = 0;
+  int kv0 = 0;
+  uint32_t n_sub;
+  if constexpr (KV) {
+    int seq = 0;
+    if (!locate_block_kv(cu_seqlens, nullptr, B, gridDim.x - 1 - blockIdx.x, seq_start, seq_len, own, seq)) return;
+    dk = (uint32_t)(kv_len[seq] - seq_len);
+    kv0 = kv_start[seq];
+    // 64-key sub-blocks 0 .. n_sub-1 cover keys [0, dk + min((own+1)*128, len))
+    n_sub = (dk + min((own + 1) * 128, (uint32_t)seq_len) + 63) / 64;
+  } else {
+    if (!locate_block_bwd(cu_seqlens, B, gridDim.x - 1 - blockIdx.x, seq_start, seq_len, own)) return;  // heavy first
+    kv0 = seq_start;
+    // 64-key sub-blocks 0 .. n_sub-1 cover keys [0, min((own+1)*128, len))
+    n_sub = min(2 * own + 2, (uint32_t)(seq_len + 63) / 64);
+  }
 
   if (threadIdx.x == 0) {
     mbar_init(res_full, 1);
@@ -216,7 +244,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_cons
 
   if (threadIdx.x == 0)
     bwd_load_prologue(smem, res_full, st_full, &tmap_q, &tmap_do, &tmap_k, &tmap_v, head * 128, seq_start + own * 128,
-                      seq_start, n_sub);
+                      kv0, n_sub);
 
   const uint32_t wg = warp >> 2;
   const uint32_t ra = wg * 64 + (warp & 3) * 16 + (lane >> 2);    // rows ra, ra + 8 of the block
@@ -245,7 +273,8 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_cons
     wgmma_wait<0>();
     reg_fence(sacc);
     reg_fence(dpacc);
-    const bool diag = (n >= 2 * own);                     // sub-blocks that touch the diagonal 128x128 block
+    // sub-blocks that touch the diagonal 128x128 block
+    const bool diag = KV ? (n * 64 + 63 > dk + own * 128) : (n >= 2 * own);
 #pragma unroll
     for (uint32_t i = 0; i < 8; ++i) {
 #pragma unroll
@@ -253,7 +282,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_cons
         const uint32_t key = n * 64 + 8 * i + cq + (e & 1);
         const uint32_t q = (e & 2) ? qb : qa;
         float p = exp2f(fmaf(sacc[4 * i + e], sl2, -((e & 2) ? lb : la)));
-        if (diag && key > q) p = 0.f;
+        if (diag && key > dk + q) p = 0.f;
         // dS = P o (dP - D) * scale
         sacc[4 * i + e] = p * ((dpacc[4 * i + e] - ((e & 2) ? db : da)) * scale);
       }
@@ -271,7 +300,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_cons
     wgmma_wait<0>();
     reg_fence(dqacc);
     if ((threadIdx.x & 127) == 0) mbar_arrive(&st_empty[st]);
-    if (threadIdx.x == 0) bwd_load_refill(smem, st_full, st_empty, &tmap_k, &tmap_v, head * 128, seq_start, n, n_sub);
+    if (threadIdx.x == 0) bwd_load_refill(smem, st_full, st_empty, &tmap_k, &tmap_v, head * 128, kv0, n, n_sub);
   }
   compute_warps_sync();                                     // every operand stage is free
   uint8_t* stage = smem + L::RES_OFF;
@@ -286,13 +315,20 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_cons
 // ======================================================================================================
 // dk/dv pass (transposed scores: accumulator rows = keys)
 // ======================================================================================================
+// KV = true (nv_attn_bwd_kv): the CTA owns a 128-key block of [0, kv_len[b]) of the cache (tmap_k / tmap_v rows kv_start[b]
+// + ...) and streams the suffix queries that see it.  Epilogue by key row j: j < dk (cached rows) -> acc_k / acc_v
+// [kv_start[b] + j] += (dK, dV) in fp32 (read-modify-write: each (row, head) slice has one owning CTA, no atomics); j >= dk
+// (the suffix's own rows) -> dK + acc_k and dV + acc_v, rounded once, into packed row seq_start + j - dk of dk / dv.
+template <bool KV>
 __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                     const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_do,
                     const float* __restrict__ lse, const float* __restrict__ Dvec, __nv_bfloat16* __restrict__ dk,
                     int64_t lddk, __nv_bfloat16* __restrict__ dv, int64_t lddv, const int* __restrict__ cu_seqlens,
                     int B, int T, float scale, const int* __restrict__ rope_pos,
-                    const __nv_bfloat16* __restrict__ cos_t, const __nv_bfloat16* __restrict__ sin_t) {
+                    const __nv_bfloat16* __restrict__ cos_t, const __nv_bfloat16* __restrict__ sin_t,
+                    const int* __restrict__ kv_start, const int* __restrict__ kv_len, float* __restrict__ acc_k,
+                    float* __restrict__ acc_v, int64_t ldacc) {
   using L = BwdSmem;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -304,10 +340,23 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
   const uint32_t warp = warp_id_uniform(), lane = threadIdx.x & 31;
   const uint32_t head = blockIdx.y;
   int seq_start = 0, seq_len = 0;
-  uint32_t own = 0;
-  if (!locate_block_bwd(cu_seqlens, B, blockIdx.x, seq_start, seq_len, own)) return;   // early key blocks are the heavy ones
-  // 64-query sub-blocks first .. n_qsub-1 can see keys of this block (causal): q >= own*128
-  const uint32_t first = 2 * own, n_qsub = (uint32_t)(seq_len + 63) / 64;
+  uint32_t own = 0, first, cdk = 0, klen = 0;
+  int kv0 = 0;
+  if constexpr (KV) {
+    int seq = 0;
+    if (!locate_block_kv(cu_seqlens, kv_len, B, blockIdx.x, seq_start, seq_len, own, seq)) return;
+    klen = (uint32_t)kv_len[seq];
+    cdk = klen - (uint32_t)seq_len;
+    kv0 = kv_start[seq];
+    // the first query that sees key own*128 is own*128 - cdk (clamped at 0)
+    first = own * 128 > cdk ? (own * 128 - cdk) / 64 : 0u;
+  } else {
+    if (!locate_block_bwd(cu_seqlens, B, blockIdx.x, seq_start, seq_len, own)) return;   // early key blocks are the heavy ones
+    kv0 = seq_start;
+    // 64-query sub-blocks first .. n_qsub-1 can see keys of this block (causal): q >= own*128
+    first = 2 * own;
+  }
+  const uint32_t n_qsub = (uint32_t)(seq_len + 63) / 64;
   const uint32_t n_it = n_qsub - first;
 
   if (threadIdx.x == 0) {
@@ -318,12 +367,15 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
   __syncthreads();
 
   if (threadIdx.x == 0)
-    bwd_load_prologue(smem, res_full, st_full, &tmap_k, &tmap_v, &tmap_q, &tmap_do, head * 128, seq_start + own * 128,
+    bwd_load_prologue(smem, res_full, st_full, &tmap_k, &tmap_v, &tmap_q, &tmap_do, head * 128, kv0 + own * 128,
                       seq_start + first * 64, n_it);
 
   const uint32_t wg = warp >> 2;
   const uint32_t ra = wg * 64 + (warp & 3) * 16 + (lane >> 2);    // key rows ra, ra + 8 of the block
   const uint32_t ka = own * 128 + ra, kb = ka + 8;
+  // KV: key rows relative to the cached count (query q sees key k iff q >= k - cdk), and the first query sub-block row
+  // past which every key of the block is visible
+  const int ea = (int)ka - (int)cdk, eb = ea + 8, dlim = (int)(own * 128 + 127) - (int)cdk;
   const uint32_t cq = 2 * (lane & 3);
   const float sl2 = scale * LOG2E;
   const uint32_t sK = smem_u32(smem + L::RES_OFF) + wg * 8192, sV = sK + AB_T128;
@@ -357,7 +409,8 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
     wgmma_wait<0>();
     reg_fence(sacc);
     reg_fence(dpacc);
-    const bool diag = (first + n) < 2 * own + 2;            // query sub-blocks inside the diagonal 128x128 block
+    // query sub-blocks inside the diagonal 128x128 block
+    const bool diag = KV ? ((int)q0 < dlim) : ((first + n) < 2 * own + 2);
 #pragma unroll
     for (uint32_t i = 0; i < 8; ++i) {
 #pragma unroll
@@ -365,7 +418,11 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
         const uint32_t c = 2 * i + (e & 1);
         const uint32_t q = q0 + 8 * i + cq + (e & 1);
         float p = exp2f(fmaf(sacc[4 * i + e], sl2, nl[c]));
-        if (diag && q < ((e & 2) ? kb : ka)) p = 0.f;     // causal: a query sees keys <= itself
+        if constexpr (KV) {
+          if (diag && (int)q < ((e & 2) ? eb : ea)) p = 0.f;      // query q sees keys <= cdk + q
+        } else {
+          if (diag && q < ((e & 2) ? kb : ka)) p = 0.f;     // causal: a query sees keys <= itself
+        }
         sacc[4 * i + e] = p;
         dpacc[4 * i + e] = p * fmaf(dpacc[4 * i + e], scale, nd[c]);   // dS^T = P^T o (dP^T - D) * scale
       }
@@ -393,17 +450,55 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
     if (threadIdx.x == 0)
       bwd_load_refill(smem, st_full, st_empty, &tmap_q, &tmap_do, head * 128, seq_start + first * 64, n, n_it);
   }
+  if constexpr (KV) {
+    // the thread's key rows ka (fragment elements 4i, 4i+1) and kb (4i+2, 4i+3), columns 8i + cq, +1
+#pragma unroll
+    for (uint32_t hf = 0; hf < 2; ++hf) {
+      const uint32_t j = own * 128 + ra + 8 * hf;
+      if (j >= klen) continue;
+      const int64_t off = ((int64_t)kv0 + j) * ldacc + head * 128 + cq;
+      float* pk = acc_k + off;
+      float* pv = acc_v + off;
+      const bool cached_row = j < cdk;
+#pragma unroll
+      for (uint32_t i = 0; i < 16; ++i) {
+        float2 a = *reinterpret_cast<const float2*>(pk + 8 * i);
+        float2 c = *reinterpret_cast<const float2*>(pv + 8 * i);
+        if (cached_row) {
+          a.x += dkacc[4 * i + 2 * hf]; a.y += dkacc[4 * i + 2 * hf + 1];
+          c.x += dvacc[4 * i + 2 * hf]; c.y += dvacc[4 * i + 2 * hf + 1];
+          *reinterpret_cast<float2*>(pk + 8 * i) = a;
+          *reinterpret_cast<float2*>(pv + 8 * i) = c;
+        } else {
+          dkacc[4 * i + 2 * hf] += a.x; dkacc[4 * i + 2 * hf + 1] += a.y;
+          dvacc[4 * i + 2 * hf] += c.x; dvacc[4 * i + 2 * hf + 1] += c.y;
+        }
+      }
+    }
+  }
   compute_warps_sync();                                     // every operand stage is free
   uint8_t* stage_v = smem + L::RES_OFF;                     // resident K/V and the Q/dO stages are free now
   uint8_t* stage_k = smem + L::ST_OFF;
   stage_acc_tile(dvacc, wg, stage_v);
   stage_acc_tile(dkacc, wg, stage_k);
   compute_warps_sync();
-  const uint32_t rows_valid = min(128u, (uint32_t)seq_len - own * 128);
-  const int64_t tok0 = (int64_t)seq_start + own * 128;
-  flush_acc_tile(stage_v, warp, lane, rows_valid, dv + tok0 * lddv + head * 128, lddv, nullptr, cos_t, sin_t);
-  flush_acc_tile(stage_k, warp, lane, rows_valid, dk + tok0 * lddk + head * 128, lddk,
-                 rope_pos != nullptr ? rope_pos + tok0 : nullptr, cos_t, sin_t);
+  if constexpr (KV) {
+    // block rows r_first .. rows_valid-1 are suffix rows: packed row seq_start + own*128 + r - cdk
+    const uint32_t rows_valid = min(128u, klen - own * 128);
+    const uint32_t r_first = cdk > own * 128 ? min(cdk - own * 128, 128u) : 0u;
+    if (r_first >= rows_valid) return;
+    const int64_t tok0 = (int64_t)seq_start + own * 128 + r_first - cdk;
+    flush_acc_tile(stage_v + r_first * AB_STAGE_LD, warp, lane, rows_valid - r_first, dv + tok0 * lddv + head * 128, lddv,
+                   nullptr, cos_t, sin_t);
+    flush_acc_tile(stage_k + r_first * AB_STAGE_LD, warp, lane, rows_valid - r_first, dk + tok0 * lddk + head * 128, lddk,
+                   rope_pos != nullptr ? rope_pos + tok0 : nullptr, cos_t, sin_t);
+  } else {
+    const uint32_t rows_valid = min(128u, (uint32_t)seq_len - own * 128);
+    const int64_t tok0 = (int64_t)seq_start + own * 128;
+    flush_acc_tile(stage_v, warp, lane, rows_valid, dv + tok0 * lddv + head * 128, lddv, nullptr, cos_t, sin_t);
+    flush_acc_tile(stage_k, warp, lane, rows_valid, dk + tok0 * lddk + head * 128, lddk,
+                   rope_pos != nullptr ? rope_pos + tok0 : nullptr, cos_t, sin_t);
+  }
 }
 
 }  // namespace nv
@@ -412,6 +507,18 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
 extern "C" int nv_debug_attn_trace(int kernel, unsigned long long* out, int max_words) {
   (void)kernel; (void)out; (void)max_words;
   return 0;
+}
+
+// D = rowsum(dO o O) unless o == nullptr: then dvec already holds D (written by the o_proj dgrad epilogue, nv_gemm_attnd_bf16)
+static int attn_bwd_prep(const void* o, int64_t ldo, const void* dout, int64_t lddo, float* dvec, int T, int H,
+                         cudaStream_t stream) {
+  using namespace nv;
+  if (o == nullptr) return NV_OK;
+  const int64_t threads = (int64_t)T * H * 32;
+  attn_bwd_prep_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, stream>>>(
+      reinterpret_cast<const __nv_bfloat16*>(o), ldo, reinterpret_cast<const __nv_bfloat16*>(dout), lddo, dvec, T, H);
+  NV_LAUNCH_CHECK();
+  return NV_OK;
 }
 
 // Inputs: q,k,v (post-RoPE) and o, do as bf16 [T, H*128]-column views; lse [H,T] from the forward.
@@ -438,25 +545,70 @@ extern "C" int nv_attn_bwd(const void* q, int64_t ldq, const void* k, int64_t ld
   if ((rc = make_tmap_2d(&tdo, dout, 2, (uint64_t)H * 128, (uint64_t)T, (uint64_t)lddo * 2, 64, 64))) return rc;
   static bool attr_set = false;
   if (!attr_set) {
-    NV_CUDA(cudaFuncSetAttribute(attn_bwd_dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BwdSmem::DYN_BYTES));
-    NV_CUDA(cudaFuncSetAttribute(attn_bwd_dkv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BwdSmem::DYN_BYTES));
+    NV_CUDA(cudaFuncSetAttribute(attn_bwd_dq_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, BwdSmem::DYN_BYTES));
+    NV_CUDA(cudaFuncSetAttribute(attn_bwd_dkv_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, BwdSmem::DYN_BYTES));
     attr_set = true;
   }
-  if (o != nullptr) {     // o == nullptr: dvec already holds D (written by the o_proj dgrad epilogue, nv_gemm_attnd_bf16)
-    const int64_t threads = (int64_t)T * H * 32;
-    attn_bwd_prep_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, stream>>>(
-        reinterpret_cast<const __nv_bfloat16*>(o), ldo, reinterpret_cast<const __nv_bfloat16*>(dout), lddo, dvec, T, H);
-    NV_LAUNCH_CHECK();
-  }
+  if ((rc = attn_bwd_prep(o, ldo, dout, lddo, dvec, T, H, stream))) return rc;
   const __nv_bfloat16* c = reinterpret_cast<const __nv_bfloat16*>(cos_t);
   const __nv_bfloat16* s = reinterpret_cast<const __nv_bfloat16*>(sin_t);
   dim3 grid(total_blocks, H);
-  attn_bwd_dkv_kernel<<<grid, AB_THREADS, BwdSmem::DYN_BYTES, stream>>>(
+  attn_bwd_dkv_kernel<false><<<grid, AB_THREADS, BwdSmem::DYN_BYTES, stream>>>(
       tq, tk, tv, tdo, lse, dvec, reinterpret_cast<__nv_bfloat16*>(dk), lddk, reinterpret_cast<__nv_bfloat16*>(dv), lddv,
-      cu_seqlens, B, T, scale, rope_pos, c, s);
+      cu_seqlens, B, T, scale, rope_pos, c, s, nullptr, nullptr, nullptr, nullptr, 0);
   NV_LAUNCH_CHECK();
-  attn_bwd_dq_kernel<<<grid, AB_THREADS, BwdSmem::DYN_BYTES, stream>>>(
-      tq, tdo, tk, tv, lse, dvec, reinterpret_cast<__nv_bfloat16*>(dq), lddq, cu_seqlens, B, T, scale, rope_pos, c, s);
+  attn_bwd_dq_kernel<false><<<grid, AB_THREADS, BwdSmem::DYN_BYTES, stream>>>(
+      tq, tdo, tk, tv, lse, dvec, reinterpret_cast<__nv_bfloat16*>(dq), lddq, cu_seqlens, B, T, scale, rope_pos, c, s,
+      nullptr, nullptr);
+  NV_LAUNCH_CHECK();
+  return NV_OK;
+}
+
+// Backward of nv_attn_fwd_kv.  q, o, dout, lse, dvec, dq, dk, dv: the Tq packed suffix rows (cu_seqlens), as in nv_attn_bwd;
+// kcache / vcache: bf16 [Tkv, H*128] (leading dimension ldkv) holding K/V of sequence b at rows kv_start[b] .. +kv_len[b];
+// acc_k / acc_v: fp32 [Tkv, >= H*128] (ldacc) gradient accumulators over the cache rows.  Key row j of sequence b:
+//   j <  kv_len[b] - q_len[b] (cached):  acc_{k,v}[kv_start[b] + j] += dK_j, dV_j
+//   j >= kv_len[b] - q_len[b] (suffix):  dk / dv[packed row of j] = bf16(dK_j + acc_k[...]) (then the inverse RoPE at
+//                                        rope_pos when given), bf16(dV_j + acc_v[...]); the accumulator is only read.
+// With kv_len == q_len (nothing cached) every row is a suffix row: the accumulated gradient of the cache rows is added to
+// the recomputed prefix's own.  Deterministic: each accumulator (row, head) slice has one owning CTA.
+// total_qblocks = sum_b ceil(q_len[b]/128), total_kblocks = sum_b ceil(kv_len[b]/128).
+extern "C" int nv_attn_bwd_kv(const void* q, int64_t ldq, const void* kcache, const void* vcache, int64_t ldkv, const void* o,
+                              int64_t ldo, const void* dout, int64_t lddo, const float* lse, float* dvec, void* dq, int64_t lddq,
+                              void* dk, int64_t lddk, void* dv, int64_t lddv, float* acc_k, float* acc_v, int64_t ldacc,
+                              const int* cu_seqlens, const int* kv_start, const int* kv_len, int B, int Tq, int Tkv, int H,
+                              int head_dim, int total_qblocks, int total_kblocks, float scale, const int* rope_pos,
+                              const void* cos_t, const void* sin_t, void* stream_) {
+  using namespace nv;
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  NV_REQUIRE(head_dim == 128, "nv_attn_bwd_kv: head_dim must be 128 (got %d)", head_dim);
+  NV_REQUIRE(B > 0 && Tq > 0 && Tkv > 0 && H > 0 && total_qblocks > 0 && total_kblocks > 0, "nv_attn_bwd_kv: empty problem");
+  NV_REQUIRE(q && kcache && vcache && dout && lse && dvec && dq && dk && dv && acc_k && acc_v && cu_seqlens && kv_start && kv_len,
+             "nv_attn_bwd_kv: null argument");
+  NV_REQUIRE((lddq & 7) == 0 && (lddk & 7) == 0 && (lddv & 7) == 0 && (ldo & 3) == 0 && (lddo & 3) == 0 && (ldacc & 1) == 0 &&
+             ldacc >= (int64_t)H * 128, "nv_attn_bwd_kv: leading-dimension alignment");
+  CUtensorMap tq, tk, tv, tdo;
+  int rc;
+  if ((rc = make_tmap_2d(&tq, q, 2, (uint64_t)H * 128, (uint64_t)Tq, (uint64_t)ldq * 2, 64, 64))) return rc;
+  if ((rc = make_tmap_2d(&tk, kcache, 2, (uint64_t)H * 128, (uint64_t)Tkv, (uint64_t)ldkv * 2, 64, 64))) return rc;
+  if ((rc = make_tmap_2d(&tv, vcache, 2, (uint64_t)H * 128, (uint64_t)Tkv, (uint64_t)ldkv * 2, 64, 64))) return rc;
+  if ((rc = make_tmap_2d(&tdo, dout, 2, (uint64_t)H * 128, (uint64_t)Tq, (uint64_t)lddo * 2, 64, 64))) return rc;
+  static bool attr_set = false;
+  if (!attr_set) {
+    NV_CUDA(cudaFuncSetAttribute(attn_bwd_dq_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BwdSmem::DYN_BYTES));
+    NV_CUDA(cudaFuncSetAttribute(attn_bwd_dkv_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BwdSmem::DYN_BYTES));
+    attr_set = true;
+  }
+  if ((rc = attn_bwd_prep(o, ldo, dout, lddo, dvec, Tq, H, stream))) return rc;
+  const __nv_bfloat16* c = reinterpret_cast<const __nv_bfloat16*>(cos_t);
+  const __nv_bfloat16* s = reinterpret_cast<const __nv_bfloat16*>(sin_t);
+  attn_bwd_dkv_kernel<true><<<dim3(total_kblocks, H), AB_THREADS, BwdSmem::DYN_BYTES, stream>>>(
+      tq, tk, tv, tdo, lse, dvec, reinterpret_cast<__nv_bfloat16*>(dk), lddk, reinterpret_cast<__nv_bfloat16*>(dv), lddv,
+      cu_seqlens, B, Tq, scale, rope_pos, c, s, kv_start, kv_len, acc_k, acc_v, ldacc);
+  NV_LAUNCH_CHECK();
+  attn_bwd_dq_kernel<true><<<dim3(total_qblocks, H), AB_THREADS, BwdSmem::DYN_BYTES, stream>>>(
+      tq, tdo, tk, tv, lse, dvec, reinterpret_cast<__nv_bfloat16*>(dq), lddq, cu_seqlens, B, Tq, scale, rope_pos, c, s,
+      kv_start, kv_len);
   NV_LAUNCH_CHECK();
   return NV_OK;
 }

@@ -489,8 +489,9 @@ class LlamaCore:
     # -------------------------------------------------------------------------------------------------
     def forward_suffix(self, x: torch.Tensor, pos: torch.Tensor, cu: torch.Tensor, q_lens, kc: List[torch.Tensor],
                        vc: List[torch.Tensor], cached: torch.Tensor, kv_start: torch.Tensor, kv_len: torch.Tensor,
-                       out_rows: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """Inference-only forward of NEW rows on top of a per-layer KV cache that already holds an encoded prefix of
+                       out_rows: Optional[torch.Tensor] = None, save: bool = False, acc: Optional[List[torch.Tensor]] = None,
+                       kv_lens=None, store: bool = True):
+        """Forward of NEW rows on top of a per-layer KV cache that already holds an encoded prefix of
         every sequence (cross-step prefix reuse, SURVEY.md §8f n1).  x: [Tn, D] packed embeddings of the new tokens,
         pos: their rotary positions, cu / q_lens: packing of the new rows, caches [B, Smax, D] (zero-initialised),
         cached / kv_start / kv_len: int32 [B] on the device (rows already cached, first cache row of the sequence,
@@ -498,16 +499,26 @@ class LlamaCore:
         [R, D] with ``out_rows``) before the final RMSNorm.
 
         The caches may also be fp8 ``(e4m3 [B, Smax, D], int8 exponents [B, Smax, H])`` pairs per layer (``is_fp8_kv``): the
-        new rows are rounded as they are stored and the attention reads the rounded rows, theirs included."""
+        new rows are rounded as they are stored and the attention reads the rounded rows, theirs included.
+
+        ``save=True`` (training; bf16 caches only): returns ``(residual, tape)``; the tape makes ``backward`` run the cache
+        form of the attention backward (``ops.attn_bwd_kv``), which adds the cached rows' dK / dV into ``acc`` (per layer,
+        fp32 [B, Smax, 2 D]) and hands the suffix rows theirs.  ``kv_lens``: host copy of ``kv_len``.  Runs the per-kernel
+        path on the bf16 weights (never the fp8 copy); the caches must still hold these K/V when ``backward`` runs.
+        ``store=False`` (the prefix flush of ``PrefixKVCache``, which recomputes rows the cache already holds): the rows' own K/V
+        are not written; the attention reads the cached ones.  The store writes packed sequence i to cache slot i, so only a
+        batch covering the slots 0..B-1 in order may store."""
         d = self.d
         H, D = d.n_heads, d.hidden
         B, T = len(q_lens), x.shape[0]
         last = d.n_layers - 1
         fused = self.fused_epilogues and T >= 1024 and d.inter % 128 == 0 and d.hidden % 256 == 0
-        f8 = self.fp8_for_inference()
+        f8 = None if save else self.fp8_for_inference()     # training forwards never read the fp8 copy
         fp8_kv = is_fp8_kv(kc)
+        if save and (fp8_kv or acc is None or kv_lens is None):
+            raise ValueError("forward_suffix(save=True) needs bf16 caches, the gradient accumulators and the host kv_lens")
         Bc, Smax = (kc[0][0] if fp8_kv else kc[0]).shape[:2]
-        if self.LAYER_CALL and not fused and d.head_dim == 128:
+        if self.LAYER_CALL and not fused and d.head_dim == 128 and not save:
             R = 0 if out_rows is None else out_rows.numel()
             run = ops.LayerRunner(T, D, d.inter, H, d.rms_eps, pos, self.cos, self.sin, cu, B, ops._qblocks(q_lens), R=R, device=x.device)
             run.set_cache_mode(4 if fp8_kv else 2, Smax, Bc * Smax, cached, kv_start, kv_len)
@@ -521,33 +532,46 @@ class LlamaCore:
                         fp8=self._fp8_layer(f8, l), fp8_max_rows=FP8_MAX_ROWS)
                 x = y
             return x
+        saved: List[_Saved] = []
         for l, lyr in enumerate(self.model.layers):
             w8 = self._fp8_layer(f8, l) or ((None, None),) * 4
-            xn, _ = ops.rmsnorm_fwd(x, lyr.input_layernorm.weight.data, d.rms_eps)
+            s = _Saved()
+            s.x = x
+            xn, s.rstd1 = ops.rmsnorm_fwd(x, lyr.input_layernorm.weight.data, d.rms_eps)
             if fused:
                 qkv = ops.gemm_rope(xn, self.wqkv[l], pos, self.cos, self.sin, 2 * D)
             else:
                 qkv = self._linear(xn, self.wqkv[l], w8[0])
                 ops.rope_(qkv, pos, self.cos, self.sin, 2 * H, d.head_dim)
+            s.lse = torch.empty((H, T), dtype=torch.float32, device=x.device) if save else None
             if fp8_kv:
                 (kq, ke), (vq, ve) = kc[l], vc[l]
                 ops.kv_store_suffix_fp8(qkv, cu, cached, kq, vq, ke, ve, B, T)
                 ao = ops.attn_fwd_kv_fp8(qkv[:, :D], kq, vq, ke, ve, cu, q_lens, kv_start, kv_len, H)
             else:
-                ops.kv_store_suffix(qkv, cu, cached, kc[l], vc[l], B, T)
-                ao = ops.attn_fwd_kv(qkv[:, :D], kc[l], vc[l], cu, q_lens, kv_start, kv_len, H)
+                if store:
+                    ops.kv_store_suffix(qkv, cu, cached, kc[l], vc[l], B, T)
+                ao = ops.attn_fwd_kv(qkv[:, :D], kc[l], vc[l], cu, q_lens, kv_start, kv_len, H, lse=s.lse)
+            s.xn, s.qkv, s.ao, s.rows = xn, qkv, ao, None
             xin = x
             if out_rows is not None and l == last:
-                ao = ops.gather_rows(ao, out_rows)
+                s.rows = out_rows
+                ao = s.ao_r = ops.gather_rows(ao, out_rows)
                 xin = ops.gather_rows(x, out_rows)
-            xm = self._linear(ao, self.wo[l], w8[1], addend=xin)
-            xn2, _ = ops.rmsnorm_fwd(xm, lyr.post_attention_layernorm.weight.data, d.rms_eps)
+            s.xm = xm = self._linear(ao, self.wo[l], w8[1], addend=xin)
+            s.xn2, s.rstd2 = xn2, _ = ops.rmsnorm_fwd(xm, lyr.post_attention_layernorm.weight.data, d.rms_eps)
             if fused and xm.shape[0] >= 1024:
-                _, h = ops.gemm_swiglu(xn2, self.wgu[l], keep_gu=False)
+                s.gu, s.h = ops.gemm_swiglu(xn2, self.wgu[l], keep_gu=save)
             else:
-                h = ops.swiglu_fwd(self._linear(xn2, self.wgu[l], w8[2]))
-            x = self._linear(h, self.wd[l], w8[3], addend=xm)
-        return x
+                s.gu = self._linear(xn2, self.wgu[l], w8[2])
+                s.h = ops.swiglu_fwd(s.gu)
+            x = self._linear(s.h, self.wd[l], w8[3], addend=xm)
+            if save:
+                saved.append(s)
+        if not save:
+            return x
+        kv = SimpleNamespace(kc=kc, vc=vc, acc=acc, kv_start=kv_start, kv_len=kv_len, kv_lens=list(kv_lens))
+        return x, (saved, (pos, cu, list(q_lens)), kv)
 
     # -------------------------------------------------------------------------------------------------
     def backward(self, dx: torch.Tensor, tape, layer_done=None) -> torch.Tensor:
@@ -558,7 +582,8 @@ class LlamaCore:
         overlap the data-parallel all-reduce with the rest of the backward)."""
         if tape is None:
             raise RuntimeError("LlamaCore.backward: the forward ran without saving activations (no_grad / eval-only)")
-        saved, (pos, cu, seqlens) = tape
+        saved, (pos, cu, seqlens) = tape[:2]
+        kv = tape[2] if len(tape) > 2 else None          # forward_suffix tape: attention over a KV cache
         d = self.d
         H = d.n_heads
         acc = not getattr(self.flat, "overwrite_layer_grads", False)
@@ -619,7 +644,11 @@ class LlamaCore:
                 ops.scatter_rows_(dxm, s.rows, full)
                 dxm = full
             # attention backward with the inverse rotary embedding of dq/dk fused into its epilogue
-            dqkv = ops.attn_bwd(s.qkv, s.ao, dao, s.lse, cu, seqlens, H, rope=(pos, self.cos, self.sin), dvec=dvec)
+            if kv is None:
+                dqkv = ops.attn_bwd(s.qkv, s.ao, dao, s.lse, cu, seqlens, H, rope=(pos, self.cos, self.sin), dvec=dvec)
+            else:
+                dqkv = ops.attn_bwd_kv(s.qkv, s.ao, dao, s.lse, kv.kc[l], kv.vc[l], kv.acc[l], cu, seqlens, kv.kv_start,
+                                       kv.kv_len, kv.kv_lens, H, rope=(pos, self.cos, self.sin), dvec=dvec)
             del dao
             dxn = ops.gemm(dqkv, self.wqkv[l], b_mn=True)
             wgrad(dqkv, s.xn, self.gqkv[l])

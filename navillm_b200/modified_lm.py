@@ -17,6 +17,7 @@ from __future__ import annotations
 import collections
 import os
 import time
+import weakref
 from types import SimpleNamespace
 from typing import List, Optional
 
@@ -128,11 +129,30 @@ class PrefixKVCache:
     head), half the memory of the bf16 cache plus 1/256 (``nbytes``), which lets a rollout run a larger batch at the same
     ``max_len``.  Every suffix step attends over the cache, so the step's new rows read their own K / V rounded to e4m3 as
     well (K' / V'); generate()'s prefill, by contrast, attends over the unrounded K / V of the prompt.  The format is the
-    caller's choice: it does not follow the model's ``kv_cache_dtype``.  Works with and without ``quantize_weights_fp8()``."""
+    caller's choice: it does not follow the model's ``kv_cache_dtype``.  Works with and without ``quantize_weights_fp8()``.
 
-    def __init__(self, lm: "ModifiedLlamaForCausalLM", batch_size: int, max_len: int = 2048, kv_dtype: str = "bf16"):
+    ``train=True`` (opt-in, bf16 only) lets the cache serve a training rollout: ``model('navigation', batch, prefix_cache=...)``
+    under grad mode, one ``backward()`` per step, weights fixed until the rollout's gradients are complete.  The gradient of
+    a step's loss then has two parts.  (a) Through the step's own suffix rows: its ``backward()`` runs the stack over the
+    suffix with the cache form of the attention backward, which also produces dK / dV of the cached rows the step attended
+    to; those are ADDED to a per-layer fp32 accumulator over the cache rows (``acc``, [B, max_len, 2 D]: dK | dV), not
+    propagated.  (b) Through the cached rows: linear in the accumulated dK / dV, so ONE backward per rollout covers every
+    step -- ``flush_grads()`` re-runs the forward of each row's reused prefix (its token ids, the ``<hist>`` vectors it was
+    given, rotary positions ``off + j``) with a tape and back-propagates the accumulator through it, the accumulated dK / dV
+    entering each layer as the gradient of that layer's K / V.  Memory: the accumulator, no activations across steps; cost:
+    one extra forward of the prefix per rollout.  A row whose reusable prefix shrinks (left truncation of a long prompt)
+    runs its part (b) first, before its cache rows are overwritten.  Part (b) attends over the cached K/V (the rows the steps' dK / dV
+    refer to; the flush writes no cache row) with the other prefix activations recomputed, which equal the steps' up to
+    bf16 rounding (different GEMM shapes).  ``flush_grads()`` must run before the optimizer step:
+    the data-parallel exchange of an armed pass does it itself; ``reset()`` of a row with pending gradient, ``zero_grad()``
+    of the model, and any step or flush after the weights changed raise."""
+
+    def __init__(self, lm: "ModifiedLlamaForCausalLM", batch_size: int, max_len: int = 2048, kv_dtype: str = "bf16",
+                 train: bool = False):
         if kv_dtype not in ("bf16", "fp8"):
             raise ValueError(f"PrefixKVCache: kv_dtype must be 'bf16' or 'fp8' (got {kv_dtype!r})")
+        if train and kv_dtype != "bf16":
+            raise ValueError("PrefixKVCache: train=True needs the bf16 cache (the fp8 store is inference-only)")
         lm._ensure()
         dev, d = lm._device(), lm.dims
         self.B, self.max_len, self.kv_dtype = batch_size, max_len, kv_dtype
@@ -152,16 +172,145 @@ class PrefixKVCache:
         self.ids: List[np.ndarray] = [np.zeros(0, dtype=np.int64) for _ in range(batch_size)]
         self.off: List[Optional[int]] = [None] * batch_size
         self.stats = {"steps": 0, "tokens": 0, "tokens_encoded": 0}
+        self.train = train
+        self.acc = [torch.zeros((batch_size, max_len, 2 * d.hidden), dtype=torch.float32, device=dev)
+                    for _ in range(d.n_layers)] if train else None
+        self.hist: List[Optional[torch.Tensor]] = [None] * batch_size   # <hist> rows each row was last given (references)
+        self.reused = [0] * batch_size        # R[b]: cached rows [0, R) whose part (b) has not run yet
+        self._pending_rows = set()            # rows whose accumulator a step's backward has written since their last flush
+        self.writes = 0                       # steps that wrote the cache: a step's tape is valid only until the next one
+        self._lm = weakref.ref(lm)
+        if train:
+            self._weights = self._weight_state()
+            lm._prefix_caches.add(self)
 
     @property
     def nbytes(self) -> int:
-        """Device bytes of the K and V caches of all layers (exponents included)."""
-        return sum(t.nbytes for c in self.kc + self.vc for t in (c if isinstance(c, tuple) else (c,)))
+        """Device bytes of the K and V caches of all layers (exponents included) and, with ``train=True``, the gradient
+        accumulator."""
+        return sum(t.nbytes for c in self.kc + self.vc for t in (c if isinstance(c, tuple) else (c,))) + \
+            sum(a.nbytes for a in (self.acc or []))
+
+    @property
+    def pending(self) -> bool:
+        """True while part (b) of some row's gradient is outstanding (``flush_grads()`` has work to do)."""
+        return bool(self._pending_rows)
 
     def reset(self, rows=None) -> None:
-        for b in (range(self.B) if rows is None else rows):
+        rows = list(range(self.B) if rows is None else rows)
+        lost = sorted(b for b in rows if b in self._pending_rows)
+        if lost:
+            raise RuntimeError(f"PrefixKVCache.reset: rows {lost} have pending gradient through their cached prefix; call "
+                               f"flush_grads() first")
+        for b in rows:
             self.ids[b] = np.zeros(0, dtype=np.int64)
             self.off[b] = None
+            self.hist[b] = None
+            self.reused[b] = 0
+        if self.train and all(i.size == 0 for i in self.ids):
+            self._weights = self._weight_state()         # nothing cached: the cache may be refilled under new weights
+
+    # ---- training ----------------------------------------------------------------------------------------------
+    def _weight_state(self):
+        flat = self._lm().flat
+        return flat.flat.data_ptr(), flat.flat._version, flat.generation, sum(p._version for p in flat.params)
+
+    def check_weights(self) -> None:
+        if self._weight_state() != self._weights:
+            raise RuntimeError("PrefixKVCache: the weights changed since the cache was filled (optimizer step, load or "
+                               "another write); its K/V and pending gradient belong to the old weights -- run flush_grads() "
+                               "before the optimizer step, and reset() the cache (or build a new one) for the next rollout")
+
+    def flush_grads(self) -> None:
+        """Part (b) of the gradient for every row with pending gradient: one forward of the rows' reused prefixes with a tape
+        and one backward that injects the accumulated dK / dV, accumulated into the model's gradients; then the accumulator
+        of those rows is zero.  A no-op when nothing is pending."""
+        self._flush_rows(sorted(self._pending_rows))
+
+    def _flush_shrinking(self, ids: np.ndarray, msk: np.ndarray, cand_id: int) -> None:
+        """Before a step overwrites the cache: flush the rows whose reusable prefix is shorter than what they reused so far."""
+        rows = [b for b in range(self.B) if self.reused[b] > 0 and _reusable_prefix(self.ids[b], ids[b][msk[b]], cand_id) < self.reused[b]]
+        self._flush_rows(rows)
+        for b in rows:
+            self.reused[b] = 0
+
+    def _flush_rows(self, rows) -> None:
+        rows = [b for b in rows if b in self._pending_rows]
+        if not rows:
+            return
+        self.check_weights()
+        lm = self._lm()
+        lm._ensure()
+        core, d, dev = lm.core, lm.dims, lm._device()
+        hist_id = lm.hist_token_id[0]
+        toks, pos, vsrc, hist, lens = [], [], [], [], []
+        nh = 0
+        for b in rows:
+            R = self.reused[b]
+            t = self.ids[b][:R]
+            is_h = t == hist_id
+            h = int(is_h.sum())
+            vs = np.full(R, -1, dtype=np.int64)
+            vs[is_h] = nh + np.arange(h)
+            nh += h
+            if h:
+                hist.append(self.hist[b][:h])
+            toks.append(t); pos.append(self.off[b] + np.arange(R)); vsrc.append(vs); lens.append(R)
+        tok = np.concatenate(toks)
+        order = np.argsort(tok, kind="stable")
+        cu = np.concatenate([[0], np.cumsum(lens)])
+        parts = [tok, np.concatenate(pos), cu, np.concatenate(vsrc), np.zeros(len(rows)), np.asarray(rows) * self.max_len,
+                 np.asarray(lens), order, tok[order]]
+        views = _to_device(parts, dev)
+        tok_d, pos_d, cu_d, vs_d, zero_d, kvs_d, kvl_d, ord_d, srt_d = views
+        vis = torch.cat(hist, 0).to(torch.float32).contiguous() if hist else None
+        E = lm.model.embed_tokens.weight
+        with torch.no_grad():
+            x = ops.embed_fwd(tok_d, E.data, vs_d if vis is not None else None, vis)
+            # the cache rows [0, R) of each flushed row already hold the K/V its steps attended over (and that the accumulated
+            # dK / dV refer to): attend over them, and leave every slot of the cache as it is
+            g, tape = core.forward_suffix(x, pos_d, cu_d, lens, self.kc, self.vc, zero_d, kvs_d, kvl_d, save=True, acc=self.acc,
+                                          kv_lens=lens, store=False)
+            lm._settle_lazy_zero()                     # part (b) adds to the gradients the steps' backwards left
+            dx = core.backward(torch.zeros_like(g), tape)
+            ops.embed_bwd_weight_(dx, tok_d, E.grad, order=ord_d, sorted_ids=srt_d)
+            idx = torch.tensor(rows, dtype=torch.int64, device=dev)
+            for a in self.acc:
+                a[:, :max(lens)].index_fill_(0, idx, 0.0)
+        self.writes += 1
+        for b in rows:
+            self.reused[b] = 0
+            self._pending_rows.discard(b)
+
+
+    def _mark_pending(self, cached) -> None:
+        """A step's backward added the dK / dV of rows [0, cached[b]) to the accumulator."""
+        for b, c in enumerate(cached):
+            if c > 0:
+                self._pending_rows.add(b)
+
+
+def _to_device(parts, dev):
+    """int32 device views of host integer arrays, shipped in ONE pinned copy."""
+    host = np.concatenate([np.asarray(p).astype(np.int32).reshape(-1) for p in parts])
+    buf = torch.from_numpy(host).pin_memory().to(dev, non_blocking=True)
+    views, o = [], 0
+    for p in parts:
+        n = np.asarray(p).size
+        views.append(buf[o:o + n]); o += n
+    return views
+
+
+def _reusable_prefix(old: np.ndarray, toks: np.ndarray, cand_id: int) -> int:
+    """Rows of a row's new prompt ``toks`` whose K/V the cache holds: the longest common token prefix with ``old``, cut
+    before the first <cand> token (candidates change every step) and at most L - 1 (the last token is always encoded)."""
+    m = min(old.size, int(toks.size) - 1)
+    neq = np.flatnonzero(old[:m] != toks[:m])
+    n = int(neq[0]) if neq.size else m
+    cpos = np.flatnonzero(toks == cand_id)
+    if cpos.size:
+        n = min(n, int(cpos[0]))
+    return n
 
 
 def plan_prefix_reuse(ids: np.ndarray, msk: np.ndarray, cache: "PrefixKVCache", hist_counts, n_cand_total: int, cand_id: int,
@@ -187,13 +336,7 @@ def plan_prefix_reuse(ids: np.ndarray, msk: np.ndarray, cache: "PrefixKVCache", 
             raise ValueError(f"prompt of {L} tokens exceeds the prefix cache length {cache.max_len}")
         if cache.off[b] is None:
             cache.off[b] = S - L                               # the row keeps this rotary offset for the rollout
-        old = cache.ids[b]
-        m = min(old.size, L - 1)                               # at least the last token is encoded
-        neq = np.flatnonzero(old[:m] != toks[:m])
-        n = int(neq[0]) if neq.size else m
-        cpos = np.flatnonzero(toks == cand_id)                 # candidates change every step: never reused
-        if cpos.size:
-            n = min(n, int(cpos[0]))
+        n = _reusable_prefix(cache.ids[b], toks, cand_id)
         new = toks[n:]
         is_h, is_c = new == hist_id, new == cand_id
         h_before = int((toks[:n] == hist_id).sum())
@@ -236,7 +379,13 @@ class _LMFn(torch.autograd.Function):
         if mode == "loss":
             rows = pp.loss_rows
         # the stack returns only the requested rows (last layer pruned to them)
-        g, ctx.tape = core.forward(x, pp.pos, pp.cu, pp.seqlens, save=train, out_rows=rows)
+        kv = getattr(pp, "kv", None)
+        if kv is not None:             # training step over a PrefixKVCache: the suffix rows only (hidden_rows_cached)
+            c = kv.cache
+            g, ctx.tape = core.forward_suffix(x, pp.pos, pp.cu, pp.seqlens, c.kc, c.vc, kv.cached, kv.kv_start, kv.kv_len,
+                                              out_rows=rows, save=True, acc=c.acc, kv_lens=kv.kv_lens)
+        else:
+            g, ctx.tape = core.forward(x, pp.pos, pp.cu, pp.seqlens, save=train, out_rows=rows)
         ctx.lm, ctx.pp, ctx.mode, ctx.has_vis = lm, pp, mode, vis is not None
         ctx.n_vis = 0 if vis is None else vis.shape[0]
         hn, rstd = ops.rmsnorm_fwd(g, lm.model.norm.weight.data, d.rms_eps)
@@ -269,9 +418,18 @@ class _LMFn(torch.autograd.Function):
             ops.scale_(dlogits, dout.detach().to(torch.float32).reshape(1))   # in place: keeps the 16-byte-aligned row stride
             dy = ops.gemm(dlogits, lm.lm_head.weight.data, b_mn=True)                    # [Nl, D]
             ops.gemm(dlogits, hn, a_mn=True, b_mn=True, out=lm.lm_head.weight.grad, addend=lm.lm_head.weight.grad)
+        kv = getattr(pp, "kv", None)
+        if kv is not None and kv.cache.writes != kv.write_id:
+            raise RuntimeError("PrefixKVCache: a later step or flush rewrote the cache before this step's backward ran "
+                               "(call backward() after every step, as the rollout does)")
         dg = ops.rmsnorm_bwd(g, normw.data, rstd, dy, dw=normw.grad)                     # [R, D]: gradient at the requested rows
         lm.grad_sync.short_backward = pp.T < lm.SHORT_BACKWARD_TOKENS
-        dx = core.backward(dg, ctx.tape, layer_done=lm._grad_sync_hook())
+        # a pass that leaves prefix-cache gradient pending is not final per layer until the flush (before the exchange):
+        # no overlapped per-layer reductions
+        overlap = kv is None and not lm.prefix_grads_pending()
+        dx = core.backward(dg, ctx.tape, layer_done=lm._grad_sync_hook() if overlap else None)
+        if kv is not None:
+            kv.cache._mark_pending(kv.cached_host)
         ops.embed_bwd_weight_(dx, pp.ids, lm.model.embed_tokens.weight.grad,
                               order=pp.tok_order if pp.tok_order.numel() == pp.T else None, sorted_ids=pp.tok_sorted)
         dvis = ops.embed_bwd_vis(dx, pp.vis_src, ctx.n_vis) if ctx.has_vis else None
@@ -302,6 +460,8 @@ class ModifiedLlamaForCausalLM(nn.Module):
         self.register_buffer("_anchor", torch.zeros((), dtype=torch.float32), persistent=False)
         self.grad_sync = GradSync()                  # replaced by NavModel's shared state when owned by a NavModel
         self.grad_sync.flats = self._own_flats
+        self.grad_sync.before_exchange = self.flush_prefix_caches
+        self._prefix_caches = weakref.WeakSet()      # PrefixKVCache(train=True) instances built on this model
         if tokenizer is not None:
             self._set_tokenizer(tokenizer)
 
@@ -403,6 +563,22 @@ class ModifiedLlamaForCausalLM(nn.Module):
     def mark_grads_zeroed(self) -> None:
         self._lm_head_grad_clean = True
 
+    def _settle_lazy_zero(self) -> None:
+        """``zero_grad(lazy=True)`` promised that the next LM backward overwrites the per-layer gradients; a backward that
+        must ADD to them (or an exchange / optimizer step with no backward in between) first makes the promise true."""
+        if self.core is not None and getattr(self.flat, "overwrite_layer_grads", False):
+            self.flat.flat_grad[:self.flat.offset_of(self.model.embed_tokens.weight)].zero_()
+            self.flat.overwrite_layer_grads = False
+
+    # ---- training prefix caches (PrefixKVCache(train=True)) ----
+    def prefix_grads_pending(self) -> bool:
+        return any(c.pending for c in list(self._prefix_caches))
+
+    def flush_prefix_caches(self) -> None:
+        """``flush_grads()`` of every training prefix cache of this model (the armed pass runs it before the exchange)."""
+        for c in list(self._prefix_caches):
+            c.flush_grads()
+
     def _own_flats(self):
         return [(self.flat, self.flat.offset_of(self.model.embed_tokens.weight))] if self.core is not None else []
 
@@ -427,40 +603,66 @@ class ModifiedLlamaForCausalLM(nn.Module):
         anchor = self._anchor.detach().requires_grad_(train)
         return _LMFn.apply(self, pp, vis, "rows", rows, train, anchor)
 
-    @torch.no_grad()
     def hidden_rows_cached(self, input_ids: torch.Tensor, attention_mask: torch.Tensor, cand_vis: Optional[torch.Tensor],
                            hist_vis: Optional[torch.Tensor], hist_counts, cache: PrefixKVCache) -> torch.Tensor:
-        """Inference twin of ``hidden_rows(pp, vis, pp.cls_rows)`` that encodes only the tokens after each row's
+        """Twin of ``hidden_rows(pp, vis, pp.cls_rows)`` that encodes only the tokens after each row's
         longest common prefix with ``cache`` (see PrefixKVCache).  cand_vis: [sum cand, D] in row-major token order;
         hist_vis: [sum_b hist_counts[b], D] flattened sample-major (NavModel._flatten_hist).  Returns the final-
-        RMSNorm'ed hidden states at the <cls_1> tokens, [B, D] bf16."""
+        RMSNorm'ed hidden states at the <cls_1> tokens, [B, D] bf16.  Inference (no grad) with any cache; under grad mode
+        with a ``train=True`` cache, differentiable w.r.t. cand_vis and the weights (see PrefixKVCache for the gradient)."""
         self._ensure()
+        train = torch.is_grad_enabled() and self.training_enabled
+        if train and not cache.train:
+            raise RuntimeError("prefix_cache: this cache is inference-only: call under torch.no_grad(), or build it with "
+                               "PrefixKVCache(..., train=True) for a training rollout")
+        if cache.train:
+            cache.check_weights()
+            if hist_vis is not None and hist_vis.requires_grad:
+                raise RuntimeError("prefix_cache(train=True): hist_vis must be detached (the rollout's <hist> vectors are "
+                                   "fuse_embeds.detach()); the cache keeps them for the prefix backward")
         dev, d = self._device(), self.dims
         ids = input_ids.detach().cpu().numpy().astype(np.int64)
         msk = attention_mask.detach().cpu().numpy().astype(bool)
         B = ids.shape[0]
         n_cand_total = 0 if cand_vis is None else cand_vis.shape[0]
+        if cache.train:
+            cache._flush_shrinking(ids, msk, self.cand_token_id[0])
         plan = plan_prefix_reuse(ids, msk, cache, hist_counts, n_cand_total, self.cand_token_id[0], self.hist_token_id[0],
                                  self.cls_token_id[0])
         tok_new, pos_new, vis_new, q_lens, cached, kv_len, cls_rows = plan
         cu = np.concatenate([[0], np.cumsum(q_lens)])
         kv_start = np.arange(B, dtype=np.int64) * cache.max_len
-        parts = [np.concatenate(tok_new), np.concatenate(pos_new), cu, np.concatenate(vis_new), np.asarray(cls_rows),
+        tok = np.concatenate(tok_new)
+        parts = [tok, np.concatenate(pos_new), cu, np.concatenate(vis_new), np.asarray(cls_rows),
                  np.asarray(cached), kv_start, np.asarray(kv_len)]
-        host = np.concatenate([p.astype(np.int32) for p in parts])
-        dev_buf = torch.from_numpy(host).pin_memory().to(dev, non_blocking=True)
-        views, o = [], 0
-        for p in parts:
-            views.append(dev_buf[o:o + p.size]); o += p.size
-        tok_d, pos_d, cu_d, vis_d, cls_d, cached_d, kvs_d, kvl_d = views
-        vis_parts = [v.to(torch.float32) for v in (cand_vis, hist_vis) if v is not None and v.shape[0] > 0]
-        vis = None if not vis_parts else (vis_parts[0].contiguous() if len(vis_parts) == 1 else torch.cat(vis_parts, 0))
-        x = ops.embed_fwd(tok_d, self.model.embed_tokens.weight.data, vis_d if vis is not None else None, vis)
-        g = self.core.forward_suffix(x, pos_d, cu_d, q_lens, cache.kc, cache.vc, cached_d, kvs_d, kvl_d, out_rows=cls_d)
-        hn, _ = ops.rmsnorm_fwd(g, self.model.norm.weight.data, d.rms_eps)
+        if train:
+            order = np.argsort(tok, kind="stable")           # token order of the deterministic embedding gradient
+            parts += [order, tok[order]]
+        views = _to_device(parts, dev)
+        tok_d, pos_d, cu_d, vis_d, cls_d, cached_d, kvs_d, kvl_d = views[:8]
         cache.stats["steps"] += 1
         cache.stats["tokens"] += int(sum(kv_len))
         cache.stats["tokens_encoded"] += int(sum(q_lens))
+        cache.writes += 1
+        if cache.train:
+            base = np.concatenate([[0], np.cumsum(np.asarray(hist_counts, dtype=np.int64))])
+            for b in range(B):
+                cache.hist[b] = None if hist_vis is None else hist_vis[base[b]:base[b + 1]].detach()
+        vis_parts = [v.to(torch.float32) for v in (cand_vis, hist_vis) if v is not None and v.shape[0] > 0]
+        vis = None if not vis_parts else (vis_parts[0].contiguous() if len(vis_parts) == 1 else torch.cat(vis_parts, 0))
+        if train:
+            for b in range(B):
+                cache.reused[b] = max(cache.reused[b], int(cached[b]))
+            kv = SimpleNamespace(cache=cache, cached=cached_d, kv_start=kvs_d, kv_len=kvl_d, kv_lens=list(kv_len),
+                                 cached_host=list(cached), write_id=cache.writes)
+            sp = SimpleNamespace(ids=tok_d, pos=pos_d, cu=cu_d, seqlens=list(q_lens), T=int(tok.size), vis_src=vis_d,
+                                 tok_order=views[8], tok_sorted=views[9], n_loss=0, kv=kv)
+            anchor = self._anchor.detach().requires_grad_(True)
+            return _LMFn.apply(self, sp, vis, "rows", cls_d, True, anchor)
+        with torch.no_grad():
+            x = ops.embed_fwd(tok_d, self.model.embed_tokens.weight.data, vis_d if vis is not None else None, vis)
+            g = self.core.forward_suffix(x, pos_d, cu_d, q_lens, cache.kc, cache.vc, cached_d, kvs_d, kvl_d, out_rows=cls_d)
+            hn, _ = ops.rmsnorm_fwd(g, self.model.norm.weight.data, d.rms_eps)
         return hn
 
     def lm_loss(self, pp: PackedPrompt, vis: Optional[torch.Tensor]) -> torch.Tensor:

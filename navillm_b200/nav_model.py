@@ -208,6 +208,7 @@ class NavModel(nn.Module):
         # data-parallel gradient exchange: ONE state shared with the language model (navillm_b200/parallel.py)
         self.grad_sync = GradSync()
         self.grad_sync.flats = self._sync_flats
+        self.grad_sync.before_exchange = self.lang_model.flush_prefix_caches
         self.lang_model.grad_sync = self.grad_sync
         if logger is not None:
             logger.info("model type: {}".format(self.model_type))
@@ -286,10 +287,7 @@ class NavModel(nn.Module):
         """``zero_grad(lazy=True)`` promised that the next LM backward overwrites the per-layer gradients.  If an
         exchange or an optimizer step arrives with no LM backward in between (a skipped / guarded iteration), the stale
         values must not be applied: make the promise true by zero-filling now."""
-        lm = self.lang_model
-        if lm.core is not None and getattr(lm.flat, "overwrite_layer_grads", False):
-            lm.flat.flat_grad[:lm.flat.offset_of(lm.model.embed_tokens.weight)].zero_()
-            lm.flat.overwrite_layer_grads = False
+        self.lang_model._settle_lazy_zero()
 
     @contextlib.contextmanager
     def no_sync(self):
@@ -307,7 +305,11 @@ class NavModel(nn.Module):
         """Gradients live in two flat buffers, so zeroing is two fills instead of one per parameter.  With
         ``lazy=True`` the per-layer LM gradients are not zeroed at all: the next backward OVERWRITES them
         (beta = 0 wgrad epilogue) -- identical result, 27 GB less HBM traffic per step; until that backward runs
-        their ``.grad`` views hold stale values."""
+        their ``.grad`` views hold stale values.  Raises while a training ``PrefixKVCache`` of the model has pending
+        gradient: it would be added after the zeroing (call ``flush_grads()`` before the optimizer step)."""
+        if self.lang_model.prefix_grads_pending():
+            raise RuntimeError("zero_grad(): a PrefixKVCache(train=True) of this model has pending gradient; call "
+                               "cache.flush_grads() before optimizer.step() / zero_grad()")
         if self.lang_model.core is None or self._flat32 is None:
             return super().zero_grad(set_to_none=set_to_none)
         self._ensure()
@@ -421,9 +423,11 @@ class NavModel(nn.Module):
         text = batch["text_input"] if batch["text_input"] is not None else self.lang_model.tokenize(batch["prompts"])
         prefix_cache = kwargs.get("prefix_cache")
         if prefix_cache is not None:
-            # evaluation rollouts (not in the reference): encode only what follows each row's cached prompt prefix
-            if torch.is_grad_enabled():
-                raise RuntimeError("prefix_cache is an inference feature: call under torch.no_grad() (weights must not change)")
+            # rollouts (not in the reference): encode only what follows each row's cached prompt prefix; training needs a
+            # PrefixKVCache(train=True), whose flush_grads() adds the gradient through the cached rows
+            if torch.is_grad_enabled() and not prefix_cache.train:
+                raise RuntimeError("prefix_cache is an inference feature: call under torch.no_grad() (weights must not change), "
+                                   "or build the cache with PrefixKVCache(..., train=True) for a training rollout")
             hist_counts = [len(v) for v in (batch["hist_vis"] or [[] for _ in range(B)])]
             h_cls = self.lang_model.hidden_rows_cached(text["input_ids"], text["attention_mask"], cand_embeds, hist_vis_input,
                                                        hist_counts, prefix_cache)

@@ -94,10 +94,13 @@ def attn_fwd(qkv: torch.Tensor, cu_seqlens: torch.Tensor, seqlens, n_heads: int,
 
 
 def attn_fwd_kv(q: torch.Tensor, kcache: torch.Tensor, vcache: torch.Tensor, cu_q: torch.Tensor, q_lens, kv_start: torch.Tensor,
-                kv_len: torch.Tensor, n_heads: int, *, out: torch.Tensor | None = None, scale: float | None = None):
+                kv_len: torch.Tensor, n_heads: int, *, out: torch.Tensor | None = None, scale: float | None = None,
+                lse: torch.Tensor | None = None):
     """Suffix attention over a KV cache (nv_attn_fwd_kv): q [Tq, >=H*128] bf16 view of the packed new rows (RoPE
     applied), caches [B, Smax, H*128] bf16 (already holding the new rows' K/V, zero-initialised), kv_start / kv_len
-    int32 [B] on the device.  Query i of sequence b sees keys <= kv_len[b] - q_lens[b] + i.  Returns o [Tq, H*128]."""
+    int32 [B] on the device.  Query i of sequence b sees keys <= kv_len[b] - q_lens[b] + i.  Returns o [Tq, H*128].
+    ``lse`` (fp32 [H, Tq], optional) receives the log-sum-exp of the scaled scores, as ``attn_fwd`` returns it (the
+    input of ``attn_bwd_kv``)."""
     _rowmajor(q, "q")
     hd = 128
     Tq = q.shape[0]
@@ -108,12 +111,14 @@ def attn_fwd_kv(q: torch.Tensor, kcache: torch.Tensor, vcache: torch.Tensor, cu_
         assert t.dtype == torch.int32 and t.is_cuda
     if out is None:
         out = torch.empty((Tq, n_heads * hd), dtype=bf16, device=q.device)
+    if lse is not None and (lse.dtype != torch.float32 or not lse.is_contiguous() or tuple(lse.shape) != (n_heads, Tq)):
+        raise ValueError(f"attn_fwd_kv: lse fp32 [{n_heads}, {Tq}] contiguous expected (got {lse.dtype} {tuple(lse.shape)})")
     if scale is None:
         scale = hd ** -0.5
     Tkv = kcache.shape[0] * kcache.shape[1]
     ldk = kcache.shape[2]
     check(_lib.load().nv_attn_fwd_kv(ptr(q), i64(q.stride(0)), ptr(kcache), i64(ldk), ptr(vcache), i64(ldk), ptr(out),
-                                     i64(out.stride(0)), ptr(None), ptr(cu_q), ptr(kv_start), ptr(kv_len), i32(B), i32(Tq),
+                                     i64(out.stride(0)), ptr(lse), ptr(cu_q), ptr(kv_start), ptr(kv_len), i32(B), i32(Tq),
                                      i32(Tkv), i32(n_heads), i32(hd), i32(_qblocks(q_lens)), f32(scale), stream_ptr()),
           "nv_attn_fwd_kv")
     return out
@@ -308,6 +313,62 @@ def attn_bwd(qkv: torch.Tensor, o: torch.Tensor, do: torch.Tensor, lse: torch.Te
                                   ptr(rope[0] if rope else None), ptr(rope[1] if rope else None), ptr(rope[2] if rope else None),
                                   stream_ptr()),
           "nv_attn_bwd")
+    if have_d:
+        _lib.launch_count -= 1          # the row-sum kernel was not launched
+    return dqkv
+
+
+def attn_bwd_kv(q: torch.Tensor, o: torch.Tensor, do: torch.Tensor, lse: torch.Tensor, kcache: torch.Tensor, vcache: torch.Tensor,
+                acc: torch.Tensor, cu_q: torch.Tensor, q_lens, kv_start: torch.Tensor, kv_len: torch.Tensor, kv_lens, n_heads: int, *,
+                dqkv: torch.Tensor | None = None, scale: float | None = None, rope=None, dvec: torch.Tensor | None = None) -> torch.Tensor:
+    """Backward of ``attn_fwd_kv`` (nv_attn_bwd_kv): returns dqkv [Tq, 3*H*128] bf16 (dq | dk | dv of the packed suffix rows).
+
+    q [Tq, >=H*128] (post-RoPE), o / do [Tq, H*128] bf16, lse fp32 [H, Tq] from ``attn_fwd_kv(lse=...)``; caches bf16
+    [B, Smax, H*128] as the forward read them; acc fp32 [B, Smax, 2*H*128] (dK | dV columns) accumulator over the cache
+    rows.  ``q_lens`` / ``kv_lens``: host lengths (``kv_len`` / ``kv_start`` int32 [B] on the device).  Rows j < kv_len - q_len
+    of sequence b accumulate their dK / dV into acc; the suffix rows get dK + acc, dV + acc.  rope / dvec: as ``attn_bwd``."""
+    hd = 128
+    HD = n_heads * hd
+    B = len(q_lens)
+    Tq = int(sum(int(l) for l in q_lens))
+    for name, t in (("q", q), ("o", o), ("do", do)):
+        if t.dtype != bf16 or t.dim() != 2 or t.stride(1) != 1 or t.shape[0] != Tq or t.shape[1] < HD or not t.is_cuda:
+            raise ValueError(f"attn_bwd_kv: {name} bf16 [{Tq}, >= {HD}] CUDA rows expected (got {t.dtype} {tuple(t.shape)})")
+    if kcache.dtype != bf16 or vcache.dtype != bf16 or kcache.dim() != 3 or kcache.shape != vcache.shape or kcache.shape[2] != HD \
+            or not kcache.is_contiguous() or not vcache.is_contiguous():
+        raise ValueError(f"attn_bwd_kv: bf16 [B, Smax, {HD}] contiguous caches expected (got {kcache.dtype} {tuple(kcache.shape)}, "
+                         f"{vcache.dtype} {tuple(vcache.shape)})")
+    Bc, Smax = kcache.shape[:2]
+    if acc.dtype != torch.float32 or tuple(acc.shape) != (Bc, Smax, 2 * HD) or not acc.is_contiguous() or acc.device != kcache.device:
+        raise ValueError(f"attn_bwd_kv: accumulator fp32 [{Bc}, {Smax}, {2 * HD}] contiguous expected "
+                         f"(got {acc.dtype} {tuple(acc.shape)})")
+    if lse.dtype != torch.float32 or tuple(lse.shape) != (n_heads, Tq) or not lse.is_contiguous():
+        raise ValueError(f"attn_bwd_kv: lse fp32 [{n_heads}, {Tq}] expected (got {lse.dtype} {tuple(lse.shape)})")
+    for name, t, n in (("cu_q", cu_q, B + 1), ("kv_start", kv_start, B), ("kv_len", kv_len, B)):
+        if t.dtype != torch.int32 or t.numel() != n or not t.is_cuda:
+            raise ValueError(f"attn_bwd_kv: {name} int32 [{n}] on the device expected (got {t.dtype} {tuple(t.shape)})")
+    if len(kv_lens) != B or any(int(k) < int(l) or int(k) > Smax for k, l in zip(kv_lens, q_lens)):
+        raise ValueError(f"attn_bwd_kv: kv_lens {list(kv_lens)} must satisfy q_len <= kv_len <= {Smax}")
+    if dqkv is None:
+        dqkv = torch.empty((Tq, 3 * HD), dtype=bf16, device=q.device)
+    if dqkv.dtype != bf16 or dqkv.stride(1) != 1 or tuple(dqkv.shape) != (Tq, 3 * HD):
+        raise ValueError(f"attn_bwd_kv: dqkv bf16 [{Tq}, {3 * HD}] expected (got {dqkv.dtype} {tuple(dqkv.shape)})")
+    if scale is None:
+        scale = hd ** -0.5
+    have_d = dvec is not None
+    if not have_d:
+        dvec = _workspace(q.device, n_heads * Tq + 16)
+    dq, dk, dv = dqkv[:, :HD], dqkv[:, HD:2 * HD], dqkv[:, 2 * HD:]
+    acc2 = acc.view(Bc * Smax, 2 * HD)
+    n_kblocks = int(sum((int(k) + 127) // 128 for k in kv_lens))
+    check(_lib.load().nv_attn_bwd_kv(ptr(q), i64(q.stride(0)), ptr(kcache), ptr(vcache), i64(HD), ptr(None if have_d else o),
+                                     i64(o.stride(0)), ptr(do), i64(do.stride(0)), ptr(lse), ptr(dvec), ptr(dq), i64(dqkv.stride(0)),
+                                     ptr(dk), i64(dqkv.stride(0)), ptr(dv), i64(dqkv.stride(0)), ptr(acc2[:, :HD]), ptr(acc2[:, HD:]),
+                                     i64(2 * HD), ptr(cu_q), ptr(kv_start), ptr(kv_len), i32(B), i32(Tq), i32(Bc * Smax),
+                                     i32(n_heads), i32(hd), i32(_qblocks(q_lens)), i32(n_kblocks), f32(scale),
+                                     ptr(rope[0] if rope else None), ptr(rope[1] if rope else None), ptr(rope[2] if rope else None),
+                                     stream_ptr()),
+          "nv_attn_bwd_kv")
     if have_d:
         _lib.launch_count -= 1          # the row-sum kernel was not launched
     return dqkv

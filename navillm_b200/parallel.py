@@ -112,6 +112,7 @@ class GradSync:
         self.overlap = True           # reduce finished layer groups while the backward is still running
         self.chunk_layers = int(os.environ.get("NAVILLM_SYNC_CHUNK", "2"))   # decoder layers per overlapped reduction
         self.flats: Callable[[], list] = lambda: []          # -> [(FlatParams, tail_offset or None), ...]
+        self.before_exchange: Callable[[], None] = lambda: None   # end of an armed pass: complete pending gradients first
         self._pending: List[tuple] = []
         self._lm_layers_reduced = False
         self.reducer: Optional[NvlsReducer] = None            # set by the DDP wrapper when NVLS multicast is available
@@ -175,6 +176,7 @@ class GradSync:
 
     def _end_of_backward(self) -> None:
         try:
+            self.before_exchange()            # training prefix caches: part (b) of the gradient (PrefixKVCache.flush_grads)
             self.exchange(covered_lm_layers=self._lm_layers_reduced)
         finally:
             self.armed = self.queued = False

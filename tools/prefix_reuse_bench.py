@@ -15,6 +15,15 @@ alternated per step, and the cache GiB of each; a bf16 cache that cannot be allo
 name, power limit and SM clocks, read in the same run.
 
     python tools/prefix_reuse_bench.py --kv fp8 --steps 5 [--kv-batches 8,32,64] [--kv-hist0 0,40]
+
+--train times teacher-forced TRAINING rollouts (one backward per step, as tasks/agents/mp3d_agent.py:660-757 does) without a
+cache (the reference's pattern) and with PrefixKVCache(train=True) plus flush_grads() at the end, for every --train-batches x
+--train-steps x instruction length (the ~80-word R2R one and a CVDN-like ~300-word one).  Per shape: one warm-up rollout per
+arm, then the arms alternated (A B B A); ms per rollout, tokens encoded per rollout (steps, and the flush's prefix recompute),
+peak allocated GiB per arm, and the largest gradient difference over all parameters relative to max|grad|.  One JSON line per
+shape, then the GPU name and power limit read in the same run.
+
+    python tools/prefix_reuse_bench.py --train [--train-batches 8,16] [--train-steps 8,15]
 """
 import argparse
 import json
@@ -69,11 +78,16 @@ def main():
                     help="fp8: time the bf16 prefix cache against PrefixKVCache(kv_dtype='fp8') (kernel and rollout)")
     ap.add_argument("--kv-batches", type=str, default="8,32,64")
     ap.add_argument("--kv-hist0", type=str, default="0,40")
+    ap.add_argument("--train", action="store_true", help="training rollouts without / with PrefixKVCache(train=True)")
+    ap.add_argument("--train-batches", type=str, default="8,16")
+    ap.add_argument("--train-steps", type=str, default="8,15")
     a = ap.parse_args()
     from navillm_b200.modified_lm import PrefixKVCache
     dev = torch.device("cuda:0")
     if a.kv == "fp8":
         return kv_compare(a, dev)
+    if a.train:
+        return train_compare(a, dev)
     model = bench.build_model(dev).eval()
     if a.fp8:
         return fp8_rollout(model, a, dev)
@@ -168,6 +182,85 @@ def fp8_rollout(model, a, dev):
         Path(a.json).write_text(json.dumps({"summary": res, "steps": rows}, indent=1))
     if not equal:
         raise SystemExit("prefix_reuse_bench --fp8: fuse_logits differ between the fp8 copy and bf16")
+
+
+def train_rollout(model, dev, B, steps, instr, hist, cache_len):
+    """One teacher-forced training rollout (loss.backward() after every step; with cache_len, a PrefixKVCache(train=True) and
+    flush_grads() at the end).  Returns (ms, tokens encoded by the steps, tokens recomputed by the flush, peak GiB)."""
+    from navillm_b200.modified_lm import PrefixKVCache
+    rng, g = np.random.RandomState(1), torch.Generator().manual_seed(1)
+    D, G, n_cand = 4096, 64, 12
+    model.zero_grad()
+    torch.cuda.synchronize()
+    torch.cuda.reset_peak_memory_stats()
+    t0 = torch.cuda.Event(enable_timing=True); t1 = torch.cuda.Event(enable_timing=True)
+    t0.record()
+    cache = PrefixKVCache(model.lang_model, batch_size=B, max_len=cache_len, train=True) if cache_len else None
+    enc, target = 0, torch.zeros(B, dtype=torch.long, device=dev)
+    for t in range(steps):
+        batch = {k: (v.to(dev) if torch.is_tensor(v) else v) for k, v in make_step(rng, g, B, t, instr, n_cand, D, G).items()}
+        batch["hist_vis"] = [h[:t] for h in hist]
+        text = model.lang_model.tokenize(batch["prompts"])
+        batch["text_input"] = text
+        torch.manual_seed(t)
+        out = model("navigation", batch, **({"prefix_cache": cache} if cache is not None else {}))
+        torch.nn.functional.cross_entropy(out["fuse_logits"].float(), target).backward()
+        enc += int(text["attention_mask"].sum()) if cache is None else 0
+    flush_tok = 0
+    if cache is not None:
+        enc = cache.stats["tokens_encoded"]
+        flush_tok = sum(cache.reused)
+        cache.flush_grads()
+    t1.record()
+    torch.cuda.synchronize()
+    return t0.elapsed_time(t1), enc, flush_tok, torch.cuda.max_memory_allocated() / 2 ** 30
+
+
+def _max_abs_diff(x, y, chunk=1 << 26):
+    """max |x - y| over a flat gradient buffer in fp32 chunks (y may be a 0-d tensor); a full fp32 copy would not fit."""
+    dev = y.device
+    return max((x[i:i + chunk].to(dev).float() - (y if y.dim() == 0 else y[i:i + chunk]).float()).abs().max().item()
+               for i in range(0, x.numel(), chunk))
+
+
+def train_compare(a, dev):
+    model = bench.build_model(dev).eval()          # dropout off; gradients still flow
+    lm = model.lang_model
+    words = [f"w{i}" for i in range(5000)]
+    results = []
+    for n_words, kind in ((80, "r2r"), (300, "cvdn")):
+        for B in [int(x) for x in a.train_batches.split(",")]:
+            for steps in [int(x) for x in a.train_steps.split(",")]:
+                rng = np.random.RandomState(n_words + B)
+                instr = [" ".join(words[i] for i in rng.randint(0, 5000, size=n_words)) for _ in range(B)]
+                gh = torch.Generator().manual_seed(B)
+                hist = [[torch.randn(4096, generator=gh).to(dev) for _ in range(steps)] for _ in range(B)]
+                longest = max(int(lm.tokenize(make_step(np.random.RandomState(0), torch.Generator(), B, steps - 1, instr, 12, 16, 64)
+                                              ["prompts"])["attention_mask"].sum(1).max()), 1)
+                cache_len = (longest + 127) // 128 * 128
+                run = lambda c: train_rollout(model, dev, B, steps, instr, hist, cache_len if c else 0)
+                run(False); run(True)                                       # warm-up of both arms at this shape
+                ms, ref, rel = {False: [], True: []}, None, None
+                for c in (False, True, True, False):
+                    ms[c].append(run(c))
+                    if not c and ref is None and rel is None:          # the first scratch run's gradients ...
+                        ref = [lm.flat.flat_grad.cpu(), model._flat32.flat_grad.cpu()]   # host: the flush's tape needs the room
+                    elif c and rel is None:                           # ... against the first cache run's
+                        scale = max(_max_abs_diff(x, torch.zeros((), dtype=x.dtype, device=dev)) for x in ref)
+                        rel = max(_max_abs_diff(x, y) for x, y in zip(ref, (lm.flat.flat_grad, model._flat32.flat_grad))) / scale
+                        ref = None
+                r = dict(instruction=kind, words=n_words, B=B, steps=steps, cache_max_len=cache_len,
+                         scratch_ms=[round(x[0], 1) for x in ms[False]], cache_ms=[round(x[0], 1) for x in ms[True]],
+                         tokens_scratch=ms[False][0][1], tokens_cache_steps=ms[True][0][1], tokens_cache_flush=ms[True][0][2],
+                         peak_gib_scratch=round(max(x[3] for x in ms[False]), 2), peak_gib_cache=round(max(x[3] for x in ms[True]), 2),
+                         max_grad_diff_rel=rel)
+                print(json.dumps(r), flush=True)
+                results.append(r)
+    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                         text=True).stdout.strip().splitlines()[0]
+    print(json.dumps({"gpu": gpu}), flush=True)
+    if a.json:
+        Path(a.json).write_text(json.dumps({"gpu": gpu, "shapes": results}, indent=1))
 
 
 def gpu_clocks() -> dict:
