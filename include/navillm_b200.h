@@ -84,6 +84,17 @@ int nv_gemm_skinny_swiglu_fp8(const void* X, int64_t ldx, const void* Wgu_q, int
  * and tile width.  block_n: 0 (auto), 32 or 128.  lda % 8 == 0, ldw (bytes) % 16 == 0. */
 int nv_gemm_fp8w_bf16(const void* A, int64_t lda, const void* Wq, int64_t ldw, const void* exps, void* C, int64_t ldc,
                       const void* addend, int64_t ld_add, int M, int N, int K, int block_n, void* stream);
+/* Opt-in W8A8 of the no-grad prompt forwards (set_activation_dtype("fp8"); no reference counterpart for the number format;
+ * csrc/gemm_fp8.cu).  nv_quantize_act_fp8 quantizes a bf16 activation X [M,K] (row stride ldx) per (row, 128-column block)
+ * with the rule of nv_quantize_fp8_rows: Q [M,K] e4m3 bytes (row stride ldq bytes) and E [M, K/128] int8 exponents (row
+ * stride lde), so a row's bytes never depend on other rows.  nv_gemm_w8a8_bf16 computes C[M,N] = A'·W'^T (+ addend) on
+ * the e4m3 tensor cores: A' = (Aq, Ae) in that format, W' = (Wq, We) in the weight format above; every 128-deep k-block
+ * is one e4m3 wgmma chain promoted into an fp32 master with its 2^Ae, in k order, and 2^We and the addend are applied
+ * in the epilogue (C = bf16(bf16(acc) + addend)).  An output element's bits do not depend on M or on the other rows.
+ * K % 128 == 0 (K <= 34688), ldx % 8, ldq / lda / ldw (bytes) % 16, ldc / ld_add % 8, 16-byte aligned bases. */
+int nv_quantize_act_fp8(const void* X, int64_t ldx, void* Q, int64_t ldq, void* E, int64_t lde, int M, int K, void* stream);
+int nv_gemm_w8a8_bf16(const void* Aq, int64_t lda, const void* Ae, int64_t lde, const void* Wq, int64_t ldw, const void* We,
+                      void* C, int64_t ldc, const void* addend, int64_t ld_add, int M, int N, int K, void* stream);
 int nv_gemm_swiglu_bf16(const void* x, int64_t ldx, const void* Wgu, int64_t ldw, void* gu, int64_t ldgu, void* h,
                         int64_t ldh, int M, int F, int K, int keep_gu, void* stream);
 int nv_gemm_dswiglu_bf16(const void* dx, int64_t lddx, const void* Wd, int64_t ldw, const void* gu, int64_t ldgu, void* dgu,
@@ -306,6 +317,9 @@ typedef struct nv_layer_args {
   const void* wgu_q; const void* wgu_e; const void* wd_q; const void* wd_e;
   int fp8_max_rows;
   void* kexp; void* vexp;   /* kv_mode 3, 4: int8 row exponents [B, Smax, H] of the fp8 caches */
+  /* 1: the four GEMMs run W8A8 at every row count (nv_quantize_act_fp8 of the GEMM input + nv_gemm_w8a8_bf16 on the fp8
+   * weight pairs above, which must all be set; D and F multiples of 128); fp8_max_rows is then ignored */
+  int act_fp8;
 } nv_layer_args;
 int nv_layer_args_size(void);                           /* sizeof(nv_layer_args): bindings check their mirror against it */
 int64_t nv_llama_layer_ws_bytes(int T, int R, int D, int F);

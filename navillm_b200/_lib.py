@@ -50,7 +50,8 @@ class LayerArgs(ctypes.Structure):
                 + [("eps", ctypes.c_float), ("scale", ctypes.c_float)]
                 + [(n, ctypes.c_void_p) for n in ("wqkv_q", "wqkv_e", "wo_q", "wo_e", "wgu_q", "wgu_e", "wd_q", "wd_e")]
                 + [("fp8_max_rows", ctypes.c_int)]
-                + [(n, ctypes.c_void_p) for n in ("kexp", "vexp")])
+                + [(n, ctypes.c_void_p) for n in ("kexp", "vexp")]
+                + [("act_fp8", ctypes.c_int)])
 
 
 launch_count = 0          # kernels launched through the C ABI since import (bench.py reports the per-step delta)

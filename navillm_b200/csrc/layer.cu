@@ -7,6 +7,8 @@
 // when each kernel is its own ctypes call from Python (~20 us per call against a few microseconds of GPU work: 328 calls
 // = 10 ms per forward at T = 192); one call per layer leaves the GPU as the limit.  Training-size batches do not
 // need it (their step is GPU-bound) and keep the per-kernel path, which also saves the activations for the backward.
+// act_fp8 (set_activation_dtype("fp8")): each of the four GEMMs is nv_quantize_act_fp8 of its input into the workspace
+// followed by nv_gemm_w8a8_bf16 on the fp8 weight copy, at every row count.
 #include <stdint.h>
 
 #include "navillm_b200.h"
@@ -38,6 +40,9 @@ extern "C" int64_t nv_llama_layer_ws_bytes(int T, int R, int D, int F) {
   int64_t b = al((int64_t)T * D * 2) + al((int64_t)T * 4) + al((int64_t)T * 3 * D * 2) + al((int64_t)T * D * 2);
   if (R > 0) b += 2 * al((int64_t)R * D * 2);
   b += 2 * al(Tm * D * 2) + al(Tm * 4) + al(Tm * 2 * F * 2) + al(Tm * F * 2);
+  // act_fp8: the e4m3 GEMM input (largest: T x D or Tm x F) and its exponents
+  const int64_t qn = (int64_t)T * D > Tm * F ? (int64_t)T * D : Tm * F;
+  b += al(qn) + al(qn / 128);
   return b + 256;
 }
 
@@ -61,11 +66,25 @@ extern "C" int nv_llama_layer_infer(const nv_layer_args* a, void* stream) {
   float* rstd2 = static_cast<float*>(c.take((int64_t)Tm * 4));
   void* gu = c.take((int64_t)Tm * 2 * F * 2);
   void* h = c.take((int64_t)Tm * F * 2);
-  NV_REQUIRE(h != nullptr, "nv_llama_layer_infer: workspace carve failed");
+  const int64_t qn = (int64_t)T * D > (int64_t)Tm * F ? (int64_t)T * D : (int64_t)Tm * F;
+  void* aq = c.take(qn);
+  void* ae = c.take(qn / 128);
+  NV_REQUIRE(ae != nullptr, "nv_llama_layer_infer: workspace carve failed");
+  if (a->act_fp8) {
+    NV_REQUIRE(a->wqkv_q && a->wqkv_e && a->wo_q && a->wo_e && a->wgu_q && a->wgu_e && a->wd_q && a->wd_e,
+               "nv_llama_layer_infer: act_fp8 needs the fp8 copies of all four weights");
+    NV_REQUIRE(D % 128 == 0 && F % 128 == 0, "nv_llama_layer_infer: act_fp8 needs D and F multiples of 128 (D=%d F=%d)", D, F);
+  }
   int rc;
-  // y[rows, N] = x[rows, K] W^T (+ addend): the fp8 copy of W when it is given and the GEMM has at most fp8_max_rows rows
+  // y[rows, N] = x[rows, K] W^T (+ addend): W8A8 on the fp8 copy of W in act_fp8 mode; else the fp8 copy of W when it is
+  // given and the GEMM has at most fp8_max_rows rows
   auto linear = [&](const void* x, const void* w, const void* wq, const void* we, void* y, const void* addend, int rows, int N,
                     int K) {
+    if (a->act_fp8) {
+      const int qrc = nv_quantize_act_fp8(x, K, aq, K, ae, K / 128, rows, K, stream);
+      if (qrc != NV_OK) return qrc;
+      return nv_gemm_w8a8_bf16(aq, K, ae, K / 128, wq, K, we, y, N, addend, D, rows, N, K, stream);
+    }
     if (wq && we && rows <= a->fp8_max_rows)
       return nv_gemm_fp8w_bf16(x, K, wq, K, we, y, N, addend, D, rows, N, K, 0, stream);
     return nv_gemm_bf16(x, K, 0, w, K, 0, y, N, addend, addend ? D : 0, rows, N, K, addend ? 1u : 0u, 0, stream);

@@ -346,6 +346,7 @@ class LlamaCore:
         self.fused_epilogues = True
         self.fp8 = None
         self.fp8_src = None
+        self.act_fp8 = False          # W8A8 in the no-grad forwards (ModifiedLlamaForCausalLM.set_activation_dtype)
 
     def set_fp8(self, fp8: Optional[Fp8Weights]) -> None:
         """Stream ``fp8``'s copy of the linear weights in the inference GEMMs (None: the bf16 weights): the decode step, and
@@ -372,9 +373,30 @@ class LlamaCore:
             return None
         return self.fp8
 
+    def act_fp8_weights(self):
+        """The per-layer fp8 weight pairs of the W8A8 GEMMs when ``act_fp8`` is on, None when it is off.  Raises rather than
+        run bf16: one evaluation must not mix two numerics."""
+        if not self.act_fp8:
+            return None
+        D, F = self.d.hidden, self.d.inter
+        if D % 128 or F % 128:
+            raise RuntimeError(f"activation dtype 'fp8': the W8A8 GEMMs need hidden and intermediate sizes that are multiples "
+                               f"of 128 (got {D}, {F}); call set_activation_dtype('bf16')")
+        if self.fp8 is None:
+            raise RuntimeError("activation dtype 'fp8' needs the fp8 copy of the weights: call quantize_weights_fp8() first, "
+                               "or set_activation_dtype('bf16')")
+        why = self.fp8_src.stale_reason(self.flat)
+        if why is not None:
+            raise RuntimeError(f"activation dtype 'fp8': the fp8 copy of the weights is stale ({why} after "
+                               f"quantize_weights_fp8()); call quantize_weights_fp8() again, or set_activation_dtype('bf16')")
+        return self.fp8
+
     @staticmethod
-    def _linear(a, w, wq, addend=None):
-        """a · w^T (+ addend) from the fp8 pair ``wq`` when it is given and a has at most FP8_MAX_ROWS rows."""
+    def _linear(a, w, wq, addend=None, w8a8=False):
+        """a · w^T (+ addend): W8A8 on the fp8 pair ``wq`` when ``w8a8``; else from ``wq`` when it is given and a has at most
+        FP8_MAX_ROWS rows."""
+        if w8a8:
+            return ops.gemm_w8a8(*ops.quantize_act_fp8(a), *wq, addend=addend)
         if wq[0] is not None and a.shape[0] <= FP8_MAX_ROWS:
             return ops.gemm_fp8w(a, *wq, addend=addend)
         return ops.gemm(a, w, addend=addend)
@@ -382,6 +404,11 @@ class LlamaCore:
     def _fp8_layer(self, f8, l):
         """(qkv, o, gate|up, down) fp8 pairs of layer l for the GEMMs above 16 rows: gate|up stays bf16 (see FP8_MAX_ROWS)."""
         return None if f8 is None else (f8.wqkv[l], f8.wo[l], (None, None), f8.wd[l])
+
+    @staticmethod
+    def _w8a8_layer(a8, l):
+        """(qkv, o, gate|up, down) fp8 pairs of layer l for the W8A8 GEMMs."""
+        return a8.wqkv[l], a8.wo[l], a8.wgu[l], a8.wd[l]
 
     def refresh_grad_views(self) -> None:
         """Re-derive the fused gradient views after ``FlatParams.rebind_grads``."""
@@ -399,7 +426,7 @@ class LlamaCore:
     # they are host-bound when every kernel is its own call from Python
     LAYER_CALL = os.environ.get("NAVILLM_LAYER_CALL", "1") != "0"
 
-    def _forward_layer_calls(self, x, pos, cu, seqlens, kv_store, out_rows):
+    def _forward_layer_calls(self, x, pos, cu, seqlens, kv_store, out_rows, a8=None):
         d = self.d
         T = x.shape[0]
         R = 0 if out_rows is None else out_rows.numel()
@@ -420,8 +447,9 @@ class LlamaCore:
             elif kv_store is not None:
                 kc, vc = kv_store[0][l], kv_store[1][l]
             run.run(x, y, lyr.input_layernorm.weight.data, self.wqkv[l], self.wo[l], lyr.post_attention_layernorm.weight.data, self.wgu[l],
-                    self.wd[l], kc=kc, vc=vc, ke=ke, ve=ve, out_rows=out_rows if pruned else None, fp8=self._fp8_layer(f8, l),
-                    fp8_max_rows=FP8_MAX_ROWS)
+                    self.wd[l], kc=kc, vc=vc, ke=ke, ve=ve, out_rows=out_rows if pruned else None,
+                    fp8=self._w8a8_layer(a8, l) if a8 is not None else self._fp8_layer(f8, l), fp8_max_rows=FP8_MAX_ROWS,
+                    act_fp8=a8 is not None)
             x = y
         return x
 
@@ -443,8 +471,10 @@ class LlamaCore:
         H = d.n_heads
         saved: List[_Saved] = []
         last = d.n_layers - 1
-        # fused-epilogue kernels (128 x 256-tile GEMM) need head_dim 128, F % 128 == 0 and at least one wave of tiles
-        fused = self.fused_epilogues and x.shape[0] >= 1024 and d.inter % 128 == 0 and d.hidden % 256 == 0
+        a8 = None if save else self.act_fp8_weights()       # W8A8 (set_activation_dtype("fp8")): no-grad forwards only
+        # fused-epilogue kernels (128 x 256-tile GEMM) need head_dim 128, F % 128 == 0 and at least one wave of tiles; W8A8
+        # runs the plain GEMM and the RoPE / SwiGLU row kernels instead
+        fused = a8 is None and self.fused_epilogues and x.shape[0] >= 1024 and d.inter % 128 == 0 and d.hidden % 256 == 0
         if kv_store is not None and kv_sink is None:                  # (kc list, vc list): post-RoPE K, V of every layer go to the caches
             B_, T_ = len(seqlens), x.shape[0]
             if is_fp8_kv(kv_store[0]):                                # fp8 cache: (e4m3 bytes, exponents) per layer
@@ -453,17 +483,18 @@ class LlamaCore:
             else:
                 kv_sink = lambda l, qkv: ops.kv_store_prefill(qkv, cu, kv_store[0][l], kv_store[1][l], B_, T_)
         if self.LAYER_CALL and not save and not fused and d.head_dim == 128 and (kv_store is not None or kv_sink is None):
-            return self._forward_layer_calls(x, pos, cu, seqlens, kv_store, out_rows), None
+            return self._forward_layer_calls(x, pos, cu, seqlens, kv_store, out_rows, a8), None
         f8 = None if save else self.fp8_for_inference()     # training forwards never read the fp8 copy
+        q8 = a8 is not None
         for l, lyr in enumerate(self.model.layers):
-            w8 = self._fp8_layer(f8, l) or ((None, None),) * 4
+            w8 = self._w8a8_layer(a8, l) if q8 else (self._fp8_layer(f8, l) or ((None, None),) * 4)
             s = _Saved()
             s.x = x
             s.xn, s.rstd1 = ops.rmsnorm_fwd(x, lyr.input_layernorm.weight.data, d.rms_eps)
             if fused:
                 s.qkv = ops.gemm_rope(s.xn, self.wqkv[l], pos, self.cos, self.sin, 2 * d.hidden)   # RoPE in the epilogue
             else:
-                s.qkv = self._linear(s.xn, self.wqkv[l], w8[0])
+                s.qkv = self._linear(s.xn, self.wqkv[l], w8[0], w8a8=q8)
                 ops.rope_(s.qkv, pos, self.cos, self.sin, 2 * H, d.head_dim)
             if kv_sink is not None:
                 kv_sink(l, s.qkv)                      # prefill of generate(): post-RoPE K,V go to the cache
@@ -474,14 +505,14 @@ class LlamaCore:
                 s.rows = out_rows
                 ao = s.ao_r = ops.gather_rows(s.ao, out_rows)
                 xin = ops.gather_rows(x, out_rows)
-            s.xm = self._linear(ao, self.wo[l], w8[1], addend=xin)
+            s.xm = self._linear(ao, self.wo[l], w8[1], addend=xin, w8a8=q8)
             s.xn2, s.rstd2 = ops.rmsnorm_fwd(s.xm, lyr.post_attention_layernorm.weight.data, d.rms_eps)
             if fused and s.rows is None:
                 s.gu, s.h = ops.gemm_swiglu(s.xn2, self.wgu[l])                                    # SwiGLU in the epilogue
             else:
-                s.gu = self._linear(s.xn2, self.wgu[l], w8[2])
+                s.gu = self._linear(s.xn2, self.wgu[l], w8[2], w8a8=q8)
                 s.h = ops.swiglu_fwd(s.gu)
-            x = self._linear(s.h, self.wd[l], w8[3], addend=s.xm)
+            x = self._linear(s.h, self.wd[l], w8[3], addend=s.xm, w8a8=q8)
             if save:
                 saved.append(s)
         return x, ((saved, (pos, cu, list(seqlens))) if save else None)
@@ -512,7 +543,9 @@ class LlamaCore:
         H, D = d.n_heads, d.hidden
         B, T = len(q_lens), x.shape[0]
         last = d.n_layers - 1
-        fused = self.fused_epilogues and T >= 1024 and d.inter % 128 == 0 and d.hidden % 256 == 0
+        a8 = None if save else self.act_fp8_weights()       # W8A8 (set_activation_dtype("fp8")): no-grad forwards only
+        q8 = a8 is not None
+        fused = not q8 and self.fused_epilogues and T >= 1024 and d.inter % 128 == 0 and d.hidden % 256 == 0
         f8 = None if save else self.fp8_for_inference()     # training forwards never read the fp8 copy
         fp8_kv = is_fp8_kv(kc)
         if save and (fp8_kv or acc is None or kv_lens is None):
@@ -529,19 +562,19 @@ class LlamaCore:
                 (kl, ke), (vl, ve) = (kc[l], vc[l]) if fp8_kv else ((kc[l], None), (vc[l], None))
                 run.run(x, y, lyr.input_layernorm.weight.data, self.wqkv[l], self.wo[l], lyr.post_attention_layernorm.weight.data,
                         self.wgu[l], self.wd[l], kc=kl, vc=vl, ke=ke, ve=ve, out_rows=out_rows if pruned else None,
-                        fp8=self._fp8_layer(f8, l), fp8_max_rows=FP8_MAX_ROWS)
+                        fp8=self._w8a8_layer(a8, l) if q8 else self._fp8_layer(f8, l), fp8_max_rows=FP8_MAX_ROWS, act_fp8=q8)
                 x = y
             return x
         saved: List[_Saved] = []
         for l, lyr in enumerate(self.model.layers):
-            w8 = self._fp8_layer(f8, l) or ((None, None),) * 4
+            w8 = self._w8a8_layer(a8, l) if q8 else (self._fp8_layer(f8, l) or ((None, None),) * 4)
             s = _Saved()
             s.x = x
             xn, s.rstd1 = ops.rmsnorm_fwd(x, lyr.input_layernorm.weight.data, d.rms_eps)
             if fused:
                 qkv = ops.gemm_rope(xn, self.wqkv[l], pos, self.cos, self.sin, 2 * D)
             else:
-                qkv = self._linear(xn, self.wqkv[l], w8[0])
+                qkv = self._linear(xn, self.wqkv[l], w8[0], w8a8=q8)
                 ops.rope_(qkv, pos, self.cos, self.sin, 2 * H, d.head_dim)
             s.lse = torch.empty((H, T), dtype=torch.float32, device=x.device) if save else None
             if fp8_kv:
@@ -558,14 +591,14 @@ class LlamaCore:
                 s.rows = out_rows
                 ao = s.ao_r = ops.gather_rows(ao, out_rows)
                 xin = ops.gather_rows(x, out_rows)
-            s.xm = xm = self._linear(ao, self.wo[l], w8[1], addend=xin)
+            s.xm = xm = self._linear(ao, self.wo[l], w8[1], addend=xin, w8a8=q8)
             s.xn2, s.rstd2 = xn2, _ = ops.rmsnorm_fwd(xm, lyr.post_attention_layernorm.weight.data, d.rms_eps)
             if fused and xm.shape[0] >= 1024:
                 s.gu, s.h = ops.gemm_swiglu(xn2, self.wgu[l], keep_gu=save)
             else:
-                s.gu = self._linear(xn2, self.wgu[l], w8[2])
+                s.gu = self._linear(xn2, self.wgu[l], w8[2], w8a8=q8)
                 s.h = ops.swiglu_fwd(s.gu)
-            x = self._linear(s.h, self.wd[l], w8[3], addend=xm)
+            x = self._linear(s.h, self.wd[l], w8[3], addend=xm, w8a8=q8)
             if save:
                 saved.append(s)
         if not save:

@@ -534,6 +534,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
         self.flat.on_zeroed = self.mark_grads_zeroed
         self._lm_head_grad_clean = False             # unknown until the next zero_grad
         self.core = LlamaCore(self.dims, self.model, self.flat)
+        self.core.act_fp8 = self.activation_dtype == "fp8"
         self.special_ids_dev = torch.tensor(self.special_token_ids, dtype=torch.int32, device=device)
         return self.flat
 
@@ -765,6 +766,28 @@ class ModifiedLlamaForCausalLM(nn.Module):
                                f"decode with them in bf16")
         if self.core.fp8 is None:                    # the decoder stack was rebuilt around the same buffer
             self.core.set_fp8(fp8)
+
+    # ---- opt-in fp8 (e4m3) activations (W8A8) in the no-grad prompt forwards ----
+    activation_dtype = "bf16"
+
+    def set_activation_dtype(self, dtype: str) -> str:
+        """Number format of the decoder-layer GEMM inputs in the no-grad prompt forwards: ``"bf16"`` (default) or ``"fp8"``.
+        Returns the previous format.
+
+        ``"fp8"`` needs ``quantize_weights_fp8()``.  The four decoder-layer linears (q|k|v, o_proj, gate|up, down) then run on
+        the e4m3 tensor cores (W8A8) in every no-grad forward at every row count: navigation and grounding evaluation, no-grad
+        LM forwards, the prefill of ``generate()``, and ``PrefixKVCache`` suffix steps with the bf16 or the fp8 store.  Each
+        GEMM input (the RMSNorm, attention or SwiGLU output) is quantized per (row, 128-column block) with the weight rule
+        (include/navillm_b200.h), so a prompt's outputs do not depend on the batch it came in.  Decode steps, lm_head, the
+        heads, the panorama encoder and every grad-enabled forward are unchanged.  A forward raises, naming the remedy, when
+        the fp8 weight copy is missing or stale or when the hidden or intermediate size is not a multiple of 128; it never
+        falls back to bf16.  Its effect on task metrics has not been measured."""
+        if dtype not in ("bf16", "fp8"):
+            raise ValueError(f"set_activation_dtype: 'bf16' or 'fp8' expected, got {dtype!r}")
+        prev, self.activation_dtype = self.activation_dtype, dtype
+        if self.core is not None:
+            self.core.act_fp8 = dtype == "fp8"
+        return prev
 
     # ---- opt-in fp8 (e4m3) KV cache in generate() ----
     kv_cache_dtype = "bf16"

@@ -259,6 +259,12 @@ class NavModel(nn.Module):
         (default) or ``"fp8"``; see ``ModifiedLlamaForCausalLM.set_kv_cache_dtype``.  Returns the previous format."""
         return self.lang_model.set_kv_cache_dtype(dtype)
 
+    def set_activation_dtype(self, dtype: str) -> str:
+        """Number format of the language model's decoder-layer GEMM inputs in no-grad forwards: ``"bf16"`` (default) or
+        ``"fp8"`` (W8A8 after ``quantize_weights_fp8()``); see ``ModifiedLlamaForCausalLM.set_activation_dtype``.  Returns the
+        previous format."""
+        return self.lang_model.set_activation_dtype(dtype)
+
     def _flat_buffers_ready(self) -> bool:
         return self.lang_model.core is not None and self._flat32 is not None
 

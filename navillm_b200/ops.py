@@ -755,15 +755,18 @@ class LayerRunner:
         a.kv_len = kv_len.data_ptr() if kv_len is not None else None
         self._keep += (cached, kv_start, kv_len)
 
-    def run(self, x, y, ln1, wqkv, wo, ln2, wgu, wd, *, kc=None, vc=None, out_rows=None, fp8=None, fp8_max_rows=0, ke=None, ve=None):
+    def run(self, x, y, ln1, wqkv, wo, ln2, wgu, wd, *, kc=None, vc=None, out_rows=None, fp8=None, fp8_max_rows=0, ke=None, ve=None,
+            act_fp8=False):
         """``fp8``: None, or the (e4m3, exponents) pairs of wqkv, wo, wgu, wd (``Fp8Weights.view``); each GEMM with at most
         ``fp8_max_rows`` rows then streams its pair through nv_gemm_fp8w_bf16 (same bits as the bf16 weights W').
+        ``act_fp8``: every GEMM runs W8A8 on the four pairs of ``fp8`` (all required) at every row count.
         ``ke`` / ``ve``: the row exponents of an fp8 cache (cache modes 3 and 4, kc / vc then hold its e4m3 bytes)."""
         a = self.args
         pairs = fp8 if fp8 is not None else ((None, None),) * 4
         (a.wqkv_q, a.wqkv_e), (a.wo_q, a.wo_e), (a.wgu_q, a.wgu_e), (a.wd_q, a.wd_e) = \
             [(q.data_ptr(), e.data_ptr()) if q is not None else (None, None) for q, e in pairs]
         a.fp8_max_rows = fp8_max_rows if fp8 is not None else 0
+        a.act_fp8 = 1 if act_fp8 else 0
         a.x, a.y = x.data_ptr(), y.data_ptr()
         a.ln1, a.wqkv, a.wo, a.ln2, a.wgu, a.wd = ln1.data_ptr(), wqkv.data_ptr(), wo.data_ptr(), ln2.data_ptr(), wgu.data_ptr(), wd.data_ptr()
         a.kcache = kc.data_ptr() if kc is not None else None
@@ -937,6 +940,58 @@ def gemm_fp8w(a: torch.Tensor, q: torch.Tensor, e: torch.Tensor, *, addend: torc
     check(_lib.load().nv_gemm_fp8w_bf16(ptr(a), i64(a.stride(0)), ptr(q), i64(q.stride(0)), ptr(e), ptr(out), i64(out.stride(0)),
                                         ptr(addend), i64(addend.stride(0) if addend is not None else 0), i32(M), i32(N), i32(K),
                                         i32(block_n), stream_ptr()), "nv_gemm_fp8w_bf16")
+    return out
+
+
+def quantize_act_fp8(x: torch.Tensor, *, q: torch.Tensor | None = None, e: torch.Tensor | None = None):
+    """Quantize the bf16 activation x [M, K] (any row stride, K % 128 == 0) per (row, 128-column block) with the rule of
+    ``quantize_fp8_`` (csrc/gemm_fp8.cu): returns (q float8_e4m3fn [M, K], e int8 [M, K / 128]) with
+    x ~ q * 2^e[:, k // 128].  x is not modified."""
+    _rowmajor(x, "x")
+    if x.dtype != bf16:
+        raise ValueError(f"quantize_act_fp8: bf16 input expected (got {x.dtype})")
+    M, K = x.shape
+    if K % 128:
+        raise ValueError(f"quantize_act_fp8: K must be a multiple of 128 (got {K})")
+    if q is None:
+        q = torch.empty((M, K), dtype=fp8, device=x.device)
+    if e is None:
+        e = torch.empty((M, K // 128), dtype=torch.int8, device=x.device)
+    _rowmajor(q, "q"); _rowmajor(e, "e")
+    if q.dtype != fp8 or e.dtype != torch.int8 or tuple(q.shape) != (M, K) or tuple(e.shape) != (M, K // 128):
+        raise ValueError(f"quantize_act_fp8: q float8_e4m3fn [M, K] and e int8 [M, K/128] expected "
+                         f"(got {q.dtype} {tuple(q.shape)}, {e.dtype} {tuple(e.shape)})")
+    check(_lib.load().nv_quantize_act_fp8(ptr(x), i64(x.stride(0)), ptr(q), i64(q.stride(0)), ptr(e), i64(e.stride(0)), i32(M),
+                                          i32(K), stream_ptr()), "nv_quantize_act_fp8")
+    return q, e
+
+
+def gemm_w8a8(aq: torch.Tensor, ae: torch.Tensor, wq: torch.Tensor, we: torch.Tensor, *, addend: torch.Tensor | None = None,
+              out: torch.Tensor | None = None) -> torch.Tensor:
+    """C [M, N] = A' · W'^T (+ addend) on the e4m3 tensor cores (csrc/gemm_fp8.cu): A' = (aq, ae) from ``quantize_act_fp8``,
+    W' = (wq, we) in the weight format of ``quantize_fp8_``; bf16 output, C = bf16(bf16(acc) + addend).  A row's output does
+    not depend on M or on the other rows."""
+    _fp8_weight(wq, we, "wq"); _rowmajor(aq, "aq"); _rowmajor(ae, "ae")
+    M, K = aq.shape
+    N = wq.shape[0]
+    if aq.dtype != fp8 or ae.dtype != torch.int8 or tuple(ae.shape) != (M, K // 128) or K % 128:
+        raise ValueError(f"gemm_w8a8: aq float8_e4m3fn [M, K] (K % 128 == 0) with int8 [M, K/128] exponents expected "
+                         f"(got {aq.dtype} {tuple(aq.shape)}, {ae.dtype} {tuple(ae.shape)})")
+    if wq.shape[1] != K:
+        raise ValueError(f"gemm_w8a8: contraction mismatch aq {tuple(aq.shape)} wq {tuple(wq.shape)}")
+    if out is None:
+        out = torch.empty((M, N), dtype=bf16, device=aq.device)
+    _rowmajor(out, "out")
+    assert out.shape == (M, N) and out.dtype == bf16
+    if addend is not None:
+        _rowmajor(addend, "addend")
+        assert addend.shape == (M, N) and addend.dtype == bf16
+    lib = _lib.load()
+    _timed(lambda: check(lib.nv_gemm_w8a8_bf16(ptr(aq), i64(aq.stride(0)), ptr(ae), i64(ae.stride(0)), ptr(wq), i64(wq.stride(0)),
+                                                ptr(we), ptr(out), i64(out.stride(0)), ptr(addend),
+                                                i64(addend.stride(0) if addend is not None else 0), i32(M), i32(N), i32(K),
+                                                stream_ptr()), "nv_gemm_w8a8_bf16"),
+           2.0 * M * N * K, M * K + N * K + 2.0 * M * N * (2 if addend is not None else 1))
     return out
 
 
