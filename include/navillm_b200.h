@@ -103,6 +103,18 @@ int nv_gemm_attnd_bf16(const void* dy, int64_t lddy, const void* Wo, int64_t ldw
                        int64_t lddo, float* dvec, int M, int D, int Dout, void* stream);
 int nv_gemm_rope_bf16(const void* x, int64_t ldx, const void* W, int64_t ldw, void* out, int64_t ldo, const int* pos,
                       const void* cos_t, const void* sin_t, int M, int N, int K, int rope_cols, void* stream);
+/* Segmented-contraction weight gradient (deferred wgrad of a training rollout, ModifiedLlamaForCausalLM.defer_weight_grads;
+ * reference: the wgrad half of loss.backward() at tasks/agents/mp3d_agent.py:750-757, one per step there):
+ *   C[M,N] = bf16(bf16(sum_s A_s^T B_s) + addend)      (addend optional; C may alias it)
+ * over n_segs row segments given as HOST arrays: A[s] [rows[s], M] with row stride lda[s], B[s] [rows[s], N] with ldb[s].
+ * All segments accumulate in one fp32 chain of 64-row k-blocks on the 128 x 256 tile (a segment's last k-block is
+ * zero-padded), so C is bit for bit nv_gemm_bf16(a_mn = 1, b_mn = 1) over the row-concatenation of the segments, each
+ * zero-padded to a multiple of 64 rows.  1 <= n_segs <= NV_WGRAD_SEG_MAX, rows[s] >= 1, lda[s] >= M and ldb[s] >= N
+ * multiples of 8, ldc / ld_add >= N, 16-byte aligned bases; anything else returns NV_ERR_BAD_ARG before touching the
+ * device. */
+#define NV_WGRAD_SEG_MAX 64
+int nv_gemm_wgrad_seg_bf16(const void* const* A, const int64_t* lda, const void* const* B, const int64_t* ldb, const int* rows,
+                           int n_segs, void* C, int64_t ldc, const void* addend, int64_t ld_add, int M, int N, void* stream);
 
 /* ---- flash attention on packed rows (csrc/attn_fwd.cu, attn_bwd.cu) ------------------------------------
  * Causal self-attention of HF LlamaAttention (eager softmax(QK^T/sqrt(d)+mask)V; call site

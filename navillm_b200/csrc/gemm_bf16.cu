@@ -32,6 +32,8 @@
 // a third mbarrier per stage; the consumers wait for it and run the unchanged SS wgmmas.  The expansion of stage s + 1
 // overlaps the MMAs of stage s.  The k-blocks, the wgmma sequence and the epilogue are those of the bf16 kernel, and the
 // expanded operand is bit for bit the W' the quantizer wrote back, so C equals nv_gemm_bf16's C on W'.
+#include <type_traits>
+
 #include "nv_common.cuh"
 #include "nv_fp8.cuh"
 #include "nv_host.h"
@@ -450,6 +452,20 @@ struct EpiMaps {
   CUtensorMap m[4];
 };
 
+// Segmented contraction of the weight gradient (nv_gemm_wgrad_seg_bf16): C = sum_s A_s^T B_s over up to WGRAD_SEG_MAX
+// row segments, each with its own pair of TMA maps ({64 m, 64 k} / {64 n, 64 k} boxes over its rows).  Segment s
+// supplies k-blocks [kb_end[s - 1], kb_end[s]) of the tile's single accumulation chain; the last k-block of a segment
+// reads TMA zero fill past its rows.  The maps travel in the kernel parameters (17 KB of the 32 KB sm_90 allows), in
+// the parameter slot that the plain epilogue leaves unused.
+constexpr uint32_t WGRAD_SEG_MAX = 64;
+struct SegMaps {
+  CUtensorMap a[WGRAD_SEG_MAX];
+  CUtensorMap b[WGRAD_SEG_MAX];
+  uint32_t kb_end[WGRAD_SEG_MAX];
+};
+template <bool SEG>
+using WideMaps = std::conditional_t<SEG, SegMaps, EpiMaps>;
+
 // Epilogue slot v (one box) in the idle stage ring: the stages in the order the producer would refill them after the
 // last k-block, three slots per stage (its A tile, then the two halves of its B tile).  Slots 0..8 lie in the stages of
 // k-blocks num_kb - 4 .. num_kb - 2 (or stages no k-block used), which are released while the last k-block computes.
@@ -463,15 +479,17 @@ __device__ __forceinline__ uint32_t frag_offset(uint32_t r, uint32_t i, uint32_t
   return sw128_offset(r, i & 7) + 4 * (lane & 3);
 }
 
-template <bool A_MN, bool B_MN, int EPI>
+// SEG: the segmented wgrad contraction (em is a SegMaps, tmap_a / tmap_b are unused, K = 64 x the total k-blocks).
+template <bool A_MN, bool B_MN, int EPI, bool SEG = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_wide(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-               const __grid_constant__ EpiMaps em, void* __restrict__ Cout, int64_t ldc,
+               const __grid_constant__ WideMaps<SEG> em, void* __restrict__ Cout, int64_t ldc,
                const __nv_bfloat16* __restrict__ addend, int64_t ld_add, uint32_t M, uint32_t N, uint32_t K,
                uint32_t flags, EpiAux ea) {
   using L = WideSmem;
   static_assert(EPI == EPI_PLAIN || (!A_MN && B_MN == (EPI == EPI_DSWIGLU || EPI == EPI_ATTND)),
                 "fused epilogues: the operand forms of their entry points");
+  static_assert(!SEG || (EPI == EPI_PLAIN && A_MN && B_MN), "segmented contraction: the plain wgrad form");
   // logical output columns per tile: WIDE_N, except SWIGLU where the 256 accumulator columns are 128 gate + 128 up
   constexpr uint32_t TILE_N = EPI == EPI_SWIGLU ? 128u : WIDE_N;
   // boxes the producer prefetches for the epilogue (g and u, or O)
@@ -513,20 +531,34 @@ gemm_bf16_wide(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     // ===================== TMA producer =====================
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
+    // SEG: tmap_a / tmap_b are the maps of segment 0; the loop moves to segment s + 1 at k-block kb_end[s]
+    const CUtensorMap* map_a = &tmap_a;
+    const CUtensorMap* map_b = &tmap_b;
+    uint32_t seg = 0, seg_kb0 = 0;
     uint32_t stage = 0, phase = 0;
     for (uint32_t kb = 0; kb < num_kb; ++kb) {
+      if constexpr (SEG) {
+        if (kb == em.kb_end[seg]) {
+          seg_kb0 = kb;
+          ++seg;
+          map_a = &em.a[seg];
+          map_b = &em.b[seg];
+          tma_prefetch_desc(map_a);
+          tma_prefetch_desc(map_b);
+        }
+      }
       mbar_wait(&empty_bar[stage], phase ^ 1);
       if (elect_one()) {
         mbar_arrive_expect_tx(&full_bar[stage], L::STAGE_BYTES);
-        const int32_t k0 = kb * GEMM_BLOCK_K;
+        const int32_t k0 = (kb - seg_kb0) * GEMM_BLOCK_K;
         uint8_t* sa = smem_a + stage * L::A_BYTES;
         uint8_t* sb = smem_b + stage * L::B_BYTES;
         if constexpr (!A_MN) {
-          tma_load_2d(sa, &tmap_a, &full_bar[stage], k0, m0);  // box {64 k, 128 m}
+          tma_load_2d(sa, map_a, &full_bar[stage], k0, m0);  // box {64 k, 128 m}
         } else {
 #pragma unroll
           for (uint32_t i = 0; i < GEMM_BLOCK_M / 64; ++i)  // box {64 m, 64 k} per 64-wide MN atom
-            tma_load_2d(sa + i * (GEMM_BLOCK_K * 128), &tmap_a, &full_bar[stage], m0 + i * 64, k0);
+            tma_load_2d(sa + i * (GEMM_BLOCK_K * 128), map_a, &full_bar[stage], m0 + i * 64, k0);
         }
         // B: K-major two boxes {64 k, 128 n} (SWIGLU: the gate rows n.. and the up rows F + n..), MN-major four boxes
         // {64 n, 64 k}; this CTA loads its 1 / WIDE_CLUSTER share of them into every CTA of the cluster
@@ -537,7 +569,7 @@ gemm_bf16_wide(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
           int32_t c0, c1;
           if constexpr (B_MN) { c0 = n_blk * WIDE_N + i * 64; c1 = k0; }
           else { c0 = k0; c1 = EPI == EPI_SWIGLU ? col0 + i * ea.F : n_blk * WIDE_N + i * 128; }
-          tma_load_2d_multicast(sb + i * BOX_BYTES, &tmap_b, &full_bar[stage], c0, c1, (1u << WIDE_CLUSTER) - 1);
+          tma_load_2d_multicast(sb + i * BOX_BYTES, map_b, &full_bar[stage], c0, c1, (1u << WIDE_CLUSTER) - 1);
         }
       }
       __syncwarp();
@@ -762,11 +794,11 @@ gemm_bf16_wide(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   cluster_sync_all();   // no CTA exits while its peer can still multicast into it or arrive on its barriers
 }
 
-template <bool A_MN, bool B_MN, int EPI = EPI_PLAIN>
+template <bool A_MN, bool B_MN, int EPI = EPI_PLAIN, bool SEG = false>
 static int launch_wide(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int64_t ldc, const void* addend,
                        int64_t ld_add, uint32_t M, uint32_t N, uint32_t K, uint32_t flags, cudaStream_t stream,
-                       const EpiMaps& em = EpiMaps{}, EpiAux ea = EpiAux{}) {
-  auto kern = gemm_bf16_wide<A_MN, B_MN, EPI>;
+                       const WideMaps<SEG>& em = WideMaps<SEG>{}, EpiAux ea = EpiAux{}) {
+  auto kern = gemm_bf16_wide<A_MN, B_MN, EPI, SEG>;
   cudaLaunchConfig_t cfg = {};
   cfg.blockDim = dim3(GEMM_THREADS);
   cfg.dynamicSmemBytes = WideSmem::DYN_BYTES;
@@ -860,6 +892,50 @@ extern "C" int nv_gemm_bf16(const void* A, int64_t lda, int a_mn, const void* B,
   }
   NV_GEMM_CASE(128, 6);
 #undef NV_GEMM_CASE
+}
+
+// C[M,N] = bf16(bf16(sum_s A_s^T B_s) (+ addend)): the weight gradient of the row segments s, A_s [rows_s, M] (row stride
+// lda[s]), B_s [rows_s, N] (ldb[s]), accumulated in ONE fp32 chain of 64-row k-blocks on the 128 x 256 cluster tile.  Bit
+// for bit nv_gemm_bf16(a_mn = b_mn = 1) over the row-concatenation of the segments, each zero-padded to a multiple of 64.
+extern "C" int nv_gemm_wgrad_seg_bf16(const void* const* A, const int64_t* lda, const void* const* B, const int64_t* ldb,
+                                      const int* rows, int n_segs, void* C, int64_t ldc, const void* addend, int64_t ld_add,
+                                      int M, int N, void* stream_) {
+  using namespace nv;
+  NV_REQUIRE(n_segs >= 1 && n_segs <= (int)WGRAD_SEG_MAX, "nv_gemm_wgrad_seg_bf16: %d segments (1..%u)", n_segs,
+             WGRAD_SEG_MAX);
+  NV_REQUIRE(A && lda && B && ldb && rows, "nv_gemm_wgrad_seg_bf16: null segment table");
+  NV_REQUIRE(M > 0 && N > 0 && C, "nv_gemm_wgrad_seg_bf16: empty problem M=%d N=%d or null C", M, N);
+  NV_REQUIRE(ldc >= N && (reinterpret_cast<uintptr_t>(C) & 15) == 0, "nv_gemm_wgrad_seg_bf16: ldc %lld < N or C %p not "
+             "16-byte aligned", (long long)ldc, C);
+  NV_REQUIRE(!addend || (ld_add >= N && (reinterpret_cast<uintptr_t>(addend) & 15) == 0),
+             "nv_gemm_wgrad_seg_bf16: ld_add %lld < N or addend %p not 16-byte aligned", (long long)ld_add, addend);
+  uint64_t total_kb = 0;
+  for (int s = 0; s < n_segs; ++s) {
+    NV_REQUIRE(A[s] && B[s], "nv_gemm_wgrad_seg_bf16: segment %d: null operand", s);
+    NV_REQUIRE(rows[s] > 0, "nv_gemm_wgrad_seg_bf16: segment %d: %d rows", s, rows[s]);
+    NV_REQUIRE((lda[s] & 7) == 0 && lda[s] >= M && (ldb[s] & 7) == 0 && ldb[s] >= N,
+               "nv_gemm_wgrad_seg_bf16: segment %d: lda %lld / ldb %lld must be multiples of 8 and at least M=%d / N=%d", s,
+               (long long)lda[s], (long long)ldb[s], M, N);
+    NV_REQUIRE(((reinterpret_cast<uintptr_t>(A[s]) | reinterpret_cast<uintptr_t>(B[s])) & 15) == 0,
+               "nv_gemm_wgrad_seg_bf16: segment %d: base pointers not 16-byte aligned", s);
+    total_kb += ceil_div_u32((uint32_t)rows[s], GEMM_BLOCK_K);
+  }
+  NV_REQUIRE(total_kb * GEMM_BLOCK_K <= 0x7fffffffu, "nv_gemm_wgrad_seg_bf16: %llu k-blocks", (unsigned long long)total_kb);
+  // heap: 17 KB of maps, copied into the launch's parameters
+  SegMaps* sm = new SegMaps();
+  int rc = NV_OK;
+  uint32_t kb = 0;
+  for (int s = 0; s < n_segs && rc == NV_OK; ++s) {
+    rc = gemm_tmaps(&sm->a[s], &sm->b[s], A[s], lda[s], 1, B[s], ldb[s], 1, M, N, rows[s], 256, (uint64_t)N);
+    kb += ceil_div_u32((uint32_t)rows[s], GEMM_BLOCK_K);
+    sm->kb_end[s] = kb;
+  }
+  if (rc == NV_OK)
+    rc = launch_wide<true, true, EPI_PLAIN, true>(sm->a[0], sm->b[0], C, ldc, addend, ld_add, (uint32_t)M, (uint32_t)N,
+                                                  kb * GEMM_BLOCK_K, addend ? GEMM_ADD : 0u,
+                                                  reinterpret_cast<cudaStream_t>(stream_), *sm);
+  delete sm;
+  return rc;
 }
 
 // C[M,N] = A[M,K] · W'[N,K]^T (+ addend) with W' = Wq * 2^exps given in the fp8 weight format (e4m3 rows, one int8

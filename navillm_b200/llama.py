@@ -172,6 +172,11 @@ class FlatParams:
         return self.params[0].data_ptr() == self._ptr0 and self.params[0].grad is not None and \
             self.params[0].grad.data_ptr() == self.flat_grad.data_ptr()
 
+    def weight_state(self):
+        """Changes with every write to the weights: new storage, a torch in-place op on the buffer or a parameter (version
+        counters), or a raw-pointer writer's ``generation`` bump."""
+        return self.flat.data_ptr(), self.flat._version, self.generation, sum(p._version for p in self.params)
+
     def offset_of(self, p: nn.Parameter) -> int:
         return self.offsets[next(k for k, q in enumerate(self.params) if q is p)]
 
@@ -310,6 +315,91 @@ def rope_tables(d: LlamaDims, device) -> tuple:
     return emb.cos().to(bf16).to(device).contiguous(), emb.sin().to(bf16).to(device).contiguous()
 
 
+class WgradStash:
+    """Deferred weight gradients of the decoder linears (q|k|v, o_proj, gate|up, down of every layer).
+
+    While a ``LlamaCore`` holds one (``wgrad_stash``), its ``backward`` records the operand pair (dY, X) of each of those
+    wgrad GEMMs instead of launching it -- references to the tape and gradient tensors, no copies -- and ``flush`` runs
+    ONE segmented-contraction GEMM per weight (``ops.gemm_wgrad_seg``) with the current gradient as addend: the same sum
+    as the per-backward path, rounded to bf16 once instead of once per backward, and one read-modify-write of the
+    gradient buffer instead of one per backward.
+
+    ``max_rows`` bounds the stash in backward rows (the tensors it keeps alive, ``nbytes``): a backward that would take it
+    past the bound, or past ``ops.WGRAD_SEG_MAX`` backwards, flushes it first; a backward of more than ``max_rows / 2`` rows
+    (one that could not share a flush with another of its size) runs its weight gradients at once.  A backward under a
+    lazy zero (``flat.overwrite_layer_grads``) records that the linears' gradients are logically zero, so that their flush
+    overwrites the stale values instead of adding to them.  A backward's pairs enter the stash only when it completes
+    (``commit``): one that raises leaves the stash as it was.  The flush raises when the weights changed after the first
+    recorded backward (the gradient belongs to the old weights)."""
+
+    def __init__(self, core: "LlamaCore", max_rows: int):
+        self.core = core
+        self.max_rows = int(max_rows)
+        self._staged = None            # (rows, acc, weight state, [(key, a, b)]) of the running backward
+        self._clear()
+
+    def _clear(self) -> None:
+        self.pairs = {}                # (gradient attribute, layer) -> [(a, b), ...], one pair per recorded backward
+        self.rows = 0                  # backward rows recorded since the last flush
+        self.backwards = 0
+        self.zero = False              # the linears' gradients are logically zero: the flush overwrites them
+        self._weights = None
+
+    @property
+    def pending(self) -> bool:
+        return self.backwards > 0
+
+    @property
+    def nbytes(self) -> int:
+        """Device bytes of the distinct tensors the stash keeps alive."""
+        seen = {}
+        for prs in self.pairs.values():
+            for a, b in prs:
+                for t in (a, b):
+                    st = t.untyped_storage()
+                    seen[st.data_ptr()] = st.nbytes()
+        return sum(seen.values())
+
+    def begin(self, rows: int, acc: bool) -> bool:
+        """A backward of ``rows`` rows starts (``acc``: it would add to the gradients).  Returns True when it defers."""
+        self._staged = None                              # the pairs of a backward that raised are dropped here
+        if rows > self.max_rows // 2:
+            self.flush()
+            return False
+        if self.rows + rows > self.max_rows or self.backwards >= ops.WGRAD_SEG_MAX:
+            self.flush()
+        if self.backwards > 0 and not acc:
+            raise RuntimeError("deferred weight gradients: a zero_grad() ran while backward rows were stashed")
+        self._staged = (rows, acc, self.core.flat.weight_state(), [])
+        return True
+
+    def record(self, grad: str, layer: int, a: torch.Tensor, b: torch.Tensor) -> None:
+        self._staged[3].append(((grad, layer), a, b))
+
+    def commit(self) -> None:
+        """The backward that ``begin`` deferred completed: its pairs join the stash."""
+        rows, acc, weights, recs = self._staged
+        self._staged = None
+        if self.backwards == 0:
+            self._weights, self.zero = weights, not acc
+        for key, a, b in recs:
+            self.pairs.setdefault(key, []).append((a, b))
+        self.rows += rows
+        self.backwards += 1
+
+    def flush(self) -> None:
+        """One segmented wgrad GEMM per stashed weight into its gradient; then the stash is empty.  A no-op when empty."""
+        if not self.pending:
+            return
+        if self.core.flat.weight_state() != self._weights:
+            raise RuntimeError("deferred weight gradients: the weights changed while backward rows were stashed (optimizer "
+                               "step, load or another write); flush_weight_grads() must run before the weights change")
+        for (grad, l), prs in self.pairs.items():
+            g = getattr(self.core, grad)[l]
+            ops.gemm_wgrad_seg(prs, g, addend=None if self.zero else g)
+        self._clear()
+
+
 class _Saved:
     __slots__ = ("x", "rstd1", "xn", "qkv", "ao", "lse", "xm", "rstd2", "xn2", "gu", "h", "rows", "ao_r")
 
@@ -347,6 +437,7 @@ class LlamaCore:
         self.fp8 = None
         self.fp8_src = None
         self.act_fp8 = False          # W8A8 in the no-grad forwards (ModifiedLlamaForCausalLM.set_activation_dtype)
+        self.wgrad_stash: Optional[WgradStash] = None   # deferred linear weight gradients (defer_weight_grads)
 
     def set_fp8(self, fp8: Optional[Fp8Weights]) -> None:
         """Stream ``fp8``'s copy of the linear weights in the inference GEMMs (None: the bf16 weights): the decode step, and
@@ -627,11 +718,17 @@ class LlamaCore:
         # Weight-gradient GEMMs on a SIDE stream (NAVILLM_WGRAD_STREAM=1): nothing downstream in the backward reads a weight
         # gradient, so they can trail the dgrad chain: when one GEMM's last, partially filled wave of tiles leaves SMs idle, the
         # other stream's kernel takes them.
-        side = WGRAD_STREAM and dx.shape[0] >= 1024
+        # deferred weight gradients (WgradStash): the four linears' wgrad operands are recorded, not launched
+        defer = self.wgrad_stash is not None and self.wgrad_stash.begin(saved[0].x.shape[0], acc)   # the backward's rows
+        side = WGRAD_STREAM and dx.shape[0] >= 1024 and not defer
         main = torch.cuda.current_stream() if side else None
         ws = self._wgrad_stream() if side else None
 
-        def wgrad(a, b, out, *, keep=()):
+        def wgrad(a, b, grad, l, *, keep=()):
+            out = getattr(self, grad)[l]
+            if defer:
+                self.wgrad_stash.record(grad, l, a, b)
+                return
             if not side:
                 ops.gemm(a, b, a_mn=True, b_mn=True, out=out, addend=add(out))
                 return
@@ -652,9 +749,9 @@ class LlamaCore:
                 dh = ops.gemm(dx, self.wd[l], b_mn=True)                               # [T,F]  dgrad
                 dgu = ops.swiglu_bwd(s.gu, dh)
                 del dh
-            wgrad(dx, s.h, self.gd[l])                                                 # dWd += dx^T h
+            wgrad(dx, s.h, "gd", l)                                                 # dWd += dx^T h
             dxn2 = ops.gemm(dgu, self.wgu[l], b_mn=True)                               # [T,D]
-            wgrad(dgu, s.xn2, self.ggu[l])
+            wgrad(dgu, s.xn2, "ggu", l)
             del dgu
             dxm = ops.rmsnorm_bwd(s.xm, lyr.post_attention_layernorm.weight.data, s.rstd2, dxn2, dres=dx,
                                   dw=lyr.post_attention_layernorm.weight.grad, accumulate_dw=acc)
@@ -666,10 +763,10 @@ class LlamaCore:
             else:
                 dao = ops.gemm(dxm, self.wo[l], b_mn=True)
             if s.rows is None:
-                wgrad(dxm, s.ao, self.go[l])
+                wgrad(dxm, s.ao, "go", l)
             else:
                 # pruned last layer: everything above ran on the R requested rows; scatter back to [T, D]
-                wgrad(dxm, s.ao_r, self.go[l])
+                wgrad(dxm, s.ao_r, "go", l)
                 full = torch.zeros_like(s.ao)
                 ops.scatter_rows_(dao, s.rows, full)
                 dao = full
@@ -684,7 +781,7 @@ class LlamaCore:
                                        kv.kv_len, kv.kv_lens, H, rope=(pos, self.cos, self.sin), dvec=dvec)
             del dao
             dxn = ops.gemm(dqkv, self.wqkv[l], b_mn=True)
-            wgrad(dqkv, s.xn, self.gqkv[l])
+            wgrad(dqkv, s.xn, "gqkv", l)
             del dqkv
             dx = ops.rmsnorm_bwd(s.x, lyr.input_layernorm.weight.data, s.rstd1, dxn, dres=dxm,
                                  dw=lyr.input_layernorm.weight.grad, accumulate_dw=acc)
@@ -700,6 +797,8 @@ class LlamaCore:
             ev = torch.cuda.Event()
             ev.record(ws)
             main.wait_event(ev)                            # whoever reads the gradients next is ordered after the wgrads
+        if defer:
+            self.wgrad_stash.commit()
         self.flat.overwrite_layer_grads = False
         return dx
 

@@ -28,7 +28,7 @@ import torch.nn as nn
 from . import llama as llama_mod
 from . import ops
 from . import trie as trie_mod
-from .llama import FlatParams, Fp8Weights, LlamaCore, LlamaDims, LlamaModelParams, _Linear
+from .llama import FlatParams, Fp8Weights, LlamaCore, LlamaDims, LlamaModelParams, WgradStash, _Linear
 from .parallel import GradSync
 from .tokenizer import HFTokenizerAdapter, SyntheticTokenizer
 
@@ -212,8 +212,7 @@ class PrefixKVCache:
 
     # ---- training ----------------------------------------------------------------------------------------------
     def _weight_state(self):
-        flat = self._lm().flat
-        return flat.flat.data_ptr(), flat.flat._version, flat.generation, sum(p._version for p in flat.params)
+        return self._lm().flat.weight_state()
 
     def check_weights(self) -> None:
         if self._weight_state() != self._weights:
@@ -426,7 +425,8 @@ class _LMFn(torch.autograd.Function):
         lm.grad_sync.short_backward = pp.T < lm.SHORT_BACKWARD_TOKENS
         # a pass that leaves prefix-cache gradient pending is not final per layer until the flush (before the exchange):
         # no overlapped per-layer reductions
-        overlap = kv is None and not lm.prefix_grads_pending()
+        # (nor does a deferred weight gradient, final only at its flush)
+        overlap = kv is None and not lm.prefix_grads_pending() and lm._wgrad_stash is None
         dx = core.backward(dg, ctx.tape, layer_done=lm._grad_sync_hook() if overlap else None)
         if kv is not None:
             kv.cache._mark_pending(kv.cached_host)
@@ -460,7 +460,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
         self.register_buffer("_anchor", torch.zeros((), dtype=torch.float32), persistent=False)
         self.grad_sync = GradSync()                  # replaced by NavModel's shared state when owned by a NavModel
         self.grad_sync.flats = self._own_flats
-        self.grad_sync.before_exchange = self.flush_prefix_caches
+        self.grad_sync.before_exchange = self.complete_pending_grads
         self._prefix_caches = weakref.WeakSet()      # PrefixKVCache(train=True) instances built on this model
         if tokenizer is not None:
             self._set_tokenizer(tokenizer)
@@ -535,6 +535,9 @@ class ModifiedLlamaForCausalLM(nn.Module):
         self._lm_head_grad_clean = False             # unknown until the next zero_grad
         self.core = LlamaCore(self.dims, self.model, self.flat)
         self.core.act_fp8 = self.activation_dtype == "fp8"
+        if self._wgrad_stash is not None:
+            self._wgrad_stash.core = self.core
+            self.core.wgrad_stash = self._wgrad_stash
         self.special_ids_dev = torch.tensor(self.special_token_ids, dtype=torch.int32, device=device)
         return self.flat
 
@@ -788,6 +791,59 @@ class ModifiedLlamaForCausalLM(nn.Module):
         if self.core is not None:
             self.core.act_fp8 = dtype == "fp8"
         return prev
+
+    # ---- opt-in deferred weight gradients of the decoder linears (WgradStash) ----
+    _wgrad_stash: Optional[WgradStash] = None
+
+    def defer_weight_grads(self, max_rows: Optional[int] = 2048) -> Optional[int]:
+        """Defer the weight gradients of the decoder linears (q|k|v, o_proj, gate|up, down of every layer) across backwards:
+        each backward records its wgrad operands (references to activations it computed anyway) and
+        ``flush_weight_grads()`` adds them with ONE segmented-contraction GEMM per weight (``ops.gemm_wgrad_seg``).  For
+        small-batch rollouts (one backward of a few hundred rows per step) this replaces a read-modify-write of the whole bf16
+        gradient buffer per backward with one per flush.  A deferred gradient is the same sum as the per-backward one,
+        rounded to bf16 once instead of once per backward.  RMSNorm weights, lm_head, embeddings, the heads and the panorama
+        encoder keep their immediate gradients.
+
+        ``max_rows`` bounds the stash in backward rows: a backward that would exceed it flushes first, and a backward of more
+        than ``max_rows / 2`` rows (which could not share a flush with another of its size) runs its weight gradients at once.  The stash keeps (8 hidden + 3 intermediate) bf16 values per
+        row and layer alive (4.2 MB a row at Vicuna-7B; ``weight_grad_stash_bytes()``).  ``None`` or 0 turns deferral off
+        (flushing first).  Returns the previous setting.
+
+        The flush runs in ``FlatAdamW.step()``, ``NavModel.allreduce_grads()`` and the data-parallel exchange of an armed pass
+        (after the training prefix caches' ``flush_grads()``); anything else that reads the linears' ``.grad`` must call
+        ``flush_weight_grads()`` first.  ``zero_grad()`` while rows are stashed raises, and so does a flush after the weights
+        changed."""
+        prev = None if self._wgrad_stash is None else self._wgrad_stash.max_rows
+        if max_rows is not None and int(max_rows) < 0:
+            raise ValueError(f"defer_weight_grads: max_rows must be >= 0 or None (got {max_rows})")
+        self.flush_weight_grads()
+        self._wgrad_stash = WgradStash(self.core, int(max_rows)) if max_rows else None
+        if self.core is not None:
+            self.core.wgrad_stash = self._wgrad_stash
+        return prev
+
+    def flush_weight_grads(self) -> None:
+        """Add the stashed weight gradients of ``defer_weight_grads`` into ``.grad``; a no-op when nothing is stashed."""
+        if self._wgrad_stash is not None:
+            self._wgrad_stash.flush()
+
+    def weight_grad_stash_bytes(self) -> int:
+        """Device bytes the deferred weight gradients keep alive (0 when nothing is stashed)."""
+        return 0 if self._wgrad_stash is None else self._wgrad_stash.nbytes
+
+    def weight_grads_pending(self) -> bool:
+        return self._wgrad_stash is not None and self._wgrad_stash.pending
+
+    def complete_pending_grads(self) -> None:
+        """Before a gradient exchange: part (b) of the training prefix caches, then the deferred weight gradients."""
+        self.flush_prefix_caches()
+        self.flush_weight_grads()
+
+    def zero_grad(self, set_to_none: bool = True) -> None:
+        if self.weight_grads_pending():
+            raise RuntimeError("zero_grad(): deferred weight gradients are stashed; call flush_weight_grads() before "
+                               "optimizer.step() / zero_grad()")
+        super().zero_grad(set_to_none=set_to_none)
 
     # ---- opt-in fp8 (e4m3) KV cache in generate() ----
     kv_cache_dtype = "bf16"

@@ -208,7 +208,7 @@ class NavModel(nn.Module):
         # data-parallel gradient exchange: ONE state shared with the language model (navillm_b200/parallel.py)
         self.grad_sync = GradSync()
         self.grad_sync.flats = self._sync_flats
-        self.grad_sync.before_exchange = self.lang_model.flush_prefix_caches
+        self.grad_sync.before_exchange = self.lang_model.complete_pending_grads
         self.lang_model.grad_sync = self.grad_sync
         if logger is not None:
             logger.info("model type: {}".format(self.model_type))
@@ -304,8 +304,21 @@ class NavModel(nn.Module):
 
     def allreduce_grads(self, average: bool = True):
         """Explicit exchange for bare use: ONE all-reduce (average) per flat gradient buffer (SURVEY.md §8e).  No-op
-        without an initialised multi-rank process group.  Returns the number of collectives issued."""
+        without an initialised multi-rank process group.  Flushes the deferred weight gradients first.  Returns the number of
+        collectives issued."""
+        self.lang_model.flush_weight_grads()
         return self.grad_sync.exchange()
+
+    def defer_weight_grads(self, max_rows: Optional[int] = 2048) -> Optional[int]:
+        """Defer the language model's decoder-linear weight gradients across backwards (small-batch rollouts); see
+        ``ModifiedLlamaForCausalLM.defer_weight_grads``.  Returns the previous setting."""
+        return self.lang_model.defer_weight_grads(max_rows)
+
+    def flush_weight_grads(self) -> None:
+        self.lang_model.flush_weight_grads()
+
+    def weight_grad_stash_bytes(self) -> int:
+        return self.lang_model.weight_grad_stash_bytes()
 
     def zero_grad(self, set_to_none: bool = False, lazy: bool = False):
         """Gradients live in two flat buffers, so zeroing is two fills instead of one per parameter.  With
@@ -316,6 +329,9 @@ class NavModel(nn.Module):
         if self.lang_model.prefix_grads_pending():
             raise RuntimeError("zero_grad(): a PrefixKVCache(train=True) of this model has pending gradient; call "
                                "cache.flush_grads() before optimizer.step() / zero_grad()")
+        if self.lang_model.weight_grads_pending():
+            raise RuntimeError("zero_grad(): deferred weight gradients are stashed; call flush_weight_grads() before "
+                               "optimizer.step() / zero_grad()")
         if self.lang_model.core is None or self._flat32 is None:
             return super().zero_grad(set_to_none=set_to_none)
         self._ensure()

@@ -62,6 +62,42 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
     return out
 
 
+WGRAD_SEG_MAX = 64          # NV_WGRAD_SEG_MAX of include/navillm_b200.h
+
+
+def gemm_wgrad_seg(segs, out: torch.Tensor, *, addend: torch.Tensor | None = None) -> torch.Tensor:
+    """out[M,N] = bf16(bf16(sum_s a_s^T b_s) (+ addend)) in one launch (nv_gemm_wgrad_seg_bf16): segs is a list of 1 ..
+    WGRAD_SEG_MAX pairs (a_s [rows_s, M], b_s [rows_s, N]) of bf16 CUDA tensors on out's device, rounded to bf16 once.  Bit for bit
+    ``gemm(a, b, a_mn=True, b_mn=True, addend=addend)`` over the row-concatenation of the segments, each zero-padded to a
+    multiple of 64 rows.  ``addend`` may be ``out``."""
+    if not 1 <= len(segs) <= WGRAD_SEG_MAX:
+        raise ValueError(f"gemm_wgrad_seg: {len(segs)} segments (1..{WGRAD_SEG_MAX})")
+    _rowmajor(out, "out")
+    M, N = out.shape
+    assert out.dtype == bf16
+    n = len(segs)
+    A, B = (ctypes.c_void_p * n)(), (ctypes.c_void_p * n)()
+    lda, ldb, rows = (ctypes.c_int64 * n)(), (ctypes.c_int64 * n)(), (ctypes.c_int * n)()
+    for s, (a, b) in enumerate(segs):
+        _rowmajor(a, "a"); _rowmajor(b, "b")
+        if a.device != out.device or b.device != out.device:
+            raise ValueError(f"gemm_wgrad_seg: segment {s} on {a.device} / {b.device}, out on {out.device}")
+        if a.dtype != bf16 or b.dtype != bf16 or a.shape[1] != M or b.shape[1] != N or a.shape[0] != b.shape[0]:
+            raise ValueError(f"gemm_wgrad_seg: segment {s}: a {tuple(a.shape)} {a.dtype}, b {tuple(b.shape)} {b.dtype} for an "
+                             f"output [{M}, {N}] (bf16 [rows, M] and [rows, N] expected)")
+        A[s], B[s] = a.data_ptr(), b.data_ptr()
+        lda[s], ldb[s], rows[s] = a.stride(0), b.stride(0), a.shape[0]
+    if addend is not None:
+        _rowmajor(addend, "addend")
+        if addend.shape != (M, N) or addend.dtype != bf16 or addend.device != out.device:
+            raise ValueError(f"gemm_wgrad_seg: addend bf16 [{M}, {N}] on {out.device} expected (got {addend.dtype} "
+                             f"{tuple(addend.shape)} on {addend.device})")
+    check(_lib.load().nv_gemm_wgrad_seg_bf16(A, lda, B, ldb, rows, i32(n), ptr(out), i64(out.stride(0)), ptr(addend),
+                                             i64(addend.stride(0) if addend is not None else 0), i32(M), i32(N), stream_ptr()),
+          "nv_gemm_wgrad_seg_bf16")
+    return out
+
+
 def _qblocks(seqlens) -> int:
     return int(sum((int(l) + 127) // 128 for l in seqlens))
 

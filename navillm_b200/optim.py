@@ -36,6 +36,7 @@ class FlatAdamW:
     @torch.no_grad()
     def step(self, max_grad_norm: float | None = None, write_clipped_grad: bool = False):
         lib = _lib.load()
+        self.model.flush_weight_grads()              # deferred weight gradients (defer_weight_grads) enter .grad first
         self.model._settle_lazy_zero()               # a lazy zero_grad with no backward since: gradients are zero, not stale
         self.step_count += 1
         lr = self.param_groups[0]["lr"]
