@@ -268,6 +268,32 @@ int nv_kv_store_prefill_fp8(const void* qkv, int64_t ld, const int* cu_seqlens, 
 int nv_decode_attn_rope_fp8(const void* qkv, int64_t ld, const int* lens, const void* cos_t, const void* sin_t, void* kq, void* vq,
                             void* kexp, void* vexp, void* out, int64_t ldo, int B, int Smax, int H, int head_dim, float scale,
                             void* stream);
+/* Beam search (HF beam_search / BeamSearchScorer of transformers 4.28, the version the reference pins), K = 1..8 beams per
+ * prompt, R = B * K beam rows, all state on the device so a whole step can be captured.
+ * nv_beam_topk: one CTA per prompt b.  Beam k's scores are bf16(log_softmax(logits[b * ld_prompt + k * ld_beam, :])) (special
+ * ids -inf, fp32 result rounded once to bf16) + beam_score[b * K + k] in fp32; the 2K best of the K * V scores by (score desc,
+ * flat index k * V + c asc) are written in that order to cand_score / cand_tok / cand_parent [B, 2K] (parent = k).
+ * nv_beam_select: one CTA per prompt, BeamSearchScorer.process over those candidates (EOS of rank < K -> hypothesis with
+ * score sum_logprobs / norm[t] in fp64, norm[t] = (S + t) ** length_penalty for S padded prompt columns and t generated tokens;
+ * EOS of rank >= K skipped, the others -> the K running beams; the done rule of BeamHypotheses.is_done), then gathers hist / src [R, G] (generated tokens, KV source rows) by parent and writes
+ * next_ids / lens / beam_score [R] and src[r, t] = r.  hyp_score fp64 [B, K + 1] (K kept scores, worst kept score; start
+ * 1e9), hyp_meta [B, K, 2] (generated length, insertion number), hyp_tok [B, K, G], prompt_state [B, 5] (tokens generated t,
+ * prompt length, hypotheses kept, next insertion number, done).  A done prompt's beams emit pad_id with score 0.
+ * nv_decode_attn_rope_beam[_fp8]: nv_decode_attn_rope[_fp8] for beam rows r: keys [0, plens[r / K]) from the prompt cache
+ * pk / pv [B, Sp, H*128] the beams of a prompt share, generated key i from row (src[r, i], i) of kgen / vgen [R, G, H*128];
+ * the new k / v go to (r, lens[r] - plens[r / K]).  Same keys in the same order as the contiguous kernel: same bits. */
+int nv_beam_topk(const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, const int* special, int n_special,
+                 const float* beam_score, float* cand_score, int* cand_tok, int* cand_parent, int B, int K, void* stream);
+int nv_beam_select(const float* cand_score, const int* cand_tok, const int* cand_parent, float* beam_score, int* hist, int* src,
+                   double* hyp_score, int* hyp_meta, int* hyp_tok, int* prompt_state, int* next_ids, int* lens, const double* norm,
+                   int B, int K, int G, int eos_id, int pad_id, int early_stopping, void* stream);
+int nv_decode_attn_rope_beam(const void* qkv, int64_t ld, const int* lens, const void* cos_t, const void* sin_t, const void* pk,
+                             const void* pv, int Sp, const int* plens, void* kgen, void* vgen, const int* src, int G, void* out,
+                             int64_t ldo, int R, int K, int H, int head_dim, float scale, void* stream);
+int nv_decode_attn_rope_beam_fp8(const void* qkv, int64_t ld, const int* lens, const void* cos_t, const void* sin_t, const void* pkq,
+                                 const void* pvq, const void* pkexp, const void* pvexp, int Sp, const int* plens, void* kq, void* vq,
+                                 void* kexp, void* vexp, const int* src, int G, void* out, int64_t ldo, int R, int K, int H,
+                                 int head_dim, float scale, void* stream);
 /* at most 64 special ids (n_special), here and in nv_sample_topk; longer lists return NV_ERR_BAD_ARG */
 int nv_argmax_masked(const void* logits, int64_t ld, int V, const int* special, int n_special, int* finished, int eos_id,
                      int pad_id, int stop_on_eos, int* next, int B, void* stream);

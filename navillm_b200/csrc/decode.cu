@@ -172,14 +172,31 @@ constexpr int DA_WARPS = 8;
 template <bool FP8>
 using kv_elem_t = typename std::conditional<FP8, uint8_t, __nv_bfloat16>::type;
 
-template <bool ROPE, bool FP8 = false>
+// BEAM = true (beam search): blockIdx.x / H is a beam row r of prompt r / nbeam.  Keys [0, plens[prompt]) come from the
+// prompt cache pk / pv ([B, Sp, HD], exponents pke / pve [B, Sp, H]) that all beams of the prompt share; generated key i (key
+// plens + i) from row (src[r, i], i) of the generated cache kc / vc ([B * nbeam, Smax, HD]).  The new token is generated key
+// lens[r] - plens: it is written at (r, that index), and src[r, that index] must name r.  Only the addresses differ from the
+// contiguous kernel: the same keys in the same order give the same bits.
+template <bool FP8>
+struct BeamKV {
+  const kv_elem_t<FP8>* pk;
+  const kv_elem_t<FP8>* pv;
+  const int8_t* pke;
+  const int8_t* pve;
+  const int* src;
+  const int* plens;
+  int nbeam;
+  int Sp;
+};
+
+template <bool ROPE, bool FP8 = false, bool BEAM = false>
 __global__ void __launch_bounds__(DA_WARPS * 32) decode_attn_kernel(const __nv_bfloat16* __restrict__ q, int64_t ldq,
                                                           kv_elem_t<FP8>* __restrict__ kc, kv_elem_t<FP8>* __restrict__ vc,
                                                           const int* __restrict__ lens, __nv_bfloat16* __restrict__ out,
                                                           int64_t ldo, int Smax, int H, float scale,
                                                           const __nv_bfloat16* __restrict__ cos_t,
                                                           const __nv_bfloat16* __restrict__ sin_t,
-                                                          int8_t* __restrict__ ke, int8_t* __restrict__ ve) {
+                                                          int8_t* __restrict__ ke, int8_t* __restrict__ ve, BeamKV<FP8> bk) {
   __shared__ float s_m[DA_WARPS], s_l[DA_WARPS];
   __shared__ float s_acc[DA_WARPS][128];
   __shared__ uint4 s_q[16];                            // rotated q of this head (bf16 x 128)
@@ -190,8 +207,14 @@ __global__ void __launch_bounds__(DA_WARPS * 32) decode_attn_kernel(const __nv_b
   const int half = lane >> 4, hl = lane & 15;          // half-warp id, lane within the half (8 dims each)
   const int n = lens[b] + 1;                            // keys visible to the new token
   const int HD = H * 128;
+  int P = 0, bp = 0;                                    // BEAM: prompt keys of this row, and its prompt
+  if constexpr (BEAM) {
+    bp = b / bk.nbeam;
+    P = bk.plens[bp];
+  }
   if (ROPE) {
     const int p = n - 1;
+    const int pw = p - P;                               // cache row of the new k / v
     if (w == 0) {
       uint4 r0 = make_uint4(0, 0, 0, 0), r1 = r0;       // FP8: this lane's chunks of the new k row (lanes 8..15) or v row (16..31)
       if (lane < 16) {                                  // lanes 0..7: q chunk c, lanes 8..15: k chunk c
@@ -219,16 +242,16 @@ __global__ void __launch_bounds__(DA_WARPS * 32) decode_attn_kernel(const __nv_b
           s_q[c] = o1; s_q[8 + c] = o2;
         } else if constexpr (FP8) {
           r0 = o1; r1 = o2;
-        } else if (p < Smax) {
-          __nv_bfloat16* dst = kc + ((int64_t)b * Smax + p) * HD + h * 128;
+        } else if (pw < Smax) {
+          __nv_bfloat16* dst = kc + ((int64_t)b * Smax + pw) * HD + h * 128;
           *reinterpret_cast<uint4*>(dst + c * 8) = o1;
           *reinterpret_cast<uint4*>(dst + 64 + c * 8) = o2;
         }
       } else if constexpr (FP8) {
         r0 = *reinterpret_cast<const uint4*>(q + (int64_t)b * ldq + 2 * HD + h * 128 + (lane - 16) * 8);
-      } else if (p < Smax) {                            // lanes 16..31: this head's v (16 x 16 bytes)
+      } else if (pw < Smax) {                           // lanes 16..31: this head's v (16 x 16 bytes)
         const int v = lane - 16;
-        *reinterpret_cast<uint4*>(vc + ((int64_t)b * Smax + p) * HD + h * 128 + v * 8) =
+        *reinterpret_cast<uint4*>(vc + ((int64_t)b * Smax + pw) * HD + h * 128 + v * 8) =
             *reinterpret_cast<const uint4*>(q + (int64_t)b * ldq + 2 * HD + h * 128 + v * 8);
       }
       if constexpr (FP8) {
@@ -241,8 +264,8 @@ __global__ void __launch_bounds__(DA_WARPS * 32) decode_attn_kernel(const __nv_b
         if (lane >= 16) m = max(m, m8);
         const int e = fp8_row_exponent(__uint_as_float(m << 16));
         const float inv = fp8_pow2(-e);
-        if (lane >= 8 && p < Smax) {
-          const int64_t row = (int64_t)b * Smax + p;
+        if (lane >= 8 && pw < Smax) {
+          const int64_t row = (int64_t)b * Smax + pw;
           if (lane < 16) {
             uint8_t* dst = kc + row * HD + h * 128 + (lane & 7) * 8;
             *reinterpret_cast<uint2*>(dst) = fp8x8_from_bf16x8(r0, inv);
@@ -271,13 +294,26 @@ __global__ void __launch_bounds__(DA_WARPS * 32) decode_attn_kernel(const __nv_b
 #pragma unroll
     for (int u = 0; u < KPI; ++u) {
       if (jb + u < n) {
-        const int64_t off = ((int64_t)b * Smax + jb + u) * HD + h * 128 + hl * 8;
-        kr[u] = *reinterpret_cast<const raw_t*>(kc + off);
-        vr[u] = *reinterpret_cast<const raw_t*>(vc + off);
+        const kv_elem_t<FP8>* kb = kc;
+        const kv_elem_t<FP8>* vb = vc;
+        const int8_t* keb = ke;
+        const int8_t* veb = ve;
+        int64_t row = (int64_t)b * Smax + jb + u;
+        if constexpr (BEAM) {
+          const int j = jb + u;
+          if (j < P) {
+            row = (int64_t)bp * bk.Sp + j;
+            kb = bk.pk; vb = bk.pv; keb = bk.pke; veb = bk.pve;
+          } else {
+            row = (int64_t)bk.src[(int64_t)b * Smax + (j - P)] * Smax + (j - P);
+          }
+        }
+        const int64_t off = row * HD + h * 128 + hl * 8;
+        kr[u] = *reinterpret_cast<const raw_t*>(kb + off);
+        vr[u] = *reinterpret_cast<const raw_t*>(vb + off);
         if constexpr (FP8) {
-          const int64_t row = ((int64_t)b * Smax + jb + u) * H + h;
-          kx[u] = ke[row];
-          vx[u] = ve[row];
+          kx[u] = keb[row * H + h];
+          vx[u] = veb[row * H + h];
         }
       } else {
         if constexpr (FP8) {
@@ -693,6 +729,248 @@ __global__ void __launch_bounds__(SMP_THREADS) sample_topk_kernel(const __nv_bfl
   }
 }
 
+// ---- beam search (HF GenerationMixin.beam_search / BeamSearchScorer of transformers 4.28, the version the reference pins) ----
+constexpr int BEAM_MAX = 8;                  // beams per prompt
+constexpr int BT_THREADS = 512;
+constexpr int BT_LIST = 2 * BEAM_MAX;        // candidates kept per thread: the 2K best overall are among each thread's 2K best
+
+__device__ __forceinline__ uint32_t f32_order(float v) {          // monotone: larger float -> larger key; -inf lowest
+  const uint32_t u = __float_as_uint(v);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+__device__ __forceinline__ float f32_unorder(uint32_t k) {
+  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+
+// One CTA per prompt b.  Beam k's next-token scores are bf16(log_softmax(logits row (b, k))) + beam_score[b, k]: special ids
+// -inf, the row max and sum in fp32 / fp64, each log-prob rounded once to bf16, then the fp32 add of HF.  The 2K best of the
+// K * V scores by (score desc, flat index k * V + c asc) go to cand_* [B, 2K] in that order.  A score and its flat index
+// make one 64-bit key, so every comparison is one integer compare and equal scores order by index.
+__global__ void __launch_bounds__(BT_THREADS) beam_topk_kernel(const __nv_bfloat16* __restrict__ logits, int64_t ld_prompt,
+                                                               int64_t ld_beam, int V, const int* __restrict__ special,
+                                                               int n_special, const float* __restrict__ beam_score, int K,
+                                                               float* __restrict__ cand_score, int* __restrict__ cand_tok,
+                                                               int* __restrict__ cand_par) {
+  __shared__ int s_special[MAX_SPECIAL];
+  __shared__ float s_m[BEAM_MAX], s_ls[BEAM_MAX], s_bs[BEAM_MAX];
+  __shared__ float redf[32];
+  __shared__ double redd[32];
+  __shared__ unsigned long long redk[32];
+  griddep_launch();
+  griddep_wait();
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  constexpr int NW = BT_THREADS / 32;
+  const int ns = n_special;
+  if (tid < ns) s_special[tid] = special[tid];
+  if (tid < K) s_bs[tid] = beam_score[b * K + tid];
+  __syncthreads();
+  auto is_special = [&](int c) {
+    bool sp = false;
+    for (int s = 0; s < ns; ++s) sp |= (s_special[s] == c);
+    return sp;
+  };
+  for (int k = 0; k < K; ++k) {
+    const __nv_bfloat16* row = logits + (int64_t)b * ld_prompt + (int64_t)k * ld_beam;
+    float mx = -INFINITY;
+    for (int c = tid; c < V; c += BT_THREADS)
+      if (!is_special(c)) mx = fmaxf(mx, __bfloat162float(row[c]));
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    if (lane == 0) redf[w] = mx;
+    __syncthreads();
+    mx = lane < NW ? redf[lane] : -INFINITY;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    double s = 0.0;                                              // fp64: the fp32 sum of torch up to its own rounding
+    for (int c = tid; c < V; c += BT_THREADS)
+      if (!is_special(c)) s += exp((double)(__bfloat162float(row[c]) - mx));
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0) redd[w] = s;
+    __syncthreads();
+    s = lane < NW ? redd[lane] : 0.0;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (tid == 0) {
+      s_m[k] = mx;
+      s_ls[k] = (float)log(s);
+    }
+    __syncthreads();
+  }
+  unsigned long long L[BT_LIST];                                 // this thread's best keys, descending; 0 = empty
+#pragma unroll
+  for (int i = 0; i < BT_LIST; ++i) L[i] = 0ull;
+  for (int k = 0; k < K; ++k) {
+    const __nv_bfloat16* row = logits + (int64_t)b * ld_prompt + (int64_t)k * ld_beam;
+    const float m = s_m[k], ls = s_ls[k], bs = s_bs[k];
+    for (int c = tid; c < V; c += BT_THREADS) {
+      float sc = -INFINITY;
+      if (!is_special(c)) sc = bf16_round((__bfloat162float(row[c]) - m) - ls) + bs;
+      if (sc != sc) sc = -INFINITY;
+      const unsigned long long key =
+          ((unsigned long long)f32_order(sc) << 32) | (unsigned long long)(0xffffffffu - (uint32_t)(k * V + c));
+      if (key > L[BT_LIST - 1]) {
+        L[BT_LIST - 1] = key;
+#pragma unroll
+        for (int i = BT_LIST - 1; i > 0; --i)
+          if (L[i] > L[i - 1]) {
+            const unsigned long long t = L[i]; L[i] = L[i - 1]; L[i - 1] = t;
+          }
+      }
+    }
+  }
+  // 2K rounds: the CTA-wide largest head wins and its owner pops it
+  for (int r = 0; r < 2 * K; ++r) {
+    unsigned long long best = L[0];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const unsigned long long x = __shfl_xor_sync(0xffffffffu, best, o);
+      best = x > best ? x : best;
+    }
+    if (lane == 0) redk[w] = best;
+    __syncthreads();
+    best = lane < NW ? redk[lane] : 0ull;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const unsigned long long x = __shfl_xor_sync(0xffffffffu, best, o);
+      best = x > best ? x : best;
+    }
+    if (L[0] == best) {
+#pragma unroll
+      for (int i = 0; i < BT_LIST - 1; ++i) L[i] = L[i + 1];
+      L[BT_LIST - 1] = 0ull;
+    }
+    if (tid == 0) {
+      const uint32_t flat = 0xffffffffu - (uint32_t)(best & 0xffffffffull);
+      cand_score[b * 2 * K + r] = f32_unorder((uint32_t)(best >> 32));
+      cand_tok[b * 2 * K + r] = (int)(flat % (uint32_t)V);
+      cand_par[b * 2 * K + r] = (int)(flat / (uint32_t)V);
+    }
+    __syncthreads();                                             // redk is reused by the next round
+  }
+}
+
+// prompt_state [B, BS_FIELDS] of nv_beam_select
+constexpr int BS_STEP = 0, BS_PLEN = 1, BS_COUNT = 2, BS_SEQ = 3, BS_DONE = 4, BS_FIELDS = 5;
+constexpr int BS_THREADS = 128, BS_CHUNK = 256;
+
+// One CTA per prompt: BeamSearchScorer.process + BeamHypotheses.add / is_done of transformers 4.28 over the 2K candidates of
+// nv_beam_topk, then the reorder of the running beams (input_ids[beam_idx] and _reorder_cache) as gathers of the generated-
+// token history and of the KV source table by parent.  t = prompt_state[b, BS_STEP] tokens have been generated; norm[t] is
+// (S + t) ** length_penalty as the host's Python floats compute it (S padded prompt columns: hyp.shape[-1] in 4.28), so the fp64
+// hypothesis scores sum_logprobs / norm[t] are 4.28's to the bit.  hyp_score [B, K + 1] holds the K kept scores and the worst kept score, hyp_meta [B, K, 2] (generated
+// length, insertion number: the later of equal scores wins in finalize), hyp_tok [B, K, G] their generated tokens.
+__global__ void __launch_bounds__(BS_THREADS) beam_select_kernel(const float* __restrict__ cand_score, const int* __restrict__ cand_tok,
+                                                                 const int* __restrict__ cand_par, float* __restrict__ beam_score,
+                                                                 int* __restrict__ hist, int* __restrict__ src,
+                                                                 double* __restrict__ hyp_score, int* __restrict__ hyp_meta,
+                                                                 int* __restrict__ hyp_tok, int* __restrict__ pstate,
+                                                                 int* __restrict__ next_ids, int* __restrict__ lens,
+                                                                 const double* __restrict__ norm, int K, int G, int eos_id, int pad_id,
+                                                                 int early_stopping) {
+  __shared__ int s_tok[BEAM_MAX], s_par[BEAM_MAX];
+  __shared__ float s_sc[BEAM_MAX];
+  __shared__ int s_op_slot[BEAM_MAX], s_op_par[BEAM_MAX], s_nops;
+  __shared__ int s_h[BEAM_MAX][BS_CHUNK], s_s[BEAM_MAX][BS_CHUNK];
+  griddep_launch();
+  griddep_wait();
+  const int b = blockIdx.x, tid = threadIdx.x;
+  int* ps = pstate + b * BS_FIELDS;
+  const int t = ps[BS_STEP];
+  if (t >= G) return;                                            // the host sizes G to the call's max_new_tokens
+  if (tid == 0) {
+    int nops = 0;
+    if (ps[BS_DONE]) {                                           // a done prompt's beams emit pad with score 0
+      for (int j = 0; j < K; ++j) { s_tok[j] = pad_id; s_par[j] = j; s_sc[j] = 0.f; }
+    } else {
+      double* hs = hyp_score + b * (K + 1);
+      int* hm = hyp_meta + b * K * 2;
+      double worst = hs[K];
+      int cnt = ps[BS_COUNT], seq = ps[BS_SEQ];
+      const double nt = norm[t];
+      int j = 0;
+      for (int rank = 0; rank < 2 * K; ++rank) {
+        const int tok = cand_tok[b * 2 * K + rank], par = cand_par[b * 2 * K + rank];
+        const float sc = cand_score[b * 2 * K + rank];
+        if (tok == eos_id) {
+          if (rank >= K) continue;                               // EOS below the top K is not a hypothesis
+          const double score = (double)sc / nt;
+          if (cnt < K || score > worst) {
+            int slot;
+            if (cnt < K) {
+              slot = cnt++;
+              worst = fmin(score, worst);
+            } else {                                             // drop the lowest (score, insertion) and take its slot
+              slot = 0;
+              for (int i = 1; i < K; ++i)
+                if (hs[i] < hs[slot] || (hs[i] == hs[slot] && hm[2 * i + 1] < hm[2 * slot + 1])) slot = i;
+            }
+            hs[slot] = score;
+            hm[2 * slot] = t;
+            hm[2 * slot + 1] = seq++;
+            if (cnt == K) {
+              worst = hs[0];
+              for (int i = 1; i < K; ++i) worst = fmin(worst, hs[i]);
+            }
+            s_op_slot[nops] = slot;
+            s_op_par[nops] = par;
+            ++nops;
+          }
+        } else {
+          s_tok[j] = tok; s_par[j] = par; s_sc[j] = sc;
+          ++j;
+        }
+        if (j == K) break;
+      }
+      int done = 0;
+      if (cnt >= K) done = early_stopping ? 1 : (worst >= (double)cand_score[b * 2 * K] / nt);
+      hs[K] = worst;
+      ps[BS_COUNT] = cnt;
+      ps[BS_SEQ] = seq;
+      ps[BS_DONE] = done;
+    }
+    s_nops = nops;
+  }
+  __syncthreads();
+  for (int o = 0; o < s_nops; ++o) {                             // in order: a later hypothesis may take an earlier one's slot
+    const int* from = hist + (int64_t)(b * K + s_op_par[o]) * G;
+    int* to = hyp_tok + (int64_t)(b * K + s_op_slot[o]) * G;
+    for (int i = tid; i < t; i += BS_THREADS) to[i] = from[i];
+  }
+  for (int c0 = 0; c0 < t; c0 += BS_CHUNK) {                     // rows of the new beams = rows of their parents
+    const int n = min(BS_CHUNK, t - c0);
+    for (int idx = tid; idx < K * BS_CHUNK; idx += BS_THREADS) {
+      const int j = idx / BS_CHUNK, i = idx % BS_CHUNK;
+      if (i < n) {
+        const int64_t from = (int64_t)(b * K + s_par[j]) * G + c0 + i;
+        s_h[j][i] = hist[from];
+        s_s[j][i] = src[from];
+      }
+    }
+    __syncthreads();
+    for (int idx = tid; idx < K * BS_CHUNK; idx += BS_THREADS) {
+      const int j = idx / BS_CHUNK, i = idx % BS_CHUNK;
+      if (i < n) {
+        const int64_t to = (int64_t)(b * K + j) * G + c0 + i;
+        hist[to] = s_h[j][i];
+        src[to] = s_s[j][i];
+      }
+    }
+    __syncthreads();
+  }
+  if (tid < K) {
+    const int r = b * K + tid;
+    hist[(int64_t)r * G + t] = s_tok[tid];
+    src[(int64_t)r * G + t] = r;                                 // the next step writes generated key t of row r at (r, t)
+    next_ids[r] = s_tok[tid];
+    lens[r] = ps[BS_PLEN] + t;
+    beam_score[r] = s_sc[tid];
+  }
+  __syncthreads();
+  if (tid == 0) ps[BS_STEP] = t + 1;
+}
+
 }  // namespace nv
 
 using namespace nv;
@@ -753,7 +1031,8 @@ int nv_decode_attn(const void* q, int64_t ldq, const void* kcache, const void* v
   if (B == 0) return NV_OK;
   NV_CUDA(launch_pdl(decode_attn_kernel<false>, dim3(B * H), dim3(DA_WARPS * 32), 0, S_(stream), CBF(q), ldq,
                      const_cast<__nv_bfloat16*>(CBF(kcache)), const_cast<__nv_bfloat16*>(CBF(vcache)), lens, BF(out), ldo, Smax, H, scale,
-                     (const __nv_bfloat16*)nullptr, (const __nv_bfloat16*)nullptr, (int8_t*)nullptr, (int8_t*)nullptr));
+                     (const __nv_bfloat16*)nullptr, (const __nv_bfloat16*)nullptr, (int8_t*)nullptr, (int8_t*)nullptr,
+                     BeamKV<false>{}));
   return NV_OK;
 }
 
@@ -765,7 +1044,7 @@ int nv_decode_attn_rope(const void* qkv, int64_t ld, const int* lens, const void
   NV_REQUIRE(head_dim == 128 && (ld & 7) == 0, "nv_decode_attn_rope: head_dim must be 128, ld %% 8 == 0");
   if (B == 0) return NV_OK;
   NV_CUDA(launch_pdl(decode_attn_kernel<true>, dim3(B * H), dim3(DA_WARPS * 32), 0, S_(stream), CBF(qkv), ld, BF(kcache), BF(vcache), lens,
-                     BF(out), ldo, Smax, H, scale, CBF(cos_t), CBF(sin_t), (int8_t*)nullptr, (int8_t*)nullptr));
+                     BF(out), ldo, Smax, H, scale, CBF(cos_t), CBF(sin_t), (int8_t*)nullptr, (int8_t*)nullptr, BeamKV<false>{}));
   return NV_OK;
 }
 
@@ -820,7 +1099,7 @@ int nv_decode_attn_rope_fp8(const void* qkv, int64_t ld, const int* lens, const 
              "nv_decode_attn_rope_fp8: alignment (16-byte qkv, 8-byte caches)");
   NV_CUDA(launch_pdl(decode_attn_kernel<true, true>, dim3(B * H), dim3(DA_WARPS * 32), 0, S_(stream), CBF(qkv), ld,
                      reinterpret_cast<uint8_t*>(kq), reinterpret_cast<uint8_t*>(vq), lens, BF(out), ldo, Smax, H, scale, CBF(cos_t),
-                     CBF(sin_t), reinterpret_cast<int8_t*>(kexp), reinterpret_cast<int8_t*>(vexp)));
+                     CBF(sin_t), reinterpret_cast<int8_t*>(kexp), reinterpret_cast<int8_t*>(vexp), BeamKV<true>{}));
   return NV_OK;
 }
 
@@ -869,6 +1148,71 @@ int nv_trie_mask(const void* logits, int64_t ld, void* out, int64_t ldo, int V, 
   if (B == 0) return NV_OK;
   NV_CUDA(launch_pdl(trie_mask_kernel, dim3(B), dim3(TM_THREADS), 0, S_(stream), CBF(logits), ld, BF(out), ldo, V, node_ptr,
                      child_tok, child_node, n_nodes, leaf_tok, special, n_special, state, last, miss));
+  return NV_OK;
+}
+
+// Beam search (see beam_topk_kernel / beam_select_kernel).  Beam k of prompt b reads logits row b * ld_prompt + k * ld_beam
+// (ld_beam = 0 at the first step, whose K beams all read the prompt's prefill row).
+int nv_beam_topk(const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, const int* special, int n_special,
+                 const float* beam_score, float* cand_score, int* cand_tok, int* cand_parent, int B, int K, void* stream) {
+  NV_REQUIRE(logits && beam_score && cand_score && cand_tok && cand_parent && V > 0 && B >= 0,
+             "nv_beam_topk: bad arguments (V=%d B=%d)", V, B);
+  NV_REQUIRE(K >= 1 && K <= BEAM_MAX && 2 * K <= V, "nv_beam_topk: %d beams: 1..%d beams and V >= 2K supported", K, BEAM_MAX);
+  NV_REQUIRE((int64_t)K * V < 0xffffffffll, "nv_beam_topk: K * V = %lld does not fit the 32-bit candidate index", (long long)K * V);
+  NV_REQUIRE(n_special >= 0 && n_special <= MAX_SPECIAL && (n_special == 0 || special),
+             "nv_beam_topk: n_special=%d out of range (max %d)", n_special, MAX_SPECIAL);
+  if (B == 0) return NV_OK;
+  NV_CUDA(launch_pdl(beam_topk_kernel, dim3(B), dim3(BT_THREADS), 0, S_(stream), CBF(logits), ld_prompt, ld_beam, V, special,
+                     n_special, beam_score, K, cand_score, cand_tok, cand_parent));
+  return NV_OK;
+}
+
+int nv_beam_select(const float* cand_score, const int* cand_tok, const int* cand_parent, float* beam_score, int* hist, int* src,
+                   double* hyp_score, int* hyp_meta, int* hyp_tok, int* prompt_state, int* next_ids, int* lens, const double* norm,
+                   int B, int K, int G, int eos_id, int pad_id, int early_stopping, void* stream) {
+  NV_REQUIRE(cand_score && cand_tok && cand_parent && beam_score && hist && src && hyp_score && hyp_meta && hyp_tok &&
+             prompt_state && next_ids && lens && norm, "nv_beam_select: null argument");
+  NV_REQUIRE(K >= 1 && K <= BEAM_MAX && G > 0 && B >= 0, "nv_beam_select: bad sizes (B=%d K=%d G=%d)", B, K, G);
+  if (B == 0) return NV_OK;
+  NV_CUDA(launch_pdl(beam_select_kernel, dim3(B), dim3(BS_THREADS), 0, S_(stream), cand_score, cand_tok, cand_parent, beam_score,
+                     hist, src, hyp_score, hyp_meta, hyp_tok, prompt_state, next_ids, lens, norm, K, G, eos_id, pad_id,
+                     early_stopping));
+  return NV_OK;
+}
+
+// nv_decode_attn_rope for R = B * K beam rows over a prompt cache shared by the K beams of a prompt and a generated cache
+// addressed through src (see BeamKV).
+int nv_decode_attn_rope_beam(const void* qkv, int64_t ld, const int* lens, const void* cos_t, const void* sin_t, const void* pk,
+                             const void* pv, int Sp, const int* plens, void* kgen, void* vgen, const int* src, int G, void* out,
+                             int64_t ldo, int R, int K, int H, int head_dim, float scale, void* stream) {
+  NV_REQUIRE(head_dim == 128 && (ld & 7) == 0, "nv_decode_attn_rope_beam: head_dim must be 128, ld %% 8 == 0");
+  NV_REQUIRE(R >= 0 && K >= 1 && R % K == 0 && Sp > 0 && G > 0 && H > 0, "nv_decode_attn_rope_beam: bad sizes (R=%d K=%d Sp=%d G=%d H=%d)",
+             R, K, Sp, G, H);
+  if (R == 0) return NV_OK;
+  NV_REQUIRE(qkv && lens && cos_t && sin_t && pk && pv && plens && kgen && vgen && src && out, "nv_decode_attn_rope_beam: null argument");
+  const BeamKV<false> bk{CBF(pk), CBF(pv), nullptr, nullptr, src, plens, K, Sp};
+  NV_CUDA(launch_pdl(decode_attn_kernel<true, false, true>, dim3(R * H), dim3(DA_WARPS * 32), 0, S_(stream), CBF(qkv), ld, BF(kgen),
+                     BF(vgen), lens, BF(out), ldo, G, H, scale, CBF(cos_t), CBF(sin_t), (int8_t*)nullptr, (int8_t*)nullptr, bk));
+  return NV_OK;
+}
+
+int nv_decode_attn_rope_beam_fp8(const void* qkv, int64_t ld, const int* lens, const void* cos_t, const void* sin_t, const void* pkq,
+                                 const void* pvq, const void* pkexp, const void* pvexp, int Sp, const int* plens, void* kq, void* vq,
+                                 void* kexp, void* vexp, const int* src, int G, void* out, int64_t ldo, int R, int K, int H,
+                                 int head_dim, float scale, void* stream) {
+  NV_REQUIRE(head_dim == 128 && (ld & 7) == 0, "nv_decode_attn_rope_beam_fp8: head_dim must be 128, ld %% 8 == 0");
+  NV_REQUIRE(R >= 0 && K >= 1 && R % K == 0 && Sp > 0 && G > 0 && H > 0,
+             "nv_decode_attn_rope_beam_fp8: bad sizes (R=%d K=%d Sp=%d G=%d H=%d)", R, K, Sp, G, H);
+  if (R == 0) return NV_OK;
+  NV_REQUIRE(qkv && lens && cos_t && sin_t && pkq && pvq && pkexp && pvexp && plens && kq && vq && kexp && vexp && src && out,
+             "nv_decode_attn_rope_beam_fp8: null argument");
+  NV_REQUIRE(((uintptr_t)qkv & 15) == 0 && ((uintptr_t)kq & 7) == 0 && ((uintptr_t)vq & 7) == 0 && ((uintptr_t)pkq & 7) == 0 &&
+             ((uintptr_t)pvq & 7) == 0, "nv_decode_attn_rope_beam_fp8: alignment (16-byte qkv, 8-byte caches)");
+  const BeamKV<true> bk{reinterpret_cast<const uint8_t*>(pkq), reinterpret_cast<const uint8_t*>(pvq),
+                        reinterpret_cast<const int8_t*>(pkexp), reinterpret_cast<const int8_t*>(pvexp), src, plens, K, Sp};
+  NV_CUDA(launch_pdl(decode_attn_kernel<true, true, true>, dim3(R * H), dim3(DA_WARPS * 32), 0, S_(stream), CBF(qkv), ld,
+                     reinterpret_cast<uint8_t*>(kq), reinterpret_cast<uint8_t*>(vq), lens, BF(out), ldo, G, H, scale, CBF(cos_t),
+                     CBF(sin_t), reinterpret_cast<int8_t*>(kexp), reinterpret_cast<int8_t*>(vexp), bk));
   return NV_OK;
 }
 

@@ -809,12 +809,16 @@ class LlamaCore:
 
 
     # -------------------------------------------------------------------------------------------------
-    def decode_step(self, x: torch.Tensor, lens: torch.Tensor, kc: List[torch.Tensor], vc: List[torch.Tensor]) -> torch.Tensor:
+    def decode_step(self, x: torch.Tensor, lens: torch.Tensor, kc: List[torch.Tensor], vc: List[torch.Tensor], beam=None) -> torch.Tensor:
         """One new token per sequence.  x: [B, D] bf16 embeddings of the new tokens; lens: int32 [B] (device) =
         number of cached tokens = position of the new token; caches [B, Smax, D] bf16 per layer, or fp8 ``(e4m3, exponents)``
         pairs per layer (``is_fp8_kv``; the new rows are rounded as they are appended).  Static shapes and
         device-resident lengths: the whole step can be captured in a CUDA graph.  Returns the residual stream
-        [B, D] before the final RMSNorm."""
+        [B, D] before the final RMSNorm.
+
+        ``beam`` (beam search): the B rows are beams, ``beam.K`` per prompt; kc / vc hold only the generated keys [B, G, D]
+        (addressed through ``beam.src``) and ``beam.pk`` / ``beam.pv`` the per-layer prompt caches [B / K, Sp, D] with
+        ``beam.plens`` keys per prompt (``ops.decode_attn_rope_beam``)."""
         d = self.d
         H, D = d.n_heads, d.hidden
         # The step is HBM-bound weight streaming.  Batches <= 16 use the swap-AB cluster-split-K kernel with the SwiGLU fused
@@ -840,12 +844,18 @@ class LlamaCore:
             else:
                 lin = lambda a, w, addend=None: ops.gemm(a, w, addend=addend, block_n=bn)
         fp8_kv = is_fp8_kv(kc)
-        if fp8_kv and d.head_dim != 128:
-            raise NotImplementedError("the fp8 KV cache is built for head_dim = 128")
+        if (fp8_kv or beam is not None) and d.head_dim != 128:
+            raise NotImplementedError("the fp8 KV cache and beam search are built for head_dim = 128")
         for l, lyr in enumerate(self.model.layers):
             xn, _ = ops.rmsnorm_fwd(x, lyr.input_layernorm.weight.data, d.rms_eps)
             qkv = lin(xn, wqkv[l])
-            if fp8_kv:                                                                   # same, quantizing the appended rows
+            if beam is not None and fp8_kv:
+                ao = ops.decode_attn_rope_beam_fp8(qkv, lens, self.cos, self.sin, beam.pk[l][0], beam.pv[l][0], beam.pk[l][1],
+                                                   beam.pv[l][1], beam.plens, kc[l][0], vc[l][0], kc[l][1], vc[l][1], beam.src, beam.K, H)
+            elif beam is not None:
+                ao = ops.decode_attn_rope_beam(qkv, lens, self.cos, self.sin, beam.pk[l], beam.pv[l], beam.plens, kc[l], vc[l],
+                                               beam.src, beam.K, H)
+            elif fp8_kv:                                                                 # same, quantizing the appended rows
                 ao = ops.decode_attn_rope_fp8(qkv, lens, self.cos, self.sin, kc[l][0], vc[l][0], kc[l][1], vc[l][1], H)
             elif d.head_dim == 128:
                 ao = ops.decode_attn_rope(qkv, lens, self.cos, self.sin, kc[l], vc[l], H)   # RoPE + cache append + attention

@@ -901,6 +901,22 @@ class ModifiedLlamaForCausalLM(nn.Module):
                 states.popitem(last=False)
         return st
 
+    def _decode_head(self, h_rows: torch.Tensor, out: torch.Tensor) -> None:
+        """Final RMSNorm + lm_head of decode rows into ``out`` [rows, V] bf16 (the fp8 weight copy when there is one)."""
+        B = h_rows.shape[0]
+        hn, _ = ops.rmsnorm_fwd(h_rows, self.model.norm.weight.data, self.dims.rms_eps)
+        fp8_head = None
+        if self.core.fp8 is not None:
+            fp8_head = self._fp8.view([self.lm_head.weight], tuple(self.lm_head.weight.shape))
+        if B <= 16 and llama_mod.DECODE_BLOCK_N == 0 and fp8_head is not None:
+            ops.gemm_skinny_fp8(hn, *fp8_head, out=out)
+        elif B <= llama_mod.FP8_MAX_ROWS and llama_mod.DECODE_BLOCK_N == 0 and fp8_head is not None:
+            ops.gemm_fp8w(hn, *fp8_head, out=out)
+        elif B <= 16 and llama_mod.DECODE_BLOCK_N == 0:
+            ops.gemm_skinny(hn, self.lm_head.weight.data, out=out)
+        else:
+            ops.gemm(hn, self.lm_head.weight.data, out=out, block_n=llama_mod.DECODE_BLOCK_N)
+
     @staticmethod
     def _load_trie(st, table) -> tuple:
         """Copy a flattened trie into the state's persistent device buffers (a captured graph keeps their pointers) in one
@@ -922,7 +938,8 @@ class ModifiedLlamaForCausalLM(nn.Module):
                  do_sample: bool = False, temperature: float = 1.0, eos_token_id: Optional[int] = None,
                  pad_token_id: Optional[int] = None, bos_token_id: Optional[int] = None, logits_processor=None, trie=None,
                  stop_on_eos: bool = True, use_cuda_graph: bool = True, stats: Optional[dict] = None, top_k: int = 50,
-                 top_p: float = 1.0, **unused) -> torch.Tensor:
+                 top_p: float = 1.0, num_beams: int = 1, length_penalty: float = 1.0, early_stopping: bool = False,
+                 num_return_sequences: int = 1, num_beam_groups: int = 1, **unused) -> torch.Tensor:
         """Prefill on the packed kernels (positions = cumsum(mask)-1 like HF generate; visual tokens injected only
         here, as in models/modified_lm.py:195-197), then one token per step over a pre-allocated KV cache.  The
         decode step of the greedy, sampled and trie-constrained modes has static shapes and is replayed as a CUDA graph
@@ -941,7 +958,23 @@ class ModifiedLlamaForCausalLM(nn.Module):
         A trie ``navillm_b200.trie.flatten_trie`` cannot represent faithfully, ``trie=`` together with
         ``logits_processor=``, and a call whose device walk reports a miss (a picked token outside the allowed set, which
         only a degenerate row can produce) run the host ``TrieLogitsProcessor`` instead - the miss case reruns the whole
-        call, with the CUDA RNG state restored, and discards the device result."""
+        call, with the CUDA RNG state restored, and discards the device result.
+
+        ``num_beams > 1`` is HF beam search as transformers 4.28 (the reference's pin) runs it, ``length_penalty``,
+        ``early_stopping`` and ``num_return_sequences`` included; see ``_generate_beam``.  Returns [B * num_return_sequences,
+        L] ids.  Beam sampling, group beam search, ``trie=`` / ``logits_processor=`` with beams and more return sequences than
+        beams raise ``NotImplementedError``."""
+        if num_beam_groups is not None and num_beam_groups > 1:
+            raise NotImplementedError("generate(num_beam_groups > 1): group (diverse) beam search is not built")
+        if num_return_sequences > max(1, num_beams):
+            raise NotImplementedError(f"generate(num_return_sequences={num_return_sequences}) needs as many beams "
+                                      f"(num_beams={num_beams}): sampled multi-sequence generation is not built")
+        if num_beams > 1:
+            if do_sample:
+                raise NotImplementedError("generate(num_beams > 1, do_sample=True): beam sampling is not built")
+            if trie is not None or logits_processor:
+                raise NotImplementedError("generate(num_beams > 1) with trie= / logits_processor=: the processors keep per-row "
+                                          "state that reordering the beams would scramble")
         if top_p is not None and top_p < 1.0:
             raise NotImplementedError("generate(top_p < 1) is not built: the reference never sets it (HF default 1.0)")
         if do_sample and not temperature > 0:
@@ -951,6 +984,10 @@ class ModifiedLlamaForCausalLM(nn.Module):
         dev = self._device()
         eos = self.tokenizer.eos_token_id if eos_token_id is None else eos_token_id
         pad = self.tokenizer.unk_token_id if pad_token_id is None else pad_token_id
+        if num_beams > 1:
+            return self._generate_beam(input_ids, attention_mask, cand_vis, hist_vis, obj_vis, max_new_tokens, int(num_beams), eos,
+                                       pad, float(length_penalty), bool(early_stopping), int(num_return_sequences), use_cuda_graph,
+                                       stats)
         procs = list(logits_processor or [])
         args = (input_ids, attention_mask, cand_vis, hist_vis, obj_vis, max_new_tokens, do_sample, temperature, eos, pad,
                 stop_on_eos, use_cuda_graph, stats, top_k)
@@ -1014,20 +1051,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
         hid_last, _ = core.forward(x, pp.pos, pp.cu, pp.seqlens, save=False, kv_store=(kc, vc), out_rows=pp.last_rows)
         special = self.special_ids_dev
 
-        fp8_head = None
-        if core.fp8 is not None:
-            fp8_head = self._fp8.view([self.lm_head.weight], tuple(self.lm_head.weight.shape))
-
-        def head(h_rows):
-            hn, _ = ops.rmsnorm_fwd(h_rows, self.model.norm.weight.data, d.rms_eps)
-            if B <= 16 and llama_mod.DECODE_BLOCK_N == 0 and fp8_head is not None:
-                ops.gemm_skinny_fp8(hn, *fp8_head, out=logits)
-            elif B <= llama_mod.FP8_MAX_ROWS and llama_mod.DECODE_BLOCK_N == 0 and fp8_head is not None:
-                ops.gemm_fp8w(hn, *fp8_head, out=logits)
-            elif B <= 16 and llama_mod.DECODE_BLOCK_N == 0:
-                ops.gemm_skinny(hn, self.lm_head.weight.data, out=logits)
-            else:
-                ops.gemm(hn, self.lm_head.weight.data, out=logits, block_n=llama_mod.DECODE_BLOCK_N)
+        head = lambda h_rows: self._decode_head(h_rows, logits)
 
         def pick_host(all_ids_host):
             """next token from `logits` -> next_ids (device), through the host processors."""
@@ -1131,3 +1155,185 @@ class ModifiedLlamaForCausalLM(nn.Module):
                 last = int(is_eos.float().argmax(dim=1).max())        # first EOS per row; the slowest row decides
                 new = new[:, :last + 1]
         return torch.cat([input_ids.to(dev), new], dim=1)
+
+    # ---- beam search (HF GenerationMixin.beam_search / BeamSearchScorer, transformers 4.28 as the reference pins it) ----
+    BEAM_MAX = 8
+
+    def _beam_state(self, B: int, K: int, Sp: int, G: int, key_extra: tuple, want_graph: bool):
+        """Persistent beam-search state, cached like ``_decode_state`` (same LRU): the prompt caches [B, Sp, D] per layer the K
+        beams of a prompt share, the generated caches [B * K, G, D] per layer, the device state of ``ops.beam_select`` and
+        the captured graph of one beam step."""
+        states = self.__dict__.setdefault("_decode_states", collections.OrderedDict())
+        key = ("beam", B, K, Sp, G) + key_extra
+        st = states.get(key) if want_graph else None
+        if st is not None:
+            states.move_to_end(key)
+            return st
+        dev, d = self._device(), self.dims
+        V, R = self.lm_head.weight.shape[0], B * K
+        if self.kv_cache_dtype == "fp8":
+            cache = lambda rows, n: [(torch.empty((rows, n, d.hidden), dtype=ops.fp8, device=dev),
+                                      torch.empty((rows, n, d.n_heads), dtype=torch.int8, device=dev)) for _ in range(d.n_layers)]
+        else:
+            cache = lambda rows, n: [torch.empty((rows, n, d.hidden), dtype=bf16, device=dev) for _ in range(d.n_layers)]
+        i32 = lambda *shape: torch.zeros(shape, dtype=torch.int32, device=dev)
+        st = SimpleNamespace(
+            pk=cache(B, Sp), pv=cache(B, Sp), kc=cache(R, G), vc=cache(R, G),
+            logits=torch.empty((R, (V + 63) // 64 * 64), dtype=bf16, device=dev)[:, :V],
+            next_ids=i32(R), lens=i32(R), plens=i32(B), beam_score=torch.zeros((R,), dtype=torch.float32, device=dev),
+            cand_score=torch.zeros((B, 2 * K), dtype=torch.float32, device=dev), cand_tok=i32(B, 2 * K), cand_par=i32(B, 2 * K),
+            hist=i32(R, G), src=i32(R, G), hyp_score=torch.zeros((B, K + 1), dtype=torch.float64, device=dev),
+            hyp_meta=i32(B, K, 2), hyp_tok=i32(B, K, G), pstate=i32(B, 5),
+            norm=torch.zeros((G,), dtype=torch.float64, device=dev), graph=None)
+        if want_graph:
+            states[key] = st
+            while len(states) > self.max_decode_states:
+                states.popitem(last=False)
+        return st
+
+    def _generate_beam(self, input_ids, attention_mask, cand_vis, hist_vis, obj_vis, max_new_tokens, K, eos, pad, length_penalty,
+                       early_stopping, n_return, use_cuda_graph, stats):
+        """Beam search over B prompts with K beams each.  The prefill runs once per prompt into the prompt cache, whose keys the
+        K beams of the prompt share; generated keys live in a [B * K, G] cache that is written once per slot and read through
+        the source table ``src`` (reordering the beams gathers ``src``, never K/V).  Each step is ``nv_beam_topk`` (2K best
+        candidates per prompt) and ``nv_beam_select`` (the scorer), all on the device, and is replayed as a CUDA graph; the
+        hypotheses are finalized on the host after one device-to-host copy.  The visual tokens of prompt b reach all K beams of
+        prompt b (the reference's HF expansion of ``cand_vis`` would hand them to other rows' slots)."""
+        if K > self.BEAM_MAX:
+            raise NotImplementedError(f"generate(num_beams={K}): at most {self.BEAM_MAX} beams are built")
+        if max_new_tokens < 1:
+            raise ValueError("generate(num_beams > 1) needs max_new_tokens >= 1")
+        dev = self._device()
+        core, d = self.core, self.dims
+        if d.head_dim != 128:
+            raise NotImplementedError("beam search is built for head_dim = 128")
+        ev = None
+        if stats is not None:
+            ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
+            ev[0].record()
+        pp = PackedPrompt(input_ids, attention_mask, self, dev, generate_positions=True)
+        vis = self.cat_vis(cand_vis, hist_vis, obj_vis, pp)
+        B, S = pp.B, int(input_ids.shape[1])
+        Sp = (max(pp.seqlens) + 127) // 128 * 128
+        G = (max_new_tokens + 127) // 128 * 128
+        key = (int(eos), int(pad), bool(early_stopping), self.kv_cache_dtype)     # what the captured step bakes in
+        st = self._beam_state(B, K, Sp, G, key, use_cuda_graph)
+        plens = torch.tensor(pp.seqlens, dtype=torch.int32)
+        st.plens.copy_(plens, non_blocking=True)
+        st.beam_score.view(B, K).fill_(-1e9)[:, 0] = 0.0             # only beam 0 of a prompt expands at the first step
+        st.hyp_score.zero_()
+        st.hyp_score[:, K] = 1e9                                      # BeamHypotheses.worst_score starts at 1e9
+        st.hyp_meta.zero_()
+        st.pstate.zero_()
+        st.pstate[:, 1].copy_(plens, non_blocking=True)
+        st.norm.copy_(ops.beam_norm(S, G, length_penalty))
+        special = self.special_ids_dev
+        E = self.model.embed_tokens.weight.data
+        x = ops.embed_fwd(pp.ids, E, pp.vis_src if vis is not None else None, vis)
+        hid_last, _ = core.forward(x, pp.pos, pp.cu, pp.seqlens, save=False, kv_store=(st.pk, st.pv), out_rows=pp.last_rows)
+        self._decode_head(hid_last, st.logits[:B])
+        sel = lambda: ops.beam_select(st.cand_score, st.cand_tok, st.cand_par, st.beam_score, st.hist, st.src, st.hyp_score,
+                                      st.hyp_meta, st.hyp_tok, st.pstate, st.next_ids, st.lens, st.norm, eos, pad,
+                                      early_stopping)
+        ops.beam_topk(st.logits, special, st.beam_score, K, st.cand_score, st.cand_tok, st.cand_par, first_step=True)
+        sel()
+        if ev is not None:
+            ev[1].record()
+        beam = SimpleNamespace(pk=st.pk, pv=st.pv, plens=st.plens, src=st.src, K=K)
+
+        def step():
+            with ops.pdl(self.decode_pdl):
+                xt = ops.embed_fwd(st.next_ids, E)
+                h = core.decode_step(xt, st.lens, st.kc, st.vc, beam=beam)
+                self._decode_head(h, st.logits)
+                ops.beam_topk(st.logits, special, st.beam_score, K, st.cand_score, st.cand_tok, st.cand_par)
+                sel()
+
+        # like the greedy loop, ask the device whether every prompt is done only every few steps: a done prompt's steps leave
+        # its hypotheses unchanged, so the extra steps change no output
+        T, replays = 1, 0                                             # T: beam steps run (tokens generated)
+        while T < max_new_tokens:
+            if T % 8 == 0 and bool(st.pstate[:, 4].all()):
+                break
+            if use_cuda_graph and st.graph is None:                   # first call with this state: eager step, then capture
+                step()
+                T += 1
+                g = torch.cuda.CUDAGraph()
+                torch.cuda.synchronize()
+                with torch.cuda.graph(g):
+                    step()
+                st.graph = g
+                continue
+            if use_cuda_graph:
+                st.graph.replay()
+                replays += 1
+            else:
+                step()
+            T += 1
+        if ev is not None:
+            ev[2].record()
+        # one copy; the fp64 scores go first, so their view starts at an even int32 offset whatever B and K are
+        parts = [st.hyp_score.flatten().view(torch.int32), st.hist.flatten(), st.hyp_meta.flatten(), st.hyp_tok.flatten(),
+                 st.pstate.flatten(), st.beam_score.view(torch.int32)]
+        host = torch.cat(parts).cpu()
+        o = np.cumsum([0] + [t.numel() for t in parts])
+        hyp_score = host[o[0]:o[1]].view(torch.float64).view(B, K + 1)
+        hist = host[o[1]:o[2]].view(B * K, G)
+        hyp_meta = host[o[2]:o[3]].view(B, K, 2)
+        hyp_tok = host[o[3]:o[4]].view(B, K, G)
+        pstate = host[o[4]:o[5]].view(B, 5)
+        beam_score = host[o[5]:o[6]].view(torch.float32)
+        if stats is not None:
+            torch.cuda.synchronize()
+            stats.update({"prefill_ms": ev[0].elapsed_time(ev[1]), "decode_ms": ev[1].elapsed_time(ev[2]) if T > 1 else None,
+                          "decode_steps": T - 1, "beam_steps": T, "graph_replays": replays, "kv_rows": Sp + G,
+                          "prompt_lens": list(pp.seqlens)})
+        T_done = int(pstate[0, 0])
+        hyps, running = [], []
+        for b in range(B):
+            n = int(pstate[b, 2])
+            kept = sorted(range(n), key=lambda i: int(hyp_meta[b, i, 1]))          # insertion order
+            hyps.append([(float(hyp_score[b, i]), hyp_tok[b, i, :int(hyp_meta[b, i, 0])].tolist()) for i in kept])
+            running.append(None if int(pstate[b, 4]) else
+                           [(float(beam_score[b * K + k]), hist[b * K + k, :T_done].tolist()) for k in range(K)])
+        seqs = beam_finalize(hyps, [float(hyp_score[b, K]) for b in range(B)], running, S, T_done, K, n_return, length_penalty)
+        return beam_output(input_ids.cpu(), seqs, S, S + max_new_tokens, eos, pad).to(dev)
+
+
+def beam_finalize(hyps, worst, running, S: int, T: int, K: int, n_return: int, length_penalty: float):
+    """BeamSearchScorer.finalize of transformers 4.28: prompts that are not done add their K running beams (score
+    sum_logprobs / (S + T) ** length_penalty, the Python float arithmetic of BeamHypotheses.add), then each prompt returns its
+    ``n_return`` best hypotheses, best first; of equal scores the one added last wins (a stable sort, popped from the end).
+    hyps[b]: the kept (score, generated tokens) in insertion order; worst[b]: their worst_score; running[b]: the K (running
+    score, tokens) of a prompt that is not done, else None.  Returns [[generated tokens] * n_return] per prompt."""
+    out = []
+    for b, beams in enumerate(hyps):
+        beams, w = list(beams), worst[b]
+        for sc, toks in (running[b] or []):
+            score = sc / ((S + T) ** length_penalty)
+            if len(beams) < K or score > w:
+                beams.append((score, toks))
+                if len(beams) > K:
+                    order = sorted([(s, i) for i, (s, _) in enumerate(beams)])
+                    del beams[order[0][1]]
+                    w = order[1][0]
+                else:
+                    w = min(score, w)
+        ranked = sorted(beams, key=lambda x: x[0])
+        out.append([ranked.pop()[1] for _ in range(n_return)])
+    return out
+
+
+def beam_output(prompt_ids: torch.Tensor, seqs, S: int, max_length: int, eos: int, pad: int) -> torch.Tensor:
+    """HF ``sequences`` of a beam search: [B * n, L] int64 rows of prompt ids and generated tokens, L = min(longest + 1,
+    max_length); a row shorter than L gets EOS after its tokens, then pad."""
+    rows = [(b, toks) for b, per in enumerate(seqs) for toks in per]
+    L = min(max(S + len(t) for _, t in rows) + 1, max_length)
+    out = torch.full((len(rows), L), pad, dtype=torch.int64)
+    for i, (b, toks) in enumerate(rows):
+        n = S + len(toks)
+        out[i, :S] = prompt_ids[b]
+        out[i, S:n] = torch.tensor(toks, dtype=torch.int64)
+        if n < L:
+            out[i, n] = eos
+    return out

@@ -728,6 +728,102 @@ def decode_attn_rope_fp8(qkv, lens, cos_t, sin_t, kq, vq, ke, ve, n_heads, *, ou
     return out
 
 
+def _beam_io(name, B, K, G, **ts):
+    """Dtype / shape / device checks of the beam-search state (include/navillm_b200.h, nv_beam_*)."""
+    want = {"cand_score": (torch.float32, (B, 2 * K)), "cand_tok": (torch.int32, (B, 2 * K)), "cand_parent": (torch.int32, (B, 2 * K)),
+            "beam_score": (torch.float32, (B * K,)), "hist": (torch.int32, (B * K, G)), "src": (torch.int32, (B * K, G)),
+            "hyp_score": (torch.float64, (B, K + 1)), "hyp_meta": (torch.int32, (B, K, 2)), "hyp_tok": (torch.int32, (B, K, G)),
+            "prompt_state": (torch.int32, (B, 5)), "next_ids": (torch.int32, (B * K,)), "lens": (torch.int32, (B * K,)),
+            "norm": (torch.float64, (G,)),
+            "plens": (torch.int32, (B,))}
+    for k, t in ts.items():
+        dt, shape = want[k]
+        if t.dtype != dt or tuple(t.shape) != shape or not t.is_cuda or not t.is_contiguous():
+            raise ValueError(f"{name}: {k} {dt} {list(shape)} contiguous on the device expected (got {t.dtype} {tuple(t.shape)})")
+
+
+def beam_topk(logits, special, beam_score, K, cand_score, cand_tok, cand_parent, *, first_step=False):
+    """The 2K best next-token candidates of each prompt (nv_beam_topk): logits bf16 [B * K, V] (beam k of prompt b in row
+    b * K + k), or with ``first_step`` [>= B, V] holding one prefill row per prompt that all K beams read.  beam_score fp32
+    [B * K].  Writes cand_score fp32, cand_tok and cand_parent int32 [B, 2K], best first."""
+    B = cand_score.shape[0]
+    V = logits.shape[1]
+    if logits.dtype != bf16 or logits.stride(1) != 1 or logits.shape[0] < (B if first_step else B * K):
+        raise ValueError(f"beam_topk: bf16 logits with {B if first_step else B * K} rows expected (got {logits.dtype} {tuple(logits.shape)})")
+    _beam_io("beam_topk", B, K, 1, cand_score=cand_score, cand_tok=cand_tok, cand_parent=cand_parent, beam_score=beam_score)
+    ld = logits.stride(0)
+    check(_lib.load().nv_beam_topk(ptr(logits), i64(ld if first_step else K * ld), i64(0 if first_step else ld), i32(V), ptr(special),
+                                   i32(special.numel()), ptr(beam_score), ptr(cand_score), ptr(cand_tok), ptr(cand_parent), i32(B),
+                                   i32(K), stream_ptr()), "nv_beam_topk")
+
+
+def beam_select(cand_score, cand_tok, cand_parent, beam_score, hist, src, hyp_score, hyp_meta, hyp_tok, prompt_state, next_ids, lens,
+                norm, eos_id, pad_id, early_stopping):
+    """One BeamSearchScorer.process step on the device (nv_beam_select); norm fp64 [G]: (S + t) ** length_penalty for S padded
+    prompt columns (``beam_norm``)."""
+    B, K2 = cand_score.shape
+    K, G = K2 // 2, hist.shape[1]
+    _beam_io("beam_select", B, K, G, cand_score=cand_score, cand_tok=cand_tok, cand_parent=cand_parent, beam_score=beam_score,
+             hist=hist, src=src, hyp_score=hyp_score, hyp_meta=hyp_meta, hyp_tok=hyp_tok, prompt_state=prompt_state,
+             next_ids=next_ids, lens=lens, norm=norm)
+    check(_lib.load().nv_beam_select(ptr(cand_score), ptr(cand_tok), ptr(cand_parent), ptr(beam_score), ptr(hist), ptr(src),
+                                     ptr(hyp_score), ptr(hyp_meta), ptr(hyp_tok), ptr(prompt_state), ptr(next_ids), ptr(lens), ptr(norm),
+                                     i32(B), i32(K), i32(G), i32(eos_id), i32(pad_id), i32(1 if early_stopping else 0), stream_ptr()),
+          "nv_beam_select")
+
+
+def beam_norm(S: int, G: int, length_penalty: float) -> torch.Tensor:
+    """The hypothesis normalisers (S + t) ** length_penalty, t < G, in the Python float arithmetic of transformers 4.28's
+    BeamHypotheses.add (host fp64 [G]; copy it to the device for ``beam_select``)."""
+    return torch.tensor([(S + t) ** length_penalty for t in range(G)], dtype=torch.float64)
+
+
+def _beam_attn_args(name, qkv, lens, plens, src, R, K, HD, n_heads, out):
+    if HD != n_heads * 128 or qkv.dtype != bf16 or qkv.stride(1) != 1 or tuple(qkv.shape) != (R, 3 * HD):
+        raise ValueError(f"{name}: qkv bf16 [{R}, {3 * HD}] and {HD // 128} heads expected (got {qkv.dtype} {tuple(qkv.shape)}, "
+                         f"{n_heads} heads)")
+    if R % K:
+        raise ValueError(f"{name}: {R} beam rows is not a multiple of {K} beams")
+    _beam_io(name, R // K, K, src.shape[1], lens=lens, plens=plens, src=src)
+    if out is None:
+        out = torch.empty((R, HD), dtype=bf16, device=qkv.device)
+    if out.dtype != bf16 or out.stride(1) != 1 or tuple(out.shape) != (R, HD):
+        raise ValueError(f"{name}: out bf16 [{R}, {HD}] expected (got {out.dtype} {tuple(out.shape)})")
+    return out
+
+
+def decode_attn_rope_beam(qkv, lens, cos_t, sin_t, pk, pv, plens, kc, vc, src, K, n_heads, *, out=None, scale=None):
+    """``decode_attn_rope`` for R = B * K beam rows (nv_decode_attn_rope_beam): keys [0, plens[b]) from the prompt cache pk / pv
+    [B, Sp, H*128] shared by the K beams of prompt b, generated key i of row r from kc / vc [R, G, H*128] at row (src[r, i], i).
+    The new k / v are written at (r, lens[r] - plens[r // K]).  Returns [R, H*128] bf16."""
+    R, G, HD = kc.shape
+    if pk.shape[2] != HD or vc.shape != kc.shape or pv.shape != pk.shape or pk.dtype != bf16 or kc.dtype != bf16:
+        raise ValueError(f"decode_attn_rope_beam: bf16 caches [B, Sp, {HD}] / [R, G, {HD}] expected")
+    out = _beam_attn_args("decode_attn_rope_beam", qkv, lens, plens, src, R, K, HD, n_heads, out)
+    check(_lib.load().nv_decode_attn_rope_beam(ptr(qkv), i64(qkv.stride(0)), ptr(lens), ptr(cos_t), ptr(sin_t), ptr(pk), ptr(pv),
+                                               i32(pk.shape[1]), ptr(plens), ptr(kc), ptr(vc), ptr(src), i32(G), ptr(out),
+                                               i64(out.stride(0)), i32(R), i32(K), i32(n_heads), i32(128),
+                                               f32(128 ** -0.5 if scale is None else scale), stream_ptr()), "nv_decode_attn_rope_beam")
+    return out
+
+
+def decode_attn_rope_beam_fp8(qkv, lens, cos_t, sin_t, pk, pv, pke, pve, plens, kq, vq, ke, ve, src, K, n_heads, *, out=None,
+                              scale=None):
+    """``decode_attn_rope_beam`` over fp8 caches (the format of ``decode_attn_rope_fp8``): bit for bit the bf16 beam kernel on
+    caches holding the rounded rows K' / V'."""
+    _fp8_kv(pk, pv, pke, pve, "decode_attn_rope_beam_fp8")
+    R, G, HD = _fp8_kv(kq, vq, ke, ve, "decode_attn_rope_beam_fp8")
+    if pk.shape[2] != HD:
+        raise ValueError(f"decode_attn_rope_beam_fp8: prompt cache width {pk.shape[2]} != {HD}")
+    out = _beam_attn_args("decode_attn_rope_beam_fp8", qkv, lens, plens, src, R, K, HD, n_heads, out)
+    check(_lib.load().nv_decode_attn_rope_beam_fp8(ptr(qkv), i64(qkv.stride(0)), ptr(lens), ptr(cos_t), ptr(sin_t), ptr(pk), ptr(pv),
+                                                   ptr(pke), ptr(pve), i32(pk.shape[1]), ptr(plens), ptr(kq), ptr(vq), ptr(ke), ptr(ve),
+                                                   ptr(src), i32(G), ptr(out), i64(out.stride(0)), i32(R), i32(K), i32(n_heads), i32(128),
+                                                   f32(128 ** -0.5 if scale is None else scale), stream_ptr()),
+          "nv_decode_attn_rope_beam_fp8")
+    return out
+
+
 def argmax_masked(logits, special, finished, eos_id, pad_id, stop_on_eos, next_ids):
     B, V = logits.shape
     check(_lib.load().nv_argmax_masked(ptr(logits), i64(logits.stride(0)), i32(V), ptr(special), i32(special.numel()),
