@@ -15,7 +15,6 @@ PyTorch is used for device memory only.  There is no CPU path.
 """
 from __future__ import annotations
 
-import os
 from dataclasses import dataclass
 from types import SimpleNamespace
 from typing import List, Optional
@@ -25,17 +24,12 @@ import torch.nn as nn
 
 from . import ops
 
-# decode GEMMs: 0 (default) = swap-AB skinny kernel for batches <= 16 (csrc/gemm_skinny.cu), nv_gemm_bf16's measured tile
-# table above that; 128 / 32 = force that column-tile width of the general kernel (A/B measurements)
-DECODE_BLOCK_N = int(os.environ.get("NAVILLM_DECODE_BLOCK_N", "0"))
 # Largest GEMM row count at which an inference GEMM above 16 rows streams the fp8 copy of its weight (Fp8Weights,
 # nv_gemm_fp8w_bf16) instead of the bf16 weights.  Measured (tools/midm_bench.py --fp8, H100 80GB HBM3 at 700 W, fp8 vs bf16):
 # qkv 1.04-1.10x and down 1.10x at M = 17..64, o_proj 0.95-1.03x; from M = 96 qkv is slower (0.96x), from M = 128 down (0.90x),
 # and at M >= 192 every shape is (0.64-0.94x).  The fused gate|up weight (N = 2F) is slower at every M (0.90-0.95x up to 128),
 # so it keeps its bf16 weight above 16 rows (_fp8_layer).  lm_head: 0.94x at 17, 0.99x at 32, 1.06x at 64.
 FP8_MAX_ROWS = 64
-# weight-gradient GEMMs on a side stream (see LlamaCore.backward)
-WGRAD_STREAM = os.environ.get("NAVILLM_WGRAD_STREAM", "0") != "0"
 
 bf16 = torch.bfloat16
 
@@ -410,30 +404,36 @@ def is_fp8_kv(caches) -> bool:
     return isinstance(caches[0], tuple)
 
 
+def kv_cache(d: LlamaDims, rows: int, length: int, dtype: str, device, zero: bool = False) -> list:
+    """A per-layer KV cache of ``rows`` sequences of ``length`` positions: bf16 [rows, length, D] tensors, or for ``dtype``
+    "fp8" the ``is_fp8_kv`` pairs.  ``zero``: zero-initialised, else uninitialised."""
+    new = torch.zeros if zero else torch.empty
+    if dtype == "fp8":
+        return [(new((rows, length, d.hidden), dtype=ops.fp8, device=device),
+                 new((rows, length, d.n_heads), dtype=torch.int8, device=device)) for _ in range(d.n_layers)]
+    return [new((rows, length, d.hidden), dtype=bf16, device=device) for _ in range(d.n_layers)]
+
+
 class LlamaCore:
     """Forward/backward driver of the decoder stack on packed rows.  Not an nn.Module: parameters live in
     ``LlamaModelParams`` (HF-named) and are accessed through fused views of a ``FlatParams`` buffer."""
 
     def __init__(self, dims: LlamaDims, model: LlamaModelParams, flat: FlatParams):
+        if dims.head_dim != 128:
+            raise ValueError(f"LlamaCore: the attention kernels are built for head_dim 128 (got {dims.head_dim})")
         self.d = dims
         self.model = model
         self.flat = flat
         D, F = dims.hidden, dims.inter
-        self.wqkv, self.gqkv, self.wo, self.go, self.wgu, self.ggu, self.wd, self.gd = [], [], [], [], [], [], [], []
+        self.wqkv, self.wo, self.wgu, self.wd = [], [], [], []
         for lyr in model.layers:
             a, m = lyr.self_attn, lyr.mlp
-            qkv = [a.q_proj.weight, a.k_proj.weight, a.v_proj.weight]
-            self.wqkv.append(flat.view(qkv, (3 * D, D)))
-            self.gqkv.append(flat.grad_view(qkv, (3 * D, D)))
+            self.wqkv.append(flat.view([a.q_proj.weight, a.k_proj.weight, a.v_proj.weight], (3 * D, D)))
             self.wo.append(a.o_proj.weight.data)
-            self.go.append(a.o_proj.weight.grad)
-            gu = [m.gate_proj.weight, m.up_proj.weight]
-            self.wgu.append(flat.view(gu, (2 * F, D)))
-            self.ggu.append(flat.grad_view(gu, (2 * F, D)))
+            self.wgu.append(flat.view([m.gate_proj.weight, m.up_proj.weight], (2 * F, D)))
             self.wd.append(m.down_proj.weight.data)
-            self.gd.append(m.down_proj.weight.grad)
+        self.refresh_grad_views()
         self.cos, self.sin = rope_tables(dims, flat.flat.device)
-        self.fused_epilogues = True
         self.fp8 = None
         self.fp8_src = None
         self.act_fp8 = False          # W8A8 in the no-grad forwards (ModifiedLlamaForCausalLM.set_activation_dtype)
@@ -502,49 +502,97 @@ class LlamaCore:
         return a8.wqkv[l], a8.wo[l], a8.wgu[l], a8.wd[l]
 
     def refresh_grad_views(self) -> None:
-        """Re-derive the fused gradient views after ``FlatParams.rebind_grads``."""
+        """(Re-)derive the fused gradient views, e.g. after ``FlatParams.rebind_grads``."""
         D, F = self.d.hidden, self.d.inter
         flat = self.flat
-        for l, lyr in enumerate(self.model.layers):
+        self.gqkv, self.go, self.ggu, self.gd = [], [], [], []
+        for lyr in self.model.layers:
             a, m = lyr.self_attn, lyr.mlp
-            self.gqkv[l] = flat.grad_view([a.q_proj.weight, a.k_proj.weight, a.v_proj.weight], (3 * D, D))
-            self.go[l] = a.o_proj.weight.grad
-            self.ggu[l] = flat.grad_view([m.gate_proj.weight, m.up_proj.weight], (2 * F, D))
-            self.gd[l] = m.down_proj.weight.grad
+            self.gqkv.append(flat.grad_view([a.q_proj.weight, a.k_proj.weight, a.v_proj.weight], (3 * D, D)))
+            self.go.append(a.o_proj.weight.grad)
+            self.ggu.append(flat.grad_view([m.gate_proj.weight, m.up_proj.weight], (2 * F, D)))
+            self.gd.append(m.down_proj.weight.grad)
 
     # -------------------------------------------------------------------------------------------------
-    # packed batches below this many rows run the inference forward through ONE C-ABI call per layer (csrc/layer.cu):
-    # they are host-bound when every kernel is its own call from Python
-    LAYER_CALL = os.environ.get("NAVILLM_LAYER_CALL", "1") != "0"
+    # Inference forwards that do not run the fused-epilogue GEMMs go through ONE C-ABI call per layer (csrc/layer.cu): they
+    # are host-bound when every kernel is its own call from Python.  Tests turn this off to run the per-kernel path as the
+    # reference.
+    LAYER_CALL = True
 
-    def _forward_layer_calls(self, x, pos, cu, seqlens, kv_store, out_rows, a8=None):
+    def _fused(self, T: int, a8) -> bool:
+        """Whether a forward of T rows runs the fused-epilogue kernels (RoPE / SwiGLU in the 128 x 256-tile GEMM's epilogue).
+        They need F % 128 == 0, D % 256 == 0 and at least one wave of tiles; W8A8 runs the plain GEMM and the RoPE / SwiGLU
+        row kernels instead."""
         d = self.d
-        T = x.shape[0]
+        return a8 is None and T >= 1024 and d.inter % 128 == 0 and d.hidden % 256 == 0
+
+    def _layer_calls(self, x, pos, cu, seqlens, out_rows, a8, kc, vc, mode, Smax, Tkv=0, cached=None, kv_start=None,
+                     kv_len=None):
+        """The inference forward of every layer through ``ops.LayerRunner``.  ``mode`` .. ``kv_len``: the cache mode of
+        ``LayerRunner.set_cache_mode`` (0: no cache, 1 / 3: prompt store, 2 / 4: suffix over the cache; 3 / 4 fp8) with the
+        per-layer caches ``kc`` / ``vc``."""
+        d = self.d
         R = 0 if out_rows is None else out_rows.numel()
-        run = ops.LayerRunner(T, d.hidden, d.inter, d.n_heads, d.rms_eps, pos, self.cos, self.sin, cu, len(seqlens), ops._qblocks(seqlens),
-                              R=R, device=x.device)
-        fp8_kv = kv_store is not None and is_fp8_kv(kv_store[0])
-        if kv_store is not None:
-            run.set_cache_mode(3 if fp8_kv else 1, kv_store[0][0][0].shape[1] if fp8_kv else kv_store[0][0].shape[1])
+        run = ops.LayerRunner(x.shape[0], d.hidden, d.inter, d.n_heads, d.rms_eps, pos, self.cos, self.sin, cu, len(seqlens),
+                              ops._qblocks(seqlens), R=R, device=x.device)
+        run.set_cache_mode(mode, Smax, Tkv, cached, kv_start, kv_len)
         bufs = [torch.empty_like(x), torch.empty_like(x)]
         last = d.n_layers - 1
         f8 = self.fp8_for_inference()
         for l, lyr in enumerate(self.model.layers):
             pruned = out_rows is not None and l == last
             y = torch.empty((R, d.hidden), dtype=bf16, device=x.device) if pruned else bufs[l & 1]
-            kc = vc = ke = ve = None
-            if fp8_kv:
-                (kc, ke), (vc, ve) = kv_store[0][l], kv_store[1][l]
-            elif kv_store is not None:
-                kc, vc = kv_store[0][l], kv_store[1][l]
-            run.run(x, y, lyr.input_layernorm.weight.data, self.wqkv[l], self.wo[l], lyr.post_attention_layernorm.weight.data, self.wgu[l],
-                    self.wd[l], kc=kc, vc=vc, ke=ke, ve=ve, out_rows=out_rows if pruned else None,
+            k = v = ke = ve = None
+            if mode in (3, 4):
+                (k, ke), (v, ve) = kc[l], vc[l]
+            elif mode:
+                k, v = kc[l], vc[l]
+            run.run(x, y, lyr.input_layernorm.weight.data, self.wqkv[l], self.wo[l], lyr.post_attention_layernorm.weight.data,
+                    self.wgu[l], self.wd[l], kc=k, vc=v, ke=ke, ve=ve, out_rows=out_rows if pruned else None,
                     fp8=self._w8a8_layer(a8, l) if a8 is not None else self._fp8_layer(f8, l), fp8_max_rows=FP8_MAX_ROWS,
                     act_fp8=a8 is not None)
             x = y
         return x
 
-    def forward(self, x: torch.Tensor, pos: torch.Tensor, cu: torch.Tensor, seqlens, save: bool = True, kv_sink=None,
+    def _layers(self, x, pos, out_rows, save, a8, fused, attend):
+        """The per-kernel forward of every layer.  ``attend(l, qkv, s)`` is the attention step, the one part the prompt and
+        the suffix forwards do differently: it returns the attention output of layer l and sets ``s.lse`` when saving.
+        Returns the residual stream and the per-layer activations (empty unless ``save``)."""
+        d = self.d
+        saved: List[_Saved] = []
+        last = d.n_layers - 1
+        f8 = None if save else self.fp8_for_inference()     # training forwards never read the fp8 copy
+        q8 = a8 is not None
+        for l, lyr in enumerate(self.model.layers):
+            w8 = self._w8a8_layer(a8, l) if q8 else (self._fp8_layer(f8, l) or ((None, None),) * 4)
+            s = _Saved()
+            s.x = x
+            s.xn, s.rstd1 = ops.rmsnorm_fwd(x, lyr.input_layernorm.weight.data, d.rms_eps)
+            if fused:
+                s.qkv = ops.gemm_rope(s.xn, self.wqkv[l], pos, self.cos, self.sin, 2 * d.hidden)   # RoPE in the epilogue
+            else:
+                s.qkv = self._linear(s.xn, self.wqkv[l], w8[0], w8a8=q8)
+                ops.rope_(s.qkv, pos, self.cos, self.sin, 2 * d.n_heads, d.head_dim)
+            s.ao = attend(l, s.qkv, s)
+            s.rows = None
+            ao, xin = s.ao, x
+            if out_rows is not None and l == last:
+                s.rows = out_rows
+                ao = s.ao_r = ops.gather_rows(s.ao, out_rows)
+                xin = ops.gather_rows(x, out_rows)
+            s.xm = self._linear(ao, self.wo[l], w8[1], addend=xin, w8a8=q8)
+            s.xn2, s.rstd2 = ops.rmsnorm_fwd(s.xm, lyr.post_attention_layernorm.weight.data, d.rms_eps)
+            if fused and s.rows is None:
+                s.gu, s.h = ops.gemm_swiglu(s.xn2, self.wgu[l], keep_gu=save)                      # SwiGLU in the epilogue
+            else:
+                s.gu = self._linear(s.xn2, self.wgu[l], w8[2], w8a8=q8)
+                s.h = ops.swiglu_fwd(s.gu)
+            x = self._linear(s.h, self.wd[l], w8[3], addend=s.xm, w8a8=q8)
+            if save:
+                saved.append(s)
+        return x, saved
+
+    def forward(self, x: torch.Tensor, pos: torch.Tensor, cu: torch.Tensor, seqlens, save: bool = True,
                 out_rows: Optional[torch.Tensor] = None, kv_store=None):
         """x: [T, D] bf16 input embeddings (packed); pos: int32 [T]; cu: int32 [B+1] (device); seqlens: host
         lengths.  Returns (residual stream after the last layer BEFORE the final RMSNorm, tape) where ``tape``
@@ -558,55 +606,25 @@ class LlamaCore:
 
         ``kv_store`` (prefill of generate): (kc, vc) per-layer caches, bf16 [B, Smax, D] or fp8 ``(e4m3 [B, Smax, D], int8
         exponents [B, Smax, H])`` pairs (``is_fp8_kv``); the prompt's own attention reads the unrounded K, V either way."""
-        d = self.d
-        H = d.n_heads
-        saved: List[_Saved] = []
-        last = d.n_layers - 1
+        B, T, H = len(seqlens), x.shape[0], self.d.n_heads
         a8 = None if save else self.act_fp8_weights()       # W8A8 (set_activation_dtype("fp8")): no-grad forwards only
-        # fused-epilogue kernels (128 x 256-tile GEMM) need head_dim 128, F % 128 == 0 and at least one wave of tiles; W8A8
-        # runs the plain GEMM and the RoPE / SwiGLU row kernels instead
-        fused = a8 is None and self.fused_epilogues and x.shape[0] >= 1024 and d.inter % 128 == 0 and d.hidden % 256 == 0
-        if kv_store is not None and kv_sink is None:                  # (kc list, vc list): post-RoPE K, V of every layer go to the caches
-            B_, T_ = len(seqlens), x.shape[0]
-            if is_fp8_kv(kv_store[0]):                                # fp8 cache: (e4m3 bytes, exponents) per layer
-                kv_sink = lambda l, qkv: ops.kv_store_prefill_fp8(qkv, cu, kv_store[0][l][0], kv_store[1][l][0], kv_store[0][l][1],
-                                                                  kv_store[1][l][1], B_, T_)
-            else:
-                kv_sink = lambda l, qkv: ops.kv_store_prefill(qkv, cu, kv_store[0][l], kv_store[1][l], B_, T_)
-        if self.LAYER_CALL and not save and not fused and d.head_dim == 128 and (kv_store is not None or kv_sink is None):
-            return self._forward_layer_calls(x, pos, cu, seqlens, kv_store, out_rows, a8), None
-        f8 = None if save else self.fp8_for_inference()     # training forwards never read the fp8 copy
-        q8 = a8 is not None
-        for l, lyr in enumerate(self.model.layers):
-            w8 = self._w8a8_layer(a8, l) if q8 else (self._fp8_layer(f8, l) or ((None, None),) * 4)
-            s = _Saved()
-            s.x = x
-            s.xn, s.rstd1 = ops.rmsnorm_fwd(x, lyr.input_layernorm.weight.data, d.rms_eps)
-            if fused:
-                s.qkv = ops.gemm_rope(s.xn, self.wqkv[l], pos, self.cos, self.sin, 2 * d.hidden)   # RoPE in the epilogue
-            else:
-                s.qkv = self._linear(s.xn, self.wqkv[l], w8[0], w8a8=q8)
-                ops.rope_(s.qkv, pos, self.cos, self.sin, 2 * H, d.head_dim)
-            if kv_sink is not None:
-                kv_sink(l, s.qkv)                      # prefill of generate(): post-RoPE K,V go to the cache
-            s.ao, s.lse = ops.attn_fwd(s.qkv, cu, seqlens, H)
-            s.rows = None
-            ao, xin = s.ao, x
-            if out_rows is not None and l == last:
-                s.rows = out_rows
-                ao = s.ao_r = ops.gather_rows(s.ao, out_rows)
-                xin = ops.gather_rows(x, out_rows)
-            s.xm = self._linear(ao, self.wo[l], w8[1], addend=xin, w8a8=q8)
-            s.xn2, s.rstd2 = ops.rmsnorm_fwd(s.xm, lyr.post_attention_layernorm.weight.data, d.rms_eps)
-            if fused and s.rows is None:
-                s.gu, s.h = ops.gemm_swiglu(s.xn2, self.wgu[l])                                    # SwiGLU in the epilogue
-            else:
-                s.gu = self._linear(s.xn2, self.wgu[l], w8[2], w8a8=q8)
-                s.h = ops.swiglu_fwd(s.gu)
-            x = self._linear(s.h, self.wd[l], w8[3], addend=s.xm, w8a8=q8)
-            if save:
-                saved.append(s)
-        return x, ((saved, (pos, cu, list(seqlens))) if save else None)
+        fused = self._fused(T, a8)
+        kc, vc = kv_store if kv_store is not None else (None, None)
+        fp8_kv = kc is not None and is_fp8_kv(kc)
+        if self.LAYER_CALL and not save and not fused:
+            mode = 0 if kc is None else 3 if fp8_kv else 1
+            Smax = 0 if kc is None else (kc[0][0] if fp8_kv else kc[0]).shape[1]
+            return self._layer_calls(x, pos, cu, seqlens, out_rows, a8, kc, vc, mode, Smax), None
+
+        def attend(l, qkv, s):
+            if fp8_kv:                                       # prefill of generate(): post-RoPE K, V go to the cache
+                ops.kv_store_prefill_fp8(qkv, cu, kc[l][0], vc[l][0], kc[l][1], vc[l][1], B, T)
+            elif kc is not None:
+                ops.kv_store_prefill(qkv, cu, kc[l], vc[l], B, T)
+            ao, s.lse = ops.attn_fwd(qkv, cu, seqlens, H)
+            return ao
+        x, saved = self._layers(x, pos, out_rows, save, a8, fused, attend)
+        return x, ((saved, (pos, cu, list(seqlens)), None) if save else None)
 
     # -------------------------------------------------------------------------------------------------
     def forward_suffix(self, x: torch.Tensor, pos: torch.Tensor, cu: torch.Tensor, q_lens, kc: List[torch.Tensor],
@@ -633,65 +651,26 @@ class LlamaCore:
         d = self.d
         H, D = d.n_heads, d.hidden
         B, T = len(q_lens), x.shape[0]
-        last = d.n_layers - 1
         a8 = None if save else self.act_fp8_weights()       # W8A8 (set_activation_dtype("fp8")): no-grad forwards only
-        q8 = a8 is not None
-        fused = not q8 and self.fused_epilogues and T >= 1024 and d.inter % 128 == 0 and d.hidden % 256 == 0
-        f8 = None if save else self.fp8_for_inference()     # training forwards never read the fp8 copy
+        fused = self._fused(T, a8)
         fp8_kv = is_fp8_kv(kc)
         if save and (fp8_kv or acc is None or kv_lens is None):
             raise ValueError("forward_suffix(save=True) needs bf16 caches, the gradient accumulators and the host kv_lens")
-        Bc, Smax = (kc[0][0] if fp8_kv else kc[0]).shape[:2]
-        if self.LAYER_CALL and not fused and d.head_dim == 128 and not save:
-            R = 0 if out_rows is None else out_rows.numel()
-            run = ops.LayerRunner(T, D, d.inter, H, d.rms_eps, pos, self.cos, self.sin, cu, B, ops._qblocks(q_lens), R=R, device=x.device)
-            run.set_cache_mode(4 if fp8_kv else 2, Smax, Bc * Smax, cached, kv_start, kv_len)
-            bufs = [torch.empty_like(x), torch.empty_like(x)]
-            for l, lyr in enumerate(self.model.layers):
-                pruned = out_rows is not None and l == last
-                y = torch.empty((R, D), dtype=bf16, device=x.device) if pruned else bufs[l & 1]
-                (kl, ke), (vl, ve) = (kc[l], vc[l]) if fp8_kv else ((kc[l], None), (vc[l], None))
-                run.run(x, y, lyr.input_layernorm.weight.data, self.wqkv[l], self.wo[l], lyr.post_attention_layernorm.weight.data,
-                        self.wgu[l], self.wd[l], kc=kl, vc=vl, ke=ke, ve=ve, out_rows=out_rows if pruned else None,
-                        fp8=self._w8a8_layer(a8, l) if q8 else self._fp8_layer(f8, l), fp8_max_rows=FP8_MAX_ROWS, act_fp8=q8)
-                x = y
-            return x
-        saved: List[_Saved] = []
-        for l, lyr in enumerate(self.model.layers):
-            w8 = self._w8a8_layer(a8, l) if q8 else (self._fp8_layer(f8, l) or ((None, None),) * 4)
-            s = _Saved()
-            s.x = x
-            xn, s.rstd1 = ops.rmsnorm_fwd(x, lyr.input_layernorm.weight.data, d.rms_eps)
-            if fused:
-                qkv = ops.gemm_rope(xn, self.wqkv[l], pos, self.cos, self.sin, 2 * D)
-            else:
-                qkv = self._linear(xn, self.wqkv[l], w8[0], w8a8=q8)
-                ops.rope_(qkv, pos, self.cos, self.sin, 2 * H, d.head_dim)
-            s.lse = torch.empty((H, T), dtype=torch.float32, device=x.device) if save else None
+        if self.LAYER_CALL and not save and not fused:
+            Bc, Smax = (kc[0][0] if fp8_kv else kc[0]).shape[:2]
+            return self._layer_calls(x, pos, cu, q_lens, out_rows, a8, kc, vc, 4 if fp8_kv else 2, Smax, Bc * Smax, cached,
+                                     kv_start, kv_len)
+
+        def attend(l, qkv, s):
             if fp8_kv:
                 (kq, ke), (vq, ve) = kc[l], vc[l]
                 ops.kv_store_suffix_fp8(qkv, cu, cached, kq, vq, ke, ve, B, T)
-                ao = ops.attn_fwd_kv_fp8(qkv[:, :D], kq, vq, ke, ve, cu, q_lens, kv_start, kv_len, H)
-            else:
-                if store:
-                    ops.kv_store_suffix(qkv, cu, cached, kc[l], vc[l], B, T)
-                ao = ops.attn_fwd_kv(qkv[:, :D], kc[l], vc[l], cu, q_lens, kv_start, kv_len, H, lse=s.lse)
-            s.xn, s.qkv, s.ao, s.rows = xn, qkv, ao, None
-            xin = x
-            if out_rows is not None and l == last:
-                s.rows = out_rows
-                ao = s.ao_r = ops.gather_rows(ao, out_rows)
-                xin = ops.gather_rows(x, out_rows)
-            s.xm = xm = self._linear(ao, self.wo[l], w8[1], addend=xin, w8a8=q8)
-            s.xn2, s.rstd2 = xn2, _ = ops.rmsnorm_fwd(xm, lyr.post_attention_layernorm.weight.data, d.rms_eps)
-            if fused and xm.shape[0] >= 1024:
-                s.gu, s.h = ops.gemm_swiglu(xn2, self.wgu[l], keep_gu=save)
-            else:
-                s.gu = self._linear(xn2, self.wgu[l], w8[2], w8a8=q8)
-                s.h = ops.swiglu_fwd(s.gu)
-            x = self._linear(s.h, self.wd[l], w8[3], addend=xm, w8a8=q8)
-            if save:
-                saved.append(s)
+                return ops.attn_fwd_kv_fp8(qkv[:, :D], kq, vq, ke, ve, cu, q_lens, kv_start, kv_len, H)
+            if store:
+                ops.kv_store_suffix(qkv, cu, cached, kc[l], vc[l], B, T)
+            s.lse = torch.empty((H, T), dtype=torch.float32, device=x.device) if save else None
+            return ops.attn_fwd_kv(qkv[:, :D], kc[l], vc[l], cu, q_lens, kv_start, kv_len, H, lse=s.lse)
+        x, saved = self._layers(x, pos, out_rows, save, a8, fused, attend)
         if not save:
             return x
         kv = SimpleNamespace(kc=kc, vc=vc, acc=acc, kv_start=kv_start, kv_len=kv_len, kv_lens=list(kv_lens))
@@ -706,44 +685,24 @@ class LlamaCore:
         overlap the data-parallel all-reduce with the rest of the backward)."""
         if tape is None:
             raise RuntimeError("LlamaCore.backward: the forward ran without saving activations (no_grad / eval-only)")
-        saved, (pos, cu, seqlens) = tape[:2]
-        kv = tape[2] if len(tape) > 2 else None          # forward_suffix tape: attention over a KV cache
+        saved, (pos, cu, seqlens), kv = tape          # kv: the cache of a forward_suffix tape, None for a prompt forward
         d = self.d
         H = d.n_heads
         acc = not getattr(self.flat, "overwrite_layer_grads", False)
-
-        def add(g):
-            return g if acc else None
-
-        # Weight-gradient GEMMs on a SIDE stream (NAVILLM_WGRAD_STREAM=1): nothing downstream in the backward reads a weight
-        # gradient, so they can trail the dgrad chain: when one GEMM's last, partially filled wave of tiles leaves SMs idle, the
-        # other stream's kernel takes them.
         # deferred weight gradients (WgradStash): the four linears' wgrad operands are recorded, not launched
         defer = self.wgrad_stash is not None and self.wgrad_stash.begin(saved[0].x.shape[0], acc)   # the backward's rows
-        side = WGRAD_STREAM and dx.shape[0] >= 1024 and not defer
-        main = torch.cuda.current_stream() if side else None
-        ws = self._wgrad_stream() if side else None
 
-        def wgrad(a, b, grad, l, *, keep=()):
+        def wgrad(a, b, grad, l):
             out = getattr(self, grad)[l]
             if defer:
                 self.wgrad_stash.record(grad, l, a, b)
-                return
-            if not side:
-                ops.gemm(a, b, a_mn=True, b_mn=True, out=out, addend=add(out))
-                return
-            ev = torch.cuda.Event()
-            ev.record(main)
-            ws.wait_event(ev)
-            for t in (a, b) + tuple(keep):
-                t.record_stream(ws)                      # the caching allocator must not recycle them under the side stream
-            with torch.cuda.stream(ws):
-                ops.gemm(a, b, a_mn=True, b_mn=True, out=out, addend=add(out))
+            else:
+                ops.gemm(a, b, a_mn=True, b_mn=True, out=out, addend=out if acc else None)
 
         for l in range(d.n_layers - 1, -1, -1):
             lyr, s = self.model.layers[l], saved[l]
             # ---- MLP:  x_out = xm + down(swiglu(gate_up(rmsnorm2(xm)))) ----
-            if self.fused_epilogues and dx.shape[0] >= 1024 and d.inter % 32 == 0:
+            if dx.shape[0] >= 1024 and d.inter % 32 == 0:
                 dgu = ops.gemm_dswiglu(dx, self.wd[l], s.gu)                           # dgrad + SwiGLU' in the epilogue
             else:
                 dh = ops.gemm(dx, self.wd[l], b_mn=True)                               # [T,F]  dgrad
@@ -758,7 +717,7 @@ class LlamaCore:
             del dxn2
             # ---- attention:  xm = x + o_proj(attn(rope(qkv(rmsnorm1(x))))) ----
             dvec = None
-            if s.rows is None and self.fused_epilogues and dxm.shape[0] >= 1024 and d.head_dim == 128:
+            if s.rows is None and dxm.shape[0] >= 1024:
                 dao, dvec = ops.gemm_attnd(dxm, self.wo[l], s.ao)      # dgrad + the attention backward's D in the epilogue
             else:
                 dao = ops.gemm(dxm, self.wo[l], b_mn=True)
@@ -788,25 +747,11 @@ class LlamaCore:
             del dxn, dxm
             saved[l] = None
             if layer_done is not None:
-                if side:                                   # the layer's gradients are complete only when the side stream is
-                    ev = torch.cuda.Event()
-                    ev.record(ws)
-                    main.wait_event(ev)
                 layer_done(l)
-        if side:
-            ev = torch.cuda.Event()
-            ev.record(ws)
-            main.wait_event(ev)                            # whoever reads the gradients next is ordered after the wgrads
         if defer:
             self.wgrad_stash.commit()
         self.flat.overwrite_layer_grads = False
         return dx
-
-    def _wgrad_stream(self):
-        if getattr(self, "_ws", None) is None:
-            self._ws = torch.cuda.Stream()
-        return self._ws
-
 
     # -------------------------------------------------------------------------------------------------
     def decode_step(self, x: torch.Tensor, lens: torch.Tensor, kc: List[torch.Tensor], vc: List[torch.Tensor], beam=None) -> torch.Tensor:
@@ -826,10 +771,9 @@ class LlamaCore:
         # from a measured table (32-column tiles for the 4096-wide projections, 256 for gate|up: tools/midm_bench.py).
         # With an fp8 copy of the weights (set_fp8), the skinny GEMMs and, up to FP8_MAX_ROWS rows, nv_gemm_fp8w_bf16 stream
         # it instead: same bits as bf16 on W'.  generate() refuses a stale copy before it gets here.
-        bn = DECODE_BLOCK_N
-        skinny = bn == 0 and x.shape[0] <= 16
+        skinny = x.shape[0] <= 16
         fuse_mlp = skinny and d.inter % 64 == 0
-        f8 = self.fp8 if bn == 0 and x.shape[0] <= FP8_MAX_ROWS else None
+        f8 = self.fp8 if x.shape[0] <= FP8_MAX_ROWS else None
         if f8 is not None:
             if skinny:
                 lin = lambda a, w, addend=None: ops.gemm_skinny_fp8(a, *w, addend=addend)
@@ -842,10 +786,8 @@ class LlamaCore:
             if skinny:
                 lin = lambda a, w, addend=None: ops.gemm_skinny(a, w, addend=addend)
             else:
-                lin = lambda a, w, addend=None: ops.gemm(a, w, addend=addend, block_n=bn)
+                lin = lambda a, w, addend=None: ops.gemm(a, w, addend=addend)
         fp8_kv = is_fp8_kv(kc)
-        if (fp8_kv or beam is not None) and d.head_dim != 128:
-            raise NotImplementedError("the fp8 KV cache and beam search are built for head_dim = 128")
         for l, lyr in enumerate(self.model.layers):
             xn, _ = ops.rmsnorm_fwd(x, lyr.input_layernorm.weight.data, d.rms_eps)
             qkv = lin(xn, wqkv[l])
@@ -857,12 +799,8 @@ class LlamaCore:
                                                beam.src, beam.K, H)
             elif fp8_kv:                                                                 # same, quantizing the appended rows
                 ao = ops.decode_attn_rope_fp8(qkv, lens, self.cos, self.sin, kc[l][0], vc[l][0], kc[l][1], vc[l][1], H)
-            elif d.head_dim == 128:
-                ao = ops.decode_attn_rope(qkv, lens, self.cos, self.sin, kc[l], vc[l], H)   # RoPE + cache append + attention
             else:
-                ops.rope_(qkv, lens, self.cos, self.sin, 2 * H, d.head_dim)
-                ops.kv_append(qkv, lens, kc[l], vc[l])
-                ao = ops.decode_attn(qkv, kc[l], vc[l], lens, H)
+                ao = ops.decode_attn_rope(qkv, lens, self.cos, self.sin, kc[l], vc[l], H)   # RoPE + cache append + attention
             xm = lin(ao, wo[l], x)
             xn2, _ = ops.rmsnorm_fwd(xm, lyr.post_attention_layernorm.weight.data, d.rms_eps)
             if fuse_mlp and f8 is not None:

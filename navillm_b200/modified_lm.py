@@ -15,7 +15,6 @@ reference holds values computed from pad embeddings that nothing reads.
 from __future__ import annotations
 
 import collections
-import os
 import time
 import weakref
 from types import SimpleNamespace
@@ -28,7 +27,7 @@ import torch.nn as nn
 from . import llama as llama_mod
 from . import ops
 from . import trie as trie_mod
-from .llama import FlatParams, Fp8Weights, LlamaCore, LlamaDims, LlamaModelParams, WgradStash, _Linear
+from .llama import FlatParams, Fp8Weights, LlamaCore, LlamaDims, LlamaModelParams, WgradStash, _Linear, kv_cache
 from .parallel import GradSync
 from .tokenizer import HFTokenizerAdapter, SyntheticTokenizer
 
@@ -157,18 +156,8 @@ class PrefixKVCache:
         dev, d = lm._device(), lm.dims
         self.B, self.max_len, self.kv_dtype = batch_size, max_len, kv_dtype
         # zero-initialised: rows past a sequence's length are masked in the attention kernel but must stay finite
-        if kv_dtype == "fp8":
-            if d.head_dim != 128:
-                raise ValueError(f"PrefixKVCache: the fp8 cache needs head_dim 128 (got {d.head_dim})")
-
-            def layer():
-                return (torch.zeros((batch_size, max_len, d.hidden), dtype=torch.float8_e4m3fn, device=dev),
-                        torch.zeros((batch_size, max_len, d.n_heads), dtype=torch.int8, device=dev))
-        else:
-            def layer():
-                return torch.zeros((batch_size, max_len, d.hidden), dtype=bf16, device=dev)
-        self.kc = [layer() for _ in range(d.n_layers)]
-        self.vc = [layer() for _ in range(d.n_layers)]
+        self.kc = kv_cache(d, batch_size, max_len, kv_dtype, dev, zero=True)
+        self.vc = kv_cache(d, batch_size, max_len, kv_dtype, dev, zero=True)
         self.ids: List[np.ndarray] = [np.zeros(0, dtype=np.int64) for _ in range(batch_size)]
         self.off: List[Optional[int]] = [None] * batch_size
         self.stats = {"steps": 0, "tokens": 0, "tokens_encoded": 0}
@@ -864,7 +853,6 @@ class ModifiedLlamaForCausalLM(nn.Module):
         return prev
 
     # ---- generation (models/nav_model.py:324-338,388-399; HF GenerationMixin greedy / sampling) ----
-    decode_pdl = os.environ.get("NAVILLM_DECODE_PDL", "1") != "0"   # developer knob: 0 = plain stream-ordered launches
     max_decode_states = 2        # cached (KV buffers + captured decode graph) sets, least recently used evicted
 
     def _decode_state(self, B: int, Smax: int, key_extra: tuple, want_graph: bool):
@@ -883,13 +871,8 @@ class ModifiedLlamaForCausalLM(nn.Module):
             return st
         dev, d = self._device(), self.dims
         V = self.lm_head.weight.shape[0]
-        if self.kv_cache_dtype == "fp8":                          # (e4m3 bytes, int8 row exponents) per layer
-            cache = lambda: [(torch.empty((B, Smax, d.hidden), dtype=ops.fp8, device=dev),
-                              torch.empty((B, Smax, d.n_heads), dtype=torch.int8, device=dev)) for _ in range(d.n_layers)]
-        else:
-            cache = lambda: [torch.empty((B, Smax, d.hidden), dtype=bf16, device=dev) for _ in range(d.n_layers)]
         st = SimpleNamespace(
-            kc=cache(), vc=cache(),
+            kc=kv_cache(d, B, Smax, self.kv_cache_dtype, dev), vc=kv_cache(d, B, Smax, self.kv_cache_dtype, dev),
             logits=torch.empty((B, (V + 63) // 64 * 64), dtype=bf16, device=dev)[:, :V],
             next_ids=torch.empty((B,), dtype=torch.int32, device=dev),
             finished=torch.zeros((B,), dtype=torch.int32, device=dev),
@@ -908,14 +891,14 @@ class ModifiedLlamaForCausalLM(nn.Module):
         fp8_head = None
         if self.core.fp8 is not None:
             fp8_head = self._fp8.view([self.lm_head.weight], tuple(self.lm_head.weight.shape))
-        if B <= 16 and llama_mod.DECODE_BLOCK_N == 0 and fp8_head is not None:
+        if B <= 16 and fp8_head is not None:
             ops.gemm_skinny_fp8(hn, *fp8_head, out=out)
-        elif B <= llama_mod.FP8_MAX_ROWS and llama_mod.DECODE_BLOCK_N == 0 and fp8_head is not None:
+        elif B <= llama_mod.FP8_MAX_ROWS and fp8_head is not None:
             ops.gemm_fp8w(hn, *fp8_head, out=out)
-        elif B <= 16 and llama_mod.DECODE_BLOCK_N == 0:
+        elif B <= 16:
             ops.gemm_skinny(hn, self.lm_head.weight.data, out=out)
         else:
-            ops.gemm(hn, self.lm_head.weight.data, out=out, block_n=llama_mod.DECODE_BLOCK_N)
+            ops.gemm(hn, self.lm_head.weight.data, out=out)
 
     @staticmethod
     def _load_trie(st, table) -> tuple:
@@ -1097,7 +1080,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
             ev[1].record()
 
         def step():
-            with ops.pdl(self.decode_pdl):          # programmatic dependent launch along the whole decode chain
+            with ops.pdl():                         # programmatic dependent launch along the whole decode chain
                 xt = ops.embed_fwd(next_ids, E)
                 h = core.decode_step(xt, lens, kc, vc)
                 head(h)
@@ -1171,11 +1154,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
             return st
         dev, d = self._device(), self.dims
         V, R = self.lm_head.weight.shape[0], B * K
-        if self.kv_cache_dtype == "fp8":
-            cache = lambda rows, n: [(torch.empty((rows, n, d.hidden), dtype=ops.fp8, device=dev),
-                                      torch.empty((rows, n, d.n_heads), dtype=torch.int8, device=dev)) for _ in range(d.n_layers)]
-        else:
-            cache = lambda rows, n: [torch.empty((rows, n, d.hidden), dtype=bf16, device=dev) for _ in range(d.n_layers)]
+        cache = lambda rows, n: kv_cache(d, rows, n, self.kv_cache_dtype, dev)
         i32 = lambda *shape: torch.zeros(shape, dtype=torch.int32, device=dev)
         st = SimpleNamespace(
             pk=cache(B, Sp), pv=cache(B, Sp), kc=cache(R, G), vc=cache(R, G),
@@ -1242,7 +1221,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
         beam = SimpleNamespace(pk=st.pk, pv=st.pv, plens=st.plens, src=st.src, K=K)
 
         def step():
-            with ops.pdl(self.decode_pdl):
+            with ops.pdl():
                 xt = ops.embed_fwd(st.next_ids, E)
                 h = core.decode_step(xt, st.lens, st.kc, st.vc, beam=beam)
                 self._decode_head(h, st.logits)

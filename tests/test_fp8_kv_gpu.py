@@ -108,7 +108,7 @@ def test_kv_store_prefill_fp8_matches_quantizer(cuda_dev, H):
 
 
 def test_layer_call_prefill_fills_the_same_fp8_cache(cuda_dev, monkeypatch):
-    """kv_mode 3 of the layer call and the per-kernel prefill (kv_sink) write the same bytes and exponents."""
+    """kv_mode 3 of the layer call and the per-kernel prefill store write the same bytes and exponents."""
     from navillm_b200 import llama, ops
     from navillm_b200.modified_lm import PackedPrompt
     g, cfg, tok, model = _golden(cuda_dev)

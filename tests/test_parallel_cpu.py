@@ -197,3 +197,13 @@ def test_fused_views_are_identity_checked():
     bad = FlatParams(list(m2.parameters()), torch.device("cpu"))
     with pytest.raises(RuntimeError):
         bad.view([m2.layers[0].mlp.gate_proj.weight, m2.layers[0].mlp.up_proj.weight], (2 * d.inter, d.hidden))
+
+
+def test_decoder_stack_needs_head_dim_128():
+    """The attention kernels are built for head_dim 128: a LlamaCore of any other head size is refused when it is built."""
+    import pytest
+    from navillm_b200.llama import FlatParams, LlamaCore, LlamaDims, LlamaModelParams
+    d = LlamaDims(hidden=128, n_layers=1, n_heads=2, inter=256, vocab=16)
+    m = LlamaModelParams(d)
+    with pytest.raises(ValueError, match="head_dim 128"):
+        LlamaCore(d, m, FlatParams(m.flat_order(), torch.device("cpu")))
