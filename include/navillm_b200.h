@@ -304,6 +304,14 @@ int nv_add_int(int* x, int n, int delta, void* stream);
  * finished / eos / pad handling as nv_argmax_masked.  probs_out: optional fp32 [B, V] copy of the distribution drawn from. */
 int nv_sample_topk(const void* logits, int64_t ld, int V, const int* special, int n_special, int* finished, int eos_id, int pad_id,
                    int stop_on_eos, float temperature, int top_k, const float* u, int* next, float* probs_out, int B, void* stream);
+/* nv_sample_topk with HF's TopPLogitsWarper between top-k and the softmax: the top-k survivors sorted by (score, token index)
+ * ascending, their bf16 probabilities summed in that order (fp32, each partial rounded to bf16), and every position whose sum
+ * is <= bf16(1 - top_p) removed, the largest always kept; then a fresh softmax over the rest.  top_p in [0, 1] (else
+ * NV_ERR_BAD_ARG); top_p = 1 is nv_sample_topk, bit for bit.  Above 1024 survivors (top_k = 0) the sum is the exact prefix
+ * sum rounded to bf16 instead (see csrc/decode.cu). */
+int nv_sample(const void* logits, int64_t ld, int V, const int* special, int n_special, int* finished, int eos_id, int pad_id,
+              int stop_on_eos, float temperature, int top_k, float top_p, const float* u, int* next, float* probs_out, int B,
+              void* stream);
 /* Trie-constrained decoding (TrieLogitsProcessor, models/modified_lm.py:10-30, reached from EQA validation,
  * tasks/agents/mp3d_agent.py:545-584), on the device.  The trie is flattened to CSR: node_ptr [n_nodes + 2], child_tok [E]
  * (ascending within a node, every id in [0, V)), child_node [E]; node 0 is the root, node n_nodes an extra childless dead node.

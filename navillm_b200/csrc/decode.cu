@@ -581,7 +581,7 @@ __global__ void add_int_kernel(int* __restrict__ x, int n, int delta) {
 // ---- sampled decoding (HF GenerationMixin.sample as the reference reaches it with do_sample=True, tasks/agents/llava.py:58-62
 // -> models/nav_model.py:388-396): next-token scores -> TemperatureLogitsWarper (scores / T, in the logits' dtype: bf16) ->
 // TopKLogitsWarper (transformers' generation default top_k = 50: every score strictly below the k-th largest becomes -inf,
-// ties at the k-th value stay) -> softmax (fp32 inside, rounded to bf16) -> one multinomial draw.  One CTA per row: the
+// ties at the k-th value stay) -> TopPLogitsWarper when top_p < 1 (see SMP_LIST) -> softmax (fp32 inside, rounded to bf16) -> one multinomial draw.  One CTA per row: the
 // row's scores live in shared memory, the k-th largest is found exactly with two 8-bit radix passes over the 16 significant
 // bits of a bf16 value, and the draw is the inverse CDF (token order) of the bf16 probabilities at the uniform number u[b]
 // the host supplies (torch.rand: the torch CUDA generator stays the seed authority, like torch.multinomial in the reference).
@@ -613,21 +613,78 @@ __device__ __forceinline__ void smp_pick_bin(const int* hist, int want, int& bin
   __syncthreads();
 }
 
+// sum of one float per thread over the CTA (SMP_THREADS = 32 warps): warp butterflies, then the 32 warp sums in warp order
+__device__ __forceinline__ float smp_cta_sum(float part, float* red) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+  if (lane == 0) red[w] = part;
+  __syncthreads();
+  float s = red[lane];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  __syncthreads();
+  return s;
+}
+
+// exclusive prefix of one int per thread over the CTA, in thread order
+__device__ __forceinline__ int smp_cta_exclusive(int x, int* ired) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  int incl = x;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int t = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += t;
+  }
+  if (lane == 31) ired[w] = incl;
+  __syncthreads();
+  const int ws = ired[lane];
+  int wincl = ws;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int t = __shfl_up_sync(0xffffffffu, wincl, o);
+    if (lane >= o) wincl += t;
+  }
+  const int wprefix = __shfl_sync(0xffffffffu, wincl - ws, w);
+  __syncthreads();
+  return wprefix + incl - x;
+}
+
+// Top-p (TopPLogitsWarper of transformers 4.28, after top-k): the survivors of top-k sorted by (score, token index) ascending,
+// their bf16 softmax probabilities p summed in that order, and every position whose bf16-rounded running sum is <= p_thr
+// (= bf16(1 - top_p)) removed, the last (largest) always kept.  Up to SMP_LIST survivors (top_k = 50 plus ties) are sorted
+// and walked with an fp32 running sum (torch's CPU cumsum of a bf16 tensor).  Above that (top_k = 0: the full vocabulary)
+// two radix passes over the 16-bit key sum the probability mass per key exactly (fixed point, 2^-60) to find the key whose
+// prefix crosses the threshold; there the running sum is the exact prefix rounded to bf16, which differs from the fp32
+// walk only within fp32 summation noise.  Scores are bf16 values, so all tokens of one key share one p, and only the
+// order inside the crossing key needs the token index: its lowest indices go first (a stable ascending sort).
+constexpr int SMP_LIST = 1024;
+constexpr double SMP_FIX = 1152921504606846976.0;      // 2^60: p < 2 always, so a sum of p fits 64 bits
+
+__device__ __forceinline__ unsigned long long smp_fix(float p) { return (unsigned long long)((double)p * SMP_FIX); }
+__device__ __forceinline__ float smp_unfix_bf16(unsigned long long x) { return __bfloat162float(__double2bfloat16((double)x / SMP_FIX)); }
+
 __global__ void __launch_bounds__(SMP_THREADS) sample_topk_kernel(const __nv_bfloat16* __restrict__ logits, int64_t ld, int V,
                                                                   const int* __restrict__ special, int n_special,
                                                                   int* __restrict__ finished, int eos_id, int pad_id, int stop_on_eos,
-                                                                  float temperature, int top_k, const float* __restrict__ u,
-                                                                  int* __restrict__ next, float* __restrict__ probs_out) {
+                                                                  float temperature, int top_k, int use_top_p, float p_thr,
+                                                                  const float* __restrict__ u, int* __restrict__ next,
+                                                                  float* __restrict__ probs_out) {
   extern __shared__ float sc[];                              // [V] scores, then probabilities
   __shared__ int hist[256];
   __shared__ float red[32];
   __shared__ int s_special[MAX_SPECIAL];
   __shared__ int s_idx, s_last;
+  __shared__ uint32_t s_lst[SMP_LIST], s_srt[SMP_LIST];     // top-p: (key << 16 | slot) of the survivors of top-k, sorted
+  __shared__ float s_lv[SMP_LIST];                           // their scores, by slot
+  __shared__ unsigned long long s_mass[256];
+  __shared__ int s_n, s_ck, s_cr, s_ci, s_bin;
+  __shared__ unsigned long long s_acc;
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   const int ns = n_special;
   if (tid < ns) s_special[tid] = special[tid];
   if (tid < 256) hist[tid] = 0;
-  if (tid == 0) { s_idx = V; s_last = -1; }
+  if (tid == 0) { s_idx = V; s_last = -1; s_n = 0; s_ck = 0; s_cr = 0; s_ci = 0; }
   __syncthreads();
   const __nv_bfloat16* row = logits + (int64_t)b * ld;
   // 1. scores = bf16(logit / T), special tokens -inf (models/modified_lm.py:122-124); histogram of the high key byte
@@ -665,21 +722,139 @@ __global__ void __launch_bounds__(SMP_THREADS) sample_topk_kernel(const __nv_bfl
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
   __syncthreads();
-  float part = 0.f;
-  for (int c = tid; c < V; c += SMP_THREADS) {
-    const float v = sc[c];
-    const float e = (smp_key16(v) >= thr_key && v > -INFINITY) ? expf(v - mx) : 0.f;
-    sc[c] = e;
-    part += e;
+  float denom;
+  if (!use_top_p) {
+    float part = 0.f;
+    for (int c = tid; c < V; c += SMP_THREADS) {
+      const float v = sc[c];
+      const float e = (smp_key16(v) >= thr_key && v > -INFINITY) ? expf(v - mx) : 0.f;
+      sc[c] = e;
+      part += e;
+    }
+    denom = smp_cta_sum(part, red);
+  } else {
+    // 3a. the same denominator with the scores kept in sc; the survivors of top-k go to the list while it has room
+    float part = 0.f;
+    for (int c = tid; c < V; c += SMP_THREADS) {
+      const float v = sc[c];
+      const uint32_t key = smp_key16(v);
+      const bool kept = key >= thr_key && v > -INFINITY;
+      // one shared-memory atomic per warp and iteration, not per survivor (top_k = 0 keeps the whole row)
+      const unsigned act = __activemask();
+      const unsigned kb = __ballot_sync(act, kept);
+      const int leader = __ffs(act) - 1;
+      int base = 0;
+      if (lane == leader && kb) base = atomicAdd(&s_n, __popc(kb));
+      base = __shfl_sync(act, base, leader);
+      if (kept) {
+        part += expf(v - mx);
+        const int slot = base + __popc(kb & ((1u << lane) - 1u));
+        if (slot < SMP_LIST) { s_lst[slot] = (key << 16) | (uint32_t)slot; s_lv[slot] = v; }
+      }
+    }
+    denom = smp_cta_sum(part, red);
+    const int n = s_n;
+    auto prob = [&](float v) { return bf16_round(expf(v - mx) / denom); };
+    // 3b. the cut: tie group s_ck, of which the s_cr lowest token indices are removed (everything below it is removed)
+    if (n <= SMP_LIST) {
+      if (tid < n) {                                         // rank sort: the list entries are distinct
+        const uint32_t x = s_lst[tid];
+        int r = 0;
+        for (int j = 0; j < n; ++j) r += s_lst[j] < x;
+        s_srt[r] = x;
+      }
+      __syncthreads();
+      if (tid == 0 && n > 0) {
+        float run = 0.f;
+        int m = 0;
+        for (; m < n - 1; ++m) {
+          run += prob(s_lv[s_srt[m] & 0xffffu]);
+          if (bf16_round(run) > p_thr) break;
+        }
+        const uint32_t ck = s_srt[m] >> 16;
+        int first = m;
+        while (first > 0 && (s_srt[first - 1] >> 16) == ck) --first;
+        s_ck = (int)ck;
+        s_cr = m - first;
+      }
+    } else {
+      // hist / s_mass: count and fixed-point mass per high key byte, then per low byte of the crossing high byte
+      for (int pass = 0; pass < 2; ++pass) {
+        if (tid < 256) { hist[tid] = 0; s_mass[tid] = 0ull; }
+        __syncthreads();
+        for (int c = tid; c < V; c += SMP_THREADS) {
+          const float v = sc[c];
+          const uint32_t key = smp_key16(v);
+          if (key >= thr_key && v > -INFINITY && (pass == 0 || (int)(key >> 8) == s_bin)) {
+            const int bin = pass == 0 ? (int)(key >> 8) : (int)(key & 255u);
+            atomicAdd(&hist[bin], 1);
+            atomicAdd(&s_mass[bin], smp_fix(prob(v)));
+          }
+        }
+        __syncthreads();
+        if (tid == 0) {
+          unsigned long long acc = pass == 0 ? 0ull : s_acc, at = acc;   // at: the mass below bin `last`
+          int cross = -1, last = -1;
+          for (int i = 0; i < 256 && cross < 0; ++i) {
+            if (hist[i] == 0) continue;
+            last = i;
+            at = acc;
+            if (smp_unfix_bf16(acc + s_mass[i]) > p_thr) cross = i;
+            else acc += s_mass[i];
+          }
+          const int bin = last;                                  // the crossing bin, or the top one when none crosses
+          acc = at;
+          if (pass == 0) {
+            s_bin = bin;
+            s_acc = acc;
+          } else {
+            const int ng = hist[bin];
+            const unsigned long long pg = s_mass[bin] / (unsigned long long)ng;   // every token of one key has the same p
+            int lo = 0, hi = ng - 1;                             // the first group member whose running sum exceeds p_thr
+            if (cross >= 0) {
+              while (lo < hi) {
+                const int mid = (lo + hi) >> 1;
+                if (smp_unfix_bf16(acc + (unsigned long long)(mid + 1) * pg) > p_thr) hi = mid;
+                else lo = mid + 1;
+              }
+            }
+            s_ck = (s_bin << 8) | bin;
+            s_cr = cross >= 0 ? lo : ng - 1;
+          }
+        }
+        __syncthreads();
+      }
+    }
+    __syncthreads();
+    // 3c. the token index where the cut falls: the s_cr-th (0-based) token of key s_ck in index order
+    const uint32_t ck = (uint32_t)s_ck;
+    const int cr = s_cr;
+    {
+      const int CH = (V + SMP_THREADS - 1) / SMP_THREADS;
+      const int c0 = min(tid * CH, V), c1 = min(c0 + CH, V);
+      int cnt = 0;
+      for (int c = c0; c < c1; ++c) cnt += smp_key16(sc[c]) == ck;
+      const int before = smp_cta_exclusive(cnt, hist);
+      if (before <= cr && cr < before + cnt) {
+        int k = before;
+        for (int c = c0; c < c1; ++c)
+          if (smp_key16(sc[c]) == ck && k++ == cr) { s_ci = c; break; }
+      }
+      __syncthreads();
+    }
+    const int ci = s_ci;
+    // 3d. a fresh softmax over the survivors of top-p (the maximum always survives, so mx stands)
+    part = 0.f;
+    for (int c = tid; c < V; c += SMP_THREADS) {
+      const float v = sc[c];
+      const uint32_t key = smp_key16(v);
+      const bool keep = key >= thr_key && v > -INFINITY && (key > ck || (key == ck && c >= ci));
+      const float e = keep ? expf(v - mx) : 0.f;
+      sc[c] = e;
+      part += e;
+    }
+    denom = smp_cta_sum(part, red);
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
-  if (lane == 0) red[w] = part;
-  __syncthreads();
-  float denom = red[lane];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) denom += __shfl_xor_sync(0xffffffffu, denom, o);
-  __syncthreads();
   // 4. probabilities + inverse CDF in token order: thread t owns the contiguous chunk [t*CH, (t+1)*CH)
   const int CH = (V + SMP_THREADS - 1) / SMP_THREADS;
   const int c0 = min(tid * CH, V), c1 = min(c0 + CH, V);
@@ -1113,24 +1288,35 @@ int nv_argmax_masked(const void* logits, int64_t ld, int V, const int* special, 
   return NV_OK;
 }
 
-// Sampled next token (HF sample: temperature -> top-k -> softmax -> multinomial); see sample_topk_kernel.  logits [B, V] bf16,
-// u [B] uniform numbers in [0, 1), probs_out: optional fp32 [B, V] copy of the sampling distribution (tests).
-int nv_sample_topk(const void* logits, int64_t ld, int V, const int* special, int n_special, int* finished, int eos_id, int pad_id,
-                   int stop_on_eos, float temperature, int top_k, const float* u, int* next, float* probs_out, int B, void* stream) {
-  NV_REQUIRE(logits && u && next && finished && V > 0 && temperature > 0.f, "nv_sample_topk: bad arguments (temperature must be > 0)");
-  NV_REQUIRE(n_special >= 0 && n_special <= MAX_SPECIAL, "nv_sample_topk: n_special=%d out of range (max %d)", n_special,
-             MAX_SPECIAL);
-  NV_REQUIRE((int64_t)V * 4 <= 200 * 1024, "nv_sample_topk: vocabulary of %d does not fit the shared-memory score row", V);
+// Sampled next token (HF sample: temperature -> top-k -> top-p -> softmax -> multinomial); see sample_topk_kernel.  logits
+// [B, V] bf16, u [B] uniform numbers in [0, 1), probs_out: optional fp32 [B, V] copy of the sampling distribution (tests).
+// top_p in [0, 1]; 1 is off, as in HF, which only adds the top-p warper below 1.
+int nv_sample(const void* logits, int64_t ld, int V, const int* special, int n_special, int* finished, int eos_id, int pad_id,
+              int stop_on_eos, float temperature, int top_k, float top_p, const float* u, int* next, float* probs_out, int B,
+              void* stream) {
+  NV_REQUIRE(logits && u && next && finished && V > 0 && temperature > 0.f, "nv_sample: bad arguments (temperature must be > 0)");
+  NV_REQUIRE(top_p >= 0.f && top_p <= 1.f, "nv_sample: top_p=%g outside [0, 1]", (double)top_p);
+  NV_REQUIRE(n_special >= 0 && n_special <= MAX_SPECIAL, "nv_sample: n_special=%d out of range (max %d)", n_special, MAX_SPECIAL);
+  NV_REQUIRE((int64_t)V * 4 <= 200 * 1024, "nv_sample: vocabulary of %d does not fit the shared-memory score row", V);
   if (B == 0) return NV_OK;
   static bool attr_set = false;
   if (!attr_set) {
     NV_CUDA(cudaFuncSetAttribute(sample_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     attr_set = true;
   }
+  // TopPLogitsWarper compares the bf16 running sum with the Python scalar 1 - top_p, which takes the bf16 dtype
+  const float p_thr = __bfloat162float(__float2bfloat16_rn((float)(1.0 - (double)top_p)));
   sample_topk_kernel<<<B, SMP_THREADS, (size_t)V * 4, S_(stream)>>>(CBF(logits), ld, V, special, n_special, finished, eos_id, pad_id,
-                                                                     stop_on_eos, temperature, top_k, u, next, probs_out);
+                                                                     stop_on_eos, temperature, top_k, top_p < 1.f ? 1 : 0, p_thr, u,
+                                                                     next, probs_out);
   NV_LAUNCH_CHECK();
   return NV_OK;
+}
+
+int nv_sample_topk(const void* logits, int64_t ld, int V, const int* special, int n_special, int* finished, int eos_id, int pad_id,
+                   int stop_on_eos, float temperature, int top_k, const float* u, int* next, float* probs_out, int B, void* stream) {
+  return nv_sample(logits, ld, V, special, n_special, finished, eos_id, pad_id, stop_on_eos, temperature, top_k, 1.f, u, next,
+                   probs_out, B, stream);
 }
 
 // Trie mask of the next-token logits (see trie_mask_kernel).  logits [B, V] bf16 (ld), out [B, V] bf16 (ldo % 8 == 0, 16-byte

@@ -855,16 +855,20 @@ class ModifiedLlamaForCausalLM(nn.Module):
     # ---- generation (models/nav_model.py:324-338,388-399; HF GenerationMixin greedy / sampling) ----
     max_decode_states = 2        # cached (KV buffers + captured decode graph) sets, least recently used evicted
 
-    def _decode_state(self, B: int, Smax: int, key_extra: tuple, want_graph: bool):
+    def _decode_state(self, B: int, Smax: int, key_extra: tuple, want_graph: bool, prompts: Optional[tuple] = None):
         """Persistent per-shape decode state: the contiguous KV cache [B, Smax, D] per layer (in ``kv_cache_dtype``; the caller
         puts that format in ``key_extra``, so a graph is never replayed over the other one), the step's I/O buffers and --
         once captured -- the CUDA graph of ONE decode step.  Capturing and instantiating the ~260-node graph costs more than
         the 127 replays of a C3 generation save, so it is done once per (batch, cache length, stop rule, decoding mode and
         the scalars the step bakes in) and reused by every later ``generate`` call (evaluation loops call generate with the
         same shapes over and over).  The trie-constrained modes keep their flattened trie in ``trie_buf`` (see
-        ``_load_trie``), sampled modes their uniform numbers in ``u``."""
+        ``_load_trie``), sampled modes their uniform numbers in ``u``.
+
+        ``prompts = (P, Sp)`` (several samples per prompt): the B rows are B / P samples of each of P prompts; the prompt
+        keys go to a prompt cache ``pk`` / ``pv`` [P, Sp, D] that the samples of a prompt share (``plens`` keys each), and
+        kc / vc hold only the generated keys, read through the identity source table ``src`` (the beam-search attention)."""
         states = self.__dict__.setdefault("_decode_states", collections.OrderedDict())
-        key = (B, Smax) + key_extra
+        key = (B, Smax, prompts) + key_extra
         st = states.get(key) if want_graph else None
         if st is not None:
             states.move_to_end(key)
@@ -878,6 +882,11 @@ class ModifiedLlamaForCausalLM(nn.Module):
             finished=torch.zeros((B,), dtype=torch.int32, device=dev),
             lens=torch.zeros((B,), dtype=torch.int32, device=dev), graph=None,
             u=None, masked=None, node=None, miss=None, trie_buf=None, trie_cap=(0, 0))
+        if prompts is not None:
+            P, Sp = prompts
+            st.pk, st.pv = kv_cache(d, P, Sp, self.kv_cache_dtype, dev), kv_cache(d, P, Sp, self.kv_cache_dtype, dev)
+            st.plens = torch.zeros((P,), dtype=torch.int32, device=dev)
+            st.src = torch.arange(B, dtype=torch.int32, device=dev)[:, None].expand(B, Smax).contiguous()
         if want_graph:
             states[key] = st
             while len(states) > self.max_decode_states:
@@ -932,7 +941,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
 
         ``do_sample=True`` follows HF ``sample`` as the reference reaches it (tasks/agents/llava.py:58-62): logits
         processors, then temperature and top-k (``top_k=50`` is transformers' generation default, which the reference
-        never overrides), bf16 softmax, one multinomial draw per row - all in ``nv_sample_topk``; the uniform numbers
+        never overrides), bf16 softmax, one multinomial draw per row - all in ``nv_sample``; the uniform numbers
         are one [B] draw per token from the default CUDA generator, so ``torch.manual_seed`` makes a run reproducible,
         and the graph replays draw the same numbers as ``use_cuda_graph=False``.
 
@@ -943,23 +952,40 @@ class ModifiedLlamaForCausalLM(nn.Module):
         only a degenerate row can produce) run the host ``TrieLogitsProcessor`` instead - the miss case reruns the whole
         call, with the CUDA RNG state restored, and discards the device result.
 
+        ``top_p < 1`` adds HF's TopPLogitsWarper after top-k in every sampled mode (``nv_sample``); greedy and beam calls
+        ignore it, as HF does.
+
         ``num_beams > 1`` is HF beam search as transformers 4.28 (the reference's pin) runs it, ``length_penalty``,
         ``early_stopping`` and ``num_return_sequences`` included; see ``_generate_beam``.  Returns [B * num_return_sequences,
         L] ids.  Beam sampling, group beam search, ``trie=`` / ``logits_processor=`` with beams and more return sequences than
-        beams raise ``NotImplementedError``."""
+        beams raise ``NotImplementedError``.
+
+        ``do_sample=True, num_return_sequences=N`` draws N samples per prompt: [B * N, L] ids, row b * N + j a sample of
+        prompt b (HF's order).  Each prompt is prefilled once and its N rows share its KV cache (``_generate``); the tokens
+        are those of the same call on the prompts repeated N times.  With ``trie=`` / ``logits_processor=``, and without
+        ``do_sample``, N > 1 raises ``NotImplementedError``."""
         if num_beam_groups is not None and num_beam_groups > 1:
             raise NotImplementedError("generate(num_beam_groups > 1): group (diverse) beam search is not built")
-        if num_return_sequences > max(1, num_beams):
-            raise NotImplementedError(f"generate(num_return_sequences={num_return_sequences}) needs as many beams "
-                                      f"(num_beams={num_beams}): sampled multi-sequence generation is not built")
+        top_p = 1.0 if top_p is None else float(top_p)
+        if not 0.0 <= top_p <= 1.0:
+            raise ValueError(f"generate(top_p={top_p}): top_p must lie in [0, 1]")
+        n_seq = int(num_return_sequences)
         if num_beams > 1:
+            if num_return_sequences > num_beams:
+                raise NotImplementedError(f"generate(num_return_sequences={num_return_sequences}) needs as many beams "
+                                          f"(num_beams={num_beams})")
             if do_sample:
                 raise NotImplementedError("generate(num_beams > 1, do_sample=True): beam sampling is not built")
             if trie is not None or logits_processor:
                 raise NotImplementedError("generate(num_beams > 1) with trie= / logits_processor=: the processors keep per-row "
                                           "state that reordering the beams would scramble")
-        if top_p is not None and top_p < 1.0:
-            raise NotImplementedError("generate(top_p < 1) is not built: the reference never sets it (HF default 1.0)")
+        elif n_seq > 1:
+            if not do_sample:
+                raise NotImplementedError(f"generate(num_return_sequences={n_seq}) without beams needs do_sample=True: greedy "
+                                          "search returns one sequence per prompt")
+            if trie is not None or logits_processor:
+                raise NotImplementedError(f"generate(num_return_sequences={n_seq}, do_sample=True) with trie= / "
+                                          "logits_processor=: the host processors have no per-sample expansion")
         if do_sample and not temperature > 0:
             raise ValueError("generate(do_sample=True) needs temperature > 0")
         self._ensure()
@@ -973,7 +999,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
                                        stats)
         procs = list(logits_processor or [])
         args = (input_ids, attention_mask, cand_vis, hist_vis, obj_vis, max_new_tokens, do_sample, temperature, eos, pad,
-                stop_on_eos, use_cuda_graph, stats, top_k)
+                stop_on_eos, use_cuda_graph, stats, top_k, top_p, max(1, n_seq))
         table, path = None, None
         if trie is not None and not procs:
             t0 = time.perf_counter()
@@ -997,9 +1023,14 @@ class ModifiedLlamaForCausalLM(nn.Module):
         return out
 
     def _generate(self, input_ids, attention_mask, cand_vis, hist_vis, obj_vis, max_new_tokens, do_sample, temperature, eos, pad,
-                  stop_on_eos, use_cuda_graph, stats, top_k, *, procs, table):
+                  stop_on_eos, use_cuda_graph, stats, top_k, top_p, n_seq, *, procs, table):
         """``generate`` with the host processors ``procs`` (the host path when not empty) or the flattened trie ``table``
-        walked on the device; returns None when the device walk reported a miss."""
+        walked on the device; returns None when the device walk reported a miss.
+
+        ``n_seq`` > 1 (sampling without processors): the prefill runs once per prompt into the prompt cache of
+        ``_decode_state(prompts=)``, its last hidden row is repeated for the n_seq rows of the prompt, and the decode steps
+        run over all B * n_seq rows with the beam-search attention over an identity source table, so no K/V is copied.
+        The visual tokens of prompt b reach all n_seq samples of prompt b."""
         dev = self._device()
         core, d = self.core, self.dims
         ev = None
@@ -1009,16 +1040,27 @@ class ModifiedLlamaForCausalLM(nn.Module):
         pp = PackedPrompt(input_ids, attention_mask, self, dev, generate_positions=True)
         vis = self.cat_vis(cand_vis, hist_vis, obj_vis, pp)
         B = pp.B
+        R = B * n_seq                                             # decode rows
         need_host = bool(procs)                                   # processors walk the generated ids on the host
         graphed = use_cuda_graph and not need_host
         mode = ("trie+sample" if do_sample else "trie") if table is not None else ("sample" if do_sample else "greedy")
-        Smax = (max(pp.seqlens) + max_new_tokens + 127) // 128 * 128          # bucketed: more reuse of the cached state
         key = (int(eos), int(pad), bool(stop_on_eos), mode, float(temperature) if do_sample else None,
-               int(top_k) if do_sample else None, table.eos if table is not None else None, self.kv_cache_dtype)
-        st = self._decode_state(B, Smax, key, graphed)
+               int(top_k) if do_sample else None, float(top_p) if do_sample else None, table.eos if table is not None else None,
+               self.kv_cache_dtype)
+        shared = n_seq > 1
+        if shared:                                                # prompt cache per prompt + generated keys per row
+            Sp = (max(pp.seqlens) + 127) // 128 * 128
+            Smax = (max_new_tokens + 127) // 128 * 128
+            st = self._decode_state(R, Smax, key, graphed, prompts=(B, Sp))
+            st.plens.copy_(torch.tensor(pp.seqlens, dtype=torch.int32), non_blocking=True)
+            beam = SimpleNamespace(pk=st.pk, pv=st.pv, plens=st.plens, src=st.src, K=n_seq)
+        else:
+            Smax = (max(pp.seqlens) + max_new_tokens + 127) // 128 * 128      # bucketed: more reuse of the cached state
+            st = self._decode_state(B, Smax, key, graphed)
+            beam = None
         kc, vc, logits, next_ids, finished, lens = st.kc, st.vc, st.logits, st.next_ids, st.finished, st.lens
         if do_sample and not need_host and st.u is None:
-            st.u = torch.empty((B,), dtype=torch.float32, device=dev)
+            st.u = torch.empty((R,), dtype=torch.float32, device=dev)
         if table is not None:
             if st.masked is None:
                 V = logits.shape[1]
@@ -1027,11 +1069,14 @@ class ModifiedLlamaForCausalLM(nn.Module):
                 st.miss = torch.zeros((1,), dtype=torch.int32, device=dev)
             trie_csr = self._load_trie(st, table)
         finished.zero_()
-        lens.copy_(torch.tensor(pp.seqlens, dtype=torch.int32), non_blocking=True)
+        lens.copy_(torch.tensor(pp.seqlens, dtype=torch.int32).repeat_interleave(n_seq), non_blocking=True)
 
         E = self.model.embed_tokens.weight.data
         x = ops.embed_fwd(pp.ids, E, pp.vis_src if vis is not None else None, vis)
-        hid_last, _ = core.forward(x, pp.pos, pp.cu, pp.seqlens, save=False, kv_store=(kc, vc), out_rows=pp.last_rows)
+        hid_last, _ = core.forward(x, pp.pos, pp.cu, pp.seqlens, save=False, kv_store=(st.pk, st.pv) if shared else (kc, vc),
+                                   out_rows=pp.last_rows)
+        if shared:                                                # the n_seq samples of a prompt start from its last row
+            hid_last = hid_last.repeat_interleave(n_seq, dim=0)
         special = self.special_ids_dev
 
         head = lambda h_rows: self._decode_head(h_rows, logits)
@@ -1043,8 +1088,8 @@ class ModifiedLlamaForCausalLM(nn.Module):
             for proc in procs:
                 lg = proc(torch.tensor(all_ids_host, device=dev), lg)
             if do_sample:
-                ops.sample_topk(lg.to(torch.bfloat16), special, finished, eos, pad, stop_on_eos, temperature, top_k,
-                                torch.rand(B, device=dev, dtype=torch.float32), next_ids)
+                ops.sample(lg.to(torch.bfloat16), special, finished, eos, pad, stop_on_eos, temperature, top_k, top_p,
+                           torch.rand(B, device=dev, dtype=torch.float32), next_ids)
                 return
             nxt = lg.argmax(dim=-1)
             fin = finished.bool()
@@ -1061,8 +1106,8 @@ class ModifiedLlamaForCausalLM(nn.Module):
                 ops.trie_mask(logits, st.masked, *trie_csr, table.eos, special, st.node, next_ids if advance else None, st.miss)
                 src = st.masked
             if do_sample:
-                st.u.uniform_()                                   # = torch.rand(B): the same numbers, into a static buffer
-                ops.sample_topk(src, special, finished, eos, pad, stop_on_eos, temperature, top_k, st.u, next_ids)
+                st.u.uniform_()                                   # = torch.rand(R): the same numbers, into a static buffer
+                ops.sample(src, special, finished, eos, pad, stop_on_eos, temperature, top_k, top_p, st.u, next_ids)
             else:
                 ops.argmax_masked(src, special, finished, eos, pad, stop_on_eos, next_ids)
 
@@ -1082,7 +1127,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
         def step():
             with ops.pdl():                         # programmatic dependent launch along the whole decode chain
                 xt = ops.embed_fwd(next_ids, E)
-                h = core.decode_step(xt, lens, kc, vc)
+                h = core.decode_step(xt, lens, kc, vc, beam=beam)
                 head(h)
                 ops.add_int_(lens, 1)
                 if not need_host:
@@ -1127,7 +1172,8 @@ class ModifiedLlamaForCausalLM(nn.Module):
             torch.cuda.synchronize()
             n_dec = len(out_tokens) - 1
             stats.update({"prefill_ms": ev[0].elapsed_time(ev[1]), "decode_ms": ev[1].elapsed_time(ev[2]) if n_dec else None,
-                          "decode_steps": n_dec, "graph_replays": replays, "kv_rows": Smax, "prompt_lens": list(pp.seqlens)})
+                          "decode_steps": n_dec, "graph_replays": replays, "kv_rows": Smax + (Sp if shared else 0),
+                          "prompt_lens": list(pp.seqlens)})
         if miss:
             return None
         new = torch.stack(out_tokens, dim=1).to(torch.int64)
@@ -1137,7 +1183,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
             if bool(is_eos.any(dim=1).all()):
                 last = int(is_eos.float().argmax(dim=1).max())        # first EOS per row; the slowest row decides
                 new = new[:, :last + 1]
-        return torch.cat([input_ids.to(dev), new], dim=1)
+        return torch.cat([input_ids.to(dev).repeat_interleave(n_seq, dim=0), new], dim=1)
 
     # ---- beam search (HF GenerationMixin.beam_search / BeamSearchScorer, transformers 4.28 as the reference pins it) ----
     BEAM_MAX = 8

@@ -845,6 +845,19 @@ def sample_topk(logits, special, finished, eos_id, pad_id, stop_on_eos, temperat
     return next_ids
 
 
+def sample(logits, special, finished, eos_id, pad_id, stop_on_eos, temperature, top_k, top_p, u, next_ids, probs_out=None):
+    """``sample_topk`` with top-p filtering after top-k (nv_sample); ``top_p`` in [0, 1], 1 is off."""
+    B, V = logits.shape
+    assert logits.dtype == bf16 and logits.stride(1) == 1 and u.dtype == torch.float32 and u.numel() == B
+    assert next_ids.dtype == torch.int32 and finished.dtype == torch.int32
+    if probs_out is not None:
+        assert probs_out.dtype == torch.float32 and probs_out.shape == (B, V) and probs_out.is_contiguous()
+    check(_lib.load().nv_sample(ptr(logits), i64(logits.stride(0)), i32(V), ptr(special), i32(special.numel()), ptr(finished),
+                                i32(eos_id), i32(pad_id), i32(1 if stop_on_eos else 0), f32(temperature), i32(top_k), f32(top_p),
+                                ptr(u), ptr(next_ids), ptr(probs_out), i32(B), stream_ptr()), "nv_sample")
+    return next_ids
+
+
 def trie_mask(logits, out, node_ptr, child_tok, child_node, n_nodes, leaf_tok, special, state, last, miss):
     """out = logits masked to the tokens the trie allows per row (nv_trie_mask); advances ``state`` by ``last`` first
     unless ``last`` is None.  logits / out [B, V] bf16, state / last int32 [B], miss int32 [1] (set on a miss, never
