@@ -284,6 +284,28 @@ int nv_decode_attn_rope_fp8(const void* qkv, int64_t ld, const int* lens, const 
  * the new k / v go to (r, lens[r] - plens[r / K]).  Same keys in the same order as the contiguous kernel: same bits. */
 int nv_beam_topk(const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, const int* special, int n_special,
                  const float* beam_score, float* cand_score, int* cand_tok, int* cand_parent, int B, int K, void* stream);
+/* HF logits processors of transformers 4.28 (the reference's pin), in its _get_logits_processor order, as generate() reaches them
+ * through models/nav_model.py:388-396 -> lang_model.generate(**kwargs) (repetition_penalty, no_repeat_ngram_size, min_length,
+ * min_new_tokens).  A row's history is HF's input_ids: its S padded prompt columns (left pads included; S read from the device
+ * int *prompt_width) followed by its t generated tokens.  RepetitionPenaltyLogitsProcessor: every distinct history id once,
+ * s < 0 -> bf16(s * penalty), else bf16(s / penalty) (IEEE division); NoRepeatNGramLogitsProcessor (ngram = n > 0): every
+ * token that completes an n-gram of the history whose first n - 1 tokens equal its last n - 1 -> -inf (nothing while
+ * S + t + 1 < n); MinLength / MinNewTokensLength: eos_id -> -inf while S + t < min_length or t < min_new_tokens.  Off:
+ * penalty 1, ngram 0, min_length 0, min_new_tokens 0.  V must fit two V-bit bitmaps in 48 KB.
+ * nv_logits_process: in place on the bf16 logits [R, ld] of the greedy / sampled decode rows, between the lm_head and the trie
+ * mask or the pick.  Row r reads prompt_ids[(r / rows_per_prompt) * ld_prompt ...] and hist[r, 0 .. hist_len[r]) ([R, G]); with
+ * append non-null, append[r] is first stored at hist[r, hist_len[r]] and hist_len[r] incremented, so a captured step keeps
+ * the history itself.  One CTA per row; PDL like the rest of the decode chain.
+ * nv_beam_topk_processed: nv_beam_topk with the processors applied to each bf16 log-prob before the fp32 beam-score add (4.28
+ * beam_search); beam k of prompt b has the history prompt_ids[b * ld_ids ...] ++ hist[b * K + k, 0 .. t) with
+ * t = prompt_state[b, 0], the state nv_beam_select keeps. */
+int nv_logits_process(void* logits, int64_t ld, int V, const int* prompt_ids, int64_t ld_prompt, const int* prompt_width,
+                      int rows_per_prompt, int* hist, int G, int* hist_len, const int* append, float penalty, int ngram,
+                      int min_length, int min_new_tokens, int eos_id, int R, void* stream);
+int nv_beam_topk_processed(const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, const int* special, int n_special,
+                           const float* beam_score, float* cand_score, int* cand_tok, int* cand_parent, const int* prompt_ids,
+                           int64_t ld_ids, const int* prompt_width, const int* hist, int G, const int* prompt_state, float penalty,
+                           int ngram, int min_length, int min_new_tokens, int eos_id, int B, int K, void* stream);
 int nv_beam_select(const float* cand_score, const int* cand_tok, const int* cand_parent, float* beam_score, int* hist, int* src,
                    double* hyp_score, int* hyp_meta, int* hyp_tok, int* prompt_state, int* next_ids, int* lens, const double* norm,
                    int B, int K, int G, int eos_id, int pad_id, int early_stopping, void* stream);

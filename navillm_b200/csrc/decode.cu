@@ -904,6 +904,101 @@ __global__ void __launch_bounds__(SMP_THREADS) sample_topk_kernel(const __nv_bfl
   }
 }
 
+// ---- logits processors (transformers 4.28 _get_logits_processor order: RepetitionPenaltyLogitsProcessor,
+// NoRepeatNGramLogitsProcessor, MinLengthLogitsProcessor, MinNewTokensLengthLogitsProcessor) ----
+// A row's history is HF's input_ids: the S padded prompt columns (left pads included) followed by its t generated tokens.
+struct ProcHist {
+  const int* prompt;                         // the row's padded prompt ids [S]
+  const int* gen;                            // its generated tokens [t]
+  int S;
+  __device__ __forceinline__ int operator[](int i) const { return i < S ? prompt[i] : gen[i - S]; }
+};
+
+// The processor scalars; "off" is penalty 1, ngram 0, min_length 0, min_new 0.
+struct ProcParams {
+  float penalty;
+  int ngram, min_length, min_new, eos;
+};
+
+// RepetitionPenaltyLogitsProcessor on one bf16 score: torch.where(s < 0, s * p, s / p) in fp32 opmath, rounded to bf16; the
+// division is the IEEE one (the build's --use_fast_math would otherwise make it approximate).
+__device__ __forceinline__ float rep_penalize(float s, float p) {
+  return bf16_round(s < 0.f ? __fmul_rn(s, p) : __fdiv_rn(s, p));
+}
+
+// Set bits[h[j + n - 1]] for every n-gram h[j .. j + n - 1] of the L-token history whose first n - 1 tokens equal the last
+// n - 1 tokens of the history (4.28 _get_ngrams / _get_generated_ngrams); nothing while L + 1 < n.  Positions strided over
+// the CTA's threads.
+__device__ __forceinline__ void ngram_bans(const ProcHist& h, int L, int n, int V, uint32_t* bits) {
+  for (int j = threadIdx.x; j + n <= L; j += blockDim.x) {
+    bool match = true;
+    for (int q = 0; q < n - 1 && match; ++q) match = h[j + q] == h[L - n + 1 + q];
+    if (match) {
+      const int id = h[j + n - 1];
+      if (id >= 0 && id < V) atomicOr(&bits[id >> 5], 1u << (id & 31));
+    }
+  }
+}
+
+__device__ __forceinline__ bool eos_banned(const ProcParams& p, int S, int t) {
+  return S + t < p.min_length || t < p.min_new;
+}
+
+constexpr int LP_THREADS = 256;
+
+// One CTA per decode row r, in place on the bf16 logits row.  Row r reads prompt row r / rows_per_prompt (the samples of a
+// prompt share it) and its generated history hist[r, 0 .. hist_len[r]); with `append`, append[r] (the token picked at the
+// previous step) is first appended there.  Phase 1: each distinct history id is penalised once (a V-bit shared bitmap; the
+// thread whose atomicOr set the bit writes).  Phase 2: n-gram bans and phase 3: the EOS bans, both -inf.  Work per row is
+// O(V / 32 + (S + t) * n), independent of V beyond clearing the bitmap.
+__global__ void __launch_bounds__(LP_THREADS) logits_process_kernel(__nv_bfloat16* __restrict__ logits, int64_t ld, int V,
+                                                                    const int* __restrict__ prompt, int64_t ld_prompt,
+                                                                    const int* __restrict__ prompt_width, int rows_per_prompt,
+                                                                    int* __restrict__ hist, int G, int* __restrict__ hist_len,
+                                                                    const int* __restrict__ append, ProcParams p) {
+  extern __shared__ uint32_t lp_bits[];                          // (V + 31) / 32 words
+  __shared__ int s_t;
+  griddep_launch();
+  griddep_wait();
+  const int r = blockIdx.x, tid = threadIdx.x;
+  const int nw = (V + 31) >> 5;
+  int* grow = hist + (int64_t)r * G;
+  if (tid == 0) {
+    int t = hist_len[r];
+    if (append != nullptr && t < G) {
+      grow[t] = append[r];
+      hist_len[r] = ++t;
+    }
+    s_t = t;
+  }
+  for (int i = tid; i < nw; i += LP_THREADS) lp_bits[i] = 0u;
+  __syncthreads();                                               // also publishes the appended token to the CTA
+  const int S = *prompt_width, t = s_t, L = S + t;
+  const ProcHist h{prompt + (int64_t)(r / rows_per_prompt) * ld_prompt, grow, S};
+  __nv_bfloat16* row = logits + (int64_t)r * ld;
+  if (p.penalty != 1.f) {
+    for (int i = tid; i < L; i += LP_THREADS) {
+      const int id = h[i];
+      if (id < 0 || id >= V) continue;
+      const uint32_t m = 1u << (id & 31);
+      if (!(atomicOr(&lp_bits[id >> 5], m) & m)) row[id] = __float2bfloat16_rn(rep_penalize(__bfloat162float(row[id]), p.penalty));
+    }
+  }
+  __syncthreads();
+  const __nv_bfloat16 ninf = __ushort_as_bfloat16((unsigned short)0xFF80u);
+  if (p.ngram > 0) {
+    for (int j = tid; j + p.ngram <= L; j += LP_THREADS) {
+      bool match = true;
+      for (int q = 0; q < p.ngram - 1 && match; ++q) match = h[j + q] == h[L - p.ngram + 1 + q];
+      if (match) {
+        const int id = h[j + p.ngram - 1];
+        if (id >= 0 && id < V) row[id] = ninf;
+      }
+    }
+  }
+  if (tid == 0 && p.eos >= 0 && p.eos < V && eos_banned(p, S, t)) row[p.eos] = ninf;
+}
+
 // ---- beam search (HF GenerationMixin.beam_search / BeamSearchScorer of transformers 4.28, the version the reference pins) ----
 constexpr int BEAM_MAX = 8;                  // beams per prompt
 constexpr int BT_THREADS = 512;
@@ -922,11 +1017,25 @@ __device__ __forceinline__ float f32_unorder(uint32_t k) {
 // -inf, the row max and sum in fp32 / fp64, each log-prob rounded once to bf16, then the fp32 add of HF.  The 2K best of the
 // K * V scores by (score desc, flat index k * V + c asc) go to cand_* [B, 2K] in that order.  A score and its flat index
 // make one 64-bit key, so every comparison is one integer compare and equal scores order by index.
-__global__ void __launch_bounds__(BT_THREADS) beam_topk_kernel(const __nv_bfloat16* __restrict__ logits, int64_t ld_prompt,
-                                                               int64_t ld_beam, int V, const int* __restrict__ special,
-                                                               int n_special, const float* __restrict__ beam_score, int K,
-                                                               float* __restrict__ cand_score, int* __restrict__ cand_tok,
-                                                               int* __restrict__ cand_par) {
+// PROC (nv_beam_topk_processed): the logits processors of ProcParams act on each bf16 log-prob before the add, as 4.28's
+// beam_search applies them to log_softmax's output.  Beam k of prompt b has the history prompt[b, 0 .. S) ++ hist[b * K + k,
+// 0 .. t), t = prompt_state[b, 0] (nv_beam_select keeps hist in beam order); per beam, a "seen" and a "banned" V-bit bitmap
+// are built in dynamic shared memory before the beam's scores are scanned.
+struct BeamProc {
+  const int* prompt;                         // [B, ld_prompt] padded prompt ids
+  int64_t ld_prompt;
+  const int* prompt_width;                   // device S
+  const int* hist;                           // [B * K, G]
+  int G;
+  const int* prompt_state;                   // [B, 5]; field 0: tokens generated
+  ProcParams p;
+};
+
+template <bool PROC>
+__device__ __forceinline__ void beam_topk_body(const __nv_bfloat16* __restrict__ logits, int64_t ld_prompt, int64_t ld_beam, int V,
+                                               const int* __restrict__ special, int n_special, const float* __restrict__ beam_score,
+                                                int K, float* __restrict__ cand_score, int* __restrict__ cand_tok,
+                                               int* __restrict__ cand_par, const BeamProc& bp) {
   __shared__ int s_special[MAX_SPECIAL];
   __shared__ float s_m[BEAM_MAX], s_ls[BEAM_MAX], s_bs[BEAM_MAX];
   __shared__ float redf[32];
@@ -979,9 +1088,40 @@ __global__ void __launch_bounds__(BT_THREADS) beam_topk_kernel(const __nv_bfloat
   for (int k = 0; k < K; ++k) {
     const __nv_bfloat16* row = logits + (int64_t)b * ld_prompt + (int64_t)k * ld_beam;
     const float m = s_m[k], ls = s_ls[k], bs = s_bs[k];
+    uint32_t* seen = nullptr;
+    uint32_t* banned = nullptr;
+    if constexpr (PROC) {
+      extern __shared__ uint32_t bt_bits[];                      // seen | banned, (V + 31) / 32 words each
+      const int nw = (V + 31) >> 5;
+      seen = bt_bits;
+      banned = bt_bits + nw;
+      __syncthreads();                                           // the previous beam's scan is done with the bitmaps
+      for (int i = tid; i < 2 * nw; i += BT_THREADS) bt_bits[i] = 0u;
+      __syncthreads();
+      const int S = *bp.prompt_width, t = bp.prompt_state[b * 5], L = S + t;
+      const ProcHist h{bp.prompt + (int64_t)b * bp.ld_prompt, bp.hist + (int64_t)(b * K + k) * bp.G, S};
+      if (bp.p.penalty != 1.f)
+        for (int i = tid; i < L; i += BT_THREADS) {
+          const int id = h[i];
+          if (id >= 0 && id < V) atomicOr(&seen[id >> 5], 1u << (id & 31));
+        }
+      if (bp.p.ngram > 0) ngram_bans(h, L, bp.p.ngram, V, banned);
+      if (tid == 0 && bp.p.eos >= 0 && bp.p.eos < V && eos_banned(bp.p, S, t)) atomicOr(&banned[bp.p.eos >> 5], 1u << (bp.p.eos & 31));
+      __syncthreads();
+    }
     for (int c = tid; c < V; c += BT_THREADS) {
       float sc = -INFINITY;
-      if (!is_special(c)) sc = bf16_round((__bfloat162float(row[c]) - m) - ls) + bs;
+      if constexpr (PROC) {
+        if (!is_special(c)) {
+          float lp = bf16_round((__bfloat162float(row[c]) - m) - ls);
+          const uint32_t bit = 1u << (c & 31);
+          if (seen[c >> 5] & bit) lp = rep_penalize(lp, bp.p.penalty);
+          if (banned[c >> 5] & bit) lp = -INFINITY;
+          sc = lp + bs;
+        }
+      } else {
+        if (!is_special(c)) sc = bf16_round((__bfloat162float(row[c]) - m) - ls) + bs;
+      }
       if (sc != sc) sc = -INFINITY;
       const unsigned long long key =
           ((unsigned long long)f32_order(sc) << 32) | (unsigned long long)(0xffffffffu - (uint32_t)(k * V + c));
@@ -1024,6 +1164,23 @@ __global__ void __launch_bounds__(BT_THREADS) beam_topk_kernel(const __nv_bfloat
     }
     __syncthreads();                                             // redk is reused by the next round
   }
+}
+
+__global__ void __launch_bounds__(BT_THREADS) beam_topk_kernel(const __nv_bfloat16* __restrict__ logits, int64_t ld_prompt,
+                                                               int64_t ld_beam, int V, const int* __restrict__ special,
+                                                               int n_special, const float* __restrict__ beam_score, int K,
+                                                               float* __restrict__ cand_score, int* __restrict__ cand_tok,
+                                                               int* __restrict__ cand_par) {
+  beam_topk_body<false>(logits, ld_prompt, ld_beam, V, special, n_special, beam_score, K, cand_score, cand_tok, cand_par, BeamProc{});
+}
+
+// one CTA per SM is what B <= 132 prompts use anyway; the bound lets the bitmap tests stay in registers beside the 2K-key list
+__global__ void __launch_bounds__(BT_THREADS, 1) beam_topk_proc_kernel(const __nv_bfloat16* __restrict__ logits, int64_t ld_prompt,
+                                                                       int64_t ld_beam, int V, const int* __restrict__ special,
+                                                                       int n_special, const float* __restrict__ beam_score, int K,
+                                                                       float* __restrict__ cand_score, int* __restrict__ cand_tok,
+                                                                       int* __restrict__ cand_par, BeamProc bp) {
+  beam_topk_body<true>(logits, ld_prompt, ld_beam, V, special, n_special, beam_score, K, cand_score, cand_tok, cand_par, bp);
 }
 
 // prompt_state [B, BS_FIELDS] of nv_beam_select
@@ -1350,6 +1507,51 @@ int nv_beam_topk(const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, 
   if (B == 0) return NV_OK;
   NV_CUDA(launch_pdl(beam_topk_kernel, dim3(B), dim3(BT_THREADS), 0, S_(stream), CBF(logits), ld_prompt, ld_beam, V, special,
                      n_special, beam_score, K, cand_score, cand_tok, cand_parent));
+  return NV_OK;
+}
+
+static int check_proc(const char* name, int V, float penalty, int ngram, int min_length, int min_new_tokens) {
+  NV_REQUIRE(penalty > 0.f && ngram >= 0 && min_length >= 0 && min_new_tokens >= 0,
+             "%s: penalty=%g must be > 0, ngram=%d / min_length=%d / min_new_tokens=%d >= 0", name, (double)penalty, ngram, min_length,
+             min_new_tokens);
+  NV_REQUIRE(V > 0 && (int64_t)((V + 31) / 32) * 4 * 2 <= 48 * 1024, "%s: vocabulary of %d does not fit the shared bitmaps", name, V);
+  return NV_OK;
+}
+
+// Logits processors in place on R bf16 rows (see logits_process_kernel).
+int nv_logits_process(void* logits, int64_t ld, int V, const int* prompt_ids, int64_t ld_prompt, const int* prompt_width,
+                      int rows_per_prompt, int* hist, int G, int* hist_len, const int* append, float penalty, int ngram,
+                      int min_length, int min_new_tokens, int eos_id, int R, void* stream) {
+  NV_REQUIRE(logits && prompt_ids && prompt_width && hist && hist_len && rows_per_prompt >= 1 && G > 0 && R >= 0 && ld >= V,
+             "nv_logits_process: bad arguments (R=%d G=%d rows_per_prompt=%d)", R, G, rows_per_prompt);
+  const int st = check_proc("nv_logits_process", V, penalty, ngram, min_length, min_new_tokens);
+  if (st != NV_OK) return st;
+  if (R == 0) return NV_OK;
+  NV_CUDA(launch_pdl(logits_process_kernel, dim3(R), dim3(LP_THREADS), (size_t)((V + 31) / 32) * 4, S_(stream), BF(logits), ld, V,
+                     prompt_ids, ld_prompt, prompt_width, rows_per_prompt, hist, G, hist_len, append,
+                     ProcParams{penalty, ngram, min_length, min_new_tokens, eos_id}));
+  return NV_OK;
+}
+
+// nv_beam_topk with the logits processors on each log-prob (see beam_topk_kernel<true>).
+int nv_beam_topk_processed(const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, const int* special, int n_special,
+                           const float* beam_score, float* cand_score, int* cand_tok, int* cand_parent, const int* prompt_ids,
+                           int64_t ld_ids, const int* prompt_width, const int* hist, int G, const int* prompt_state, float penalty,
+                           int ngram, int min_length, int min_new_tokens, int eos_id, int B, int K, void* stream) {
+  NV_REQUIRE(logits && beam_score && cand_score && cand_tok && cand_parent && prompt_ids && prompt_width && hist && prompt_state &&
+             V > 0 && B >= 0 && G > 0, "nv_beam_topk_processed: bad arguments (V=%d B=%d G=%d)", V, B, G);
+  NV_REQUIRE(K >= 1 && K <= BEAM_MAX && 2 * K <= V, "nv_beam_topk_processed: %d beams: 1..%d beams and V >= 2K supported", K,
+             BEAM_MAX);
+  NV_REQUIRE((int64_t)K * V < 0xffffffffll, "nv_beam_topk_processed: K * V = %lld does not fit the 32-bit candidate index",
+             (long long)K * V);
+  NV_REQUIRE(n_special >= 0 && n_special <= MAX_SPECIAL && (n_special == 0 || special),
+             "nv_beam_topk_processed: n_special=%d out of range (max %d)", n_special, MAX_SPECIAL);
+  const int st = check_proc("nv_beam_topk_processed", V, penalty, ngram, min_length, min_new_tokens);
+  if (st != NV_OK) return st;
+  if (B == 0) return NV_OK;
+  const BeamProc bp{prompt_ids, ld_ids, prompt_width, hist, G, prompt_state, ProcParams{penalty, ngram, min_length, min_new_tokens, eos_id}};
+  NV_CUDA(launch_pdl(beam_topk_proc_kernel, dim3(B), dim3(BT_THREADS), (size_t)((V + 31) / 32) * 4 * 2, S_(stream), CBF(logits),
+                     ld_prompt, ld_beam, V, special, n_special, beam_score, K, cand_score, cand_tok, cand_parent, bp));
   return NV_OK;
 }
 

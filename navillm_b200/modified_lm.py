@@ -925,13 +925,57 @@ class ModifiedLlamaForCausalLM(nn.Module):
         o = ncap + 2
         return st.trie_buf[:o], st.trie_buf[o:o + ecap], st.trie_buf[o + ecap:], ncap
 
+    @staticmethod
+    def _load_proc(st, input_ids, rows: int, G: int) -> None:
+        """The logits processors' device state in persistent buffers of ``st`` (a captured step keeps their pointers): the padded
+        prompt ids ``proc_ids`` [P, >= S] and their width S ``proc_width`` [1], copied once per call, and -- for ``rows`` > 0 --
+        the generated history ``proc_hist`` [rows, >= G] with its per-row length ``proc_len`` (zeroed; the step appends to it).
+        Capacities grow in powers of two; growing drops the state's graph."""
+        P, S = input_ids.shape
+        dev = st.next_ids.device
+        scap, gcap = getattr(st, "proc_cap", (0, 0))
+        if S > scap or (rows and G > gcap):
+            pow2 = lambda n: 1 << max(0, int(n) - 1).bit_length()
+            scap, gcap = max(scap, pow2(S)), max(gcap, pow2(G) if rows else 0)
+            st.proc_ids = torch.zeros((P, scap), dtype=torch.int32, device=dev)
+            st.proc_width = torch.zeros((1,), dtype=torch.int32, device=dev)
+            if rows:
+                st.proc_hist = torch.zeros((rows, gcap), dtype=torch.int32, device=dev)
+                st.proc_len = torch.zeros((rows,), dtype=torch.int32, device=dev)
+            st.proc_cap = (scap, gcap)
+            st.graph = None
+        st.proc_ids[:, :S].copy_(input_ids.to(torch.int32))
+        st.proc_width.fill_(S)
+        if rows:
+            st.proc_len.zero_()
+
+    @staticmethod
+    def _processors(repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens, eos: int) -> Optional[tuple]:
+        """Validate HF's processor kwargs as transformers does; returns (penalty, n, min_length, min_new_tokens, eos) for the
+        kernels, or None when every one is at its default (off), which keeps the call on the processor-free path."""
+        p = 1.0 if repetition_penalty is None else repetition_penalty
+        if p != 1.0 and (isinstance(p, bool) or not isinstance(p, float) or not p > 0):
+            raise ValueError(f"generate(repetition_penalty={repetition_penalty!r}): has to be a strictly positive float")
+        named = (("no_repeat_ngram_size", no_repeat_ngram_size), ("min_length", min_length), ("min_new_tokens", min_new_tokens))
+        ints = []
+        for name, v in named:
+            v = 0 if v is None else v
+            if isinstance(v, bool) or not isinstance(v, int) or v < 0:
+                raise ValueError(f"generate({name}={v!r}): has to be a non-negative integer")
+            ints.append(v)
+        if p == 1.0 and not any(ints):
+            return None
+        return (float(p), *ints, int(eos))
+
     @torch.no_grad()
     def generate(self, input_ids, attention_mask, cand_vis=None, hist_vis=None, obj_vis=None, max_new_tokens: int = 20,
                  do_sample: bool = False, temperature: float = 1.0, eos_token_id: Optional[int] = None,
                  pad_token_id: Optional[int] = None, bos_token_id: Optional[int] = None, logits_processor=None, trie=None,
                  stop_on_eos: bool = True, use_cuda_graph: bool = True, stats: Optional[dict] = None, top_k: int = 50,
                  top_p: float = 1.0, num_beams: int = 1, length_penalty: float = 1.0, early_stopping: bool = False,
-                 num_return_sequences: int = 1, num_beam_groups: int = 1, **unused) -> torch.Tensor:
+                 num_return_sequences: int = 1, num_beam_groups: int = 1, repetition_penalty: Optional[float] = None,
+                 no_repeat_ngram_size: Optional[int] = None, min_length: Optional[int] = None,
+                 min_new_tokens: Optional[int] = None, **unused) -> torch.Tensor:
         """Prefill on the packed kernels (positions = cumsum(mask)-1 like HF generate; visual tokens injected only
         here, as in models/modified_lm.py:195-197), then one token per step over a pre-allocated KV cache.  The
         decode step of the greedy, sampled and trie-constrained modes has static shapes and is replayed as a CUDA graph
@@ -963,7 +1007,15 @@ class ModifiedLlamaForCausalLM(nn.Module):
         ``do_sample=True, num_return_sequences=N`` draws N samples per prompt: [B * N, L] ids, row b * N + j a sample of
         prompt b (HF's order).  Each prompt is prefilled once and its N rows share its KV cache (``_generate``); the tokens
         are those of the same call on the prompts repeated N times.  With ``trie=`` / ``logits_processor=``, and without
-        ``do_sample``, N > 1 raises ``NotImplementedError``."""
+        ``do_sample``, N > 1 raises ``NotImplementedError``.
+
+        ``repetition_penalty``, ``no_repeat_ngram_size``, ``min_length`` and ``min_new_tokens`` are HF's logits processors as
+        transformers 4.28 applies them, in every mode above: after the special-token mask and before ``trie=`` /
+        ``logits_processor=``, on the bf16 next-token logits (greedy, sampled: before the warpers) or on the bf16 log-probs
+        before the beam-score add (beams).  Their history is HF's ``input_ids``: the padded prompt row as passed, left pads
+        included, then the row's (beam's, sample's) generated tokens.  They run on the device (``nv_logits_process``,
+        ``nv_beam_topk_processed``) inside the captured step; values are checked as HF checks them (``ValueError``), and the
+        defaults (1.0 / None or 0) leave the call on the processor-free path."""
         if num_beam_groups is not None and num_beam_groups > 1:
             raise NotImplementedError("generate(num_beam_groups > 1): group (diverse) beam search is not built")
         top_p = 1.0 if top_p is None else float(top_p)
@@ -993,13 +1045,14 @@ class ModifiedLlamaForCausalLM(nn.Module):
         dev = self._device()
         eos = self.tokenizer.eos_token_id if eos_token_id is None else eos_token_id
         pad = self.tokenizer.unk_token_id if pad_token_id is None else pad_token_id
+        proc = self._processors(repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens, eos)
         if num_beams > 1:
             return self._generate_beam(input_ids, attention_mask, cand_vis, hist_vis, obj_vis, max_new_tokens, int(num_beams), eos,
                                        pad, float(length_penalty), bool(early_stopping), int(num_return_sequences), use_cuda_graph,
-                                       stats)
+                                       stats, proc)
         procs = list(logits_processor or [])
         args = (input_ids, attention_mask, cand_vis, hist_vis, obj_vis, max_new_tokens, do_sample, temperature, eos, pad,
-                stop_on_eos, use_cuda_graph, stats, top_k, top_p, max(1, n_seq))
+                stop_on_eos, use_cuda_graph, stats, top_k, top_p, max(1, n_seq), proc)
         table, path = None, None
         if trie is not None and not procs:
             t0 = time.perf_counter()
@@ -1023,7 +1076,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
         return out
 
     def _generate(self, input_ids, attention_mask, cand_vis, hist_vis, obj_vis, max_new_tokens, do_sample, temperature, eos, pad,
-                  stop_on_eos, use_cuda_graph, stats, top_k, top_p, n_seq, *, procs, table):
+                  stop_on_eos, use_cuda_graph, stats, top_k, top_p, n_seq, proc=None, *, procs, table):
         """``generate`` with the host processors ``procs`` (the host path when not empty) or the flattened trie ``table``
         walked on the device; returns None when the device walk reported a miss.
 
@@ -1047,6 +1100,8 @@ class ModifiedLlamaForCausalLM(nn.Module):
         key = (int(eos), int(pad), bool(stop_on_eos), mode, float(temperature) if do_sample else None,
                int(top_k) if do_sample else None, float(top_p) if do_sample else None, table.eos if table is not None else None,
                self.kv_cache_dtype)
+        if proc is not None:                                      # the processor scalars the captured step bakes in
+            key += (("proc",) + proc,)
         shared = n_seq > 1
         if shared:                                                # prompt cache per prompt + generated keys per row
             Sp = (max(pp.seqlens) + 127) // 128 * 128
@@ -1068,6 +1123,8 @@ class ModifiedLlamaForCausalLM(nn.Module):
                 st.node = torch.zeros((B,), dtype=torch.int32, device=dev)
                 st.miss = torch.zeros((1,), dtype=torch.int32, device=dev)
             trie_csr = self._load_trie(st, table)
+        if proc is not None:
+            self._load_proc(st, input_ids, R, max_new_tokens)
         finished.zero_()
         lens.copy_(torch.tensor(pp.seqlens, dtype=torch.int32).repeat_interleave(n_seq), non_blocking=True)
 
@@ -1079,7 +1136,12 @@ class ModifiedLlamaForCausalLM(nn.Module):
             hid_last = hid_last.repeat_interleave(n_seq, dim=0)
         special = self.special_ids_dev
 
-        head = lambda h_rows: self._decode_head(h_rows, logits)
+        def head(h_rows, append=None):
+            """lm_head into `logits`, then the logits processors, whose history first takes the token in `append`."""
+            self._decode_head(h_rows, logits)
+            if proc is not None:
+                ops.logits_process_(logits, st.proc_ids, st.proc_width, st.proc_hist, st.proc_len, append, proc,
+                                    rows_per_prompt=n_seq)
 
         def pick_host(all_ids_host):
             """next token from `logits` -> next_ids (device), through the host processors."""
@@ -1128,7 +1190,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
             with ops.pdl():                         # programmatic dependent launch along the whole decode chain
                 xt = ops.embed_fwd(next_ids, E)
                 h = core.decode_step(xt, lens, kc, vc, beam=beam)
-                head(h)
+                head(h, append=next_ids)
                 ops.add_int_(lens, 1)
                 if not need_host:
                     pick(advance=True)
@@ -1217,13 +1279,14 @@ class ModifiedLlamaForCausalLM(nn.Module):
         return st
 
     def _generate_beam(self, input_ids, attention_mask, cand_vis, hist_vis, obj_vis, max_new_tokens, K, eos, pad, length_penalty,
-                       early_stopping, n_return, use_cuda_graph, stats):
+                       early_stopping, n_return, use_cuda_graph, stats, proc=None):
         """Beam search over B prompts with K beams each.  The prefill runs once per prompt into the prompt cache, whose keys the
         K beams of the prompt share; generated keys live in a [B * K, G] cache that is written once per slot and read through
         the source table ``src`` (reordering the beams gathers ``src``, never K/V).  Each step is ``nv_beam_topk`` (2K best
         candidates per prompt) and ``nv_beam_select`` (the scorer), all on the device, and is replayed as a CUDA graph; the
         hypotheses are finalized on the host after one device-to-host copy.  The visual tokens of prompt b reach all K beams of
-        prompt b (the reference's HF expansion of ``cand_vis`` would hand them to other rows' slots)."""
+        prompt b (the reference's HF expansion of ``cand_vis`` would hand them to other rows' slots).  With logits processors
+        (``proc``) the scoring is ``nv_beam_topk_processed`` over the beams' histories (prompt ids, ``hist``)."""
         if K > self.BEAM_MAX:
             raise NotImplementedError(f"generate(num_beams={K}): at most {self.BEAM_MAX} beams are built")
         if max_new_tokens < 1:
@@ -1242,7 +1305,11 @@ class ModifiedLlamaForCausalLM(nn.Module):
         Sp = (max(pp.seqlens) + 127) // 128 * 128
         G = (max_new_tokens + 127) // 128 * 128
         key = (int(eos), int(pad), bool(early_stopping), self.kv_cache_dtype)     # what the captured step bakes in
+        if proc is not None:
+            key += (("proc",) + proc,)
         st = self._beam_state(B, K, Sp, G, key, use_cuda_graph)
+        if proc is not None:
+            self._load_proc(st, input_ids, 0, G)
         plens = torch.tensor(pp.seqlens, dtype=torch.int32)
         st.plens.copy_(plens, non_blocking=True)
         st.beam_score.view(B, K).fill_(-1e9)[:, 0] = 0.0             # only beam 0 of a prompt expands at the first step
@@ -1260,7 +1327,14 @@ class ModifiedLlamaForCausalLM(nn.Module):
         sel = lambda: ops.beam_select(st.cand_score, st.cand_tok, st.cand_par, st.beam_score, st.hist, st.src, st.hyp_score,
                                       st.hyp_meta, st.hyp_tok, st.pstate, st.next_ids, st.lens, st.norm, eos, pad,
                                       early_stopping)
-        ops.beam_topk(st.logits, special, st.beam_score, K, st.cand_score, st.cand_tok, st.cand_par, first_step=True)
+        def topk(first_step=False):
+            if proc is None:
+                ops.beam_topk(st.logits, special, st.beam_score, K, st.cand_score, st.cand_tok, st.cand_par, first_step=first_step)
+            else:
+                ops.beam_topk_processed(st.logits, special, st.beam_score, K, st.cand_score, st.cand_tok, st.cand_par, st.proc_ids,
+                                        st.proc_width, st.hist, st.pstate, proc, first_step=first_step)
+
+        topk(first_step=True)
         sel()
         if ev is not None:
             ev[1].record()
@@ -1271,7 +1345,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
                 xt = ops.embed_fwd(st.next_ids, E)
                 h = core.decode_step(xt, st.lens, st.kc, st.vc, beam=beam)
                 self._decode_head(h, st.logits)
-                ops.beam_topk(st.logits, special, st.beam_score, K, st.cand_score, st.cand_tok, st.cand_par)
+                topk()
                 sel()
 
         # like the greedy loop, ask the device whether every prompt is done only every few steps: a done prompt's steps leave

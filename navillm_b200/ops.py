@@ -757,6 +757,55 @@ def beam_topk(logits, special, beam_score, K, cand_score, cand_tok, cand_parent,
                                    i32(K), stream_ptr()), "nv_beam_topk")
 
 
+def _proc_io(name, V, prompt_ids, prompt_width, hist, proc):
+    penalty, ngram, min_length, min_new, eos = proc
+    if prompt_ids.dtype != torch.int32 or prompt_ids.dim() != 2 or prompt_ids.stride(1) != 1 or not prompt_ids.is_cuda:
+        raise ValueError(f"{name}: prompt_ids int32 [P, >= S] with unit inner stride on the device expected")
+    if prompt_width.dtype != torch.int32 or prompt_width.numel() != 1 or not prompt_width.is_cuda:
+        raise ValueError(f"{name}: prompt_width int32 [1] on the device expected")
+    if hist.dtype != torch.int32 or hist.dim() != 2 or not hist.is_contiguous() or not hist.is_cuda:
+        raise ValueError(f"{name}: hist int32 [rows, G] contiguous on the device expected")
+    return f32(penalty), i32(ngram), i32(min_length), i32(min_new), i32(eos)
+
+
+def logits_process_(logits, prompt_ids, prompt_width, hist, hist_len, append, proc, *, rows_per_prompt=1):
+    """HF's repetition-penalty / no-repeat-n-gram / min-length / min-new-tokens processors in place on bf16 logits [R, V]
+    (nv_logits_process).  proc = (penalty, ngram, min_length, min_new_tokens, eos_id); prompt_ids int32 [P, >= S] (row r reads
+    prompt r // rows_per_prompt), prompt_width int32 [1] = S, hist int32 [R, G] and hist_len int32 [R] the generated history;
+    ``append`` (int32 [R] or None) is appended to it first."""
+    R, V = logits.shape
+    if logits.dtype != bf16 or logits.stride(1) != 1:
+        raise ValueError(f"logits_process_: bf16 logits with unit inner stride expected (got {logits.dtype})")
+    if hist.shape[0] != R or hist_len.dtype != torch.int32 or hist_len.numel() != R or \
+            (append is not None and (append.dtype != torch.int32 or append.numel() != R)):
+        raise ValueError(f"logits_process_: hist [{R}, G], hist_len / append int32 [{R}] expected")
+    args = _proc_io("logits_process_", V, prompt_ids, prompt_width, hist, proc)
+    check(_lib.load().nv_logits_process(ptr(logits), i64(logits.stride(0)), i32(V), ptr(prompt_ids), i64(prompt_ids.stride(0)),
+                                        ptr(prompt_width), i32(rows_per_prompt), ptr(hist), i32(hist.shape[1]), ptr(hist_len),
+                                        ptr(append), *args, i32(R), stream_ptr()), "nv_logits_process")
+    return logits
+
+
+def beam_topk_processed(logits, special, beam_score, K, cand_score, cand_tok, cand_parent, prompt_ids, prompt_width, hist,
+                        prompt_state, proc, *, first_step=False):
+    """``beam_topk`` with the processors of ``logits_process_`` applied to each bf16 log-prob before the beam-score add
+    (nv_beam_topk_processed); beam k of prompt b has the history prompt_ids[b, :S] ++ hist[b * K + k, :prompt_state[b, 0]]."""
+    B = cand_score.shape[0]
+    V = logits.shape[1]
+    if logits.dtype != bf16 or logits.stride(1) != 1 or logits.shape[0] < (B if first_step else B * K):
+        raise ValueError(f"beam_topk_processed: bf16 logits with {B if first_step else B * K} rows expected "
+                         f"(got {logits.dtype} {tuple(logits.shape)})")
+    _beam_io("beam_topk_processed", B, K, hist.shape[1], cand_score=cand_score, cand_tok=cand_tok, cand_parent=cand_parent,
+             beam_score=beam_score, hist=hist, prompt_state=prompt_state)
+    args = _proc_io("beam_topk_processed", V, prompt_ids, prompt_width, hist, proc)
+    ld = logits.stride(0)
+    check(_lib.load().nv_beam_topk_processed(ptr(logits), i64(ld if first_step else K * ld), i64(0 if first_step else ld), i32(V),
+                                             ptr(special), i32(special.numel()), ptr(beam_score), ptr(cand_score), ptr(cand_tok),
+                                             ptr(cand_parent), ptr(prompt_ids), i64(prompt_ids.stride(0)), ptr(prompt_width),
+                                             ptr(hist), i32(hist.shape[1]), ptr(prompt_state), *args, i32(B), i32(K), stream_ptr()),
+          "nv_beam_topk_processed")
+
+
 def beam_select(cand_score, cand_tok, cand_parent, beam_score, hist, src, hyp_score, hyp_meta, hyp_tok, prompt_state, next_ids, lens,
                 norm, eos_id, pad_id, early_stopping):
     """One BeamSearchScorer.process step on the device (nv_beam_select); norm fp64 [G]: (S + t) ** length_penalty for S padded
