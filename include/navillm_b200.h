@@ -357,6 +357,14 @@ int nv_grad_sumsq(const void* g, int64_t n, int is_bf16, float* partial, void* s
 int nv_clip_coef(const float* partial, int n_partial, float max_norm, float* state, void* stream);
 int nv_adamw_flat(void* p, void* g, void* m, void* v, int64_t n, int is_bf16, float lr, float beta1, float beta2, float eps,
                   float weight_decay, int step, const float* clip_state, int write_clipped_grad, void* stream);
+/* Opt-in error-compensated form of the same optimizer.step() (tools/optims.py:43) for bf16 buffers: r is a bf16 residual
+ * beside each weight, and the pair stands for the master value p + r.  Per element, in fp32: m and v advance exactly as in
+ * nv_adamw_flat, x = p + r takes the AdamW update, then p = bf16_rn(x) and r = bf16_rn(x - p), rounded toward zero instead
+ * where that keeps bf16_rn(p + r) == p.  With r == 0 on entry, p, m and v come out bit for bit as from nv_adamw_flat.  All operands bf16
+ * and 16-byte aligned; 9 x 2 bytes of HBM traffic per element (10 with write_clipped_grad). */
+int nv_adamw_flat_compensated(void* p, void* r, void* g, void* m, void* v, int64_t n, float lr, float beta1, float beta2,
+                              float eps, float weight_decay, int step, const float* clip_state, int write_clipped_grad,
+                              void* stream);
 
 /* ---- one decoder layer of the inference forward in ONE call (csrc/layer.cu) ----------------------------------------
  * transformers LlamaDecoderLayer (reached through models/modified_lm.py:112-116): RMSNorm -> fused qkv projection -> RoPE

@@ -244,6 +244,7 @@ class Fp8Weights:
         dev = flat.flat.device
         self.q = torch.empty(total, dtype=ops.fp8, device=dev)
         self.exps = torch.empty(rows, dtype=torch.int8, device=dev)
+        flat.generation += 1                     # the rounding below writes the weights through raw pointers
         for p in self.params:
             q, e = self.view([p], tuple(p.shape))
             ops.quantize_fp8_(p.data, q, e)
