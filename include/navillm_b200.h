@@ -365,6 +365,21 @@ int nv_adamw_flat(void* p, void* g, void* m, void* v, int64_t n, int is_bf16, fl
 int nv_adamw_flat_compensated(void* p, void* r, void* g, void* m, void* v, int64_t n, float lr, float beta1, float beta2,
                               float eps, float weight_decay, int step, const float* clip_state, int write_clipped_grad,
                               void* stream);
+/* Opt-in block-wise 8-bit moments for the bf16 buffer (Dettmers et al., ICLR 2022).  Each 64-element block of m and of v
+ * is one fp32 absmax and 64 uint8 codes, valued maps[code] * absmax; maps is fp32 [512]: the signed map of m, then the
+ * unsigned map of v, both sorted (navillm_b200/optim.py builds them).  Per element, in fp32: m and v are dequantized, the
+ * update of nv_adamw_flat (r null) or nv_adamw_flat_compensated runs on them, and each block is requantized to the nearest
+ * code (a tie to the smaller magnitude) of x / absmax with its new absmax.  Codes [n] and absmax [ceil(n / 64)] per
+ * moment; p, r and g 16-byte aligned, the codes 8-byte aligned.  10.25 bytes of HBM traffic per element, 14.25 with r. */
+int nv_adamw_flat_8bit(void* p, void* r, void* g, void* m_code, float* m_absmax, void* v_code, float* v_absmax,
+                       const float* maps, int64_t n, float lr, float beta1, float beta2, float eps, float weight_decay, int step,
+                       const float* clip_state, int write_clipped_grad, void* stream);
+/* One moment of n elements (bf16 or fp32) to the 8-bit form and back, in the blocks of nv_adamw_flat_8bit (is_signed: m's
+ * map, else v's).  For optimizer state (de)serialisation. */
+int nv_moments_quantize_8bit(const void* src, int is_bf16, void* code, float* absmax, int64_t n, int is_signed,
+                             const float* maps, void* stream);
+int nv_moments_dequantize_8bit(const void* code, const float* absmax, void* dst, int is_bf16, int64_t n, int is_signed,
+                               const float* maps, void* stream);
 
 /* ---- one decoder layer of the inference forward in ONE call (csrc/layer.cu) ----------------------------------------
  * transformers LlamaDecoderLayer (reached through models/modified_lm.py:112-116): RMSNorm -> fused qkv projection -> RoPE
