@@ -1,0 +1,471 @@
+"""``ModifiedLlamaForCausalLM.generate``'s decoding (HF GenerationMixin greedy / sampling / beam search): the call's record,
+the decode states, the prefill, the graph-replayed step loop and the drivers ``decode`` and ``beam_search``."""
+from __future__ import annotations
+
+import collections
+import dataclasses
+from types import SimpleNamespace
+from typing import Optional
+
+import torch
+
+from . import llama as llama_mod
+from . import ops
+
+bf16 = torch.bfloat16
+BEAM_MAX = 8                   # beams per prompt the beam kernels are built for
+
+
+@dataclasses.dataclass(frozen=True)
+class Decoding:
+    """One ``generate()`` call's decoding rule, after validation.  Fields a mode does not use are None."""
+    eos: int
+    pad: int
+    stop_on_eos: Optional[bool]          # None for beams: a prompt stops when its hypotheses are done
+    mode: str                            # "greedy", "sample", "trie", "trie+sample" or "beam"
+    kv: str                              # the KV cache format, "bf16" or "fp8"
+    temperature: Optional[float] = None  # sampled modes
+    top_k: Optional[int] = None
+    top_p: Optional[float] = None
+    trie_eos: Optional[int] = None       # trie modes: the flattened trie's end-of-answer id
+    n: int = 1                           # rows per prompt: samples, or beams
+    early_stopping: Optional[bool] = None
+    proc: Optional[tuple] = None         # the device logits processors (``processors``)
+    n_return: int = 1                    # beams: sequences returned per prompt (host finalisation)
+    length_penalty: Optional[float] = None   # beams: its normalisers are copied into the state every call
+
+    @property
+    def sampled(self) -> bool:
+        return self.mode in ("sample", "trie+sample")
+
+    def key(self) -> tuple:
+        """The graph key: every field a captured step bakes in (not ``n_return`` or ``length_penalty``), the format last."""
+        return (self.eos, self.pad, self.stop_on_eos, self.mode, self.temperature, self.top_k, self.top_p, self.trie_eos, self.n,
+                self.early_stopping, self.proc, self.kv)
+
+
+def processors(repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens, eos: int) -> Optional[tuple]:
+    """Validate HF's processor kwargs as transformers does; returns (penalty, n, min_length, min_new_tokens, eos) for the
+    kernels, or None when every one is at its default (off), which keeps the call on the processor-free path."""
+    p = 1.0 if repetition_penalty is None else repetition_penalty
+    if p != 1.0 and (isinstance(p, bool) or not isinstance(p, float) or not p > 0):
+        raise ValueError(f"generate(repetition_penalty={repetition_penalty!r}): has to be a strictly positive float")
+    named = (("no_repeat_ngram_size", no_repeat_ngram_size), ("min_length", min_length), ("min_new_tokens", min_new_tokens))
+    ints = []
+    for name, v in named:
+        v = 0 if v is None else v
+        if isinstance(v, bool) or not isinstance(v, int) or v < 0:
+            raise ValueError(f"generate({name}={v!r}): has to be a non-negative integer")
+        ints.append(v)
+    if p == 1.0 and not any(ints):
+        return None
+    return (float(p), *ints, int(eos))
+
+
+def logits_buffer(rows: int, V: int, device) -> torch.Tensor:
+    """Uninitialised bf16 [rows, V] logits whose rows start 16-byte aligned (a row stride of V rounded up to 64)."""
+    return torch.empty((rows, (V + 63) // 64 * 64), dtype=bf16, device=device)[:, :V]
+
+
+class DecodeStates(collections.OrderedDict):
+    """A model's persistent decode states by key (shapes and ``Decoding.key()``), least recently used first.  A state holds
+    the KV caches, the step's I/O buffers and -- once captured -- the CUDA graph of ONE decode step.  Capturing and
+    instantiating the ~260-node graph costs more than the 127 replays of a C3 generation save, so a state is kept for later
+    calls with the same key (evaluation loops call generate with the same shapes over and over), at most ``max_states`` of
+    them.  Whatever changes the weight buffers or the kernels a captured graph launches must ``clear()`` them."""
+
+    max_states = 2
+
+    def lookup(self, key, build, want_graph: bool):
+        """The state under ``key``, now the most recently used, or a new one from ``build()``.  A call that will not replay a
+        graph neither looks up nor keeps a state."""
+        if not want_graph:
+            return build()
+        if key in self:
+            self.move_to_end(key)
+            return self[key]
+        st = self[key] = build()
+        while len(self) > self.max_states:
+            self.popitem(last=False)
+        return st
+
+
+def _grow(st, cap_name: str, need: tuple, alloc) -> tuple:
+    """Capacities ``getattr(st, cap_name)`` of persistent buffers of ``st`` (a captured graph keeps their pointers): when
+    ``need`` exceeds them, each grows to the next power of two (a need of 0 stays 0), ``alloc(*caps)`` re-allocates the
+    buffers and the state's graph is dropped.  Returns the capacities."""
+    cap = getattr(st, cap_name, (0,) * len(need))
+    if any(n > c for n, c in zip(need, cap)):
+        cap = tuple(max(c, 1 << (n - 1).bit_length() if n else 0) for n, c in zip(need, cap))
+        alloc(*cap)
+        setattr(st, cap_name, cap)
+        st.graph = None
+    return cap
+
+
+def load_trie(st, table) -> tuple:
+    """Copy a flattened trie into the state's ``trie_buf`` in one host-to-device copy and put every row at its root.  Returns
+    the kernel's (node_ptr, child_tok, child_node, n_nodes) views."""
+    def alloc(ncap, ecap):
+        st.trie_buf = torch.empty(ncap + 2 + 2 * ecap, dtype=torch.int32, device=st.next_ids.device)
+    ncap, ecap = _grow(st, "trie_cap", (table.n_nodes, max(table.n_edges, 1)), alloc)
+    st.trie_buf.copy_(torch.from_numpy(table.pack(ncap, ecap)))
+    st.node.zero_()                                 # every row starts at the root
+    st.miss.zero_()
+    o = ncap + 2
+    return st.trie_buf[:o], st.trie_buf[o:o + ecap], st.trie_buf[o + ecap:], ncap
+
+
+def load_proc(st, input_ids, rows: int, G: int) -> None:
+    """The logits processors' device state in persistent buffers of ``st``: the padded prompt ids ``proc_ids`` [P, >= S] and
+    their width S ``proc_width`` [1], copied once per call, and -- for ``rows`` > 0 -- the generated history ``proc_hist``
+    [rows, >= G] with its per-row length ``proc_len`` (zeroed; the step appends to it)."""
+    P, S = input_ids.shape
+    dev = st.next_ids.device
+
+    def alloc(scap, gcap):
+        st.proc_ids = torch.zeros((P, scap), dtype=torch.int32, device=dev)
+        st.proc_width = torch.zeros((1,), dtype=torch.int32, device=dev)
+        if rows:
+            st.proc_hist = torch.zeros((rows, gcap), dtype=torch.int32, device=dev)
+            st.proc_len = torch.zeros((rows,), dtype=torch.int32, device=dev)
+    _grow(st, "proc_cap", (S, G if rows else 0), alloc)
+    st.proc_ids[:, :S].copy_(input_ids.to(torch.int32))
+    st.proc_width.fill_(S)
+    if rows:
+        st.proc_len.zero_()
+
+
+def prefill(lm, dec: Decoding, input_ids, attention_mask, vis, max_new_tokens: int, want_graph: bool, host: bool = False):
+    """Pack the prompts (positions = cumsum(mask) - 1, as HF generate), find or build the call's decode state and run the
+    prompt forward into its cache; the visual rows (cand, hist, obj) are injected here only, as in
+    models/modified_lm.py:195-197.  Returns the packed prompt, the state and the last hidden row of every prompt.
+
+    One sequence per prompt: kc / vc [B, G, D] per layer hold each row's prompt and generated keys.  Several samples, or
+    beams, per prompt (``dec.n`` > 1): the prompt keys go to a prompt cache ``pk`` / ``pv`` [B, Sp, D] that the n rows of a
+    prompt share (``plens`` keys each), and kc / vc [B * n, G, D] hold only the generated keys, read through the source table
+    ``src`` (``st.beam``), so no K/V is copied.  Sampling adds its uniform numbers ``u`` (the host processors draw their
+    own), tries their masked logits and walk state, beams the scorer's buffers (``ops.beam_select``)."""
+    from .modified_lm import PackedPrompt           # modified_lm imports this module
+    dev, d = lm._device(), lm.dims
+    pp = PackedPrompt(input_ids, attention_mask, lm, dev, generate_positions=True)
+    vis = lm.cat_vis(*vis, pp)
+    bucket = lambda n: (n + 127) // 128 * 128       # cache lengths in multiples of 128: more calls share a state
+    B, n, V = pp.B, dec.n, lm.lm_head.weight.shape[0]
+    R, shared = B * n, n > 1
+    Sp, G = (bucket(max(pp.seqlens)), bucket(max_new_tokens)) if shared else (0, bucket(max(pp.seqlens) + max_new_tokens))
+
+    def build():
+        cache = lambda rows, length: llama_mod.kv_cache(d, rows, length, dec.kv, dev)
+        zeros = lambda dtype, *shape: torch.zeros(shape, dtype=dtype, device=dev)
+        i32 = lambda *shape: zeros(torch.int32, *shape)
+        st = SimpleNamespace(kc=cache(R, G), vc=cache(R, G), logits=logits_buffer(R, V, dev), next_ids=i32(R), lens=i32(R),
+                             Sp=Sp, G=G, graph=None)
+        if dec.mode == "beam":
+            st.beam_score, st.cand_score, st.cand_tok = zeros(torch.float32, R), zeros(torch.float32, B, 2 * n), i32(B, 2 * n)
+            st.cand_par, st.hist, st.src, st.hyp_score = i32(B, 2 * n), i32(R, G), i32(R, G), zeros(torch.float64, B, n + 1)
+            st.hyp_meta, st.hyp_tok, st.pstate, st.norm = i32(B, n, 2), i32(B, n, G), i32(B, 5), zeros(torch.float64, G)
+        else:
+            st.finished = i32(R)
+            if shared:                                                      # the identity source table
+                st.src = torch.arange(R, dtype=torch.int32, device=dev)[:, None].expand(R, G).contiguous()
+        if shared:
+            st.pk, st.pv, st.plens = cache(B, Sp), cache(B, Sp), i32(B)
+            st.beam = SimpleNamespace(pk=st.pk, pv=st.pv, plens=st.plens, src=st.src, K=n)
+        if dec.sampled and not host:
+            st.u = torch.empty((R,), dtype=torch.float32, device=dev)
+        if dec.trie_eos is not None:
+            st.masked, st.node, st.miss = logits_buffer(R, V, dev), i32(R), i32(1)
+        return st
+    st = lm._decode_states.lookup((R, G, (B, Sp) if shared else None) + dec.key(), build, want_graph)
+    if shared:
+        st.plens.copy_(torch.tensor(pp.seqlens, dtype=torch.int32), non_blocking=True)
+    x = ops.embed_fwd(pp.ids, lm.model.embed_tokens.weight.data, pp.vis_src if vis is not None else None, vis)
+    h, _ = lm.core.forward(x, pp.pos, pp.cu, pp.seqlens, save=False, kv_store=(st.pk, st.pv) if shared else (st.kc, st.vc),
+                           out_rows=pp.last_rows)
+    return pp, st, h
+
+
+def decode_head(lm, h_rows: torch.Tensor, out: torch.Tensor) -> None:
+    """Final RMSNorm + lm_head of decode rows into ``out`` [rows, V] bf16 (the fp8 weight copy when there is one)."""
+    B = h_rows.shape[0]
+    hn, _ = ops.rmsnorm_fwd(h_rows, lm.model.norm.weight.data, lm.dims.rms_eps)
+    fp8_head = lm._fp8.view([lm.lm_head.weight], tuple(lm.lm_head.weight.shape)) if lm.core.fp8 is not None else None
+    if B <= 16 and fp8_head is not None:
+        ops.gemm_skinny_fp8(hn, *fp8_head, out=out)
+    elif B <= llama_mod.FP8_MAX_ROWS and fp8_head is not None:
+        ops.gemm_fp8w(hn, *fp8_head, out=out)
+    elif B <= 16:
+        ops.gemm_skinny(hn, lm.lm_head.weight.data, out=out)
+    else:
+        ops.gemm(hn, lm.lm_head.weight.data, out=out)
+
+
+def step_loop(st, step, n_tokens: int, done, every: int, graphed: bool, before=None, after=None) -> tuple:
+    """Steps for tokens 1 .. n_tokens - 1: ``step()``, or -- ``graphed`` -- replays of ``st.graph``, captured after the eager
+    step of the first iteration that finds none (which yields that iteration's token).  ``done()`` (if not None) is asked
+    every ``every`` tokens and ends the loop; ``before()`` / ``after()`` run around each step.  Returns (steps, replays)."""
+    it, replays = 1, 0
+    while it < n_tokens:
+        if done is not None and it % every == 0 and done():
+            break
+        if before is not None:
+            before()
+        if graphed and st.graph is not None:
+            st.graph.replay()
+            replays += 1
+        else:
+            step()
+        if after is not None:
+            after()
+        if graphed and st.graph is None:
+            g = torch.cuda.CUDAGraph()
+            torch.cuda.synchronize()
+            with torch.cuda.graph(g):
+                step()
+            st.graph = g
+        it += 1
+    return it - 1, replays
+
+
+class PhaseTimer:
+    """Device-side phase times of one call for ``stats=`` (bench.py reads prefill_ms, decode_ms and decode_steps): events at
+    the start, after the prefill's token (``mark()``) and after the decode steps; one synchronise at the end."""
+
+    def __init__(self, stats: Optional[dict]):
+        self.stats, self.ev = stats, []
+        self.mark()
+
+    def mark(self) -> None:
+        if self.stats is not None:
+            self.ev.append(torch.cuda.Event(enable_timing=True))
+            self.ev[-1].record()
+
+    def finish(self, pp, steps: int, replays: int, kv_rows: int, **extra) -> None:
+        if self.stats is not None:
+            self.mark()
+            torch.cuda.synchronize()
+            ev = self.ev
+            self.stats.update({"prefill_ms": ev[0].elapsed_time(ev[1]), "decode_ms": ev[1].elapsed_time(ev[2]) if steps else None,
+                              "decode_steps": steps, "graph_replays": replays, "kv_rows": kv_rows,
+                              "prompt_lens": list(pp.seqlens), **extra})
+
+
+def decode(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph, stats, dec: Decoding, procs=(), table=None):
+    """``generate`` without beams, with the host processors ``procs`` (the host path when not empty) or the flattened trie
+    ``table`` walked on the device; returns None when the device walk reported a miss.  ``dec.n`` > 1 (sampling without
+    processors): the n samples of a prompt start from its last hidden row, over its prompt cache; the visual tokens of
+    prompt b reach all n samples of prompt b."""
+    timer = PhaseTimer(stats)
+    host = bool(procs)                                        # processors walk the generated ids on the host
+    graphed = use_cuda_graph and not host
+    pp, st, hid_last = prefill(lm, dec, input_ids, attention_mask, vis, max_new_tokens, graphed, host)
+    dev, n = lm._device(), dec.n
+    R, shared = pp.B * n, n > 1                               # decode rows; shared: a prompt cache per prompt
+    logits, next_ids, finished, lens = st.logits, st.next_ids, st.finished, st.lens
+    if table is not None:
+        trie_csr = load_trie(st, table)
+    if dec.proc is not None:
+        load_proc(st, input_ids, R, max_new_tokens)
+    finished.zero_()
+    lens.copy_(torch.tensor(pp.seqlens, dtype=torch.int32).repeat_interleave(n), non_blocking=True)
+    if shared:                                                # the n samples of a prompt start from its last row
+        hid_last = hid_last.repeat_interleave(n, dim=0)
+    special, eos, pad, stop = lm.special_ids_dev, dec.eos, dec.pad, dec.stop_on_eos
+
+    def head(h_rows, append=None):
+        """lm_head into `logits`, then the logits processors, whose history first takes the token in `append`."""
+        decode_head(lm, h_rows, logits)
+        if dec.proc is not None:
+            ops.logits_process_(logits, st.proc_ids, st.proc_width, st.proc_hist, st.proc_len, append, dec.proc,
+                                rows_per_prompt=n)
+
+    def pick_host(all_ids_host):
+        """next token from `logits` -> next_ids (device), through the host processors."""
+        lg = logits.float()
+        lg[:, lm.special_token_ids] = float("-inf")
+        for p in procs:
+            lg = p(torch.tensor(all_ids_host, device=dev), lg)
+        if dec.sampled:
+            ops.sample(lg.to(torch.bfloat16), special, finished, eos, pad, stop, dec.temperature, dec.top_k, dec.top_p,
+                       torch.rand(R, device=dev, dtype=torch.float32), next_ids)
+            return
+        nxt = lg.argmax(dim=-1)
+        fin = finished.bool()
+        nxt = torch.where(fin, torch.full_like(nxt, pad), nxt)
+        if stop:
+            finished.copy_((fin | (nxt == eos)).to(torch.int32))
+        next_ids.copy_(nxt.to(torch.int32))
+
+    def pick(advance):
+        """next token from `logits` -> next_ids (device) without host work; with a trie, the row's node first advances by
+        the token in next_ids (``advance``) and the pick reads the trie-masked copy of the logits."""
+        src = logits
+        if table is not None:
+            ops.trie_mask(logits, st.masked, *trie_csr, table.eos, special, st.node, next_ids if advance else None, st.miss)
+            src = st.masked
+        if dec.sampled:
+            st.u.uniform_()                                   # = torch.rand(R): the same numbers, into a static buffer
+            ops.sample(src, special, finished, eos, pad, stop, dec.temperature, dec.top_k, dec.top_p, st.u, next_ids)
+        else:
+            ops.argmax_masked(src, special, finished, eos, pad, stop, next_ids)
+
+    head(hid_last)
+    host_ids = [row.tolist() for row in input_ids.cpu()] if host else None
+    if host:
+        pick_host(host_ids)
+    else:
+        pick(advance=False)
+    out_tokens = [next_ids.clone()]
+    timer.mark()
+
+    def step():
+        with ops.pdl():                         # programmatic dependent launch along the whole decode chain
+            xt = ops.embed_fwd(next_ids, lm.model.embed_tokens.weight.data)
+            h = lm.core.decode_step(xt, lens, st.kc, st.vc, beam=st.beam if shared else None)
+            head(h, append=next_ids)
+            ops.add_int_(lens, 1)
+            if not host:
+                pick(advance=True)
+        if host:
+            pick_host(host_ids)
+
+    def append_host_ids():
+        for bn, t in enumerate(out_tokens[-1].tolist()):
+            host_ids[bn].append(t)
+
+    # HF stops when every sequence has finished.  Asking the device after EVERY token would serialise host and device
+    # (one blocking read per token); finished rows only emit pad tokens, so the greedy and sampled loops look every
+    # `check_every` tokens and the surplus pad columns are trimmed below -- same ids as a per-token check.  Trie-constrained
+    # answers are a handful of tokens: there the check stays per token, as on the host path.
+    check_every = 1 if host or table is not None else 8
+    steps, replays = step_loop(st, step, max_new_tokens, (lambda: bool(finished.all())) if stop else None, check_every, graphed,
+                               before=append_host_ids if host else None, after=lambda: out_tokens.append(next_ids.clone()))
+    miss = False
+    if table is not None:
+        # one more advance, outside the graph: a token picked at the last step that is not a child is a miss as well
+        ops.trie_mask(logits, st.masked, *trie_csr, table.eos, special, st.node, next_ids, st.miss)
+        miss = bool(st.miss.item())
+    timer.finish(pp, steps, replays, st.Sp + st.G)
+    if miss:
+        return None
+    new = torch.stack(out_tokens, dim=1).to(torch.int64)
+    if stop and check_every > 1 and new.shape[1] > 1:
+        # trim the columns generated after the step at which the last row emitted EOS (see check_every above)
+        is_eos = (new == eos)
+        if bool(is_eos.any(dim=1).all()):
+            last = int(is_eos.float().argmax(dim=1).max())        # first EOS per row; the slowest row decides
+            new = new[:, :last + 1]
+    return torch.cat([input_ids.to(dev).repeat_interleave(n, dim=0), new], dim=1)
+
+
+# ---- beam search (HF GenerationMixin.beam_search / BeamSearchScorer, transformers 4.28 as the reference pins it) ----
+def beam_search(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph, stats, dec: Decoding):
+    """Beam search over B prompts with K = ``dec.n`` beams each.  The prefill runs once per prompt into the prompt cache, whose
+    keys the K beams of the prompt share; generated keys live in a [B * K, G] cache that is written once per slot and read
+    through the source table ``src`` (reordering the beams gathers ``src``, never K/V).  Each step is ``nv_beam_topk`` (2K
+    best candidates per prompt) and ``nv_beam_select`` (the scorer), all on the device, and is replayed as a CUDA graph; the
+    hypotheses are finalized on the host after one device-to-host copy.  The visual tokens of prompt b reach all K beams of
+    prompt b (the reference's HF expansion of ``cand_vis`` would hand them to other rows' slots).  With logits processors
+    (``dec.proc``) the scoring is ``nv_beam_topk_processed`` over the beams' histories (prompt ids, ``hist``)."""
+    K, eos, pad, proc, special = dec.n, dec.eos, dec.pad, dec.proc, lm.special_ids_dev
+    if K > BEAM_MAX:
+        raise NotImplementedError(f"generate(num_beams={K}): at most {BEAM_MAX} beams are built")
+    if max_new_tokens < 1:
+        raise ValueError("generate(num_beams > 1) needs max_new_tokens >= 1")
+    timer = PhaseTimer(stats)
+    pp, st, hid_last = prefill(lm, dec, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph)
+    B, S, G = pp.B, int(input_ids.shape[1]), st.G
+    if proc is not None:
+        load_proc(st, input_ids, 0, G)
+    st.beam_score.view(B, K).fill_(-1e9)[:, 0] = 0.0             # only beam 0 of a prompt expands at the first step
+    st.hyp_score.zero_()
+    st.hyp_score[:, K] = 1e9                                      # BeamHypotheses.worst_score starts at 1e9
+    st.hyp_meta.zero_()
+    st.pstate.zero_()
+    st.pstate[:, 1].copy_(st.plens)
+    st.norm.copy_(ops.beam_norm(S, G, dec.length_penalty))
+    decode_head(lm, hid_last, st.logits[:B])
+    sel = lambda: ops.beam_select(st.cand_score, st.cand_tok, st.cand_par, st.beam_score, st.hist, st.src, st.hyp_score,
+                                  st.hyp_meta, st.hyp_tok, st.pstate, st.next_ids, st.lens, st.norm, eos, pad,
+                                  dec.early_stopping)
+
+    def topk(first_step=False):
+        if proc is None:
+            ops.beam_topk(st.logits, special, st.beam_score, K, st.cand_score, st.cand_tok, st.cand_par, first_step=first_step)
+        else:
+            ops.beam_topk_processed(st.logits, special, st.beam_score, K, st.cand_score, st.cand_tok, st.cand_par, st.proc_ids,
+                                    st.proc_width, st.hist, st.pstate, proc, first_step=first_step)
+
+    topk(first_step=True)
+    sel()
+    timer.mark()
+
+    def step():
+        with ops.pdl():
+            xt = ops.embed_fwd(st.next_ids, lm.model.embed_tokens.weight.data)
+            h = lm.core.decode_step(xt, st.lens, st.kc, st.vc, beam=st.beam)
+            decode_head(lm, h, st.logits)
+            topk()
+            sel()
+
+    # like the greedy loop, ask the device whether every prompt is done only every few steps: a done prompt's steps leave
+    # its hypotheses unchanged, so the extra steps change no output
+    steps, replays = step_loop(st, step, max_new_tokens, lambda: bool(st.pstate[:, 4].all()), 8, use_cuda_graph)
+    timer.finish(pp, steps, replays, st.Sp + G, beam_steps=steps + 1)          # beam steps: tokens generated
+    # one copy; the fp64 scores go first, so their view starts at an even int32 offset whatever B and K are
+    parts = [st.hyp_score.flatten().view(torch.int32), st.hist.flatten(), st.hyp_meta.flatten(), st.hyp_tok.flatten(),
+             st.pstate.flatten(), st.beam_score.view(torch.int32)]
+    hyp_score, hist, hyp_meta, hyp_tok, pstate, beam_score = torch.cat(parts).cpu().split([t.numel() for t in parts])
+    hyp_score, beam_score = hyp_score.view(torch.float64).view(B, K + 1), beam_score.view(torch.float32)
+    hist, hyp_meta, hyp_tok, pstate = hist.view(B * K, G), hyp_meta.view(B, K, 2), hyp_tok.view(B, K, G), pstate.view(B, 5)
+    T_done = int(pstate[0, 0])
+    hyps, running = [], []
+    for b in range(B):
+        n = int(pstate[b, 2])
+        kept = sorted(range(n), key=lambda i: int(hyp_meta[b, i, 1]))          # insertion order
+        hyps.append([(float(hyp_score[b, i]), hyp_tok[b, i, :int(hyp_meta[b, i, 0])].tolist()) for i in kept])
+        running.append(None if int(pstate[b, 4]) else
+                       [(float(beam_score[b * K + k]), hist[b * K + k, :T_done].tolist()) for k in range(K)])
+    seqs = beam_finalize(hyps, [float(hyp_score[b, K]) for b in range(B)], running, S, T_done, K, dec.n_return,
+                         dec.length_penalty)
+    return beam_output(input_ids.cpu(), seqs, S, S + max_new_tokens, eos, pad).to(lm._device())
+
+
+def beam_finalize(hyps, worst, running, S: int, T: int, K: int, n_return: int, length_penalty: float):
+    """BeamSearchScorer.finalize of transformers 4.28: prompts that are not done add their K running beams (score
+    sum_logprobs / (S + T) ** length_penalty, the Python float arithmetic of BeamHypotheses.add), then each prompt returns its
+    ``n_return`` best hypotheses, best first; of equal scores the one added last wins (a stable sort, popped from the end).
+    hyps[b]: the kept (score, generated tokens) in insertion order; worst[b]: their worst_score; running[b]: the K (running
+    score, tokens) of a prompt that is not done, else None.  Returns [[generated tokens] * n_return] per prompt."""
+    out = []
+    for b, beams in enumerate(hyps):
+        beams, w = list(beams), worst[b]
+        for sc, toks in (running[b] or []):
+            score = sc / ((S + T) ** length_penalty)
+            if len(beams) < K or score > w:
+                beams.append((score, toks))
+                if len(beams) > K:
+                    order = sorted([(s, i) for i, (s, _) in enumerate(beams)])
+                    del beams[order[0][1]]
+                    w = order[1][0]
+                else:
+                    w = min(score, w)
+        ranked = sorted(beams, key=lambda x: x[0])
+        out.append([ranked.pop()[1] for _ in range(n_return)])
+    return out
+
+
+def beam_output(prompt_ids: torch.Tensor, seqs, S: int, max_length: int, eos: int, pad: int) -> torch.Tensor:
+    """HF ``sequences`` of a beam search: [B * n, L] int64 rows of prompt ids and generated tokens, L = min(longest + 1,
+    max_length); a row shorter than L gets EOS after its tokens, then pad."""
+    rows = [(b, toks) for b, per in enumerate(seqs) for toks in per]
+    L = min(max(S + len(t) for _, t in rows) + 1, max_length)
+    out = torch.full((len(rows), L), pad, dtype=torch.int64)
+    for i, (b, toks) in enumerate(rows):
+        n = S + len(toks)
+        out[i, :S] = prompt_ids[b]
+        out[i, S:n] = torch.tensor(toks, dtype=torch.int64)
+        if n < L:
+            out[i, n] = eos
+    return out

@@ -14,7 +14,7 @@ reference holds values computed from pad embeddings that nothing reads.
 """
 from __future__ import annotations
 
-import collections
+import dataclasses
 import time
 import weakref
 from types import SimpleNamespace
@@ -24,7 +24,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from . import llama as llama_mod
+from . import generation
 from . import ops
 from . import trie as trie_mod
 from .llama import FlatParams, Fp8Weights, LlamaCore, LlamaDims, LlamaModelParams, WgradStash, _Linear, kv_cache
@@ -382,7 +382,7 @@ class _LMFn(torch.autograd.Function):
             return hn
         # ---- LM loss on the label rows only ----
         V = lm.lm_head.weight.shape[0]
-        logits = torch.empty((g.shape[0], (V + 63) // 64 * 64), dtype=bf16, device=g.device)[:, :V]   # 16-byte aligned rows
+        logits = generation.logits_buffer(g.shape[0], V, g.device)
         ops.gemm(hn, lm.lm_head.weight.data, out=logits)                 # [Nl, V] bf16
         row_loss, dlogits = ops.ce_fwd_bwd(logits, pp.loss_tgt, lm.special_ids_dev,
                                            grad_scale=(1.0 / max(pp.n_loss, 1)) if train else None)
@@ -451,6 +451,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
         self.grad_sync.flats = self._own_flats
         self.grad_sync.before_exchange = self.complete_pending_grads
         self._prefix_caches = weakref.WeakSet()      # PrefixKVCache(train=True) instances built on this model
+        self._decode_states = generation.DecodeStates()  # generate()'s KV caches and captured decode graphs
         if tokenizer is not None:
             self._set_tokenizer(tokenizer)
 
@@ -517,7 +518,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
         if extra_params is not None:
             self._extra_params = list(extra_params)
         params = self.lm_parameters() + list(getattr(self, "_extra_params", []))
-        self.__dict__.pop("_decode_states", None)     # captured decode graphs hold pointers into the old buffers
+        self._decode_states.clear()                  # captured decode graphs hold pointers into the old buffers
         self.flat = FlatParams(params, device)
         self.flat.clean_segments = self._clean_grad_segments
         self.flat.on_zeroed = self.mark_grads_zeroed
@@ -741,7 +742,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
         self._fp8 = None
         if self.core is not None:
             self.core.set_fp8(None)
-        self.__dict__.pop("_decode_states", None)     # captured decode graphs hold the pointers of the other kernels
+        self._decode_states.clear()                  # captured decode graphs hold the pointers of the other kernels
 
     @property
     def fp8_weights(self) -> Optional[Fp8Weights]:
@@ -852,121 +853,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
         prev, self.kv_cache_dtype = self.kv_cache_dtype, dtype
         return prev
 
-    # ---- generation (models/nav_model.py:324-338,388-399; HF GenerationMixin greedy / sampling) ----
-    max_decode_states = 2        # cached (KV buffers + captured decode graph) sets, least recently used evicted
-
-    def _decode_state(self, B: int, Smax: int, key_extra: tuple, want_graph: bool, prompts: Optional[tuple] = None):
-        """Persistent per-shape decode state: the contiguous KV cache [B, Smax, D] per layer (in ``kv_cache_dtype``; the caller
-        puts that format in ``key_extra``, so a graph is never replayed over the other one), the step's I/O buffers and --
-        once captured -- the CUDA graph of ONE decode step.  Capturing and instantiating the ~260-node graph costs more than
-        the 127 replays of a C3 generation save, so it is done once per (batch, cache length, stop rule, decoding mode and
-        the scalars the step bakes in) and reused by every later ``generate`` call (evaluation loops call generate with the
-        same shapes over and over).  The trie-constrained modes keep their flattened trie in ``trie_buf`` (see
-        ``_load_trie``), sampled modes their uniform numbers in ``u``.
-
-        ``prompts = (P, Sp)`` (several samples per prompt): the B rows are B / P samples of each of P prompts; the prompt
-        keys go to a prompt cache ``pk`` / ``pv`` [P, Sp, D] that the samples of a prompt share (``plens`` keys each), and
-        kc / vc hold only the generated keys, read through the identity source table ``src`` (the beam-search attention)."""
-        states = self.__dict__.setdefault("_decode_states", collections.OrderedDict())
-        key = (B, Smax, prompts) + key_extra
-        st = states.get(key) if want_graph else None
-        if st is not None:
-            states.move_to_end(key)
-            return st
-        dev, d = self._device(), self.dims
-        V = self.lm_head.weight.shape[0]
-        st = SimpleNamespace(
-            kc=kv_cache(d, B, Smax, self.kv_cache_dtype, dev), vc=kv_cache(d, B, Smax, self.kv_cache_dtype, dev),
-            logits=torch.empty((B, (V + 63) // 64 * 64), dtype=bf16, device=dev)[:, :V],
-            next_ids=torch.empty((B,), dtype=torch.int32, device=dev),
-            finished=torch.zeros((B,), dtype=torch.int32, device=dev),
-            lens=torch.zeros((B,), dtype=torch.int32, device=dev), graph=None,
-            u=None, masked=None, node=None, miss=None, trie_buf=None, trie_cap=(0, 0))
-        if prompts is not None:
-            P, Sp = prompts
-            st.pk, st.pv = kv_cache(d, P, Sp, self.kv_cache_dtype, dev), kv_cache(d, P, Sp, self.kv_cache_dtype, dev)
-            st.plens = torch.zeros((P,), dtype=torch.int32, device=dev)
-            st.src = torch.arange(B, dtype=torch.int32, device=dev)[:, None].expand(B, Smax).contiguous()
-        if want_graph:
-            states[key] = st
-            while len(states) > self.max_decode_states:
-                states.popitem(last=False)
-        return st
-
-    def _decode_head(self, h_rows: torch.Tensor, out: torch.Tensor) -> None:
-        """Final RMSNorm + lm_head of decode rows into ``out`` [rows, V] bf16 (the fp8 weight copy when there is one)."""
-        B = h_rows.shape[0]
-        hn, _ = ops.rmsnorm_fwd(h_rows, self.model.norm.weight.data, self.dims.rms_eps)
-        fp8_head = None
-        if self.core.fp8 is not None:
-            fp8_head = self._fp8.view([self.lm_head.weight], tuple(self.lm_head.weight.shape))
-        if B <= 16 and fp8_head is not None:
-            ops.gemm_skinny_fp8(hn, *fp8_head, out=out)
-        elif B <= llama_mod.FP8_MAX_ROWS and fp8_head is not None:
-            ops.gemm_fp8w(hn, *fp8_head, out=out)
-        elif B <= 16:
-            ops.gemm_skinny(hn, self.lm_head.weight.data, out=out)
-        else:
-            ops.gemm(hn, self.lm_head.weight.data, out=out)
-
-    @staticmethod
-    def _load_trie(st, table) -> tuple:
-        """Copy a flattened trie into the state's persistent device buffers (a captured graph keeps their pointers) in one
-        host-to-device copy.  Capacities grow in powers of two; growing drops the state's graph.  Returns the kernel's
-        (node_ptr, child_tok, child_node, n_nodes) views."""
-        ncap, ecap = st.trie_cap
-        if table.n_nodes > ncap or table.n_edges > ecap:
-            pow2 = lambda n: 1 << max(0, int(n) - 1).bit_length()
-            ncap, ecap = max(ncap, pow2(table.n_nodes)), max(ecap, pow2(max(table.n_edges, 1)))
-            st.trie_buf = torch.empty(ncap + 2 + 2 * ecap, dtype=torch.int32, device=st.next_ids.device)
-            st.trie_cap = (ncap, ecap)
-            st.graph = None
-        st.trie_buf.copy_(torch.from_numpy(table.pack(ncap, ecap)))
-        o = ncap + 2
-        return st.trie_buf[:o], st.trie_buf[o:o + ecap], st.trie_buf[o + ecap:], ncap
-
-    @staticmethod
-    def _load_proc(st, input_ids, rows: int, G: int) -> None:
-        """The logits processors' device state in persistent buffers of ``st`` (a captured step keeps their pointers): the padded
-        prompt ids ``proc_ids`` [P, >= S] and their width S ``proc_width`` [1], copied once per call, and -- for ``rows`` > 0 --
-        the generated history ``proc_hist`` [rows, >= G] with its per-row length ``proc_len`` (zeroed; the step appends to it).
-        Capacities grow in powers of two; growing drops the state's graph."""
-        P, S = input_ids.shape
-        dev = st.next_ids.device
-        scap, gcap = getattr(st, "proc_cap", (0, 0))
-        if S > scap or (rows and G > gcap):
-            pow2 = lambda n: 1 << max(0, int(n) - 1).bit_length()
-            scap, gcap = max(scap, pow2(S)), max(gcap, pow2(G) if rows else 0)
-            st.proc_ids = torch.zeros((P, scap), dtype=torch.int32, device=dev)
-            st.proc_width = torch.zeros((1,), dtype=torch.int32, device=dev)
-            if rows:
-                st.proc_hist = torch.zeros((rows, gcap), dtype=torch.int32, device=dev)
-                st.proc_len = torch.zeros((rows,), dtype=torch.int32, device=dev)
-            st.proc_cap = (scap, gcap)
-            st.graph = None
-        st.proc_ids[:, :S].copy_(input_ids.to(torch.int32))
-        st.proc_width.fill_(S)
-        if rows:
-            st.proc_len.zero_()
-
-    @staticmethod
-    def _processors(repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens, eos: int) -> Optional[tuple]:
-        """Validate HF's processor kwargs as transformers does; returns (penalty, n, min_length, min_new_tokens, eos) for the
-        kernels, or None when every one is at its default (off), which keeps the call on the processor-free path."""
-        p = 1.0 if repetition_penalty is None else repetition_penalty
-        if p != 1.0 and (isinstance(p, bool) or not isinstance(p, float) or not p > 0):
-            raise ValueError(f"generate(repetition_penalty={repetition_penalty!r}): has to be a strictly positive float")
-        named = (("no_repeat_ngram_size", no_repeat_ngram_size), ("min_length", min_length), ("min_new_tokens", min_new_tokens))
-        ints = []
-        for name, v in named:
-            v = 0 if v is None else v
-            if isinstance(v, bool) or not isinstance(v, int) or v < 0:
-                raise ValueError(f"generate({name}={v!r}): has to be a non-negative integer")
-            ints.append(v)
-        if p == 1.0 and not any(ints):
-            return None
-        return (float(p), *ints, int(eos))
-
+    # ---- generation (models/nav_model.py:324-338,388-399; HF GenerationMixin; navillm_b200/generation.py) ----
     @torch.no_grad()
     def generate(self, input_ids, attention_mask, cand_vis=None, hist_vis=None, obj_vis=None, max_new_tokens: int = 20,
                  do_sample: bool = False, temperature: float = 1.0, eos_token_id: Optional[int] = None,
@@ -979,7 +866,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
         """Prefill on the packed kernels (positions = cumsum(mask)-1 like HF generate; visual tokens injected only
         here, as in models/modified_lm.py:195-197), then one token per step over a pre-allocated KV cache.  The
         decode step of the greedy, sampled and trie-constrained modes has static shapes and is replayed as a CUDA graph
-        (captured once per shape and mode, see ``_decode_state``); generic ``logits_processor=`` calls run eagerly.
+        (captured once per shape and mode, see ``generation.DecodeStates``); generic ``logits_processor=`` calls run eagerly.
         Returns [B, S0 + n_new] int64 ids (prompt part copied from the input; finished rows continue with pad_token_id
         like HF greedy search).
 
@@ -1000,12 +887,12 @@ class ModifiedLlamaForCausalLM(nn.Module):
         ignore it, as HF does.
 
         ``num_beams > 1`` is HF beam search as transformers 4.28 (the reference's pin) runs it, ``length_penalty``,
-        ``early_stopping`` and ``num_return_sequences`` included; see ``_generate_beam``.  Returns [B * num_return_sequences,
+        ``early_stopping`` and ``num_return_sequences`` included; see ``generation.beam_search``.  Returns [B * num_return_sequences,
         L] ids.  Beam sampling, group beam search, ``trie=`` / ``logits_processor=`` with beams and more return sequences than
         beams raise ``NotImplementedError``.
 
         ``do_sample=True, num_return_sequences=N`` draws N samples per prompt: [B * N, L] ids, row b * N + j a sample of
-        prompt b (HF's order).  Each prompt is prefilled once and its N rows share its KV cache (``_generate``); the tokens
+        prompt b (HF's order).  Each prompt is prefilled once and its N rows share its KV cache (``generation.decode``); the tokens
         are those of the same call on the prompts repeated N times.  With ``trie=`` / ``logits_processor=``, and without
         ``do_sample``, N > 1 raises ``NotImplementedError``.
 
@@ -1045,394 +932,35 @@ class ModifiedLlamaForCausalLM(nn.Module):
         dev = self._device()
         eos = self.tokenizer.eos_token_id if eos_token_id is None else eos_token_id
         pad = self.tokenizer.unk_token_id if pad_token_id is None else pad_token_id
-        proc = self._processors(repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens, eos)
+        proc = generation.processors(repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens, eos)
+        call = (self, input_ids, attention_mask, (cand_vis, hist_vis, obj_vis), max_new_tokens, use_cuda_graph, stats)
         if num_beams > 1:
-            return self._generate_beam(input_ids, attention_mask, cand_vis, hist_vis, obj_vis, max_new_tokens, int(num_beams), eos,
-                                       pad, float(length_penalty), bool(early_stopping), int(num_return_sequences), use_cuda_graph,
-                                       stats, proc)
+            dec = generation.Decoding(int(eos), int(pad), None, "beam", self.kv_cache_dtype, n=int(num_beams), n_return=n_seq,
+                                      length_penalty=float(length_penalty), early_stopping=bool(early_stopping), proc=proc)
+            return generation.beam_search(*call, dec)
         procs = list(logits_processor or [])
-        args = (input_ids, attention_mask, cand_vis, hist_vis, obj_vis, max_new_tokens, do_sample, temperature, eos, pad,
-                stop_on_eos, use_cuda_graph, stats, top_k, top_p, max(1, n_seq), proc)
-        table, path = None, None
+        table = None
         if trie is not None and not procs:
             t0 = time.perf_counter()
             table = trie_mod.flatten_trie(trie, self.lm_head.weight.shape[0])
             flatten_ms = 1e3 * (time.perf_counter() - t0)
+        sampling = dict(temperature=float(temperature), top_k=int(top_k), top_p=top_p) if do_sample else {}
+        dec = generation.Decoding(int(eos), int(pad), bool(stop_on_eos), "sample" if do_sample else "greedy", self.kv_cache_dtype,
+                                  n=max(1, n_seq), proc=proc, **sampling)
         if table is not None:
             rng = torch.cuda.get_rng_state(dev) if do_sample else None
-            out = self._generate(*args, procs=[], table=table)
+            trie_dec = dataclasses.replace(dec, mode="trie+sample" if do_sample else "trie", trie_eos=table.eos)
+            out = generation.decode(*call, trie_dec, table=table)
             path = "device" if out is not None else "device_miss_host"
             if out is None:
                 if rng is not None:
                     torch.cuda.set_rng_state(rng, dev)
-                out = self._generate(*args, procs=[trie_mod.TrieLogitsProcessor(trie)], table=None)
+                out = generation.decode(*call, dec, procs=[trie_mod.TrieLogitsProcessor(trie)])
         else:
             if trie is not None:
                 procs = [trie_mod.TrieLogitsProcessor(trie)] + procs
                 path = "host"
-            out = self._generate(*args, procs=procs, table=None)
+            out = generation.decode(*call, dec, procs=procs)
         if stats is not None and trie is not None:
             stats.update({"trie_path": path, "trie_flatten_ms": flatten_ms if table is not None else None})
         return out
-
-    def _generate(self, input_ids, attention_mask, cand_vis, hist_vis, obj_vis, max_new_tokens, do_sample, temperature, eos, pad,
-                  stop_on_eos, use_cuda_graph, stats, top_k, top_p, n_seq, proc=None, *, procs, table):
-        """``generate`` with the host processors ``procs`` (the host path when not empty) or the flattened trie ``table``
-        walked on the device; returns None when the device walk reported a miss.
-
-        ``n_seq`` > 1 (sampling without processors): the prefill runs once per prompt into the prompt cache of
-        ``_decode_state(prompts=)``, its last hidden row is repeated for the n_seq rows of the prompt, and the decode steps
-        run over all B * n_seq rows with the beam-search attention over an identity source table, so no K/V is copied.
-        The visual tokens of prompt b reach all n_seq samples of prompt b."""
-        dev = self._device()
-        core, d = self.core, self.dims
-        ev = None
-        if stats is not None:                                     # bench.py: device-side phase times (forces one sync at the end)
-            ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
-            ev[0].record()
-        pp = PackedPrompt(input_ids, attention_mask, self, dev, generate_positions=True)
-        vis = self.cat_vis(cand_vis, hist_vis, obj_vis, pp)
-        B = pp.B
-        R = B * n_seq                                             # decode rows
-        need_host = bool(procs)                                   # processors walk the generated ids on the host
-        graphed = use_cuda_graph and not need_host
-        mode = ("trie+sample" if do_sample else "trie") if table is not None else ("sample" if do_sample else "greedy")
-        key = (int(eos), int(pad), bool(stop_on_eos), mode, float(temperature) if do_sample else None,
-               int(top_k) if do_sample else None, float(top_p) if do_sample else None, table.eos if table is not None else None,
-               self.kv_cache_dtype)
-        if proc is not None:                                      # the processor scalars the captured step bakes in
-            key += (("proc",) + proc,)
-        shared = n_seq > 1
-        if shared:                                                # prompt cache per prompt + generated keys per row
-            Sp = (max(pp.seqlens) + 127) // 128 * 128
-            Smax = (max_new_tokens + 127) // 128 * 128
-            st = self._decode_state(R, Smax, key, graphed, prompts=(B, Sp))
-            st.plens.copy_(torch.tensor(pp.seqlens, dtype=torch.int32), non_blocking=True)
-            beam = SimpleNamespace(pk=st.pk, pv=st.pv, plens=st.plens, src=st.src, K=n_seq)
-        else:
-            Smax = (max(pp.seqlens) + max_new_tokens + 127) // 128 * 128      # bucketed: more reuse of the cached state
-            st = self._decode_state(B, Smax, key, graphed)
-            beam = None
-        kc, vc, logits, next_ids, finished, lens = st.kc, st.vc, st.logits, st.next_ids, st.finished, st.lens
-        if do_sample and not need_host and st.u is None:
-            st.u = torch.empty((R,), dtype=torch.float32, device=dev)
-        if table is not None:
-            if st.masked is None:
-                V = logits.shape[1]
-                st.masked = torch.empty((B, (V + 63) // 64 * 64), dtype=bf16, device=dev)[:, :V]
-                st.node = torch.zeros((B,), dtype=torch.int32, device=dev)
-                st.miss = torch.zeros((1,), dtype=torch.int32, device=dev)
-            trie_csr = self._load_trie(st, table)
-        if proc is not None:
-            self._load_proc(st, input_ids, R, max_new_tokens)
-        finished.zero_()
-        lens.copy_(torch.tensor(pp.seqlens, dtype=torch.int32).repeat_interleave(n_seq), non_blocking=True)
-
-        E = self.model.embed_tokens.weight.data
-        x = ops.embed_fwd(pp.ids, E, pp.vis_src if vis is not None else None, vis)
-        hid_last, _ = core.forward(x, pp.pos, pp.cu, pp.seqlens, save=False, kv_store=(st.pk, st.pv) if shared else (kc, vc),
-                                   out_rows=pp.last_rows)
-        if shared:                                                # the n_seq samples of a prompt start from its last row
-            hid_last = hid_last.repeat_interleave(n_seq, dim=0)
-        special = self.special_ids_dev
-
-        def head(h_rows, append=None):
-            """lm_head into `logits`, then the logits processors, whose history first takes the token in `append`."""
-            self._decode_head(h_rows, logits)
-            if proc is not None:
-                ops.logits_process_(logits, st.proc_ids, st.proc_width, st.proc_hist, st.proc_len, append, proc,
-                                    rows_per_prompt=n_seq)
-
-        def pick_host(all_ids_host):
-            """next token from `logits` -> next_ids (device), through the host processors."""
-            lg = logits.float()
-            lg[:, self.special_token_ids] = float("-inf")
-            for proc in procs:
-                lg = proc(torch.tensor(all_ids_host, device=dev), lg)
-            if do_sample:
-                ops.sample(lg.to(torch.bfloat16), special, finished, eos, pad, stop_on_eos, temperature, top_k, top_p,
-                           torch.rand(B, device=dev, dtype=torch.float32), next_ids)
-                return
-            nxt = lg.argmax(dim=-1)
-            fin = finished.bool()
-            nxt = torch.where(fin, torch.full_like(nxt, pad), nxt)
-            if stop_on_eos:
-                finished.copy_((fin | (nxt == eos)).to(torch.int32))
-            next_ids.copy_(nxt.to(torch.int32))
-
-        def pick(advance):
-            """next token from `logits` -> next_ids (device) without host work; with a trie, the row's node first advances by
-            the token in next_ids (``advance``) and the pick reads the trie-masked copy of the logits."""
-            src = logits
-            if table is not None:
-                ops.trie_mask(logits, st.masked, *trie_csr, table.eos, special, st.node, next_ids if advance else None, st.miss)
-                src = st.masked
-            if do_sample:
-                st.u.uniform_()                                   # = torch.rand(R): the same numbers, into a static buffer
-                ops.sample(src, special, finished, eos, pad, stop_on_eos, temperature, top_k, top_p, st.u, next_ids)
-            else:
-                ops.argmax_masked(src, special, finished, eos, pad, stop_on_eos, next_ids)
-
-        head(hid_last)
-        host_ids = [row.tolist() for row in input_ids.cpu()] if need_host else None
-        if need_host:
-            pick_host(host_ids)
-        else:
-            if table is not None:                                 # every row starts at the root, in stream order
-                st.node.zero_()
-                st.miss.zero_()
-            pick(advance=False)
-        out_tokens = [next_ids.clone()]
-        if ev is not None:
-            ev[1].record()
-
-        def step():
-            with ops.pdl():                         # programmatic dependent launch along the whole decode chain
-                xt = ops.embed_fwd(next_ids, E)
-                h = core.decode_step(xt, lens, kc, vc, beam=beam)
-                head(h, append=next_ids)
-                ops.add_int_(lens, 1)
-                if not need_host:
-                    pick(advance=True)
-
-        # HF stops when every sequence has finished.  Asking the device after EVERY token would serialise host and device
-        # (one blocking read per token); finished rows only emit pad tokens, so the greedy and sampled loops look every
-        # `check_every` tokens and the surplus pad columns are trimmed below -- same ids as a per-token check.  Trie-constrained
-        # answers are a handful of tokens: there the check stays per token, as on the host path.
-        check_every = 1 if need_host or table is not None else 8
-        replays = 0
-        for it in range(1, max_new_tokens):
-            if stop_on_eos and it % check_every == 0 and bool(finished.all()):
-                break
-            if need_host:
-                for bn, t in enumerate(out_tokens[-1].tolist()):
-                    host_ids[bn].append(t)
-            if graphed:
-                if st.graph is None:                              # first generation with this shape: eager step, then capture
-                    step()
-                    out_tokens.append(next_ids.clone())
-                    g = torch.cuda.CUDAGraph()
-                    torch.cuda.synchronize()
-                    with torch.cuda.graph(g):
-                        step()
-                    st.graph = g
-                    continue
-                st.graph.replay()
-                replays += 1
-            else:
-                step()
-                if need_host:
-                    pick_host(host_ids)
-            out_tokens.append(next_ids.clone())
-        miss = False
-        if table is not None:
-            # one more advance, outside the graph: a token picked at the last step that is not a child is a miss as well
-            ops.trie_mask(logits, st.masked, *trie_csr, table.eos, special, st.node, next_ids, st.miss)
-            miss = bool(st.miss.item())
-        if ev is not None:
-            ev[2].record()
-            torch.cuda.synchronize()
-            n_dec = len(out_tokens) - 1
-            stats.update({"prefill_ms": ev[0].elapsed_time(ev[1]), "decode_ms": ev[1].elapsed_time(ev[2]) if n_dec else None,
-                          "decode_steps": n_dec, "graph_replays": replays, "kv_rows": Smax + (Sp if shared else 0),
-                          "prompt_lens": list(pp.seqlens)})
-        if miss:
-            return None
-        new = torch.stack(out_tokens, dim=1).to(torch.int64)
-        if stop_on_eos and check_every > 1 and new.shape[1] > 1:
-            # trim the columns generated after the step at which the last row emitted EOS (see check_every above)
-            is_eos = (new == eos)
-            if bool(is_eos.any(dim=1).all()):
-                last = int(is_eos.float().argmax(dim=1).max())        # first EOS per row; the slowest row decides
-                new = new[:, :last + 1]
-        return torch.cat([input_ids.to(dev).repeat_interleave(n_seq, dim=0), new], dim=1)
-
-    # ---- beam search (HF GenerationMixin.beam_search / BeamSearchScorer, transformers 4.28 as the reference pins it) ----
-    BEAM_MAX = 8
-
-    def _beam_state(self, B: int, K: int, Sp: int, G: int, key_extra: tuple, want_graph: bool):
-        """Persistent beam-search state, cached like ``_decode_state`` (same LRU): the prompt caches [B, Sp, D] per layer the K
-        beams of a prompt share, the generated caches [B * K, G, D] per layer, the device state of ``ops.beam_select`` and
-        the captured graph of one beam step."""
-        states = self.__dict__.setdefault("_decode_states", collections.OrderedDict())
-        key = ("beam", B, K, Sp, G) + key_extra
-        st = states.get(key) if want_graph else None
-        if st is not None:
-            states.move_to_end(key)
-            return st
-        dev, d = self._device(), self.dims
-        V, R = self.lm_head.weight.shape[0], B * K
-        cache = lambda rows, n: kv_cache(d, rows, n, self.kv_cache_dtype, dev)
-        i32 = lambda *shape: torch.zeros(shape, dtype=torch.int32, device=dev)
-        st = SimpleNamespace(
-            pk=cache(B, Sp), pv=cache(B, Sp), kc=cache(R, G), vc=cache(R, G),
-            logits=torch.empty((R, (V + 63) // 64 * 64), dtype=bf16, device=dev)[:, :V],
-            next_ids=i32(R), lens=i32(R), plens=i32(B), beam_score=torch.zeros((R,), dtype=torch.float32, device=dev),
-            cand_score=torch.zeros((B, 2 * K), dtype=torch.float32, device=dev), cand_tok=i32(B, 2 * K), cand_par=i32(B, 2 * K),
-            hist=i32(R, G), src=i32(R, G), hyp_score=torch.zeros((B, K + 1), dtype=torch.float64, device=dev),
-            hyp_meta=i32(B, K, 2), hyp_tok=i32(B, K, G), pstate=i32(B, 5),
-            norm=torch.zeros((G,), dtype=torch.float64, device=dev), graph=None)
-        if want_graph:
-            states[key] = st
-            while len(states) > self.max_decode_states:
-                states.popitem(last=False)
-        return st
-
-    def _generate_beam(self, input_ids, attention_mask, cand_vis, hist_vis, obj_vis, max_new_tokens, K, eos, pad, length_penalty,
-                       early_stopping, n_return, use_cuda_graph, stats, proc=None):
-        """Beam search over B prompts with K beams each.  The prefill runs once per prompt into the prompt cache, whose keys the
-        K beams of the prompt share; generated keys live in a [B * K, G] cache that is written once per slot and read through
-        the source table ``src`` (reordering the beams gathers ``src``, never K/V).  Each step is ``nv_beam_topk`` (2K best
-        candidates per prompt) and ``nv_beam_select`` (the scorer), all on the device, and is replayed as a CUDA graph; the
-        hypotheses are finalized on the host after one device-to-host copy.  The visual tokens of prompt b reach all K beams of
-        prompt b (the reference's HF expansion of ``cand_vis`` would hand them to other rows' slots).  With logits processors
-        (``proc``) the scoring is ``nv_beam_topk_processed`` over the beams' histories (prompt ids, ``hist``)."""
-        if K > self.BEAM_MAX:
-            raise NotImplementedError(f"generate(num_beams={K}): at most {self.BEAM_MAX} beams are built")
-        if max_new_tokens < 1:
-            raise ValueError("generate(num_beams > 1) needs max_new_tokens >= 1")
-        dev = self._device()
-        core, d = self.core, self.dims
-        if d.head_dim != 128:
-            raise NotImplementedError("beam search is built for head_dim = 128")
-        ev = None
-        if stats is not None:
-            ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
-            ev[0].record()
-        pp = PackedPrompt(input_ids, attention_mask, self, dev, generate_positions=True)
-        vis = self.cat_vis(cand_vis, hist_vis, obj_vis, pp)
-        B, S = pp.B, int(input_ids.shape[1])
-        Sp = (max(pp.seqlens) + 127) // 128 * 128
-        G = (max_new_tokens + 127) // 128 * 128
-        key = (int(eos), int(pad), bool(early_stopping), self.kv_cache_dtype)     # what the captured step bakes in
-        if proc is not None:
-            key += (("proc",) + proc,)
-        st = self._beam_state(B, K, Sp, G, key, use_cuda_graph)
-        if proc is not None:
-            self._load_proc(st, input_ids, 0, G)
-        plens = torch.tensor(pp.seqlens, dtype=torch.int32)
-        st.plens.copy_(plens, non_blocking=True)
-        st.beam_score.view(B, K).fill_(-1e9)[:, 0] = 0.0             # only beam 0 of a prompt expands at the first step
-        st.hyp_score.zero_()
-        st.hyp_score[:, K] = 1e9                                      # BeamHypotheses.worst_score starts at 1e9
-        st.hyp_meta.zero_()
-        st.pstate.zero_()
-        st.pstate[:, 1].copy_(plens, non_blocking=True)
-        st.norm.copy_(ops.beam_norm(S, G, length_penalty))
-        special = self.special_ids_dev
-        E = self.model.embed_tokens.weight.data
-        x = ops.embed_fwd(pp.ids, E, pp.vis_src if vis is not None else None, vis)
-        hid_last, _ = core.forward(x, pp.pos, pp.cu, pp.seqlens, save=False, kv_store=(st.pk, st.pv), out_rows=pp.last_rows)
-        self._decode_head(hid_last, st.logits[:B])
-        sel = lambda: ops.beam_select(st.cand_score, st.cand_tok, st.cand_par, st.beam_score, st.hist, st.src, st.hyp_score,
-                                      st.hyp_meta, st.hyp_tok, st.pstate, st.next_ids, st.lens, st.norm, eos, pad,
-                                      early_stopping)
-        def topk(first_step=False):
-            if proc is None:
-                ops.beam_topk(st.logits, special, st.beam_score, K, st.cand_score, st.cand_tok, st.cand_par, first_step=first_step)
-            else:
-                ops.beam_topk_processed(st.logits, special, st.beam_score, K, st.cand_score, st.cand_tok, st.cand_par, st.proc_ids,
-                                        st.proc_width, st.hist, st.pstate, proc, first_step=first_step)
-
-        topk(first_step=True)
-        sel()
-        if ev is not None:
-            ev[1].record()
-        beam = SimpleNamespace(pk=st.pk, pv=st.pv, plens=st.plens, src=st.src, K=K)
-
-        def step():
-            with ops.pdl():
-                xt = ops.embed_fwd(st.next_ids, E)
-                h = core.decode_step(xt, st.lens, st.kc, st.vc, beam=beam)
-                self._decode_head(h, st.logits)
-                topk()
-                sel()
-
-        # like the greedy loop, ask the device whether every prompt is done only every few steps: a done prompt's steps leave
-        # its hypotheses unchanged, so the extra steps change no output
-        T, replays = 1, 0                                             # T: beam steps run (tokens generated)
-        while T < max_new_tokens:
-            if T % 8 == 0 and bool(st.pstate[:, 4].all()):
-                break
-            if use_cuda_graph and st.graph is None:                   # first call with this state: eager step, then capture
-                step()
-                T += 1
-                g = torch.cuda.CUDAGraph()
-                torch.cuda.synchronize()
-                with torch.cuda.graph(g):
-                    step()
-                st.graph = g
-                continue
-            if use_cuda_graph:
-                st.graph.replay()
-                replays += 1
-            else:
-                step()
-            T += 1
-        if ev is not None:
-            ev[2].record()
-        # one copy; the fp64 scores go first, so their view starts at an even int32 offset whatever B and K are
-        parts = [st.hyp_score.flatten().view(torch.int32), st.hist.flatten(), st.hyp_meta.flatten(), st.hyp_tok.flatten(),
-                 st.pstate.flatten(), st.beam_score.view(torch.int32)]
-        host = torch.cat(parts).cpu()
-        o = np.cumsum([0] + [t.numel() for t in parts])
-        hyp_score = host[o[0]:o[1]].view(torch.float64).view(B, K + 1)
-        hist = host[o[1]:o[2]].view(B * K, G)
-        hyp_meta = host[o[2]:o[3]].view(B, K, 2)
-        hyp_tok = host[o[3]:o[4]].view(B, K, G)
-        pstate = host[o[4]:o[5]].view(B, 5)
-        beam_score = host[o[5]:o[6]].view(torch.float32)
-        if stats is not None:
-            torch.cuda.synchronize()
-            stats.update({"prefill_ms": ev[0].elapsed_time(ev[1]), "decode_ms": ev[1].elapsed_time(ev[2]) if T > 1 else None,
-                          "decode_steps": T - 1, "beam_steps": T, "graph_replays": replays, "kv_rows": Sp + G,
-                          "prompt_lens": list(pp.seqlens)})
-        T_done = int(pstate[0, 0])
-        hyps, running = [], []
-        for b in range(B):
-            n = int(pstate[b, 2])
-            kept = sorted(range(n), key=lambda i: int(hyp_meta[b, i, 1]))          # insertion order
-            hyps.append([(float(hyp_score[b, i]), hyp_tok[b, i, :int(hyp_meta[b, i, 0])].tolist()) for i in kept])
-            running.append(None if int(pstate[b, 4]) else
-                           [(float(beam_score[b * K + k]), hist[b * K + k, :T_done].tolist()) for k in range(K)])
-        seqs = beam_finalize(hyps, [float(hyp_score[b, K]) for b in range(B)], running, S, T_done, K, n_return, length_penalty)
-        return beam_output(input_ids.cpu(), seqs, S, S + max_new_tokens, eos, pad).to(dev)
-
-
-def beam_finalize(hyps, worst, running, S: int, T: int, K: int, n_return: int, length_penalty: float):
-    """BeamSearchScorer.finalize of transformers 4.28: prompts that are not done add their K running beams (score
-    sum_logprobs / (S + T) ** length_penalty, the Python float arithmetic of BeamHypotheses.add), then each prompt returns its
-    ``n_return`` best hypotheses, best first; of equal scores the one added last wins (a stable sort, popped from the end).
-    hyps[b]: the kept (score, generated tokens) in insertion order; worst[b]: their worst_score; running[b]: the K (running
-    score, tokens) of a prompt that is not done, else None.  Returns [[generated tokens] * n_return] per prompt."""
-    out = []
-    for b, beams in enumerate(hyps):
-        beams, w = list(beams), worst[b]
-        for sc, toks in (running[b] or []):
-            score = sc / ((S + T) ** length_penalty)
-            if len(beams) < K or score > w:
-                beams.append((score, toks))
-                if len(beams) > K:
-                    order = sorted([(s, i) for i, (s, _) in enumerate(beams)])
-                    del beams[order[0][1]]
-                    w = order[1][0]
-                else:
-                    w = min(score, w)
-        ranked = sorted(beams, key=lambda x: x[0])
-        out.append([ranked.pop()[1] for _ in range(n_return)])
-    return out
-
-
-def beam_output(prompt_ids: torch.Tensor, seqs, S: int, max_length: int, eos: int, pad: int) -> torch.Tensor:
-    """HF ``sequences`` of a beam search: [B * n, L] int64 rows of prompt ids and generated tokens, L = min(longest + 1,
-    max_length); a row shorter than L gets EOS after its tokens, then pad."""
-    rows = [(b, toks) for b, per in enumerate(seqs) for toks in per]
-    L = min(max(S + len(t) for _, t in rows) + 1, max_length)
-    out = torch.full((len(rows), L), pad, dtype=torch.int64)
-    for i, (b, toks) in enumerate(rows):
-        n = S + len(toks)
-        out[i, :S] = prompt_ids[b]
-        out[i, S:n] = torch.tensor(toks, dtype=torch.int64)
-        if n < L:
-            out[i, n] = eos
-    return out

@@ -163,7 +163,7 @@ def test_length_penalty_normalises_by_the_prompt_inclusive_length(lp):
 def test_host_finalisation_of_generate_matches_the_restatement():
     """ModifiedLlamaForCausalLM's host finalisation (beam_finalize / beam_output) against the restated finalize / sequences on
     random hypothesis sets, ties included."""
-    from navillm_b200.modified_lm import beam_finalize, beam_output
+    from navillm_b200.generation import beam_finalize, beam_output
     gen = torch.Generator().manual_seed(0)
     for trial in range(200):
         B, K, S, T = 3, int(torch.randint(2, 6, (1,), generator=gen)), 7, int(torch.randint(1, 9, (1,), generator=gen))

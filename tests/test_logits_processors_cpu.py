@@ -68,18 +68,18 @@ def test_repetition_penalty_is_ieee_division_in_bf16():
 
 
 def test_processor_arguments_are_checked_like_hf():
-    from navillm_b200.modified_lm import ModifiedLlamaForCausalLM as M
-    assert M._processors(None, None, None, None, 2) is None
-    assert M._processors(1.0, 0, 0, 0, 2) is None
-    assert M._processors(1, 0, None, 0, 2) is None                   # HF builds no processor for 1: no type check either
-    assert M._processors(1.3, 3, 0, 4, 2) == (1.3, 3, 0, 4, 2)
+    from navillm_b200.generation import processors
+    assert processors(None, None, None, None, 2) is None
+    assert processors(1.0, 0, 0, 0, 2) is None
+    assert processors(1, 0, None, 0, 2) is None                   # HF builds no processor for 1: no type check either
+    assert processors(1.3, 3, 0, 4, 2) == (1.3, 3, 0, 4, 2)
     for bad in (dict(repetition_penalty=0.0), dict(repetition_penalty=-1.0), dict(repetition_penalty=2),
                 dict(no_repeat_ngram_size=-1), dict(no_repeat_ngram_size=2.0), dict(min_length=-1), dict(min_new_tokens=-2),
                 dict(min_new_tokens=True)):
         kw = dict(repetition_penalty=None, no_repeat_ngram_size=None, min_length=None, min_new_tokens=None)
         kw.update(bad)
         with pytest.raises(ValueError):
-            M._processors(*kw.values(), 2)
+            processors(*kw.values(), 2)
 
 
 @pytest.mark.parametrize("precision", ["fp32", "amp_bf16"])

@@ -63,7 +63,7 @@ def case(model, dev, B, K, new, gens, NV, NT):
     if K > 1:
         tb, cb = prompts(model, B * K, NV, NT, dev)
         r["greedy_BK"] = timed(lm, tb, cb, new, gens)
-    lm.__dict__.pop("_decode_states", None)
+    lm._decode_states.clear()
     torch.cuda.empty_cache()
     print(json.dumps(r), flush=True)
     return r

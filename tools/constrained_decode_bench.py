@@ -128,7 +128,7 @@ def eqa(model, dev, n_answers, n_calls, seed=0):
             equal.append(all(torch.equal(outs["host"], outs[k]) for k in names[1:]))
         return ms, flat, equal, steps, misses
 
-    lm.__dict__.pop("_decode_states", None)                          # start without a captured graph
+    lm._decode_states.clear()                                        # start without a captured graph
     seq = [short if i % 2 == 0 else long_ for i in range(n_calls)]
     ms, flat, equal, steps, misses = run(seq)
     res = {"B": B, "answers": n_answers, "trie_nodes_edges": None, "buckets": lens, "calls": n_calls,

@@ -228,7 +228,7 @@ def c3_generate_kv(dev, layers, gens, batch, rounds=2):
     ids = {}
     for rnd in range(2 * rounds):
         w = ("bf16", "fp8")[rnd % 2]
-        lm.__dict__.pop("_decode_states", None)                             # graphs bake in the weight kernels
+        lm._decode_states.clear()                                           # graphs bake in the weight kernels
         lm._fp8 = fp8w if w == "fp8" else None
         lm.core.set_fp8(lm._fp8)
         for kv in (("bf16", "fp8") if rnd % 4 < 2 else ("fp8", "bf16")):

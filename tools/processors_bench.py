@@ -103,7 +103,7 @@ def main():
         text, cand = prompts(model, B, wl["n_cand_tok"], wl["n_text"], dev)
         r = {"B": B, **{k: v for k, v in kw.items()}, "new_tokens": wl["n_new"]}
         r.update(alternated(lm, text, cand, wl["n_new"], a.gens, **kw))
-        lm.__dict__.pop("_decode_states", None)
+        lm._decode_states.clear()
         torch.cuda.empty_cache()
         print(json.dumps(r), flush=True)
         rows.append(r)

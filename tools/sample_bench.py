@@ -41,7 +41,7 @@ def arm(lm, text, cand, new, seed, **kw):
 def peak(lm, text, cand, new, **kw):
     """Peak device memory of one call with no other generate() state resident: the weights, this call's own KV caches and
     captured graph, and its transients."""
-    lm.__dict__.pop("_decode_states", None)
+    lm._decode_states.clear()
     torch.cuda.synchronize()
     torch.cuda.empty_cache()
     return arm(lm, text, cand, new, seed=0, **kw)[3]
@@ -69,7 +69,7 @@ def e2e(model, dev, B, N, new, gens, NV, NT):
                   "ms_per_step": round(float(np.median(v[:, 1])), 4)}
     out["shared"]["peak_GB"] = round(peak(lm, text, cand, new, num_return_sequences=N) / 1e9, 2)
     out["repeated"]["peak_GB"] = round(peak(lm, text_rep, cand_rep, new) / 1e9, 2)
-    lm.__dict__.pop("_decode_states", None)
+    lm._decode_states.clear()
     torch.cuda.empty_cache()
     print(json.dumps(out), flush=True)
     return out
