@@ -78,6 +78,20 @@ int nv_gemm_skinny_fp8(const void* X, int64_t ldx, const void* Wq, int64_t ldw, 
                        const void* addend, int64_t ld_add, int M, int N, int K, void* stream);
 int nv_gemm_skinny_swiglu_fp8(const void* X, int64_t ldx, const void* Wgu_q, int64_t ldw, const void* exps, void* H,
                               int64_t ldh, int M, int F, int K, void* stream);
+/* Opt-in 4-bit group-wise weight streaming (W4A16) of the same decode-step GEMMs (no reference counterpart for the number
+ * format; csrc/nv_int4.cuh).  nv_quantize_int4_groups (csrc/quant.cu) rounds a bf16 weight W [N,K], K % 128 == 0, in groups
+ * of one row and 128 columns, in fp32 with IEEE division and round-half-even rint: lo = min(0, min w), hi = max(0, max w),
+ * s = max(bf16(((hi - lo) / 15)), 2^-126), z = clamp(rint(-lo / s), 0, 15), q = clamp(rint(w / s) + z, 0, 15), and W is
+ * overwritten in place with W' = bf16((q - z) * s) (-0 becomes +0; groups with bf16 subnormals follow the rule too).
+ * scales [N, K/128] bf16 and zeros [N, K/128] uint8 hold s and z; codes (ceil(N/64) * 64 * K/2 bytes, 16-byte aligned)
+ * hold q packed in a layout private to the library.  nv_gemm_skinny_int4 / nv_gemm_skinny_swiglu_int4 are
+ * nv_gemm_skinny_bf16 / nv_gemm_skinny_swiglu_bf16 with the weight given as (codes, scales, zeros): they stream a quarter
+ * of the bytes and return bit for bit what the bf16 kernels return on W'.  M <= 16, K % 128 == 0. */
+int nv_quantize_int4_groups(void* W, int64_t ldw, void* codes, void* scales, void* zeros, int N, int K, void* stream);
+int nv_gemm_skinny_int4(const void* X, int64_t ldx, const void* codes, const void* scales, const void* zeros, void* C,
+                        int64_t ldc, const void* addend, int64_t ld_add, int M, int N, int K, void* stream);
+int nv_gemm_skinny_swiglu_int4(const void* X, int64_t ldx, const void* codes, const void* scales, const void* zeros, void* H,
+                               int64_t ldh, int M, int F, int K, void* stream);
 /* nv_gemm_fp8w_bf16 is nv_gemm_bf16 with K-major operands (a_mn = b_mn = 0) and the weight given as (Wq, exps) in the same
  * format, for the inference GEMMs above 16 rows (prefix-cached navigation suffixes, pruned last layers, decode batches
  * 17..256): C = bf16(bf16(A Wq'^T) + addend) with addend optional, bit for bit nv_gemm_bf16's result on W' at every M, N, K

@@ -23,11 +23,16 @@
 // wrote back, so the fp8 kernel's output equals the bf16 kernel's on W'.  The fp8 stages use 10 KB instead of 18 KB; the
 // freed shared memory holds the double-buffered bf16 expansion (2 warpgroups x 2 x 8 KB), so both kernels occupy the same
 // 73 KB and three CTAs share an SM either way.
+// 4-bit group-wise weights (SkInt4, nv_int4.cuh) take the other road: in swap-AB the weights are the wgmma A operand, which
+// may come from registers, so each consumer thread dequantizes its pre-shuffled codes straight into m64n16k16 register-A
+// fragments (exactly W') and issues register-A wgmmas over the same k range in the same order -- no expansion buffer,
+// fence or barrier, and the next k-block's dequantization runs under the current wgmmas.
 #include <stdlib.h>
 
 #include "nv_common.cuh"
 #include "nv_fp8.cuh"
 #include "nv_host.h"
+#include "nv_int4.cuh"
 
 namespace nv {
 
@@ -43,7 +48,8 @@ constexpr uint32_t SK_CVT_BYTES = 64 * SK_BK * 2;      // one warpgroup's bf16 e
 // Shared-memory layout per weight type: [weight stages][fp8 only: 2 x 2 expansion buffers][activation stages][barriers]
 template <typename WT>
 struct SkLayout {
-  static constexpr bool kFp8 = sizeof(WT) == 1;
+  static constexpr bool kFp8 = sizeof(WT) == 1, kInt4 = false;
+  static constexpr uint32_t STAGES = SK_STAGES;
   static constexpr uint32_t W_BYTES = SK_BN * SK_BK * sizeof(WT);
   static constexpr uint32_t STAGE_BYTES = W_BYTES + SK_X_BYTES;            // TMA bytes per stage
   static constexpr uint32_t CVT_OFF = SK_STAGES * W_BYTES;
@@ -51,6 +57,21 @@ struct SkLayout {
   static constexpr uint32_t BAR_OFF = X_OFF + SK_STAGES * SK_X_BYTES;
   static constexpr uint32_t DYN_BYTES = BAR_OFF + 2 * SK_STAGES * 8 + 1024;
   static_assert(8 * SK_RED_BYTES <= X_OFF, "reduction buffers and the output tile reuse the weight stages (and expansion buffers)");
+};
+
+// 4-bit group-wise weights (nv_int4.cuh).  A k-block carries 4 KB of codes (two 2 KB chunks, one per consumer warpgroup),
+// so ten 6 KB stages fit where the reduction needs 64 KB anyway; the reduction reuses weight and activation stages (all
+// TMA loads have landed when the cluster synchronises after the main loop).  67 KB: three CTAs share an SM, as above.
+struct SkInt4 {};
+template <>
+struct SkLayout<SkInt4> {
+  static constexpr bool kFp8 = false, kInt4 = true;
+  static constexpr uint32_t STAGES = 10;
+  static constexpr uint32_t W_BYTES = 2 * Q4_CHUNK_BYTES;
+  static constexpr uint32_t STAGE_BYTES = W_BYTES + SK_X_BYTES;
+  static constexpr uint32_t X_OFF = STAGES * W_BYTES;
+  static constexpr uint32_t BAR_OFF = X_OFF + STAGES * SK_X_BYTES > 8 * SK_RED_BYTES ? X_OFF + STAGES * SK_X_BYTES : 8 * SK_RED_BYTES;
+  static constexpr uint32_t DYN_BYTES = BAR_OFF + 2 * STAGES * 8 + 1024;
 };
 
 __device__ __forceinline__ uint32_t sk_cluster_rank() {
@@ -73,14 +94,17 @@ __device__ __forceinline__ void sk_st_remote_f32(float* p, uint32_t cta, float v
 // swiglu_f != 0: W is the fused gate|up weight [2F, K]; tile n_blk stages 64 gate rows n_blk*64.. and the matching 64 up
 // rows F + n_blk*64.. (two 64-row TMA boxes), the leader pairs them and writes h[m, n] = bf16(bf16(silu(g)) * u), the
 // same rounding points as swiglu_fwd_kernel on the bf16 gate|up buffer (which is not materialised here).
-// WT = uint8_t: W holds e4m3 bytes and w_exp[r] the exponent of weight row r (W' = e4m3 * 2^w_exp); unused for bf16.
+// WT = uint8_t: W holds e4m3 bytes and w_scale the int8 exponent of each weight row (W' = e4m3 * 2^exp); unused for bf16.
+// WT = SkInt4: tmap_w maps the packed codes (nv_int4.cuh) as [chunks x 2, 256] words, w_scale is the bf16 scale and w_zero
+// the zero-point of each (row, 128-column group) ([rows, K / 128] row-major).
 template <typename WT>
 __global__ void __launch_bounds__(SK_THREADS)
 gemm_skinny_wgmma(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_x,
                   __nv_bfloat16* __restrict__ C, int64_t ldc, const __nv_bfloat16* __restrict__ addend, int64_t ld_add,
-                  uint32_t M, uint32_t N, uint32_t K, uint32_t splits, uint32_t swiglu_f, const int8_t* __restrict__ w_exp) {
+                  uint32_t M, uint32_t N, uint32_t K, uint32_t splits, uint32_t swiglu_f, const void* __restrict__ w_scale,
+                  const uint8_t* __restrict__ w_zero) {
   using L = SkLayout<WT>;
-  constexpr uint32_t SK_W_BYTES = L::W_BYTES, SK_STAGE_BYTES = L::STAGE_BYTES;
+  constexpr uint32_t SK_W_BYTES = L::W_BYTES, SK_STAGE_BYTES = L::STAGE_BYTES, SK_STAGES = L::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_w = smem;
@@ -114,7 +138,12 @@ gemm_skinny_wgmma(const __grid_constant__ CUtensorMap tmap_w, const __grid_const
     tma_prefetch_desc(&tmap_x);
     const int32_t n0 = swiglu_f ? n_blk * 64 : n_blk * SK_BN;
     auto load_w = [&](uint32_t stage, int32_t k0) {
-      if (swiglu_f) {                                                                   // box {64 k, 64 n}: gate half, up half
+      if constexpr (L::kInt4) {                                                         // box {256 words, 2}: one chunk
+        const int32_t kb = k0 / SK_BK, nkb_all = K / SK_BK;
+        const int32_t rb0 = swiglu_f ? n_blk : 2 * n_blk, rb1 = swiglu_f ? swiglu_f / 64 + n_blk : 2 * n_blk + 1;
+        tma_load_2d(smem_w + stage * SK_W_BYTES, &tmap_w, &full_bar[stage], 0, 2 * (rb0 * nkb_all + kb));
+        tma_load_2d(smem_w + stage * SK_W_BYTES + Q4_CHUNK_BYTES, &tmap_w, &full_bar[stage], 0, 2 * (rb1 * nkb_all + kb));
+      } else if (swiglu_f) {                                                                   // box {64 k, 64 n}: gate half, up half
         tma_load_2d(smem_w + stage * SK_W_BYTES, &tmap_w, &full_bar[stage], k0, n0);
         tma_load_2d(smem_w + stage * SK_W_BYTES + SK_W_BYTES / 2, &tmap_w, &full_bar[stage], k0, (int32_t)swiglu_f + n0);
       } else {
@@ -149,6 +178,74 @@ gemm_skinny_wgmma(const __grid_constant__ CUtensorMap tmap_w, const __grid_const
       }
       __syncwarp();
     }
+  } else if constexpr (L::kInt4) {
+    // Register-A wgmmas: thread t of the warpgroup dequantizes its 16 code bytes of a k-block (nv_int4.cuh) straight into
+    // the A fragments of the four m64n16k16 steps.  While the wgmmas of k-block i run, the codes of k-block i + 1 are read
+    // and dequantized into the other fragment set, and the scales / zero-points of k-block i + 2 are requested from global
+    // memory.  Same k16 chain, per-rank k range and reduction as the bf16 kernel, on the bf16 values W'.
+    const uint32_t t = threadIdx.x & 127;
+    const int32_t n0 = swiglu_f ? n_blk * 64 : n_blk * SK_BN;
+    const uint32_t w_rows = swiglu_f ? 2 * swiglu_f : N, G = K / Q4_GROUP;
+    const __nv_bfloat16* sc = reinterpret_cast<const __nv_bfloat16*>(w_scale);
+    int64_t gbase[2];                                        // (row, group 0) of the thread's rows r0, r1; -1: row >= w_rows
+#pragma unroll
+    for (uint32_t j = 0; j < 2; ++j) {
+      const uint32_t tr = wg * 64 + ((t >> 5) << 4) + ((t & 31) >> 2) + 8 * j;
+      const uint32_t r = swiglu_f ? (tr < 64 ? n0 + tr : swiglu_f + n0 + tr - 64) : n0 + tr;
+      gbase[j] = r < w_rows ? (int64_t)r * G : -1;
+    }
+    // (s0x, z0x, s1x, z1x) of k-block kb; rows >= w_rows: s = 0 (their codes are TMA zero fill or padding)
+    auto params = [&](uint32_t kb, uint32_t (&p)[4]) {
+#pragma unroll
+      for (uint32_t j = 0; j < 2; ++j) {
+        uint32_t s = 0, z = 0;
+        if (gbase[j] >= 0) {
+          const int64_t gi = gbase[j] + (kb >> 1);
+          s = __bfloat16_as_ushort(sc[gi]);
+          z = w_zero[gi];
+        }
+        p[2 * j] = s * 0x10001u;
+        p[2 * j + 1] = (0x4300u + z) * 0x10001u;
+      }
+    };
+    auto dequant = [&](uint32_t stage, const uint32_t (&p)[4], uint32_t (&a)[4][4]) {
+      const uint4 c = lds128(smem_u32(smem_w + stage * SK_W_BYTES + wg * Q4_CHUNK_BYTES) + 16 * t);
+      q4_dequant_k16(c.x, p[0], p[1], p[2], p[3], a[0]);
+      q4_dequant_k16(c.y, p[0], p[1], p[2], p[3], a[1]);
+      q4_dequant_k16(c.z, p[0], p[1], p[2], p[3], a[2]);
+      q4_dequant_k16(c.w, p[0], p[1], p[2], p[3], a[3]);
+    };
+    uint32_t pa[4], pb[4], fa[4][4], fb[4][4];
+    // one k-block: wgmmas on `cur`; under them the next k-block's fragments into `nxt` (with its parameters `puse`) and
+    // the request of k-block i + 2's parameters into `pload` (free: they served k-block i)
+    auto step = [&](uint32_t i, uint32_t (&cur)[4][4], uint32_t (&nxt)[4][4], const uint32_t (&puse)[4], uint32_t (&pload)[4]) {
+      const uint32_t stage = i % SK_STAGES;
+      if (i + 2 < nkb) params(kb0 + i + 2, pload);
+      const uint64_t xdesc = gmma_desc_sw128(smem_u32(smem_x + stage * SK_X_BYTES), 0, 1024);
+      wgmma_fence();
+#pragma unroll
+      for (uint32_t k = 0; k < SK_BK / 16; ++k) wgmma_rs_bf16<16, 0>(acc, cur[k], xdesc + k * 2, 1u);
+      wgmma_commit();
+      if (i + 1 < nkb) {
+        const uint32_t s1 = (i + 1) % SK_STAGES;
+        mbar_wait(&full_bar[s1], ((i + 1) / SK_STAGES) & 1);
+        dequant(s1, puse, nxt);
+      }
+      wgmma_wait<0>();
+      if (t == 0) mbar_arrive(&empty_bar[stage]);
+    };
+    if (nkb > 0) {
+      params(kb0, pa);
+      if (nkb > 1) params(kb0 + 1, pb);
+      mbar_wait(&full_bar[0], 0);
+      dequant(0, pa, fa);
+    }
+    for (uint32_t i = 0; i < nkb; i += 2) {
+      step(i, fa, fb, pb, pa);
+      if (i + 1 < nkb) step(i + 1, fb, fa, pa, pb);
+    }
+    reg_fence(acc);
+    griddep_wait();                                        // before the first read of `addend` / write of C
   } else if constexpr (L::kFp8) {
     // Expansion: thread t of the warpgroup owns 16-byte fp8 chunks q = t and t + 128 of the warpgroup's 64 x 64-byte rows
     // (row q / 4, k 16 (q % 4) ..+15) and writes them as bf16 chunks 2 (q % 4), 2 (q % 4) + 1 of the swizzled row.
@@ -160,7 +257,7 @@ gemm_skinny_wgmma(const __grid_constant__ CUtensorMap tmap_w, const __grid_const
     for (uint32_t j = 0; j < 2; ++j) {
       const uint32_t tr = wg * 64 + (t >> 2) + 32 * j;                       // row of the 128-row tile
       const uint32_t r = swiglu_f ? (tr < 64 ? n0 + tr : swiglu_f + n0 + tr - 64) : n0 + tr;
-      scale[j] = r < w_rows ? fp8_pow2(w_exp[r]) : 1.f;                    // rows >= w_rows are TMA zero fill
+      scale[j] = r < w_rows ? fp8_pow2(reinterpret_cast<const int8_t*>(w_scale)[r]) : 1.f;                    // rows >= w_rows are TMA zero fill
     }
     uint8_t* cvt = smem + L::CVT_OFF + wg * 2 * SK_CVT_BYTES;
     for (uint32_t i = 0; i < nkb; ++i) {
@@ -287,17 +384,24 @@ gemm_skinny_wgmma(const __grid_constant__ CUtensorMap tmap_w, const __grid_const
 }  // namespace nv
 
 template <typename WT>
-static int skinny_launch(const void* X, int64_t ldx, const void* W, int64_t ldw, const int8_t* w_exp, void* C, int64_t ldc,
-                         const void* addend, int64_t ld_add, int M, int N, int K, uint32_t swiglu_f, cudaStream_t stream) {
+static int skinny_launch(const void* X, int64_t ldx, const void* W, int64_t ldw, const void* w_scale, void* C, int64_t ldc,
+                         const void* addend, int64_t ld_add, int M, int N, int K, uint32_t swiglu_f, cudaStream_t stream,
+                         const uint8_t* w_zero = nullptr) {
   using namespace nv;
   using L = SkLayout<WT>;
   CUtensorMap tw, tx;
   int rc;
   const uint64_t w_rows = swiglu_f ? 2ull * swiglu_f : (uint64_t)N;
-  // bf16: 128-byte swizzled box (wgmma reads it in place); fp8: plain 64-byte rows, expanded by the consumers
-  if ((rc = make_tmap_2d(&tw, W, (int)sizeof(WT), (uint64_t)K, w_rows, (uint64_t)ldw * sizeof(WT), 64, swiglu_f ? 64 : SK_BN,
-                         /*swizzle128=*/!L::kFp8)))
-    return rc;
+  if constexpr (L::kInt4) {
+    // the packed codes as rows of 256 words, two per 2 KB chunk: chunks of row blocks past the weight are zero fill
+    const uint64_t chunks = (w_rows + 63) / 64 * (uint64_t)(K / SK_BK);
+    if ((rc = make_tmap_2d(&tw, W, 4, 256, 2 * chunks, 1024, 256, 2, /*swizzle128=*/false))) return rc;
+  } else {
+    // bf16: 128-byte swizzled box (wgmma reads it in place); fp8: plain 64-byte rows, expanded by the consumers
+    if ((rc = make_tmap_2d(&tw, W, (int)sizeof(WT), (uint64_t)K, w_rows, (uint64_t)ldw * sizeof(WT), 64, swiglu_f ? 64 : SK_BN,
+                           /*swizzle128=*/!L::kFp8)))
+      return rc;
+  }
   if ((rc = make_tmap_2d(&tx, X, 2, (uint64_t)K, (uint64_t)M, (uint64_t)ldx * 2, 64, SK_BM))) return rc;
   static bool attr_set = false;
   if (!attr_set) {
@@ -335,7 +439,7 @@ static int skinny_launch(const void* X, int64_t ldx, const void* W, int64_t ldw,
   }
   NV_CUDA(cudaLaunchKernelEx(&cfg, gemm_skinny_wgmma<WT>, tw, tx, reinterpret_cast<__nv_bfloat16*>(C), ldc,
                              reinterpret_cast<const __nv_bfloat16*>(addend), ld_add, (uint32_t)M, (uint32_t)N, (uint32_t)K,
-                             splits, swiglu_f, w_exp));
+                             splits, swiglu_f, w_scale, w_zero));
   return NV_OK;
 }
 
@@ -372,7 +476,7 @@ extern "C" int nv_gemm_skinny_fp8(const void* X, int64_t ldx, const void* Wq, in
   NV_REQUIRE(M > 0 && M <= (int)SK_BM && N > 0 && K > 0, "nv_gemm_skinny_fp8: needs 1 <= M <= 16 (got M=%d N=%d K=%d)", M, N, K);
   NV_REQUIRE(X && Wq && w_exp && C, "nv_gemm_skinny_fp8: null operand");
   NV_REQUIRE((ldx & 7) == 0 && (ldw & 15) == 0, "nv_gemm_skinny_fp8: ldx must be a multiple of 8 and ldw (bytes) of 16");
-  return skinny_launch<uint8_t>(X, ldx, Wq, ldw, reinterpret_cast<const int8_t*>(w_exp), C, ldc, addend, ld_add, M, N, K, 0u,
+  return skinny_launch<uint8_t>(X, ldx, Wq, ldw, w_exp, C, ldc, addend, ld_add, M, N, K, 0u,
                                 reinterpret_cast<cudaStream_t>(stream_));
 }
 
@@ -383,6 +487,30 @@ extern "C" int nv_gemm_skinny_swiglu_fp8(const void* X, int64_t ldx, const void*
              "nv_gemm_skinny_swiglu_fp8: needs 1 <= M <= 16 and F %% 64 == 0 (got M=%d F=%d K=%d)", M, F, K);
   NV_REQUIRE(X && Wgu_q && w_exp && H && (ldx & 7) == 0 && (ldw & 15) == 0,
              "nv_gemm_skinny_swiglu_fp8: null operand / alignment");
-  return skinny_launch<uint8_t>(X, ldx, Wgu_q, ldw, reinterpret_cast<const int8_t*>(w_exp), H, ldh, nullptr, 0, M, F, K,
+  return skinny_launch<uint8_t>(X, ldx, Wgu_q, ldw, w_exp, H, ldh, nullptr, 0, M, F, K,
                                 (uint32_t)F, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+// The 4-bit forms (W4A16): codes packed by nv_quantize_int4_groups, scales [N, K / 128] bf16 and zeros [N, K / 128] uint8
+// (for the SwiGLU form, of the fused [2F, K] gate|up weight).  The result is bit-identical to the bf16 kernel on
+// W' = bf16((q - z) * s): same cluster split, k ranges, k16 MMA chain and reduction; a rank's range may start inside a group.
+extern "C" int nv_gemm_skinny_int4(const void* X, int64_t ldx, const void* codes, const void* scales, const void* zeros, void* C,
+                                   int64_t ldc, const void* addend, int64_t ld_add, int M, int N, int K, void* stream_) {
+  using namespace nv;
+  NV_REQUIRE(M > 0 && M <= (int)SK_BM && N > 0 && K > 0 && (K % (int)Q4_GROUP) == 0,
+             "nv_gemm_skinny_int4: needs 1 <= M <= 16 and K %% 128 == 0 (got M=%d N=%d K=%d)", M, N, K);
+  NV_REQUIRE(X && codes && scales && zeros && C, "nv_gemm_skinny_int4: null operand");
+  NV_REQUIRE((ldx & 7) == 0, "nv_gemm_skinny_int4: ldx must be a multiple of 8");
+  return skinny_launch<SkInt4>(X, ldx, codes, 0, scales, C, ldc, addend, ld_add, M, N, K, 0u,
+                               reinterpret_cast<cudaStream_t>(stream_), reinterpret_cast<const uint8_t*>(zeros));
+}
+
+extern "C" int nv_gemm_skinny_swiglu_int4(const void* X, int64_t ldx, const void* codes, const void* scales, const void* zeros,
+                                          void* H, int64_t ldh, int M, int F, int K, void* stream_) {
+  using namespace nv;
+  NV_REQUIRE(M > 0 && M <= (int)SK_BM && F > 0 && K > 0 && (F % 64) == 0 && (K % (int)Q4_GROUP) == 0,
+             "nv_gemm_skinny_swiglu_int4: needs 1 <= M <= 16, F %% 64 == 0 and K %% 128 == 0 (got M=%d F=%d K=%d)", M, F, K);
+  NV_REQUIRE(X && codes && scales && zeros && H && (ldx & 7) == 0, "nv_gemm_skinny_swiglu_int4: null operand / alignment");
+  return skinny_launch<SkInt4>(X, ldx, codes, 0, scales, H, ldh, nullptr, 0, M, F, K, (uint32_t)F,
+                               reinterpret_cast<cudaStream_t>(stream_), reinterpret_cast<const uint8_t*>(zeros));
 }

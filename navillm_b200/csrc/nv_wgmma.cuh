@@ -58,6 +58,15 @@ __device__ __forceinline__ void wgmma_ss_bf16_n256(float (&d)[128], uint64_t ade
 }
 
 template <int TB>
+__device__ __forceinline__ void wgmma_rs_bf16_n16(float (&d)[8], const uint32_t (&a)[4], uint64_t bdesc, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, %14;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d), "n"(TB));
+}
+
+template <int TB>
 __device__ __forceinline__ void wgmma_rs_bf16_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
@@ -103,7 +112,8 @@ __device__ __forceinline__ void wgmma_ss_bf16(float (&d)[N / 2], uint64_t adesc,
 }
 template <int N, int TB>
 __device__ __forceinline__ void wgmma_rs_bf16(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t bdesc, uint32_t scale_d) {
-  if constexpr (N == 64) wgmma_rs_bf16_n64<TB>(d, a, bdesc, scale_d);
+  if constexpr (N == 16) wgmma_rs_bf16_n16<TB>(d, a, bdesc, scale_d);
+  else if constexpr (N == 64) wgmma_rs_bf16_n64<TB>(d, a, bdesc, scale_d);
   else { static_assert(N == 128, "wgmma_rs_bf16: N"); wgmma_rs_bf16_n128<TB>(d, a, bdesc, scale_d); }
 }
 

@@ -216,57 +216,58 @@ class FlatParams:
         return self.flat_grad[o:o + numel].view(shape)
 
 
-class Fp8Weights:
-    """e4m3 copy of linear weights of a ``FlatParams`` buffer for the inference GEMMs: the decode-step skinny GEMMs
-    (csrc/gemm_skinny.cu) and, up to ``FP8_MAX_ROWS`` rows, nv_gemm_fp8w_bf16 (csrc/gemm_bf16.cu).
+class _WeightCopy:
+    """Quantized copy of linear weights of a ``FlatParams`` buffer (``Fp8Weights``, ``Int4Weights``).
 
-    Building it rounds every listed weight IN PLACE to W' = e4m3(W / 2^e_n) * 2^e_n (one power-of-two exponent per output
-    row, csrc/quant.cu), so the bf16 buffer and the fp8 copy describe the same model.  The copy keeps the flat buffer's
-    parameter order and 64-element alignment (non-listed parameters are skipped), so members that are adjacent there --
-    q|k|v, gate|up -- are adjacent here too and the fused weights are plain views.  ``stale_reason`` reports any write to
-    the weights since: a torch in-place op on a parameter or on the buffer (version counters), or a bump of
-    ``FlatParams.generation`` by a raw-pointer writer."""
+    Building it rounds every listed weight IN PLACE to the W' the copy encodes (``_quantize``), so the bf16 buffer and the
+    copy describe the same model.  Each storage of the copy (``_sizes``: elements per weight) keeps the flat buffer's
+    parameter order, non-listed parameters skipped, so members that are adjacent there -- q|k|v, gate|up -- are adjacent
+    here too and the fused weights are plain views.  ``stale_reason`` reports any write to the weights since: a torch
+    in-place op on a parameter or on the buffer (version counters), or a bump of ``FlatParams.generation`` by a raw-pointer
+    writer."""
+    _align = (1,)                                # per storage: element alignment of each weight's start
 
     def __init__(self, flat: FlatParams, params: List[nn.Parameter]):
+        name = type(self).__name__
         want = {id(p) for p in params}
-        align = 64
         self.flat = flat
         self.params = [p for p in flat.params if id(p) in want]
         if len(self.params) != len(want):
-            raise RuntimeError("Fp8Weights: every weight must live in the flat buffer")
-        self._off, self._row, total, rows = {}, {}, 0, 0
+            raise RuntimeError(f"{name}: every weight must live in the flat buffer")
+        self._off, totals = {}, [0] * len(self._align)
         for p in self.params:
             if p.dim() != 2:
-                raise RuntimeError(f"Fp8Weights: 2-D weights only, got {tuple(p.shape)}")
-            self._off[id(p)], self._row[id(p)] = total, rows
-            total += (p.numel() + align - 1) // align * align
-            rows += p.shape[0]
-        dev = flat.flat.device
-        self.q = torch.empty(total, dtype=ops.fp8, device=dev)
-        self.exps = torch.empty(rows, dtype=torch.int8, device=dev)
+                raise RuntimeError(f"{name}: 2-D weights only, got {tuple(p.shape)}")
+            self._check(p)
+            self._off[id(p)] = tuple(totals)
+            totals = [t + (n + a - 1) // a * a for t, n, a in zip(totals, self._sizes(tuple(p.shape)), self._align)]
+        self._storage = self._allocate(totals, flat.flat.device)
         flat.generation += 1                     # the rounding below writes the weights through raw pointers
         for p in self.params:
-            q, e = self.view([p], tuple(p.shape))
-            ops.quantize_fp8_(p.data, q, e)
+            self._quantize(p.data, self.view([p], tuple(p.shape)))
         self._versions = self._version_state()
         self._generation = flat.generation
 
+    def _check(self, p: nn.Parameter) -> None:
+        pass
+
     @property
     def nbytes(self) -> int:
-        return self.q.numel() + self.exps.numel()
+        return sum(t.numel() * t.element_size() for t in self._storage)
 
     def view(self, members, shape):
-        """(e4m3 [N, K], int8 exponents [N]) of the weight formed by ``members`` stacked in order (``FlatParams.view``)."""
-        o, r = self._off[id(members[0])], self._row[id(members[0])]
-        end_o, end_r = o, r
+        """The copy's tensors of the weight formed by ``members`` stacked in order (``FlatParams.view``)."""
+        name = type(self).__name__
+        start = self._off[id(members[0])]
+        end = list(start)
         for m in members:
-            if self._off.get(id(m)) != end_o or self._row[id(m)] != end_r:
-                raise RuntimeError("Fp8Weights.view: the members are not adjacent, in order and unpadded")
-            end_o += m.numel()
-            end_r += m.shape[0]
-        if end_o - o != shape[0] * shape[1] or end_r - r != shape[0]:
-            raise RuntimeError(f"Fp8Weights.view: members hold {end_o - o} elements, shape {tuple(shape)} needs {shape[0] * shape[1]}")
-        return self.q[o:end_o].view(shape), self.exps[r:end_r]
+            if self._off.get(id(m)) != tuple(end):
+                raise RuntimeError(f"{name}.view: the members are not adjacent, in order and unpadded")
+            end = [e + n for e, n in zip(end, self._sizes(tuple(m.shape)))]
+        if [e - o for e, o in zip(end, start)] != list(self._sizes(tuple(shape))):
+            raise RuntimeError(f"{name}.view: members hold {end[0] - start[0]} elements, shape {tuple(shape)} needs "
+                               f"{self._sizes(tuple(shape))[0]}")
+        return self._views([t[o:e] for t, o, e in zip(self._storage, start, end)], shape)
 
     def _version_state(self):
         return self.flat.flat._version, sum(p._version for p in self.params)
@@ -279,6 +280,70 @@ class Fp8Weights:
         if self._version_state() != self._versions:
             return "the weights were modified in place (optimizer step, load_state_dict or another write)"
         return None
+
+
+class Fp8Weights(_WeightCopy):
+    """e4m3 copy of linear weights for the inference GEMMs: the decode-step skinny GEMMs (csrc/gemm_skinny.cu) and, up to
+    ``FP8_MAX_ROWS`` rows, nv_gemm_fp8w_bf16 (csrc/gemm_bf16.cu).  W' = e4m3(W / 2^e_n) * 2^e_n with one power-of-two
+    exponent per output row (csrc/quant.cu); ``view`` gives (e4m3 [N, K], int8 exponents [N])."""
+    _align = (64, 1)
+
+    @staticmethod
+    def _sizes(shape):
+        return shape[0] * shape[1], shape[0]
+
+    @staticmethod
+    def _allocate(totals, dev):
+        return torch.empty(totals[0], dtype=ops.fp8, device=dev), torch.empty(totals[1], dtype=torch.int8, device=dev)
+
+    @property
+    def q(self) -> torch.Tensor:
+        return self._storage[0]
+
+    @property
+    def exps(self) -> torch.Tensor:
+        return self._storage[1]
+
+    @staticmethod
+    def _views(parts, shape):
+        return parts[0].view(shape), parts[1]
+
+    @staticmethod
+    def _quantize(w, v):
+        ops.quantize_fp8_(w, *v)
+
+
+class Int4Weights(_WeightCopy):
+    """4-bit group-wise copy (W4A16) of the decoder-layer linear weights for the decode-step skinny GEMMs
+    (csrc/gemm_skinny.cu, at most 16 rows).  W' = bf16((q - z) * s) with one bf16 scale s and one 4-bit zero-point z per
+    row and 128 columns (csrc/quant.cu, rule in include/navillm_b200.h); ``view`` gives (codes, scales [N, K / 128] bf16,
+    zeros [N, K / 128] uint8) in the form ``ops.gemm_skinny_int4`` takes.  Every weight needs K % 128 == 0 and, so that the
+    packed codes of q|k|v and gate|up concatenate, N % 64 == 0."""
+    _align = (16, 1, 1)
+
+    def _check(self, p):
+        if p.shape[0] % 64 or p.shape[1] % ops.INT4_GROUP:
+            raise RuntimeError(f"Int4Weights: weights [N, K] with N % 64 == 0 and K % {ops.INT4_GROUP} == 0 only, "
+                               f"got {tuple(p.shape)}")
+
+    @staticmethod
+    def _sizes(shape):
+        g = shape[0] * shape[1] // ops.INT4_GROUP
+        return shape[0] * shape[1] // 2, g, g
+
+    @staticmethod
+    def _allocate(totals, dev):
+        return (torch.zeros(totals[0], dtype=torch.uint8, device=dev), torch.empty(totals[1], dtype=bf16, device=dev),
+                torch.empty(totals[2], dtype=torch.uint8, device=dev))
+
+    @staticmethod
+    def _views(parts, shape):
+        n, k = shape
+        return parts[0].view(n, k // 2), parts[1].view(n, k // ops.INT4_GROUP), parts[2].view(n, k // ops.INT4_GROUP)
+
+    @staticmethod
+    def _quantize(w, v):
+        ops.quantize_int4_(w, *v)
 
 
 def allreduce_flat_grads(flats, average: bool = True) -> int:
@@ -437,6 +502,7 @@ class LlamaCore:
         self.cos, self.sin = rope_tables(dims, flat.flat.device)
         self.fp8 = None
         self.fp8_src = None
+        self.int4 = None              # per-layer int4 weight triples of the decode step (set_int4)
         self.act_fp8 = False          # W8A8 in the no-grad forwards (ModifiedLlamaForCausalLM.set_activation_dtype)
         self.wgrad_stash: Optional[WgradStash] = None   # deferred linear weight gradients (defer_weight_grads)
 
@@ -456,6 +522,22 @@ class LlamaCore:
             w.wgu.append(fp8.view([m.gate_proj.weight, m.up_proj.weight], (2 * F, D)))
             w.wd.append(fp8.view([m.down_proj.weight], (D, F)))
         self.fp8 = w
+
+    def set_int4(self, int4: Optional[Int4Weights]) -> None:
+        """Stream ``int4``'s copy of the decoder-layer linear weights in the decode-step GEMMs of at most 16 rows (None: the
+        bf16 weights).  Nothing else reads it: lm_head, prefills, no-grad forwards and training run bf16 on W'."""
+        self.int4 = None
+        if int4 is None:
+            return
+        D, F = self.d.hidden, self.d.inter
+        w = SimpleNamespace(wqkv=[], wo=[], wgu=[], wd=[])
+        for lyr in self.model.layers:
+            a, m = lyr.self_attn, lyr.mlp
+            w.wqkv.append(int4.view([a.q_proj.weight, a.k_proj.weight, a.v_proj.weight], (3 * D, D)))
+            w.wo.append(int4.view([a.o_proj.weight], (D, D)))
+            w.wgu.append(int4.view([m.gate_proj.weight, m.up_proj.weight], (2 * F, D)))
+            w.wd.append(int4.view([m.down_proj.weight], (D, F)))
+        self.int4 = w
 
     def fp8_for_inference(self):
         """The per-layer fp8 weight pairs when the copy still describes the current weights, else None.  The inference
@@ -771,11 +853,16 @@ class LlamaCore:
         # (gemm_skinny.cu); larger batches go through nv_gemm_bf16's auto dispatch, which picks the tile variant per (M, N)
         # from a measured table (32-column tiles for the 4096-wide projections, 256 for gate|up: tools/midm_bench.py).
         # With an fp8 copy of the weights (set_fp8), the skinny GEMMs and, up to FP8_MAX_ROWS rows, nv_gemm_fp8w_bf16 stream
-        # it instead: same bits as bf16 on W'.  generate() refuses a stale copy before it gets here.
+        # it instead: same bits as bf16 on W'.  With an int4 copy (set_int4), the skinny GEMMs stream it; above 16 rows the
+        # bf16 kernels run on W', again the same bits.  generate() refuses a stale copy before it gets here.
         skinny = x.shape[0] <= 16
         fuse_mlp = skinny and d.inter % 64 == 0
         f8 = self.fp8 if x.shape[0] <= FP8_MAX_ROWS else None
-        if f8 is not None:
+        q4 = self.int4 if skinny else None
+        if q4 is not None:
+            lin = lambda a, w, addend=None: ops.gemm_skinny_int4(a, *w, addend=addend)
+            wqkv, wo, wgu, wd = q4.wqkv, q4.wo, q4.wgu, q4.wd
+        elif f8 is not None:
             if skinny:
                 lin = lambda a, w, addend=None: ops.gemm_skinny_fp8(a, *w, addend=addend)
             else:
@@ -804,7 +891,9 @@ class LlamaCore:
                 ao = ops.decode_attn_rope(qkv, lens, self.cos, self.sin, kc[l], vc[l], H)   # RoPE + cache append + attention
             xm = lin(ao, wo[l], x)
             xn2, _ = ops.rmsnorm_fwd(xm, lyr.post_attention_layernorm.weight.data, d.rms_eps)
-            if fuse_mlp and f8 is not None:
+            if q4 is not None:                                                           # Int4Weights: F % 64 == 0
+                h = ops.gemm_skinny_swiglu_int4(xn2, *wgu[l])
+            elif fuse_mlp and f8 is not None:
                 h = ops.gemm_skinny_swiglu_fp8(xn2, *wgu[l])
             elif fuse_mlp:
                 h = ops.gemm_skinny_swiglu(xn2, wgu[l])                                 # gate|up projection + SwiGLU

@@ -27,7 +27,7 @@ import torch.nn as nn
 from . import generation
 from . import ops
 from . import trie as trie_mod
-from .llama import FlatParams, Fp8Weights, LlamaCore, LlamaDims, LlamaModelParams, WgradStash, _Linear, kv_cache
+from .llama import FlatParams, Fp8Weights, Int4Weights, LlamaCore, LlamaDims, LlamaModelParams, WgradStash, _Linear, kv_cache
 from .parallel import GradSync
 from .tokenizer import HFTokenizerAdapter, SyntheticTokenizer
 
@@ -730,8 +730,10 @@ class ModifiedLlamaForCausalLM(nn.Module):
         last layer).  Training forwards and the LM-loss lm_head keep the bf16 weights.  Irreversible: reload the checkpoint
         to get W back.  Any later write to the weights (an optimizer step, ``load_state_dict``) makes ``generate`` raise
         until this is called again (or ``drop_fp8_weights``); the no-grad forwards then run bf16 on the current weights.
-        Returns the size of the copy in bytes."""
+        Returns the size of the copy in bytes.  Drops the int4 copy (``quantize_weights_int4``) if there is one; quantizing
+        after that rounds its W' further."""
         self._ensure()
+        self.drop_int4_weights()
         self.drop_fp8_weights()
         self._fp8 = Fp8Weights(self.flat, self.fp8_linear_weights())
         self.core.set_fp8(self._fp8)
@@ -759,6 +761,57 @@ class ModifiedLlamaForCausalLM(nn.Module):
                                f"decode with them in bf16")
         if self.core.fp8 is None:                    # the decoder stack was rebuilt around the same buffer
             self.core.set_fp8(fp8)
+
+    # ---- opt-in 4-bit group-wise weight streaming (W4A16) in the decode step ----
+    def int4_linear_weights(self) -> List[nn.Parameter]:
+        """The weights ``quantize_weights_int4`` rounds: q/k/v/o and gate/up/down of every layer (lm_head stays bf16)."""
+        return self.fp8_linear_weights()[:-1]
+
+    @torch.no_grad()
+    def quantize_weights_int4(self) -> int:
+        """Round every decoder-layer linear weight IN PLACE to W' = bf16((q - z) * s): 4-bit codes q with one bf16 scale s
+        and one 4-bit zero-point z per row and 128 columns (round to nearest, no calibration; rule in
+        include/navillm_b200.h), and keep a 4-bit copy of them (about 3.4 GB at Vicuna-7B).  The model afterwards IS the
+        model with weights W': prefill, navigation, training and ``state_dict()`` all see W'.  The decode-step GEMMs of
+        ``generate`` with at most 16 rows (q|k|v, o_proj, gate|up with SwiGLU, down_proj) then stream the copy, a quarter of
+        the bf16 bytes, with the same bits as the bf16 kernels on W'; above 16 rows the step runs those bf16 kernels on W'.
+        lm_head is neither rounded nor streamed in 4 bits, and prefills, no-grad forwards and training keep the bf16
+        kernels.  Needs hidden and intermediate sizes that are multiples of 128.  Irreversible: reload the checkpoint to
+        get W back.  Any later write to the weights makes ``generate`` raise until this is called again (or
+        ``drop_int4_weights``).
+
+        The fp8 and int4 copies exclude each other: this drops the fp8 copy (``quantize_weights_fp8``), and quantizing to
+        fp8 drops this one.  The roundings compose: after ``quantize_weights_fp8()`` the weights are the fp8 W', and this
+        rounds that W' to 4 bits (and the other way round).  Returns the size of the copy in bytes."""
+        self._ensure()
+        self.drop_fp8_weights()
+        self.drop_int4_weights()
+        self._int4 = Int4Weights(self.flat, self.int4_linear_weights())
+        self.core.set_int4(self._int4)
+        return self._int4.nbytes
+
+    def drop_int4_weights(self) -> None:
+        """Free the int4 copy; ``generate`` goes back to the bf16 kernels (on the weights as they are, W' if quantized)."""
+        self._int4 = None
+        if self.core is not None:
+            self.core.set_int4(None)
+        self._decode_states.clear()                  # captured decode graphs hold the pointers of the other kernels
+
+    @property
+    def int4_weights(self) -> Optional[Int4Weights]:
+        return self.__dict__.get("_int4")
+
+    def _check_int4_fresh(self) -> None:
+        int4 = self.int4_weights
+        if int4 is None:
+            return
+        why = int4.stale_reason(self.flat)
+        if why is not None:
+            raise RuntimeError(f"generate(): the int4 copy of the weights is stale ({why} after quantize_weights_int4()); call "
+                               f"quantize_weights_int4() again to re-quantize the current weights, or drop_int4_weights() to "
+                               f"decode with them in bf16")
+        if self.core.int4 is None:                   # the decoder stack was rebuilt around the same buffer
+            self.core.set_int4(int4)
 
     # ---- opt-in fp8 (e4m3) activations (W8A8) in the no-grad prompt forwards ----
     activation_dtype = "bf16"
@@ -929,6 +982,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
             raise ValueError("generate(do_sample=True) needs temperature > 0")
         self._ensure()
         self._check_fp8_fresh()
+        self._check_int4_fresh()
         dev = self._device()
         eos = self.tokenizer.eos_token_id if eos_token_id is None else eos_token_id
         pad = self.tokenizer.unk_token_id if pad_token_id is None else pad_token_id

@@ -254,6 +254,16 @@ class NavModel(nn.Module):
     def drop_fp8_weights(self) -> None:
         self.lang_model.drop_fp8_weights()
 
+    def quantize_weights_int4(self) -> int:
+        """Opt-in 4-bit group-wise weight streaming (W4A16) in the decode step: ``ModifiedLlamaForCausalLM.quantize_weights_int4``
+        on the language model, so the 3dqa, summarization and embodied_qa modes decode from the int4 copy.  Returns its size
+        in bytes."""
+        self._ensure()
+        return self.lang_model.quantize_weights_int4()
+
+    def drop_int4_weights(self) -> None:
+        self.lang_model.drop_int4_weights()
+
     def set_kv_cache_dtype(self, dtype: str) -> str:
         """KV-cache format of the language model's ``generate()`` (the 3dqa, summarization and embodied_qa modes): ``"bf16"``
         (default) or ``"fp8"``; see ``ModifiedLlamaForCausalLM.set_kv_cache_dtype``.  Returns the previous format."""

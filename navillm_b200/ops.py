@@ -1113,6 +1113,101 @@ def gemm_skinny_swiglu_fp8(x: torch.Tensor, wgu_q: torch.Tensor, exps: torch.Ten
     return out
 
 
+INT4_GROUP = 128
+
+
+def int4_codes_shape(n: int, k: int) -> tuple:
+    """Shape of the uint8 code buffer ``quantize_int4_`` fills for a weight [n, k]: rows padded to a multiple of 64, two
+    codes per byte (in a layout private to csrc/quant.cu and csrc/gemm_skinny.cu)."""
+    return ((n + 63) // 64 * 64, k // 2)
+
+
+def _int4_weight(codes: torch.Tensor, scales: torch.Tensor, zeros: torch.Tensor, n: int, k: int, name: str) -> None:
+    if not (codes.is_cuda and scales.is_cuda and zeros.is_cuda):
+        raise _lib.NvError(f"{name}: navillm_b200 kernels need CUDA tensors (no CPU fallback)")
+    if k % INT4_GROUP:
+        raise ValueError(f"{name}: K must be a multiple of {INT4_GROUP} (got {k})")
+    if codes.dtype != torch.uint8 or tuple(codes.shape) != int4_codes_shape(n, k) or not codes.is_contiguous():
+        raise ValueError(f"{name}: contiguous uint8 codes {int4_codes_shape(n, k)} expected "
+                         f"(got {codes.dtype} {tuple(codes.shape)})")
+    g = k // INT4_GROUP
+    for t, dt, what in ((scales, bf16, "scales"), (zeros, torch.uint8, "zeros")):
+        if t.dtype != dt or tuple(t.shape) != (n, g) or not t.is_contiguous():
+            raise ValueError(f"{name}: contiguous {dt} {what} [{n}, {g}] expected (got {t.dtype} {tuple(t.shape)})")
+    if codes.data_ptr() % 16:
+        raise ValueError(f"{name}: codes must be 16-byte aligned")
+
+
+def quantize_int4_(w: torch.Tensor, codes: torch.Tensor, scales: torch.Tensor, zeros: torch.Tensor) -> torch.Tensor:
+    """Round the bf16 weight w [N, K] (K % 128 == 0) in place to W' = bf16((q - z) * s) in groups of one row and 128
+    columns (csrc/quant.cu, rule in include/navillm_b200.h): codes (``int4_codes_shape``) receives the 4-bit q, scales
+    [N, K / 128] bf16 the s and zeros [N, K / 128] uint8 the z.  Returns w."""
+    _rowmajor(w, "w")
+    if w.dtype != bf16:
+        raise ValueError(f"quantize_int4_: bf16 w expected (got {w.dtype})")
+    N, K = w.shape
+    _int4_weight(codes, scales, zeros, N, K, "quantize_int4_")
+    if w.stride(0) % 8 or w.data_ptr() % 16:
+        raise ValueError("quantize_int4_: w must be 16-byte aligned with a row stride that is a multiple of 8")
+    check(_lib.load().nv_quantize_int4_groups(ptr(w), i64(w.stride(0)), ptr(codes), ptr(scales), ptr(zeros), i32(N), i32(K),
+                                              stream_ptr()), "nv_quantize_int4_groups")
+    return w
+
+
+def _skinny_x(x: torch.Tensor, k: int, name: str) -> int:
+    _rowmajor(x, "x")
+    if x.dtype != bf16 or x.dim() != 2 or x.shape[1] != k or not 1 <= x.shape[0] <= 16:
+        raise ValueError(f"{name}: x bf16 [M <= 16, {k}] expected (got {x.dtype} {tuple(x.shape)})")
+    return x.shape[0]
+
+
+def gemm_skinny_int4(x: torch.Tensor, codes: torch.Tensor, scales: torch.Tensor, zeros: torch.Tensor, *,
+                     addend: torch.Tensor | None = None, out: torch.Tensor | None = None) -> torch.Tensor:
+    """``gemm_skinny`` with the weight in the 4-bit format of ``quantize_int4_`` (codes, scales [N, K / 128], zeros
+    [N, K / 128]): bit for bit ``gemm_skinny(x, W')`` while reading about a quarter of the weight bytes."""
+    if scales.dim() != 2:
+        raise ValueError(f"gemm_skinny_int4: scales [N, K / 128] expected (got {tuple(scales.shape)})")
+    N, G = scales.shape
+    K = G * INT4_GROUP
+    _int4_weight(codes, scales, zeros, N, K, "gemm_skinny_int4")
+    M = _skinny_x(x, K, "gemm_skinny_int4")
+    if out is None:
+        out = torch.empty((M, N), dtype=bf16, device=x.device)
+    _rowmajor(out, "out")
+    if out.shape != (M, N) or out.dtype != bf16:
+        raise ValueError(f"gemm_skinny_int4: out bf16 [{M}, {N}] expected (got {out.dtype} {tuple(out.shape)})")
+    if addend is not None:
+        _rowmajor(addend, "addend")
+        if addend.shape != (M, N) or addend.dtype != bf16:
+            raise ValueError(f"gemm_skinny_int4: addend bf16 [{M}, {N}] expected (got {addend.dtype} {tuple(addend.shape)})")
+    check(_lib.load().nv_gemm_skinny_int4(ptr(x), i64(x.stride(0)), ptr(codes), ptr(scales), ptr(zeros), ptr(out),
+                                          i64(out.stride(0)), ptr(addend), i64(addend.stride(0) if addend is not None else 0),
+                                          i32(M), i32(N), i32(K), stream_ptr()), "nv_gemm_skinny_int4")
+    return out
+
+
+def gemm_skinny_swiglu_int4(x: torch.Tensor, codes: torch.Tensor, scales: torch.Tensor, zeros: torch.Tensor, *,
+                            out: torch.Tensor | None = None) -> torch.Tensor:
+    """``gemm_skinny_swiglu`` with the fused gate|up weight [2F, K] in the 4-bit format (F % 64 == 0)."""
+    if scales.dim() != 2:
+        raise ValueError(f"gemm_skinny_swiglu_int4: scales [2F, K / 128] expected (got {tuple(scales.shape)})")
+    N2, G = scales.shape
+    K, F = G * INT4_GROUP, N2 // 2
+    if N2 != 2 * F or F % 64:
+        raise ValueError(f"gemm_skinny_swiglu_int4: gate|up [2F, K] with F % 64 == 0 expected (got {N2} rows)")
+    _int4_weight(codes, scales, zeros, N2, K, "gemm_skinny_swiglu_int4")
+    M = _skinny_x(x, K, "gemm_skinny_swiglu_int4")
+    if out is None:
+        out = torch.empty((M, F), dtype=bf16, device=x.device)
+    _rowmajor(out, "out")
+    if out.shape != (M, F) or out.dtype != bf16:
+        raise ValueError(f"gemm_skinny_swiglu_int4: out bf16 [{M}, {F}] expected (got {out.dtype} {tuple(out.shape)})")
+    check(_lib.load().nv_gemm_skinny_swiglu_int4(ptr(x), i64(x.stride(0)), ptr(codes), ptr(scales), ptr(zeros), ptr(out),
+                                                 i64(out.stride(0)), i32(M), i32(F), i32(K), stream_ptr()),
+          "nv_gemm_skinny_swiglu_int4")
+    return out
+
+
 def gemm_fp8w(a: torch.Tensor, q: torch.Tensor, e: torch.Tensor, *, addend: torch.Tensor | None = None,
               out: torch.Tensor | None = None, block_n: int = 0) -> torch.Tensor:
     """``gemm(a, W', addend=addend, block_n=block_n)`` with the weight in the fp8 format of ``quantize_fp8_`` (q e4m3 [N, K],

@@ -17,6 +17,15 @@ a bf16 and over an fp8 cache at H = 32, Smax = 512 and C3's context lengths (CUD
 rotated over copies larger than L2, bytes moved and GB/s); (ii) C3-shaped decode ms/token for {bf16 on W', fp8 weights} x
 {bf16 KV, fp8 KV}, alternated, medians over the generations after each capture; (iii) for information, the token agreement
 between the two KV formats (not required to be 100 %: fp8 KV attends over rounded keys and values).
+
+    python tools/fp8_decode_bench.py --int4 [--batch 1 8 16] [--layers 32] [--gens 3] [--rounds 2] [--out FILE.json]
+
+adds the 4-bit group-wise weight copy (quantize_weights_int4): (i) per-GEMM time of the bf16, fp8 and int4 skinny kernels,
+alternated, at M = 1, 8, 16 and the four decoder shapes, weights rotated, bytes moved and GB/s on each format's bytes
+(int4: K/2 bytes of codes per row plus 3 bytes of scale and zero-point per 128 columns); (ii) C3-shaped decode ms/token at
+each batch for bf16 on the int4 W', the fp8 copy and the int4 copy, the arms alternated over ``rounds`` rounds (each visit
+restores W, quantizes, captures once and times ``gens`` generations); (iii) token agreement: int4 vs bf16 on its W' (must
+be 100 %), and for information int4 vs fp8 and vs the unquantized W.
 """
 import argparse
 import gc
@@ -252,6 +261,142 @@ def c3_generate_kv(dev, layers, gens, batch, rounds=2):
     return r
 
 
+INT4_SHAPES = SHAPES[:4]
+
+
+def gemm_table_int4(dev, iters):
+    """bf16 / fp8 / int4 skinny GEMMs alternated at the four decoder shapes, M = 1, 8, 16."""
+    rows = []
+    g = torch.Generator(device=dev).manual_seed(0)
+    for name, N, K, swiglu in INT4_SHAPES:
+        wrows = 2 * N if swiglu else N
+        ncopy = max(2, -(-160 * 2 ** 20 // (wrows * K)))
+        w16, w8, w4 = [], [], []
+        for _ in range(ncopy):
+            w = (torch.randn(wrows, K, device=dev, generator=g) * 0.02).to(torch.bfloat16)
+            q = torch.empty((wrows, K), dtype=ops.fp8, device=dev)
+            e = torch.empty(wrows, dtype=torch.int8, device=dev)
+            ops.quantize_fp8_(w.clone(), q, e)
+            c = torch.empty(ops.int4_codes_shape(wrows, K), dtype=torch.uint8, device=dev)
+            sc = torch.empty((wrows, K // 128), dtype=torch.bfloat16, device=dev)
+            z = torch.empty((wrows, K // 128), dtype=torch.uint8, device=dev)
+            ops.quantize_int4_(w, c, sc, z)                                   # w is now the int4 W'
+            w16.append(w); w8.append((q, e)); w4.append((c, sc, z))
+        for M in (1, 8, 16):
+            x = torch.randn(M, K, device=dev, generator=g).to(torch.bfloat16)
+            if swiglu:
+                fs = {"bf16": lambda i: ops.gemm_skinny_swiglu(x, w16[i % ncopy]),
+                      "fp8": lambda i: ops.gemm_skinny_swiglu_fp8(x, *w8[i % ncopy]),
+                      "int4": lambda i: ops.gemm_skinny_swiglu_int4(x, *w4[i % ncopy])}
+            else:
+                fs = {"bf16": lambda i: ops.gemm_skinny(x, w16[i % ncopy]),
+                      "fp8": lambda i: ops.gemm_skinny_fp8(x, *w8[i % ncopy]),
+                      "int4": lambda i: ops.gemm_skinny_int4(x, *w4[i % ncopy])}
+            same = torch.equal(fs["bf16"](0), fs["int4"](0))
+            t = {k: [] for k in fs}
+            for i in range(5):
+                for f in fs.values():
+                    f(i)
+            torch.cuda.synchronize()
+            order = list(fs)
+            for rep in range(6):                                              # rotate the order of the three kernels
+                for kind in order[rep % 3:] + order[:rep % 3]:
+                    st, en = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    st.record()
+                    for i in range(iters):
+                        fs[kind](i)
+                    en.record()
+                    torch.cuda.synchronize()
+                    t[kind].append(st.elapsed_time(en) / iters)
+            io = M * K * 2 + M * N * 2
+            by = {"bf16": wrows * K * 2 + io, "fp8": wrows * K + wrows + io, "int4": wrows * K // 2 + wrows * (K // 128) * 3 + io}
+            r = {"gemm": name, "M": M, "N": N, "K": K, "int4_bit_identical_to_bf16_on_Wq": same}
+            for kind in fs:
+                us = 1e3 * float(np.median(t[kind]))
+                r[f"{kind}_us"] = round(us, 2)
+                r[f"{kind}_bytes"] = by[kind]
+                r[f"{kind}_GBps"] = round(by[kind] / us / 1e3, 1)
+            r["int4_vs_fp8"] = round(r["fp8_us"] / r["int4_us"], 3)
+            r["int4_vs_bf16"] = round(r["bf16_us"] / r["int4_us"], 3)
+            rows.append(r)
+            print(json.dumps(r), flush=True)
+        del w16, w8, w4
+        torch.cuda.empty_cache()
+    return rows
+
+
+def c3_model(dev, layers):
+    if layers != bench.N_LAYERS:
+        import navillm_b200.nav_model as nm
+        nm.VICUNA_7B["num_hidden_layers"] = layers
+    model = bench.build_model(dev, seed=0).eval()
+    model._ensure()
+    return model, model.lang_model.flat.flat.clone()
+
+
+def c3_generate_int4(dev, model, W, layers, gens, batch, rounds):
+    """C3-shaped decode ms/token for bf16 on the int4 W', the fp8 copy and the int4 copy, alternated: every visit restores
+    the weights W, quantizes for its arm, captures once and times ``gens`` generations."""
+    wl = bench.WORKLOADS["c3"]
+    B, NV, NT, NEW = batch, wl["n_cand_tok"], wl["n_text"], wl["n_new"]
+    lm = model.lang_model
+    lm.drop_fp8_weights()
+    lm.drop_int4_weights()
+    with torch.no_grad():
+        lm.flat.flat.copy_(W)
+    rng = np.random.RandomState(1234)
+    words = [f"w{i}" for i in range(5000)]
+    prompts = ["Scene " + " ".join(["<cand>"] * NV) + " Question " + " ".join(words[i] for i in rng.randint(0, 5000, size=NT - 5))
+               + " Answer" for _ in range(B)]
+    text = lm.tokenize(prompts)
+    S0 = int(text["attention_mask"].sum(1).max())
+    g = torch.Generator().manual_seed(1234)
+    with torch.no_grad():
+        view = torch.stack([torch.randn(NV, bench.IMG_FEAT, generator=g) for _ in range(B)], 0).to(dev)
+        pano = model.img_embeddings.forward_panorama_per_step(view_img_fts=view, view_lens=torch.full((B,), NV, device=dev))
+        cand = model._masked_rows_plus_const(pano["pano_embeds"].reshape(B * NV, -1), np.ones((B, NV), dtype=bool)).detach()
+
+    def run(n):
+        per_tok, out = [], None
+        for i in range(n + 1):                                                # the first one captures the CUDA graph
+            st = {}
+            out = lm.generate(input_ids=text["input_ids"], attention_mask=text["attention_mask"], cand_vis=cand,
+                              max_new_tokens=NEW, stop_on_eos=False, use_cuda_graph=True, stats=st)
+            if i > 0:
+                per_tok.append(st["decode_ms"] / st["decode_steps"])
+        return per_tok, out[:, text["input_ids"].shape[1]:].cpu()
+
+    _, ids_w = run(0)                                                         # bf16 on the unquantized W
+    arms = ("int4", "fp8", "bf16_Wq4")
+    times, ids, nbytes = {a: [] for a in arms}, {}, {}
+    for rnd in range(rounds):
+        for arm in arms[rnd % 3:] + arms[:rnd % 3]:
+            lm.drop_fp8_weights()
+            lm.drop_int4_weights()
+            with torch.no_grad():
+                lm.flat.flat.copy_(W)
+            if arm == "fp8":
+                nbytes["fp8"] = model.quantize_weights_fp8()
+            else:
+                nbytes["int4"] = model.quantize_weights_int4()
+                if arm == "bf16_Wq4":
+                    lm.drop_int4_weights()
+            pt, ids[arm] = run(gens)
+            times[arm] += pt
+    lm.drop_fp8_weights()
+    lm.drop_int4_weights()
+    med = {a: float(np.median(v)) for a, v in times.items()}
+    agree = lambda a, b: float((a == b).float().mean())
+    return {"B": B, "S0": S0, "new_tokens": NEW, "layers": layers, "generations_per_arm": len(times["int4"]),
+            "int4_copy_GB": round(nbytes["int4"] / 1e9, 3), "fp8_copy_GB": round(nbytes["fp8"] / 1e9, 3),
+            "decode_ms_per_token_bf16_Wq4": round(med["bf16_Wq4"], 4), "decode_ms_per_token_fp8": round(med["fp8"], 4),
+            "decode_ms_per_token_int4": round(med["int4"], 4),
+            "decode_ms_per_token_spread": {a: [round(min(v), 4), round(max(v), 4)] for a, v in times.items()},
+            "int4_vs_fp8": round(med["fp8"] / med["int4"], 3), "int4_vs_bf16_Wq4": round(med["bf16_Wq4"] / med["int4"], 3),
+            "token_agreement_int4_vs_bf16_Wq4": agree(ids["int4"], ids["bf16_Wq4"]),
+            "token_agreement_int4_vs_fp8": agree(ids["int4"], ids["fp8"]), "token_agreement_int4_vs_bf16_W": agree(ids["int4"], ids_w)}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--layers", type=int, default=32)
@@ -261,6 +406,9 @@ def main():
     ap.add_argument("--batch", type=int, nargs="*", default=[], help="decode batch sizes of the generate comparison (default: C3's)")
     ap.add_argument("--kv", action="store_true", help="compare the bf16 and the fp8 KV cache instead of the weight formats alone: "
                                                        "decode-attention kernel times, then generate() over weights x KV formats")
+    ap.add_argument("--int4", action="store_true", help="add the int4 weight copy: bf16 / fp8 / int4 GEMMs, then generate() "
+                                                         "for bf16 on the int4 W', fp8 and int4, alternated")
+    ap.add_argument("--rounds", type=int, default=2, help="--int4: visits of each arm per batch size")
     ap.add_argument("--out", default=None, help="also write the result as JSON here")
     a = ap.parse_args()
     if not torch.cuda.is_available():
@@ -268,6 +416,20 @@ def main():
     dev = torch.device("cuda:0")
     res = {"gpu": bench.gpu_info(0)}
     print(json.dumps(res["gpu"]), flush=True)
+    if a.int4:
+        res["gemm_int4"] = [] if a.skip_gemm else gemm_table_int4(dev, a.iters)
+        res["c3_generate_int4"] = []
+        model, W = c3_model(dev, a.layers)
+        for b in a.batch or [1, 8, 16]:
+            res["c3_generate_int4"].append(c3_generate_int4(dev, model, W, a.layers, a.gens, b, a.rounds))
+            print(json.dumps(res["c3_generate_int4"][-1]), flush=True)
+            gc.collect()
+            torch.cuda.empty_cache()
+        res["gpu_after"] = bench.gpu_info(0)
+        if a.out:
+            Path(a.out).parent.mkdir(parents=True, exist_ok=True)
+            Path(a.out).write_text(json.dumps(res, indent=1))
+        return
     if a.kv:
         batches = a.batch or [8, 32, 64]
         res["kv_attention"] = kv_attn_table(dev, a.iters, batches)
