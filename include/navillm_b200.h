@@ -98,6 +98,14 @@ int nv_gemm_skinny_swiglu_int4(const void* X, int64_t ldx, const void* codes, co
  * and tile width.  block_n: 0 (auto), 32 or 128.  lda % 8 == 0, ldw (bytes) % 16 == 0. */
 int nv_gemm_fp8w_bf16(const void* A, int64_t lda, const void* Wq, int64_t ldw, const void* exps, void* C, int64_t ldc,
                       const void* addend, int64_t ld_add, int M, int N, int K, int block_n, void* stream);
+/* nv_gemm_int4w_bf16 is nv_gemm_fp8w_bf16 with the weight given as (codes, scales, zeros) in the 4-bit format above, for
+ * the same inference GEMMs above 16 rows (decode batches, beams and samples of 17..64 rows, pruned last layers, small
+ * prefix-cached suffixes and prefills; nv_llama_layer_infer and LlamaCore.decode_step): bit for bit nv_gemm_bf16's result
+ * on W' at every M, N, K and tile width, reading about a quarter of the weight bytes.  block_n: 0 (auto), 32 or 128.
+ * K % 128 == 0, N % 64 == 0, lda % 8 == 0 and lda >= K, ldc (and ld_add) >= N; A, codes, C and addend 16-byte aligned.
+ * The codes have no leading dimension: N and K fix their layout. */
+int nv_gemm_int4w_bf16(const void* A, int64_t lda, const void* codes, const void* scales, const void* zeros, void* C,
+                       int64_t ldc, const void* addend, int64_t ld_add, int M, int N, int K, int block_n, void* stream);
 /* Opt-in W8A8 of the no-grad prompt forwards (set_activation_dtype("fp8"); no reference counterpart for the number format;
  * csrc/gemm_fp8.cu).  nv_quantize_act_fp8 quantizes a bf16 activation X [M,K] (row stride ldx) per (row, 128-column block)
  * with the rule of nv_quantize_fp8_rows: Q [M,K] e4m3 bytes (row stride ldq bytes) and E [M, K/128] int8 exponents (row
@@ -425,6 +433,12 @@ typedef struct nv_layer_args {
   /* 1: the four GEMMs run W8A8 at every row count (nv_quantize_act_fp8 of the GEMM input + nv_gemm_w8a8_bf16 on the fp8
    * weight pairs above, which must all be set; D and F multiples of 128); fp8_max_rows is then ignored */
   int act_fp8;
+  /* optional int4 copies of the four weights (codes, bf16 scales, uint8 zero-points: nv_quantize_int4_groups); a GEMM
+   * whose triple is set and whose row count is in 17..int4_max_rows runs nv_gemm_int4w_bf16 (at most 16 rows: bf16, as
+   * without the copy).  Exclusive with the fp8 pairs and act_fp8. */
+  const void* wqkv_c; const void* wqkv_s; const void* wqkv_z; const void* wo_c; const void* wo_s; const void* wo_z;
+  const void* wgu_c; const void* wgu_s; const void* wgu_z; const void* wd_c; const void* wd_s; const void* wd_z;
+  int int4_max_rows;
 } nv_layer_args;
 int nv_layer_args_size(void);                           /* sizeof(nv_layer_args): bindings check their mirror against it */
 int64_t nv_llama_layer_ws_bytes(int T, int R, int D, int F);

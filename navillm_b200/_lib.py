@@ -51,7 +51,10 @@ class LayerArgs(ctypes.Structure):
                 + [(n, ctypes.c_void_p) for n in ("wqkv_q", "wqkv_e", "wo_q", "wo_e", "wgu_q", "wgu_e", "wd_q", "wd_e")]
                 + [("fp8_max_rows", ctypes.c_int)]
                 + [(n, ctypes.c_void_p) for n in ("kexp", "vexp")]
-                + [("act_fp8", ctypes.c_int)])
+                + [("act_fp8", ctypes.c_int)]
+                + [(n, ctypes.c_void_p) for n in ("wqkv_c", "wqkv_s", "wqkv_z", "wo_c", "wo_s", "wo_z",
+                                                  "wgu_c", "wgu_s", "wgu_z", "wd_c", "wd_s", "wd_z")]
+                + [("int4_max_rows", ctypes.c_int)])
 
 
 launch_count = 0          # kernels launched through the C ABI since import (bench.py reports the per-step delta)

@@ -32,11 +32,18 @@
 // a third mbarrier per stage; the consumers wait for it and run the unchanged SS wgmmas.  The expansion of stage s + 1
 // overlaps the MMAs of stage s.  The k-blocks, the wgmma sequence and the epilogue are those of the bf16 kernel, and the
 // expanded operand is bit for bit the W' the quantizer wrote back, so C equals nv_gemm_bf16's C on W'.
+//
+// 4-bit weights (WT = Int4W; same restrictions): B is the packed code copy of nv_int4.cuh with its bf16 scales and uint8
+// zero-points per (row, 128-column group).  The producer TMA-loads the tile's codes as they lie in HBM: a 128-row tile is
+// two 2 KB chunks, a 32-row tile the half of one chunk that holds its rows (the codes of chunk rows 0..31 are its first
+// 1024 bytes).  The expansion warpgroup dequantizes them with q4_dequant_pair (exact bf16x2 subtract, one bf16x2 multiply:
+// the rule's W') into the 128-byte-swizzled bf16 stage; the rest is the fp8 path's, so C again equals nv_gemm_bf16's on W'.
 #include <type_traits>
 
 #include "nv_common.cuh"
 #include "nv_fp8.cuh"
 #include "nv_host.h"
+#include "nv_int4.cuh"
 
 namespace nv {
 
@@ -73,20 +80,27 @@ struct EpiAux {
   const __nv_bfloat16* sin_t;
   uint32_t rope_cols;   // ROPE: q and k columns (2 * H * 128)
   const int8_t* w_exp;  // fp8 weights: w_exp[n] = exponent of weight row n (W' = e4m3 * 2^w_exp)
+  const __nv_bfloat16* q4_scale;  // 4-bit weights: scale and zero-point of (row n, group g) at [n * K / 128 + g]
+  const uint8_t* q4_zero;
 };
 
-// Shared memory: [A stages][B stages][fp8 only: expanded bf16 B stages][full | empty | fp8 only: expanded barriers]
+// tag of the 4-bit weight type (nv_int4.cuh)
+struct Int4W {};
+
+// Shared memory: [A stages][B stages][fp8 / int4 only: expanded bf16 B stages][full | empty | fp8 / int4 only: expanded barriers]
 template <uint32_t BLOCK_N, uint32_t STAGES, typename WT = __nv_bfloat16>
 struct GemmSmem {
-  static constexpr bool kFp8 = sizeof(WT) == 1;
-  static constexpr uint32_t THREADS = kFp8 ? GEMM_THREADS + 128 : GEMM_THREADS;   // + the expansion warpgroup
+  static constexpr bool kInt4 = std::is_same<WT, Int4W>::value;
+  static constexpr bool kFp8 = !kInt4 && sizeof(WT) == 1;
+  static constexpr bool kExpand = kFp8 || kInt4;                                 // B is expanded to bf16 in shared memory
+  static constexpr uint32_t THREADS = kExpand ? GEMM_THREADS + 128 : GEMM_THREADS;   // + the expansion warpgroup
   static constexpr uint32_t A_BYTES = GEMM_BLOCK_M * GEMM_BLOCK_K * 2;
-  static constexpr uint32_t B_BYTES = BLOCK_N * GEMM_BLOCK_K * sizeof(WT);
+  static constexpr uint32_t B_BYTES = kInt4 ? BLOCK_N * GEMM_BLOCK_K / 2 : BLOCK_N * GEMM_BLOCK_K * sizeof(WT);
   static constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;                      // TMA bytes per stage
-  static constexpr uint32_t CVT_BYTES = kFp8 ? BLOCK_N * GEMM_BLOCK_K * 2 : 0;
+  static constexpr uint32_t CVT_BYTES = kExpand ? BLOCK_N * GEMM_BLOCK_K * 2 : 0;
   static constexpr uint32_t CVT_OFF = STAGES * STAGE_BYTES;
   static constexpr uint32_t BAR_OFF = CVT_OFF + STAGES * CVT_BYTES;
-  static constexpr uint32_t DYN_BYTES = BAR_OFF + (kFp8 ? 3 : 2) * STAGES * 8 + 1024;  // + slack for 1024-byte alignment
+  static constexpr uint32_t DYN_BYTES = BAR_OFF + (kExpand ? 3 : 2) * STAGES * 8 + 1024;  // + slack for 1024-byte alignment
   static_assert(CVT_OFF % 1024 == 0, "the expanded stages are 128-byte-swizzle atoms");
   static constexpr uint32_t ACC_LD = BLOCK_N + 4;                         // staged fp32 row (+16 B: conflict-free)
   static_assert(GEMM_BLOCK_M * ACC_LD * 4 <= BAR_OFF, "accumulator staging reuses the stage ring");
@@ -122,7 +136,8 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
                 uint32_t M, uint32_t N, uint32_t K, uint32_t flags, EpiAux ea) {
   using L = GemmSmem<BLOCK_N, STAGES, WT>;
   static_assert(BLOCK_N <= 128, "the 128 x 256 tile is gemm_bf16_wide");
-  static_assert(!L::kFp8 || (!A_MN && !B_MN), "fp8 weights: K-major operands");
+  static_assert(!L::kExpand || (!A_MN && !B_MN), "fp8 / int4 weights: K-major operands");
+  static_assert(!L::kInt4 || BLOCK_N == 32 || BLOCK_N == 128, "int4 weights: half a code chunk or two chunks per tile");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
@@ -130,7 +145,7 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
   uint8_t* smem_cvt = smem + L::CVT_OFF;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* cvt_bar = empty_bar + STAGES;                 // fp8: the expanded bf16 B tile of the stage is complete
+  uint64_t* cvt_bar = empty_bar + STAGES;                 // fp8 / int4: the expanded bf16 B tile of the stage is complete
 
   const uint32_t warp = warp_id_uniform();
   const uint32_t num_m = ceil_div_u32(M, GEMM_BLOCK_M);
@@ -142,9 +157,9 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
   if (threadIdx.x == 0) {
     for (uint32_t i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      // one arrive per consumer warpgroup (fp8: + one per expansion thread, after its reads of the raw tile)
-      mbar_init(&empty_bar[i], L::kFp8 ? 2 + 128 : 2);
-      if constexpr (L::kFp8) mbar_init(&cvt_bar[i], 128);
+      // one arrive per consumer warpgroup (fp8 / int4: + one per expansion thread, after its reads of the raw tile)
+      mbar_init(&empty_bar[i], L::kExpand ? 2 + 128 : 2);
+      if constexpr (L::kExpand) mbar_init(&cvt_bar[i], 128);
     }
     fence_mbar_init();
   }
@@ -170,7 +185,18 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
           for (uint32_t i = 0; i < GEMM_BLOCK_M / 64; ++i)  // box {64 m, 64 k} per 64-wide MN atom
             tma_load_2d(sa + i * (GEMM_BLOCK_K * 128), &tmap_a, &full_bar[stage], m0 + i * 64, k0);
         }
-        if constexpr (L::kFp8) {
+        if constexpr (L::kInt4) {
+          // tmap_b: the codes as rows of 256 words, two per 2 KB chunk (rb, kb) at row 2 (rb K / 64 + kb); chunks of row
+          // blocks past N are TMA zero fill
+          const int32_t nkb_all = K / GEMM_BLOCK_K;
+          if constexpr (BLOCK_N == 32) {        // box {256, 1}: the half of chunk n_blk / 2 that holds rows 32 (n_blk % 2)..
+            tma_load_2d(sb, &tmap_b, &full_bar[stage], 0, 2 * ((n_blk >> 1) * nkb_all + kb) + (n_blk & 1));
+          } else {                              // box {256, 2}: chunks 2 n_blk, 2 n_blk + 1
+#pragma unroll
+            for (uint32_t i = 0; i < 2; ++i)
+              tma_load_2d(sb + i * Q4_CHUNK_BYTES, &tmap_b, &full_bar[stage], 0, 2 * ((2 * n_blk + i) * nkb_all + kb));
+          }
+        } else if constexpr (L::kFp8) {
           tma_load_2d(sb, &tmap_b, &full_bar[stage], k0, n_blk * BLOCK_N);   // box {64 k, BLOCK_N n}, unswizzled e4m3
         } else if constexpr (!B_MN) {
           constexpr uint32_t BOX = BLOCK_N < 128 ? BLOCK_N : 128;  // box {64 k, BOX n}
@@ -229,6 +255,76 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
       }
       return;
     }
+  } else if constexpr (L::kInt4) {
+    if (warp >= 9) {
+      // ===================== int4 expansion (warps 9..12) =====================
+      // 128 rows: thread t dequantizes the 16 code bytes t of both chunks (rows 64 c + r0, 64 c + r1, nv_int4.cuh).  32 rows:
+      // the half chunk holds the bytes of units u = 0..63 (rows r0, r1 of u < 32 rows); thread t takes words 2 (t % 2),
+      // 2 (t % 2) + 1 of unit t / 2.  Word j of a unit is the k16 step j: pair p goes to row r0 (p even) or r1, columns
+      // 16 j + 2 (l % 4) + 8 (p / 2) ..+1 of the swizzled bf16 row.  Rows >= N (zero fill) get scale 0.
+      constexpr uint32_t NR = BLOCK_N == 32 ? 1 : 2;     // chunks (row pairs r0, r1) per thread
+      constexpr uint32_t NW = BLOCK_N == 32 ? 2 : 4;     // words per chunk per thread
+      const uint32_t t = threadIdx.x - GEMM_THREADS;
+      const uint32_t u = BLOCK_N == 32 ? t >> 1 : t, w0 = BLOCK_N == 32 ? 2 * (t & 1) : 0;
+      const uint32_t l = u & 31, r0 = ((u >> 5) << 4) + (l >> 2), c0 = 2 * (l & 3);
+      const uint32_t G = K / Q4_GROUP;
+      int64_t gbase[NR][2];                              // (row, group 0) of rows 64 c + r0, 64 c + r0 + 8; -1: row >= N
+#pragma unroll
+      for (uint32_t c = 0; c < NR; ++c)
+#pragma unroll
+        for (uint32_t h = 0; h < 2; ++h) {
+          const uint32_t n = n_blk * BLOCK_N + 64 * c + r0 + 8 * h;
+          gbase[c][h] = n < N ? (int64_t)n * G : -1;
+        }
+      uint32_t sx[NR][2], zx[NR][2];
+      uint32_t stage = 0, phase = 0;
+      for (uint32_t kb = 0; kb < num_kb; ++kb) {
+        if ((kb & 1) == 0) {                             // a group spans two k-blocks: its parameters, before the wait
+#pragma unroll
+          for (uint32_t c = 0; c < NR; ++c)
+#pragma unroll
+            for (uint32_t h = 0; h < 2; ++h) {
+              uint32_t s = 0, z = 0;
+              if (gbase[c][h] >= 0) {
+                const int64_t gi = gbase[c][h] + (kb >> 1);
+                s = __ldg(reinterpret_cast<const unsigned short*>(ea.q4_scale) + gi);
+                z = __ldg(ea.q4_zero + gi);
+              }
+              sx[c][h] = s * 0x10001u;
+              zx[c][h] = (0x4300u + z) * 0x10001u;
+            }
+        }
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t src = smem_u32(smem_b + stage * L::B_BYTES);
+        const uint32_t dst = smem_u32(smem_cvt + stage * L::CVT_BYTES);
+#pragma unroll
+        for (uint32_t c = 0; c < NR; ++c) {
+          uint32_t wd[NW];
+          if constexpr (NW == 4) {
+            const uint4 v = lds128(src + c * Q4_CHUNK_BYTES + 16 * u);
+            wd[0] = v.x; wd[1] = v.y; wd[2] = v.z; wd[3] = v.w;
+          } else {
+            const uint2 v = lds64(src + 16 * u + 4 * w0);
+            wd[0] = v.x; wd[1] = v.y;
+          }
+#pragma unroll
+          for (uint32_t i = 0; i < NW; ++i) {
+            const uint32_t j = w0 + i, row = 64 * c + r0;
+            uint32_t a[4];
+            q4_dequant_k16(wd[i], sx[c][0], zx[c][0], sx[c][1], zx[c][1], a);
+            sts32(dst + sw128_offset(row, 2 * j) + 2 * c0, a[0]);
+            sts32(dst + sw128_offset(row + 8, 2 * j) + 2 * c0, a[1]);
+            sts32(dst + sw128_offset(row, 2 * j + 1) + 2 * c0, a[2]);
+            sts32(dst + sw128_offset(row + 8, 2 * j + 1) + 2 * c0, a[3]);
+          }
+        }
+        fence_proxy_async_smem();                          // generic-proxy writes -> wgmma operand reads
+        mbar_arrive(&cvt_bar[stage]);
+        mbar_arrive(&empty_bar[stage]);                    // this thread's part of the raw code tile has been read
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      return;
+    }
   }
 
   // ===================== consumers (warpgroups 0, 1) =====================
@@ -248,9 +344,9 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
     __builtin_assume(num_kb > 0);
     for (uint32_t kb = 0; kb < num_kb; ++kb) {
       mbar_wait(&full_bar[stage], phase);
-      if constexpr (L::kFp8) mbar_wait(&cvt_bar[stage], phase);
+      if constexpr (L::kExpand) mbar_wait(&cvt_bar[stage], phase);
       const uint64_t adesc = gmma_desc_sw128(smem_u32(smem_a + stage * L::A_BYTES + wg * 8192), A_LBO, 1024);
-      const uint64_t bdesc = gmma_desc_sw128(smem_u32(L::kFp8 ? smem_cvt + stage * L::CVT_BYTES : smem_b + stage * L::B_BYTES),
+      const uint64_t bdesc = gmma_desc_sw128(smem_u32(L::kExpand ? smem_cvt + stage * L::CVT_BYTES : smem_b + stage * L::B_BYTES),
                                              B_LBO, 1024);
       wgmma_fence();
 #pragma unroll
@@ -966,6 +1062,47 @@ extern "C" int nv_gemm_fp8w_bf16(const void* A, int64_t lda, const void* Wq, int
   if (block_n == 32)
     return launch_gemm<32, 10, false, false, uint8_t>(ta, tb, C, ldc, addend, ld_add, M, N, K, flags, stream, ea);
   return launch_gemm<128, 5, false, false, uint8_t>(ta, tb, C, ldc, addend, ld_add, M, N, K, flags, stream, ea);
+}
+
+// C[M,N] = A[M,K] · W'[N,K]^T (+ addend) with W' = bf16((q - z) * s) given in the 4-bit format of nv_quantize_int4_groups
+// (packed codes, bf16 scales [N, K / 128], uint8 zero-points [N, K / 128]): bit for bit nv_gemm_bf16(A, W', block_n) for
+// every M, N, K, reading about a quarter of the weight bytes.  The codes have no leading dimension: their layout is fixed
+// by N and K (nv_int4.cuh).
+extern "C" int nv_gemm_int4w_bf16(const void* A, int64_t lda, const void* codes, const void* scales, const void* zeros, void* C,
+                                  int64_t ldc, const void* addend, int64_t ld_add, int M, int N, int K, int block_n,
+                                  void* stream_) {
+  using namespace nv;
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  NV_REQUIRE(M > 0 && N > 0 && K > 0, "nv_gemm_int4w_bf16: empty problem M=%d N=%d K=%d", M, N, K);
+  NV_REQUIRE(A && codes && scales && zeros && C, "nv_gemm_int4w_bf16: null operand");
+  NV_REQUIRE(K % (int)Q4_GROUP == 0 && N % 64 == 0, "nv_gemm_int4w_bf16: needs K %% 128 == 0 and N %% 64 == 0 (got N=%d K=%d)",
+             N, K);
+  NV_REQUIRE((lda & 7) == 0 && lda >= K, "nv_gemm_int4w_bf16: lda must be a multiple of 8 and at least K (got %lld)",
+             (long long)lda);
+  NV_REQUIRE(ldc >= N && (!addend || ld_add >= N), "nv_gemm_int4w_bf16: ldc %lld / ld_add %lld below N=%d", (long long)ldc,
+             (long long)ld_add, N);
+  NV_REQUIRE(((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(codes) | reinterpret_cast<uintptr_t>(C)) & 15) == 0,
+             "nv_gemm_int4w_bf16: A %p, codes %p and C %p must be 16-byte aligned", A, codes, C);
+  NV_REQUIRE((reinterpret_cast<uintptr_t>(scales) & 1) == 0, "nv_gemm_int4w_bf16: scales %p not 2-byte aligned", scales);
+  NV_REQUIRE(!addend || (reinterpret_cast<uintptr_t>(addend) & 15) == 0, "nv_gemm_int4w_bf16: addend %p not 16-byte aligned",
+             addend);
+  // auto: nv_gemm_bf16's choice for K-major operands below M = 512 (the 256-wide tile is not built for int4 weights)
+  if (block_n == 0) block_n = (M <= 128 && N <= 4096) ? 32 : 128;
+  NV_REQUIRE(block_n == 32 || block_n == 128, "nv_gemm_int4w_bf16: block_n must be 0, 32 or 128 (got %d)", block_n);
+  CUtensorMap ta, tb;
+  int rc = make_tmap_2d(&ta, A, 2, (uint64_t)K, (uint64_t)M, (uint64_t)lda * 2, 64, GEMM_BLOCK_M);
+  if (rc) return rc;
+  // the codes as rows of 256 words, two per 2 KB chunk (nv_int4.cuh)
+  const uint64_t chunks = (uint64_t)(N / 64) * (uint64_t)(K / GEMM_BLOCK_K);
+  if ((rc = make_tmap_2d(&tb, codes, 4, 256, 2 * chunks, 1024, 256, block_n == 32 ? 1 : 2, /*swizzle128=*/false))) return rc;
+  EpiAux ea{};
+  ea.q4_scale = reinterpret_cast<const __nv_bfloat16*>(scales);
+  ea.q4_zero = reinterpret_cast<const uint8_t*>(zeros);
+  const uint32_t flags = addend ? GEMM_ADD : 0u;
+  // stages: 10 of 21 KB (A, codes, expanded B) at BLOCK_N = 32, as the bf16 kernel; 6 of 36 KB at 128
+  if (block_n == 32)
+    return launch_gemm<32, 10, false, false, Int4W>(ta, tb, C, ldc, addend, ld_add, M, N, K, flags, stream, ea);
+  return launch_gemm<128, 6, false, false, Int4W>(ta, tb, C, ldc, addend, ld_add, M, N, K, flags, stream, ea);
 }
 
 // ---- fused-epilogue entry points (K-major activations x nn.Linear weights) -------------------------------------

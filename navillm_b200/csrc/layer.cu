@@ -9,6 +9,7 @@
 // need it (their step is GPU-bound) and keep the per-kernel path, which also saves the activations for the backward.
 // act_fp8 (set_activation_dtype("fp8")): each of the four GEMMs is nv_quantize_act_fp8 of its input into the workspace
 // followed by nv_gemm_w8a8_bf16 on the fp8 weight copy, at every row count.
+// int4 weight triples: a GEMM of 17..int4_max_rows rows runs nv_gemm_int4w_bf16 on its triple, with the bits of bf16 on W'.
 #include <stdint.h>
 
 #include "navillm_b200.h"
@@ -75,11 +76,17 @@ extern "C" int nv_llama_layer_infer(const nv_layer_args* a, void* stream) {
                "nv_llama_layer_infer: act_fp8 needs the fp8 copies of all four weights");
     NV_REQUIRE(D % 128 == 0 && F % 128 == 0, "nv_llama_layer_infer: act_fp8 needs D and F multiples of 128 (D=%d F=%d)", D, F);
   }
+  const bool any_fp8 = a->wqkv_q || a->wqkv_e || a->wo_q || a->wo_e || a->wgu_q || a->wgu_e || a->wd_q || a->wd_e;
+  const bool any_int4 = a->wqkv_c || a->wo_c || a->wgu_c || a->wd_c;
+  NV_REQUIRE(!(any_int4 && (any_fp8 || a->act_fp8)), "nv_llama_layer_infer: the int4 and the fp8 weight copies exclude each other");
   int rc;
   // y[rows, N] = x[rows, K] W^T (+ addend): W8A8 on the fp8 copy of W in act_fp8 mode; else the fp8 copy of W when it is
-  // given and the GEMM has at most fp8_max_rows rows
-  auto linear = [&](const void* x, const void* w, const void* wq, const void* we, void* y, const void* addend, int rows, int N,
-                    int K) {
+  // given and the GEMM has at most fp8_max_rows rows; else the int4 copy (c, s, z) when it is given and the GEMM has
+  // 17..int4_max_rows rows
+  auto linear = [&](const void* x, const void* w, const void* wq, const void* we, const void* c, const void* s, const void* z,
+                    void* y, const void* addend, int rows, int N, int K) {
+    if (c && s && z && rows > 16 && rows <= a->int4_max_rows)
+      return nv_gemm_int4w_bf16(x, K, c, s, z, y, N, addend, D, rows, N, K, 0, stream);
     if (a->act_fp8) {
       const int qrc = nv_quantize_act_fp8(x, K, aq, K, ae, K / 128, rows, K, stream);
       if (qrc != NV_OK) return qrc;
@@ -92,7 +99,7 @@ extern "C" int nv_llama_layer_infer(const nv_layer_args* a, void* stream) {
 #define STEP(call) do { rc = (call); if (rc != NV_OK) return rc; } while (0)
   // ---- attention block:  xm = x + o_proj(attn(rope(qkv(rmsnorm1(x))))) ----
   STEP(nv_rmsnorm_fwd(a->x, D, a->ln1, xn, D, rstd, T, D, a->eps, stream));
-  STEP(linear(xn, a->wqkv, a->wqkv_q, a->wqkv_e, qkv, nullptr, T, 3 * D, D));
+  STEP(linear(xn, a->wqkv, a->wqkv_q, a->wqkv_e, a->wqkv_c, a->wqkv_s, a->wqkv_z, qkv, nullptr, T, 3 * D, D));
   STEP(nv_rope_inplace(qkv, 3 * (int64_t)D, a->pos, a->cos_t, a->sin_t, T, 2 * H, 128, 0, stream));
   if (a->kv_mode == 2) {            // new rows appended to a cache that already holds a prefix; attention over the cache
     STEP(nv_kv_store_suffix(qkv, 3 * (int64_t)D, a->cu_seqlens, a->cached, a->kcache, a->vcache, a->B, T, a->Smax, D, stream));
@@ -116,12 +123,12 @@ extern "C" int nv_llama_layer_infer(const nv_layer_args* a, void* stream) {
     STEP(nv_gather_rows(ao, D, a->out_rows, aor, D, R, D, stream));
     STEP(nv_gather_rows(a->x, D, a->out_rows, xr, D, R, D, stream));
   }
-  STEP(linear(aor, a->wo, a->wo_q, a->wo_e, xm, xr, Tm, D, D));
+  STEP(linear(aor, a->wo, a->wo_q, a->wo_e, a->wo_c, a->wo_s, a->wo_z, xm, xr, Tm, D, D));
   // ---- MLP:  y = xm + down(silu(gate(xn2)) * up(xn2)) ----
   STEP(nv_rmsnorm_fwd(xm, D, a->ln2, xn2, D, rstd2, Tm, D, a->eps, stream));
-  STEP(linear(xn2, a->wgu, a->wgu_q, a->wgu_e, gu, nullptr, Tm, 2 * F, D));
+  STEP(linear(xn2, a->wgu, a->wgu_q, a->wgu_e, a->wgu_c, a->wgu_s, a->wgu_z, gu, nullptr, Tm, 2 * F, D));
   STEP(nv_swiglu_fwd(gu, 2 * (int64_t)F, h, F, Tm, F, stream));
-  STEP(linear(h, a->wd, a->wd_q, a->wd_e, a->y, xm, Tm, D, F));
+  STEP(linear(h, a->wd, a->wd_q, a->wd_e, a->wd_c, a->wd_s, a->wd_z, a->y, xm, Tm, D, F));
 #undef STEP
   return NV_OK;
 }

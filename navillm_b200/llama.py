@@ -31,6 +31,15 @@ from . import ops
 # so it keeps its bf16 weight above 16 rows (_fp8_layer).  lm_head: 0.94x at 17, 0.99x at 32, 1.06x at 64.
 FP8_MAX_ROWS = 64
 
+# Largest GEMM row count at which the fused q|k|v projection of an inference GEMM of 17 or more rows streams the int4 copy
+# of its weight (Int4Weights, nv_gemm_int4w_bf16) instead of the bf16 weights; at most 16 rows the decode step's skinny
+# int4 kernels read all four.  Measured (tools/midm_bench.py --int4, H100 80GB HBM3 at 700 W, int4 at its best tile width
+# vs bf16 on W', auto tiles): q|k|v 1.15x / 1.21x / 1.20x / 1.15x / 1.11x at M = 17 / 24 / 32 / 48 / 64 and 1.00x at 96 and
+# 128.  The other three stay bf16 above 16 rows (_int4_layer): o_proj 0.79-0.98x and down_proj 0.71-0.91x at every M,
+# gate|up 0.93-1.02x (1.02x at 17, 1.00x at 24-48, 0.98x at 64).  The expansion of the 4-bit tile, not HBM, limits the
+# kernel: it reaches 0.2-0.65 TB/s on its bytes.
+INT4_MAX_ROWS = 64
+
 bf16 = torch.bfloat16
 
 
@@ -502,7 +511,8 @@ class LlamaCore:
         self.cos, self.sin = rope_tables(dims, flat.flat.device)
         self.fp8 = None
         self.fp8_src = None
-        self.int4 = None              # per-layer int4 weight triples of the decode step (set_int4)
+        self.int4 = None              # per-layer int4 weight triples (set_int4)
+        self.int4_src = None
         self.act_fp8 = False          # W8A8 in the no-grad forwards (ModifiedLlamaForCausalLM.set_activation_dtype)
         self.wgrad_stash: Optional[WgradStash] = None   # deferred linear weight gradients (defer_weight_grads)
 
@@ -524,9 +534,12 @@ class LlamaCore:
         self.fp8 = w
 
     def set_int4(self, int4: Optional[Int4Weights]) -> None:
-        """Stream ``int4``'s copy of the decoder-layer linear weights in the decode-step GEMMs of at most 16 rows (None: the
-        bf16 weights).  Nothing else reads it: lm_head, prefills, no-grad forwards and training run bf16 on W'."""
+        """Stream ``int4``'s copy of the decoder-layer linear weights in the inference GEMMs (None: the bf16 weights): the
+        decode step's GEMMs of at most 16 rows, and the q|k|v projections of 17..``INT4_MAX_ROWS`` rows in the decode step
+        and, while the copy is fresh (``int4_for_inference``), in the no-grad forwards.  lm_head and training run bf16 on
+        W'."""
         self.int4 = None
+        self.int4_src = int4
         if int4 is None:
             return
         D, F = self.d.hidden, self.d.inter
@@ -547,6 +560,19 @@ class LlamaCore:
             return None
         return self.fp8
 
+    def int4_for_inference(self):
+        """The per-layer int4 weight triples when the copy still describes the current weights, else None: as
+        ``fp8_for_inference``, the no-grad forwards then run bf16 on the current weights."""
+        if self.int4 is None or self.int4_src.stale_reason(self.flat) is not None:
+            return None
+        return self.int4
+
+    @staticmethod
+    def _int4_layer(q4, l):
+        """(qkv, o, gate|up, down) int4 triples of layer l for the GEMMs of 17..INT4_MAX_ROWS rows: only q|k|v streams the
+        copy (see INT4_MAX_ROWS)."""
+        return None if q4 is None else (q4.wqkv[l], None, None, None)
+
     def act_fp8_weights(self):
         """The per-layer fp8 weight pairs of the W8A8 GEMMs when ``act_fp8`` is on, None when it is off.  Raises rather than
         run bf16: one evaluation must not mix two numerics."""
@@ -566,13 +592,15 @@ class LlamaCore:
         return self.fp8
 
     @staticmethod
-    def _linear(a, w, wq, addend=None, w8a8=False):
+    def _linear(a, w, wq, addend=None, w8a8=False, w4=None):
         """a · w^T (+ addend): W8A8 on the fp8 pair ``wq`` when ``w8a8``; else from ``wq`` when it is given and a has at most
-        FP8_MAX_ROWS rows."""
+        FP8_MAX_ROWS rows; else from the int4 triple ``w4`` when it is given and a has 17..INT4_MAX_ROWS rows."""
         if w8a8:
             return ops.gemm_w8a8(*ops.quantize_act_fp8(a), *wq, addend=addend)
         if wq[0] is not None and a.shape[0] <= FP8_MAX_ROWS:
             return ops.gemm_fp8w(a, *wq, addend=addend)
+        if w4 is not None and 16 < a.shape[0] <= INT4_MAX_ROWS:
+            return ops.gemm_int4w(a, *w4, addend=addend)
         return ops.gemm(a, w, addend=addend)
 
     def _fp8_layer(self, f8, l):
@@ -622,6 +650,7 @@ class LlamaCore:
         bufs = [torch.empty_like(x), torch.empty_like(x)]
         last = d.n_layers - 1
         f8 = self.fp8_for_inference()
+        q4 = self.int4_for_inference()
         for l, lyr in enumerate(self.model.layers):
             pruned = out_rows is not None and l == last
             y = torch.empty((R, d.hidden), dtype=bf16, device=x.device) if pruned else bufs[l & 1]
@@ -633,7 +662,7 @@ class LlamaCore:
             run.run(x, y, lyr.input_layernorm.weight.data, self.wqkv[l], self.wo[l], lyr.post_attention_layernorm.weight.data,
                     self.wgu[l], self.wd[l], kc=k, vc=v, ke=ke, ve=ve, out_rows=out_rows if pruned else None,
                     fp8=self._w8a8_layer(a8, l) if a8 is not None else self._fp8_layer(f8, l), fp8_max_rows=FP8_MAX_ROWS,
-                    act_fp8=a8 is not None)
+                    act_fp8=a8 is not None, int4=self._int4_layer(q4, l), int4_max_rows=INT4_MAX_ROWS)
             x = y
         return x
 
@@ -644,17 +673,19 @@ class LlamaCore:
         d = self.d
         saved: List[_Saved] = []
         last = d.n_layers - 1
-        f8 = None if save else self.fp8_for_inference()     # training forwards never read the fp8 copy
+        f8 = None if save else self.fp8_for_inference()     # training forwards never read the fp8 or int4 copy
+        q4 = None if save else self.int4_for_inference()
         q8 = a8 is not None
         for l, lyr in enumerate(self.model.layers):
             w8 = self._w8a8_layer(a8, l) if q8 else (self._fp8_layer(f8, l) or ((None, None),) * 4)
+            w4 = self._int4_layer(q4, l) or (None,) * 4
             s = _Saved()
             s.x = x
             s.xn, s.rstd1 = ops.rmsnorm_fwd(x, lyr.input_layernorm.weight.data, d.rms_eps)
             if fused:
                 s.qkv = ops.gemm_rope(s.xn, self.wqkv[l], pos, self.cos, self.sin, 2 * d.hidden)   # RoPE in the epilogue
             else:
-                s.qkv = self._linear(s.xn, self.wqkv[l], w8[0], w8a8=q8)
+                s.qkv = self._linear(s.xn, self.wqkv[l], w8[0], w8a8=q8, w4=w4[0])
                 ops.rope_(s.qkv, pos, self.cos, self.sin, 2 * d.n_heads, d.head_dim)
             s.ao = attend(l, s.qkv, s)
             s.rows = None
@@ -663,14 +694,14 @@ class LlamaCore:
                 s.rows = out_rows
                 ao = s.ao_r = ops.gather_rows(s.ao, out_rows)
                 xin = ops.gather_rows(x, out_rows)
-            s.xm = self._linear(ao, self.wo[l], w8[1], addend=xin, w8a8=q8)
+            s.xm = self._linear(ao, self.wo[l], w8[1], addend=xin, w8a8=q8, w4=w4[1])
             s.xn2, s.rstd2 = ops.rmsnorm_fwd(s.xm, lyr.post_attention_layernorm.weight.data, d.rms_eps)
             if fused and s.rows is None:
                 s.gu, s.h = ops.gemm_swiglu(s.xn2, self.wgu[l], keep_gu=save)                      # SwiGLU in the epilogue
             else:
-                s.gu = self._linear(s.xn2, self.wgu[l], w8[2], w8a8=q8)
+                s.gu = self._linear(s.xn2, self.wgu[l], w8[2], w8a8=q8, w4=w4[2])
                 s.h = ops.swiglu_fwd(s.gu)
-            x = self._linear(s.h, self.wd[l], w8[3], addend=s.xm, w8a8=q8)
+            x = self._linear(s.h, self.wd[l], w8[3], addend=s.xm, w8a8=q8, w4=w4[3])
             if save:
                 saved.append(s)
         return x, saved
@@ -853,15 +884,18 @@ class LlamaCore:
         # (gemm_skinny.cu); larger batches go through nv_gemm_bf16's auto dispatch, which picks the tile variant per (M, N)
         # from a measured table (32-column tiles for the 4096-wide projections, 256 for gate|up: tools/midm_bench.py).
         # With an fp8 copy of the weights (set_fp8), the skinny GEMMs and, up to FP8_MAX_ROWS rows, nv_gemm_fp8w_bf16 stream
-        # it instead: same bits as bf16 on W'.  With an int4 copy (set_int4), the skinny GEMMs stream it; above 16 rows the
-        # bf16 kernels run on W', again the same bits.  generate() refuses a stale copy before it gets here.
+        # it instead: same bits as bf16 on W'.  With an int4 copy (set_int4), the skinny GEMMs stream it, and up to
+        # INT4_MAX_ROWS rows nv_gemm_int4w_bf16 does for q|k|v; again the same bits.  generate() refuses a stale copy before it gets here.
         skinny = x.shape[0] <= 16
         fuse_mlp = skinny and d.inter % 64 == 0
         f8 = self.fp8 if x.shape[0] <= FP8_MAX_ROWS else None
-        q4 = self.int4 if skinny else None
-        if q4 is not None:
+        q4 = self.int4 if x.shape[0] <= INT4_MAX_ROWS else None
+        if q4 is not None and skinny:
             lin = lambda a, w, addend=None: ops.gemm_skinny_int4(a, *w, addend=addend)
             wqkv, wo, wgu, wd = q4.wqkv, q4.wo, q4.wgu, q4.wd
+        elif q4 is not None:                                  # q|k|v from the int4 copy, the others bf16 (INT4_MAX_ROWS)
+            lin = lambda a, w, addend=None: ops.gemm(a, w, addend=addend) if torch.is_tensor(w) else ops.gemm_int4w(a, *w, addend=addend)
+            wqkv, wo, wgu, wd = q4.wqkv, self.wo, self.wgu, self.wd
         elif f8 is not None:
             if skinny:
                 lin = lambda a, w, addend=None: ops.gemm_skinny_fp8(a, *w, addend=addend)
@@ -891,7 +925,7 @@ class LlamaCore:
                 ao = ops.decode_attn_rope(qkv, lens, self.cos, self.sin, kc[l], vc[l], H)   # RoPE + cache append + attention
             xm = lin(ao, wo[l], x)
             xn2, _ = ops.rmsnorm_fwd(xm, lyr.post_attention_layernorm.weight.data, d.rms_eps)
-            if q4 is not None:                                                           # Int4Weights: F % 64 == 0
+            if q4 is not None and skinny:                                                # Int4Weights: F % 64 == 0
                 h = ops.gemm_skinny_swiglu_int4(xn2, *wgu[l])
             elif fuse_mlp and f8 is not None:
                 h = ops.gemm_skinny_swiglu_fp8(xn2, *wgu[l])

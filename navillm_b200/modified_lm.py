@@ -774,11 +774,12 @@ class ModifiedLlamaForCausalLM(nn.Module):
         include/navillm_b200.h), and keep a 4-bit copy of them (about 3.4 GB at Vicuna-7B).  The model afterwards IS the
         model with weights W': prefill, navigation, training and ``state_dict()`` all see W'.  The decode-step GEMMs of
         ``generate`` with at most 16 rows (q|k|v, o_proj, gate|up with SwiGLU, down_proj) then stream the copy, a quarter of
-        the bf16 bytes, with the same bits as the bf16 kernels on W'; above 16 rows the step runs those bf16 kernels on W'.
-        lm_head is neither rounded nor streamed in 4 bits, and prefills, no-grad forwards and training keep the bf16
-        kernels.  Needs hidden and intermediate sizes that are multiples of 128.  Irreversible: reload the checkpoint to
-        get W back.  Any later write to the weights makes ``generate`` raise until this is called again (or
-        ``drop_int4_weights``).
+        the bf16 bytes, with the same bits as the bf16 kernels on W'; so do the q|k|v projections of 17..``llama.INT4_MAX_ROWS``
+        rows, in the decode step (larger batches, beams, several samples per prompt) and in the no-grad forwards while the
+        copy is fresh.  The other GEMMs above 16 rows run the bf16 kernels on W'.  lm_head is neither rounded nor streamed in
+        4 bits, and training keeps the bf16 kernels.  Needs hidden and intermediate sizes that are multiples of 128.
+        Irreversible: reload the checkpoint to get W back.  Any later write to the weights makes ``generate`` raise until
+        this is called again (or ``drop_int4_weights``); the no-grad forwards then run bf16 on the current weights.
 
         The fp8 and int4 copies exclude each other: this drops the fp8 copy (``quantize_weights_fp8``), and quantizing to
         fp8 drops this one.  The roundings compose: after ``quantize_weights_fp8()`` the weights are the fp8 W', and this

@@ -950,9 +950,12 @@ class LayerRunner:
         self._keep += (cached, kv_start, kv_len)
 
     def run(self, x, y, ln1, wqkv, wo, ln2, wgu, wd, *, kc=None, vc=None, out_rows=None, fp8=None, fp8_max_rows=0, ke=None, ve=None,
-            act_fp8=False):
+            act_fp8=False, int4=None, int4_max_rows=0):
         """``fp8``: None, or the (e4m3, exponents) pairs of wqkv, wo, wgu, wd (``Fp8Weights.view``); each GEMM with at most
         ``fp8_max_rows`` rows then streams its pair through nv_gemm_fp8w_bf16 (same bits as the bf16 weights W').
+        ``int4``: None, or the (codes, scales, zeros) triples of wqkv, wo, wgu, wd (``Int4Weights.view``; a triple may be
+        None); each GEMM with 17..``int4_max_rows`` rows then streams its triple through nv_gemm_int4w_bf16 (same bits as
+        W').  Exclusive with ``fp8``.
         ``act_fp8``: every GEMM runs W8A8 on the four pairs of ``fp8`` (all required) at every row count.
         ``ke`` / ``ve``: the row exponents of an fp8 cache (cache modes 3 and 4, kc / vc then hold its e4m3 bytes)."""
         a = self.args
@@ -961,6 +964,11 @@ class LayerRunner:
             [(q.data_ptr(), e.data_ptr()) if q is not None else (None, None) for q, e in pairs]
         a.fp8_max_rows = fp8_max_rows if fp8 is not None else 0
         a.act_fp8 = 1 if act_fp8 else 0
+        triples = int4 if int4 is not None else (None,) * 4
+        for name, tr in zip(("wqkv", "wo", "wgu", "wd"), triples):
+            c, sc, z = (t.data_ptr() for t in tr) if tr is not None else (None, None, None)
+            setattr(a, name + "_c", c); setattr(a, name + "_s", sc); setattr(a, name + "_z", z)
+        a.int4_max_rows = int4_max_rows if int4 is not None else 0
         a.x, a.y = x.data_ptr(), y.data_ptr()
         a.ln1, a.wqkv, a.wo, a.ln2, a.wgu, a.wd = ln1.data_ptr(), wqkv.data_ptr(), wo.data_ptr(), ln2.data_ptr(), wgu.data_ptr(), wd.data_ptr()
         a.kcache = kc.data_ptr() if kc is not None else None
@@ -1229,6 +1237,42 @@ def gemm_fp8w(a: torch.Tensor, q: torch.Tensor, e: torch.Tensor, *, addend: torc
     check(_lib.load().nv_gemm_fp8w_bf16(ptr(a), i64(a.stride(0)), ptr(q), i64(q.stride(0)), ptr(e), ptr(out), i64(out.stride(0)),
                                         ptr(addend), i64(addend.stride(0) if addend is not None else 0), i32(M), i32(N), i32(K),
                                         i32(block_n), stream_ptr()), "nv_gemm_fp8w_bf16")
+    return out
+
+
+def gemm_int4w(a: torch.Tensor, codes: torch.Tensor, scales: torch.Tensor, zeros: torch.Tensor, *,
+               addend: torch.Tensor | None = None, out: torch.Tensor | None = None, block_n: int = 0) -> torch.Tensor:
+    """``gemm(a, W', addend=addend, block_n=block_n)`` with the weight in the 4-bit format of ``quantize_int4_`` (codes,
+    scales [N, K / 128], zeros [N, K / 128]): bit for bit the same result at any M while reading about a quarter of the
+    weight bytes (csrc/gemm_bf16.cu).  N % 64 == 0.  block_n: 0 (auto), 32 or 128."""
+    if scales.dim() != 2:
+        raise ValueError(f"gemm_int4w: scales [N, K / 128] expected (got {tuple(scales.shape)})")
+    N, G = scales.shape
+    K = G * INT4_GROUP
+    if N % 64:
+        raise ValueError(f"gemm_int4w: N must be a multiple of 64 (got {N})")
+    _int4_weight(codes, scales, zeros, N, K, "gemm_int4w")
+    _rowmajor(a, "a")
+    if a.dtype != bf16 or a.dim() != 2 or a.shape[1] != K or a.shape[0] < 1:
+        raise ValueError(f"gemm_int4w: a bf16 [M, {K}] expected (got {a.dtype} {tuple(a.shape)})")
+    if a.stride(0) % 8 or a.data_ptr() % 16:
+        raise ValueError("gemm_int4w: a must be 16-byte aligned with a row stride that is a multiple of 8")
+    if block_n not in (0, 32, 128):
+        raise ValueError(f"gemm_int4w: block_n must be 0, 32 or 128 (got {block_n})")
+    M = a.shape[0]
+    if out is None:
+        out = torch.empty((M, N), dtype=bf16, device=a.device)
+    _rowmajor(out, "out")
+    if out.shape != (M, N) or out.dtype != bf16 or out.data_ptr() % 16:
+        raise ValueError(f"gemm_int4w: 16-byte aligned out bf16 [{M}, {N}] expected (got {out.dtype} {tuple(out.shape)})")
+    if addend is not None:
+        _rowmajor(addend, "addend")
+        if addend.shape != (M, N) or addend.dtype != bf16 or addend.data_ptr() % 16:
+            raise ValueError(f"gemm_int4w: 16-byte aligned addend bf16 [{M}, {N}] expected "
+                             f"(got {addend.dtype} {tuple(addend.shape)})")
+    check(_lib.load().nv_gemm_int4w_bf16(ptr(a), i64(a.stride(0)), ptr(codes), ptr(scales), ptr(zeros), ptr(out),
+                                         i64(out.stride(0)), ptr(addend), i64(addend.stride(0) if addend is not None else 0),
+                                         i32(M), i32(N), i32(K), i32(block_n), stream_ptr()), "nv_gemm_int4w_bf16")
     return out
 
 

@@ -18,7 +18,8 @@ rotated over copies larger than L2, bytes moved and GB/s); (ii) C3-shaped decode
 {bf16 KV, fp8 KV}, alternated, medians over the generations after each capture; (iii) for information, the token agreement
 between the two KV formats (not required to be 100 %: fp8 KV attends over rounded keys and values).
 
-    python tools/fp8_decode_bench.py --int4 [--batch 1 8 16] [--layers 32] [--gens 3] [--rounds 2] [--out FILE.json]
+    python tools/fp8_decode_bench.py --int4 [--batch 1 8 16] [--beams K | --samples N] [--layers 32] [--gens 3] [--rounds 2]
+                                     [--out FILE.json]
 
 adds the 4-bit group-wise weight copy (quantize_weights_int4): (i) per-GEMM time of the bf16, fp8 and int4 skinny kernels,
 alternated, at M = 1, 8, 16 and the four decoder shapes, weights rotated, bytes moved and GB/s on each format's bytes
@@ -334,9 +335,10 @@ def c3_model(dev, layers):
     return model, model.lang_model.flat.flat.clone()
 
 
-def c3_generate_int4(dev, model, W, layers, gens, batch, rounds):
+def c3_generate_int4(dev, model, W, layers, gens, batch, rounds, beams=1, samples=1):
     """C3-shaped decode ms/token for bf16 on the int4 W', the fp8 copy and the int4 copy, alternated: every visit restores
-    the weights W, quantizes for its arm, captures once and times ``gens`` generations."""
+    the weights W, quantizes for its arm, captures once and times ``gens`` generations.  ``beams`` > 1: beam search with
+    that many beams per prompt; ``samples`` > 1: that many sampled sequences per prompt (top-p 0.9, one seed per call)."""
     wl = bench.WORKLOADS["c3"]
     B, NV, NT, NEW = batch, wl["n_cand_tok"], wl["n_text"], wl["n_new"]
     lm = model.lang_model
@@ -356,12 +358,15 @@ def c3_generate_int4(dev, model, W, layers, gens, batch, rounds):
         pano = model.img_embeddings.forward_panorama_per_step(view_img_fts=view, view_lens=torch.full((B,), NV, device=dev))
         cand = model._masked_rows_plus_const(pano["pano_embeds"].reshape(B * NV, -1), np.ones((B, NV), dtype=bool)).detach()
 
+    mode = dict(num_beams=beams) if beams > 1 else dict(do_sample=True, top_p=0.9, num_return_sequences=samples) if samples > 1 else {}
+
     def run(n):
         per_tok, out = [], None
         for i in range(n + 1):                                                # the first one captures the CUDA graph
             st = {}
+            torch.manual_seed(0)
             out = lm.generate(input_ids=text["input_ids"], attention_mask=text["attention_mask"], cand_vis=cand,
-                              max_new_tokens=NEW, stop_on_eos=False, use_cuda_graph=True, stats=st)
+                              max_new_tokens=NEW, stop_on_eos=False, use_cuda_graph=True, stats=st, **mode)
             if i > 0:
                 per_tok.append(st["decode_ms"] / st["decode_steps"])
         return per_tok, out[:, text["input_ids"].shape[1]:].cpu()
@@ -387,7 +392,8 @@ def c3_generate_int4(dev, model, W, layers, gens, batch, rounds):
     lm.drop_int4_weights()
     med = {a: float(np.median(v)) for a, v in times.items()}
     agree = lambda a, b: float((a == b).float().mean())
-    return {"B": B, "S0": S0, "new_tokens": NEW, "layers": layers, "generations_per_arm": len(times["int4"]),
+    return {"B": B, "beams": beams, "samples": samples, "decode_rows": B * beams * samples, "S0": S0, "new_tokens": NEW,
+            "layers": layers, "generations_per_arm": len(times["int4"]),
             "int4_copy_GB": round(nbytes["int4"] / 1e9, 3), "fp8_copy_GB": round(nbytes["fp8"] / 1e9, 3),
             "decode_ms_per_token_bf16_Wq4": round(med["bf16_Wq4"], 4), "decode_ms_per_token_fp8": round(med["fp8"], 4),
             "decode_ms_per_token_int4": round(med["int4"], 4),
@@ -409,6 +415,8 @@ def main():
     ap.add_argument("--int4", action="store_true", help="add the int4 weight copy: bf16 / fp8 / int4 GEMMs, then generate() "
                                                          "for bf16 on the int4 W', fp8 and int4, alternated")
     ap.add_argument("--rounds", type=int, default=2, help="--int4: visits of each arm per batch size")
+    ap.add_argument("--beams", type=int, default=1, help="--int4: beam search with this many beams per prompt")
+    ap.add_argument("--samples", type=int, default=1, help="--int4: this many sampled sequences per prompt")
     ap.add_argument("--out", default=None, help="also write the result as JSON here")
     a = ap.parse_args()
     if not torch.cuda.is_available():
@@ -421,7 +429,7 @@ def main():
         res["c3_generate_int4"] = []
         model, W = c3_model(dev, a.layers)
         for b in a.batch or [1, 8, 16]:
-            res["c3_generate_int4"].append(c3_generate_int4(dev, model, W, a.layers, a.gens, b, a.rounds))
+            res["c3_generate_int4"].append(c3_generate_int4(dev, model, W, a.layers, a.gens, b, a.rounds, a.beams, a.samples))
             print(json.dumps(res["c3_generate_int4"][-1]), flush=True)
             gc.collect()
             torch.cuda.empty_cache()
