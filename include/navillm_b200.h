@@ -88,6 +88,18 @@ int nv_gemm_skinny_swiglu_fp8(const void* X, int64_t ldx, const void* Wgu_q, int
  * nv_gemm_skinny_bf16 / nv_gemm_skinny_swiglu_bf16 with the weight given as (codes, scales, zeros): they stream a quarter
  * of the bytes and return bit for bit what the bf16 kernels return on W'.  M <= 16, K % 128 == 0. */
 int nv_quantize_int4_groups(void* W, int64_t ldw, void* codes, void* scales, void* zeros, int N, int K, void* stream);
+/* GPTQ-calibrated form of the same format (Frantar et al., 2022; no act-order, no static groups).  With U the upper
+ * Cholesky factor of H^-1 (H = X^T X of the linear's inputs, dampened) the columns are quantized in order and each one's
+ * scaled error e_j = (w_j - W'_j) / U_jj is subtracted as e_j U[j, c] from every later column c.  nv_gptq_int4_block runs
+ * block g = the 128-column group g: it reads columns 128 g .. 128 g + 127 of the fp32 working copy Wf [N, K] (row stride
+ * ldwf) and U_gg, the 128 x 128 diagonal block of U (row stride ldu), applies the rule above to each row's values as they
+ * stand (lo, hi, s and z when the block starts, q when the column is reached), and writes the group's codes (same layout),
+ * scales and zeros, W' over the group's columns of the bf16 W (row stride ldw) and -E [N, 128] (row stride lde).  The
+ * caller then adds -E U[block rows, later columns] to the later columns of Wf (nv_sgemm with accumulate).  Wf is only
+ * read.  N % 64 == 0, K % 128 == 0, 0 <= g < K / 128, codes 16-byte aligned; bad arguments return an error before any
+ * launch. */
+int nv_gptq_int4_block(const void* Wf, int64_t ldwf, const void* U, int64_t ldu, int g, void* W, int64_t ldw, void* codes,
+                       void* scales, void* zeros, void* negE, int64_t lde, int N, int K, void* stream);
 int nv_gemm_skinny_int4(const void* X, int64_t ldx, const void* codes, const void* scales, const void* zeros, void* C,
                         int64_t ldc, const void* addend, int64_t ld_add, int M, int N, int K, void* stream);
 int nv_gemm_skinny_swiglu_int4(const void* X, int64_t ldx, const void* codes, const void* scales, const void* zeros, void* H,

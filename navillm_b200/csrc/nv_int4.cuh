@@ -7,6 +7,9 @@
 // (q - z) * s is exact in fp32, so W' is rounded once; |q - z| >= 1 and s >= 2^-126 keep every nonzero W' normal.  The
 // library is built with --use_fast_math (subnormals flushed), so the fp32 steps below are inline PTX without .ftz: a
 // group holding bf16 subnormals gets the bits of the rule.
+// GPTQ (nv_gptq_int4_block) applies the same rule to the fp32 error-updated weights of the group instead of the bf16 ones:
+// lo, hi, s and z come from the row's 128 values as they stand when the group's block starts, and each q from the value
+// as it stands when its column is reached.
 //
 // Packed codes (private to csrc/quant.cu and csrc/gemm_skinny.cu): W [N, K] is cut into chunks of 64 rows x 64 columns;
 // chunk (rb, kb) = rows 64 rb.., columns 64 kb.. is 2048 bytes at byte offset (rb * K / 64 + kb) * 2048, so the codes of
@@ -30,6 +33,7 @@ __device__ __forceinline__ float q4_max(float a, float b) { float r; asm("max.f3
 __device__ __forceinline__ float q4_sub(float a, float b) { float r; asm("sub.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b)); return r; }
 __device__ __forceinline__ float q4_div(float a, float b) { float r; asm("div.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b)); return r; }
 __device__ __forceinline__ float q4_mul(float a, float b) { float r; asm("mul.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b)); return r; }
+__device__ __forceinline__ float q4_fma(float a, float b, float c) { float r; asm("fma.rn.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c)); return r; }
 __device__ __forceinline__ int q4_rint(float a) { int r; asm("cvt.rni.s32.f32 %0, %1;" : "=r"(r) : "f"(a)); return r; }
 __device__ __forceinline__ uint16_t q4_bf16_bits(float a) { uint16_t r; asm("cvt.rn.bf16.f32 %0, %1;" : "=h"(r) : "f"(a)); return r; }
 __device__ __forceinline__ float q4_bf16_float(uint32_t bits) { return __uint_as_float(bits << 16); }
@@ -41,6 +45,36 @@ __device__ __forceinline__ void q4_group_params(float lo, float hi, float& s, in
 }
 __device__ __forceinline__ int q4_code(float w, float s, int z) { return min(max(q4_rint(q4_div(w, s)) + z, 0), 15); }
 __device__ __forceinline__ uint16_t q4_value_bits(int q, int z, float s) { return q4_bf16_bits(q4_mul((float)(q - z), s)); }
+
+// ---- the one writer of the packed layout ----
+// Thread t (0..127) of the quantizer writes bytes 16 t .. 16 t + 15 of both 64-column chunks of one 64-row block and
+// 128-column group: chunks chunk0 (columns 0..63) and chunk0 + 1 (64..127) of codes.  code(r, c) is the 4-bit code of
+// row r (0..63) and column c (0..127) of the block; thread t reads rows 16 (t / 32) .. 16 (t / 32) + 15 only.
+template <class Code>
+__device__ __forceinline__ void q4_pack_group(int t, uint8_t* __restrict__ codes, int64_t chunk0, Code code) {
+  const int warp = t >> 5, lane = t & 31;
+  const int r0 = warp * 16 + (lane >> 2);
+#pragma unroll
+  for (int half = 0; half < 2; ++half) {
+    uint32_t words[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      uint32_t word = 0;
+#pragma unroll
+      for (int p = 0; p < 4; ++p) {
+        const int r = r0 + 8 * (p & 1);
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int c = 64 * half + 16 * j + 2 * (lane & 3) + 8 * (p >> 1) + e;
+          word |= (uint32_t)code(r, c) << (4 * (p + 4 * e));
+        }
+      }
+      words[j] = word;
+    }
+    const int64_t chunk = chunk0 + half;
+    *reinterpret_cast<uint4*>(codes + chunk * Q4_CHUNK_BYTES + 16 * t) = make_uint4(words[0], words[1], words[2], words[3]);
+  }
+}
 
 // ---- dequantization into a register-A fragment (skinny GEMM) ----
 // sx: the bf16 scale in both halves; zx: bf16(128 + z) in both halves.  0x4300 | q is bf16(128 + q), the subtraction is

@@ -225,7 +225,29 @@ class FlatParams:
         return self.flat_grad[o:o + numel].view(shape)
 
 
-class _WeightCopy:
+class _WeightStamp:
+    """Something derived from weights ``params`` of ``flat`` (a quantized copy, a calibration): ``stale_reason`` reports any
+    write to the weights since ``_stamp``: new storage, a torch in-place op on a parameter or on the buffer (version
+    counters), or a bump of ``FlatParams.generation`` by a raw-pointer writer."""
+
+    def _stamp(self) -> None:
+        self._versions = self._version_state()
+        self._generation = self.flat.generation
+
+    def _version_state(self):
+        return self.flat.flat._version, sum(p._version for p in self.params)
+
+    def stale_reason(self, flat: FlatParams) -> Optional[str]:
+        if flat is not self.flat or flat.params[0].data_ptr() != flat._ptr0:
+            return "the weights were moved to new storage"
+        if flat.generation != self._generation:
+            return "an optimizer step updated the weights"
+        if self._version_state() != self._versions:
+            return "the weights were modified in place (optimizer step, load_state_dict or another write)"
+        return None
+
+
+class _WeightCopy(_WeightStamp):
     """Quantized copy of linear weights of a ``FlatParams`` buffer (``Fp8Weights``, ``Int4Weights``).
 
     Building it rounds every listed weight IN PLACE to the W' the copy encodes (``_quantize``), so the bf16 buffer and the
@@ -254,8 +276,7 @@ class _WeightCopy:
         flat.generation += 1                     # the rounding below writes the weights through raw pointers
         for p in self.params:
             self._quantize(p.data, self.view([p], tuple(p.shape)))
-        self._versions = self._version_state()
-        self._generation = flat.generation
+        self._stamp()
 
     def _check(self, p: nn.Parameter) -> None:
         pass
@@ -277,18 +298,6 @@ class _WeightCopy:
             raise RuntimeError(f"{name}.view: members hold {end[0] - start[0]} elements, shape {tuple(shape)} needs "
                                f"{self._sizes(tuple(shape))[0]}")
         return self._views([t[o:e] for t, o, e in zip(self._storage, start, end)], shape)
-
-    def _version_state(self):
-        return self.flat.flat._version, sum(p._version for p in self.params)
-
-    def stale_reason(self, flat: FlatParams) -> Optional[str]:
-        if flat is not self.flat or flat.params[0].data_ptr() != flat._ptr0:
-            return "the weights were moved to new storage"
-        if flat.generation != self._generation:
-            return "an optimizer step updated the weights"
-        if self._version_state() != self._versions:
-            return "the weights were modified in place (optimizer step, load_state_dict or another write)"
-        return None
 
 
 class Fp8Weights(_WeightCopy):
@@ -327,8 +336,30 @@ class Int4Weights(_WeightCopy):
     (csrc/gemm_skinny.cu, at most 16 rows).  W' = bf16((q - z) * s) with one bf16 scale s and one 4-bit zero-point z per
     row and 128 columns (csrc/quant.cu, rule in include/navillm_b200.h); ``view`` gives (codes, scales [N, K / 128] bf16,
     zeros [N, K / 128] uint8) in the form ``ops.gemm_skinny_int4`` takes.  Every weight needs K % 128 == 0 and, so that the
-    packed codes of q|k|v and gate|up concatenate, N % 64 == 0."""
+    packed codes of q|k|v and gate|up concatenate, N % 64 == 0.
+
+    ``calibration`` (an ``Int4Calibration`` of these weights, closed and fresh): the codes come from GPTQ
+    (``ops.gptq_int4_``) instead of round to nearest, with the factor U of each (layer, input) computed once (``damp``) and
+    reused by the weights that share the input (q, k, v; gate, up).  The copy is the same kind of object either way."""
     _align = (16, 1, 1)
+
+    def __init__(self, flat: FlatParams, params: List[nn.Parameter], calibration: Optional["Int4Calibration"] = None,
+                 damp: float = 0.01):
+        self._cal, self._damp, self._u = calibration, damp, None
+        try:
+            super().__init__(flat, params)
+        finally:
+            self._cal = self._u = None           # keeps neither the Hessians nor a factor alive
+
+    def _quantize(self, w, v):
+        if self._cal is None:
+            ops.quantize_int4_(w, *v)
+            return
+        key = self._cal.input_of(w)
+        if self._u is None or self._u[0] != key:
+            self._u = None
+            self._u = (key, self._cal.factor(*key, damp=self._damp))
+        ops.gptq_int4_(w, self._u[1], *v, damp=None)
 
     def _check(self, p):
         if p.shape[0] % 64 or p.shape[1] % ops.INT4_GROUP:
@@ -350,9 +381,74 @@ class Int4Weights(_WeightCopy):
         n, k = shape
         return parts[0].view(n, k // 2), parts[1].view(n, k // ops.INT4_GROUP), parts[2].view(n, k // ops.INT4_GROUP)
 
-    @staticmethod
-    def _quantize(w, v):
-        ops.quantize_int4_(w, *v)
+
+class Int4Calibration(_WeightStamp):
+    """Second-order statistics of the decoder-layer linear inputs for GPTQ (``ModifiedLlamaForCausalLM.int4_calibration``):
+    per layer one fp32 H = X^T X per distinct input, ``INPUTS``: the q|k|v input (the first RMSNorm's output), the o_proj
+    input (the attention output; in a pruned last layer its gathered rows), the gate|up input (the second RMSNorm's
+    output) and the down_proj input (the SwiGLU output).  ``h[(layer, input)]`` and ``rows[(layer, input)]`` (rows added
+    so far) are keyed by layer index and input name.
+
+    While it is open (``LlamaCore.calibration``), every forward through ``LlamaCore.forward`` or ``forward_suffix`` adds
+    its rows: prompt forwards, prefix-cached suffixes, the prefill of ``generate()``, training forwards.  The decode steps
+    of ``generate()`` add nothing.  Packed rows are real tokens only, so padding never enters H.  Each product is the
+    wgmma bf16 GEMM in its weight-gradient form with fp32 output (bf16 products are exact in fp32, the sums are fp32),
+    added to H.  At Vicuna-7B widths H takes 32 x (3 x 4096^2 + 11008^2) x 4 B = 21.95 GB (``nbytes``)."""
+    INPUTS = ("qkv", "o_proj", "gate_up", "down_proj")
+
+    def __init__(self, core: "LlamaCore"):
+        d, dev = core.d, core.flat.flat.device
+        self.flat = core.flat
+        self.params, self._input = [], {}
+        for l, lyr in enumerate(core.model.layers):
+            a, m = lyr.self_attn, lyr.mlp
+            for i, ps in enumerate(((a.q_proj, a.k_proj, a.v_proj), (a.o_proj,), (m.gate_proj, m.up_proj), (m.down_proj,))):
+                for p in ps:
+                    self.params.append(p.weight)
+                    self._input[p.weight.data_ptr()] = (l, self.INPUTS[i])
+        width = dict(qkv=d.hidden, o_proj=d.hidden, gate_up=d.hidden, down_proj=d.inter)
+        self.h = {(l, n): torch.zeros((width[n], width[n]), dtype=torch.float32, device=dev)
+                  for l in range(d.n_layers) for n in self.INPUTS}
+        self.rows = {k: 0 for k in self.h}
+        self.open = True
+        self._stamp()
+
+    @property
+    def nbytes(self) -> int:
+        return sum(h.numel() * h.element_size() for h in self.h.values())
+
+    def record(self, layer: int, name: str, x: torch.Tensor) -> None:
+        """H[(layer, name)] += x^T x for the bf16 rows x [T, K]."""
+        if x.shape[0] == 0:
+            return
+        self.h[(layer, name)].add_(ops.gemm(x, x, a_mn=True, b_mn=True, out_f32=True))
+        self.rows[(layer, name)] += x.shape[0]
+
+    def check(self, flat: FlatParams, damp: float = 0.01) -> None:
+        """Raises unless the calibration can quantize the weights of ``flat`` as they are now, before any weight is written:
+        a failing factorisation (``ops.CholeskyError``) leaves the weights and the calibration usable with a larger damp."""
+        if self.open:
+            raise RuntimeError("int4 calibration: the calibration is still open; leave its `with model.int4_calibration()` "
+                               "block before quantize_weights_int4(calibration=...)")
+        empty = [k for k, n in self.rows.items() if n == 0]
+        if empty:
+            raise RuntimeError(f"int4 calibration: no rows were recorded for layer {empty[0][0]}'s {empty[0][1]} input "
+                               f"({len(empty)} of {len(self.rows)} inputs empty); run LM forwards (model(mode, batch)) "
+                               f"inside the calibration block")
+        why = self.stale_reason(flat)
+        if why is not None:
+            raise RuntimeError(f"int4 calibration: the calibration is stale ({why} after it was opened); open a new "
+                               f"calibration on the current weights")
+        for (l, name), h in self.h.items():
+            ops.gptq_factor(h, damp, what=f"layer {l}'s {name} input Hessian", check_only=True)
+
+    def input_of(self, w: torch.Tensor):
+        """(layer, input name) of a decoder-layer linear weight."""
+        return self._input[w.data_ptr()]
+
+    def factor(self, layer: int, name: str, damp: float = 0.01) -> torch.Tensor:
+        """``ops.gptq_factor`` of H[(layer, name)]."""
+        return ops.gptq_factor(self.h[(layer, name)], damp, what=f"layer {layer}'s {name} input Hessian")
 
 
 def allreduce_flat_grads(flats, average: bool = True) -> int:
@@ -515,6 +611,7 @@ class LlamaCore:
         self.int4_src = None
         self.act_fp8 = False          # W8A8 in the no-grad forwards (ModifiedLlamaForCausalLM.set_activation_dtype)
         self.wgrad_stash: Optional[WgradStash] = None   # deferred linear weight gradients (defer_weight_grads)
+        self.calibration: Optional[Int4Calibration] = None   # open GPTQ calibration: the forwards record their linear inputs
 
     def set_fp8(self, fp8: Optional[Fp8Weights]) -> None:
         """Stream ``fp8``'s copy of the linear weights in the inference GEMMs (None: the bf16 weights): the decode step, and
@@ -627,7 +724,8 @@ class LlamaCore:
     # -------------------------------------------------------------------------------------------------
     # Inference forwards that do not run the fused-epilogue GEMMs go through ONE C-ABI call per layer (csrc/layer.cu): they
     # are host-bound when every kernel is its own call from Python.  Tests turn this off to run the per-kernel path as the
-    # reference.
+    # reference.  An open calibration also takes the per-kernel path: the layer call keeps the linear inputs it records in
+    # its workspace.
     LAYER_CALL = True
 
     def _fused(self, T: int, a8) -> bool:
@@ -669,8 +767,10 @@ class LlamaCore:
     def _layers(self, x, pos, out_rows, save, a8, fused, attend):
         """The per-kernel forward of every layer.  ``attend(l, qkv, s)`` is the attention step, the one part the prompt and
         the suffix forwards do differently: it returns the attention output of layer l and sets ``s.lse`` when saving.
-        Returns the residual stream and the per-layer activations (empty unless ``save``)."""
+        Returns the residual stream and the per-layer activations (empty unless ``save``).  With an open ``calibration``,
+        each layer's four linear inputs are added to its Hessians."""
         d = self.d
+        cal = self.calibration
         saved: List[_Saved] = []
         last = d.n_layers - 1
         f8 = None if save else self.fp8_for_inference()     # training forwards never read the fp8 or int4 copy
@@ -701,6 +801,9 @@ class LlamaCore:
             else:
                 s.gu = self._linear(s.xn2, self.wgu[l], w8[2], w8a8=q8, w4=w4[2])
                 s.h = ops.swiglu_fwd(s.gu)
+            if cal is not None:
+                for name, inp in zip(cal.INPUTS, (s.xn, ao, s.xn2, s.h)):
+                    cal.record(l, name, inp)
             x = self._linear(s.h, self.wd[l], w8[3], addend=s.xm, w8a8=q8, w4=w4[3])
             if save:
                 saved.append(s)
@@ -725,7 +828,7 @@ class LlamaCore:
         fused = self._fused(T, a8)
         kc, vc = kv_store if kv_store is not None else (None, None)
         fp8_kv = kc is not None and is_fp8_kv(kc)
-        if self.LAYER_CALL and not save and not fused:
+        if self.LAYER_CALL and not save and not fused and self.calibration is None:
             mode = 0 if kc is None else 3 if fp8_kv else 1
             Smax = 0 if kc is None else (kc[0][0] if fp8_kv else kc[0]).shape[1]
             return self._layer_calls(x, pos, cu, seqlens, out_rows, a8, kc, vc, mode, Smax), None
@@ -770,7 +873,7 @@ class LlamaCore:
         fp8_kv = is_fp8_kv(kc)
         if save and (fp8_kv or acc is None or kv_lens is None):
             raise ValueError("forward_suffix(save=True) needs bf16 caches, the gradient accumulators and the host kv_lens")
-        if self.LAYER_CALL and not save and not fused:
+        if self.LAYER_CALL and not save and not fused and self.calibration is None:
             Bc, Smax = (kc[0][0] if fp8_kv else kc[0]).shape[:2]
             return self._layer_calls(x, pos, cu, q_lens, out_rows, a8, kc, vc, 4 if fp8_kv else 2, Smax, Bc * Smax, cached,
                                      kv_start, kv_len)

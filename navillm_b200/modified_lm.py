@@ -14,6 +14,7 @@ reference holds values computed from pad embeddings that nothing reads.
 """
 from __future__ import annotations
 
+import contextlib
 import dataclasses
 import time
 import weakref
@@ -27,7 +28,7 @@ import torch.nn as nn
 from . import generation
 from . import ops
 from . import trie as trie_mod
-from .llama import FlatParams, Fp8Weights, Int4Weights, LlamaCore, LlamaDims, LlamaModelParams, WgradStash, _Linear, kv_cache
+from .llama import FlatParams, Fp8Weights, Int4Calibration, Int4Weights, LlamaCore, LlamaDims, LlamaModelParams, WgradStash, _Linear, kv_cache
 from .parallel import GradSync
 from .tokenizer import HFTokenizerAdapter, SyntheticTokenizer
 
@@ -767,11 +768,45 @@ class ModifiedLlamaForCausalLM(nn.Module):
         """The weights ``quantize_weights_int4`` rounds: q/k/v/o and gate/up/down of every layer (lm_head stays bf16)."""
         return self.fp8_linear_weights()[:-1]
 
+    @contextlib.contextmanager
+    def int4_calibration(self):
+        """Record the Hessians GPTQ needs from the forwards run inside the block; yields an ``Int4Calibration``::
+
+            with model.int4_calibration() as cal:
+                with torch.no_grad():
+                    model('navigation', batch)          # any LM forward: prompts, prefix-cached suffixes, prefills
+            model.quantize_weights_int4(calibration=cal)
+            del cal                                     # frees the Hessians
+
+        Every forward through the decoder stack adds its rows (the decode steps of ``generate()`` do not); its outputs are
+        bit for bit those of the per-kernel path, which the forwards take while the block is open.  All Hessians come
+        from the unquantized model in one pass (no sequential re-recording through already-quantized layers).  The
+        Hessians take ``cal.nbytes`` of device memory (21.95 GB at Vicuna-7B widths).  One calibration at a time."""
+        self._ensure()
+        if self.core.calibration is not None:
+            raise RuntimeError("int4_calibration(): a calibration is already open on this model; leave its `with` block "
+                               "first")
+        cal = Int4Calibration(self.core)
+        core = self.core
+        core.calibration = cal
+        try:
+            yield cal
+        finally:
+            cal.open = False
+            if core.calibration is cal:
+                core.calibration = None
+
     @torch.no_grad()
-    def quantize_weights_int4(self) -> int:
+    def quantize_weights_int4(self, calibration: Optional[Int4Calibration] = None, damp: float = 0.01) -> int:
         """Round every decoder-layer linear weight IN PLACE to W' = bf16((q - z) * s): 4-bit codes q with one bf16 scale s
-        and one 4-bit zero-point z per row and 128 columns (round to nearest, no calibration; rule in
-        include/navillm_b200.h), and keep a 4-bit copy of them (about 3.4 GB at Vicuna-7B).  The model afterwards IS the
+        and one 4-bit zero-point z per row and 128 columns (round to nearest; rule in include/navillm_b200.h), and keep a
+        4-bit copy of them (about 3.4 GB at Vicuna-7B).
+
+        ``calibration`` (from ``int4_calibration()``, closed, taken on the current weights): the codes come from GPTQ
+        instead, which feeds each column's rounding error forward onto the columns not yet rounded so that the layer's
+        output error on the recorded inputs, not the weight error, is minimised.  ``damp`` adds damp * mean(diag H) to
+        H's diagonal before the factorisation; raise it if a factorisation fails.  The format, the copy and everything
+        below are the same either way.  The model afterwards IS the
         model with weights W': prefill, navigation, training and ``state_dict()`` all see W'.  The decode-step GEMMs of
         ``generate`` with at most 16 rows (q|k|v, o_proj, gate|up with SwiGLU, down_proj) then stream the copy, a quarter of
         the bf16 bytes, with the same bits as the bf16 kernels on W'; so do the q|k|v projections of 17..``llama.INT4_MAX_ROWS``
@@ -785,9 +820,11 @@ class ModifiedLlamaForCausalLM(nn.Module):
         fp8 drops this one.  The roundings compose: after ``quantize_weights_fp8()`` the weights are the fp8 W', and this
         rounds that W' to 4 bits (and the other way round).  Returns the size of the copy in bytes."""
         self._ensure()
+        if calibration is not None:
+            calibration.check(self.flat, damp)
         self.drop_fp8_weights()
         self.drop_int4_weights()
-        self._int4 = Int4Weights(self.flat, self.int4_linear_weights())
+        self._int4 = Int4Weights(self.flat, self.int4_linear_weights(), calibration=calibration, damp=damp)
         self.core.set_int4(self._int4)
         return self._int4.nbytes
 

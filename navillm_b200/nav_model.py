@@ -254,12 +254,18 @@ class NavModel(nn.Module):
     def drop_fp8_weights(self) -> None:
         self.lang_model.drop_fp8_weights()
 
-    def quantize_weights_int4(self) -> int:
+    def quantize_weights_int4(self, calibration=None, damp: float = 0.01) -> int:
         """Opt-in 4-bit group-wise weight streaming (W4A16) in the decode step: ``ModifiedLlamaForCausalLM.quantize_weights_int4``
-        on the language model, so the 3dqa, summarization and embodied_qa modes decode from the int4 copy.  Returns its size
-        in bytes."""
+        on the language model, so the 3dqa, summarization and embodied_qa modes decode from the int4 copy; GPTQ-calibrated
+        with a ``calibration`` from ``int4_calibration()``.  Returns its size in bytes."""
         self._ensure()
-        return self.lang_model.quantize_weights_int4()
+        return self.lang_model.quantize_weights_int4(calibration=calibration, damp=damp)
+
+    def int4_calibration(self):
+        """``ModifiedLlamaForCausalLM.int4_calibration`` of the language model: a ``with`` block inside which the LM forwards
+        of ``model(mode, batch)`` record the Hessians that ``quantize_weights_int4(calibration=...)`` uses."""
+        self._ensure()
+        return self.lang_model.int4_calibration()
 
     def drop_int4_weights(self) -> None:
         self.lang_model.drop_int4_weights()

@@ -1162,6 +1162,76 @@ def quantize_int4_(w: torch.Tensor, codes: torch.Tensor, scales: torch.Tensor, z
     return w
 
 
+class CholeskyError(RuntimeError):
+    pass
+
+
+def _gptq_cholesky(h: torch.Tensor, damp: float, what: str) -> torch.Tensor:
+    """fp64 lower Cholesky factor of the dampened H: a column no recorded row touched (H_ii = 0) gets H_ii = 1, then
+    H += damp * mean(diag H) * I."""
+    if h.dim() != 2 or h.shape[0] != h.shape[1] or h.dtype != f32_t or not h.is_cuda:
+        raise ValueError(f"gptq_factor: fp32 CUDA H [K, K] expected (got {h.dtype} {tuple(h.shape)} on {h.device})")
+    if not damp >= 0.0:
+        raise ValueError(f"gptq_factor: damp must be >= 0 (got {damp})")
+    H = h.double()
+    d = H.diagonal()
+    d[d == 0] = 1.0
+    d += damp * d.mean()
+    L, info = torch.linalg.cholesky_ex(H)
+    if int(info) != 0:
+        raise CholeskyError(f"GPTQ: the Cholesky factorisation of {what} failed (not positive definite at column "
+                            f"{int(info) - 1} with damp={damp}); quantize again with a larger damp")
+    return L
+
+
+def gptq_factor(h: torch.Tensor, damp: float = 0.01, what: str = "the Hessian", check_only: bool = False):
+    """U, the upper Cholesky factor of H^-1 (H^-1 = U^T U), fp32 [K, K] on h's device, for ``gptq_int4_``.  In fp64 with
+    torch.linalg (a one-off O(K^3) factorisation per linear input): a column no recorded row touched (H_ii = 0) gets
+    H_ii = 1, then H += damp * mean(diag H) * I.  Raises ``CholeskyError`` naming ``what`` when H is not positive definite.
+    ``check_only``: only the factorisation of H, which is where that shows; returns None."""
+    L = _gptq_cholesky(h, damp, what)
+    if check_only:
+        return None
+    U, info = torch.linalg.cholesky_ex(torch.cholesky_inverse(L), upper=True)
+    if int(info) != 0:
+        raise CholeskyError(f"GPTQ: the Cholesky factorisation of the inverse of {what} failed (column {int(info) - 1} with "
+                            f"damp={damp}); quantize again with a larger damp")
+    return U.float().contiguous()                # torch returns the upper factor column-major
+
+
+def gptq_int4_(w: torch.Tensor, h_or_u: torch.Tensor, codes: torch.Tensor, scales: torch.Tensor, zeros: torch.Tensor,
+               damp: float | None = 0.01) -> torch.Tensor:
+    """``quantize_int4_`` calibrated by GPTQ: the same format and outputs, with each column's rounding error fed forward onto
+    the columns not yet rounded so that ||X (W - W')^T|| is what gets minimised (include/navillm_b200.h).  ``h_or_u``: the
+    fp32 Hessian H = X^T X [K, K] of the linear's inputs, factored here by ``gptq_factor(h, damp)``, or with ``damp=None``
+    the factor U that ``gptq_factor`` returned.  Per 128-column group: one nv_gptq_int4_block launch, then the exact fp32
+    CUDA-core nv_sgemm adds -E U[group rows, later columns] to the later columns of an fp32 working copy of w.  w [N, K]
+    bf16 with N % 64 == 0 and K % 128 == 0 is overwritten with W'.  Returns w."""
+    _rowmajor(w, "w")
+    if w.dtype != bf16:
+        raise ValueError(f"gptq_int4_: bf16 w expected (got {w.dtype})")
+    N, K = w.shape
+    if N % 64:
+        raise ValueError(f"gptq_int4_: N must be a multiple of 64 (got {N})")
+    _int4_weight(codes, scales, zeros, N, K, "gptq_int4_")
+    if h_or_u.dtype != f32_t or tuple(h_or_u.shape) != (K, K) or not h_or_u.is_contiguous() or h_or_u.device != w.device:
+        raise ValueError(f"gptq_int4_: contiguous fp32 [{K}, {K}] H or U on {w.device} expected (got {h_or_u.dtype} "
+                         f"{tuple(h_or_u.shape)} on {h_or_u.device})")
+    u = h_or_u if damp is None else gptq_factor(h_or_u, damp)
+    wf = w.float()
+    ne = torch.empty((N, INT4_GROUP), dtype=f32_t, device=w.device)
+    lib, st, G = _lib.load(), stream_ptr(), K // INT4_GROUP
+    for g in range(G):
+        c0 = g * INT4_GROUP
+        check(lib.nv_gptq_int4_block(ptr(wf), i64(K), ptr(u[c0:, c0:]), i64(K), i32(g), ptr(w), i64(w.stride(0)), ptr(codes),
+                                     ptr(scales), ptr(zeros), ptr(ne), i64(INT4_GROUP), i32(N), i32(K), st), "nv_gptq_int4_block")
+        c1 = c0 + INT4_GROUP
+        if c1 < K:
+            check(lib.nv_sgemm(ptr(ne), i64(INT4_GROUP), i32(0), ptr(u[c0:, c1:]), i64(K), i32(1), ptr(wf[:, c1:]), i64(K),
+                               ptr(None), i32(N), i32(K - c1), i32(INT4_GROUP), i32(1), st), "nv_sgemm")
+    return w
+
+
 def _skinny_x(x: torch.Tensor, k: int, name: str) -> int:
     _rowmajor(x, "x")
     if x.dtype != bf16 or x.dim() != 2 or x.shape[1] != k or not 1 <= x.shape[0] <= 16:
