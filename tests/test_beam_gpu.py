@@ -69,15 +69,21 @@ def test_beam_topk_first_step_and_forced_ties(cuda_dev):
         assert cp[b].tolist() == [0] * 8 and ct[b].tolist() == list(range(100, 108))
         assert (cs[b] == cs[b, 0]).all()
     bs = torch.tensor([0.0, -1e9, -1e9, -1e9] * B, device=cuda_dev)
-    pre = torch.randn(B, V, device=cuda_dev).to(bf16)
+    g = torch.Generator(device=cuda_dev).manual_seed(3)
+    pre = torch.randn(B, V, generator=g, device=cuda_dev).to(bf16)
     big = torch.empty((B * K, V), dtype=bf16, device=cuda_dev)
     big[:B] = pre
     cs, ct, cp = _topk_run(big, bs, K, first_step=True)
+    # beam 0's scores as the kernel forms them (the restatement of test_beam_topk_matches_torch): near -11 a bf16 log-prob
+    # step is 2^-4, so logits one bf16 step apart often share a score, and the tie goes to the lower token index
     x = pre.float().cpu()
     x[:, SPECIAL] = float("-inf")
+    m = x.max(dim=1, keepdim=True).values
+    lp = ((x - m) - torch.log(torch.exp((x - m).double()).sum(dim=1, keepdim=True)).float()).to(bf16).float()
+    ws, wt = torch.sort(lp, dim=1, descending=True, stable=True)
     for b in range(B):
         assert (cp[b] == 0).all()
-        assert set(ct[b].tolist()) == set(torch.topk(x[b], 2 * K).indices.tolist())
+        assert torch.equal(ct[b], wt[b, :2 * K]) and torch.equal(cs[b], ws[b, :2 * K]), (b, ct[b], wt[b, :2 * K])
 
 
 # ---------------------------------------------------------------------------------------------------------------------

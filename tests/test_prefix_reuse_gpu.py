@@ -1,8 +1,7 @@
-"""Cross-step prompt-prefix KV reuse (SURVEY.md §8f n1): suffix attention kernel and the NavModel rollout API.
+"""Cross-step prompt-prefix KV reuse (SURVEY.md §8f n1): the NavModel rollout API.  The suffix attention kernel itself
+(nv_attn_fwd_kv) is checked against fp64 with per-element bounds in tests/test_prefix_attn_kernels_gpu.py.
 
 Tolerances, stated:
-  * nv_attn_fwd_kv vs an fp32 PyTorch reference of the same masked attention: bf16 output, fp32 softmax -> 2e-2
-    absolute on O(1) outputs (same bound as tests/test_attn_gpu.py).
   * fuse_logits with the cache vs the from-scratch forward of the same prompts: the math is identical except that a
     row keeps the rotary offset of its first step (rotary attention depends on position differences only), so only
     bf16 rounding differs (cos/sin table entries, accumulation order of the split softmax): 3e-2 of max|logit|.
@@ -14,54 +13,6 @@ import pytest
 import torch
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.mark.parametrize("case", [
-    dict(q=[128, 70, 1, 300], kv=[128, 75, 130, 300]),           # dk = 0, 5, 129, 0
-    dict(q=[40, 257, 200], kv=[1000, 600, 333]),                 # long cached prefixes, misaligned diagonals
-    dict(q=[5], kv=[5]),
-    dict(q=[256, 129], kv=[511, 129 + 384]),
-])
-def test_suffix_attention_matches_reference(cuda_dev, case):
-    from navillm_b200 import ops
-    H, HD, Smax = 2, 128, 1024
-    q_lens, kv_lens = case["q"], case["kv"]
-    B = len(q_lens)
-    g = torch.Generator().manual_seed(sum(q_lens) + sum(kv_lens))
-    Tq = sum(q_lens)
-    q = torch.randn(Tq, H * HD, generator=g).to(cuda_dev, torch.bfloat16)
-    kc = torch.zeros(B, Smax, H * HD, dtype=torch.bfloat16, device=cuda_dev)
-    vc = torch.zeros_like(kc)
-    for b in range(B):
-        kc[b, :kv_lens[b]] = torch.randn(kv_lens[b], H * HD, generator=g).to(cuda_dev, torch.bfloat16)
-        vc[b, :kv_lens[b]] = torch.randn(kv_lens[b], H * HD, generator=g).to(cuda_dev, torch.bfloat16)
-        # stale (finite) data past the sequence must not matter
-        kc[b, kv_lens[b]:kv_lens[b] + 7] = 3.0
-        vc[b, kv_lens[b]:kv_lens[b] + 7] = -5.0
-    cu = torch.tensor([0] + list(np.cumsum(q_lens)), dtype=torch.int32, device=cuda_dev)
-    kv_start = torch.arange(B, dtype=torch.int32, device=cuda_dev) * Smax
-    kv_len = torch.tensor(kv_lens, dtype=torch.int32, device=cuda_dev)
-    out = ops.attn_fwd_kv(q, kc, vc, cu, q_lens, kv_start, kv_len, H)
-    torch.cuda.synchronize()
-    scale = HD ** -0.5
-    t0 = 0
-    for b in range(B):
-        nq, nk = q_lens[b], kv_lens[b]
-        dk = nk - nq
-        qi = torch.arange(nq, device=cuda_dev)[:, None]
-        kj = torch.arange(nk, device=cuda_dev)[None, :]
-        mask = kj <= dk + qi
-        for h in range(H):
-            qq = q[t0:t0 + nq, h * HD:(h + 1) * HD].float()
-            kk = kc[b, :nk, h * HD:(h + 1) * HD].float()
-            vv = vc[b, :nk, h * HD:(h + 1) * HD].float()
-            s = (qq @ kk.t()) * scale
-            p = torch.softmax(s.masked_fill(~mask, float("-inf")), dim=-1)
-            ref = p @ vv
-            got = out[t0:t0 + nq, h * HD:(h + 1) * HD].float()
-            assert torch.isfinite(got).all()
-            assert (got - ref).abs().max().item() < 2e-2, (b, h, (got - ref).abs().max().item())
-        t0 += nq
 
 
 def _build(cuda_dev):

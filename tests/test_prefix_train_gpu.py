@@ -1,10 +1,10 @@
 """Training over a PrefixKVCache (PrefixKVCache(train=True)): the cache form of the attention backward
 (nv_attn_bwd_kv), the suffix-only training step and the deferred prefix backward (``flush_grads``).
 
+nv_attn_bwd_kv's values are checked against fp64 with per-element bounds in tests/test_prefix_attn_kernels_gpu.py; here
+its determinism, its fused inverse RoPE and the accumulator rows it must not touch are checked bit for bit.
+
 Tolerances, stated:
-  * nv_attn_bwd_kv vs autograd of the fp32 masked attention: the kernel rounds P and dS to bf16 before the products and the
-    gradients to bf16 (as nv_attn_bwd): 3e-2 of the gradient's max, the bound of tests/test_attn_gpu.py.  Accumulated rows:
-    the same bound on (acc_after - acc_before), and rows the kernel must not touch are compared bit for bit.
   * Rollout gradients with the cache vs the from-scratch CUDA path: the cached path computes the same sums, but a row keeps
     the rotary offset of its first step and part (b) runs on recomputed prefix activations, so only bf16 rounding
     differs; each parameter gradient must lie within 5e-2 of its max|grad| (the gradient floor of the boundary rule of
@@ -49,34 +49,10 @@ def _setup(cuda_dev, case):
     return H, q, kc, vc, do, acc0, cu, kv_start, kv_len
 
 
-def _reference(q, kc, vc, do, q_lens, kv_lens, H):
-    """fp32 autograd of the masked attention per sequence: (o, lse, dq, dk, dv) with dk / dv over the kv_len rows."""
-    scale = HD ** -0.5
-    out, t0 = [], 0
-    for b, (nq, nk) in enumerate(zip(q_lens, kv_lens)):
-        dkc = nk - nq
-        mask = torch.arange(nk, device=q.device)[None, :] <= dkc + torch.arange(nq, device=q.device)[:, None]
-        qq = q[t0:t0 + nq].float().view(nq, H, HD).transpose(0, 1).requires_grad_(True)
-        kk = kc[b, :nk].float().view(nk, H, HD).transpose(0, 1).requires_grad_(True)
-        vv = vc[b, :nk].float().view(nk, H, HD).transpose(0, 1).requires_grad_(True)
-        s = (qq @ kk.transpose(1, 2)) * scale
-        s = s.masked_fill(~mask, float("-inf"))
-        lse = torch.logsumexp(s, -1)
-        o = torch.softmax(s, -1) @ vv
-        o.backward(do[t0:t0 + nq].float().view(nq, H, HD).transpose(0, 1))
-        flat = lambda t: t.transpose(0, 1).reshape(t.shape[1], H * HD)
-        out.append((flat(o.detach()), lse.detach(), flat(qq.grad), flat(kk.grad), flat(vv.grad)))
-        t0 += nq
-    return out
-
-
-def _close(name, got, ref, frac=3e-2):
-    err = (got.float() - ref).abs().max().item()
-    assert err <= frac * ref.abs().max().item() + 1e-6, f"{name}: err {err} vs max {ref.abs().max().item()}"
-
-
 @pytest.mark.parametrize("case", CASES)
-def test_attn_bwd_kv_matches_autograd(cuda_dev, case):
+def test_attn_bwd_kv_is_deterministic_and_fuses_rope(cuda_dev, case):
+    """A second run from the same accumulator gives the same bits; the inverse RoPE of the epilogue is bit for bit the plain
+    output rotated back; the accumulator rows [dk, Smax) of every slot keep their bits."""
     from navillm_b200 import ops
     from navillm_b200.llama import LlamaDims, rope_tables
     H, q, kc, vc, do, acc0, cu, kv_start, kv_len = _setup(cuda_dev, case)
@@ -99,23 +75,9 @@ def test_attn_bwd_kv_matches_autograd(cuda_dev, case):
     plain = dqkv.clone()
     ops.rope_(plain, pos, cos_t, sin_t, 2 * H, backward=True)
     assert torch.equal(roped, plain) and torch.equal(acc3, acc)
-
-    ref = _reference(q, kc, vc, do, q_lens, kv_lens, H)
-    t0 = 0
+    # cached rows accumulate; every other row of the sequence's slot (suffix rows, rows past kv_len) is untouched
     for b, (nq, nk) in enumerate(zip(q_lens, kv_lens)):
-        o_r, lse_r, dq_r, dk_r, dv_r = ref[b]
-        c = nk - nq
-        assert torch.allclose(lse[:, t0:t0 + nq], lse_r, rtol=1e-3, atol=2e-3), (lse[:, t0:t0 + nq] - lse_r).abs().max().item()
-        _close(f"dq[{b}]", dqkv[t0:t0 + nq, :D], dq_r)
-        # suffix rows: dK + acc, dV + acc (acc read, not written)
-        _close(f"dk[{b}]", dqkv[t0:t0 + nq, D:2 * D], dk_r[c:] + acc0[b, c:nk, :D])
-        _close(f"dv[{b}]", dqkv[t0:t0 + nq, 2 * D:], dv_r[c:] + acc0[b, c:nk, D:])
-        # cached rows accumulate; every other row of the sequence's slot (suffix rows, rows past kv_len) is untouched
-        if c:
-            _close(f"acc dk[{b}]", acc[b, :c, :D] - acc0[b, :c, :D], dk_r[:c])
-            _close(f"acc dv[{b}]", acc[b, :c, D:] - acc0[b, :c, D:], dv_r[:c])
-        assert torch.equal(acc[b, c:], acc0[b, c:]), b
-        t0 += nq
+        assert torch.equal(acc[b, nk - nq:], acc0[b, nk - nq:]), b
 
 
 def test_attn_bwd_kv_rejects_bad_accumulator(cuda_dev):

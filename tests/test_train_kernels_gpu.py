@@ -10,9 +10,14 @@ tensor cores' fp32 accumulation is not IEEE round-to-nearest; it is budgeted at 
 wgmma k-step of 16.  The library is built with --use_fast_math: exp2f is ex2.approx (2 ulp), __expf has at most
 2 + floor(1.173·|x|) ulp, __logf at most 2^-21.41 absolute on [0.5, 2] and 3 ulp elsewhere, rsqrtf and 1/x 2 ulp.
 
-1. Packed causal attention (nv_attn_fwd, nv_attn_bwd), head_dim 128, scale s = 128^-0.5.
-   Per row i and visible key j (j <= i): scores S = s·q·k, P = softmax(S), A_i = max_j s·sum_d |q_d||k_d|,
-   Z_i = max_j |S_ij|·log2(e), nb_i = i // 128 + 1 key blocks, n_i = i + 1 keys.
+1. Causal attention, packed (nv_attn_fwd, nv_attn_bwd) and over a KV cache (nv_attn_fwd_kv, nv_attn_bwd_kv), head_dim 128,
+   scale s = 128^-0.5.  A sequence has q_len query rows and kv_len keys; query i sits at key position dk + i with
+   dk = kv_len - q_len (the packed form is dk = 0, kv_len = q_len) and sees the keys j <= dk + i.
+   Per row i and visible key j: scores S = s·q·k, P = softmax(S), A_i = max_j s·sum_d |q_d||k_d|, Z_i = max_j |S_ij|·log2(e)
+   (both maxima over the visible keys), n_i = dk + i + 1 visible keys, and nb_i = (dk + min(q0 + 128, q_len) + 127) // 128
+   key blocks: the count the CTA of row i's 128-row query block (first row q0) walks (i // 128 + 1 when dk = 0).  With
+   dk > 0 the last of them may be fully masked for row i: its p are exactly 0 and it rescales by alpha = exp2(0) = 1
+   exactly, so it is only counted.
    Forward.  The kernel rounds P (unnormalised, against the running maximum) to bf16 before P·V and O once at the end.
      fp32 error of one unnormalised p_j:  eps_i = u·(4 + 3·Z_i + 64·A_i)
        (4u ex2.approx; <= 4u·Z_i of argument rounding in log2 units — fma, s·log2e and s itself rounded to fp32 — times ln 2;
@@ -26,13 +31,20 @@ wgmma k-step of 16.  The library is built with --use_fast_math: exp2f is ex2.app
    dS = p·(dP - D)·s in fp32 with dP = dO·v on the tensor cores and D = sum_d dO·O from the forward's bf16 O, and rounds dS to
    bf16 for dK and dQ.  Relative error of p: rho_i = |lse_i - lse_ref,i| + u·(4 + 3·(Z_i + |lse_i|·log2 e) + 64·A_i); R = max_i rho_i.
    Error of D: dD_i = |sum_d dO_id·(o_id - o_ref,id)| (the rounded O the kernel reads, measured) + 12u·sum_d |dO_id||o_id|.
-   E_ij = s·P_ij·(64u·sum_d |dO_id||v_jd| + dD_i) is the resulting absolute error of dS_ij; tc = 8u·ceil(L/16) the accumulation
-   over the <= L partners.  Under --use_fast_math a p or dS below 2^-126 may be flushed to 0 (keys no query attends to in the
+   E_ij = s·P_ij·(64u·sum_d |dO_id||v_jd| + dD_i) is the resulting absolute error of dS_ij; tc = 8u·ceil(n/16) the accumulation
+   over the <= n partners: n = kv_len keys for dQ, n = q_len queries for dK and dV.  Under --use_fast_math a p or dS below 2^-126 may be flushed to 0 (keys no query attends to in the
    heads with scores of std 8 have p ~ e^-120): each such term moves a product by at most 2^-126·|partner|·(1 + s·max|dP - D|),
    and a result below 2^-126 may itself flush.  With fz = 1 + s·max_ij |dP_ij - D_i|, sums over the sequence's rows:
      dV: |dv - dv_ref| <= b·|dv_ref| + (1 + 2^-7)·(b + R + tc)·(|P|^T |dO|) + 2^-126·(1 + sum_i |dO_i|)
      dK: |dk - dk_ref| <= b·|dk_ref| + (1 + 2^-7)·((b + R + tc + 3u)·(|dS|^T |Q|) + E^T |Q|) + 2^-126·(1 + fz·sum_i |q_i|)
      dQ: |dq - dq_ref| <= b·|dq_ref| + (1 + 2^-7)·((b + R + tc + 3u)·(|dS| |K|) + E |K|) + 2^-126·(1 + fz·sum_j |k_j|)
+   Over a KV cache the key rows' gradients meet an fp32 accumulator acc (dK | dV columns, acc0 before the call).  Write G
+   for everything but the leading b·|ref| in the dK (dV) bound: the error of the fp32 gradient before it is stored.
+     Cached rows j < dk: acc_j += dK_j in fp32, never rounded to bf16, so acc - acc0 (exact in fp64) is checked without the
+       b·|ref| term; the bf16 P and dS inside G stay, and the fp32 add costs u·|acc0 + dK| <= u·(|acc0| + |dk_ref|) (to first
+       order):  |(acc - acc0) - dk_ref| <= G + u·(|acc0| + |dk_ref|), the same for dV.
+     Suffix rows j >= dk: bf16(dK_j + acc0_j) from the fp32 sum, so the reference is ref = dk_ref + acc0 and the add's
+       rounding is carried through the bf16 rounding:  |dk - ref| <= b·|ref| + G + (1 + 2^-7)·u·|ref|, the same for dV.
    The same bounds hold with dvec = D handed over by nv_gemm_attnd_bf16 (fp32 row sums of dO·O, the same budget).
    Masked probabilities are exactly 0, so a sequence's o, lse and gradients do not depend on its neighbours: they are
    checked bit for bit across packings and against a second run.
@@ -83,12 +95,14 @@ HD = 128
 
 
 def _check(name, got, ref, tol):
+    """Asserts |got - ref| <= tol per element; returns the worst err/tol."""
     got = got.double()
     assert bool(torch.isfinite(got).all()), f"{name}: non-finite values"
     err = (got - ref).abs()
     bad = err > tol
     assert not bool(bad.any()), (f"{name}: {int(bad.sum())} of {bad.numel()} elements out of bound, worst err/tol "
                                  f"{(err / tol).max().item():.3g}, first at {tuple(bad.nonzero()[0].tolist())}")
+    return (err / tol).max().item() if err.numel() else 0.0
 
 
 def _cu(lens, dev):
@@ -127,62 +141,93 @@ def _attn_inputs(lens, H, seed, dev, stress):
     return x.reshape(T, 3 * H * HD).to(bf16)
 
 
+def _attn_seq_check(q, k, v, dO, o, lse, grads, scale, where, acc0=None):
+    """One sequence (a few of its heads) against fp64 autograd of its masked softmax, with the bounds of §1.  fp64 tensors
+    [heads, rows, 128] of the values the kernel read or wrote: q, dO and the kernel's o over the q_len query rows, k and v
+    over the kv_len keys (dk = kv_len - q_len); lse [heads, q_len] the kernel's.  grads: {tag: (dq, dk, dv)} with dk / dv
+    over the kv_len key rows: rows j >= dk the kernel's bf16 gradients, rows j < dk its accumulator after the call.  acc0:
+    None in the packed form (no accumulator, kv_len = q_len), else the (dK, dV) accumulator columns before the call.
+    Returns {quantity: worst err/tol}."""
+    Lq, Lk = q.shape[1], k.shape[1]
+    dk = Lk - Lq
+    assert dk >= 0 and (acc0 is not None or dk == 0), (Lq, Lk)
+    dev = q.device
+    i = torch.arange(Lq, device=dev, dtype=torch.float64)
+    mask = torch.arange(Lk, device=dev)[None, :] <= dk + torch.arange(Lq, device=dev)[:, None]
+    q0 = torch.div(i, 128, rounding_mode="floor") * 128
+    nb = torch.div(dk + torch.clamp(q0 + 128, max=Lq) + 127, 128, rounding_mode="floor")
+    tc_q = 8 * U * math.ceil(Lk / 16)          # dQ contracts over the keys
+    tc_k = 8 * U * math.ceil(Lq / 16)          # dK and dV over the queries
+    worst = {}
+
+    def chk(name, tag, got, ref, tol):
+        r = _check(" ".join(s for s in (name, tag, where) if s), got, ref, tol)
+        worst[name] = max(worst.get(name, 0.0), r)
+
+    qa, ka, va = (t.clone().requires_grad_(True) for t in (q, k, v))
+    with torch.enable_grad():
+        sc = (qa @ ka.transpose(1, 2) * scale).masked_fill(~mask, float("-inf"))
+        p = torch.softmax(sc, dim=-1)
+        oref = p @ va
+        dq, dkr, dvr = torch.autograd.grad(oref, (qa, ka, va), dO)
+    sc, p, oref = sc.detach(), p.detach(), oref.detach()
+    del qa, ka, va
+    lref = torch.logsumexp(sc, dim=-1)
+    A = (q.abs() @ k.abs().transpose(1, 2) * scale).masked_fill(~mask, 0).amax(-1)
+    Z = sc.abs().masked_fill(~mask, 0).amax(-1) * LOG2E
+    del sc
+    eps = U * (4 + 3 * Z + 64 * A)
+    F = 2 * eps + U * (39 + 71 * nb)
+    chk("o", "", o, oref, B8 * oref.abs() + F7 * (B8 + F)[..., None] * (p @ v.abs()))
+    chk("lse", "", lse, lref, 2.0 ** -21 + U * (6 * torch.log(dk + i + 1) + 2 * lref.abs() + 2 * Z + 34 + 2 * nb) + eps)
+
+    D = (dO * oref).sum(-1)
+    dD = (dO * (o - oref)).sum(-1).abs() + 12 * U * (dO.abs() * o.abs()).sum(-1)
+    R = ((lse - lref).abs() + U * (4 + 3 * (Z + lse.abs() * LOG2E) + 64 * A)).amax(-1)[:, None, None]
+    dPD = (dO @ v.transpose(1, 2) - D[..., None]).masked_fill(~mask, 0)
+    dS = (p * dPD * scale).abs()
+    E = scale * p * (64 * U * (dO.abs() @ v.abs().transpose(1, 2)) + dD[..., None])
+    fz = 1 + scale * dPD.abs().amax(dim=(1, 2))[:, None, None]
+    # G of §1: the error of the fp32 gradient before it is rounded to bf16 or added to the accumulator
+    g_dv = F7 * (B8 + R + tc_k) * (p.transpose(1, 2) @ dO.abs()) + TINY * (1 + dO.abs().sum(1, keepdim=True))
+    g_dk = (F7 * ((B8 + R + tc_k + 3 * U) * (dS.transpose(1, 2) @ q.abs()) + E.transpose(1, 2) @ q.abs())
+            + TINY * (1 + fz * q.abs().sum(1, keepdim=True)))
+    tol_dq = (B8 * dq.abs() + F7 * ((B8 + R + tc_q + 3 * U) * (dS @ k.abs()) + E @ k.abs())
+              + TINY * (1 + fz * k.abs().sum(1, keepdim=True)))
+    del dPD, p, dS, E
+
+    def key_rows(name, tag, got, ref, g, a0):
+        if a0 is None:
+            chk(name, tag, got, ref, B8 * ref.abs() + g)
+            return
+        if dk:
+            c0, c = a0[:, :dk], ref[:, :dk]
+            chk("acc " + name, tag, got[:, :dk] - c0, c, g[:, :dk] + U * (c0.abs() + c.abs()))
+        r = ref[:, dk:] + a0[:, dk:]
+        chk(name, tag, got[:, dk:], r, B8 * r.abs() + g[:, dk:] + F7 * U * r.abs())
+
+    for tag, (gq, gk, gv) in grads.items():
+        key_rows("dv", tag, gv, dvr, g_dv, None if acc0 is None else acc0[1])
+        key_rows("dk", tag, gk, dkr, g_dk, None if acc0 is None else acc0[0])
+        chk("dq", tag, gq, dq, tol_dq)
+    return worst
+
+
 def _attn_ref_check(qkv, o, lse, dqkvs, do, lens, H, scale):
-    """Checks o, lse and every dqkv in dqkvs against fp64 autograd of the masked softmax, one sequence (and a few heads) at a
-    time, with the bounds of the module docstring."""
+    """Checks o, lse and every dqkv in dqkvs of the packed form against fp64 autograd of the masked softmax, one sequence
+    (and a few heads) at a time, with the bounds of the module docstring."""
     T = qkv.shape[0]
-    dev = qkv.device
     s0 = 0
     for b, L in enumerate(lens):
         hc = max(1, min(H, (1 << 23) // (L * L)))
-        mask = torch.ones(L, L, dtype=torch.bool, device=dev).tril()
-        i = torch.arange(L, device=dev, dtype=torch.float64)
-        nb = torch.div(i, 128, rounding_mode="floor") + 1
-        tc = 8 * U * math.ceil(L / 16)
         for h0 in range(0, H, hc):
             hs = slice(h0, min(H, h0 + hc))
-            where = f"seq {b} (len {L}) heads {h0}..{min(H, h0 + hc) - 1}"
-            x = qkv[s0:s0 + L].view(L, 3, H, HD)[:, :, hs].double().permute(1, 2, 0, 3)
-            q, k, v = x[0], x[1], x[2]
-            dO = do[s0:s0 + L].view(L, H, HD)[:, hs].double().transpose(0, 1)
-            ok = o[s0:s0 + L].view(L, H, HD)[:, hs].double().transpose(0, 1)
-            lk = lse.view(H, T)[hs, s0:s0 + L].double()
-            qa, ka, va = (t.clone().requires_grad_(True) for t in (q, k, v))
-            with torch.enable_grad():
-                sc = (qa @ ka.transpose(1, 2) * scale).masked_fill(~mask, float("-inf"))
-                p = torch.softmax(sc, dim=-1)
-                oref = p @ va
-                dq, dk, dv = torch.autograd.grad(oref, (qa, ka, va), dO)
-            sc, p, oref = sc.detach(), p.detach(), oref.detach()
-            del qa, ka, va
-            lref = torch.logsumexp(sc, dim=-1)
-            A = (q.abs() @ k.abs().transpose(1, 2) * scale).masked_fill(~mask, 0).amax(-1)
-            Z = sc.abs().masked_fill(~mask, 0).amax(-1) * LOG2E
-            del sc
-            eps = U * (4 + 3 * Z + 64 * A)
-            F = 2 * eps + U * (39 + 71 * nb)
-            _check(f"o {where}", ok, oref, B8 * oref.abs() + F7 * (B8 + F)[..., None] * (p @ v.abs()))
-            _check(f"lse {where}", lk, lref, 2.0 ** -21 + U * (6 * torch.log(i + 1) + 2 * lref.abs() + 2 * Z + 34 + 2 * nb) + eps)
-
-            D = (dO * oref).sum(-1)
-            dD = (dO * (ok - oref)).sum(-1).abs() + 12 * U * (dO.abs() * ok.abs()).sum(-1)
-            R = ((lk - lref).abs() + U * (4 + 3 * (Z + lk.abs() * LOG2E) + 64 * A)).amax(-1)[:, None, None]
-            dPD = (dO @ v.transpose(1, 2) - D[..., None]).masked_fill(~mask, 0)
-            dS = (p * dPD * scale).abs()
-            E = scale * p * (64 * U * (dO.abs() @ v.abs().transpose(1, 2)) + dD[..., None])
-            fz = 1 + scale * dPD.abs().amax(dim=(1, 2))[:, None, None]
-            tol_dv = B8 * dv.abs() + F7 * (B8 + R + tc) * (p.transpose(1, 2) @ dO.abs()) + TINY * (1 + dO.abs().sum(1, keepdim=True))
-            tol_dk = (B8 * dk.abs() + F7 * ((B8 + R + tc + 3 * U) * (dS.transpose(1, 2) @ q.abs()) + E.transpose(1, 2) @ q.abs())
-                      + TINY * (1 + fz * q.abs().sum(1, keepdim=True)))
-            tol_dq = (B8 * dq.abs() + F7 * ((B8 + R + tc + 3 * U) * (dS @ k.abs()) + E @ k.abs())
-                      + TINY * (1 + fz * k.abs().sum(1, keepdim=True)))
-            del dPD
-            del p, dS, E
-            for tag, dqkv in dqkvs.items():
-                gk = dqkv[s0:s0 + L].view(L, 3, H, HD)[:, :, hs].double().permute(1, 2, 0, 3)
-                _check(f"dv {tag} {where}", gk[2], dv, tol_dv)
-                _check(f"dk {tag} {where}", gk[1], dk, tol_dk)
-                _check(f"dq {tag} {where}", gk[0], dq, tol_dq)
+            heads = lambda t: t[s0:s0 + L].view(L, H, HD)[:, hs].double().transpose(0, 1)
+            split = lambda t: t[s0:s0 + L].view(L, 3, H, HD)[:, :, hs].double().permute(1, 2, 0, 3).unbind(0)
+            q, k, v = split(qkv)
+            _attn_seq_check(q, k, v, heads(do), heads(o), lse.view(H, T)[hs, s0:s0 + L].double(),
+                            {tag: split(dqkv) for tag, dqkv in dqkvs.items()}, scale,
+                            f"seq {b} (len {L}) heads {h0}..{min(H, h0 + hc) - 1}")
         s0 += L
 
 
