@@ -350,6 +350,31 @@ int nv_decode_attn_rope_beam_fp8(const void* qkv, int64_t ld, const int* lens, c
                                  const void* pvq, const void* pkexp, const void* pvexp, int Sp, const int* plens, void* kq, void* vq,
                                  void* kexp, void* vexp, const int* src, int G, void* out, int64_t ldo, int R, int K, int H,
                                  int head_dim, float scale, void* stream);
+/* Contrastive search = transformers 4.28 GenerationMixin.contrastive_search / _ranking_fast as generate(penalty_alpha > 0,
+ * top_k > 1) reaches it through models/nav_model.py:388-396 -> lang_model.generate(**kwargs), for a model that returns HF's
+ * hidden-state tuple (the reference's ModifiedLM returns one tensor, models/modified_lm.py:119,144).  K = top_k = 1..64
+ * candidates per prompt, run as decode rows b * K + j; x^ = bf16(x / bf16(||x||)) of a final-norm hidden row.
+ * nv_contrastive_topk: one CTA per prompt, p = bf16(softmax(logits)) (special ids -inf; computed in fp64 and rounded once, where
+ * torch's bf16 softmax rounds an fp32 value: they can differ by one ulp next to a rounding midpoint) and the K largest p by
+ * (p desc, token id asc) -> p [B, K] bf16, tok [B, K] int32.  V <= 51200.
+ * nv_contrastive_context: ctx[b, i] = x^ of the packed final-norm prompt row hn[cu_seqlens[b] + i] ([T, D]), ctx_len[b] = its
+ * length; ctx [B, Sc, D] bf16 is prompt b's context (left pads are not part of it).
+ * nv_contrastive_rank: pen_j = max over the ctx_len[b] context rows of bf16(c^_i . h^_j) for the candidates' final-norm rows hn
+ * [B * K, D], score_j = bf16(bf16(fp32(1 - alpha) p_j) - bf16(fp32(alpha) pen_j)), sel[b] = the first best j; next[b] = its
+ * token, or pad_id once finished[b] (EOS sets finished[b] when stop_on_eos); x^ of its row is appended to ctx, the row itself
+ * copied to hsel [B, D], plens[b] and lens[b * K .. b * K + K) advance by one.  pen_key uint32 [B * K] is zero before the call
+ * and after it.  pen_out / score_out: optional fp32 [B, K].  Two launches: the context rows are split over 16 CTAs per prompt.
+ * nv_contrastive_commit: per layer l, the K and V rows of candidate b * K + sel[b] in its one-slot cache ([B * K, 1, D]) go to
+ * row plens[b] - 1 of prompt b's cache ([B, Sp, D]); table [L, 8] holds the layer's kc, vc, pk, pv pointers and, with fp8,
+ * the four exponent arrays ([.., H] int8; the rows then hold D e4m3 bytes).  A byte copy: the bits are the candidate's. */
+int nv_contrastive_topk(const void* logits, int64_t ld, int V, const int* special, int n_special, int K, void* p, int* tok, int B,
+                        void* stream);
+int nv_contrastive_context(const void* hn, const int* cu_seqlens, int B, int T, void* ctx, int* ctx_len, int Sc, int D, void* stream);
+int nv_contrastive_rank(const void* hn, void* ctx, int* ctx_len, int Sc, int D, int K, unsigned* pen_key, const void* p,
+                        const int* tok, double alpha, int* finished, int eos_id, int pad_id, int stop_on_eos, int* next, int* sel,
+                        void* hsel, int* plens, int* lens, float* pen_out, float* score_out, int B, void* stream);
+int nv_contrastive_commit(const unsigned long long* table, int L, const int* sel, const int* plens, int K, int Sp, int D, int H,
+                          int fp8, int B, void* stream);
 /* at most 64 special ids (n_special), here and in nv_sample_topk; longer lists return NV_ERR_BAD_ARG */
 int nv_argmax_masked(const void* logits, int64_t ld, int V, const int* special, int n_special, int* finished, int eos_id,
                      int pad_id, int stop_on_eos, int* next, int B, void* stream);

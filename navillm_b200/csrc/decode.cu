@@ -1303,6 +1303,295 @@ __global__ void __launch_bounds__(BS_THREADS) beam_select_kernel(const float* __
   if (tid == 0) ps[BS_STEP] = t + 1;
 }
 
+// ---- contrastive search (GenerationMixin.contrastive_search / _ranking_fast of transformers 4.28) ----
+// A step: the K candidates of prompt b (the K most probable tokens) run as decode rows b * K + j over the prompt cache, each is
+// scored bf16(bf16((1 - a) p_j) - bf16(a pen_j)) with pen_j = max_i bf16(c^_i . h^_j) over the normalised context rows of the
+// prompt, and the best one's token, K/V and hidden state are kept.  x^ = bf16(x / bf16(||x||)) (4.28's bf16 tensor ops: a norm
+// summed in fp32 and rounded, an fp32 division rounded).  --use_fast_math makes '/' and sqrtf approximate, hence the _rn forms.
+constexpr int CT_KMAX = 64;                  // candidates per prompt
+constexpr int CT_THREADS = 1024;             // nv_contrastive_topk: one CTA per prompt (the smp_* helpers assume 32 warps)
+constexpr int CR_SPLIT = 16;                 // nv_contrastive_rank: CTAs per prompt over its context rows
+constexpr int CR_CHUNK = 8;                  // candidates staged in shared memory per pass over the rows
+constexpr int CR_THREADS = 256;
+constexpr int CS_THREADS = 128;
+
+// x^ of a D-element bf16 row (D % 8 == 0) by one warp; `out` may be shared or global memory
+__device__ __forceinline__ void ct_normalize_row(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ out, int D, int lane) {
+  float ss = 0.f;
+  for (int c = lane * 8; c < D; c += 256) {
+    float f[8];
+    unpack8d(*reinterpret_cast<const uint4*>(x + c), f);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) ss = __fmaf_rn(f[i], f[i], ss);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+  const float nrm = bf16_round(__fsqrt_rn(ss));
+  for (int c = lane * 8; c < D; c += 256) {
+    float f[8];
+    unpack8d(*reinterpret_cast<const uint4*>(x + c), f);
+    uint4 o;
+    o.x = pack_bf16x2(__fdiv_rn(f[0], nrm), __fdiv_rn(f[1], nrm));
+    o.y = pack_bf16x2(__fdiv_rn(f[2], nrm), __fdiv_rn(f[3], nrm));
+    o.z = pack_bf16x2(__fdiv_rn(f[4], nrm), __fdiv_rn(f[5], nrm));
+    o.w = pack_bf16x2(__fdiv_rn(f[6], nrm), __fdiv_rn(f[7], nrm));
+    *reinterpret_cast<uint4*>(out + c) = o;
+  }
+}
+
+// exp(x) in fp64 for x <= 0 (or -inf), within 2e-16 relative: exp(x) = 2^k exp(r), |r| <= ln2 / 2, Taylor to degree 12.  The
+// library's exp calls an out-of-line slow path that spills at 1024 threads.
+__device__ __forceinline__ double ct_exp_neg(double x) {
+  if (!(x > -745.0)) return 0.0;
+  const double k = rint(x * 1.4426950408889634);
+  const double r = fma(k, -1.90821492927058770002e-10, fma(k, -6.93147180369123816490e-01, x));
+  double e = 1.0 / 479001600.0;
+#pragma unroll
+  for (int n = 11; n >= 1; --n) {
+    double f = 1.0;
+    for (int i = 2; i <= n; ++i) f *= i;
+    e = fma(e, r, 1.0 / f);
+  }
+  e = fma(e, r, 1.0);
+  const int k1 = (int)k / 2, k2 = (int)k - k1;
+  return e * __hiloint2double((1023 + k1) << 20, 0) * __hiloint2double((1023 + k2) << 20, 0);
+}
+
+// One CTA per prompt: p = bf16(softmax(logits)) with special ids -inf (row max, exponentials and their sum in fp64, one
+// rounding to bf16; 4.28's bf16 softmax computes in fp32 with torch's own summation order, so the two can differ by one bf16
+// ulp where the fp32 value sits next to a rounding midpoint: fp64 gives the exact value, independent of any order), then the K largest p ordered by (p desc, token id asc).  The K-th largest key is found with sample_topk_kernel's
+// two radix passes over the 16-bit key; of the tokens sharing it, the lowest ids are taken (contiguous chunks in token order).
+__global__ void __launch_bounds__(CT_THREADS) contrastive_topk_kernel(const __nv_bfloat16* __restrict__ logits, int64_t ld, int V,
+                                                                      const int* __restrict__ special, int n_special, int K,
+                                                                      __nv_bfloat16* __restrict__ p_out, int* __restrict__ tok_out) {
+  extern __shared__ float sc[];                              // [V] logits, then p
+  __shared__ int hist[256];
+  __shared__ float red[32];
+  __shared__ double redd[32];
+  __shared__ int s_special[MAX_SPECIAL];
+  __shared__ int s_n;
+  __shared__ uint32_t s_key[CT_KMAX];                        // (p bits << 17) | (0x1ffff - token): larger is better
+  griddep_launch();
+  griddep_wait();
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  if (tid < n_special) s_special[tid] = special[tid];
+  if (tid < 256) hist[tid] = 0;
+  if (tid == 0) s_n = 0;
+  __syncthreads();
+  const __nv_bfloat16* row = logits + (int64_t)b * ld;
+  float mx = -INFINITY;
+  for (int c = tid; c < V; c += CT_THREADS) {
+    bool sp = false;
+    for (int s = 0; s < n_special; ++s) sp |= (s_special[s] == c);
+    const float v = sp ? -INFINITY : __bfloat162float(row[c]);
+    sc[c] = v;
+    mx = fmaxf(mx, v);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  if (lane == 0) red[w] = mx;
+  __syncthreads();
+  mx = red[lane];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  double s = 0.0;
+  for (int c = tid; c < V; c += CT_THREADS) s += ct_exp_neg((double)sc[c] - (double)mx);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane == 0) redd[w] = s;
+  __syncthreads();
+  s = redd[lane];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  const double inv = __drcp_rn(s);                         // 1 ulp of fp64 is far below the bf16 rounding of p
+  for (int c = tid; c < V; c += CT_THREADS) {
+    const float p = __bfloat162float(__double2bfloat16(ct_exp_neg((double)sc[c] - (double)mx) * inv));
+    sc[c] = p;
+    atomicAdd(&hist[smp_key16(p) >> 8], 1);
+  }
+  __syncthreads();
+  int hi_bin, above;
+  smp_pick_bin(hist, K, hi_bin, above);
+  if (tid < 256) hist[tid] = 0;
+  __syncthreads();
+  for (int c = tid; c < V; c += CT_THREADS) {
+    const uint32_t key = smp_key16(sc[c]);
+    if ((int)(key >> 8) == hi_bin) atomicAdd(&hist[key & 255u], 1);
+  }
+  __syncthreads();
+  int lo_bin, above2;
+  smp_pick_bin(hist, K - above, lo_bin, above2);
+  const uint32_t thr = ((uint32_t)hi_bin << 8) | (uint32_t)lo_bin;
+  const int need = K - above - above2;                      // tokens of key thr taken, lowest ids first
+  const int CH = (V + CT_THREADS - 1) / CT_THREADS;
+  const int c0 = min(tid * CH, V), c1 = min(c0 + CH, V);
+  int cnt = 0;
+  for (int c = c0; c < c1; ++c) cnt += smp_key16(sc[c]) == thr;
+  int before = smp_cta_exclusive(cnt, hist);
+  for (int c = c0; c < c1; ++c) {
+    const float p = sc[c];
+    const uint32_t key = smp_key16(p);
+    bool take = key > thr;
+    if (key == thr) take = before++ < need;
+    if (take) s_key[atomicAdd(&s_n, 1)] = ((__float_as_uint(p) >> 16) << 17) | (0x1ffffu - (uint32_t)c);
+  }
+  __syncthreads();
+  if (tid < K) {                                             // rank sort: the keys are distinct
+    const uint32_t x = s_key[tid];
+    int r = 0;
+    for (int j = 0; j < K; ++j) r += s_key[j] > x;
+    tok_out[b * K + r] = (int)(0x1ffffu - (x & 0x1ffffu));
+    p_out[b * K + r] = __ushort_as_bfloat16((unsigned short)(x >> 17));
+  }
+}
+
+// One warp per packed prompt row: ctx[b, i] = x^ of hn[cu[b] + i] (i < Sc), ctx_len[b] = the prompt's length.
+__global__ void __launch_bounds__(256) contrastive_context_kernel(const __nv_bfloat16* __restrict__ hn, const int* __restrict__ cu, int B,
+                                                                 int T, __nv_bfloat16* __restrict__ ctx, int* __restrict__ ctx_len, int Sc,
+                                                                 int D) {
+  griddep_launch();
+  griddep_wait();
+  const int row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (row >= T) return;
+  int b = 0;
+  while (b + 1 < B && cu[b + 1] <= row) ++b;
+  const int i = row - cu[b];
+  if (i < Sc) ct_normalize_row(hn + (int64_t)row * D, ctx + ((int64_t)b * Sc + i) * D, D, lane);
+  if (i == 0 && lane == 0) ctx_len[b] = cu[b + 1] - cu[b];
+}
+
+// grid (CR_SPLIT, B): CTA (s, b) takes its share of the ctx_len[b] context rows of prompt b and folds max_i bf16(c^_i . h^_j) of
+// each candidate j into pen_key[b * K + j] (an f32_order key; 0 is below every value, and the select kernel resets it).  The
+// candidates are normalised into shared memory CR_CHUNK at a time; a warp walks a context row per iteration.
+__global__ void __launch_bounds__(CR_THREADS) contrastive_pen_kernel(const __nv_bfloat16* __restrict__ hn, const __nv_bfloat16* __restrict__ ctx,
+                                                                     const int* __restrict__ ctx_len, int Sc, int D, int K,
+                                                                     unsigned* __restrict__ pen_key) {
+  extern __shared__ uint4 cr_smem[];                         // [CR_CHUNK, D] bf16 normalised candidates
+  __nv_bfloat16* s_h = reinterpret_cast<__nv_bfloat16*>(cr_smem);
+  __shared__ unsigned s_max[CR_CHUNK];
+  griddep_launch();
+  griddep_wait();
+  constexpr int NW = CR_THREADS / 32;
+  const int b = blockIdx.y, tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  const int n = min(ctx_len[b], Sc);
+  const int per = (n + CR_SPLIT - 1) / CR_SPLIT;
+  const int i0 = blockIdx.x * per, i1 = min(n, i0 + per);
+  if (i0 >= i1) return;                                      // uniform over the CTA
+  for (int j0 = 0; j0 < K; j0 += CR_CHUNK) {
+    const int nj = min(CR_CHUNK, K - j0);
+    __syncthreads();                                         // the previous chunk is consumed
+    for (int jj = w; jj < nj; jj += NW) ct_normalize_row(hn + (int64_t)(b * K + j0 + jj) * D, s_h + (int64_t)jj * D, D, lane);
+    if (tid < CR_CHUNK) s_max[tid] = 0u;
+    __syncthreads();
+    unsigned wmax[CR_CHUNK];
+#pragma unroll
+    for (int jj = 0; jj < CR_CHUNK; ++jj) wmax[jj] = 0u;
+    for (int i = i0 + w; i < i1; i += NW) {
+      const __nv_bfloat16* c = ctx + ((int64_t)b * Sc + i) * D;
+      float acc[CR_CHUNK];
+#pragma unroll
+      for (int jj = 0; jj < CR_CHUNK; ++jj) acc[jj] = 0.f;
+      for (int d = lane * 8; d < D; d += 256) {
+        float cf[8];
+        unpack8d(*reinterpret_cast<const uint4*>(c + d), cf);
+#pragma unroll
+        for (int jj = 0; jj < CR_CHUNK; ++jj) {
+          if (jj < nj) {
+            float hf[8];
+            unpack8d(*reinterpret_cast<const uint4*>(s_h + (int64_t)jj * D + d), hf);
+#pragma unroll
+            for (int e = 0; e < 8; ++e) acc[jj] = __fmaf_rn(cf[e], hf[e], acc[jj]);
+          }
+        }
+      }
+#pragma unroll
+      for (int jj = 0; jj < CR_CHUNK; ++jj) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) acc[jj] += __shfl_xor_sync(0xffffffffu, acc[jj], o);
+        wmax[jj] = max(wmax[jj], f32_order(bf16_round(acc[jj])));
+      }
+    }
+    if (lane == 0)
+      for (int jj = 0; jj < nj; ++jj) atomicMax(&s_max[jj], wmax[jj]);
+    __syncthreads();
+    if (tid < nj) atomicMax(&pen_key[b * K + j0 + tid], s_max[tid]);
+  }
+}
+
+// One CTA per prompt: scores, the first best candidate sel[b], its token (pad once the row is finished; EOS finishes it as in
+// argmax_kernel), x^ of its row appended to the context, its final-norm row gathered into hsel[b] for the lm_head; then plens[b]
+// and the K candidate rows' lens advance (nv_contrastive_commit stores the K/V at plens[b] - 1).  pen_key is reset for the next
+// step.  pen_out / score_out (optional, fp32 [B, K]) receive pen and the score.
+__global__ void __launch_bounds__(CS_THREADS) contrastive_select_kernel(const __nv_bfloat16* __restrict__ hn, __nv_bfloat16* __restrict__ ctx,
+                                                                        int* __restrict__ ctx_len, int Sc, int D, int K,
+                                                                        unsigned* __restrict__ pen_key, const __nv_bfloat16* __restrict__ p,
+                                                                        const int* __restrict__ tok, float a1, float a,
+                                                                        int* __restrict__ finished, int eos_id, int pad_id, int stop_on_eos,
+                                                                        int* __restrict__ next, int* __restrict__ sel,
+                                                                        __nv_bfloat16* __restrict__ hsel, int* __restrict__ plens,
+                                                                        int* __restrict__ lens, float* __restrict__ pen_out,
+                                                                        float* __restrict__ score_out) {
+  __shared__ int s_sel;
+  griddep_launch();
+  griddep_wait();
+  const int b = blockIdx.x, tid = threadIdx.x;
+  if (tid == 0) {
+    float best = -INFINITY;
+    int bj = 0;
+    for (int j = 0; j < K; ++j) {
+      const float pen = f32_unorder(pen_key[b * K + j]);
+      pen_key[b * K + j] = 0u;
+      const float pj = __bfloat162float(p[b * K + j]);
+      const float score = bf16_round(__fsub_rn(bf16_round(__fmul_rn(a1, pj)), bf16_round(__fmul_rn(a, pen))));
+      if (j == 0 || score > best) { best = score; bj = j; }
+      if (pen_out) pen_out[b * K + j] = pen;
+      if (score_out) score_out[b * K + j] = score;
+    }
+    s_sel = bj;
+    sel[b] = bj;
+    int t = tok[b * K + bj];
+    if (finished[b]) t = pad_id;
+    else if (stop_on_eos && t == eos_id) finished[b] = 1;
+    next[b] = t;
+  }
+  __syncthreads();
+  const int64_t r = (int64_t)b * K + s_sel;
+  const int n = ctx_len[b];
+  if (tid < 32 && n < Sc) ct_normalize_row(hn + r * D, ctx + ((int64_t)b * Sc + n) * D, D, tid);
+  for (int c = tid * 8; c < D; c += CS_THREADS * 8)
+    *reinterpret_cast<uint4*>(hsel + (int64_t)b * D + c) = *reinterpret_cast<const uint4*>(hn + r * D + c);
+  __syncthreads();
+  if (tid == 0) {
+    if (n < Sc) ctx_len[b] = n + 1;
+    plens[b] += 1;
+  }
+  if (tid < K) lens[b * K + tid] += 1;
+}
+
+// grid (L, B): layer l's K and V rows of the selected candidate (row b * K + sel[b] of the one-slot candidate caches) go to row
+// plens[b] - 1 of prompt b's cache.  table[l * 8 ..]: kc, vc, pk, pv, then for fp8 the four exponent arrays (else null).  A row
+// is row_bytes of K or V (bf16, or e4m3 bytes) and exp_bytes exponents; a plain byte copy, so the bits are the candidate's.
+__global__ void __launch_bounds__(256) contrastive_commit_kernel(const unsigned long long* __restrict__ table, const int* __restrict__ sel,
+                                                                 const int* __restrict__ plens, int K, int Sp, int row_bytes,
+                                                                 int exp_bytes) {
+  griddep_launch();
+  griddep_wait();
+  const int l = blockIdx.x, b = blockIdx.y;
+  const unsigned long long* t = table + (int64_t)l * 8;
+  const int64_t src = (int64_t)b * K + sel[b], dst = (int64_t)b * Sp + plens[b] - 1;
+  const int n16 = row_bytes >> 4;
+  for (int kv = 0; kv < 2; ++kv) {
+    const uint4* s = reinterpret_cast<const uint4*>(t[kv]) + src * n16;
+    uint4* d = reinterpret_cast<uint4*>(t[2 + kv]) + dst * n16;
+    for (int i = threadIdx.x; i < n16; i += blockDim.x) d[i] = s[i];
+    if (exp_bytes) {
+      const int8_t* se = reinterpret_cast<const int8_t*>(t[4 + kv]) + src * exp_bytes;
+      int8_t* de = reinterpret_cast<int8_t*>(t[6 + kv]) + dst * exp_bytes;
+      for (int i = threadIdx.x; i < exp_bytes; i += blockDim.x) de[i] = se[i];
+    }
+  }
+}
+
 }  // namespace nv
 
 using namespace nv;
@@ -1607,6 +1896,68 @@ int nv_decode_attn_rope_beam_fp8(const void* qkv, int64_t ld, const int* lens, c
 int nv_add_int(int* x, int n, int delta, void* stream) {
   if (n == 0) return NV_OK;
   NV_CUDA(launch_pdl(add_int_kernel, dim3((n + 255) / 256), dim3(256), 0, S_(stream), x, n, delta));
+  return NV_OK;
+}
+
+// Contrastive search (see contrastive_topk_kernel .. contrastive_commit_kernel).
+int nv_contrastive_topk(const void* logits, int64_t ld, int V, const int* special, int n_special, int K, void* p, int* tok, int B,
+                        void* stream) {
+  NV_REQUIRE(logits && p && tok && B >= 0 && ld >= V, "nv_contrastive_topk: bad arguments (B=%d V=%d)", B, V);
+  NV_REQUIRE(K >= 1 && K <= CT_KMAX && K <= V, "nv_contrastive_topk: top_k=%d: 1..%d candidates (and <= V) supported", K, CT_KMAX);
+  NV_REQUIRE(V > 0 && V <= (1 << 17) && (int64_t)V * 4 <= 200 * 1024, "nv_contrastive_topk: vocabulary of %d not supported", V);
+  NV_REQUIRE(n_special >= 0 && n_special <= MAX_SPECIAL && (n_special == 0 || special),
+             "nv_contrastive_topk: n_special=%d out of range (max %d)", n_special, MAX_SPECIAL);
+  if (B == 0) return NV_OK;
+  static bool attr_set = false;
+  if (!attr_set) {
+    NV_CUDA(cudaFuncSetAttribute(contrastive_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    attr_set = true;
+  }
+  NV_CUDA(launch_pdl(contrastive_topk_kernel, dim3(B), dim3(CT_THREADS), (size_t)V * 4, S_(stream), CBF(logits), ld, V, special,
+                     n_special, K, BF(p), tok));
+  return NV_OK;
+}
+
+int nv_contrastive_context(const void* hn, const int* cu_seqlens, int B, int T, void* ctx, int* ctx_len, int Sc, int D, void* stream) {
+  NV_REQUIRE(hn && cu_seqlens && ctx && ctx_len && B >= 1 && T >= 0 && Sc > 0 && D > 0 && (D & 7) == 0,
+             "nv_contrastive_context: bad arguments (B=%d T=%d Sc=%d D=%d; D %% 8 == 0)", B, T, Sc, D);
+  if (T == 0) return NV_OK;
+  NV_CUDA(launch_pdl(contrastive_context_kernel, dim3((T + 7) / 8), dim3(256), 0, S_(stream), CBF(hn), cu_seqlens, B, T, BF(ctx),
+                     ctx_len, Sc, D));
+  return NV_OK;
+}
+
+int nv_contrastive_rank(const void* hn, void* ctx, int* ctx_len, int Sc, int D, int K, unsigned* pen_key, const void* p,
+                        const int* tok, double alpha, int* finished, int eos_id, int pad_id, int stop_on_eos, int* next, int* sel,
+                        void* hsel, int* plens, int* lens, float* pen_out, float* score_out, int B, void* stream) {
+  NV_REQUIRE(hn && ctx && ctx_len && pen_key && p && tok && finished && next && sel && hsel && plens && lens && B >= 0,
+             "nv_contrastive_rank: null argument");
+  NV_REQUIRE(K >= 1 && K <= CT_KMAX && Sc > 0 && D > 0 && (D & 7) == 0 && D <= 8192,
+             "nv_contrastive_rank: bad sizes (K=%d Sc=%d D=%d; K <= %d, D %% 8 == 0, D <= 8192)", K, Sc, D, CT_KMAX);
+  NV_REQUIRE(alpha == alpha && alpha - alpha == 0.0, "nv_contrastive_rank: penalty_alpha must be finite");
+  if (B == 0) return NV_OK;
+  const size_t smem = (size_t)CR_CHUNK * D * 2;
+  static size_t smem_set = 48 * 1024;
+  if (smem > smem_set) {
+    NV_CUDA(cudaFuncSetAttribute(contrastive_pen_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    smem_set = smem;
+  }
+  NV_CUDA(launch_pdl(contrastive_pen_kernel, dim3(CR_SPLIT, B), dim3(CR_THREADS), smem, S_(stream), CBF(hn), CBF(ctx), ctx_len, Sc,
+                     D, K, pen_key));
+  // 4.28 multiplies the bf16 tensors by the Python floats 1 - alpha and alpha, which take the fp32 opmath type
+  NV_CUDA(launch_pdl(contrastive_select_kernel, dim3(B), dim3(CS_THREADS), 0, S_(stream), CBF(hn), BF(ctx), ctx_len, Sc, D, K, pen_key,
+                     CBF(p), tok, (float)(1.0 - alpha), (float)alpha, finished, eos_id, pad_id, stop_on_eos, next, sel, BF(hsel),
+                     plens, lens, pen_out, score_out));
+  return NV_OK;
+}
+
+int nv_contrastive_commit(const unsigned long long* table, int L, const int* sel, const int* plens, int K, int Sp, int D, int H,
+                          int fp8, int B, void* stream) {
+  NV_REQUIRE(table && sel && plens && L >= 1 && K >= 1 && Sp > 0 && H > 0 && D == H * 128 && B >= 0,
+             "nv_contrastive_commit: bad arguments (L=%d K=%d Sp=%d D=%d H=%d)", L, K, Sp, D, H);
+  if (B == 0) return NV_OK;
+  NV_CUDA(launch_pdl(contrastive_commit_kernel, dim3(L, B), dim3(256), 0, S_(stream), table, sel, plens, K, Sp, fp8 ? D : 2 * D,
+                     fp8 ? H : 0));
   return NV_OK;
 }
 

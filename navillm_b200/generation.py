@@ -1,5 +1,6 @@
-"""``ModifiedLlamaForCausalLM.generate``'s decoding (HF GenerationMixin greedy / sampling / beam search): the call's record,
-the decode states, the prefill, the graph-replayed step loop and the drivers ``decode`` and ``beam_search``."""
+"""``ModifiedLlamaForCausalLM.generate``'s decoding (HF GenerationMixin greedy / sampling / beam / contrastive search): the call's
+record, the decode states, the prefill, the graph-replayed step loop and the drivers ``decode``, ``beam_search`` and
+``contrastive_search``."""
 from __future__ import annotations
 
 import collections
@@ -22,10 +23,10 @@ class Decoding:
     eos: int
     pad: int
     stop_on_eos: Optional[bool]          # None for beams: a prompt stops when its hypotheses are done
-    mode: str                            # "greedy", "sample", "trie", "trie+sample" or "beam"
+    mode: str                            # "greedy", "sample", "trie", "trie+sample", "beam" or "contrastive"
     kv: str                              # the KV cache format, "bf16" or "fp8"
     temperature: Optional[float] = None  # sampled modes
-    top_k: Optional[int] = None
+    top_k: Optional[int] = None          # sampled modes, and contrastive search's candidates per prompt (= n)
     top_p: Optional[float] = None
     trie_eos: Optional[int] = None       # trie modes: the flattened trie's end-of-answer id
     n: int = 1                           # rows per prompt: samples, or beams
@@ -33,6 +34,7 @@ class Decoding:
     proc: Optional[tuple] = None         # the device logits processors (``processors``)
     n_return: int = 1                    # beams: sequences returned per prompt (host finalisation)
     length_penalty: Optional[float] = None   # beams: its normalisers are copied into the state every call
+    penalty_alpha: Optional[float] = None    # contrastive search: the degeneration penalty's weight
 
     @property
     def sampled(self) -> bool:
@@ -41,7 +43,7 @@ class Decoding:
     def key(self) -> tuple:
         """The graph key: every field a captured step bakes in (not ``n_return`` or ``length_penalty``), the format last."""
         return (self.eos, self.pad, self.stop_on_eos, self.mode, self.temperature, self.top_k, self.top_p, self.trie_eos, self.n,
-                self.early_stopping, self.proc, self.kv)
+                self.early_stopping, self.proc, self.penalty_alpha, self.kv)
 
 
 def processors(repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens, eos: int) -> Optional[tuple]:
@@ -145,33 +147,45 @@ def prefill(lm, dec: Decoding, input_ids, attention_mask, vis, max_new_tokens: i
     beams, per prompt (``dec.n`` > 1): the prompt keys go to a prompt cache ``pk`` / ``pv`` [B, Sp, D] that the n rows of a
     prompt share (``plens`` keys each), and kc / vc [B * n, G, D] hold only the generated keys, read through the source table
     ``src`` (``st.beam``), so no K/V is copied.  Sampling adds its uniform numbers ``u`` (the host processors draw their
-    own), tries their masked logits and walk state, beams the scorer's buffers (``ops.beam_select``)."""
+    own), tries their masked logits and walk state, beams the scorer's buffers (``ops.beam_select``).
+
+    Contrastive search (``dec.n`` = k candidates per prompt): the prompt cache holds the prompt and then the selected tokens
+    (Sp = bucket(longest prompt + max_new_tokens)), kc / vc [B * k, 1, D] the candidates' own keys, one slot each; the logits,
+    ids and flags are per prompt ([B]), and the prefill returns every prompt row of the last layer (the context).  See
+    ``contrastive_search``."""
     from .modified_lm import PackedPrompt           # modified_lm imports this module
     dev, d = lm._device(), lm.dims
     pp = PackedPrompt(input_ids, attention_mask, lm, dev, generate_positions=True)
     vis = lm.cat_vis(*vis, pp)
     bucket = lambda n: (n + 127) // 128 * 128       # cache lengths in multiples of 128: more calls share a state
     B, n, V = pp.B, dec.n, lm.lm_head.weight.shape[0]
-    R, shared = B * n, n > 1
+    R, shared, cs = B * n, n > 1, dec.mode == "contrastive"
     Sp, G = (bucket(max(pp.seqlens)), bucket(max_new_tokens)) if shared else (0, bucket(max(pp.seqlens) + max_new_tokens))
+    if cs:
+        Sp, G = bucket(max(pp.seqlens) + max_new_tokens), 1
+    P = B if cs else R                              # rows with their own logits, ids and finished flag
 
     def build():
         cache = lambda rows, length: llama_mod.kv_cache(d, rows, length, dec.kv, dev)
         zeros = lambda dtype, *shape: torch.zeros(shape, dtype=dtype, device=dev)
         i32 = lambda *shape: zeros(torch.int32, *shape)
-        st = SimpleNamespace(kc=cache(R, G), vc=cache(R, G), logits=logits_buffer(R, V, dev), next_ids=i32(R), lens=i32(R),
+        st = SimpleNamespace(kc=cache(R, G), vc=cache(R, G), logits=logits_buffer(P, V, dev), next_ids=i32(P), lens=i32(R),
                              Sp=Sp, G=G, graph=None)
         if dec.mode == "beam":
             st.beam_score, st.cand_score, st.cand_tok = zeros(torch.float32, R), zeros(torch.float32, B, 2 * n), i32(B, 2 * n)
             st.cand_par, st.hist, st.src, st.hyp_score = i32(B, 2 * n), i32(R, G), i32(R, G), zeros(torch.float64, B, n + 1)
             st.hyp_meta, st.hyp_tok, st.pstate, st.norm = i32(B, n, 2), i32(B, n, G), i32(B, 5), zeros(torch.float64, G)
         else:
-            st.finished = i32(R)
+            st.finished = i32(P)
             if shared:                                                      # the identity source table
                 st.src = torch.arange(R, dtype=torch.int32, device=dev)[:, None].expand(R, G).contiguous()
         if shared:
             st.pk, st.pv, st.plens = cache(B, Sp), cache(B, Sp), i32(B)
             st.beam = SimpleNamespace(pk=st.pk, pv=st.pv, plens=st.plens, src=st.src, K=n)
+        if cs:
+            st.cand_p, st.cand_ids, st.sel, st.pen_key = zeros(bf16, B, n), i32(B, n), i32(B), i32(R)
+            st.ctx, st.ctx_len, st.hsel = zeros(bf16, B, Sp, d.hidden), i32(B), zeros(bf16, B, d.hidden)
+            st.commit_table = ops.contrastive_commit_table(st.kc, st.vc, st.pk, st.pv)
         if dec.sampled and not host:
             st.u = torch.empty((R,), dtype=torch.float32, device=dev)
         if dec.trie_eos is not None:
@@ -182,14 +196,19 @@ def prefill(lm, dec: Decoding, input_ids, attention_mask, vis, max_new_tokens: i
         st.plens.copy_(torch.tensor(pp.seqlens, dtype=torch.int32), non_blocking=True)
     x = ops.embed_fwd(pp.ids, lm.model.embed_tokens.weight.data, pp.vis_src if vis is not None else None, vis)
     h, _ = lm.core.forward(x, pp.pos, pp.cu, pp.seqlens, save=False, kv_store=(st.pk, st.pv) if shared else (st.kc, st.vc),
-                           out_rows=pp.last_rows)
+                           out_rows=None if cs else pp.last_rows)
     return pp, st, h
 
 
 def decode_head(lm, h_rows: torch.Tensor, out: torch.Tensor) -> None:
     """Final RMSNorm + lm_head of decode rows into ``out`` [rows, V] bf16 (the fp8 weight copy when there is one)."""
-    B = h_rows.shape[0]
     hn, _ = ops.rmsnorm_fwd(h_rows, lm.model.norm.weight.data, lm.dims.rms_eps)
+    lm_head_rows(lm, hn, out)
+
+
+def lm_head_rows(lm, hn: torch.Tensor, out: torch.Tensor) -> None:
+    """lm_head of final-norm rows ``hn`` into ``out`` [rows, V] bf16 (the fp8 weight copy when there is one)."""
+    B = hn.shape[0]
     fp8_head = lm._fp8.view([lm.lm_head.weight], tuple(lm.lm_head.weight.shape)) if lm.core.fp8 is not None else None
     if B <= 16 and fp8_head is not None:
         ops.gemm_skinny_fp8(hn, *fp8_head, out=out)
@@ -350,13 +369,74 @@ def decode(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph, s
     if miss:
         return None
     new = torch.stack(out_tokens, dim=1).to(torch.int64)
-    if stop and check_every > 1 and new.shape[1] > 1:
-        # trim the columns generated after the step at which the last row emitted EOS (see check_every above)
+    if stop and check_every > 1:
+        new = trim_after_eos(new, eos)                        # see check_every above
+    return torch.cat([input_ids.to(dev).repeat_interleave(n, dim=0), new], dim=1)
+
+
+def trim_after_eos(new: torch.Tensor, eos: int) -> torch.Tensor:
+    """The generated columns [rows, n] without those after the step at which the last row emitted EOS: a loop that asks the
+    device only every few tokens whether every row has finished runs a few steps too many, and they only emit pad."""
+    if new.shape[1] > 1:
         is_eos = (new == eos)
         if bool(is_eos.any(dim=1).all()):
             last = int(is_eos.float().argmax(dim=1).max())        # first EOS per row; the slowest row decides
             new = new[:, :last + 1]
-    return torch.cat([input_ids.to(dev).repeat_interleave(n, dim=0), new], dim=1)
+    return new
+
+
+# ---- contrastive search (HF GenerationMixin.contrastive_search / _ranking_fast, transformers 4.28) ----
+def contrastive_search(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph, stats, dec: Decoding):
+    """Contrastive search (Su et al. 2022) over B prompts with k = ``dec.n`` candidates and alpha = ``dec.penalty_alpha``.  The
+    prefill keeps the normalised final-norm row of every prompt position as the prompt's context (``ops.contrastive_context``)
+    and the last row's logits.  A step: the processors (``dec.proc``) on the B logits rows, the k most probable tokens
+    (``ops.contrastive_topk``), the B * k candidates as one decode step over the prompt caches (each candidate's own key in its
+    one-slot cache), their final-norm rows ranked against the context (``ops.contrastive_rank``: the token, the context grows by
+    the selected row), the selected candidate's K/V committed to the prompt cache (``ops.contrastive_commit``) and the lm_head
+    on its row only.  All on the device and replayed as a CUDA graph; ids, trimming and ``stats`` as in greedy decoding."""
+    k, eos, pad, stop, proc, special = dec.n, dec.eos, dec.pad, dec.stop_on_eos, dec.proc, lm.special_ids_dev
+    timer = PhaseTimer(stats)
+    pp, st, h_all = prefill(lm, dec, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph)
+    B, H, norm_w, eps = pp.B, lm.dims.n_heads, lm.model.norm.weight.data, lm.dims.rms_eps
+    fp8_kv = llama_mod.is_fp8_kv(st.kc)
+    if proc is not None:
+        load_proc(st, input_ids, B, max_new_tokens)
+    st.finished.zero_()
+    st.pen_key.zero_()
+    st.ctx_len.zero_()
+    st.lens.copy_(torch.tensor(pp.seqlens, dtype=torch.int32).repeat_interleave(k), non_blocking=True)
+    hn_all, _ = ops.rmsnorm_fwd(h_all, norm_w, eps)
+    ops.contrastive_context(hn_all, pp.cu, st.ctx, st.ctx_len)
+
+    def head_topk(hn_rows, append=None):
+        lm_head_rows(lm, hn_rows, st.logits)
+        if proc is not None:
+            ops.logits_process_(st.logits, st.proc_ids, st.proc_width, st.proc_hist, st.proc_len, append, proc)
+        ops.contrastive_topk(st.logits, special, k, st.cand_p, st.cand_ids)
+
+    head_topk(ops.gather_rows(hn_all, pp.last_rows))
+
+    def step():
+        with ops.pdl():
+            xt = ops.embed_fwd(st.cand_ids.view(-1), lm.model.embed_tokens.weight.data)
+            h = lm.core.decode_step(xt, st.lens, st.kc, st.vc, beam=st.beam)
+            hn, _ = ops.rmsnorm_fwd(h, norm_w, eps)
+            ops.contrastive_rank(hn, st.ctx, st.ctx_len, st.pen_key, st.cand_p, st.cand_ids, dec.penalty_alpha, st.finished, eos,
+                                 pad, stop, st.next_ids, st.sel, st.hsel, st.plens, st.lens)
+            ops.contrastive_commit(st.commit_table, st.sel, st.plens, k, st.Sp, H, fp8_kv)
+            head_topk(st.hsel, append=st.next_ids)
+
+    timer.mark()                                                  # prefill_ms: the prefill and the first candidates
+    out_tokens = []
+    # every token, the first included, is a candidate step: max_new_tokens steps, timed as decode_ms
+    steps, replays = step_loop(st, step, max_new_tokens + 1, (lambda: bool(st.finished.all())) if stop else None, 8,
+                               use_cuda_graph, after=lambda: out_tokens.append(st.next_ids.clone()))
+    timer.finish(pp, steps, replays, st.Sp, contrastive_steps=steps)
+    new = (torch.stack(out_tokens, dim=1).to(torch.int64) if out_tokens else
+           torch.zeros((B, 0), dtype=torch.int64, device=lm._device()))
+    if stop:
+        new = trim_after_eos(new, eos)
+    return torch.cat([input_ids.to(lm._device()), new], dim=1)
 
 
 # ---- beam search (HF GenerationMixin.beam_search / BeamSearchScorer, transformers 4.28 as the reference pins it) ----

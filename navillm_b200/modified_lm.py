@@ -16,6 +16,7 @@ from __future__ import annotations
 
 import contextlib
 import dataclasses
+import math
 import time
 import weakref
 from types import SimpleNamespace
@@ -953,7 +954,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
                  top_p: float = 1.0, num_beams: int = 1, length_penalty: float = 1.0, early_stopping: bool = False,
                  num_return_sequences: int = 1, num_beam_groups: int = 1, repetition_penalty: Optional[float] = None,
                  no_repeat_ngram_size: Optional[int] = None, min_length: Optional[int] = None,
-                 min_new_tokens: Optional[int] = None, **unused) -> torch.Tensor:
+                 min_new_tokens: Optional[int] = None, penalty_alpha: Optional[float] = None, **unused) -> torch.Tensor:
         """Prefill on the packed kernels (positions = cumsum(mask)-1 like HF generate; visual tokens injected only
         here, as in models/modified_lm.py:195-197), then one token per step over a pre-allocated KV cache.  The
         decode step of the greedy, sampled and trie-constrained modes has static shapes and is replayed as a CUDA graph
@@ -993,7 +994,29 @@ class ModifiedLlamaForCausalLM(nn.Module):
         before the beam-score add (beams).  Their history is HF's ``input_ids``: the padded prompt row as passed, left pads
         included, then the row's (beam's, sample's) generated tokens.  They run on the device (``nv_logits_process``,
         ``nv_beam_topk_processed``) inside the captured step; values are checked as HF checks them (``ValueError``), and the
-        defaults (1.0 / None or 0) leave the call on the processor-free path."""
+        defaults (1.0 / None or 0) leave the call on the processor-free path.
+
+        ``penalty_alpha > 0`` with ``top_k > 1`` (the default 50 included), ``do_sample=False`` and ``num_beams=1`` is 4.28's
+        contrastive search: each step the ``top_k`` most probable tokens run as candidate rows over the prompt's cache, and the
+        one with the best (1 - penalty_alpha) * p - penalty_alpha * (its largest cosine similarity to the hidden states so far)
+        is kept (``generation.contrastive_search``; the context starts at the prompt's non-pad positions).  Returns [B, S0 +
+        n_new] ids like greedy decoding.  ``num_return_sequences > 1`` and a non-finite ``penalty_alpha`` raise ``ValueError``;
+        ``trie=`` / ``logits_processor=`` and ``top_k`` above ``ops.CONTRASTIVE_KMAX`` raise ``NotImplementedError``.  Every
+        other ``penalty_alpha`` (None, 0, or with ``top_k <= 1``, sampling or beams) is ignored, as in HF."""
+        contrastive = (penalty_alpha is not None and not (penalty_alpha <= 0) and top_k is not None and top_k > 1 and not do_sample
+                       and num_beams == 1 and (num_beam_groups is None or num_beam_groups <= 1))
+        if contrastive:
+            if not math.isfinite(penalty_alpha):
+                raise ValueError(f"generate(penalty_alpha={penalty_alpha!r}): has to be a finite number")
+            if num_return_sequences > 1:
+                raise ValueError(f"generate(num_return_sequences={num_return_sequences}): contrastive search returns one sequence "
+                                 "per prompt")
+            if trie is not None or logits_processor:
+                raise NotImplementedError("generate(penalty_alpha > 0) with trie= / logits_processor=: contrastive search runs "
+                                          "the device processors only")
+            if top_k > ops.CONTRASTIVE_KMAX:
+                raise NotImplementedError(f"generate(penalty_alpha > 0, top_k={top_k}): at most {ops.CONTRASTIVE_KMAX} candidates "
+                                          "per prompt are built")
         if num_beam_groups is not None and num_beam_groups > 1:
             raise NotImplementedError("generate(num_beam_groups > 1): group (diverse) beam search is not built")
         top_p = 1.0 if top_p is None else float(top_p)
@@ -1026,6 +1049,10 @@ class ModifiedLlamaForCausalLM(nn.Module):
         pad = self.tokenizer.unk_token_id if pad_token_id is None else pad_token_id
         proc = generation.processors(repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens, eos)
         call = (self, input_ids, attention_mask, (cand_vis, hist_vis, obj_vis), max_new_tokens, use_cuda_graph, stats)
+        if contrastive:
+            dec = generation.Decoding(int(eos), int(pad), bool(stop_on_eos), "contrastive", self.kv_cache_dtype, top_k=int(top_k),
+                                      n=int(top_k), proc=proc, penalty_alpha=float(penalty_alpha))
+            return generation.contrastive_search(*call, dec)
         if num_beams > 1:
             dec = generation.Decoding(int(eos), int(pad), None, "beam", self.kv_cache_dtype, n=int(num_beams), n_return=n_seq,
                                       length_penalty=float(length_penalty), early_stopping=bool(early_stopping), proc=proc)

@@ -921,6 +921,90 @@ def trie_mask(logits, out, node_ptr, child_tok, child_node, n_nodes, leaf_tok, s
     return out
 
 
+CONTRASTIVE_KMAX = 64          # candidates per prompt the contrastive-search kernels are built for
+
+
+def _dev_t(t, dtype, shape, name, what):
+    if t.dtype != dtype or tuple(t.shape) != tuple(shape) or not t.is_cuda or not t.is_contiguous():
+        raise ValueError(f"{name}: {what} {dtype} {list(shape)} contiguous on the device expected (got {t.dtype} {tuple(t.shape)})")
+
+
+def contrastive_topk(logits, special, K, p, tok):
+    """The K most probable tokens per row (nv_contrastive_topk): p = bf16(softmax(logits)) with the special ids at -inf, largest p
+    first, equal p by lower token id.  logits bf16 [B, V] (unit inner stride); writes p bf16 and tok int32 [B, K]."""
+    B, V = logits.shape
+    if logits.dtype != bf16 or logits.stride(1) != 1 or not logits.is_cuda:
+        raise ValueError(f"contrastive_topk: bf16 logits with unit inner stride on the device expected (got {logits.dtype})")
+    _dev_t(p, bf16, (B, K), "contrastive_topk", "p")
+    _dev_t(tok, torch.int32, (B, K), "contrastive_topk", "tok")
+    check(_lib.load().nv_contrastive_topk(ptr(logits), i64(logits.stride(0)), i32(V), ptr(special), i32(special.numel()), i32(K),
+                                          ptr(p), ptr(tok), i32(B), stream_ptr()), "nv_contrastive_topk")
+
+
+def contrastive_context(hn, cu, ctx, ctx_len):
+    """ctx[b, :len_b] = bf16(x / bf16(||x||)) of the packed final-norm prompt rows hn [T, D] (cu_seqlens ``cu`` int32 [B + 1]),
+    ctx_len[b] = len_b (nv_contrastive_context).  ctx bf16 [B, Sc, D]."""
+    T, D = hn.shape
+    B, Sc = ctx.shape[0], ctx.shape[1]
+    _dev_t(hn, bf16, (T, D), "contrastive_context", "hn")
+    _dev_t(ctx, bf16, (B, Sc, D), "contrastive_context", "ctx")
+    _dev_t(ctx_len, torch.int32, (B,), "contrastive_context", "ctx_len")
+    _dev_t(cu, torch.int32, (B + 1,), "contrastive_context", "cu")
+    check(_lib.load().nv_contrastive_context(ptr(hn), ptr(cu), i32(B), i32(T), ptr(ctx), ptr(ctx_len), i32(Sc), i32(D), stream_ptr()),
+          "nv_contrastive_context")
+
+
+def contrastive_rank(hn, ctx, ctx_len, pen_key, p, tok, alpha, finished, eos_id, pad_id, stop_on_eos, next_ids, sel, hsel, plens, lens,
+                     pen_out=None, score_out=None):
+    """One contrastive-search selection (nv_contrastive_rank): the candidates' final-norm rows hn bf16 [B * K, D] against the
+    context ctx bf16 [B, Sc, D] (ctx_len int32 [B] rows each), their p bf16 / tok int32 [B, K] from ``contrastive_topk`` ->
+    next_ids, sel int32 [B], finished updated, the selected row's x^ appended to ctx, the row copied to hsel bf16 [B, D], plens
+    int32 [B] and lens int32 [B * K] advanced.  pen_key int32 [B * K] zero before and after; pen_out / score_out fp32 [B, K]."""
+    B, K = p.shape
+    Sc, D = ctx.shape[1], ctx.shape[2]
+    name = "contrastive_rank"
+    _dev_t(hn, bf16, (B * K, D), name, "hn")
+    _dev_t(ctx, bf16, (B, Sc, D), name, "ctx")
+    _dev_t(hsel, bf16, (B, D), name, "hsel")
+    _dev_t(p, bf16, (B, K), name, "p")
+    for what, t, n in (("ctx_len", ctx_len, B), ("pen_key", pen_key, B * K), ("finished", finished, B), ("next_ids", next_ids, B),
+                       ("sel", sel, B), ("plens", plens, B), ("lens", lens, B * K)):
+        _dev_t(t, torch.int32, (n,), name, what)
+    _dev_t(tok, torch.int32, (B, K), name, "tok")
+    for what, t in (("pen_out", pen_out), ("score_out", score_out)):
+        if t is not None:
+            _dev_t(t, torch.float32, (B, K), name, what)
+    check(_lib.load().nv_contrastive_rank(ptr(hn), ptr(ctx), ptr(ctx_len), i32(Sc), i32(D), i32(K), ptr(pen_key), ptr(p), ptr(tok),
+                                          ctypes.c_double(alpha), ptr(finished), i32(eos_id), i32(pad_id), i32(1 if stop_on_eos else 0),
+                                          ptr(next_ids), ptr(sel), ptr(hsel), ptr(plens), ptr(lens), ptr(pen_out), ptr(score_out), i32(B),
+                                          stream_ptr()), "nv_contrastive_rank")
+
+
+def contrastive_commit_table(kc, vc, pk, pv) -> torch.Tensor:
+    """The per-layer pointer table of ``contrastive_commit`` for the candidate caches kc / vc [B * K, 1, D] and the prompt caches
+    pk / pv [B, Sp, D] (bf16 tensors, or ``(e4m3, exponents)`` pairs per layer): int64 [L, 8] on the device."""
+    rows = []
+    for layer in zip(kc, vc, pk, pv):
+        if isinstance(layer[0], tuple):
+            rows.append([c[0].data_ptr() for c in layer] + [c[1].data_ptr() for c in layer])
+        else:
+            rows.append([c.data_ptr() for c in layer] + [0] * 4)
+    dev = (kc[0][0] if isinstance(kc[0], tuple) else kc[0]).device
+    return torch.tensor(rows, dtype=torch.int64).to(dev)
+
+
+def contrastive_commit(table, sel, plens, K, Sp, n_heads, fp8):
+    """The selected candidate's K / V rows of every layer into row plens[b] - 1 of the prompt caches (nv_contrastive_commit);
+    ``table`` from ``contrastive_commit_table`` (the tensors behind it must outlive the call)."""
+    B = sel.numel()
+    _dev_t(sel, torch.int32, (B,), "contrastive_commit", "sel")
+    _dev_t(plens, torch.int32, (B,), "contrastive_commit", "plens")
+    if table.dtype != torch.int64 or table.dim() != 2 or table.shape[1] != 8 or not table.is_cuda:
+        raise ValueError("contrastive_commit: an int64 [L, 8] pointer table on the device expected")
+    check(_lib.load().nv_contrastive_commit(ptr(table), i32(table.shape[0]), ptr(sel), ptr(plens), i32(K), i32(Sp), i32(n_heads * 128),
+                                            i32(n_heads), i32(1 if fp8 else 0), i32(B), stream_ptr()), "nv_contrastive_commit")
+
+
 class LayerRunner:
     """Inference forward of decoder layers through nv_llama_layer_infer (csrc/layer.cu): ONE C-ABI call per layer instead of
     ten.  Holds the argument block and a workspace for a given packing; ``run`` fills in what changes per layer."""
