@@ -375,6 +375,32 @@ int nv_contrastive_rank(const void* hn, void* ctx, int* ctx_len, int Sc, int D, 
                         void* hsel, int* plens, int* lens, float* pen_out, float* score_out, int B, void* stream);
 int nv_contrastive_commit(const unsigned long long* table, int L, const int* sel, const int* plens, int K, int Sp, int D, int H,
                           int fp8, int B, void* stream);
+/* Prompt-lookup speculative decoding (greedy generate(prompt_lookup_num_tokens=K), K = 1..15, window W = K + 1 rows per prompt).
+ * nv_decode_attn_rope_window[_fp8]: nv_decode_attn_rope[_fp8] for W consecutive new tokens per sequence, qkv row b * W + r
+ * (pre-RoPE) at position lens[b] + r: the rotated k and the v of every row are stored (fp8: quantized) at rows lens[b] .. lens[b]
+ * + W - 1, and query r attends over keys 0 .. lens[b] + r.  Query r's output and every cache byte equal those of W sequential
+ * nv_decode_attn_rope[_fp8] calls at lens[b] + r.  A cached key is read once per 8 queries.  1 <= W <= 16; sizes and alignment as
+ * nv_decode_attn_rope[_fp8], ldo % 8 == 0.
+ * nv_lookup_draft: one CTA per row, HF's PromptLookupCandidateGenerator (max_matching_ngram_size = ngram) on the row's history
+ * hist[b, 0 .. hist_len[b]) (int32, row stride ld_hist): the earliest earlier occurrence of its last n tokens, n = ngram down to
+ * 1, proposes the up to K tokens after it, cut at the history's end and at the first special id or eos_id.  drafts [B, K] (-1
+ * past the drafts) and win_ids [B, W] (the history's last token, the drafts, the last token again for a missing draft); a
+ * finished row gets none.
+ * nv_lookup_accept: one CTA per row; t_j = nv_argmax_masked's pick of logits row b * W + j, taken while drafts[b, j - 1] = t_{j-1}.
+ * The row emits t_0 .. t_m (m accepted drafts), cut after EOS (stop_on_eos) and at max_new tokens, into out[b, n_out[b] ..]
+ * (row stride ld_out >= max_new) and hist[b, hist_len[b] ..]; n_out, hist_len and lens[b] advance by the tokens emitted, n_acc by
+ * the accepted drafts among them.  A row that emitted EOS or max_new tokens is finished and emits nothing more. */
+int nv_decode_attn_rope_window(const void* qkv, int64_t ld, const int* lens, const void* cos_t, const void* sin_t, void* kcache,
+                               void* vcache, void* out, int64_t ldo, int B, int W, int Smax, int H, int head_dim, float scale,
+                               void* stream);
+int nv_decode_attn_rope_window_fp8(const void* qkv, int64_t ld, const int* lens, const void* cos_t, const void* sin_t, void* kq,
+                                   void* vq, void* kexp, void* vexp, void* out, int64_t ldo, int B, int W, int Smax, int H,
+                                   int head_dim, float scale, void* stream);
+int nv_lookup_draft(const int* hist, int ld_hist, const int* hist_len, const int* finished, const int* special, int n_special,
+                    int eos_id, int K, int ngram, int* drafts, int* win_ids, int B, void* stream);
+int nv_lookup_accept(const void* logits, int64_t ld, int V, const int* special, int n_special, const int* drafts, int K, int* finished,
+                     int eos_id, int stop_on_eos, int max_new, int* out, int ld_out, int* hist, int ld_hist, int* hist_len, int* n_out,
+                     int* lens, int* n_acc, int B, void* stream);
 /* at most 64 special ids (n_special), here and in nv_sample_topk; longer lists return NV_ERR_BAD_ARG */
 int nv_argmax_masked(const void* logits, int64_t ld, int V, const int* special, int n_special, int* finished, int eos_id,
                      int pad_id, int stop_on_eos, int* next, int B, void* stream);

@@ -10,6 +10,7 @@
 // Opt-in fp8 cache (nv_kv_store_prefill_fp8, nv_decode_attn_rope_fp8, nv_kv_store_suffix_fp8): the same layout in e4m3 bytes
 // plus one int8 exponent per (sequence, position, head) row of 128 elements, quantized with the weight format of nv_fp8.cuh as
 // rows are stored.
+#include <climits>
 #include <type_traits>
 
 #include "nv_common.cuh"
@@ -159,6 +160,29 @@ __global__ void decode_rope_kv_kernel(__nv_bfloat16* __restrict__ qkv, int64_t l
   }
 }
 
+// Rotary embedding of the chunk pair (c * 8 .. c * 8 + 7, 64 + c * 8 ..) of one pre-RoPE head row at position p, with the
+// rounding points of rope_kernel: o1 / o2 are the rotated bf16 chunks.
+__device__ __forceinline__ void rope_chunk(const __nv_bfloat16* base, const __nv_bfloat16* __restrict__ cos_t,
+                                           const __nv_bfloat16* __restrict__ sin_t, int p, int c, uint4& o1, uint4& o2) {
+  float x1[8], x2[8], c1[8], s1[8], c2[8], s2[8];
+  unpack8d(*reinterpret_cast<const uint4*>(base + c * 8), x1);
+  unpack8d(*reinterpret_cast<const uint4*>(base + 64 + c * 8), x2);
+  unpack8d(*reinterpret_cast<const uint4*>(cos_t + (int64_t)p * 128 + c * 8), c1);
+  unpack8d(*reinterpret_cast<const uint4*>(sin_t + (int64_t)p * 128 + c * 8), s1);
+  unpack8d(*reinterpret_cast<const uint4*>(cos_t + (int64_t)p * 128 + 64 + c * 8), c2);
+  unpack8d(*reinterpret_cast<const uint4*>(sin_t + (int64_t)p * 128 + 64 + c * 8), s2);
+  uint32_t* q1 = &o1.x; uint32_t* q2 = &o2.x;
+#pragma unroll
+  for (int j = 0; j < 8; j += 2) {
+    const float a0 = bf16_round(x1[j] * c1[j]) + bf16_round(-x2[j] * s1[j]);
+    const float a1 = bf16_round(x1[j + 1] * c1[j + 1]) + bf16_round(-x2[j + 1] * s1[j + 1]);
+    const float b0 = bf16_round(x2[j] * c2[j]) + bf16_round(x1[j] * s2[j]);
+    const float b1 = bf16_round(x2[j + 1] * c2[j + 1]) + bf16_round(x1[j + 1] * s2[j + 1]);
+    q1[j >> 1] = pack_bf16x2(a0, a1);
+    q2[j >> 1] = pack_bf16x2(b0, b1);
+  }
+}
+
 // One new query per sequence over its cache (keys 0..lens[b], the new token included: call after append).
 // CTA = (b, h), DA_WARPS warps; half-warps stream keys with 16-byte loads; per-warp online softmax, merged in smem.
 // (8 warps: 256 (b, h) CTAs of 4 warps kept too few loads in flight for a 50 MB cache read; all CTAs are co-resident.)
@@ -220,24 +244,8 @@ __global__ void __launch_bounds__(DA_WARPS * 32) decode_attn_kernel(const __nv_b
       if (lane < 16) {                                  // lanes 0..7: q chunk c, lanes 8..15: k chunk c
         const int c = lane & 7, is_k = lane >> 3;
         const __nv_bfloat16* base = q + (int64_t)b * ldq + (is_k ? HD : 0) + h * 128;
-        float x1[8], x2[8], c1[8], s1[8], c2[8], s2[8];
-        unpack8d(*reinterpret_cast<const uint4*>(base + c * 8), x1);
-        unpack8d(*reinterpret_cast<const uint4*>(base + 64 + c * 8), x2);
-        unpack8d(*reinterpret_cast<const uint4*>(cos_t + (int64_t)p * 128 + c * 8), c1);
-        unpack8d(*reinterpret_cast<const uint4*>(sin_t + (int64_t)p * 128 + c * 8), s1);
-        unpack8d(*reinterpret_cast<const uint4*>(cos_t + (int64_t)p * 128 + 64 + c * 8), c2);
-        unpack8d(*reinterpret_cast<const uint4*>(sin_t + (int64_t)p * 128 + 64 + c * 8), s2);
         uint4 o1, o2;
-        uint32_t* q1 = &o1.x; uint32_t* q2 = &o2.x;
-#pragma unroll
-        for (int j = 0; j < 8; j += 2) {
-          const float a0 = bf16_round(x1[j] * c1[j]) + bf16_round(-x2[j] * s1[j]);
-          const float a1 = bf16_round(x1[j + 1] * c1[j + 1]) + bf16_round(-x2[j + 1] * s1[j + 1]);
-          const float b0 = bf16_round(x2[j] * c2[j]) + bf16_round(x1[j] * s2[j]);
-          const float b1 = bf16_round(x2[j + 1] * c2[j + 1]) + bf16_round(x1[j + 1] * s2[j + 1]);
-          q1[j >> 1] = pack_bf16x2(a0, a1);
-          q2[j >> 1] = pack_bf16x2(b0, b1);
-        }
+        rope_chunk(base, cos_t, sin_t, p, c, o1, o2);
         if (!is_k) {
           s_q[c] = o1; s_q[8 + c] = o2;
         } else if constexpr (FP8) {
@@ -415,28 +423,255 @@ __global__ void __launch_bounds__(DA_WARPS * 32) decode_attn_kernel(const __nv_b
   }
 }
 
+// ---- speculative verify step: w consecutive query rows per sequence (prompt-lookup decoding) ----
+// decode_attn_kernel<true, FP8> for a window of W <= WIN_MAX new tokens per sequence: qkv row b * W + r (pre-RoPE) is the token at
+// position lens[b] + r.  Every CTA rotates the q, k and v of the window rows its queries see into shared memory, stores the
+// rotated k and the v of its own query rows at rows lens[b] + r of the caches (fp8: quantized as the decode kernel quantizes
+// them), and query r attends over keys 0 .. lens[b] + r: cached keys from global memory, the window's from shared memory.  A
+// cached key is read once for the QPC queries of the CTA; grid (B * H, ceil(W / QPC)), so a window of more than QPC rows reads
+// the cache once per QPC queries (the second read mostly from L2).
+// Bit-identity: for each query the keys go to warps and half-warps by absolute index and the per-warp states merge in warp
+// order, exactly as in decode_attn_kernel at lens[b] + r; a key past a query's range leaves its (m, l, acc) unchanged (the
+// correction factor is exp2(0) = 1, and no term is added), so query r's output and every cache byte equal those of W
+// sequential decode_attn_rope calls.  The arithmetic is spelled out with _rn intrinsics in the order ptxas gives
+// decode_attn_kernel (fma dot products from 0, the rescale a separate multiply, p * v fused into the sum, the merges as
+// fma(x, a, y * ao)), so that no contraction choice can differ between the two kernels.
+constexpr int WIN_MAX = 16;
+
+template <bool FP8, int QPC>
+__global__ void __launch_bounds__(DA_WARPS * 32) decode_attn_window_kernel(const __nv_bfloat16* __restrict__ qkv, int64_t ld,
+                                                                           kv_elem_t<FP8>* __restrict__ kc, kv_elem_t<FP8>* __restrict__ vc,
+                                                                           int8_t* __restrict__ ke, int8_t* __restrict__ ve,
+                                                                           const int* __restrict__ lens, __nv_bfloat16* __restrict__ out,
+                                                                           int64_t ldo, int Smax, int H, int W, float scale,
+                                                                           const __nv_bfloat16* __restrict__ cos_t,
+                                                                           const __nv_bfloat16* __restrict__ sin_t) {
+  using raw_t = typename std::conditional<FP8, uint2, uint4>::type;
+  __shared__ float s_m[QPC][DA_WARPS], s_l[QPC][DA_WARPS];
+  __shared__ float s_acc[QPC][DA_WARPS][128];
+  __shared__ uint4 s_q[QPC][16];                       // rotated q of the CTA's queries (bf16 x 128)
+  __shared__ raw_t s_kw[WIN_MAX][16], s_vw[WIN_MAX][16];   // the window's K / V rows as the cache holds them
+  __shared__ int s_kx[WIN_MAX], s_vx[WIN_MAX];         // FP8: their exponents
+  griddep_launch();
+  griddep_wait();
+  const int b = blockIdx.x / H, h = blockIdx.x % H;
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int half = lane >> 4, hl = lane & 15;
+  const int HD = H * 128;
+  const int L = lens[b];
+  const int q0 = blockIdx.y * QPC, qe = min(W, q0 + QPC);   // this CTA's queries q0 .. qe - 1
+  // rotate: warp w takes window rows w, w + 8, ..; lanes 0..7 the q chunk pairs, 8..15 the k chunk pairs, 16..31 the v chunks
+  for (int r = w; r < qe; r += DA_WARPS) {
+    const int p = L + r;
+    const __nv_bfloat16* row = qkv + (int64_t)(b * W + r) * ld;
+    const bool store = r >= q0 && p < Smax;            // this CTA writes the K / V of its own query rows
+    uint4 r0 = make_uint4(0, 0, 0, 0), r1 = r0;
+    if (lane < 16) {
+      const int c = lane & 7, is_k = lane >> 3;
+      if (is_k || r >= q0) {
+        rope_chunk(row + (is_k ? HD : 0) + h * 128, cos_t, sin_t, p, c, r0, r1);
+        if (!is_k) {
+          s_q[r - q0][c] = r0; s_q[r - q0][8 + c] = r1;
+        } else if constexpr (!FP8) {
+          s_kw[r][c] = r0; s_kw[r][8 + c] = r1;
+          if (store) {
+            __nv_bfloat16* dst = kc + ((int64_t)b * Smax + p) * HD + h * 128;
+            *reinterpret_cast<uint4*>(dst + c * 8) = r0;
+            *reinterpret_cast<uint4*>(dst + 64 + c * 8) = r1;
+          }
+        }
+      }
+    } else {
+      r0 = *reinterpret_cast<const uint4*>(row + 2 * HD + h * 128 + (lane - 16) * 8);
+      if constexpr (!FP8) {
+        s_vw[r][lane - 16] = r0;
+        if (store) *reinterpret_cast<uint4*>(vc + ((int64_t)b * Smax + p) * HD + h * 128 + (lane - 16) * 8) = r0;
+      }
+    }
+    if constexpr (FP8) {
+      // the row amax and exponent of the k row (lanes 8..15) and the v row (16..31), as decode_attn_kernel finds them
+      if (lane < 8) r0 = r1 = make_uint4(0, 0, 0, 0);
+      uint32_t m = max(bf16x8_amax_bits(r0), bf16x8_amax_bits(r1));
+#pragma unroll
+      for (int o = 1; o < 8; o <<= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+      const uint32_t m8 = __shfl_xor_sync(0xffffffffu, m, 8);
+      if (lane >= 16) m = max(m, m8);
+      const int e = fp8_row_exponent(__uint_as_float(m << 16));
+      const float inv = fp8_pow2(-e);
+      const int64_t crow = (int64_t)b * Smax + p;
+      if (lane >= 8 && lane < 16) {
+        const int c = lane & 7;
+        const uint2 k0 = fp8x8_from_bf16x8(r0, inv), k1 = fp8x8_from_bf16x8(r1, inv);
+        s_kw[r][c] = k0; s_kw[r][8 + c] = k1;
+        if (lane == 8) s_kx[r] = e;
+        if (store) {
+          *reinterpret_cast<uint2*>(kc + crow * HD + h * 128 + c * 8) = k0;
+          *reinterpret_cast<uint2*>(kc + crow * HD + h * 128 + 64 + c * 8) = k1;
+          if (lane == 8) ke[crow * H + h] = (int8_t)e;
+        }
+      } else if (lane >= 16) {
+        const uint2 v0 = fp8x8_from_bf16x8(r0, inv);
+        s_vw[r][lane - 16] = v0;
+        if (lane == 16) s_vx[r] = e;
+        if (store) {
+          *reinterpret_cast<uint2*>(vc + crow * HD + h * 128 + (lane - 16) * 8) = v0;
+          if (lane == 16) ve[crow * H + h] = (int8_t)e;
+        }
+      }
+    }
+  }
+  __syncthreads();
+  const int nq = qe - q0;
+  const int n = L + qe;                                 // keys the CTA's last query sees
+  const float sl2 = scale * 1.4426950408889634f;
+  float m[QPC], l[QPC], acc[QPC][8];
+#pragma unroll
+  for (int qi = 0; qi < QPC; ++qi) {
+    m[qi] = -INFINITY; l[qi] = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) acc[qi][i] = 0.f;
+  }
+  constexpr int KPI = 4;
+  auto load_keys = [&](int jb, raw_t (&kr)[KPI], raw_t (&vr)[KPI], int (&kx)[KPI], int (&vx)[KPI]) {
+#pragma unroll
+    for (int u = 0; u < KPI; ++u) {
+      const int j = jb + u;
+      if (j < L) {
+        const int64_t row = (int64_t)b * Smax + j;
+        const int64_t off = row * HD + h * 128 + hl * 8;
+        kr[u] = *reinterpret_cast<const raw_t*>(kc + off);
+        vr[u] = *reinterpret_cast<const raw_t*>(vc + off);
+        if constexpr (FP8) {
+          kx[u] = ke[row * H + h];
+          vx[u] = ve[row * H + h];
+        }
+      } else if (j < n) {
+        kr[u] = s_kw[j - L][hl];
+        vr[u] = s_vw[j - L][hl];
+        if constexpr (FP8) {
+          kx[u] = s_kx[j - L];
+          vx[u] = s_vx[j - L];
+        }
+      } else {
+        if constexpr (FP8) {
+          kr[u] = make_uint2(0, 0);
+          vr[u] = make_uint2(0, 0);
+          kx[u] = vx[u] = 0;
+        } else {
+          kr[u] = make_uint4(0, 0, 0, 0);
+          vr[u] = make_uint4(0, 0, 0, 0);
+        }
+      }
+    }
+  };
+  auto unpack = [&](const raw_t& r, int x, float (&f)[8]) {
+    if constexpr (FP8) unpack8q(r, x, f);
+    else unpack8d(r, f);
+  };
+  raw_t knext[KPI], vnext[KPI];
+  int kxnext[KPI], vxnext[KPI];
+  load_keys(w * 2 * KPI + half * KPI, knext, vnext, kxnext, vxnext);
+  for (int j0 = w * 2 * KPI; j0 < n; j0 += DA_WARPS * 2 * KPI) {
+    const int jb = j0 + half * KPI;
+    raw_t kraw[KPI], vraw[KPI];
+    int kx[KPI], vx[KPI];
+#pragma unroll
+    for (int u = 0; u < KPI; ++u) { kraw[u] = knext[u]; vraw[u] = vnext[u]; kx[u] = kxnext[u]; vx[u] = vxnext[u]; }
+    if (j0 + DA_WARPS * 2 * KPI < n) load_keys(jb + DA_WARPS * 2 * KPI, knext, vnext, kxnext, vxnext);
+#pragma unroll
+    for (int qi = 0; qi < QPC; ++qi) {
+      if (qi < nq) {                                    // uniform over the CTA
+        const int nk = L + q0 + qi + 1;                 // keys visible to this query
+        float qf[8];
+        unpack8d(s_q[qi][hl], qf);
+        float sc[KPI];
+#pragma unroll
+        for (int u = 0; u < KPI; ++u) {
+          float kf[8];
+          unpack(kraw[u], kx[u], kf);
+          float s = 0.f;
+#pragma unroll
+          for (int i = 0; i < 8; ++i) s = __fmaf_rn(qf[i], kf[i], s);
+          sc[u] = s;
+        }
+#pragma unroll
+        for (int o = 8; o > 0; o >>= 1)
+#pragma unroll
+          for (int u = 0; u < KPI; ++u) sc[u] += __shfl_xor_sync(0xffffffffu, sc[u], o);
+        float mn = m[qi];
+#pragma unroll
+        for (int u = 0; u < KPI; ++u)
+          if (jb + u < nk) mn = fmaxf(mn, sc[u]);
+        if (mn != -INFINITY) {
+          const float a = exp2f(__fmul_rn(__fsub_rn(m[qi], mn), sl2));
+          l[qi] = __fmul_rn(l[qi], a);
+#pragma unroll
+          for (int i = 0; i < 8; ++i) acc[qi][i] = __fmul_rn(acc[qi][i], a);
+#pragma unroll
+          for (int u = 0; u < KPI; ++u) {
+            if (jb + u < nk) {
+              const float p = exp2f(__fmul_rn(__fsub_rn(sc[u], mn), sl2));
+              float vf[8];
+              unpack(vraw[u], vx[u], vf);
+              l[qi] = __fadd_rn(l[qi], p);
+#pragma unroll
+              for (int i = 0; i < 8; ++i) acc[qi][i] = __fmaf_rn(p, vf[i], acc[qi][i]);
+            }
+          }
+          m[qi] = mn;
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int qi = 0; qi < QPC; ++qi) {
+    if (qi < nq) {
+      const float mo = __shfl_xor_sync(0xffffffffu, m[qi], 16), lo = __shfl_xor_sync(0xffffffffu, l[qi], 16);
+      const float mn = fmaxf(m[qi], mo);
+      const float a = (m[qi] == -INFINITY) ? 0.f : exp2f(__fmul_rn(__fsub_rn(m[qi], mn), sl2));
+      const float ao = (mo == -INFINITY) ? 0.f : exp2f(__fmul_rn(__fsub_rn(mo, mn), sl2));
+      l[qi] = __fmaf_rn(l[qi], a, __fmul_rn(lo, ao));
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const float other = __shfl_xor_sync(0xffffffffu, acc[qi][i], 16);
+        acc[qi][i] = __fmaf_rn(acc[qi][i], a, __fmul_rn(other, ao));
+      }
+      m[qi] = mn;
+      if (lane < 16) {
+        if (lane == 0) { s_m[qi][w] = m[qi]; s_l[qi][w] = l[qi]; }
+#pragma unroll
+        for (int i = 0; i < 8; ++i) s_acc[qi][w][hl * 8 + i] = acc[qi][i];
+      }
+    }
+  }
+  __syncthreads();
+  for (int idx = threadIdx.x; idx < nq * 128; idx += DA_WARPS * 32) {
+    const int qi = idx >> 7, d = idx & 127;
+    float mm = s_m[qi][0];
+#pragma unroll
+    for (int k = 1; k < DA_WARPS; ++k) mm = fmaxf(mm, s_m[qi][k]);
+    float num = 0.f, den = 0.f;
+#pragma unroll
+    for (int k = 0; k < DA_WARPS; ++k) {
+      const float a = (s_m[qi][k] == -INFINITY) ? 0.f : exp2f(__fmul_rn(__fsub_rn(s_m[qi][k], mm), sl2));
+      num = __fmaf_rn(s_acc[qi][k][d], a, num);
+      den = __fmaf_rn(s_l[qi][k], a, den);
+    }
+    out[(int64_t)(b * W + q0 + qi) * ldo + h * 128 + d] = __float2bfloat16_rn(num / den);
+  }
+}
+
 // Special ids masked by argmax_kernel and sample_topk_kernel: they are staged in shared memory, so the host entry points
 // reject longer lists.
 constexpr int MAX_SPECIAL = 64;
 
-// next[b] = finished[b] ? pad_id : argmax_c logits[b,c] over non-special columns (first index wins ties, like
-// torch.argmax); finished[b] |= next == eos (when stop_on_eos).  One CTA per row.
-__global__ void __launch_bounds__(1024) argmax_kernel(const __nv_bfloat16* __restrict__ logits, int64_t ld, int V,
-                                                      const int* __restrict__ special, int n_special,
-                                                      int* __restrict__ finished, int eos_id, int pad_id, int stop_on_eos,
-                                                      int* __restrict__ next) {
-  __shared__ float sv[32];
-  __shared__ int si[32];
-  __shared__ int s_special[MAX_SPECIAL];
-  griddep_launch();
-  griddep_wait();
-  const int b = blockIdx.x;
-  const int ns = n_special;
-  if (threadIdx.x < ns) s_special[threadIdx.x] = special[threadIdx.x];
-  __syncthreads();
+// The masked argmax of one logits row over the whole CTA (s_special: the n_special special ids, already in shared memory;
+// sv / si: 32 floats / ints of shared scratch): the first index of the largest value over non-special columns, like
+// torch.argmax.  Valid in thread 0.
+__device__ __forceinline__ int argmax_row(const __nv_bfloat16* __restrict__ row, int64_t ld, int V, const int* s_special, int ns,
+                                          float* sv, int* si) {
   float best = -INFINITY;
   int bi = V;
-  const __nv_bfloat16* row = logits + (int64_t)b * ld;
   const bool vec_ok = (ld & 7) == 0;                       // 16-byte aligned rows
   const int nvec = vec_ok ? (V >> 3) : 0;
   for (int v = threadIdx.x; v < nvec; v += blockDim.x) {
@@ -476,12 +711,146 @@ __global__ void __launch_bounds__(1024) argmax_kernel(const __nv_bfloat16* __res
       const int i2 = __shfl_xor_sync(0xffffffffu, bi, o);
       if (v2 > best || (v2 == best && i2 < bi)) { best = v2; bi = i2; }
     }
-    if (lane == 0) {
-      int tok = bi;
-      if (finished[b]) tok = pad_id;
-      else if (stop_on_eos && tok == eos_id) finished[b] = 1;
-      next[b] = tok;
+  }
+  return bi;
+}
+
+// next[b] = finished[b] ? pad_id : argmax_c logits[b,c] over non-special columns (first index wins ties, like
+// torch.argmax); finished[b] |= next == eos (when stop_on_eos).  One CTA per row.
+__global__ void __launch_bounds__(1024) argmax_kernel(const __nv_bfloat16* __restrict__ logits, int64_t ld, int V,
+                                                      const int* __restrict__ special, int n_special,
+                                                      int* __restrict__ finished, int eos_id, int pad_id, int stop_on_eos,
+                                                      int* __restrict__ next) {
+  __shared__ float sv[32];
+  __shared__ int si[32];
+  __shared__ int s_special[MAX_SPECIAL];
+  griddep_launch();
+  griddep_wait();
+  const int b = blockIdx.x;
+  const int ns = n_special;
+  if (threadIdx.x < ns) s_special[threadIdx.x] = special[threadIdx.x];
+  __syncthreads();
+  const int bi = argmax_row(logits + (int64_t)b * ld, ld, V, s_special, ns, sv, si);
+  if (threadIdx.x == 0) {
+    int tok = bi;
+    if (finished[b]) tok = pad_id;
+    else if (stop_on_eos && tok == eos_id) finished[b] = 1;
+    next[b] = tok;
+  }
+}
+
+// ---- prompt-lookup drafts and their verification (generation.lookup_decode) ----
+constexpr int LD_THREADS = 128;
+
+// One CTA per row: HF's PromptLookupCandidateGenerator on the row's history hist[b, :hist_len[b]] (its non-pad prompt ids, then
+// its generated tokens).  For n = min(ngram, len - 1) down to 1, the earliest i with hist[i .. i + n) equal to the last n tokens
+// and i + n < len: the drafts are the up to K tokens from i + n on, cut at the end of the history and at the first special id or
+// EOS (the argmax never accepts a special id; HF cuts at EOS); the first n that matches decides, even if its drafts come out
+// empty.  drafts [B, K] = the drafts, -1 past them; win [B, K + 1] = the verify window's ids: the last token, then the drafts,
+// then the last token again in place of a missing draft (any valid id: its row's argmax is never looked at).  A finished row
+// gets no drafts.
+__global__ void __launch_bounds__(LD_THREADS) lookup_draft_kernel(const int* __restrict__ hist, int ld_hist,
+                                                                  const int* __restrict__ hist_len, const int* __restrict__ finished,
+                                                                  const int* __restrict__ special, int n_special, int eos_id, int K,
+                                                                  int ngram, int* __restrict__ drafts, int* __restrict__ win) {
+  __shared__ int s_special[MAX_SPECIAL];
+  __shared__ int s_best;
+  griddep_launch();
+  griddep_wait();
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int* row = hist + (int64_t)b * ld_hist;
+  const int L = hist_len[b];
+  const bool live = !finished[b];
+  if (tid < n_special) s_special[tid] = special[tid];
+  int start = -1;
+  for (int n = live ? min(ngram, L - 1) : 0; n >= 1; --n) {  // uniform over the CTA
+    __syncthreads();                                         // s_best of the previous n is read
+    if (tid == 0) s_best = INT_MAX;
+    __syncthreads();
+    for (int i = tid; i + n < L; i += LD_THREADS) {
+      bool match = true;
+      for (int t = 0; t < n && match; ++t) match = row[i + t] == row[L - n + t];
+      if (match) atomicMin(&s_best, i);
     }
+    __syncthreads();
+    if (s_best != INT_MAX) {
+      start = s_best + n;
+      break;
+    }
+  }
+  __syncthreads();
+  if (tid == 0) {
+    const int last = row[L - 1];
+    win[b * (K + 1)] = last;
+    bool go = start >= 0;
+    for (int i = 0; i < K; ++i) {
+      int tok = -1;
+      if (go && start + i < L) {
+        tok = row[start + i];
+        bool sp = tok == eos_id;
+        for (int s = 0; s < n_special; ++s) sp |= s_special[s] == tok;
+        if (sp) tok = -1;
+      }
+      go = tok >= 0;
+      drafts[b * K + i] = tok;
+      win[b * (K + 1) + 1 + i] = go ? tok : last;
+    }
+  }
+}
+
+// One CTA per row of a verify window (K + 1 logits rows b * (K + 1) + j, row j the prediction after window token j): t_j = the
+// masked argmax of row j (argmax_kernel's rule), computed for j = 0, 1, .. while draft d_{j+1} = drafts[b, j] equals t_j.  The row
+// emits t_0 .. t_m (m accepted drafts), cut after the first EOS when stop_on_eos and at max_new tokens: each goes to out[b, n_out[b]]
+// and to the history.  lens[b] advances by the tokens emitted (the window rows whose K / V are now valid), n_acc[b] by the
+// accepted drafts among them, and a row that emitted EOS or reached max_new is finished: it emits nothing more.
+__global__ void __launch_bounds__(1024) lookup_accept_kernel(const __nv_bfloat16* __restrict__ logits, int64_t ld, int V,
+                                                             const int* __restrict__ special, int n_special,
+                                                             const int* __restrict__ drafts, int K, int* __restrict__ finished,
+                                                             int eos_id, int stop_on_eos, int max_new, int* __restrict__ out,
+                                                             int ld_out, int* __restrict__ hist, int ld_hist,
+                                                             int* __restrict__ hist_len, int* __restrict__ n_out,
+                                                             int* __restrict__ lens, int* __restrict__ n_acc) {
+  __shared__ float sv[32];
+  __shared__ int si[32];
+  __shared__ int s_special[MAX_SPECIAL];
+  __shared__ int s_t[WIN_MAX];
+  __shared__ int s_more;
+  griddep_launch();
+  griddep_wait();
+  const int b = blockIdx.x;
+  if (finished[b]) return;                                   // uniform over the CTA
+  if (threadIdx.x < n_special) s_special[threadIdx.x] = special[threadIdx.x];
+  __syncthreads();
+  int m = 0;
+  for (int j = 0; j <= K; ++j) {
+    const int t = argmax_row(logits + (int64_t)(b * (K + 1) + j) * ld, ld, V, s_special, n_special, sv, si);
+    if (threadIdx.x == 0) {
+      s_t[j] = t;
+      s_more = j < K && drafts[b * K + j] == t;
+    }
+    __syncthreads();
+    m = j;
+    if (!s_more) break;
+    __syncthreads();                                         // sv / si and s_more are read before the next row
+  }
+  if (threadIdx.x == 0) {
+    int cnt = n_out[b], hl = hist_len[b], e = 0;
+    bool fin = false;
+    for (int j = 0; j <= m && cnt < max_new; ++j) {
+      const int tok = s_t[j];
+      out[(int64_t)b * ld_out + cnt++] = tok;
+      hist[(int64_t)b * ld_hist + hl++] = tok;
+      ++e;
+      if (stop_on_eos && tok == eos_id) {
+        fin = true;
+        break;
+      }
+    }
+    n_out[b] = cnt;
+    hist_len[b] = hl;
+    lens[b] += e;
+    n_acc[b] += e > 0 ? e - 1 : 0;
+    if (fin || cnt >= max_new) finished[b] = 1;
   }
 }
 
@@ -1599,6 +1968,37 @@ using namespace nv;
 #define BF(x) reinterpret_cast<__nv_bfloat16*>(x)
 #define CBF(x) reinterpret_cast<const __nv_bfloat16*>(x)
 
+// Prompt-lookup speculative decoding (generation.lookup_decode): the verify window's attention, the drafts and the accept step.
+template <bool FP8>
+static int launch_window(const char* name, const void* qkv, int64_t ld, const int* lens, const void* cos_t, const void* sin_t,
+                         void* kc, void* vc, void* kexp, void* vexp, void* out, int64_t ldo, int B, int W, int Smax, int H,
+                         int head_dim, float scale, void* stream) {
+  NV_REQUIRE(head_dim == 128 && (ld & 7) == 0 && (ldo & 7) == 0, "%s: head_dim must be 128, ld %% 8 == 0, ldo %% 8 == 0", name);
+  NV_REQUIRE(B >= 0 && W >= 1 && W <= WIN_MAX && Smax > 0 && H > 0, "%s: bad sizes (B=%d W=%d Smax=%d H=%d; 1 <= W <= %d)", name, B,
+             W, Smax, H, WIN_MAX);
+  if (B == 0) return NV_OK;
+  NV_REQUIRE(qkv && lens && cos_t && sin_t && kc && vc && out && (!FP8 || (kexp && vexp)), "%s: null argument", name);
+  NV_REQUIRE(((uintptr_t)qkv & 15) == 0 && ((uintptr_t)kc & 7) == 0 && ((uintptr_t)vc & 7) == 0, "%s: alignment", name);
+  using E = kv_elem_t<FP8>;
+  E* k = reinterpret_cast<E*>(kc);
+  E* v = reinterpret_cast<E*>(vc);
+  int8_t* kx = reinterpret_cast<int8_t*>(kexp);
+  int8_t* vx = reinterpret_cast<int8_t*>(vexp);
+  // the fewest queries per CTA that hold the window, at most 8 (the registers of 8 queries' states next to the loads in flight)
+  const int qpc = W <= 2 ? 2 : W <= 4 ? 4 : 8;
+  const dim3 grid(B * H, (W + qpc - 1) / qpc), block(DA_WARPS * 32);
+  if (qpc == 2)
+    NV_CUDA(launch_pdl(decode_attn_window_kernel<FP8, 2>, grid, block, 0, S_(stream), CBF(qkv), ld, k, v, kx, vx, lens, BF(out), ldo,
+                       Smax, H, W, scale, CBF(cos_t), CBF(sin_t)));
+  else if (qpc == 4)
+    NV_CUDA(launch_pdl(decode_attn_window_kernel<FP8, 4>, grid, block, 0, S_(stream), CBF(qkv), ld, k, v, kx, vx, lens, BF(out), ldo,
+                       Smax, H, W, scale, CBF(cos_t), CBF(sin_t)));
+  else
+    NV_CUDA(launch_pdl(decode_attn_window_kernel<FP8, 8>, grid, block, 0, S_(stream), CBF(qkv), ld, k, v, kx, vx, lens, BF(out), ldo,
+                       Smax, H, W, scale, CBF(cos_t), CBF(sin_t)));
+  return NV_OK;
+}
+
 extern "C" {
 
 int nv_kv_store_prefill(const void* qkv, int64_t ld, const int* cu_seqlens, void* kcache, void* vcache, int B, int T,
@@ -1721,6 +2121,45 @@ int nv_decode_attn_rope_fp8(const void* qkv, int64_t ld, const int* lens, const 
   NV_CUDA(launch_pdl(decode_attn_kernel<true, true>, dim3(B * H), dim3(DA_WARPS * 32), 0, S_(stream), CBF(qkv), ld,
                      reinterpret_cast<uint8_t*>(kq), reinterpret_cast<uint8_t*>(vq), lens, BF(out), ldo, Smax, H, scale, CBF(cos_t),
                      CBF(sin_t), reinterpret_cast<int8_t*>(kexp), reinterpret_cast<int8_t*>(vexp), BeamKV<true>{}));
+  return NV_OK;
+}
+
+int nv_decode_attn_rope_window(const void* qkv, int64_t ld, const int* lens, const void* cos_t, const void* sin_t, void* kcache,
+                               void* vcache, void* out, int64_t ldo, int B, int W, int Smax, int H, int head_dim, float scale,
+                               void* stream) {
+  return launch_window<false>("nv_decode_attn_rope_window", qkv, ld, lens, cos_t, sin_t, kcache, vcache, nullptr, nullptr, out, ldo,
+                              B, W, Smax, H, head_dim, scale, stream);
+}
+
+int nv_decode_attn_rope_window_fp8(const void* qkv, int64_t ld, const int* lens, const void* cos_t, const void* sin_t, void* kq,
+                                   void* vq, void* kexp, void* vexp, void* out, int64_t ldo, int B, int W, int Smax, int H,
+                                   int head_dim, float scale, void* stream) {
+  return launch_window<true>("nv_decode_attn_rope_window_fp8", qkv, ld, lens, cos_t, sin_t, kq, vq, kexp, vexp, out, ldo, B, W, Smax,
+                             H, head_dim, scale, stream);
+}
+
+int nv_lookup_draft(const int* hist, int ld_hist, const int* hist_len, const int* finished, const int* special, int n_special,
+                    int eos_id, int K, int ngram, int* drafts, int* win_ids, int B, void* stream) {
+  NV_REQUIRE(K >= 1 && K < WIN_MAX && ngram >= 1 && n_special >= 0 && n_special <= MAX_SPECIAL && B >= 0,
+             "nv_lookup_draft: bad arguments (K=%d ngram=%d n_special=%d B=%d)", K, ngram, n_special, B);
+  if (B == 0) return NV_OK;
+  NV_REQUIRE(hist && hist_len && finished && drafts && win_ids && (special || n_special == 0), "nv_lookup_draft: null argument");
+  NV_CUDA(launch_pdl(lookup_draft_kernel, dim3(B), dim3(LD_THREADS), 0, S_(stream), hist, ld_hist, hist_len, finished, special,
+                     n_special, eos_id, K, ngram, drafts, win_ids));
+  return NV_OK;
+}
+
+int nv_lookup_accept(const void* logits, int64_t ld, int V, const int* special, int n_special, const int* drafts, int K, int* finished,
+                     int eos_id, int stop_on_eos, int max_new, int* out, int ld_out, int* hist, int ld_hist, int* hist_len, int* n_out,
+                     int* lens, int* n_acc, int B, void* stream) {
+  NV_REQUIRE(K >= 1 && K < WIN_MAX && V > 0 && n_special >= 0 && n_special <= MAX_SPECIAL && B >= 0 && max_new <= ld_out,
+             "nv_lookup_accept: bad arguments (K=%d V=%d n_special=%d B=%d max_new=%d ld_out=%d)", K, V, n_special, B, max_new,
+             ld_out);
+  if (B == 0) return NV_OK;
+  NV_REQUIRE(logits && drafts && finished && out && hist && hist_len && n_out && lens && n_acc && (special || n_special == 0),
+             "nv_lookup_accept: null argument");
+  NV_CUDA(launch_pdl(lookup_accept_kernel, dim3(B), dim3(1024), 0, S_(stream), CBF(logits), ld, V, special, n_special, drafts, K,
+                     finished, eos_id, stop_on_eos, max_new, out, ld_out, hist, ld_hist, hist_len, n_out, lens, n_acc));
   return NV_OK;
 }
 

@@ -1,6 +1,6 @@
 """``ModifiedLlamaForCausalLM.generate``'s decoding (HF GenerationMixin greedy / sampling / beam / contrastive search): the call's
-record, the decode states, the prefill, the graph-replayed step loop and the drivers ``decode``, ``beam_search`` and
-``contrastive_search``."""
+record, the decode states, the prefill, the graph-replayed step loop and the drivers ``decode``, ``lookup_decode``,
+``beam_search`` and ``contrastive_search``."""
 from __future__ import annotations
 
 import collections
@@ -8,6 +8,7 @@ import dataclasses
 from types import SimpleNamespace
 from typing import Optional
 
+import numpy as np
 import torch
 
 from . import llama as llama_mod
@@ -23,7 +24,7 @@ class Decoding:
     eos: int
     pad: int
     stop_on_eos: Optional[bool]          # None for beams: a prompt stops when its hypotheses are done
-    mode: str                            # "greedy", "sample", "trie", "trie+sample", "beam" or "contrastive"
+    mode: str                            # "greedy", "sample", "trie", "trie+sample", "beam", "contrastive" or "lookup"
     kv: str                              # the KV cache format, "bf16" or "fp8"
     temperature: Optional[float] = None  # sampled modes
     top_k: Optional[int] = None          # sampled modes, and contrastive search's candidates per prompt (= n)
@@ -35,6 +36,8 @@ class Decoding:
     n_return: int = 1                    # beams: sequences returned per prompt (host finalisation)
     length_penalty: Optional[float] = None   # beams: its normalisers are copied into the state every call
     penalty_alpha: Optional[float] = None    # contrastive search: the degeneration penalty's weight
+    lookup_k: Optional[int] = None           # prompt-lookup decoding: drafts per step (the window is lookup_k + 1 rows)
+    lookup_ngram: Optional[int] = None       # prompt-lookup decoding: max_matching_ngram_size
 
     @property
     def sampled(self) -> bool:
@@ -43,7 +46,7 @@ class Decoding:
     def key(self) -> tuple:
         """The graph key: every field a captured step bakes in (not ``n_return`` or ``length_penalty``), the format last."""
         return (self.eos, self.pad, self.stop_on_eos, self.mode, self.temperature, self.top_k, self.top_p, self.trie_eos, self.n,
-                self.early_stopping, self.proc, self.penalty_alpha, self.kv)
+                self.early_stopping, self.proc, self.penalty_alpha, self.lookup_k, self.lookup_ngram, self.kv)
 
 
 def processors(repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens, eos: int) -> Optional[tuple]:
@@ -152,7 +155,10 @@ def prefill(lm, dec: Decoding, input_ids, attention_mask, vis, max_new_tokens: i
     Contrastive search (``dec.n`` = k candidates per prompt): the prompt cache holds the prompt and then the selected tokens
     (Sp = bucket(longest prompt + max_new_tokens)), kc / vc [B * k, 1, D] the candidates' own keys, one slot each; the logits,
     ids and flags are per prompt ([B]), and the prefill returns every prompt row of the last layer (the context).  See
-    ``contrastive_search``."""
+    ``contrastive_search``.
+
+    Prompt-lookup decoding (``dec.lookup_k`` = k): one sequence per prompt in a cache of bucket(longest prompt + max_new_tokens
+    + k) rows, so that every verify window's k + 1 writes fit, and [B * (k + 1)] logits rows.  See ``lookup_decode``."""
     from .modified_lm import PackedPrompt           # modified_lm imports this module
     dev, d = lm._device(), lm.dims
     pp = PackedPrompt(input_ids, attention_mask, lm, dev, generate_positions=True)
@@ -163,13 +169,16 @@ def prefill(lm, dec: Decoding, input_ids, attention_mask, vis, max_new_tokens: i
     Sp, G = (bucket(max(pp.seqlens)), bucket(max_new_tokens)) if shared else (0, bucket(max(pp.seqlens) + max_new_tokens))
     if cs:
         Sp, G = bucket(max(pp.seqlens) + max_new_tokens), 1
+    W = 1 if dec.lookup_k is None else dec.lookup_k + 1   # decode rows per sequence in a step
+    if W > 1:
+        G = bucket(max(pp.seqlens) + max_new_tokens + dec.lookup_k)
     P = B if cs else R                              # rows with their own logits, ids and finished flag
 
     def build():
         cache = lambda rows, length: llama_mod.kv_cache(d, rows, length, dec.kv, dev)
         zeros = lambda dtype, *shape: torch.zeros(shape, dtype=dtype, device=dev)
         i32 = lambda *shape: zeros(torch.int32, *shape)
-        st = SimpleNamespace(kc=cache(R, G), vc=cache(R, G), logits=logits_buffer(P, V, dev), next_ids=i32(P), lens=i32(R),
+        st = SimpleNamespace(kc=cache(R, G), vc=cache(R, G), logits=logits_buffer(P * W, V, dev), next_ids=i32(P), lens=i32(R),
                              Sp=Sp, G=G, graph=None)
         if dec.mode == "beam":
             st.beam_score, st.cand_score, st.cand_tok = zeros(torch.float32, R), zeros(torch.float32, B, 2 * n), i32(B, 2 * n)
@@ -191,7 +200,9 @@ def prefill(lm, dec: Decoding, input_ids, attention_mask, vis, max_new_tokens: i
         if dec.trie_eos is not None:
             st.masked, st.node, st.miss = logits_buffer(R, V, dev), i32(R), i32(1)
         return st
-    st = lm._decode_states.lookup((R, G, (B, Sp) if shared else None) + dec.key(), build, want_graph)
+    # a verify step bakes max_new_tokens into its accept launch
+    st = lm._decode_states.lookup((R, G, (B, Sp) if shared else None, max_new_tokens if W > 1 else None) + dec.key(), build,
+                                  want_graph)
     if shared:
         st.plens.copy_(torch.tensor(pp.seqlens, dtype=torch.int32), non_blocking=True)
     x = ops.embed_fwd(pp.ids, lm.model.embed_tokens.weight.data, pp.vis_src if vis is not None else None, vis)
@@ -372,6 +383,82 @@ def decode(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph, s
     if stop and check_every > 1:
         new = trim_after_eos(new, eos)                        # see check_every above
     return torch.cat([input_ids.to(dev).repeat_interleave(n, dim=0), new], dim=1)
+
+
+# ---- prompt-lookup speculative decoding (HF generate(prompt_lookup_num_tokens=k), greedy) ----
+# A step that accepts drafts finishes a row in fewer steps than greedy's 8-step check interval would notice; a check is one
+# blocking read between two graph replays.
+LOOKUP_CHECK_EVERY = 4
+
+
+def lookup_history(input_ids, attention_mask, cap: int) -> tuple:
+    """Each prompt's non-pad ids, left-aligned in an int32 [B, cap] host array, and their counts: where the drafts of
+    ``ops.lookup_draft`` are looked up (the generated tokens are appended on the device)."""
+    ids = input_ids.detach().cpu().numpy()
+    msk = np.ones(ids.shape, dtype=bool) if attention_mask is None else attention_mask.detach().cpu().numpy().astype(bool)
+    hist = np.zeros((ids.shape[0], cap), dtype=np.int32)
+    lens = msk.sum(1).astype(np.int32)
+    for b in range(ids.shape[0]):
+        hist[b, :lens[b]] = ids[b][msk[b]]
+    return hist, lens
+
+
+def lookup_decode(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph, stats, dec: Decoding):
+    """Greedy decoding that verifies k = ``dec.lookup_k`` drafted tokens per step.  After the prefill and its first token (as
+    in ``decode``), a step is: ``ops.lookup_draft`` proposes k tokens per prompt from n-grams of its history (prompt and
+    generated tokens, HF's PromptLookupCandidateGenerator); the last token and the k drafts run as one causal window of k + 1
+    decode rows per prompt (``decode_step(window=k + 1)``, all rows through the lm_head); ``ops.lookup_accept`` keeps the drafts
+    that equal the argmax of the row before them and emits those plus one token, 1 .. k + 1 per prompt and step.  A row's tokens
+    are the argmax of its own prefix, so the ids are greedy decoding's whatever the drafts are; they differ from ``decode`` only
+    where a different row count in a GEMM moves a near tie.  Static shapes: the step is captured once and replayed; the
+    generated ids stay on the device until one copy at the end.  Returns [B, S0 + n_new] with ``decode``'s width and pads."""
+    k, eos, pad, stop, special = dec.lookup_k, dec.eos, dec.pad, dec.stop_on_eos, lm.special_ids_dev
+    W, n_out = k + 1, max(max_new_tokens, 1)
+    timer = PhaseTimer(stats)
+    pp, st, hid_last = prefill(lm, dec, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph)
+    B, dev = pp.B, lm._device()
+    hist0, plens = lookup_history(input_ids, attention_mask, int(input_ids.shape[1]) + n_out)
+
+    def alloc(hcap, ocap):
+        i32 = lambda *shape: torch.zeros(shape, dtype=torch.int32, device=dev)
+        st.hist, st.out, st.drafts, st.win = i32(B, hcap), i32(B, ocap), i32(B, k), i32(B, W)
+        st.hist_len, st.n_out, st.n_acc = i32(B), i32(B), i32(B)
+    _grow(st, "lookup_cap", (hist0.shape[1], n_out), alloc)
+    st.hist[:, :hist0.shape[1]].copy_(torch.from_numpy(hist0), non_blocking=True)
+    st.finished.zero_()
+    st.lens.copy_(torch.from_numpy(plens), non_blocking=True)
+    decode_head(lm, hid_last, st.logits[:B])
+    ops.argmax_masked(st.logits[:B], special, st.finished, eos, pad, stop, st.next_ids)
+    st.hist.scatter_(1, st.lens[:, None].long(), st.next_ids[:, None])        # the first token ends the history
+    st.hist_len.copy_(st.lens).add_(1)
+    st.out.fill_(pad)
+    st.out[:, 0].copy_(st.next_ids)
+    st.n_out.fill_(1)
+    st.n_acc.zero_()
+    if n_out == 1:
+        st.finished.fill_(1)
+    timer.mark()
+
+    def step():
+        with ops.pdl():
+            ops.lookup_draft(st.hist, st.hist_len, st.finished, special, eos, dec.lookup_ngram, st.drafts, st.win)
+            xt = ops.embed_fwd(st.win.view(-1), lm.model.embed_tokens.weight.data)
+            h = lm.core.decode_step(xt, st.lens, st.kc, st.vc, window=W)
+            decode_head(lm, h, st.logits)
+            ops.lookup_accept(st.logits, special, st.drafts, st.finished, eos, stop, n_out, st.out, st.hist, st.hist_len,
+                              st.n_out, st.lens, st.n_acc)
+
+    # every row is done once it emitted EOS or n_out tokens; the device is asked every LOOKUP_CHECK_EVERY steps, and a done
+    # row's extra steps emit nothing.  At most n_out - 1 steps: each emits at least one token per unfinished row.
+    steps, replays = step_loop(st, step, n_out, lambda: bool(st.finished.all()), LOOKUP_CHECK_EVERY, use_cuda_graph)
+    counts = torch.cat([st.n_out, st.n_acc, st.out.flatten()]).cpu()
+    n_emit, n_acc, out = counts[:B], counts[B:2 * B], counts[2 * B:].view(B, -1)[:, :n_out]
+    timer.finish(pp, steps, replays, st.G, lookup_steps=steps, lookup_tokens=int(n_emit.sum()) - B,
+                 lookup_accepted=int(n_acc.sum()))
+    new = out.to(torch.int64)
+    if stop:
+        new = trim_after_eos(new, eos)
+    return torch.cat([input_ids.to(dev), new.to(dev)], dim=1)
 
 
 def trim_after_eos(new: torch.Tensor, eos: int) -> torch.Tensor:

@@ -971,7 +971,8 @@ class LlamaCore:
         return dx
 
     # -------------------------------------------------------------------------------------------------
-    def decode_step(self, x: torch.Tensor, lens: torch.Tensor, kc: List[torch.Tensor], vc: List[torch.Tensor], beam=None) -> torch.Tensor:
+    def decode_step(self, x: torch.Tensor, lens: torch.Tensor, kc: List[torch.Tensor], vc: List[torch.Tensor], beam=None,
+                    window: int = 1) -> torch.Tensor:
         """One new token per sequence.  x: [B, D] bf16 embeddings of the new tokens; lens: int32 [B] (device) =
         number of cached tokens = position of the new token; caches [B, Smax, D] bf16 per layer, or fp8 ``(e4m3, exponents)``
         pairs per layer (``is_fp8_kv``; the new rows are rounded as they are appended).  Static shapes and
@@ -980,7 +981,11 @@ class LlamaCore:
 
         ``beam`` (beam search): the B rows are beams, ``beam.K`` per prompt; kc / vc hold only the generated keys [B, G, D]
         (addressed through ``beam.src``) and ``beam.pk`` / ``beam.pv`` the per-layer prompt caches [B / K, Sp, D] with
-        ``beam.plens`` keys per prompt (``ops.decode_attn_rope_beam``)."""
+        ``beam.plens`` keys per prompt (``ops.decode_attn_rope_beam``).
+
+        ``window`` = w > 1 (the verify step of prompt-lookup decoding): x holds w consecutive tokens per sequence, row b * w + r
+        at position lens[b] + r (lens stays [B]); the attention is ``ops.decode_attn_rope_window``, everything else the same
+        loop over B * w rows."""
         d = self.d
         H, D = d.n_heads, d.hidden
         # The step is HBM-bound weight streaming.  Batches <= 16 use the swap-AB cluster-split-K kernel with the SwiGLU fused
@@ -1022,6 +1027,10 @@ class LlamaCore:
             elif beam is not None:
                 ao = ops.decode_attn_rope_beam(qkv, lens, self.cos, self.sin, beam.pk[l], beam.pv[l], beam.plens, kc[l], vc[l],
                                                beam.src, beam.K, H)
+            elif window > 1 and fp8_kv:
+                ao = ops.decode_attn_rope_window_fp8(qkv, lens, self.cos, self.sin, kc[l][0], vc[l][0], kc[l][1], vc[l][1], H, window)
+            elif window > 1:
+                ao = ops.decode_attn_rope_window(qkv, lens, self.cos, self.sin, kc[l], vc[l], H, window)
             elif fp8_kv:                                                                 # same, quantizing the appended rows
                 ao = ops.decode_attn_rope_fp8(qkv, lens, self.cos, self.sin, kc[l][0], vc[l][0], kc[l][1], vc[l][1], H)
             else:

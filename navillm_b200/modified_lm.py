@@ -43,6 +43,20 @@ class LMOutput(SimpleNamespace):
         return getattr(self, k)
 
 
+def _lookup_k(k, ngram) -> tuple:
+    """``generate(prompt_lookup_num_tokens=k, max_matching_ngram_size=ngram)`` as (drafts per step, ngram): k = 0 for None or 0
+    (plain greedy decoding), else an int in 1 .. 15 (the window kernel's 16 rows); ngram None is HF's 2.  Any other k, or an
+    ngram below 1, is a ``ValueError``."""
+    if k is None or (not isinstance(k, bool) and isinstance(k, int) and k == 0):
+        return 0, 0
+    ngram = 2 if ngram is None else ngram
+    if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= ops.LOOKUP_WMAX - 1:
+        raise ValueError(f"generate(prompt_lookup_num_tokens={k!r}): an int in 1 .. {ops.LOOKUP_WMAX - 1} expected (0 or None: off)")
+    if isinstance(ngram, bool) or not isinstance(ngram, int) or ngram < 1:
+        raise ValueError(f"generate(max_matching_ngram_size={ngram!r}): a positive int expected")
+    return k, ngram
+
+
 class PackedPrompt:
     """Host-side packing of a left-padded [B,S] prompt batch: everything the kernels need, built with numpy
     on the tokenizer's CPU tensors and shipped to the device in ONE int32 copy."""
@@ -954,7 +968,9 @@ class ModifiedLlamaForCausalLM(nn.Module):
                  top_p: float = 1.0, num_beams: int = 1, length_penalty: float = 1.0, early_stopping: bool = False,
                  num_return_sequences: int = 1, num_beam_groups: int = 1, repetition_penalty: Optional[float] = None,
                  no_repeat_ngram_size: Optional[int] = None, min_length: Optional[int] = None,
-                 min_new_tokens: Optional[int] = None, penalty_alpha: Optional[float] = None, **unused) -> torch.Tensor:
+                 min_new_tokens: Optional[int] = None, penalty_alpha: Optional[float] = None,
+                 prompt_lookup_num_tokens: Optional[int] = None, max_matching_ngram_size: Optional[int] = 2,
+                 **unused) -> torch.Tensor:
         """Prefill on the packed kernels (positions = cumsum(mask)-1 like HF generate; visual tokens injected only
         here, as in models/modified_lm.py:195-197), then one token per step over a pre-allocated KV cache.  The
         decode step of the greedy, sampled and trie-constrained modes has static shapes and is replayed as a CUDA graph
@@ -1002,7 +1018,28 @@ class ModifiedLlamaForCausalLM(nn.Module):
         is kept (``generation.contrastive_search``; the context starts at the prompt's non-pad positions).  Returns [B, S0 +
         n_new] ids like greedy decoding.  ``num_return_sequences > 1`` and a non-finite ``penalty_alpha`` raise ``ValueError``;
         ``trie=`` / ``logits_processor=`` and ``top_k`` above ``ops.CONTRASTIVE_KMAX`` raise ``NotImplementedError``.  Every
-        other ``penalty_alpha`` (None, 0, or with ``top_k <= 1``, sampling or beams) is ignored, as in HF."""
+        other ``penalty_alpha`` (None, 0, or with ``top_k <= 1``, sampling or beams) is ignored, as in HF.
+
+        ``prompt_lookup_num_tokens=k`` (1 .. 15; HF's name) is greedy decoding that verifies k drafted tokens per step
+        (``generation.lookup_decode``): the drafts are the tokens that followed the latest n-gram (n = ``max_matching_ngram_size``
+        down to 1) at its earliest earlier occurrence in the prompt or the generated text, and one step of k + 1 decode rows keeps
+        those that equal greedy's own argmax, plus one more token.  The ids are greedy decoding's, with ``decode``'s width and
+        pads; they can differ from a plain greedy call only at a near tie, because the step's GEMMs run over more rows.  bf16,
+        fp8 or int4 weights, bf16 or fp8 KV cache, graphed or eager.  Sampling, beams, contrastive search, ``trie=``,
+        ``logits_processor=``, the device processors and ``num_return_sequences > 1`` raise ``NotImplementedError``; a k
+        outside 0 .. 15 or ``max_matching_ngram_size < 1`` raises ``ValueError``.  0 or None is plain greedy decoding."""
+        lookup, ngram = _lookup_k(prompt_lookup_num_tokens, max_matching_ngram_size)
+        if lookup:
+            excluded = [("do_sample=True", do_sample), ("num_beams > 1", num_beams > 1),
+                        ("penalty_alpha > 0 (contrastive search)", penalty_alpha is not None and penalty_alpha > 0),
+                        ("trie=", trie is not None), ("logits_processor=", bool(logits_processor)),
+                        ("repetition_penalty", repetition_penalty not in (None, 1.0)),
+                        ("no_repeat_ngram_size", bool(no_repeat_ngram_size)), ("min_length", bool(min_length)),
+                        ("min_new_tokens", bool(min_new_tokens)), ("num_return_sequences > 1", num_return_sequences > 1)]
+            for name, on in excluded:
+                if on:
+                    raise NotImplementedError(f"generate(prompt_lookup_num_tokens={lookup}) with {name}: prompt-lookup decoding "
+                                              "is built for plain greedy decoding only")
         contrastive = (penalty_alpha is not None and not (penalty_alpha <= 0) and top_k is not None and top_k > 1 and not do_sample
                        and num_beams == 1 and (num_beam_groups is None or num_beam_groups <= 1))
         if contrastive:
@@ -1049,6 +1086,10 @@ class ModifiedLlamaForCausalLM(nn.Module):
         pad = self.tokenizer.unk_token_id if pad_token_id is None else pad_token_id
         proc = generation.processors(repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens, eos)
         call = (self, input_ids, attention_mask, (cand_vis, hist_vis, obj_vis), max_new_tokens, use_cuda_graph, stats)
+        if lookup:
+            dec = generation.Decoding(int(eos), int(pad), bool(stop_on_eos), "lookup", self.kv_cache_dtype, lookup_k=lookup,
+                                      lookup_ngram=ngram)
+            return generation.lookup_decode(*call, dec)
         if contrastive:
             dec = generation.Decoding(int(eos), int(pad), bool(stop_on_eos), "contrastive", self.kv_cache_dtype, top_k=int(top_k),
                                       n=int(top_k), proc=proc, penalty_alpha=float(penalty_alpha))

@@ -728,6 +728,47 @@ def decode_attn_rope_fp8(qkv, lens, cos_t, sin_t, kq, vq, ke, ve, n_heads, *, ou
     return out
 
 
+def _window_args(name, qkv, lens, B, W, HD, n_heads, out):
+    if not 1 <= W <= LOOKUP_WMAX:
+        raise ValueError(f"{name}: window of {W} rows (1 .. {LOOKUP_WMAX} expected)")
+    if HD != n_heads * 128 or qkv.dtype != bf16 or qkv.stride(1) != 1 or tuple(qkv.shape) != (B * W, 3 * HD):
+        raise ValueError(f"{name}: qkv bf16 [{B * W}, {3 * HD}] and {HD // 128} heads expected (got {qkv.dtype} {tuple(qkv.shape)}, "
+                         f"{n_heads} heads)")
+    if lens.dtype != torch.int32 or lens.numel() != B or not lens.is_cuda:
+        raise ValueError(f"{name}: lens int32 [{B}] on the device expected (got {lens.dtype} {tuple(lens.shape)})")
+    if out is None:
+        out = torch.empty((B * W, HD), dtype=bf16, device=qkv.device)
+    if out.dtype != bf16 or out.stride(1) != 1 or tuple(out.shape) != (B * W, HD):
+        raise ValueError(f"{name}: out bf16 [{B * W}, {HD}] expected (got {out.dtype} {tuple(out.shape)})")
+    return out
+
+
+def decode_attn_rope_window(qkv, lens, cos_t, sin_t, kc, vc, n_heads, W, *, out=None, scale=None):
+    """``decode_attn_rope`` for W consecutive new tokens per sequence (nv_decode_attn_rope_window): qkv [B * W, 3*H*128] bf16
+    PRE-RoPE, row b * W + r at position lens[b] + r; the rotated k and the v of every row go to cache rows lens[b] + r, and query
+    r attends over keys 0 .. lens[b] + r.  Bit for bit W sequential ``decode_attn_rope`` calls.  Returns [B * W, H*128] bf16."""
+    B, Smax, HD = kc.shape
+    if kc.dtype != bf16 or vc.shape != kc.shape or vc.dtype != bf16:
+        raise ValueError(f"decode_attn_rope_window: bf16 caches [B, Smax, {HD}] expected")
+    out = _window_args("decode_attn_rope_window", qkv, lens, B, W, HD, n_heads, out)
+    check(_lib.load().nv_decode_attn_rope_window(ptr(qkv), i64(qkv.stride(0)), ptr(lens), ptr(cos_t), ptr(sin_t), ptr(kc), ptr(vc),
+                                                 ptr(out), i64(out.stride(0)), i32(B), i32(W), i32(Smax), i32(n_heads), i32(128),
+                                                 f32(128 ** -0.5 if scale is None else scale), stream_ptr()),
+          "nv_decode_attn_rope_window")
+    return out
+
+
+def decode_attn_rope_window_fp8(qkv, lens, cos_t, sin_t, kq, vq, ke, ve, n_heads, W, *, out=None, scale=None):
+    """``decode_attn_rope_window`` over an fp8 cache: bit for bit W sequential ``decode_attn_rope_fp8`` calls."""
+    B, Smax, HD = _fp8_kv(kq, vq, ke, ve, "decode_attn_rope_window_fp8")
+    out = _window_args("decode_attn_rope_window_fp8", qkv, lens, B, W, HD, n_heads, out)
+    check(_lib.load().nv_decode_attn_rope_window_fp8(ptr(qkv), i64(qkv.stride(0)), ptr(lens), ptr(cos_t), ptr(sin_t), ptr(kq), ptr(vq),
+                                                     ptr(ke), ptr(ve), ptr(out), i64(out.stride(0)), i32(B), i32(W), i32(Smax),
+                                                     i32(n_heads), i32(128), f32(128 ** -0.5 if scale is None else scale),
+                                                     stream_ptr()), "nv_decode_attn_rope_window_fp8")
+    return out
+
+
 def _beam_io(name, B, K, G, **ts):
     """Dtype / shape / device checks of the beam-search state (include/navillm_b200.h, nv_beam_*)."""
     want = {"cand_score": (torch.float32, (B, 2 * K)), "cand_tok": (torch.int32, (B, 2 * K)), "cand_parent": (torch.int32, (B, 2 * K)),
@@ -1081,6 +1122,46 @@ class pdl:
 
     def __exit__(self, *a):
         _lib.load().nv_set_pdl(i32(self.prev))
+
+
+LOOKUP_WMAX = 16               # verify-window rows per prompt the window kernel is built for (k drafts + 1)
+
+
+def lookup_draft(hist, hist_len, finished, special, eos_id, ngram, drafts, win_ids):
+    """Prompt-lookup drafts (nv_lookup_draft): for each row of the history hist int32 [B, G] (hist_len [B] tokens: the row's
+    non-pad prompt ids, then its generated tokens), HF's PromptLookupCandidateGenerator with ``max_matching_ngram_size`` =
+    ngram.  Writes drafts int32 [B, k] (-1 past the drafts) and the verify window's ids win_ids int32 [B, k + 1]."""
+    B, k = drafts.shape
+    _dev_t(hist_len, torch.int32, (B,), "lookup_draft", "hist_len")
+    _dev_t(finished, torch.int32, (B,), "lookup_draft", "finished")
+    _dev_t(win_ids, torch.int32, (B, k + 1), "lookup_draft", "win_ids")
+    _dev_t(drafts, torch.int32, (B, k), "lookup_draft", "drafts")
+    if hist.dtype != torch.int32 or hist.dim() != 2 or hist.shape[0] != B or hist.stride(1) != 1 or not hist.is_cuda:
+        raise ValueError(f"lookup_draft: hist int32 [{B}, G] on the device expected (got {hist.dtype} {tuple(hist.shape)})")
+    check(_lib.load().nv_lookup_draft(ptr(hist), i32(hist.stride(0)), ptr(hist_len), ptr(finished), ptr(special), i32(special.numel()),
+                                      i32(eos_id), i32(k), i32(ngram), ptr(drafts), ptr(win_ids), i32(B), stream_ptr()),
+          "nv_lookup_draft")
+
+
+def lookup_accept(logits, special, drafts, finished, eos_id, stop_on_eos, max_new, out, hist, hist_len, n_out, lens, n_acc):
+    """Verify a window (nv_lookup_accept): logits bf16 [B * (k + 1), V], row b * (k + 1) + j the prediction after window token j.
+    Each unfinished row emits the masked argmax t_0 .. t_m of its rows while drafts[b, j] = t_j, cut after EOS (stop_on_eos) and
+    at max_new tokens, into out int32 [B, >= max_new] at n_out[b] and into hist at hist_len[b]; lens advances by the tokens
+    emitted, n_acc by the accepted drafts, and finished is set once a row is done."""
+    B, k = drafts.shape
+    V = logits.shape[1]
+    if logits.dtype != bf16 or logits.stride(1) != 1 or logits.shape[0] != B * (k + 1):
+        raise ValueError(f"lookup_accept: bf16 logits [{B * (k + 1)}, V] expected (got {logits.dtype} {tuple(logits.shape)})")
+    for name, t in (("finished", finished), ("hist_len", hist_len), ("n_out", n_out), ("lens", lens), ("n_acc", n_acc)):
+        _dev_t(t, torch.int32, (B,), "lookup_accept", name)
+    _dev_t(drafts, torch.int32, (B, k), "lookup_accept", "drafts")
+    for name, t in (("out", out), ("hist", hist)):
+        if t.dtype != torch.int32 or t.dim() != 2 or t.shape[0] != B or t.stride(1) != 1 or not t.is_cuda:
+            raise ValueError(f"lookup_accept: {name} int32 [{B}, n] on the device expected (got {t.dtype} {tuple(t.shape)})")
+    check(_lib.load().nv_lookup_accept(ptr(logits), i64(logits.stride(0)), i32(V), ptr(special), i32(special.numel()), ptr(drafts),
+                                       i32(k), ptr(finished), i32(eos_id), i32(1 if stop_on_eos else 0), i32(max_new), ptr(out),
+                                       i32(out.shape[1]), ptr(hist), i32(hist.stride(0)), ptr(hist_len), ptr(n_out), ptr(lens),
+                                       ptr(n_acc), i32(B), stream_ptr()), "nv_lookup_accept")
 
 
 def add_int_(x, delta):
