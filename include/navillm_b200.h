@@ -325,7 +325,7 @@ int nv_beam_topk(const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, 
  * s < 0 -> bf16(s * penalty), else bf16(s / penalty) (IEEE division); NoRepeatNGramLogitsProcessor (ngram = n > 0): every
  * token that completes an n-gram of the history whose first n - 1 tokens equal its last n - 1 -> -inf (nothing while
  * S + t + 1 < n); MinLength / MinNewTokensLength: eos_id -> -inf while S + t < min_length or t < min_new_tokens.  Off:
- * penalty 1, ngram 0, min_length 0, min_new_tokens 0.  V must fit two V-bit bitmaps in 48 KB.
+ * penalty 1, ngram 0, min_length 0, min_new_tokens 0.  V must fit two V-bit bitmaps in 48 KB (three for nv_beam_topk_trie).
  * nv_logits_process: in place on the bf16 logits [R, ld] of the greedy / sampled decode rows, between the lm_head and the trie
  * mask or the pick.  Row r reads prompt_ids[(r / rows_per_prompt) * ld_prompt ...] and hist[r, 0 .. hist_len[r]) ([R, G]); with
  * append non-null, append[r] is first stored at hist[r, hist_len[r]] and hist_len[r] incremented, so a captured step keeps
@@ -340,6 +340,19 @@ int nv_beam_topk_processed(const void* logits, int64_t ld_prompt, int64_t ld_bea
                            const float* beam_score, float* cand_score, int* cand_tok, int* cand_parent, const int* prompt_ids,
                            int64_t ld_ids, const int* prompt_width, const int* hist, int G, const int* prompt_state, float penalty,
                            int ngram, int min_length, int min_new_tokens, int eos_id, int B, int K, void* stream);
+/* nv_beam_topk_trie: nv_beam_topk_processed followed by 4.28's PrefixConstrainedLogitsProcessor walking a trie: after the
+ * processors, every log-prob of beam k of prompt b outside the allowed set becomes -inf (allowed ones keep their value).  The
+ * beam's node is found by walking its generated tokens hist[b * K + k, 0 .. t), t = prompt_state[b, 0], from the root with
+ * the rule of nv_trie_mask (a node without children stays; a token that is not a child of a node with children leads to the
+ * childless dead node n_nodes); the allowed set is the node's children, or leaf_tok at a childless node.  The trie is the CSR
+ * table of nv_trie_mask (node_ptr [n_nodes + 2], child_tok / child_node [E], children ascending).  At the first step
+ * (ld_beam = 0, t = 0) every beam is at the root.  The processors' off values (penalty 1, ngram 0, min_length 0,
+ * min_new_tokens 0) give trie-only beams.  V must fit three V-bit bitmaps in 48 KB. */
+int nv_beam_topk_trie(const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, const int* special, int n_special,
+                      const float* beam_score, float* cand_score, int* cand_tok, int* cand_parent, const int* prompt_ids,
+                      int64_t ld_ids, const int* prompt_width, const int* hist, int G, const int* prompt_state, float penalty,
+                      int ngram, int min_length, int min_new_tokens, int eos_id, const int* node_ptr, const int* child_tok,
+                      const int* child_node, int n_nodes, int leaf_tok, int B, int K, void* stream);
 int nv_beam_select(const float* cand_score, const int* cand_tok, const int* cand_parent, float* beam_score, int* hist, int* src,
                    double* hyp_score, int* hyp_meta, int* hyp_tok, int* prompt_state, int* next_ids, int* lens, const double* norm,
                    int B, int K, int G, int eos_id, int pad_id, int early_stopping, void* stream);

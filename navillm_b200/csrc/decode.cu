@@ -1400,11 +1400,43 @@ struct BeamProc {
   ProcParams p;
 };
 
-template <bool PROC>
+// TRIE (nv_beam_topk_trie, always with PROC): after the processors, every log-prob the trie does not allow at the beam's node
+// becomes -inf, as 4.28's PrefixConstrainedLogitsProcessor does to log_softmax's output.  The node is found statelessly: one
+// thread walks the beam's generated tokens hist[b * K + k, 0 .. t) from the root by the rule of nv_trie_mask (a node without
+// children stays; a token that is not a child leads to the dead node n_nodes), so the walk follows the beam through every
+// reorder nv_beam_select makes.  The allowed tokens (the node's children, or leaf_tok at a node without any) fill a third
+// V-bit bitmap beside seen / banned.
+struct BeamTrie {
+  const int* node_ptr;                       // [n_nodes + 2]
+  const int* child_tok;                      // [E], ascending per node
+  const int* child_node;                     // [E]
+  int n_nodes;
+  int leaf_tok;
+};
+
+__device__ __forceinline__ int trie_walk(const BeamTrie& tr, const int* __restrict__ toks, int t) {
+  int node = 0;
+  for (int i = 0; i < t; ++i) {
+    const int e0 = tr.node_ptr[node], e1 = tr.node_ptr[node + 1];
+    if (e1 == e0) break;                                          // childless: the walk stays here for good
+    const int tok = toks[i];
+    int lo = e0, hi = e1;                                         // first edge with child_tok >= tok
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (tr.child_tok[mid] < tok) lo = mid + 1;
+      else hi = mid;
+    }
+    node = (lo < e1 && tr.child_tok[lo] == tok) ? tr.child_node[lo] : tr.n_nodes;
+  }
+  return node;
+}
+
+template <bool PROC, bool TRIE = false>
 __device__ __forceinline__ void beam_topk_body(const __nv_bfloat16* __restrict__ logits, int64_t ld_prompt, int64_t ld_beam, int V,
                                                const int* __restrict__ special, int n_special, const float* __restrict__ beam_score,
                                                 int K, float* __restrict__ cand_score, int* __restrict__ cand_tok,
-                                               int* __restrict__ cand_par, const BeamProc& bp) {
+                                               int* __restrict__ cand_par, const BeamProc& bp, const BeamTrie& tr = BeamTrie{}) {
+  static_assert(PROC || !TRIE, "the trie mask runs inside the processed scan");
   __shared__ int s_special[MAX_SPECIAL];
   __shared__ float s_m[BEAM_MAX], s_ls[BEAM_MAX], s_bs[BEAM_MAX];
   __shared__ float redf[32];
@@ -1459,16 +1491,21 @@ __device__ __forceinline__ void beam_topk_body(const __nv_bfloat16* __restrict__
     const float m = s_m[k], ls = s_ls[k], bs = s_bs[k];
     uint32_t* seen = nullptr;
     uint32_t* banned = nullptr;
+    uint32_t* allowed = nullptr;
     if constexpr (PROC) {
-      extern __shared__ uint32_t bt_bits[];                      // seen | banned, (V + 31) / 32 words each
+      extern __shared__ uint32_t bt_bits[];                      // seen | banned (| allowed), (V + 31) / 32 words each
       const int nw = (V + 31) >> 5;
+      constexpr int NMAPS = TRIE ? 3 : 2;
       seen = bt_bits;
       banned = bt_bits + nw;
       __syncthreads();                                           // the previous beam's scan is done with the bitmaps
-      for (int i = tid; i < 2 * nw; i += BT_THREADS) bt_bits[i] = 0u;
+      for (int i = tid; i < NMAPS * nw; i += BT_THREADS) bt_bits[i] = 0u;
       __syncthreads();
       const int S = *bp.prompt_width, t = bp.prompt_state[b * 5], L = S + t;
       const ProcHist h{bp.prompt + (int64_t)b * bp.ld_prompt, bp.hist + (int64_t)(b * K + k) * bp.G, S};
+      __shared__ int s_node;                                     // TRIE: the beam's node
+      if constexpr (TRIE)
+        if (tid == 0) s_node = trie_walk(tr, bp.hist + (int64_t)(b * K + k) * bp.G, t);
       if (bp.p.penalty != 1.f)
         for (int i = tid; i < L; i += BT_THREADS) {
           const int id = h[i];
@@ -1477,6 +1514,19 @@ __device__ __forceinline__ void beam_topk_body(const __nv_bfloat16* __restrict__
       if (bp.p.ngram > 0) ngram_bans(h, L, bp.p.ngram, V, banned);
       if (tid == 0 && bp.p.eos >= 0 && bp.p.eos < V && eos_banned(bp.p, S, t)) atomicOr(&banned[bp.p.eos >> 5], 1u << (bp.p.eos & 31));
       __syncthreads();
+      if constexpr (TRIE) {
+        allowed = bt_bits + 2 * nw;
+        const int node = s_node, e0 = tr.node_ptr[node], e1 = tr.node_ptr[node + 1];
+        if (e1 == e0) {
+          if (tid == 0) atomicOr(&allowed[tr.leaf_tok >> 5], 1u << (tr.leaf_tok & 31));
+        } else {
+          for (int e = e0 + tid; e < e1; e += BT_THREADS) {        // fan-outs of any size: looped, not capped
+            const int c = tr.child_tok[e];
+            if (c >= 0 && c < V) atomicOr(&allowed[c >> 5], 1u << (c & 31));
+          }
+        }
+        __syncthreads();
+      }
     }
     for (int c = tid; c < V; c += BT_THREADS) {
       float sc = -INFINITY;
@@ -1486,6 +1536,8 @@ __device__ __forceinline__ void beam_topk_body(const __nv_bfloat16* __restrict__
           const uint32_t bit = 1u << (c & 31);
           if (seen[c >> 5] & bit) lp = rep_penalize(lp, bp.p.penalty);
           if (banned[c >> 5] & bit) lp = -INFINITY;
+          if constexpr (TRIE)
+            if (!(allowed[c >> 5] & bit)) lp = -INFINITY;
           sc = lp + bs;
         }
       } else {
@@ -1550,6 +1602,15 @@ __global__ void __launch_bounds__(BT_THREADS, 1) beam_topk_proc_kernel(const __n
                                                                        float* __restrict__ cand_score, int* __restrict__ cand_tok,
                                                                        int* __restrict__ cand_par, BeamProc bp) {
   beam_topk_body<true>(logits, ld_prompt, ld_beam, V, special, n_special, beam_score, K, cand_score, cand_tok, cand_par, bp);
+}
+
+// the bound as for beam_topk_proc_kernel; the walk and the third bitmap add no per-thread state to the scan
+__global__ void __launch_bounds__(BT_THREADS, 1) beam_topk_trie_kernel(const __nv_bfloat16* __restrict__ logits, int64_t ld_prompt,
+                                                                       int64_t ld_beam, int V, const int* __restrict__ special,
+                                                                       int n_special, const float* __restrict__ beam_score, int K,
+                                                                       float* __restrict__ cand_score, int* __restrict__ cand_tok,
+                                                                       int* __restrict__ cand_par, BeamProc bp, BeamTrie tr) {
+  beam_topk_body<true, true>(logits, ld_prompt, ld_beam, V, special, n_special, beam_score, K, cand_score, cand_tok, cand_par, bp, tr);
 }
 
 // prompt_state [B, BS_FIELDS] of nv_beam_select
@@ -2280,6 +2341,35 @@ int nv_beam_topk_processed(const void* logits, int64_t ld_prompt, int64_t ld_bea
   const BeamProc bp{prompt_ids, ld_ids, prompt_width, hist, G, prompt_state, ProcParams{penalty, ngram, min_length, min_new_tokens, eos_id}};
   NV_CUDA(launch_pdl(beam_topk_proc_kernel, dim3(B), dim3(BT_THREADS), (size_t)((V + 31) / 32) * 4 * 2, S_(stream), CBF(logits),
                      ld_prompt, ld_beam, V, special, n_special, beam_score, K, cand_score, cand_tok, cand_parent, bp));
+  return NV_OK;
+}
+
+// nv_beam_topk_processed with the trie mask after the processors (see beam_topk_trie_kernel).  The CSR trie as nv_trie_mask
+// reads it; V must fit three V-bit bitmaps in 48 KB.
+int nv_beam_topk_trie(const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, const int* special, int n_special,
+                      const float* beam_score, float* cand_score, int* cand_tok, int* cand_parent, const int* prompt_ids,
+                      int64_t ld_ids, const int* prompt_width, const int* hist, int G, const int* prompt_state, float penalty,
+                      int ngram, int min_length, int min_new_tokens, int eos_id, const int* node_ptr, const int* child_tok,
+                      const int* child_node, int n_nodes, int leaf_tok, int B, int K, void* stream) {
+  NV_REQUIRE(logits && beam_score && cand_score && cand_tok && cand_parent && prompt_ids && prompt_width && hist && prompt_state &&
+             node_ptr && child_tok && child_node && V > 0 && B >= 0 && G > 0,
+             "nv_beam_topk_trie: bad arguments (V=%d B=%d G=%d)", V, B, G);
+  NV_REQUIRE(K >= 1 && K <= BEAM_MAX && 2 * K <= V, "nv_beam_topk_trie: %d beams: 1..%d beams and V >= 2K supported", K, BEAM_MAX);
+  NV_REQUIRE((int64_t)K * V < 0xffffffffll, "nv_beam_topk_trie: K * V = %lld does not fit the 32-bit candidate index",
+             (long long)K * V);
+  NV_REQUIRE(n_special >= 0 && n_special <= MAX_SPECIAL && (n_special == 0 || special),
+             "nv_beam_topk_trie: n_special=%d out of range (max %d)", n_special, MAX_SPECIAL);
+  NV_REQUIRE(n_nodes >= 1 && leaf_tok >= 0 && leaf_tok < V, "nv_beam_topk_trie: n_nodes=%d (>= 1), leaf_tok=%d outside [0, %d)",
+             n_nodes, leaf_tok, V);
+  const int st = check_proc("nv_beam_topk_trie", V, penalty, ngram, min_length, min_new_tokens);
+  if (st != NV_OK) return st;
+  const size_t smem = (size_t)((V + 31) / 32) * 4 * 3;
+  NV_REQUIRE(smem <= 48 * 1024, "nv_beam_topk_trie: vocabulary of %d does not fit the three shared bitmaps", V);
+  if (B == 0) return NV_OK;
+  const BeamProc bp{prompt_ids, ld_ids, prompt_width, hist, G, prompt_state, ProcParams{penalty, ngram, min_length, min_new_tokens, eos_id}};
+  const BeamTrie tr{node_ptr, child_tok, child_node, n_nodes, leaf_tok};
+  NV_CUDA(launch_pdl(beam_topk_trie_kernel, dim3(B), dim3(BT_THREADS), smem, S_(stream), CBF(logits), ld_prompt, ld_beam, V,
+                     special, n_special, beam_score, K, cand_score, cand_tok, cand_parent, bp, tr));
   return NV_OK;
 }
 

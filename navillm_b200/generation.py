@@ -109,14 +109,12 @@ def _grow(st, cap_name: str, need: tuple, alloc) -> tuple:
 
 
 def load_trie(st, table) -> tuple:
-    """Copy a flattened trie into the state's ``trie_buf`` in one host-to-device copy and put every row at its root.  Returns
-    the kernel's (node_ptr, child_tok, child_node, n_nodes) views."""
+    """Copy a flattened trie into the state's ``trie_buf`` in one host-to-device copy (a trie that outgrows it drops the
+    state's graph).  Returns the kernels' (node_ptr, child_tok, child_node, n_nodes) views."""
     def alloc(ncap, ecap):
         st.trie_buf = torch.empty(ncap + 2 + 2 * ecap, dtype=torch.int32, device=st.next_ids.device)
     ncap, ecap = _grow(st, "trie_cap", (table.n_nodes, max(table.n_edges, 1)), alloc)
     st.trie_buf.copy_(torch.from_numpy(table.pack(ncap, ecap)))
-    st.node.zero_()                                 # every row starts at the root
-    st.miss.zero_()
     o = ncap + 2
     return st.trie_buf[:o], st.trie_buf[o:o + ecap], st.trie_buf[o + ecap:], ncap
 
@@ -150,7 +148,8 @@ def prefill(lm, dec: Decoding, input_ids, attention_mask, vis, max_new_tokens: i
     beams, per prompt (``dec.n`` > 1): the prompt keys go to a prompt cache ``pk`` / ``pv`` [B, Sp, D] that the n rows of a
     prompt share (``plens`` keys each), and kc / vc [B * n, G, D] hold only the generated keys, read through the source table
     ``src`` (``st.beam``), so no K/V is copied.  Sampling adds its uniform numbers ``u`` (the host processors draw their
-    own), tries their masked logits and walk state, beams the scorer's buffers (``ops.beam_select``).
+    own), tries their masked logits and walk state (beams walk statelessly inside ``ops.beam_topk_trie``), beams the scorer's
+    buffers (``ops.beam_select``).
 
     Contrastive search (``dec.n`` = k candidates per prompt): the prompt cache holds the prompt and then the selected tokens
     (Sp = bucket(longest prompt + max_new_tokens)), kc / vc [B * k, 1, D] the candidates' own keys, one slot each; the logits,
@@ -197,7 +196,7 @@ def prefill(lm, dec: Decoding, input_ids, attention_mask, vis, max_new_tokens: i
             st.commit_table = ops.contrastive_commit_table(st.kc, st.vc, st.pk, st.pv)
         if dec.sampled and not host:
             st.u = torch.empty((R,), dtype=torch.float32, device=dev)
-        if dec.trie_eos is not None:
+        if dec.trie_eos is not None and dec.mode != "beam":
             st.masked, st.node, st.miss = logits_buffer(R, V, dev), i32(R), i32(1)
         return st
     # a verify step bakes max_new_tokens into its accept launch
@@ -295,6 +294,8 @@ def decode(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph, s
     logits, next_ids, finished, lens = st.logits, st.next_ids, st.finished, st.lens
     if table is not None:
         trie_csr = load_trie(st, table)
+        st.node.zero_()                                       # every row starts at the root
+        st.miss.zero_()
     if dec.proc is not None:
         load_proc(st, input_ids, R, max_new_tokens)
     finished.zero_()
@@ -527,14 +528,17 @@ def contrastive_search(lm, input_ids, attention_mask, vis, max_new_tokens, use_c
 
 
 # ---- beam search (HF GenerationMixin.beam_search / BeamSearchScorer, transformers 4.28 as the reference pins it) ----
-def beam_search(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph, stats, dec: Decoding):
+def beam_search(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph, stats, dec: Decoding, table=None):
     """Beam search over B prompts with K = ``dec.n`` beams each.  The prefill runs once per prompt into the prompt cache, whose
     keys the K beams of the prompt share; generated keys live in a [B * K, G] cache that is written once per slot and read
     through the source table ``src`` (reordering the beams gathers ``src``, never K/V).  Each step is ``nv_beam_topk`` (2K
     best candidates per prompt) and ``nv_beam_select`` (the scorer), all on the device, and is replayed as a CUDA graph; the
     hypotheses are finalized on the host after one device-to-host copy.  The visual tokens of prompt b reach all K beams of
     prompt b (the reference's HF expansion of ``cand_vis`` would hand them to other rows' slots).  With logits processors
-    (``dec.proc``) the scoring is ``nv_beam_topk_processed`` over the beams' histories (prompt ids, ``hist``)."""
+    (``dec.proc``) the scoring is ``nv_beam_topk_processed`` over the beams' histories (prompt ids, ``hist``).  With the
+    flattened trie ``table`` it is ``nv_beam_topk_trie`` (processors or not): each beam walks its own generated tokens from the
+    root, and the log-probs its node does not allow become -inf after the processors, as 4.28's PrefixConstrainedLogitsProcessor
+    masks log_softmax's output; the trie is loaded as in ``decode``, and one that outgrows the buffers is recaptured."""
     K, eos, pad, proc, special = dec.n, dec.eos, dec.pad, dec.proc, lm.special_ids_dev
     if K > BEAM_MAX:
         raise NotImplementedError(f"generate(num_beams={K}): at most {BEAM_MAX} beams are built")
@@ -543,8 +547,10 @@ def beam_search(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_gra
     timer = PhaseTimer(stats)
     pp, st, hid_last = prefill(lm, dec, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph)
     B, S, G = pp.B, int(input_ids.shape[1]), st.G
-    if proc is not None:
+    if proc is not None or table is not None:
         load_proc(st, input_ids, 0, G)
+    if table is not None:
+        trie_csr = load_trie(st, table)
     st.beam_score.view(B, K).fill_(-1e9)[:, 0] = 0.0             # only beam 0 of a prompt expands at the first step
     st.hyp_score.zero_()
     st.hyp_score[:, K] = 1e9                                      # BeamHypotheses.worst_score starts at 1e9
@@ -558,7 +564,10 @@ def beam_search(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_gra
                                   dec.early_stopping)
 
     def topk(first_step=False):
-        if proc is None:
+        if table is not None:
+            ops.beam_topk_trie(st.logits, special, st.beam_score, K, st.cand_score, st.cand_tok, st.cand_par, st.proc_ids,
+                               st.proc_width, st.hist, st.pstate, proc, *trie_csr, table.eos, first_step=first_step)
+        elif proc is None:
             ops.beam_topk(st.logits, special, st.beam_score, K, st.cand_score, st.cand_tok, st.cand_par, first_step=first_step)
         else:
             ops.beam_topk_processed(st.logits, special, st.beam_score, K, st.cand_score, st.cand_tok, st.cand_par, st.proc_ids,

@@ -996,8 +996,18 @@ class ModifiedLlamaForCausalLM(nn.Module):
 
         ``num_beams > 1`` is HF beam search as transformers 4.28 (the reference's pin) runs it, ``length_penalty``,
         ``early_stopping`` and ``num_return_sequences`` included; see ``generation.beam_search``.  Returns [B * num_return_sequences,
-        L] ids.  Beam sampling, group beam search, ``trie=`` / ``logits_processor=`` with beams and more return sequences than
-        beams raise ``NotImplementedError``.
+        L] ids.  Beam sampling, group beam search, ``logits_processor=`` with beams and more return sequences than beams raise
+        ``NotImplementedError``.
+
+        ``trie=`` with ``num_beams > 1`` is 4.28's beam search with a PrefixConstrainedLogitsProcessor whose allowed tokens come
+        from walking the trie: each beam walks its own generated tokens from ``trie.root`` (a node without children stays; a token
+        that is not a child leads to a childless node), and at its node every log-prob but the node's children (``[trie.eos]`` at a
+        childless node) becomes -inf, after the device processors and before the beam-score add.  A beam's score is therefore its
+        log-probability under the full vocabulary, and ``num_return_sequences=n`` returns the n best answers of the trie, best
+        first.  The walk runs inside the beam top-k on the device (``nv_beam_topk_trie``) and is graph-replayed; ``length_penalty``,
+        ``early_stopping``, the device processors, the fp8 / int4 weight copies and the fp8 KV cache all apply.  The caller's trie
+        is never modified.  A trie ``flatten_trie`` cannot represent raises ``NotImplementedError``, as the host processor's
+        per-row state cannot follow reordered beams; ``stats`` gets ``trie_path = "device"`` and ``trie_flatten_ms``.
 
         ``do_sample=True, num_return_sequences=N`` draws N samples per prompt: [B * N, L] ids, row b * N + j a sample of
         prompt b (HF's order).  Each prompt is prefilled once and its N rows share its KV cache (``generation.decode``); the tokens
@@ -1066,9 +1076,9 @@ class ModifiedLlamaForCausalLM(nn.Module):
                                           f"(num_beams={num_beams})")
             if do_sample:
                 raise NotImplementedError("generate(num_beams > 1, do_sample=True): beam sampling is not built")
-            if trie is not None or logits_processor:
-                raise NotImplementedError("generate(num_beams > 1) with trie= / logits_processor=: the processors keep per-row "
-                                          "state that reordering the beams would scramble")
+            if logits_processor:
+                raise NotImplementedError("generate(num_beams > 1) with logits_processor=: the processors keep per-row state that "
+                                          "reordering the beams would scramble")
         elif n_seq > 1:
             if not do_sample:
                 raise NotImplementedError(f"generate(num_return_sequences={n_seq}) without beams needs do_sample=True: greedy "
@@ -1095,9 +1105,21 @@ class ModifiedLlamaForCausalLM(nn.Module):
                                       n=int(top_k), proc=proc, penalty_alpha=float(penalty_alpha))
             return generation.contrastive_search(*call, dec)
         if num_beams > 1:
+            table = None
+            if trie is not None:
+                t0 = time.perf_counter()
+                table = trie_mod.flatten_trie(trie, self.lm_head.weight.shape[0])
+                flatten_ms = 1e3 * (time.perf_counter() - t0)
+                if table is None:
+                    raise NotImplementedError("generate(num_beams > 1) with a trie= that flatten_trie cannot represent: the host "
+                                              "processors keep per-row state that reordering the beams would scramble")
             dec = generation.Decoding(int(eos), int(pad), None, "beam", self.kv_cache_dtype, n=int(num_beams), n_return=n_seq,
-                                      length_penalty=float(length_penalty), early_stopping=bool(early_stopping), proc=proc)
-            return generation.beam_search(*call, dec)
+                                      length_penalty=float(length_penalty), early_stopping=bool(early_stopping), proc=proc,
+                                      trie_eos=None if table is None else table.eos)
+            out = generation.beam_search(*call, dec, table=table)
+            if stats is not None and table is not None:
+                stats.update({"trie_path": "device", "trie_flatten_ms": flatten_ms})
+            return out
         procs = list(logits_processor or [])
         table = None
         if trie is not None and not procs:

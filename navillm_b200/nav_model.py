@@ -520,10 +520,12 @@ class NavModel(nn.Module):
             vis = self.lang_model.cat_vis(cand_vis, hist_vis_input, None, pp)
             return {"loss": self.lang_model.lm_loss(pp, vis)}
         trie = kwargs.get("trie", None)
+        # beam search over the answer trie: the beam kwargs reach generate() only when the caller passes them
+        beams = {k: kwargs[k] for k in ("num_beams", "num_return_sequences", "length_penalty", "early_stopping") if k in kwargs}
         ids = self.lang_model.generate(input_ids=text["input_ids"], attention_mask=text["attention_mask"], cand_vis=cand_vis,
                                        hist_vis=hist_vis_input, eos_token_id=self.lang_model.tokenizer.eos_token_id,
                                        pad_token_id=self.lang_model.tokenizer.unk_token_id, max_new_tokens=50, do_sample=False,
-                                       trie=trie).tolist()
+                                       trie=trie, **beams).tolist()
         ids = [s[text["input_ids"].shape[1]:] for s in ids]
         return {"generated_sentences": self.lang_model.tokenizer.batch_decode(ids, skip_special_tokens=True,
                                                                               clean_up_tokenization_spaces=False)}

@@ -847,6 +847,38 @@ def beam_topk_processed(logits, special, beam_score, K, cand_score, cand_tok, ca
           "nv_beam_topk_processed")
 
 
+PROC_OFF = (1.0, 0, 0, 0, -1)  # the processors' off values: beam_topk_trie without processors
+
+
+def beam_topk_trie(logits, special, beam_score, K, cand_score, cand_tok, cand_parent, prompt_ids, prompt_width, hist, prompt_state,
+                   proc, node_ptr, child_tok, child_node, n_nodes, leaf_tok, *, first_step=False):
+    """``beam_topk_processed`` followed by the trie mask (nv_beam_topk_trie): every log-prob the trie does not allow at the beam's
+    node becomes -inf.  Beam k of prompt b walks its generated tokens hist[b * K + k, :prompt_state[b, 0]] from the root;
+    node_ptr / child_tok / child_node: the CSR trie of ``trie_mask`` with n_nodes real nodes plus the dead node n_nodes, leaf_tok
+    the token a childless node allows.  ``proc`` = None (or ``PROC_OFF``) runs the trie mask alone."""
+    B = cand_score.shape[0]
+    V = logits.shape[1]
+    if logits.dtype != bf16 or logits.stride(1) != 1 or logits.shape[0] < (B if first_step else B * K):
+        raise ValueError(f"beam_topk_trie: bf16 logits with {B if first_step else B * K} rows expected "
+                         f"(got {logits.dtype} {tuple(logits.shape)})")
+    _beam_io("beam_topk_trie", B, K, hist.shape[1], cand_score=cand_score, cand_tok=cand_tok, cand_parent=cand_parent,
+             beam_score=beam_score, hist=hist, prompt_state=prompt_state)
+    args = _proc_io("beam_topk_trie", V, prompt_ids, prompt_width, hist, PROC_OFF if proc is None else proc)
+    n_nodes = int(n_nodes)
+    for name, t, n in (("node_ptr", node_ptr, n_nodes + 2), ("child_tok", child_tok, None), ("child_node", child_node, None)):
+        if t.dtype != torch.int32 or t.dim() != 1 or not t.is_contiguous() or not t.is_cuda or (n is not None and t.numel() < n):
+            raise ValueError(f"beam_topk_trie: {name} int32 [{n if n is not None else 'E'}] contiguous on the device expected "
+                             f"(got {t.dtype} {tuple(t.shape)})")
+    if child_tok.numel() != child_node.numel():
+        raise ValueError(f"beam_topk_trie: child_tok [{child_tok.numel()}] and child_node [{child_node.numel()}] differ in length")
+    ld = logits.stride(0)
+    check(_lib.load().nv_beam_topk_trie(ptr(logits), i64(ld if first_step else K * ld), i64(0 if first_step else ld), i32(V),
+                                        ptr(special), i32(special.numel()), ptr(beam_score), ptr(cand_score), ptr(cand_tok),
+                                        ptr(cand_parent), ptr(prompt_ids), i64(prompt_ids.stride(0)), ptr(prompt_width), ptr(hist),
+                                        i32(hist.shape[1]), ptr(prompt_state), *args, ptr(node_ptr), ptr(child_tok), ptr(child_node),
+                                        i32(n_nodes), i32(leaf_tok), i32(B), i32(K), stream_ptr()), "nv_beam_topk_trie")
+
+
 def beam_select(cand_score, cand_tok, cand_parent, beam_score, hist, src, hyp_score, hyp_meta, hyp_tok, prompt_state, next_ids, lens,
                 norm, eos_id, pad_id, early_stopping):
     """One BeamSearchScorer.process step on the device (nv_beam_select); norm fp64 [G]: (S + t) ** length_penalty for S padded
