@@ -171,6 +171,17 @@ int nv_attn_fwd_kv(const void* q, int64_t ldq, const void* kcache, int64_t ldk, 
 int nv_attn_fwd_kv_fp8(const void* q, int64_t ldq, const void* kq, const void* vq, const void* kexp, const void* vexp, void* o,
                        int64_t ldo, float* lse, const int* cu_seqlens, const int* kv_start, const int* kv_len, int B, int Tq,
                        int Tkv, int H, int head_dim, int total_qblocks, float scale, void* stream);
+/* nv_attn_fwd_tree[_fp8]: nv_attn_fwd_kv[_fp8] whose Tq = B * q_len query rows are the q_len nodes of one tree per sequence, in
+ * DFS preorder (answer scoring: every node of an answer trie over each prompt's cache).  Query i of sequence b sees the
+ * kv_len[b] - q_len >= 1 cached keys, and the key of tree row j only when j <= i < tree_end[j]: tree_end (int32 [q_len], device,
+ * shared by every sequence) is the first row after node j's subtree, so a query sees its ancestors and itself.  The fp8 form
+ * reads the rounded rows K' / V' as nv_attn_fwd_kv_fp8 does. */
+int nv_attn_fwd_tree(const void* q, int64_t ldq, const void* kcache, int64_t ldk, const void* vcache, int64_t ldv, void* o,
+                     int64_t ldo, float* lse, const int* cu_seqlens, const int* kv_start, const int* kv_len, const int* tree_end,
+                     int B, int Tq, int Tkv, int H, int head_dim, int total_qblocks, float scale, void* stream);
+int nv_attn_fwd_tree_fp8(const void* q, int64_t ldq, const void* kq, const void* vq, const void* kexp, const void* vexp, void* o,
+                         int64_t ldo, float* lse, const int* cu_seqlens, const int* kv_start, const int* kv_len, const int* tree_end,
+                         int B, int Tq, int Tkv, int H, int head_dim, int total_qblocks, float scale, void* stream);
 int nv_attn_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, const void* o,
                 int64_t ldo, const void* dout, int64_t lddo, const float* lse, float* dvec, void* dq, int64_t lddq,
                 void* dk, int64_t lddk, void* dv, int64_t lddv, const int* cu_seqlens, int B, int T, int H, int head_dim,
@@ -353,6 +364,15 @@ int nv_beam_topk_trie(const void* logits, int64_t ld_prompt, int64_t ld_beam, in
                       int64_t ld_ids, const int* prompt_width, const int* hist, int G, const int* prompt_state, float penalty,
                       int ngram, int min_length, int min_new_tokens, int eos_id, const int* node_ptr, const int* child_tok,
                       const int* child_node, int n_nodes, int leaf_tok, int B, int K, void* stream);
+/* nv_trie_score: the log-probability of every answer of a trie under each prompt.  logits bf16 [B * R, ld], R = 1 + N': row
+ * b * R holds prompt b's next-token logits after its prompt, row b * R + 1 + j those after tree node j (DFS preorder).  The
+ * log-prob of token c at a row is nv_beam_topk's: special ids -inf, fp32 max, fp64 sum, (x - m) - ls rounded once to bf16,
+ * NaN -> -inf.  Answer a walks tree rows path_rows[path_off[a] .. path_off[a + 1]) from the root (tokens tok[row]), then EOS:
+ * logprob[b, a] (fp32 [B, A]) is the fp32 left fold s = lp(row 0, t_1) + 0, s = lp(row of t_1, t_2) + s, ..., s = lp(row of
+ * t_d, eos) + s.  stats (fp32 [B * R, 2]) is scratch for each row's max and log-sum.  tok and path_rows may be null when
+ * R = 1 (a root without children: one empty answer).  Two kernels under PDL. */
+int nv_trie_score(const void* logits, int64_t ld, int V, const int* special, int n_special, const int* tok, const int* path_off,
+                  const int* path_rows, int eos, float* stats, float* logprob, int B, int R, int A, void* stream);
 int nv_beam_select(const float* cand_score, const int* cand_tok, const int* cand_parent, float* beam_score, int* hist, int* src,
                    double* hyp_score, int* hyp_meta, int* hyp_tok, int* prompt_state, int* next_ids, int* lens, const double* norm,
                    int B, int K, int G, int eos_id, int pad_id, int early_stopping, void* stream);

@@ -30,6 +30,12 @@
 // the HBM latency nor the widening sits between two key blocks of the consumers.  That takes 64 KB on top of the 160 KB
 // (225.6 KB of the 227 KB an H100 CTA may use); single-buffered staging would leave the load of tile j + 1 exposed
 // whenever it has to wait for the widening of tile j.  384 threads leave the consumers 168 registers a thread.
+//
+// Tree mask (TREE = true, nv_attn_fwd_tree[_fp8]): the query rows of a sequence are the nodes of a tree in DFS preorder, and
+// tree_end[j] (int32 [q_len], shared by every sequence) is the first row after node j's subtree, so key dk + j is an ancestor-
+// or-self of query i iff j <= i < tree_end[j].  A query sees the dk cached keys and the keys of its ancestors and itself.
+// Preorder puts every ancestor before its descendants, so the causal block count still bounds the blocks a query needs; the
+// tree test runs on every block that holds keys at or past dk, not only on the diagonal one.
 #include "nv_common.cuh"
 #include "nv_fp8.cuh"
 #include "nv_host.h"
@@ -94,13 +100,14 @@ __device__ __forceinline__ bool locate_qblock(const int* __restrict__ cu, int B,
 }
 
 // FP8: tmap_k / tmap_v describe the e4m3 caches and kexp / vexp are their row exponents ([Tkv, H] int8); unused otherwise.
-template <bool FP8>
+// TREE: tree_end is the subtree table of the tree mask (see above); unused otherwise.
+template <bool FP8, bool TREE = false>
 __global__ void __launch_bounds__(AttnFwdSmem<FP8>::THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                 const __grid_constant__ CUtensorMap tmap_v, __nv_bfloat16* __restrict__ O, int64_t ldo,
                 float* __restrict__ lse, const int* __restrict__ cu_seqlens, int B, int T, float scale,
                 const int* __restrict__ kv_start, const int* __restrict__ kv_len, const int8_t* __restrict__ kexp,
-                const int8_t* __restrict__ vexp, int Tkv) {
+                const int8_t* __restrict__ vexp, int Tkv, const int* __restrict__ tree_end) {
   using L = AttnFwdSmem<FP8>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -255,7 +262,22 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
       wgmma_wait<0>();
       reg_fence(sacc);
     }
-    if (j * 128 + 127 > vis_first) {                               // block holds keys some row must not see
+    if constexpr (TREE) {
+      if (j * 128 + 127 >= dk) {                                   // block holds tree keys: causal and ancestor test
+        const int rel0 = (int)(j * 128) - (int)dk;                 // tree row of the block's first key
+#pragma unroll
+        for (uint32_t i = 0; i < 16; ++i) {
+          const int r0 = rel0 + (int)(8 * i + cq), r1 = r0 + 1;
+          // cached keys are seen by every row; tree rows past the sequence's exist for no real row
+          const int e0 = r0 < 0 ? 0x7fffffff : r0 < seq_len ? __ldg(tree_end + r0) : 0;
+          const int e1 = r1 < 0 ? 0x7fffffff : r1 < seq_len ? __ldg(tree_end + r1) : 0;
+          if ((int)qa < r0 || (int)qa >= e0) sacc[4 * i] = -INFINITY;
+          if ((int)qa < r1 || (int)qa >= e1) sacc[4 * i + 1] = -INFINITY;
+          if ((int)qb < r0 || (int)qb >= e0) sacc[4 * i + 2] = -INFINITY;
+          if ((int)qb < r1 || (int)qb >= e1) sacc[4 * i + 3] = -INFINITY;
+        }
+      }
+    } else if (j * 128 + 127 > vis_first) {                        // block holds keys some row must not see
       const int lim_a = (int)(dk + qa) - (int)(j * 128), lim_b = lim_a + 8;
 #pragma unroll
       for (uint32_t i = 0; i < 16; ++i) {
@@ -276,7 +298,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     mxa = fmaxf(mxa, __shfl_xor_sync(0xffffffffu, mxa, 2));
     mxb = fmaxf(mxb, __shfl_xor_sync(0xffffffffu, mxb, 1));
     mxb = fmaxf(mxb, __shfl_xor_sync(0xffffffffu, mxb, 2));
-    // key 0 is visible to every row, so the maximum is finite from the first block on
+    // key 0 is visible to every row (TREE: a cached key, dk >= 1), so the maximum is finite from the first block on
     const float mna = fmaxf(m_a, mxa * sl2), mnb = fmaxf(m_b, mxb * sl2);
     const float alpha_a = exp2f(m_a - mna), alpha_b = exp2f(m_b - mnb);
     m_a = mna; m_b = mnb;
@@ -360,7 +382,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 static int attn_fwd_launch(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* o,
                            int64_t ldo, float* lse, const int* cu_seqlens, const int* kv_start, const int* kv_len, int B, int T,
                            int Tkv, int H, int head_dim, int total_qblocks, float scale, void* stream,
-                           const void* kexp = nullptr, const void* vexp = nullptr) {
+                           const void* kexp = nullptr, const void* vexp = nullptr, const int* tree_end = nullptr) {
   using namespace nv;
   NV_REQUIRE(head_dim == 128, "nv_attn_fwd: head_dim must be 128 (got %d)", head_dim);
   NV_REQUIRE(B > 0 && T > 0 && H > 0 && total_qblocks > 0, "nv_attn_fwd: empty problem");
@@ -376,22 +398,32 @@ static int attn_fwd_launch(const void* q, int64_t ldq, const void* k, int64_t ld
     if ((rc = make_tmap_2d(&tk, k, 2, (uint64_t)H * 128, (uint64_t)Tkv, (uint64_t)ldk * 2, 64, 128))) return rc;
     if ((rc = make_tmap_2d(&tv, v, 2, (uint64_t)H * 128, (uint64_t)Tkv, (uint64_t)ldv * 2, 64, 128))) return rc;
   }
-  static bool attr_set[2] = {false, false};
-  if (!attr_set[fp8]) {
-    if (fp8)
-      NV_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnFwdSmem<true>::DYN_BYTES));
-    else
-      NV_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnFwdSmem<false>::DYN_BYTES));
-    attr_set[fp8] = true;
+  const bool tree = tree_end != nullptr;
+  static bool attr_set[2][2] = {{false, false}, {false, false}};
+  if (!attr_set[tree][fp8]) {
+    const int bytes = fp8 ? AttnFwdSmem<true>::DYN_BYTES : AttnFwdSmem<false>::DYN_BYTES;
+    const void* fn = tree ? (fp8 ? (const void*)attn_fwd_kernel<true, true> : (const void*)attn_fwd_kernel<false, true>)
+                          : (fp8 ? (const void*)attn_fwd_kernel<true> : (const void*)attn_fwd_kernel<false>);
+    NV_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    attr_set[tree][fp8] = true;
   }
   dim3 grid(total_qblocks, H);
-  if (fp8)
-    attn_fwd_kernel<true><<<grid, AttnFwdSmem<true>::THREADS, AttnFwdSmem<true>::DYN_BYTES, reinterpret_cast<cudaStream_t>(stream)>>>(
-        tq, tk, tv, reinterpret_cast<__nv_bfloat16*>(o), ldo, lse, cu_seqlens, B, T, scale, kv_start, kv_len,
-        reinterpret_cast<const int8_t*>(kexp), reinterpret_cast<const int8_t*>(vexp), Tkv);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  __nv_bfloat16* O = reinterpret_cast<__nv_bfloat16*>(o);
+  const int8_t* ke = reinterpret_cast<const int8_t*>(kexp);
+  const int8_t* ve = reinterpret_cast<const int8_t*>(vexp);
+  if (fp8 && tree)
+    attn_fwd_kernel<true, true><<<grid, AttnFwdSmem<true>::THREADS, AttnFwdSmem<true>::DYN_BYTES, st>>>(
+        tq, tk, tv, O, ldo, lse, cu_seqlens, B, T, scale, kv_start, kv_len, ke, ve, Tkv, tree_end);
+  else if (fp8)
+    attn_fwd_kernel<true><<<grid, AttnFwdSmem<true>::THREADS, AttnFwdSmem<true>::DYN_BYTES, st>>>(
+        tq, tk, tv, O, ldo, lse, cu_seqlens, B, T, scale, kv_start, kv_len, ke, ve, Tkv, nullptr);
+  else if (tree)
+    attn_fwd_kernel<false, true><<<grid, ATT_THREADS, AttnFwdSmem<false>::DYN_BYTES, st>>>(
+        tq, tk, tv, O, ldo, lse, cu_seqlens, B, T, scale, kv_start, kv_len, nullptr, nullptr, Tkv, tree_end);
   else
-    attn_fwd_kernel<false><<<grid, ATT_THREADS, AttnFwdSmem<false>::DYN_BYTES, reinterpret_cast<cudaStream_t>(stream)>>>(
-        tq, tk, tv, reinterpret_cast<__nv_bfloat16*>(o), ldo, lse, cu_seqlens, B, T, scale, kv_start, kv_len, nullptr, nullptr, Tkv);
+    attn_fwd_kernel<false><<<grid, ATT_THREADS, AttnFwdSmem<false>::DYN_BYTES, st>>>(
+        tq, tk, tv, O, ldo, lse, cu_seqlens, B, T, scale, kv_start, kv_len, nullptr, nullptr, Tkv, nullptr);
   NV_LAUNCH_CHECK();
   return NV_OK;
 }
@@ -428,4 +460,33 @@ extern "C" int nv_attn_fwd_kv_fp8(const void* q, int64_t ldq, const void* kq, co
   NV_REQUIRE(Tkv > 0 && H > 0, "nv_attn_fwd_kv_fp8: bad sizes (Tkv=%d H=%d)", Tkv, H);
   return attn_fwd_launch(q, ldq, kq, (int64_t)H * 128, vq, (int64_t)H * 128, o, ldo, lse, cu_seqlens, kv_start, kv_len, B, Tq, Tkv,
                          H, head_dim, total_qblocks, scale, stream, kexp, vexp);
+}
+
+// nv_attn_fwd_kv with the tree mask: the q_len rows of every sequence are the nodes of one tree in DFS preorder (the same
+// tree for every sequence, so Tq = B * q_len), and query i sees the kv_len - q_len >= 1 cached keys and tree key j only when
+// j <= i < tree_end[j] (int32 [q_len] on the device: the first row after node j's subtree).  Rows of the cache past kv_len
+// must be finite (allocate it zeroed).
+extern "C" int nv_attn_fwd_tree(const void* q, int64_t ldq, const void* kcache, int64_t ldk, const void* vcache, int64_t ldv,
+                                void* o, int64_t ldo, float* lse, const int* cu_seqlens, const int* kv_start, const int* kv_len,
+                                const int* tree_end, int B, int Tq, int Tkv, int H, int head_dim, int total_qblocks, float scale,
+                                void* stream) {
+  using namespace nv;
+  NV_REQUIRE(kv_start && kv_len && tree_end, "nv_attn_fwd_tree: kv_start / kv_len / tree_end are required");
+  return attn_fwd_launch(q, ldq, kcache, ldk, vcache, ldv, o, ldo, lse, cu_seqlens, kv_start, kv_len, B, Tq, Tkv, H,
+                         head_dim, total_qblocks, scale, stream, nullptr, nullptr, tree_end);
+}
+
+// nv_attn_fwd_tree over an fp8 cache (the layout of nv_attn_fwd_kv_fp8): bit for bit nv_attn_fwd_tree over a bf16 cache holding
+// the rounded rows K' / V'.
+extern "C" int nv_attn_fwd_tree_fp8(const void* q, int64_t ldq, const void* kq, const void* vq, const void* kexp, const void* vexp,
+                                    void* o, int64_t ldo, float* lse, const int* cu_seqlens, const int* kv_start, const int* kv_len,
+                                    const int* tree_end, int B, int Tq, int Tkv, int H, int head_dim, int total_qblocks, float scale,
+                                    void* stream) {
+  using namespace nv;
+  NV_REQUIRE(head_dim == 128, "nv_attn_fwd_tree_fp8: head_dim must be 128 (got %d)", head_dim);
+  NV_REQUIRE(q && kq && vq && kexp && vexp && o && cu_seqlens && kv_start && kv_len && tree_end,
+             "nv_attn_fwd_tree_fp8: null argument");
+  NV_REQUIRE(Tkv > 0 && H > 0, "nv_attn_fwd_tree_fp8: bad sizes (Tkv=%d H=%d)", Tkv, H);
+  return attn_fwd_launch(q, ldq, kq, (int64_t)H * 128, vq, (int64_t)H * 128, o, ldo, lse, cu_seqlens, kv_start, kv_len, B, Tq, Tkv,
+                         H, head_dim, total_qblocks, scale, stream, kexp, vexp, tree_end);
 }

@@ -1613,6 +1613,94 @@ __global__ void __launch_bounds__(BT_THREADS, 1) beam_topk_trie_kernel(const __n
   beam_topk_body<true, true>(logits, ld_prompt, ld_beam, V, special, n_special, beam_score, K, cand_score, cand_tok, cand_par, bp, tr);
 }
 
+// ---- answer scoring (nv_trie_score): every answer of a trie teacher-forced over one tree-masked forward ----
+constexpr int TS_THREADS = 512;
+constexpr int TF_THREADS = 256;
+
+// One CTA per logits row: the row's max and log-sum over the non-special ids, as beam_topk_body computes them (fp32 max, fp64
+// sum of exp(x - m), log rounded to fp32), into stats[row] = (m, ls).
+__global__ void __launch_bounds__(TS_THREADS) trie_row_stats_kernel(const __nv_bfloat16* __restrict__ logits, int64_t ld, int V,
+                                                                    const int* __restrict__ special, int n_special,
+                                                                    float* __restrict__ stats) {
+  __shared__ int s_special[MAX_SPECIAL];
+  __shared__ float redf[32];
+  __shared__ double redd[32];
+  griddep_launch();
+  griddep_wait();
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  constexpr int NW = TS_THREADS / 32;
+  const int ns = n_special;
+  if (tid < ns) s_special[tid] = special[tid];
+  __syncthreads();
+  auto is_special = [&](int c) {
+    bool sp = false;
+    for (int s = 0; s < ns; ++s) sp |= (s_special[s] == c);
+    return sp;
+  };
+  const __nv_bfloat16* row = logits + (int64_t)blockIdx.x * ld;
+  float mx = -INFINITY;
+  for (int c = tid; c < V; c += TS_THREADS)
+    if (!is_special(c)) mx = fmaxf(mx, __bfloat162float(row[c]));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  if (lane == 0) redf[w] = mx;
+  __syncthreads();
+  mx = lane < NW ? redf[lane] : -INFINITY;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  double s = 0.0;
+#pragma unroll 1                                                  // unrolled, ptxas spills a register around exp
+  for (int c = tid; c < V; c += TS_THREADS)
+    if (!is_special(c)) s += exp((double)(__bfloat162float(row[c]) - mx));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane == 0) redd[w] = s;
+  __syncthreads();
+  s = lane < NW ? redd[lane] : 0.0;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (tid == 0) {
+    stats[2 * blockIdx.x] = mx;
+    stats[2 * blockIdx.x + 1] = (float)log(s);
+  }
+}
+
+// One CTA per prompt, one thread per answer: the answer's path folded root to leaf in fp32, each term the bf16 log-prob of
+// beam_topk_body (special ids -inf, NaN -> -inf).
+__global__ void __launch_bounds__(TF_THREADS) trie_fold_kernel(const __nv_bfloat16* __restrict__ logits, int64_t ld, int V,
+                                                               const int* __restrict__ special, int n_special,
+                                                               const int* __restrict__ tok, const int* __restrict__ path_off,
+                                                               const int* __restrict__ path_rows, int eos,
+                                                               const float* __restrict__ stats, float* __restrict__ logprob,
+                                                               int R, int A) {
+  __shared__ int s_special[MAX_SPECIAL];
+  griddep_launch();
+  griddep_wait();
+  const int b = blockIdx.x, tid = threadIdx.x, ns = n_special;
+  if (tid < ns) s_special[tid] = special[tid];
+  __syncthreads();
+  const int64_t row0 = (int64_t)b * R;
+  auto lp = [&](int r, int c) {                                   // log-prob of token c at source row r of prompt b
+    bool sp = false;
+    for (int i = 0; i < ns; ++i) sp |= (s_special[i] == c);
+    if (sp) return -INFINITY;
+    const float m = stats[2 * (row0 + r)], ls = stats[2 * (row0 + r) + 1];
+    const float v = bf16_round((__bfloat162float(logits[(row0 + r) * ld + c]) - m) - ls);
+    return v != v ? -INFINITY : v;
+  };
+  for (int a = tid; a < A; a += TF_THREADS) {
+    float s = 0.f;
+    int src = 0;                                                  // row 0: the prompt's last row
+    for (int p = path_off[a]; p < path_off[a + 1]; ++p) {
+      const int node = path_rows[p];
+      s = lp(src, tok[node]) + s;
+      src = node + 1;
+    }
+    s = lp(src, eos) + s;
+    logprob[(int64_t)b * A + a] = s;
+  }
+}
+
 // prompt_state [B, BS_FIELDS] of nv_beam_select
 constexpr int BS_STEP = 0, BS_PLEN = 1, BS_COUNT = 2, BS_SEQ = 3, BS_DONE = 4, BS_FIELDS = 5;
 constexpr int BS_THREADS = 128, BS_CHUNK = 256;
@@ -2370,6 +2458,22 @@ int nv_beam_topk_trie(const void* logits, int64_t ld_prompt, int64_t ld_beam, in
   const BeamTrie tr{node_ptr, child_tok, child_node, n_nodes, leaf_tok};
   NV_CUDA(launch_pdl(beam_topk_trie_kernel, dim3(B), dim3(BT_THREADS), smem, S_(stream), CBF(logits), ld_prompt, ld_beam, V,
                      special, n_special, beam_score, K, cand_score, cand_tok, cand_parent, bp, tr));
+  return NV_OK;
+}
+
+// nv_trie_score: see include/navillm_b200.h.
+int nv_trie_score(const void* logits, int64_t ld, int V, const int* special, int n_special, const int* tok, const int* path_off,
+                  const int* path_rows, int eos, float* stats, float* logprob, int B, int R, int A, void* stream) {
+  NV_REQUIRE(logits && (R == 1 || (tok && path_rows)) && path_off && stats && logprob && (special || n_special == 0) && V > 0 &&
+             ld >= V && B > 0 && R >= 1 && A >= 1, "nv_trie_score: bad arguments (V=%d ld=%lld B=%d R=%d A=%d)", V, (long long)ld,
+             B, R, A);
+  NV_REQUIRE(n_special >= 0 && n_special <= MAX_SPECIAL, "nv_trie_score: n_special=%d out of range (max %d)", n_special,
+             MAX_SPECIAL);
+  NV_REQUIRE(eos >= 0 && eos < V, "nv_trie_score: eos=%d outside [0, %d)", eos, V);
+  NV_CUDA(launch_pdl(trie_row_stats_kernel, dim3(B * R), dim3(TS_THREADS), 0, S_(stream), CBF(logits), ld, V, special, n_special,
+                     stats));
+  NV_CUDA(launch_pdl(trie_fold_kernel, dim3(B), dim3(TF_THREADS), 0, S_(stream), CBF(logits), ld, V, special, n_special, tok,
+                     path_off, path_rows, eos, (const float*)stats, logprob, R, A));
   return NV_OK;
 }
 

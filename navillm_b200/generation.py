@@ -24,7 +24,8 @@ class Decoding:
     eos: int
     pad: int
     stop_on_eos: Optional[bool]          # None for beams: a prompt stops when its hypotheses are done
-    mode: str                            # "greedy", "sample", "trie", "trie+sample", "beam", "contrastive" or "lookup"
+    mode: str                            # "greedy", "sample", "trie", "trie+sample", "beam", "contrastive", "lookup" or
+                                         # "trie_score" (``score_answers``)
     kv: str                              # the KV cache format, "bf16" or "fp8"
     temperature: Optional[float] = None  # sampled modes
     top_k: Optional[int] = None          # sampled modes, and contrastive search's candidates per prompt (= n)
@@ -157,7 +158,11 @@ def prefill(lm, dec: Decoding, input_ids, attention_mask, vis, max_new_tokens: i
     ``contrastive_search``.
 
     Prompt-lookup decoding (``dec.lookup_k`` = k): one sequence per prompt in a cache of bucket(longest prompt + max_new_tokens
-    + k) rows, so that every verify window's k + 1 writes fit, and [B * (k + 1)] logits rows.  See ``lookup_decode``."""
+    + k) rows, so that every verify window's k + 1 writes fit, and [B * (k + 1)] logits rows.  See ``lookup_decode``.
+
+    Answer scoring (``dec.mode`` "trie_score", ``max_new_tokens`` = the trie's N' tree rows): one sequence per prompt in a
+    zeroed cache of bucket(longest prompt + N') rows (the tree attention reads rows past kv_len as masked zeros), never
+    graphed.  See ``score_answers``."""
     from .modified_lm import PackedPrompt           # modified_lm imports this module
     dev, d = lm._device(), lm.dims
     pp = PackedPrompt(input_ids, attention_mask, lm, dev, generate_positions=True)
@@ -174,7 +179,7 @@ def prefill(lm, dec: Decoding, input_ids, attention_mask, vis, max_new_tokens: i
     P = B if cs else R                              # rows with their own logits, ids and finished flag
 
     def build():
-        cache = lambda rows, length: llama_mod.kv_cache(d, rows, length, dec.kv, dev)
+        cache = lambda rows, length: llama_mod.kv_cache(d, rows, length, dec.kv, dev, zero=dec.mode == "trie_score")
         zeros = lambda dtype, *shape: torch.zeros(shape, dtype=dtype, device=dev)
         i32 = lambda *shape: zeros(torch.int32, *shape)
         st = SimpleNamespace(kc=cache(R, G), vc=cache(R, G), logits=logits_buffer(P * W, V, dev), next_ids=i32(P), lens=i32(R),
@@ -384,6 +389,83 @@ def decode(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph, s
     if stop and check_every > 1:
         new = trim_after_eos(new, eos)                        # see check_every above
     return torch.cat([input_ids.to(dev).repeat_interleave(n, dim=0), new], dim=1)
+
+
+# ---- answer scoring: every answer of a trie teacher-forced in one tree-masked forward over the prompt cache ----
+TREE_MAX_ROWS = 16384          # tree rows (prompts x N') per suffix forward: bounds its activations and the [rows, V] logits
+
+
+def score_answers(lm, input_ids, attention_mask, vis, rows, length_penalty: float, stats, dec: Decoding) -> dict:
+    """The log-probability of every answer of a trie under each prompt (``ModifiedLlamaForCausalLM.score_answers``).  ``rows``:
+    the trie's ``trie.TreeRows`` (N' nodes, A answers).  The prompts are prefilled once into a zeroed cache of
+    bucket(longest prompt + N') rows (``prefill``, mode "trie_score"); then, for chunks of prompts with at most
+    ``TREE_MAX_ROWS`` tree rows in all, the N' tree tokens of each prompt run as one suffix forward with the tree mask
+    (``forward_suffix(tree_end=...)``: node (t_1 .. t_i) holds t_i at position p_b + i - 1 and attends to the prompt and to
+    t_1 .. t_i, the keys decode steps along that path would have), the final RMSNorm and the lm_head run on the prompt's last
+    row and the tree rows, and ``ops.trie_score`` folds each answer's bf16 log-probs in fp32.  One device-to-host copy at the
+    end.  Returns dict(answers, logprob fp32 [B, A], score fp64 [B, A], best int64 [B]) on the host; score is
+    logprob / (S + d) ** length_penalty in Python floats, as ``nv_beam_select`` scores that hypothesis."""
+    N, A = rows.n, len(rows.paths)
+    if N > TREE_MAX_ROWS:
+        raise NotImplementedError(f"score_answers: a trie of {N} nodes; at most {TREE_MAX_ROWS} (TREE_MAX_ROWS) are built")
+    timer = [torch.cuda.Event(enable_timing=True) for _ in range(2)] if stats is not None else None
+    if timer:
+        timer[0].record()
+    pp, st, hid_last = prefill(lm, dec, input_ids, attention_mask, vis, N, False)
+    if timer:
+        timer[1].record()
+    dev, d, B, G, S = lm._device(), lm.dims, pp.B, st.G, int(input_ids.shape[1])
+    R = N + 1                                                  # logits rows per prompt: the prompt's last row, then the tree
+    # one host-to-device copy: tok | end | depth - 1 | path_off | path_rows (never empty, so no view has a null pointer)
+    path_off = np.concatenate([[0], np.cumsum([len(p) for p in rows.paths])])
+    path_rows = np.array([r for p in rows.paths for r in p], dtype=np.int64)
+    host = np.concatenate([rows.tok, rows.end, rows.depth - 1, path_off, path_rows, [0]]).astype(np.int32)
+    buf = torch.from_numpy(host).to(dev)
+    o = np.cumsum([0, N, N, N, A + 1, len(path_rows)])
+    tok, tree_end, dpos, poff, prow = (buf[o[i]:o[i + 1]] for i in range(5))
+    plens = torch.tensor(pp.seqlens, dtype=torch.int32, device=dev)
+    per = max(1, TREE_MAX_ROWS // max(N, 1))                   # prompts per chunk
+    norm_w, eps, E = lm.model.norm.weight.data, d.rms_eps, lm.model.embed_tokens.weight.data
+    V = lm.lm_head.weight.shape[0]
+    logprob = torch.empty((B, A), dtype=torch.float32, device=dev)
+    events, chunks = [], 0
+    for c0 in range(0, B, per):
+        c1 = min(B, c0 + per)
+        nb = c1 - c0
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)] if stats is not None else None
+        if ev:
+            ev[0].record()
+        h = torch.empty((nb, R, d.hidden), dtype=bf16, device=dev)
+        h[:, 0] = hid_last[c0:c1]
+        if N:
+            pl = plens[c0:c1]
+            x = ops.embed_fwd(tok.repeat(nb), E)
+            pos = (pl[:, None] + dpos[None, :]).view(-1)
+            cu = torch.arange(0, (nb + 1) * N, N, dtype=torch.int32, device=dev)
+            kv_start = torch.arange(0, nb * G, G, dtype=torch.int32, device=dev)
+            part = lambda caches: [(c[0][c0:c1], c[1][c0:c1]) if isinstance(c, tuple) else c[c0:c1] for c in caches]
+            h[:, 1:] = lm.core.forward_suffix(x, pos, cu, [N] * nb, part(st.kc), part(st.vc), pl, kv_start, pl + N,
+                                              tree_end=tree_end).view(nb, N, d.hidden)
+        if ev:
+            ev[1].record()
+        hn, _ = ops.rmsnorm_fwd(h.view(nb * R, d.hidden), norm_w, eps)
+        logits = logits_buffer(nb * R, V, dev)
+        lm_head_rows(lm, hn, logits)
+        ops.trie_score(logits, lm.special_ids_dev, tok, poff, prow, rows.eos, nb, logprob=logprob[c0:c1])
+        if ev:
+            ev[2].record()
+            events.append(ev)
+        chunks += 1
+    lp = logprob.cpu()
+    norm = torch.tensor([(S + len(p)) ** length_penalty for p in rows.paths], dtype=torch.float64)
+    score = lp.to(torch.float64) / norm
+    best = score.argmax(dim=1)                                 # the first of equal maxima: the lowest answer index
+    if stats is not None:
+        stats.update({"prefill_ms": timer[0].elapsed_time(timer[1]),
+                      "tree_ms": sum(e[0].elapsed_time(e[1]) for e in events),
+                      "score_ms": sum(e[1].elapsed_time(e[2]) for e in events),
+                      "tree_rows": B * N, "chunks": chunks, "prompt_lens": list(pp.seqlens)})
+    return {"answers": [list(a) for a in rows.answers], "logprob": lp, "score": score, "best": best}
 
 
 # ---- prompt-lookup speculative decoding (HF generate(prompt_lookup_num_tokens=k), greedy) ----

@@ -847,7 +847,7 @@ class LlamaCore:
     def forward_suffix(self, x: torch.Tensor, pos: torch.Tensor, cu: torch.Tensor, q_lens, kc: List[torch.Tensor],
                        vc: List[torch.Tensor], cached: torch.Tensor, kv_start: torch.Tensor, kv_len: torch.Tensor,
                        out_rows: Optional[torch.Tensor] = None, save: bool = False, acc: Optional[List[torch.Tensor]] = None,
-                       kv_lens=None, store: bool = True):
+                       kv_lens=None, store: bool = True, tree_end: Optional[torch.Tensor] = None):
         """Forward of NEW rows on top of a per-layer KV cache that already holds an encoded prefix of
         every sequence (cross-step prefix reuse, SURVEY.md §8f n1).  x: [Tn, D] packed embeddings of the new tokens,
         pos: their rotary positions, cu / q_lens: packing of the new rows, caches [B, Smax, D] (zero-initialised),
@@ -864,7 +864,12 @@ class LlamaCore:
         path on the bf16 weights (never the fp8 copy); the caches must still hold these K/V when ``backward`` runs.
         ``store=False`` (the prefix flush of ``PrefixKVCache``, which recomputes rows the cache already holds): the rows' own K/V
         are not written; the attention reads the cached ones.  The store writes packed sequence i to cache slot i, so only a
-        batch covering the slots 0..B-1 in order may store."""
+        batch covering the slots 0..B-1 in order may store.
+
+        ``tree_end`` (int32 [q_len] on the device, answer scoring): the q_len new rows of every sequence are the nodes of one
+        tree in DFS preorder (``trie.tree_rows``), and a row attends to the cached rows and to its ancestors and itself only
+        (``ops.attn_fwd_tree`` / ``ops.attn_fwd_tree_fp8``).  The rows' K/V are stored as without it; the call runs the
+        per-kernel path (inference only)."""
         d = self.d
         H, D = d.n_heads, d.hidden
         B, T = len(q_lens), x.shape[0]
@@ -873,7 +878,10 @@ class LlamaCore:
         fp8_kv = is_fp8_kv(kc)
         if save and (fp8_kv or acc is None or kv_lens is None):
             raise ValueError("forward_suffix(save=True) needs bf16 caches, the gradient accumulators and the host kv_lens")
-        if self.LAYER_CALL and not save and not fused and self.calibration is None:
+        tree = tree_end is not None
+        if tree and (save or not store):
+            raise ValueError("forward_suffix(tree_end=...) is an inference forward that stores its rows (save=False, store=True)")
+        if self.LAYER_CALL and not save and not fused and self.calibration is None and not tree:
             Bc, Smax = (kc[0][0] if fp8_kv else kc[0]).shape[:2]
             return self._layer_calls(x, pos, cu, q_lens, out_rows, a8, kc, vc, 4 if fp8_kv else 2, Smax, Bc * Smax, cached,
                                      kv_start, kv_len)
@@ -882,9 +890,14 @@ class LlamaCore:
             if fp8_kv:
                 (kq, ke), (vq, ve) = kc[l], vc[l]
                 ops.kv_store_suffix_fp8(qkv, cu, cached, kq, vq, ke, ve, B, T)
+                if tree:
+                    return ops.attn_fwd_tree_fp8(qkv[:, :D], kq, vq, ke, ve, cu, q_lens, kv_start, kv_len, tree_end, H)
                 return ops.attn_fwd_kv_fp8(qkv[:, :D], kq, vq, ke, ve, cu, q_lens, kv_start, kv_len, H)
             if store:
                 ops.kv_store_suffix(qkv, cu, cached, kc[l], vc[l], B, T)
+            if tree:
+                s.lse = None
+                return ops.attn_fwd_tree(qkv[:, :D], kc[l], vc[l], cu, q_lens, kv_start, kv_len, tree_end, H)
             s.lse = torch.empty((H, T), dtype=torch.float32, device=x.device) if save else None
             return ops.attn_fwd_kv(qkv[:, :D], kc[l], vc[l], cu, q_lens, kv_start, kv_len, H, lse=s.lse)
         x, saved = self._layers(x, pos, out_rows, save, a8, fused, attend)

@@ -1146,3 +1146,43 @@ class ModifiedLlamaForCausalLM(nn.Module):
         if stats is not None and trie is not None:
             stats.update({"trie_path": path, "trie_flatten_ms": flatten_ms if table is not None else None})
         return out
+
+    @torch.no_grad()
+    def score_answers(self, input_ids, attention_mask, trie, cand_vis=None, hist_vis=None, obj_vis=None,
+                      length_penalty: float = 1.0, stats: Optional[dict] = None) -> dict:
+        """Score every answer of ``trie`` under each prompt exactly: the ranking ``generate(trie=...)`` can only approximate
+        (greedy commits to the likeliest first token; trie beams see at most 8 answers).  An answer is a path from
+        ``trie.root`` to a childless node, tokens (t_1 .. t_d), followed by ``trie.eos``; answers are listed in DFS preorder
+        with children by ascending token id (``trie.tree_rows``).  A path that ends at a node with children is a prefix of
+        longer answers, not an answer (every trie mode allows EOS only at a childless node); a root without children gives
+        one empty answer.  ``trie`` is read as ``generate`` reads it and never modified.
+
+        ``logprob[b, a]`` (fp32) folds, in fp32 and root to leaf, the bf16 log-probs of t_1 .. t_d and EOS as beam search
+        computes them (special ids -inf, the log-softmax over the full vocabulary rounded once to bf16): the score a beam
+        following that path would carry.  ``score[b, a]`` (fp64) is logprob / (S + d) ** length_penalty, S the padded prompt
+        width, the value 4.28's beam search gives that hypothesis; ``best[b]`` its argmax, the lowest index on ties.  With
+        ``length_penalty=0``, a trie of A <= K answers without EOS edges and enough ``max_new_tokens``, ``generate(trie=trie,
+        num_beams=K, num_return_sequences=n)`` returns the n best answers by this score.
+
+        One prefill per prompt (visual tokens injected there, as in ``generate``), then every trie node of every prompt as
+        one row of a tree-masked suffix forward over the prompt cache (``generation.score_answers``).  bf16 / fp8 / int4
+        weights and the bf16 / fp8 KV cache (``set_kv_cache_dtype``) apply as in ``generate``.  Returns dict(answers: token
+        lists, logprob [B, A], score [B, A], best [B]) on the host.  A trie ``flatten_trie`` cannot represent, one whose
+        nodes are shared between parents, or one with more than ``generation.TREE_MAX_ROWS`` nodes raises
+        ``NotImplementedError``.  ``stats`` gets prefill_ms, tree_ms, score_ms, tree_rows and chunks."""
+        lp = float(length_penalty)
+        if not math.isfinite(lp):
+            raise ValueError(f"score_answers(length_penalty={length_penalty!r}): has to be a finite number")
+        self._ensure()
+        self._check_fp8_fresh()
+        self._check_int4_fresh()
+        table = trie_mod.flatten_trie(trie, self.lm_head.weight.shape[0])
+        if table is None:
+            raise NotImplementedError("score_answers: a trie= that flatten_trie cannot represent")
+        rows = trie_mod.tree_rows(table)
+        if rows is None:
+            raise NotImplementedError("score_answers: the trie shares a node between two parents; answer scoring needs a tree")
+        eos = self.tokenizer.eos_token_id
+        dec = generation.Decoding(int(eos), int(self.tokenizer.unk_token_id), True, "trie_score", self.kv_cache_dtype,
+                                  trie_eos=table.eos)
+        return generation.score_answers(self, input_ids, attention_mask, (cand_vis, hist_vis, obj_vis), rows, lp, stats, dec)

@@ -519,6 +519,8 @@ class NavModel(nn.Module):
             pp = PackedPrompt(text["input_ids"], text["attention_mask"], self.lang_model, dev, labels=self._lm_labels(text))
             vis = self.lang_model.cat_vis(cand_vis, hist_vis_input, None, pp)
             return {"loss": self.lang_model.lm_loss(pp, vis)}
+        if kwargs.get("rank_answers", False):
+            return self._rank_answers(text, cand_vis, hist_vis_input, kwargs)
         trie = kwargs.get("trie", None)
         # beam search over the answer trie: the beam kwargs reach generate() only when the caller passes them
         beams = {k: kwargs[k] for k in ("num_beams", "num_return_sequences", "length_penalty", "early_stopping") if k in kwargs}
@@ -555,12 +557,31 @@ class NavModel(nn.Module):
             vis = self.lang_model.cat_vis(cand_vis, None, None, pp)
             loss = self.lang_model.lm_loss(pp, vis)
             return LMOutput(loss=loss, logits=None, past_key_values=None, hidden_states=None, attentions=None)
+        if kwargs.pop("rank_answers", False):
+            return self._rank_answers(text, cand_vis, None, kwargs)
         ids = self.lang_model.generate(input_ids=text["input_ids"], attention_mask=text["attention_mask"], cand_vis=cand_vis,
                                        eos_token_id=self.lang_model.tokenizer.eos_token_id,
                                        pad_token_id=self.lang_model.tokenizer.unk_token_id, **kwargs).tolist()
         ids = [s[text["input_ids"].shape[1]:] for s in ids]
         return {"generated_sentences": self.lang_model.tokenizer.batch_decode(ids, skip_special_tokens=True,
                                                                               clean_up_tokenization_spaces=False)}
+
+    def _rank_answers(self, text, cand_vis, hist_vis, kwargs) -> Dict[str, Any]:
+        """``rank_answers=True`` of the summarization / embodied_qa and 3dqa modes: every answer of ``trie=`` scored under each
+        prompt (``ModifiedLlamaForCausalLM.score_answers``, ``length_penalty`` as there).  Returns generated_sentences (the
+        best answer per prompt, decoded as generated ids are), answers (every answer, decoded) and answer_scores (the fp64
+        score [B, A]).  Any other decoding kwarg raises ``ValueError``."""
+        other = sorted(k for k in kwargs if k not in ("rank_answers", "trie", "length_penalty"))
+        if other:
+            raise ValueError(f"rank_answers=True with {other[0]}=: answer ranking takes trie= and length_penalty= only")
+        if kwargs.get("trie") is None:
+            raise ValueError("rank_answers=True needs trie=: the answers to rank")
+        r = self.lang_model.score_answers(text["input_ids"], text["attention_mask"], kwargs["trie"], cand_vis=cand_vis,
+                                          hist_vis=hist_vis, length_penalty=kwargs.get("length_penalty", 1.0))
+        decode = lambda ids: self.lang_model.tokenizer.batch_decode(ids, skip_special_tokens=True,
+                                                                    clean_up_tokenization_spaces=False)
+        return {"generated_sentences": decode([r["answers"][int(i)] for i in r["best"]]), "answers": decode(r["answers"]),
+                "answer_scores": r["score"]}
 
     def forward_object_grounding(self, mode, batch: Dict[str, Any], training: bool = True, **kwargs) -> Dict[str, Any]:
         """models/nav_model.py:407-451."""

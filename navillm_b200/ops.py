@@ -160,6 +160,43 @@ def attn_fwd_kv(q: torch.Tensor, kcache: torch.Tensor, vcache: torch.Tensor, cu_
     return out
 
 
+def _tree_args(name, q_lens, tree_end):
+    """Every sequence of a tree-masked attention holds the q_len rows of one tree: tree_end int32 [q_len] on the device."""
+    n = {int(l) for l in q_lens}
+    if len(n) != 1 or tree_end.dtype != torch.int32 or tree_end.dim() != 1 or not tree_end.is_contiguous() \
+            or not tree_end.is_cuda or tree_end.numel() != next(iter(n)):
+        raise ValueError(f"{name}: every sequence needs the same number of query rows and tree_end int32 [rows] contiguous on "
+                         f"the device (got q_lens {sorted(n)}, tree_end {tree_end.dtype} {tuple(tree_end.shape)})")
+
+
+def attn_fwd_tree(q: torch.Tensor, kcache: torch.Tensor, vcache: torch.Tensor, cu_q: torch.Tensor, q_lens, kv_start: torch.Tensor,
+                  kv_len: torch.Tensor, tree_end: torch.Tensor, n_heads: int, *, out: torch.Tensor | None = None,
+                  scale: float | None = None):
+    """``attn_fwd_kv`` with the tree mask (nv_attn_fwd_tree): the q_len rows of every sequence are the nodes of one tree in DFS
+    preorder, and query i sees the kv_len - q_len >= 1 cached keys and tree key j only when j <= i < tree_end[j] (its ancestors
+    and itself; ``trie.tree_rows``).  Returns o [Tq, H*128]."""
+    _rowmajor(q, "q")
+    hd = 128
+    Tq = q.shape[0]
+    B = len(q_lens)
+    assert q.dtype == bf16 and kcache.dtype == bf16 and vcache.dtype == bf16 and kcache.is_contiguous() and vcache.is_contiguous()
+    assert kcache.dim() == 3 and kcache.shape[2] == n_heads * hd and kcache.shape == vcache.shape
+    for t in (cu_q, kv_start, kv_len):
+        assert t.dtype == torch.int32 and t.is_cuda
+    _tree_args("attn_fwd_tree", q_lens, tree_end)
+    if out is None:
+        out = torch.empty((Tq, n_heads * hd), dtype=bf16, device=q.device)
+    if scale is None:
+        scale = hd ** -0.5
+    Tkv = kcache.shape[0] * kcache.shape[1]
+    ldk = kcache.shape[2]
+    check(_lib.load().nv_attn_fwd_tree(ptr(q), i64(q.stride(0)), ptr(kcache), i64(ldk), ptr(vcache), i64(ldk), ptr(out),
+                                       i64(out.stride(0)), ptr(None), ptr(cu_q), ptr(kv_start), ptr(kv_len), ptr(tree_end), i32(B),
+                                       i32(Tq), i32(Tkv), i32(n_heads), i32(hd), i32(_qblocks(q_lens)), f32(scale), stream_ptr()),
+          "nv_attn_fwd_tree")
+    return out
+
+
 # ---------------------------------------------------------------------------------------------------
 # row-wise LM kernels (csrc/lm_ops.cu)
 # ---------------------------------------------------------------------------------------------------
@@ -706,6 +743,33 @@ def attn_fwd_kv_fp8(q: torch.Tensor, kq, vq, ke, ve, cu_q: torch.Tensor, q_lens,
     return out
 
 
+def attn_fwd_tree_fp8(q: torch.Tensor, kq, vq, ke, ve, cu_q: torch.Tensor, q_lens, kv_start: torch.Tensor, kv_len: torch.Tensor,
+                      tree_end: torch.Tensor, n_heads: int, *, out: torch.Tensor | None = None, scale: float | None = None):
+    """``attn_fwd_tree`` over an fp8 cache (the layout of ``attn_fwd_kv_fp8``): bit for bit ``attn_fwd_tree`` on bf16 caches
+    holding the rounded rows K' / V'.  Returns o [Tq, H*128] bf16."""
+    Bc, Smax, HD = _fp8_kv(kq, vq, ke, ve, "attn_fwd_tree_fp8")
+    B = len(q_lens)
+    Tq = int(sum(int(l) for l in q_lens))
+    if HD != n_heads * 128 or q.dtype != bf16 or q.dim() != 2 or q.stride(1) != 1 or q.shape[1] < HD or q.shape[0] != Tq:
+        raise ValueError(f"attn_fwd_tree_fp8: q bf16 [{Tq}, >= {HD}] and {HD // 128} heads expected "
+                         f"(got {q.dtype} {tuple(q.shape)}, {n_heads} heads)")
+    for name, t, n in (("cu_q", cu_q, B + 1), ("kv_start", kv_start, B), ("kv_len", kv_len, B)):
+        if t.dtype != torch.int32 or t.numel() != n or not t.is_cuda:
+            raise ValueError(f"attn_fwd_tree_fp8: {name} int32 [{n}] on the device expected (got {t.dtype} {tuple(t.shape)})")
+    _tree_args("attn_fwd_tree_fp8", q_lens, tree_end)
+    if out is None:
+        out = torch.empty((Tq, HD), dtype=bf16, device=q.device)
+    if out.dtype != bf16 or out.stride(1) != 1 or tuple(out.shape) != (Tq, HD):
+        raise ValueError(f"attn_fwd_tree_fp8: out bf16 [{Tq}, {HD}] expected (got {out.dtype} {tuple(out.shape)})")
+    if scale is None:
+        scale = 128 ** -0.5
+    check(_lib.load().nv_attn_fwd_tree_fp8(ptr(q), i64(q.stride(0)), ptr(kq), ptr(vq), ptr(ke), ptr(ve), ptr(out), i64(out.stride(0)),
+                                           ptr(None), ptr(cu_q), ptr(kv_start), ptr(kv_len), ptr(tree_end), i32(B), i32(Tq),
+                                           i32(Bc * Smax), i32(n_heads), i32(128), i32(_qblocks(q_lens)), f32(scale), stream_ptr()),
+          "nv_attn_fwd_tree_fp8")
+    return out
+
+
 def decode_attn_rope_fp8(qkv, lens, cos_t, sin_t, kq, vq, ke, ve, n_heads, *, out=None, scale=None):
     """``decode_attn_rope`` over an fp8 cache: the rotated k and the v of the new token are rounded to e4m3 (one exponent per
     head row) as they are appended at row lens[b]; the output equals ``decode_attn_rope`` on a bf16 cache holding the rounded
@@ -898,6 +962,37 @@ def beam_norm(S: int, G: int, length_penalty: float) -> torch.Tensor:
     """The hypothesis normalisers (S + t) ** length_penalty, t < G, in the Python float arithmetic of transformers 4.28's
     BeamHypotheses.add (host fp64 [G]; copy it to the device for ``beam_select``)."""
     return torch.tensor([(S + t) ** length_penalty for t in range(G)], dtype=torch.float64)
+
+
+def trie_score(logits, special, tok, path_off, path_rows, eos, B, *, logprob=None, stats=None):
+    """The log-probability of every answer of a trie under each of B prompts (nv_trie_score).  logits bf16 [B * R, V] (unit inner
+    stride): row b * R the prompt's next-token logits, row b * R + 1 + j those after tree row j (``trie.tree_rows``).  tok int32
+    [R - 1] the rows' tokens; path_off int32 [A + 1] / path_rows int32 the answers' rows, root to leaf; eos ends every answer.
+    Each log-prob is ``beam_topk``'s bf16 one, folded along the path in fp32.  Returns logprob fp32 [B, A]."""
+    V = logits.shape[1]
+    if logits.dtype != bf16 or logits.dim() != 2 or logits.stride(1) != 1 or not logits.is_cuda or B < 1 or logits.shape[0] % B:
+        raise ValueError(f"trie_score: bf16 logits [B * R, V] with unit inner stride on the device expected for B = {B} "
+                         f"(got {logits.dtype} {tuple(logits.shape)})")
+    R = logits.shape[0] // B
+    A = path_off.numel() - 1
+    for name, t, n in (("tok", tok, R - 1), ("path_off", path_off, None), ("path_rows", path_rows, None)):
+        if t.dtype != torch.int32 or t.dim() != 1 or not t.is_contiguous() or not t.is_cuda or (n is not None and t.numel() != n):
+            raise ValueError(f"trie_score: {name} int32 [{n if n is not None else 'n'}] contiguous on the device expected "
+                             f"(got {t.dtype} {tuple(t.shape)})")
+    if A < 1 or not 0 <= int(eos) < V:
+        raise ValueError(f"trie_score: {A} answers (>= 1) and eos {eos} in [0, {V}) expected")
+    if special.dtype != torch.int32 or not special.is_cuda:
+        raise ValueError("trie_score: special int32 on the device expected")
+    if logprob is None:
+        logprob = torch.empty((B, A), dtype=torch.float32, device=logits.device)
+    if logprob.dtype != torch.float32 or tuple(logprob.shape) != (B, A) or not logprob.is_contiguous():
+        raise ValueError(f"trie_score: logprob fp32 [{B}, {A}] contiguous expected (got {logprob.dtype} {tuple(logprob.shape)})")
+    if stats is None:
+        stats = torch.empty((B * R, 2), dtype=torch.float32, device=logits.device)
+    check(_lib.load().nv_trie_score(ptr(logits), i64(logits.stride(0)), i32(V), ptr(special), i32(special.numel()), ptr(tok),
+                                    ptr(path_off), ptr(path_rows), i32(eos), ptr(stats), ptr(logprob), i32(B), i32(R), i32(A),
+                                    stream_ptr()), "nv_trie_score")
+    return logprob
 
 
 def _beam_attn_args(name, qkv, lens, plens, src, R, K, HD, n_heads, out):

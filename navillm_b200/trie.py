@@ -108,3 +108,60 @@ def flatten_trie(trie, V: int) -> Optional[TrieTable]:
             kids.append(j)
         ptr.append(len(toks))
     return TrieTable(ptr, toks, kids, eos)
+
+
+class TreeRows:
+    """The non-root nodes of a flattened trie as the rows of one tree-masked forward (``tree_rows``), in DFS preorder with
+    children by ascending token id.  Row i holds ``tok[i]`` at ``depth[i]`` (1 for a child of the root) under ``parent[i]``
+    (-1: the root), and ``end[i]`` is the first row after its subtree, so row j is an ancestor-or-self of row i iff
+    j <= i < end[j].  An answer is a path from the root to a childless node: ``answers[a]`` its tokens, ``paths[a]`` its rows
+    (root to leaf), ``leaves[a]`` its last row (-1 for the one empty answer of a root without children).  ``eos`` ends every
+    answer.  Arrays are int32 numpy arrays of length ``n`` = N'."""
+
+    def __init__(self, tok, depth, parent, end, paths, eos: int):
+        self.tok, self.depth, self.parent, self.end = (np.asarray(a, dtype=np.int32) for a in (tok, depth, parent, end))
+        self.n = len(self.tok)
+        self.paths = paths
+        self.leaves = [p[-1] if p else -1 for p in paths]
+        self.answers = [[int(self.tok[r]) for r in p] for p in paths]
+        self.eos = eos
+
+    @property
+    def max_depth(self) -> int:
+        return int(self.depth.max()) if self.n else 0
+
+
+def tree_rows(table: TrieTable) -> Optional[TreeRows]:
+    """The tree rows of ``table`` (``TreeRows``), or None when a node is reachable from two parents (``flatten_trie`` keeps
+    one node per child object, so a trie whose child objects are shared, or a cycle, is not a tree)."""
+    seen = np.zeros(table.n_nodes, dtype=np.int64)
+    for k in table.kids:
+        seen[k] += 1
+    if table.n_nodes and (seen[0] or (seen > 1).any()):
+        return None
+    tok, depth, parent, end, paths = [], [], [], [], []
+    # iterative preorder: a frame is (node, its row, the next edge to visit)
+    stack = [(0, -1, table.ptr[0])]
+    path = []
+    while stack:
+        node, row, e = stack[-1]
+        if e == table.ptr[node + 1]:
+            stack.pop()
+            if row >= 0:
+                end[row] = len(tok)
+                path.pop()
+            continue
+        stack[-1] = (node, row, e + 1)
+        kid = table.kids[e]
+        r = len(tok)
+        tok.append(table.toks[e])
+        depth.append(len(path) + 1)
+        parent.append(row)
+        end.append(0)
+        path.append(r)
+        if table.ptr[kid + 1] == table.ptr[kid]:
+            paths.append(list(path))
+        stack.append((kid, r, table.ptr[kid]))
+    if not tok:
+        paths = [[]]
+    return TreeRows(tok, depth, parent, end, paths, table.eos)
