@@ -465,6 +465,48 @@ int nv_sample(const void* logits, int64_t ld, int V, const int* special, int n_s
 int nv_trie_mask(const void* logits, int64_t ld, void* out, int64_t ldo, int V, const int* node_ptr, const int* child_tok,
                  const int* child_node, int n_nodes, int leaf_tok, const int* special, int n_special, int* state, const int* last,
                  int* miss, int B, void* stream);
+/* Per-step scores of generate(return_dict_in_generate=True, output_scores=True): HF GenerationMixin's `scores` (transformers
+ * 4.28, the reference's pin; models/nav_model.py:388-399 reaches generate()).  The scores live in bf16 planes [G, rows,
+ * ld_scores] (plane >= rows * ld_scores elements apart); a launch writes the plane its step pointer names on the device, so a
+ * captured step writes a new plane at every replay.  Each entry below is the base entry's computation, unchanged, plus that
+ * output; the base entries launch what they launched before.
+ * nv_scores_store: rows r < R of src (ld) to plane step[0], row r, with the special ids -inf (greedy / trie / contrastive: the
+ * values nv_argmax_masked, nv_trie_mask's output or nv_contrastive_topk read, as the reference's logits carry the mask).
+ * nv_sample_scores: nv_sample, and row b of plane step[0] gets its warped scores: bf16(logit / T), -inf for the special ids and
+ * outside the top-k / top-p set (4.28 next_token_scores after logits_warper).
+ * nv_lookup_scores: after nv_lookup_accept, window row j of prompt b (logits row b * W + j) goes to plane n_prev[b] + j, row b,
+ * for every j < n_out[b] - n_prev[b] (the tokens that step emitted), special ids -inf.
+ * nv_beam_topk[_processed|_trie]_scores: beam k of prompt b writes its processed bf16 log-probs before the beam-score add
+ * (4.28 next_token_scores_processed; special ids -inf) to plane prompt_state[b, 0], row b * K + k.
+ * nv_beam_select_scores: nv_beam_select keeping 4.28's beam_indices: par_hist int32 [R, G] (each running beam's rows b * K +
+ * parent so far) is gathered by parent like hist and gets this step's parent row at t; a hypothesis added at step t stores its
+ * parent's rows and then that parent's row in hyp_par [B, K, G] (t + 1 entries); done_step[b] = t + 1 at the step prompt b
+ * becomes done (the host zeroes it). */
+int nv_scores_store(const void* src, int64_t ld, int V, const int* special, int n_special, void* scores, int64_t ld_scores,
+                    int64_t plane, const int* step, int R, void* stream);
+int nv_sample_scores(const void* logits, int64_t ld, int V, const int* special, int n_special, int* finished, int eos_id, int pad_id,
+                     int stop_on_eos, float temperature, int top_k, float top_p, const float* u, int* next, float* probs_out,
+                     void* scores, int64_t ld_scores, int64_t plane, const int* step, int B, void* stream);
+int nv_lookup_scores(const void* logits, int64_t ld, int V, const int* special, int n_special, const int* n_prev, const int* n_out,
+                     int W, void* scores, int64_t ld_scores, int64_t plane, int B, void* stream);
+int nv_beam_topk_scores(const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, const int* special, int n_special,
+                        const float* beam_score, float* cand_score, int* cand_tok, int* cand_parent, const int* prompt_state,
+                        void* scores, int64_t ld_scores, int64_t plane, int B, int K, void* stream);
+int nv_beam_topk_processed_scores(const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, const int* special, int n_special,
+                                  const float* beam_score, float* cand_score, int* cand_tok, int* cand_parent, const int* prompt_ids,
+                                  int64_t ld_ids, const int* prompt_width, const int* hist, int G, const int* prompt_state,
+                                  float penalty, int ngram, int min_length, int min_new_tokens, int eos_id, void* scores,
+                                  int64_t ld_scores, int64_t plane, int B, int K, void* stream);
+int nv_beam_topk_trie_scores(const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, const int* special, int n_special,
+                             const float* beam_score, float* cand_score, int* cand_tok, int* cand_parent, const int* prompt_ids,
+                             int64_t ld_ids, const int* prompt_width, const int* hist, int G, const int* prompt_state, float penalty,
+                             int ngram, int min_length, int min_new_tokens, int eos_id, const int* node_ptr, const int* child_tok,
+                             const int* child_node, int n_nodes, int leaf_tok, void* scores, int64_t ld_scores, int64_t plane, int B,
+                             int K, void* stream);
+int nv_beam_select_scores(const float* cand_score, const int* cand_tok, const int* cand_parent, float* beam_score, int* hist, int* src,
+                          double* hyp_score, int* hyp_meta, int* hyp_tok, int* prompt_state, int* next_ids, int* lens,
+                          const double* norm, int* par_hist, int* hyp_par, int* done_step, int B, int K, int G, int eos_id, int pad_id,
+                          int early_stopping, void* stream);
 
 /* ---- fused clip + AdamW over flat buffers (csrc/optim.cu) ------------------------------------------------------
  * torch.nn.utils.clip_grad_norm_(model.parameters(), 40.) + torch.optim.AdamW.step() of the reference

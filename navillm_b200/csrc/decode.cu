@@ -947,6 +947,65 @@ __global__ void add_int_kernel(int* __restrict__ x, int n, int delta) {
   if (i < n) x[i] += delta;
 }
 
+// ---- per-step scores (generate(return_dict_in_generate=True, output_scores=True): HF's `scores`) ----
+// The scores live in bf16 planes [G, rows, ld]; the plane a launch writes is read on the device, step[b * step_stride] (a
+// counter the captured step advances, or the beams' prompt_state), so one captured graph writes a new plane at every replay.
+struct ScoresOut {
+  __nv_bfloat16* p;
+  int64_t ld;                                // row stride
+  int64_t plane;                             // plane stride (elements)
+  const int* step;
+  int step_stride;
+  __device__ __forceinline__ __nv_bfloat16* row(int b, int r) const {
+    return p + (int64_t)step[b * step_stride] * plane + (int64_t)r * ld;
+  }
+};
+
+constexpr int SS_THREADS = 256;
+constexpr int SS_CHUNK = SS_THREADS * 8;     // columns per CTA: one 16-byte copy per thread
+
+// Columns [c0, c0 + SS_CHUNK) of one row: out = in, then the special ids among them -inf (models/modified_lm.py:121-123: the
+// reference's logits carry the mask).  16-byte copies when both rows are 16-byte aligned (the logits and scores buffers are),
+// element copies otherwise and at the row's end.
+__device__ __forceinline__ void scores_copy_chunk(const __nv_bfloat16* __restrict__ in, __nv_bfloat16* __restrict__ out, int V,
+                                                  int c0, const int* __restrict__ special, int ns) {
+  const int c = c0 + threadIdx.x * 8;
+  const bool vec = ((reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(out)) & 15) == 0;
+  if (vec && c + 8 <= V) {
+    *reinterpret_cast<uint4*>(out + c) = *reinterpret_cast<const uint4*>(in + c);
+  } else {
+    for (int i = c; i < min(c + 8, V); ++i) out[i] = in[i];
+  }
+  __syncthreads();
+  if (threadIdx.x < ns) {
+    const int sp = special[threadIdx.x];
+    if (sp >= c0 && sp < c0 + SS_CHUNK && sp < V) out[sp] = __float2bfloat16_rn(-INFINITY);
+  }
+}
+
+// Grid (R, column chunks): plane step[0], row r = src row r with the special ids -inf (greedy / trie / contrastive: the values
+// the pick reads, which mask the special ids internally).
+__global__ void __launch_bounds__(SS_THREADS) scores_store_kernel(const __nv_bfloat16* __restrict__ src, int64_t ld, int V,
+                                                                  const int* __restrict__ special, int n_special, ScoresOut so) {
+  griddep_launch();
+  griddep_wait();
+  scores_copy_chunk(src + (int64_t)blockIdx.x * ld, so.row(0, blockIdx.x), V, blockIdx.y * SS_CHUNK, special, n_special);
+}
+
+// Grid (B, W, column chunks): after nv_lookup_accept, window row j of prompt b emitted a token iff j < n_out[b] - n_prev[b]; its
+// logits (the row that picked it) go to plane n_prev[b] + j, row b, special ids -inf.
+__global__ void __launch_bounds__(SS_THREADS) lookup_scores_kernel(const __nv_bfloat16* __restrict__ logits, int64_t ld, int V,
+                                                                   const int* __restrict__ special, int n_special,
+                                                                   const int* __restrict__ n_prev, const int* __restrict__ n_out, int W,
+                                                                   __nv_bfloat16* __restrict__ scores, int64_t ld_s, int64_t plane) {
+  griddep_launch();
+  griddep_wait();
+  const int b = blockIdx.x, j = blockIdx.y, t0 = n_prev[b];
+  if (j >= n_out[b] - t0) return;                            // uniform over the CTA
+  scores_copy_chunk(logits + (int64_t)(b * W + j) * ld, scores + (int64_t)(t0 + j) * plane + (int64_t)b * ld_s, V,
+                    blockIdx.z * SS_CHUNK, special, n_special);
+}
+
 // ---- sampled decoding (HF GenerationMixin.sample as the reference reaches it with do_sample=True, tasks/agents/llava.py:58-62
 // -> models/nav_model.py:388-396): next-token scores -> TemperatureLogitsWarper (scores / T, in the logits' dtype: bf16) ->
 // TopKLogitsWarper (transformers' generation default top_k = 50: every score strictly below the k-th largest becomes -inf,
@@ -1033,12 +1092,13 @@ constexpr double SMP_FIX = 1152921504606846976.0;      // 2^60: p < 2 always, so
 __device__ __forceinline__ unsigned long long smp_fix(float p) { return (unsigned long long)((double)p * SMP_FIX); }
 __device__ __forceinline__ float smp_unfix_bf16(unsigned long long x) { return __bfloat162float(__double2bfloat16((double)x / SMP_FIX)); }
 
-__global__ void __launch_bounds__(SMP_THREADS) sample_topk_kernel(const __nv_bfloat16* __restrict__ logits, int64_t ld, int V,
-                                                                  const int* __restrict__ special, int n_special,
-                                                                  int* __restrict__ finished, int eos_id, int pad_id, int stop_on_eos,
-                                                                  float temperature, int top_k, int use_top_p, float p_thr,
-                                                                  const float* __restrict__ u, int* __restrict__ next,
-                                                                  float* __restrict__ probs_out) {
+// SCORES (nv_sample_scores): the warped bf16 scores -- bf16(logit / T), -inf for the special ids and outside the kept set of
+// top-k / top-p (4.28's next_token_scores after logits_warper) -- also go to so.row(0, b).
+template <bool SCORES>
+__device__ __forceinline__ void sample_body(const __nv_bfloat16* __restrict__ logits, int64_t ld, int V, const int* __restrict__ special,
+                                            int n_special, int* __restrict__ finished, int eos_id, int pad_id, int stop_on_eos,
+                                            float temperature, int top_k, int use_top_p, float p_thr, const float* __restrict__ u,
+                                            int* __restrict__ next, float* __restrict__ probs_out, const ScoresOut& so) {
   extern __shared__ float sc[];                              // [V] scores, then probabilities
   __shared__ int hist[256];
   __shared__ float red[32];
@@ -1092,11 +1152,14 @@ __global__ void __launch_bounds__(SMP_THREADS) sample_topk_kernel(const __nv_bfl
   for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
   __syncthreads();
   float denom;
+  __nv_bfloat16* srow = nullptr;
+  if constexpr (SCORES) srow = so.row(0, b);
   if (!use_top_p) {
     float part = 0.f;
     for (int c = tid; c < V; c += SMP_THREADS) {
       const float v = sc[c];
       const float e = (smp_key16(v) >= thr_key && v > -INFINITY) ? expf(v - mx) : 0.f;
+      if constexpr (SCORES) srow[c] = __float2bfloat16_rn((smp_key16(v) >= thr_key && v > -INFINITY) ? v : -INFINITY);
       sc[c] = e;
       part += e;
     }
@@ -1219,6 +1282,7 @@ __global__ void __launch_bounds__(SMP_THREADS) sample_topk_kernel(const __nv_bfl
       const uint32_t key = smp_key16(v);
       const bool keep = key >= thr_key && v > -INFINITY && (key > ck || (key == ck && c >= ci));
       const float e = keep ? expf(v - mx) : 0.f;
+      if constexpr (SCORES) srow[c] = __float2bfloat16_rn(keep ? v : -INFINITY);
       sc[c] = e;
       part += e;
     }
@@ -1271,6 +1335,26 @@ __global__ void __launch_bounds__(SMP_THREADS) sample_topk_kernel(const __nv_bfl
     else if (stop_on_eos && tok == eos_id) finished[b] = 1;
     next[b] = tok;
   }
+}
+
+__global__ void __launch_bounds__(SMP_THREADS) sample_topk_kernel(const __nv_bfloat16* __restrict__ logits, int64_t ld, int V,
+                                                                  const int* __restrict__ special, int n_special,
+                                                                  int* __restrict__ finished, int eos_id, int pad_id, int stop_on_eos,
+                                                                  float temperature, int top_k, int use_top_p, float p_thr,
+                                                                  const float* __restrict__ u, int* __restrict__ next,
+                                                                  float* __restrict__ probs_out) {
+  sample_body<false>(logits, ld, V, special, n_special, finished, eos_id, pad_id, stop_on_eos, temperature, top_k, use_top_p, p_thr,
+                     u, next, probs_out, ScoresOut{});
+}
+
+__global__ void __launch_bounds__(SMP_THREADS) sample_scores_kernel(const __nv_bfloat16* __restrict__ logits, int64_t ld, int V,
+                                                                    const int* __restrict__ special, int n_special,
+                                                                    int* __restrict__ finished, int eos_id, int pad_id,
+                                                                    int stop_on_eos, float temperature, int top_k, int use_top_p,
+                                                                    float p_thr, const float* __restrict__ u, int* __restrict__ next,
+                                                                    float* __restrict__ probs_out, ScoresOut so) {
+  sample_body<true>(logits, ld, V, special, n_special, finished, eos_id, pad_id, stop_on_eos, temperature, top_k, use_top_p, p_thr,
+                    u, next, probs_out, so);
 }
 
 // ---- logits processors (transformers 4.28 _get_logits_processor order: RepetitionPenaltyLogitsProcessor,
@@ -1431,11 +1515,14 @@ __device__ __forceinline__ int trie_walk(const BeamTrie& tr, const int* __restri
   return node;
 }
 
-template <bool PROC, bool TRIE = false>
+// SCORES (nv_beam_topk*_scores): each beam's processed bf16 log-probs before the beam-score add (4.28's
+// next_token_scores_processed; special ids -inf) also go to so.row(b, b * K + k), the plane of step t = prompt_state[b, 0].
+template <bool PROC, bool TRIE = false, bool SCORES = false>
 __device__ __forceinline__ void beam_topk_body(const __nv_bfloat16* __restrict__ logits, int64_t ld_prompt, int64_t ld_beam, int V,
                                                const int* __restrict__ special, int n_special, const float* __restrict__ beam_score,
                                                 int K, float* __restrict__ cand_score, int* __restrict__ cand_tok,
-                                               int* __restrict__ cand_par, const BeamProc& bp, const BeamTrie& tr = BeamTrie{}) {
+                                               int* __restrict__ cand_par, const BeamProc& bp, const BeamTrie& tr = BeamTrie{},
+                                               const ScoresOut& so = ScoresOut{}) {
   static_assert(PROC || !TRIE, "the trie mask runs inside the processed scan");
   __shared__ int s_special[MAX_SPECIAL];
   __shared__ float s_m[BEAM_MAX], s_ls[BEAM_MAX], s_bs[BEAM_MAX];
@@ -1489,6 +1576,8 @@ __device__ __forceinline__ void beam_topk_body(const __nv_bfloat16* __restrict__
   for (int k = 0; k < K; ++k) {
     const __nv_bfloat16* row = logits + (int64_t)b * ld_prompt + (int64_t)k * ld_beam;
     const float m = s_m[k], ls = s_ls[k], bs = s_bs[k];
+    __nv_bfloat16* srow = nullptr;
+    if constexpr (SCORES) srow = so.row(b, b * K + k);
     uint32_t* seen = nullptr;
     uint32_t* banned = nullptr;
     uint32_t* allowed = nullptr;
@@ -1538,10 +1627,23 @@ __device__ __forceinline__ void beam_topk_body(const __nv_bfloat16* __restrict__
           if (banned[c >> 5] & bit) lp = -INFINITY;
           if constexpr (TRIE)
             if (!(allowed[c >> 5] & bit)) lp = -INFINITY;
+          if constexpr (SCORES) srow[c] = __float2bfloat16_rn(lp);
           sc = lp + bs;
+        } else if constexpr (SCORES) {
+          srow[c] = __float2bfloat16_rn(-INFINITY);
         }
       } else {
-        if (!is_special(c)) sc = bf16_round((__bfloat162float(row[c]) - m) - ls) + bs;
+        if constexpr (SCORES) {
+          if (!is_special(c)) {
+            const float lp = bf16_round((__bfloat162float(row[c]) - m) - ls);
+            srow[c] = __float2bfloat16_rn(lp);
+            sc = lp + bs;
+          } else {
+            srow[c] = __float2bfloat16_rn(-INFINITY);
+          }
+        } else {
+          if (!is_special(c)) sc = bf16_round((__bfloat162float(row[c]) - m) - ls) + bs;
+        }
       }
       if (sc != sc) sc = -INFINITY;
       const unsigned long long key =
@@ -1611,6 +1713,37 @@ __global__ void __launch_bounds__(BT_THREADS, 1) beam_topk_trie_kernel(const __n
                                                                        float* __restrict__ cand_score, int* __restrict__ cand_tok,
                                                                        int* __restrict__ cand_par, BeamProc bp, BeamTrie tr) {
   beam_topk_body<true, true>(logits, ld_prompt, ld_beam, V, special, n_special, beam_score, K, cand_score, cand_tok, cand_par, bp, tr);
+}
+
+// the three beam top-k kernels with the SCORES output (nv_beam_topk*_scores); bounds as above
+__global__ void __launch_bounds__(BT_THREADS) beam_topk_scores_kernel(const __nv_bfloat16* __restrict__ logits, int64_t ld_prompt,
+                                                                      int64_t ld_beam, int V, const int* __restrict__ special,
+                                                                      int n_special, const float* __restrict__ beam_score, int K,
+                                                                      float* __restrict__ cand_score, int* __restrict__ cand_tok,
+                                                                      int* __restrict__ cand_par, ScoresOut so) {
+  beam_topk_body<false, false, true>(logits, ld_prompt, ld_beam, V, special, n_special, beam_score, K, cand_score, cand_tok, cand_par,
+                                     BeamProc{}, BeamTrie{}, so);
+}
+
+__global__ void __launch_bounds__(BT_THREADS, 1) beam_topk_proc_scores_kernel(const __nv_bfloat16* __restrict__ logits,
+                                                                              int64_t ld_prompt, int64_t ld_beam, int V,
+                                                                              const int* __restrict__ special, int n_special,
+                                                                              const float* __restrict__ beam_score, int K,
+                                                                              float* __restrict__ cand_score, int* __restrict__ cand_tok,
+                                                                              int* __restrict__ cand_par, BeamProc bp, ScoresOut so) {
+  beam_topk_body<true, false, true>(logits, ld_prompt, ld_beam, V, special, n_special, beam_score, K, cand_score, cand_tok, cand_par,
+                                    bp, BeamTrie{}, so);
+}
+
+__global__ void __launch_bounds__(BT_THREADS, 1) beam_topk_trie_scores_kernel(const __nv_bfloat16* __restrict__ logits,
+                                                                              int64_t ld_prompt, int64_t ld_beam, int V,
+                                                                              const int* __restrict__ special, int n_special,
+                                                                              const float* __restrict__ beam_score, int K,
+                                                                              float* __restrict__ cand_score, int* __restrict__ cand_tok,
+                                                                              int* __restrict__ cand_par, BeamProc bp, BeamTrie tr,
+                                                                              ScoresOut so) {
+  beam_topk_body<true, true, true>(logits, ld_prompt, ld_beam, V, special, n_special, beam_score, K, cand_score, cand_tok, cand_par,
+                                   bp, tr, so);
 }
 
 // ---- answer scoring (nv_trie_score): every answer of a trie teacher-forced over one tree-masked forward ----
@@ -1711,14 +1844,22 @@ constexpr int BS_THREADS = 128, BS_CHUNK = 256;
 // (S + t) ** length_penalty as the host's Python floats compute it (S padded prompt columns: hyp.shape[-1] in 4.28), so the fp64
 // hypothesis scores sum_logprobs / norm[t] are 4.28's to the bit.  hyp_score [B, K + 1] holds the K kept scores and the worst kept score, hyp_meta [B, K, 2] (generated
 // length, insertion number: the later of equal scores wins in finalize), hyp_tok [B, K, G] their generated tokens.
-__global__ void __launch_bounds__(BS_THREADS) beam_select_kernel(const float* __restrict__ cand_score, const int* __restrict__ cand_tok,
-                                                                 const int* __restrict__ cand_par, float* __restrict__ beam_score,
-                                                                 int* __restrict__ hist, int* __restrict__ src,
-                                                                 double* __restrict__ hyp_score, int* __restrict__ hyp_meta,
-                                                                 int* __restrict__ hyp_tok, int* __restrict__ pstate,
-                                                                 int* __restrict__ next_ids, int* __restrict__ lens,
-                                                                 const double* __restrict__ norm, int K, int G, int eos_id, int pad_id,
-                                                                 int early_stopping) {
+// SCORES (nv_beam_select_scores): 4.28's beam_indices as well.  par_hist [R, G] holds each running beam's rows (b * K + parent)
+// of the steps so far and is gathered by parent like hist; a hypothesis added at step t gets its parent's rows and then that
+// parent's row at t in hyp_par [B, K, G]; done_step[b] = t + 1 at the step prompt b becomes done.
+struct BeamTrace {
+  int* par_hist;
+  int* hyp_par;
+  int* done_step;
+};
+
+template <bool SCORES>
+__device__ __forceinline__ void beam_select_body(const float* __restrict__ cand_score, const int* __restrict__ cand_tok,
+                                                 const int* __restrict__ cand_par, float* __restrict__ beam_score,
+                                                 int* __restrict__ hist, int* __restrict__ src, double* __restrict__ hyp_score,
+                                                 int* __restrict__ hyp_meta, int* __restrict__ hyp_tok, int* __restrict__ pstate,
+                                                 int* __restrict__ next_ids, int* __restrict__ lens, const double* __restrict__ norm,
+                                                 int K, int G, int eos_id, int pad_id, int early_stopping, const BeamTrace& tr) {
   __shared__ int s_tok[BEAM_MAX], s_par[BEAM_MAX];
   __shared__ float s_sc[BEAM_MAX];
   __shared__ int s_op_slot[BEAM_MAX], s_op_par[BEAM_MAX], s_nops;
@@ -1775,6 +1916,8 @@ __global__ void __launch_bounds__(BS_THREADS) beam_select_kernel(const float* __
       }
       int done = 0;
       if (cnt >= K) done = early_stopping ? 1 : (worst >= (double)cand_score[b * 2 * K] / nt);
+      if constexpr (SCORES)
+        if (done) tr.done_step[b] = t + 1;
       hs[K] = worst;
       ps[BS_COUNT] = cnt;
       ps[BS_SEQ] = seq;
@@ -1787,6 +1930,12 @@ __global__ void __launch_bounds__(BS_THREADS) beam_select_kernel(const float* __
     const int* from = hist + (int64_t)(b * K + s_op_par[o]) * G;
     int* to = hyp_tok + (int64_t)(b * K + s_op_slot[o]) * G;
     for (int i = tid; i < t; i += BS_THREADS) to[i] = from[i];
+    if constexpr (SCORES) {
+      const int* pf = tr.par_hist + (int64_t)(b * K + s_op_par[o]) * G;
+      int* pt = tr.hyp_par + (int64_t)(b * K + s_op_slot[o]) * G;
+      for (int i = tid; i < t; i += BS_THREADS) pt[i] = pf[i];
+      if (tid == 0) pt[t] = b * K + s_op_par[o];
+    }
   }
   for (int c0 = 0; c0 < t; c0 += BS_CHUNK) {                     // rows of the new beams = rows of their parents
     const int n = min(BS_CHUNK, t - c0);
@@ -1809,8 +1958,24 @@ __global__ void __launch_bounds__(BS_THREADS) beam_select_kernel(const float* __
     }
     __syncthreads();
   }
+  if constexpr (SCORES) {
+    for (int c0 = 0; c0 < t; c0 += BS_CHUNK) {                   // par_hist by parent, through s_h
+      const int n = min(BS_CHUNK, t - c0);
+      for (int idx = tid; idx < K * BS_CHUNK; idx += BS_THREADS) {
+        const int j = idx / BS_CHUNK, i = idx % BS_CHUNK;
+        if (i < n) s_h[j][i] = tr.par_hist[(int64_t)(b * K + s_par[j]) * G + c0 + i];
+      }
+      __syncthreads();
+      for (int idx = tid; idx < K * BS_CHUNK; idx += BS_THREADS) {
+        const int j = idx / BS_CHUNK, i = idx % BS_CHUNK;
+        if (i < n) tr.par_hist[(int64_t)(b * K + j) * G + c0 + i] = s_h[j][i];
+      }
+      __syncthreads();
+    }
+  }
   if (tid < K) {
     const int r = b * K + tid;
+    if constexpr (SCORES) tr.par_hist[(int64_t)r * G + t] = b * K + s_par[tid];
     hist[(int64_t)r * G + t] = s_tok[tid];
     src[(int64_t)r * G + t] = r;                                 // the next step writes generated key t of row r at (r, t)
     next_ids[r] = s_tok[tid];
@@ -1819,6 +1984,30 @@ __global__ void __launch_bounds__(BS_THREADS) beam_select_kernel(const float* __
   }
   __syncthreads();
   if (tid == 0) ps[BS_STEP] = t + 1;
+}
+
+__global__ void __launch_bounds__(BS_THREADS) beam_select_kernel(const float* __restrict__ cand_score, const int* __restrict__ cand_tok,
+                                                                 const int* __restrict__ cand_par, float* __restrict__ beam_score,
+                                                                 int* __restrict__ hist, int* __restrict__ src,
+                                                                 double* __restrict__ hyp_score, int* __restrict__ hyp_meta,
+                                                                 int* __restrict__ hyp_tok, int* __restrict__ pstate,
+                                                                 int* __restrict__ next_ids, int* __restrict__ lens,
+                                                                 const double* __restrict__ norm, int K, int G, int eos_id, int pad_id,
+                                                                 int early_stopping) {
+  beam_select_body<false>(cand_score, cand_tok, cand_par, beam_score, hist, src, hyp_score, hyp_meta, hyp_tok, pstate, next_ids, lens,
+                          norm, K, G, eos_id, pad_id, early_stopping, BeamTrace{});
+}
+
+__global__ void __launch_bounds__(BS_THREADS) beam_select_scores_kernel(const float* __restrict__ cand_score,
+                                                                        const int* __restrict__ cand_tok, const int* __restrict__ cand_par,
+                                                                        float* __restrict__ beam_score, int* __restrict__ hist,
+                                                                        int* __restrict__ src, double* __restrict__ hyp_score,
+                                                                        int* __restrict__ hyp_meta, int* __restrict__ hyp_tok,
+                                                                        int* __restrict__ pstate, int* __restrict__ next_ids,
+                                                                        int* __restrict__ lens, const double* __restrict__ norm, int K,
+                                                                        int G, int eos_id, int pad_id, int early_stopping, BeamTrace tr) {
+  beam_select_body<true>(cand_score, cand_tok, cand_par, beam_score, hist, src, hyp_score, hyp_meta, hyp_tok, pstate, next_ids, lens,
+                         norm, K, G, eos_id, pad_id, early_stopping, tr);
 }
 
 // ---- contrastive search (GenerationMixin.contrastive_search / _ranking_fast of transformers 4.28) ----
@@ -2353,6 +2542,61 @@ int nv_sample_topk(const void* logits, int64_t ld, int V, const int* special, in
                    probs_out, B, stream);
 }
 
+static int check_scores(const char* name, const void* scores, int64_t ld_scores, int64_t plane, const int* step, int V, int rows) {
+  NV_REQUIRE(scores && step && ld_scores >= V && plane >= (int64_t)rows * ld_scores,
+             "%s: scores planes [G, %d, ld_scores >= %d] and a step pointer expected (ld_scores=%lld, plane=%lld)", name, rows, V,
+             (long long)ld_scores, (long long)plane);
+  return NV_OK;
+}
+
+// nv_sample that also writes the warped scores of each row to plane step[0] of scores (see sample_body<true>).  The argument
+// checks are nv_sample's (its B = 0 call launches nothing).
+int nv_sample_scores(const void* logits, int64_t ld, int V, const int* special, int n_special, int* finished, int eos_id, int pad_id,
+                     int stop_on_eos, float temperature, int top_k, float top_p, const float* u, int* next, float* probs_out,
+                     void* scores, int64_t ld_scores, int64_t plane, const int* step, int B, void* stream) {
+  int st = nv_sample(logits, ld, V, special, n_special, finished, eos_id, pad_id, stop_on_eos, temperature, top_k, top_p, u, next,
+                     probs_out, 0, stream);
+  if (st == NV_OK) st = check_scores("nv_sample_scores", scores, ld_scores, plane, step, V, B);
+  if (st != NV_OK || B == 0) return st;
+  static bool attr_set = false;
+  if (!attr_set) {
+    NV_CUDA(cudaFuncSetAttribute(sample_scores_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    attr_set = true;
+  }
+  const float p_thr = __bfloat162float(__float2bfloat16_rn((float)(1.0 - (double)top_p)));
+  sample_scores_kernel<<<B, SMP_THREADS, (size_t)V * 4, S_(stream)>>>(CBF(logits), ld, V, special, n_special, finished, eos_id, pad_id,
+                                                                       stop_on_eos, temperature, top_k, top_p < 1.f ? 1 : 0, p_thr, u,
+                                                                       next, probs_out, ScoresOut{BF(scores), ld_scores, plane, step, 0});
+  NV_LAUNCH_CHECK();
+  return NV_OK;
+}
+
+// R rows of src to plane step[0] of scores, special ids -inf (see scores_store_kernel).
+int nv_scores_store(const void* src, int64_t ld, int V, const int* special, int n_special, void* scores, int64_t ld_scores,
+                    int64_t plane, const int* step, int R, void* stream) {
+  NV_REQUIRE(src && V > 0 && ld >= V && R >= 0 && n_special >= 0 && n_special <= MAX_SPECIAL && (special || n_special == 0),
+             "nv_scores_store: bad arguments (V=%d ld=%lld R=%d n_special=%d)", V, (long long)ld, R, n_special);
+  const int st = check_scores("nv_scores_store", scores, ld_scores, plane, step, V, R);
+  if (st != NV_OK || R == 0) return st;
+  NV_CUDA(launch_pdl(scores_store_kernel, dim3(R, (V + SS_CHUNK - 1) / SS_CHUNK), dim3(SS_THREADS), 0, S_(stream), CBF(src), ld, V,
+                     special, n_special,
+                     ScoresOut{BF(scores), ld_scores, plane, step, 0}));
+  return NV_OK;
+}
+
+// After nv_lookup_accept: the logits rows of the emitted tokens to their planes (see lookup_scores_kernel).
+int nv_lookup_scores(const void* logits, int64_t ld, int V, const int* special, int n_special, const int* n_prev, const int* n_out,
+                     int W, void* scores, int64_t ld_scores, int64_t plane, int B, void* stream) {
+  NV_REQUIRE(logits && n_prev && n_out && scores && V > 0 && ld >= V && ld_scores >= V && plane >= (int64_t)B * ld_scores && W >= 1 &&
+             W <= WIN_MAX && B >= 0 && n_special >= 0 && n_special <= MAX_SPECIAL && (special || n_special == 0),
+             "nv_lookup_scores: bad arguments (V=%d W=%d B=%d ld_scores=%lld plane=%lld)", V, W, B, (long long)ld_scores,
+             (long long)plane);
+  if (B == 0) return NV_OK;
+  NV_CUDA(launch_pdl(lookup_scores_kernel, dim3(B, W, (V + SS_CHUNK - 1) / SS_CHUNK), dim3(SS_THREADS), 0, S_(stream), CBF(logits),
+                     ld, V, special, n_special, n_prev, n_out, W, BF(scores), ld_scores, plane));
+  return NV_OK;
+}
+
 // Trie mask of the next-token logits (see trie_mask_kernel).  logits [B, V] bf16 (ld), out [B, V] bf16 (ldo % 8 == 0, 16-byte
 // aligned base), state int32 [B] node per row, last int32 [B] or null (no advance), miss int32 [1] (set, never cleared).
 int nv_trie_mask(const void* logits, int64_t ld, void* out, int64_t ldo, int V, const int* node_ptr, const int* child_tok,
@@ -2384,6 +2628,20 @@ int nv_beam_topk(const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, 
   if (B == 0) return NV_OK;
   NV_CUDA(launch_pdl(beam_topk_kernel, dim3(B), dim3(BT_THREADS), 0, S_(stream), CBF(logits), ld_prompt, ld_beam, V, special,
                      n_special, beam_score, K, cand_score, cand_tok, cand_parent));
+  return NV_OK;
+}
+
+// nv_beam_topk that also writes each beam's bf16 log-probs to plane prompt_state[b, 0] of scores [G, B * K, ld_scores] (see
+// beam_topk_body<..., true>).  The argument checks are nv_beam_topk's (its B = 0 call launches nothing).
+int nv_beam_topk_scores(const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, const int* special, int n_special,
+                        const float* beam_score, float* cand_score, int* cand_tok, int* cand_parent, const int* prompt_state,
+                        void* scores, int64_t ld_scores, int64_t plane, int B, int K, void* stream) {
+  int st = nv_beam_topk(logits, ld_prompt, ld_beam, V, special, n_special, beam_score, cand_score, cand_tok, cand_parent, 0, K, stream);
+  if (st == NV_OK) st = check_scores("nv_beam_topk_scores", scores, ld_scores, plane, prompt_state, V, B * K);
+  if (st != NV_OK || B == 0) return st;
+  NV_CUDA(launch_pdl(beam_topk_scores_kernel, dim3(B), dim3(BT_THREADS), 0, S_(stream), CBF(logits), ld_prompt, ld_beam, V, special,
+                     n_special, beam_score, K, cand_score, cand_tok, cand_parent,
+                     ScoresOut{BF(scores), ld_scores, plane, prompt_state, BS_FIELDS}));
   return NV_OK;
 }
 
@@ -2432,6 +2690,24 @@ int nv_beam_topk_processed(const void* logits, int64_t ld_prompt, int64_t ld_bea
   return NV_OK;
 }
 
+// nv_beam_topk_processed with the scores output of nv_beam_topk_scores.
+int nv_beam_topk_processed_scores(const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, const int* special, int n_special,
+                                  const float* beam_score, float* cand_score, int* cand_tok, int* cand_parent, const int* prompt_ids,
+                                  int64_t ld_ids, const int* prompt_width, const int* hist, int G, const int* prompt_state,
+                                  float penalty, int ngram, int min_length, int min_new_tokens, int eos_id, void* scores,
+                                  int64_t ld_scores, int64_t plane, int B, int K, void* stream) {
+  int st = nv_beam_topk_processed(logits, ld_prompt, ld_beam, V, special, n_special, beam_score, cand_score, cand_tok, cand_parent,
+                                  prompt_ids, ld_ids, prompt_width, hist, G, prompt_state, penalty, ngram, min_length, min_new_tokens,
+                                  eos_id, 0, K, stream);
+  if (st == NV_OK) st = check_scores("nv_beam_topk_processed_scores", scores, ld_scores, plane, prompt_state, V, B * K);
+  if (st != NV_OK || B == 0) return st;
+  const BeamProc bp{prompt_ids, ld_ids, prompt_width, hist, G, prompt_state, ProcParams{penalty, ngram, min_length, min_new_tokens, eos_id}};
+  NV_CUDA(launch_pdl(beam_topk_proc_scores_kernel, dim3(B), dim3(BT_THREADS), (size_t)((V + 31) / 32) * 4 * 2, S_(stream),
+                     CBF(logits), ld_prompt, ld_beam, V, special, n_special, beam_score, K, cand_score, cand_tok, cand_parent, bp,
+                     ScoresOut{BF(scores), ld_scores, plane, prompt_state, BS_FIELDS}));
+  return NV_OK;
+}
+
 // nv_beam_topk_processed with the trie mask after the processors (see beam_topk_trie_kernel).  The CSR trie as nv_trie_mask
 // reads it; V must fit three V-bit bitmaps in 48 KB.
 int nv_beam_topk_trie(const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, const int* special, int n_special,
@@ -2461,6 +2737,26 @@ int nv_beam_topk_trie(const void* logits, int64_t ld_prompt, int64_t ld_beam, in
   return NV_OK;
 }
 
+// nv_beam_topk_trie with the scores output of nv_beam_topk_scores.
+int nv_beam_topk_trie_scores(const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, const int* special, int n_special,
+                             const float* beam_score, float* cand_score, int* cand_tok, int* cand_parent, const int* prompt_ids,
+                             int64_t ld_ids, const int* prompt_width, const int* hist, int G, const int* prompt_state, float penalty,
+                             int ngram, int min_length, int min_new_tokens, int eos_id, const int* node_ptr, const int* child_tok,
+                             const int* child_node, int n_nodes, int leaf_tok, void* scores, int64_t ld_scores, int64_t plane, int B,
+                             int K, void* stream) {
+  int st = nv_beam_topk_trie(logits, ld_prompt, ld_beam, V, special, n_special, beam_score, cand_score, cand_tok, cand_parent,
+                             prompt_ids, ld_ids, prompt_width, hist, G, prompt_state, penalty, ngram, min_length, min_new_tokens, eos_id,
+                             node_ptr, child_tok, child_node, n_nodes, leaf_tok, 0, K, stream);
+  if (st == NV_OK) st = check_scores("nv_beam_topk_trie_scores", scores, ld_scores, plane, prompt_state, V, B * K);
+  if (st != NV_OK || B == 0) return st;
+  const BeamProc bp{prompt_ids, ld_ids, prompt_width, hist, G, prompt_state, ProcParams{penalty, ngram, min_length, min_new_tokens, eos_id}};
+  const BeamTrie tr{node_ptr, child_tok, child_node, n_nodes, leaf_tok};
+  NV_CUDA(launch_pdl(beam_topk_trie_scores_kernel, dim3(B), dim3(BT_THREADS), (size_t)((V + 31) / 32) * 4 * 3, S_(stream),
+                     CBF(logits), ld_prompt, ld_beam, V, special, n_special, beam_score, K, cand_score, cand_tok, cand_parent, bp, tr,
+                     ScoresOut{BF(scores), ld_scores, plane, prompt_state, BS_FIELDS}));
+  return NV_OK;
+}
+
 // nv_trie_score: see include/navillm_b200.h.
 int nv_trie_score(const void* logits, int64_t ld, int V, const int* special, int n_special, const int* tok, const int* path_off,
                   const int* path_rows, int eos, float* stats, float* logprob, int B, int R, int A, void* stream) {
@@ -2487,6 +2783,21 @@ int nv_beam_select(const float* cand_score, const int* cand_tok, const int* cand
   NV_CUDA(launch_pdl(beam_select_kernel, dim3(B), dim3(BS_THREADS), 0, S_(stream), cand_score, cand_tok, cand_parent, beam_score,
                      hist, src, hyp_score, hyp_meta, hyp_tok, prompt_state, next_ids, lens, norm, K, G, eos_id, pad_id,
                      early_stopping));
+  return NV_OK;
+}
+
+// nv_beam_select that also keeps 4.28's beam_indices: par_hist [R, G], hyp_par [B, K, G], done_step [B] (see beam_select_body<true>).
+int nv_beam_select_scores(const float* cand_score, const int* cand_tok, const int* cand_parent, float* beam_score, int* hist, int* src,
+                          double* hyp_score, int* hyp_meta, int* hyp_tok, int* prompt_state, int* next_ids, int* lens,
+                          const double* norm, int* par_hist, int* hyp_par, int* done_step, int B, int K, int G, int eos_id, int pad_id,
+                          int early_stopping, void* stream) {
+  NV_REQUIRE(par_hist && hyp_par && done_step, "nv_beam_select_scores: null argument");
+  const int st = nv_beam_select(cand_score, cand_tok, cand_parent, beam_score, hist, src, hyp_score, hyp_meta, hyp_tok, prompt_state,
+                                next_ids, lens, norm, 0, K, G, eos_id, pad_id, early_stopping, stream);
+  if (st != NV_OK || B == 0) return st;
+  NV_CUDA(launch_pdl(beam_select_scores_kernel, dim3(B), dim3(BS_THREADS), 0, S_(stream), cand_score, cand_tok, cand_parent,
+                     beam_score, hist, src, hyp_score, hyp_meta, hyp_tok, prompt_state, next_ids, lens, norm, K, G, eos_id, pad_id,
+                     early_stopping, BeamTrace{par_hist, hyp_par, done_step}));
   return NV_OK;
 }
 

@@ -39,6 +39,7 @@ class Decoding:
     penalty_alpha: Optional[float] = None    # contrastive search: the degeneration penalty's weight
     lookup_k: Optional[int] = None           # prompt-lookup decoding: drafts per step (the window is lookup_k + 1 rows)
     lookup_ngram: Optional[int] = None       # prompt-lookup decoding: max_matching_ngram_size
+    scores: bool = False                     # return_dict_in_generate + output_scores: the step stores HF's per-step scores
 
     @property
     def sampled(self) -> bool:
@@ -47,7 +48,7 @@ class Decoding:
     def key(self) -> tuple:
         """The graph key: every field a captured step bakes in (not ``n_return`` or ``length_penalty``), the format last."""
         return (self.eos, self.pad, self.stop_on_eos, self.mode, self.temperature, self.top_k, self.top_p, self.trie_eos, self.n,
-                self.early_stopping, self.proc, self.penalty_alpha, self.lookup_k, self.lookup_ngram, self.kv)
+                self.early_stopping, self.proc, self.penalty_alpha, self.lookup_k, self.lookup_ngram, self.scores, self.kv)
 
 
 def processors(repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens, eos: int) -> Optional[tuple]:
@@ -120,6 +121,26 @@ def load_trie(st, table) -> tuple:
     return st.trie_buf[:o], st.trie_buf[o:o + ecap], st.trie_buf[o + ecap:], ncap
 
 
+def load_scores(st, planes: int, rows: int, V: int) -> None:
+    """The per-step scores of a ``dec.scores`` call in persistent buffers of ``st``: ``st.scores`` bf16 [>= planes, rows, V]
+    (``ops.scores_buffer``; a captured step writes plane ``st.score_t[0]`` and advances it, so the counter is zeroed here) and
+    ``st.score_prev`` int32 [rows] (prompt lookup: the columns emitted before a step)."""
+    dev = st.next_ids.device
+
+    def alloc(cap):
+        st.scores = ops.scores_buffer(cap, rows, V, dev)
+        st.score_t = torch.zeros((1,), dtype=torch.int32, device=dev)
+        st.score_prev = torch.zeros((rows,), dtype=torch.int32, device=dev)
+    _grow(st, "score_cap", (max(planes, 1),), alloc)
+    st.score_t.zero_()
+
+
+def take_scores(st, n: int) -> tuple:
+    """HF's ``scores`` tuple: the first ``n`` planes copied once into a fresh tensor (the next call reuses the state's
+    buffer), one [rows, V] entry per plane."""
+    return tuple(st.scores[:n].clone().unbind(0))
+
+
 def load_proc(st, input_ids, rows: int, G: int) -> None:
     """The logits processors' device state in persistent buffers of ``st``: the padded prompt ids ``proc_ids`` [P, >= S] and
     their width S ``proc_width`` [1], copied once per call, and -- for ``rows`` > 0 -- the generated history ``proc_hist``
@@ -188,6 +209,8 @@ def prefill(lm, dec: Decoding, input_ids, attention_mask, vis, max_new_tokens: i
             st.beam_score, st.cand_score, st.cand_tok = zeros(torch.float32, R), zeros(torch.float32, B, 2 * n), i32(B, 2 * n)
             st.cand_par, st.hist, st.src, st.hyp_score = i32(B, 2 * n), i32(R, G), i32(R, G), zeros(torch.float64, B, n + 1)
             st.hyp_meta, st.hyp_tok, st.pstate, st.norm = i32(B, n, 2), i32(B, n, G), i32(B, 5), zeros(torch.float64, G)
+            if dec.scores:                                                  # 4.28's beam_indices (ops.beam_select trace=)
+                st.par_hist, st.hyp_par, st.done_step = i32(R, G), i32(B, n, G), i32(B)
         else:
             st.finished = i32(P)
             if shared:                                                      # the identity source table
@@ -285,11 +308,14 @@ class PhaseTimer:
                               "prompt_lens": list(pp.seqlens), **extra})
 
 
-def decode(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph, stats, dec: Decoding, procs=(), table=None):
+def decode(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph, stats, dec: Decoding, procs=(), table=None,
+           out_fields: Optional[dict] = None):
     """``generate`` without beams, with the host processors ``procs`` (the host path when not empty) or the flattened trie
     ``table`` walked on the device; returns None when the device walk reported a miss.  ``dec.n`` > 1 (sampling without
     processors): the n samples of a prompt start from its last hidden row, over its prompt cache; the visual tokens of
-    prompt b reach all n samples of prompt b."""
+    prompt b reach all n samples of prompt b.  ``dec.scores``: every pick also stores what it read -- the processed (trie-masked)
+    logits with the special ids -inf (``ops.scores_store``), or the warped scores of ``ops.sample`` -- in plane ``st.score_t``
+    of ``st.scores``, inside the captured step; ``out_fields["scores"]`` gets one [R, V] entry per generated column."""
     timer = PhaseTimer(stats)
     host = bool(procs)                                        # processors walk the generated ids on the host
     graphed = use_cuda_graph and not host
@@ -303,6 +329,8 @@ def decode(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph, s
         st.miss.zero_()
     if dec.proc is not None:
         load_proc(st, input_ids, R, max_new_tokens)
+    if dec.scores:
+        load_scores(st, max_new_tokens, R, logits.shape[1])
     finished.zero_()
     lens.copy_(torch.tensor(pp.seqlens, dtype=torch.int32).repeat_interleave(n), non_blocking=True)
     if shared:                                                # the n samples of a prompt start from its last row
@@ -324,8 +352,13 @@ def decode(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph, s
             lg = p(torch.tensor(all_ids_host, device=dev), lg)
         if dec.sampled:
             ops.sample(lg.to(torch.bfloat16), special, finished, eos, pad, stop, dec.temperature, dec.top_k, dec.top_p,
-                       torch.rand(R, device=dev, dtype=torch.float32), next_ids)
+                       torch.rand(R, device=dev, dtype=torch.float32), next_ids, **scored)
+            if dec.scores:
+                ops.add_int_(st.score_t, 1)
             return
+        if dec.scores:
+            ops.scores_store(lg.to(torch.bfloat16), special, st.scores, st.score_t)
+            ops.add_int_(st.score_t, 1)
         nxt = lg.argmax(dim=-1)
         fin = finished.bool()
         nxt = torch.where(fin, torch.full_like(nxt, pad), nxt)
@@ -342,10 +375,15 @@ def decode(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph, s
             src = st.masked
         if dec.sampled:
             st.u.uniform_()                                   # = torch.rand(R): the same numbers, into a static buffer
-            ops.sample(src, special, finished, eos, pad, stop, dec.temperature, dec.top_k, dec.top_p, st.u, next_ids)
+            ops.sample(src, special, finished, eos, pad, stop, dec.temperature, dec.top_k, dec.top_p, st.u, next_ids, **scored)
         else:
+            if dec.scores:
+                ops.scores_store(src, special, st.scores, st.score_t)
             ops.argmax_masked(src, special, finished, eos, pad, stop, next_ids)
+        if dec.scores:
+            ops.add_int_(st.score_t, 1)
 
+    scored = dict(scores=st.scores, step=st.score_t) if dec.scores else {}
     head(hid_last)
     host_ids = [row.tolist() for row in input_ids.cpu()] if host else None
     if host:
@@ -388,6 +426,8 @@ def decode(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph, s
     new = torch.stack(out_tokens, dim=1).to(torch.int64)
     if stop and check_every > 1:
         new = trim_after_eos(new, eos)                        # see check_every above
+    if out_fields is not None:
+        out_fields["scores"] = take_scores(st, new.shape[1]) if dec.scores else None
     return torch.cat([input_ids.to(dev).repeat_interleave(n, dim=0), new], dim=1)
 
 
@@ -486,7 +526,8 @@ def lookup_history(input_ids, attention_mask, cap: int) -> tuple:
     return hist, lens
 
 
-def lookup_decode(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph, stats, dec: Decoding):
+def lookup_decode(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph, stats, dec: Decoding,
+                  out_fields: Optional[dict] = None):
     """Greedy decoding that verifies k = ``dec.lookup_k`` drafted tokens per step.  After the prefill and its first token (as
     in ``decode``), a step is: ``ops.lookup_draft`` proposes k tokens per prompt from n-grams of its history (prompt and
     generated tokens, HF's PromptLookupCandidateGenerator); the last token and the k drafts run as one causal window of k + 1
@@ -494,7 +535,9 @@ def lookup_decode(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_g
     that equal the argmax of the row before them and emits those plus one token, 1 .. k + 1 per prompt and step.  A row's tokens
     are the argmax of its own prefix, so the ids are greedy decoding's whatever the drafts are; they differ from ``decode`` only
     where a different row count in a GEMM moves a near tie.  Static shapes: the step is captured once and replayed; the
-    generated ids stay on the device until one copy at the end.  Returns [B, S0 + n_new] with ``decode``'s width and pads."""
+    generated ids stay on the device until one copy at the end.  Returns [B, S0 + n_new] with ``decode``'s width and pads.
+    ``dec.scores``: column c of prompt b gets the logits row that picked its token (``ops.lookup_scores`` after the accept, inside
+    the captured step); the planes start at -inf, so a column after a row's EOS, which that row never runs, stays -inf."""
     k, eos, pad, stop, special = dec.lookup_k, dec.eos, dec.pad, dec.stop_on_eos, lm.special_ids_dev
     W, n_out = k + 1, max(max_new_tokens, 1)
     timer = PhaseTimer(stats)
@@ -518,6 +561,10 @@ def lookup_decode(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_g
     st.out[:, 0].copy_(st.next_ids)
     st.n_out.fill_(1)
     st.n_acc.zero_()
+    if dec.scores:
+        load_scores(st, n_out, B, st.logits.shape[1])
+        st.scores[:n_out].fill_(float("-inf"))
+        ops.scores_store(st.logits[:B], special, st.scores, st.score_t)       # plane 0: the first token's row
     if n_out == 1:
         st.finished.fill_(1)
     timer.mark()
@@ -528,8 +575,12 @@ def lookup_decode(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_g
             xt = ops.embed_fwd(st.win.view(-1), lm.model.embed_tokens.weight.data)
             h = lm.core.decode_step(xt, st.lens, st.kc, st.vc, window=W)
             decode_head(lm, h, st.logits)
+            if dec.scores:
+                st.score_prev.copy_(st.n_out)
             ops.lookup_accept(st.logits, special, st.drafts, st.finished, eos, stop, n_out, st.out, st.hist, st.hist_len,
                               st.n_out, st.lens, st.n_acc)
+            if dec.scores:
+                ops.lookup_scores(st.logits, special, st.score_prev, st.n_out, W, st.scores)
 
     # every row is done once it emitted EOS or n_out tokens; the device is asked every LOOKUP_CHECK_EVERY steps, and a done
     # row's extra steps emit nothing.  At most n_out - 1 steps: each emits at least one token per unfinished row.
@@ -541,6 +592,8 @@ def lookup_decode(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_g
     new = out.to(torch.int64)
     if stop:
         new = trim_after_eos(new, eos)
+    if out_fields is not None:
+        out_fields["scores"] = take_scores(st, new.shape[1]) if dec.scores else None
     return torch.cat([input_ids.to(dev), new.to(dev)], dim=1)
 
 
@@ -556,14 +609,17 @@ def trim_after_eos(new: torch.Tensor, eos: int) -> torch.Tensor:
 
 
 # ---- contrastive search (HF GenerationMixin.contrastive_search / _ranking_fast, transformers 4.28) ----
-def contrastive_search(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph, stats, dec: Decoding):
+def contrastive_search(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph, stats, dec: Decoding,
+                       out_fields: Optional[dict] = None):
     """Contrastive search (Su et al. 2022) over B prompts with k = ``dec.n`` candidates and alpha = ``dec.penalty_alpha``.  The
     prefill keeps the normalised final-norm row of every prompt position as the prompt's context (``ops.contrastive_context``)
     and the last row's logits.  A step: the processors (``dec.proc``) on the B logits rows, the k most probable tokens
     (``ops.contrastive_topk``), the B * k candidates as one decode step over the prompt caches (each candidate's own key in its
     one-slot cache), their final-norm rows ranked against the context (``ops.contrastive_rank``: the token, the context grows by
     the selected row), the selected candidate's K/V committed to the prompt cache (``ops.contrastive_commit``) and the lm_head
-    on its row only.  All on the device and replayed as a CUDA graph; ids, trimming and ``stats`` as in greedy decoding."""
+    on its row only.  All on the device and replayed as a CUDA graph; ids, trimming and ``stats`` as in greedy decoding.
+    ``dec.scores``: each step first stores the processed logits whose top-k formed its candidates (4.28's
+    processed_logit_for_next_step, special ids -inf; ``ops.scores_store``)."""
     k, eos, pad, stop, proc, special = dec.n, dec.eos, dec.pad, dec.stop_on_eos, dec.proc, lm.special_ids_dev
     timer = PhaseTimer(stats)
     pp, st, h_all = prefill(lm, dec, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph)
@@ -574,6 +630,8 @@ def contrastive_search(lm, input_ids, attention_mask, vis, max_new_tokens, use_c
     st.finished.zero_()
     st.pen_key.zero_()
     st.ctx_len.zero_()
+    if dec.scores:
+        load_scores(st, max_new_tokens, B, st.logits.shape[1])
     st.lens.copy_(torch.tensor(pp.seqlens, dtype=torch.int32).repeat_interleave(k), non_blocking=True)
     hn_all, _ = ops.rmsnorm_fwd(h_all, norm_w, eps)
     ops.contrastive_context(hn_all, pp.cu, st.ctx, st.ctx_len)
@@ -588,6 +646,9 @@ def contrastive_search(lm, input_ids, attention_mask, vis, max_new_tokens, use_c
 
     def step():
         with ops.pdl():
+            if dec.scores:
+                ops.scores_store(st.logits, special, st.scores, st.score_t)
+                ops.add_int_(st.score_t, 1)
             xt = ops.embed_fwd(st.cand_ids.view(-1), lm.model.embed_tokens.weight.data)
             h = lm.core.decode_step(xt, st.lens, st.kc, st.vc, beam=st.beam)
             hn, _ = ops.rmsnorm_fwd(h, norm_w, eps)
@@ -606,11 +667,14 @@ def contrastive_search(lm, input_ids, attention_mask, vis, max_new_tokens, use_c
            torch.zeros((B, 0), dtype=torch.int64, device=lm._device()))
     if stop:
         new = trim_after_eos(new, eos)
+    if out_fields is not None:
+        out_fields["scores"] = take_scores(st, new.shape[1]) if dec.scores else None
     return torch.cat([input_ids.to(lm._device()), new], dim=1)
 
 
 # ---- beam search (HF GenerationMixin.beam_search / BeamSearchScorer, transformers 4.28 as the reference pins it) ----
-def beam_search(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph, stats, dec: Decoding, table=None):
+def beam_search(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_graph, stats, dec: Decoding, table=None,
+                out_fields: Optional[dict] = None):
     """Beam search over B prompts with K = ``dec.n`` beams each.  The prefill runs once per prompt into the prompt cache, whose
     keys the K beams of the prompt share; generated keys live in a [B * K, G] cache that is written once per slot and read
     through the source table ``src`` (reordering the beams gathers ``src``, never K/V).  Each step is ``nv_beam_topk`` (2K
@@ -620,7 +684,13 @@ def beam_search(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_gra
     (``dec.proc``) the scoring is ``nv_beam_topk_processed`` over the beams' histories (prompt ids, ``hist``).  With the
     flattened trie ``table`` it is ``nv_beam_topk_trie`` (processors or not): each beam walks its own generated tokens from the
     root, and the log-probs its node does not allow become -inf after the processors, as 4.28's PrefixConstrainedLogitsProcessor
-    masks log_softmax's output; the trie is loaded as in ``decode``, and one that outgrows the buffers is recaptured."""
+    masks log_softmax's output; the trie is loaded as in ``decode``, and one that outgrows the buffers is recaptured.
+
+    ``out_fields`` (return_dict_in_generate) gets ``sequences_scores`` fp32 [B * n], the returned hypotheses' scores from the host
+    finalisation.  ``dec.scores`` (and output_scores) adds ``scores``: the top-k kernel of step t writes each beam's processed
+    log-probs to plane t (``prompt_state[:, 0]``), one entry per step 4.28 runs (until every prompt is done, not the extra steps
+    of the every-8-steps check); and ``beam_indices`` int64 [B * n, L]: ``nv_beam_select_scores`` keeps each beam's rows
+    (``par_hist``) and each hypothesis' rows (``hyp_par``), padded with -1."""
     K, eos, pad, proc, special = dec.n, dec.eos, dec.pad, dec.proc, lm.special_ids_dev
     if K > BEAM_MAX:
         raise NotImplementedError(f"generate(num_beams={K}): at most {BEAM_MAX} beams are built")
@@ -639,21 +709,27 @@ def beam_search(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_gra
     st.hyp_meta.zero_()
     st.pstate.zero_()
     st.pstate[:, 1].copy_(st.plens)
+    if dec.scores:
+        load_scores(st, max_new_tokens, B * K, st.logits.shape[1])      # step t writes plane t < max_new_tokens
+        st.done_step.zero_()
+    sc = dict(scores=st.scores, prompt_state=st.pstate) if dec.scores else {}
+    trace = (st.par_hist, st.hyp_par, st.done_step) if dec.scores else None
     st.norm.copy_(ops.beam_norm(S, G, dec.length_penalty))
     decode_head(lm, hid_last, st.logits[:B])
     sel = lambda: ops.beam_select(st.cand_score, st.cand_tok, st.cand_par, st.beam_score, st.hist, st.src, st.hyp_score,
                                   st.hyp_meta, st.hyp_tok, st.pstate, st.next_ids, st.lens, st.norm, eos, pad,
-                                  dec.early_stopping)
+                                  dec.early_stopping, trace=trace)
 
     def topk(first_step=False):
         if table is not None:
             ops.beam_topk_trie(st.logits, special, st.beam_score, K, st.cand_score, st.cand_tok, st.cand_par, st.proc_ids,
-                               st.proc_width, st.hist, st.pstate, proc, *trie_csr, table.eos, first_step=first_step)
+                               st.proc_width, st.hist, st.pstate, proc, *trie_csr, table.eos, first_step=first_step,
+                               scores=sc.get("scores"))
         elif proc is None:
-            ops.beam_topk(st.logits, special, st.beam_score, K, st.cand_score, st.cand_tok, st.cand_par, first_step=first_step)
+            ops.beam_topk(st.logits, special, st.beam_score, K, st.cand_score, st.cand_tok, st.cand_par, first_step=first_step, **sc)
         else:
             ops.beam_topk_processed(st.logits, special, st.beam_score, K, st.cand_score, st.cand_tok, st.cand_par, st.proc_ids,
-                                    st.proc_width, st.hist, st.pstate, proc, first_step=first_step)
+                                    st.proc_width, st.hist, st.pstate, proc, first_step=first_step, scores=sc.get("scores"))
 
     topk(first_step=True)
     sel()
@@ -674,43 +750,65 @@ def beam_search(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_gra
     # one copy; the fp64 scores go first, so their view starts at an even int32 offset whatever B and K are
     parts = [st.hyp_score.flatten().view(torch.int32), st.hist.flatten(), st.hyp_meta.flatten(), st.hyp_tok.flatten(),
              st.pstate.flatten(), st.beam_score.view(torch.int32)]
-    hyp_score, hist, hyp_meta, hyp_tok, pstate, beam_score = torch.cat(parts).cpu().split([t.numel() for t in parts])
+    if dec.scores:
+        parts += [st.par_hist.flatten(), st.hyp_par.flatten(), st.done_step]
+    hyp_score, hist, hyp_meta, hyp_tok, pstate, beam_score, *tr = torch.cat(parts).cpu().split([t.numel() for t in parts])
     hyp_score, beam_score = hyp_score.view(torch.float64).view(B, K + 1), beam_score.view(torch.float32)
     hist, hyp_meta, hyp_tok, pstate = hist.view(B * K, G), hyp_meta.view(B, K, 2), hyp_tok.view(B, K, G), pstate.view(B, 5)
     T_done = int(pstate[0, 0])
+    if dec.scores:
+        par_hist, hyp_par, done_step = tr[0].view(B * K, G), tr[1].view(B, K, G), tr[2]
+    # the beam rows of each hypothesis (beam_indices) ride along as a third element when they are kept
+    idx = (lambda rows, n: (rows[:n].tolist(),)) if dec.scores else (lambda rows, n: ())
     hyps, running = [], []
     for b in range(B):
         n = int(pstate[b, 2])
         kept = sorted(range(n), key=lambda i: int(hyp_meta[b, i, 1]))          # insertion order
-        hyps.append([(float(hyp_score[b, i]), hyp_tok[b, i, :int(hyp_meta[b, i, 0])].tolist()) for i in kept])
+        hyps.append([(float(hyp_score[b, i]), hyp_tok[b, i, :int(hyp_meta[b, i, 0])].tolist(),
+                      *idx(hyp_par[b, i] if dec.scores else None, int(hyp_meta[b, i, 0]) + 1)) for i in kept])
         running.append(None if int(pstate[b, 4]) else
-                       [(float(beam_score[b * K + k]), hist[b * K + k, :T_done].tolist()) for k in range(K)])
-    seqs = beam_finalize(hyps, [float(hyp_score[b, K]) for b in range(B)], running, S, T_done, K, dec.n_return,
-                         dec.length_penalty)
-    return beam_output(input_ids.cpu(), seqs, S, S + max_new_tokens, eos, pad).to(lm._device())
+                       [(float(beam_score[b * K + k]), hist[b * K + k, :T_done].tolist(),
+                         *idx(par_hist[b * K + k] if dec.scores else None, T_done)) for k in range(K)])
+    best = beam_finalize(hyps, [float(hyp_score[b, K]) for b in range(B)], running, S, T_done, K, dec.n_return,
+                         dec.length_penalty, entries=True)
+    seqs = [[e[1] for e in per] for per in best]
+    out = beam_output(input_ids.cpu(), seqs, S, S + max_new_tokens, eos, pad)
+    if out_fields is not None:
+        out_fields["sequences_scores"] = torch.tensor([e[0] for per in best for e in per], dtype=torch.float32).to(lm._device())
+        out_fields["scores"] = out_fields["beam_indices"] = None
+        if dec.scores:
+            # 4.28 stops once every prompt is done; the device checks every 8 steps, and its extra steps are not 4.28's
+            n_steps = int(done_step.max()) if bool(pstate[:, 4].all()) else T_done
+            out_fields["scores"] = take_scores(st, n_steps)
+            bi = torch.full(out.shape, -1, dtype=torch.int64)
+            for i, e in enumerate(e for per in best for e in per):
+                bi[i, :len(e[2])] = torch.tensor(e[2], dtype=torch.int64)
+            out_fields["beam_indices"] = bi.to(lm._device())
+    return out.to(lm._device())
 
 
-def beam_finalize(hyps, worst, running, S: int, T: int, K: int, n_return: int, length_penalty: float):
+def beam_finalize(hyps, worst, running, S: int, T: int, K: int, n_return: int, length_penalty: float, entries: bool = False):
     """BeamSearchScorer.finalize of transformers 4.28: prompts that are not done add their K running beams (score
     sum_logprobs / (S + T) ** length_penalty, the Python float arithmetic of BeamHypotheses.add), then each prompt returns its
     ``n_return`` best hypotheses, best first; of equal scores the one added last wins (a stable sort, popped from the end).
     hyps[b]: the kept (score, generated tokens) in insertion order; worst[b]: their worst_score; running[b]: the K (running
-    score, tokens) of a prompt that is not done, else None.  Returns [[generated tokens] * n_return] per prompt."""
+    score, tokens) of a prompt that is not done, else None.  Returns [[generated tokens] * n_return] per prompt; with ``entries``
+    the whole (score, tokens, ...) entries instead (an entry may carry more elements, e.g. its beam rows; they ride along)."""
     out = []
     for b, beams in enumerate(hyps):
         beams, w = list(beams), worst[b]
-        for sc, toks in (running[b] or []):
+        for sc, toks, *rest in (running[b] or []):
             score = sc / ((S + T) ** length_penalty)
             if len(beams) < K or score > w:
-                beams.append((score, toks))
+                beams.append((score, toks, *rest))
                 if len(beams) > K:
-                    order = sorted([(s, i) for i, (s, _) in enumerate(beams)])
+                    order = sorted([(e[0], i) for i, e in enumerate(beams)])
                     del beams[order[0][1]]
                     w = order[1][0]
                 else:
                     w = min(score, w)
         ranked = sorted(beams, key=lambda x: x[0])
-        out.append([ranked.pop()[1] for _ in range(n_return)])
+        out.append([ranked.pop() if entries else ranked.pop()[1] for _ in range(n_return)])
     return out
 
 

@@ -43,6 +43,61 @@ class LMOutput(SimpleNamespace):
         return getattr(self, k)
 
 
+class _GenerateOutput(LMOutput):
+    """Stand-in for transformers 4.28's generate() output classes: the fields in 4.28's order, attribute access, item access by
+    name, and by position over the fields that are not None (ModelOutput.to_tuple)."""
+    FIELDS: tuple = ()
+
+    def __init__(self, **kw):
+        super().__init__(**{f: kw.get(f) for f in self.FIELDS})
+
+    def to_tuple(self) -> tuple:
+        return tuple(getattr(self, f) for f in self.FIELDS if getattr(self, f) is not None)
+
+    def __getitem__(self, k):
+        return self.to_tuple()[k] if isinstance(k, int) else getattr(self, k)
+
+
+class GreedySearchDecoderOnlyOutput(_GenerateOutput):
+    FIELDS = ("sequences", "scores", "attentions", "hidden_states")
+
+
+class SampleDecoderOnlyOutput(_GenerateOutput):
+    FIELDS = ("sequences", "scores", "attentions", "hidden_states")
+
+
+class ContrastiveSearchDecoderOnlyOutput(_GenerateOutput):
+    FIELDS = ("sequences", "scores", "attentions", "hidden_states")
+
+
+class BeamSearchDecoderOnlyOutput(_GenerateOutput):
+    FIELDS = ("sequences", "sequences_scores", "scores", "beam_indices", "attentions", "hidden_states")
+
+
+def compute_transition_scores(sequences: torch.Tensor, scores, beam_indices: Optional[torch.Tensor] = None,
+                              normalize_logits: bool = False) -> torch.Tensor:
+    """transformers 4.28's GenerationMixin.compute_transition_scores: the score of each generated token, fp32 [rows, n] (the
+    scores are cast to fp32 first, so ``normalize_logits`` log-softmaxes in fp32).  Without ``beam_indices`` row r reads
+    scores[t][r] (greedy / sampled / contrastive); with them, step t of hypothesis i reads row beam_indices[i, t], a -1 reads
+    row 0 and is zeroed, and the columns stop at the longest hypothesis."""
+    if beam_indices is None:
+        beam_indices = torch.arange(scores[0].shape[0]).view(-1, 1).to(sequences.device)
+        beam_indices = beam_indices.expand(-1, len(scores))
+    V = scores[0].shape[-1]
+    sc = torch.stack(scores).float().reshape(len(scores), -1).transpose(0, 1)          # [rows * V, steps]
+    if normalize_logits:
+        sc = torch.nn.functional.log_softmax(sc.reshape(-1, V, sc.shape[-1]), dim=1).reshape(-1, sc.shape[-1])
+    mask = beam_indices < 0
+    max_len = int((1 - mask.long()).sum(-1).max())
+    beam_indices = beam_indices.clone()[:, :max_len]
+    mask = mask[:, :max_len]
+    beam_indices[mask] = 0
+    indices = sequences[:, sequences.shape[-1] - max_len:] + beam_indices * V
+    out = sc.gather(0, indices)
+    out[mask] = 0
+    return out
+
+
 def _lookup_k(k, ngram) -> tuple:
     """``generate(prompt_lookup_num_tokens=k, max_matching_ngram_size=ngram)`` as (drafts per step, ngram): k = 0 for None or 0
     (plain greedy decoding), else an int in 1 .. 15 (the window kernel's 16 rows); ngram None is HF's 2.  Any other k, or an
@@ -970,7 +1025,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
                  no_repeat_ngram_size: Optional[int] = None, min_length: Optional[int] = None,
                  min_new_tokens: Optional[int] = None, penalty_alpha: Optional[float] = None,
                  prompt_lookup_num_tokens: Optional[int] = None, max_matching_ngram_size: Optional[int] = 2,
-                 **unused) -> torch.Tensor:
+                 return_dict_in_generate: bool = False, output_scores: bool = False, **unused):
         """Prefill on the packed kernels (positions = cumsum(mask)-1 like HF generate; visual tokens injected only
         here, as in models/modified_lm.py:195-197), then one token per step over a pre-allocated KV cache.  The
         decode step of the greedy, sampled and trie-constrained modes has static shapes and is replayed as a CUDA graph
@@ -1037,7 +1092,17 @@ class ModifiedLlamaForCausalLM(nn.Module):
         pads; they can differ from a plain greedy call only at a near tie, because the step's GEMMs run over more rows.  bf16,
         fp8 or int4 weights, bf16 or fp8 KV cache, graphed or eager.  Sampling, beams, contrastive search, ``trie=``,
         ``logits_processor=``, the device processors and ``num_return_sequences > 1`` raise ``NotImplementedError``; a k
-        outside 0 .. 15 or ``max_matching_ngram_size < 1`` raises ``ValueError``.  0 or None is plain greedy decoding."""
+        outside 0 .. 15 or ``max_matching_ngram_size < 1`` raises ``ValueError``.  0 or None is plain greedy decoding.
+
+        ``return_dict_in_generate=True`` returns transformers 4.28's output object instead of the ids (``GreedySearchDecoderOnlyOutput``
+        for greedy, trie and prompt-lookup calls, ``SampleDecoderOnlyOutput``, ``BeamSearchDecoderOnlyOutput``,
+        ``ContrastiveSearchDecoderOnlyOutput``); ``sequences`` is the ids tensor the same call returns without it, and beam calls set
+        ``sequences_scores`` fp32 [B * n].  Adding ``output_scores=True`` fills ``scores``: one bf16 [rows, V] tensor per generated
+        column (per step 4.28 runs, for beams) holding what that step's pick read -- the processed logits (greedy, trie, prompt
+        lookup: the verify row that picked the column; contrastive search: the logits whose top-k formed the candidates), the
+        warped scores (sampling) or the processed log-probs before the beam-score add (beams), special ids -inf -- and, for beams,
+        ``beam_indices`` int64 [B * n, L] (-1 padded).  The kernels store them inside the captured step; see DESIGN §2.
+        ``output_scores`` alone changes nothing, as in 4.28.  ``compute_transition_scores`` turns them into per-token scores."""
         lookup, ngram = _lookup_k(prompt_lookup_num_tokens, max_matching_ngram_size)
         if lookup:
             excluded = [("do_sample=True", do_sample), ("num_beams > 1", num_beams > 1),
@@ -1096,14 +1161,20 @@ class ModifiedLlamaForCausalLM(nn.Module):
         pad = self.tokenizer.unk_token_id if pad_token_id is None else pad_token_id
         proc = generation.processors(repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens, eos)
         call = (self, input_ids, attention_mask, (cand_vis, hist_vis, obj_vis), max_new_tokens, use_cuda_graph, stats)
+        rd = bool(return_dict_in_generate)
+        scores = rd and bool(output_scores)                  # the only combination that stores anything on the device
+        fields = {} if rd else None
+
+        def result(cls, ids):
+            return ids if not rd else cls(sequences=ids, **fields)
         if lookup:
             dec = generation.Decoding(int(eos), int(pad), bool(stop_on_eos), "lookup", self.kv_cache_dtype, lookup_k=lookup,
-                                      lookup_ngram=ngram)
-            return generation.lookup_decode(*call, dec)
+                                      lookup_ngram=ngram, scores=scores)
+            return result(GreedySearchDecoderOnlyOutput, generation.lookup_decode(*call, dec, out_fields=fields))
         if contrastive:
             dec = generation.Decoding(int(eos), int(pad), bool(stop_on_eos), "contrastive", self.kv_cache_dtype, top_k=int(top_k),
-                                      n=int(top_k), proc=proc, penalty_alpha=float(penalty_alpha))
-            return generation.contrastive_search(*call, dec)
+                                      n=int(top_k), proc=proc, penalty_alpha=float(penalty_alpha), scores=scores)
+            return result(ContrastiveSearchDecoderOnlyOutput, generation.contrastive_search(*call, dec, out_fields=fields))
         if num_beams > 1:
             table = None
             if trie is not None:
@@ -1115,11 +1186,11 @@ class ModifiedLlamaForCausalLM(nn.Module):
                                               "processors keep per-row state that reordering the beams would scramble")
             dec = generation.Decoding(int(eos), int(pad), None, "beam", self.kv_cache_dtype, n=int(num_beams), n_return=n_seq,
                                       length_penalty=float(length_penalty), early_stopping=bool(early_stopping), proc=proc,
-                                      trie_eos=None if table is None else table.eos)
-            out = generation.beam_search(*call, dec, table=table)
+                                      trie_eos=None if table is None else table.eos, scores=scores)
+            out = generation.beam_search(*call, dec, table=table, out_fields=fields)
             if stats is not None and table is not None:
                 stats.update({"trie_path": "device", "trie_flatten_ms": flatten_ms})
-            return out
+            return result(BeamSearchDecoderOnlyOutput, out)
         procs = list(logits_processor or [])
         table = None
         if trie is not None and not procs:
@@ -1128,24 +1199,30 @@ class ModifiedLlamaForCausalLM(nn.Module):
             flatten_ms = 1e3 * (time.perf_counter() - t0)
         sampling = dict(temperature=float(temperature), top_k=int(top_k), top_p=top_p) if do_sample else {}
         dec = generation.Decoding(int(eos), int(pad), bool(stop_on_eos), "sample" if do_sample else "greedy", self.kv_cache_dtype,
-                                  n=max(1, n_seq), proc=proc, **sampling)
+                                  n=max(1, n_seq), proc=proc, scores=scores, **sampling)
         if table is not None:
             rng = torch.cuda.get_rng_state(dev) if do_sample else None
             trie_dec = dataclasses.replace(dec, mode="trie+sample" if do_sample else "trie", trie_eos=table.eos)
-            out = generation.decode(*call, trie_dec, table=table)
+            out = generation.decode(*call, trie_dec, table=table, out_fields=fields)
             path = "device" if out is not None else "device_miss_host"
             if out is None:
                 if rng is not None:
                     torch.cuda.set_rng_state(rng, dev)
-                out = generation.decode(*call, dec, procs=[trie_mod.TrieLogitsProcessor(trie)])
+                out = generation.decode(*call, dec, procs=[trie_mod.TrieLogitsProcessor(trie)], out_fields=fields)
         else:
             if trie is not None:
                 procs = [trie_mod.TrieLogitsProcessor(trie)] + procs
                 path = "host"
-            out = generation.decode(*call, dec, procs=procs)
+            out = generation.decode(*call, dec, procs=procs, out_fields=fields)
         if stats is not None and trie is not None:
             stats.update({"trie_path": path, "trie_flatten_ms": flatten_ms if table is not None else None})
-        return out
+        return result(SampleDecoderOnlyOutput if do_sample else GreedySearchDecoderOnlyOutput, out)
+
+    @staticmethod
+    def compute_transition_scores(sequences, scores, beam_indices=None, normalize_logits: bool = False) -> torch.Tensor:
+        """transformers 4.28's ``compute_transition_scores`` on ``generate(return_dict_in_generate=True, output_scores=True)``'s
+        output: fp32 [rows, n] scores of the generated tokens (see the module-level ``compute_transition_scores``)."""
+        return compute_transition_scores(sequences, scores, beam_indices, normalize_logits)
 
     @torch.no_grad()
     def score_answers(self, input_ids, attention_mask, trie, cand_vis=None, hist_vis=None, obj_vis=None,

@@ -522,15 +522,35 @@ class NavModel(nn.Module):
         if kwargs.get("rank_answers", False):
             return self._rank_answers(text, cand_vis, hist_vis_input, kwargs)
         trie = kwargs.get("trie", None)
-        # beam search over the answer trie: the beam kwargs reach generate() only when the caller passes them
-        beams = {k: kwargs[k] for k in ("num_beams", "num_return_sequences", "length_penalty", "early_stopping") if k in kwargs}
-        ids = self.lang_model.generate(input_ids=text["input_ids"], attention_mask=text["attention_mask"], cand_vis=cand_vis,
-                                       hist_vis=hist_vis_input, eos_token_id=self.lang_model.tokenizer.eos_token_id,
-                                       pad_token_id=self.lang_model.tokenizer.unk_token_id, max_new_tokens=50, do_sample=False,
-                                       trie=trie, **beams).tolist()
-        ids = [s[text["input_ids"].shape[1]:] for s in ids]
-        return {"generated_sentences": self.lang_model.tokenizer.batch_decode(ids, skip_special_tokens=True,
-                                                                              clean_up_tokenization_spaces=False)}
+        # beam search over the answer trie: the beam kwargs (and output_scores) reach generate() only when the caller passes them
+        beams = {k: kwargs[k] for k in ("num_beams", "num_return_sequences", "length_penalty", "early_stopping", "output_scores")
+                 if k in kwargs}
+        return self._generate_sentences(text, input_ids=text["input_ids"], attention_mask=text["attention_mask"], cand_vis=cand_vis,
+                                        hist_vis=hist_vis_input, eos_token_id=self.lang_model.tokenizer.eos_token_id,
+                                        pad_token_id=self.lang_model.tokenizer.unk_token_id, max_new_tokens=50, do_sample=False,
+                                        trie=trie, **beams)
+
+    def _generate_sentences(self, text, **gen) -> Dict[str, Any]:
+        """``generate(**gen)`` decoded to generated_sentences (the prompt columns cut off); ``return_dict_in_generate`` alone changes
+        nothing here.  With ``output_scores=True`` the call
+        returns 4.28's output object (``return_dict_in_generate``, which the reference's ``.tolist()`` could not take) and the
+        result gains transition_scores fp32 [rows, n_new] (``compute_transition_scores``: log-softmax-normalised for the modes
+        without beams, by ``beam_indices`` for beams) and, for beams, sequences_scores."""
+        scored = bool(gen.get("output_scores", False))
+        if scored:
+            gen["return_dict_in_generate"] = True
+        out = self.lang_model.generate(**gen)
+        ids = out if isinstance(out, torch.Tensor) else out.sequences      # return_dict_in_generate alone: the object's ids
+        S = text["input_ids"].shape[1]
+        res = {"generated_sentences": self.lang_model.tokenizer.batch_decode([s[S:] for s in ids.tolist()], skip_special_tokens=True,
+                                                                             clean_up_tokenization_spaces=False)}
+        if scored:
+            beam = getattr(out, "beam_indices", None) is not None
+            res["transition_scores"] = self.lang_model.compute_transition_scores(
+                out.sequences, out.scores, out.beam_indices if beam else None, normalize_logits=not beam)
+            if beam:
+                res["sequences_scores"] = out.sequences_scores
+        return res
 
     def forward_3dqa(self, mode, batch: Dict[str, Any], training: bool = True, **kwargs):
         """models/nav_model.py:346-404."""
@@ -559,12 +579,9 @@ class NavModel(nn.Module):
             return LMOutput(loss=loss, logits=None, past_key_values=None, hidden_states=None, attentions=None)
         if kwargs.pop("rank_answers", False):
             return self._rank_answers(text, cand_vis, None, kwargs)
-        ids = self.lang_model.generate(input_ids=text["input_ids"], attention_mask=text["attention_mask"], cand_vis=cand_vis,
-                                       eos_token_id=self.lang_model.tokenizer.eos_token_id,
-                                       pad_token_id=self.lang_model.tokenizer.unk_token_id, **kwargs).tolist()
-        ids = [s[text["input_ids"].shape[1]:] for s in ids]
-        return {"generated_sentences": self.lang_model.tokenizer.batch_decode(ids, skip_special_tokens=True,
-                                                                              clean_up_tokenization_spaces=False)}
+        return self._generate_sentences(text, input_ids=text["input_ids"], attention_mask=text["attention_mask"], cand_vis=cand_vis,
+                                        eos_token_id=self.lang_model.tokenizer.eos_token_id,
+                                        pad_token_id=self.lang_model.tokenizer.unk_token_id, **kwargs)
 
     def _rank_answers(self, text, cand_vis, hist_vis, kwargs) -> Dict[str, Any]:
         """``rank_answers=True`` of the summarization / embodied_qa and 3dqa modes: every answer of ``trie=`` scored under each

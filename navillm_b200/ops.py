@@ -847,19 +847,75 @@ def _beam_io(name, B, K, G, **ts):
             raise ValueError(f"{name}: {k} {dt} {list(shape)} contiguous on the device expected (got {t.dtype} {tuple(t.shape)})")
 
 
-def beam_topk(logits, special, beam_score, K, cand_score, cand_tok, cand_parent, *, first_step=False):
+def _scores_io(name, scores, rows: int, V: int, step=None, step_numel: int = 1):
+    """(ptr, ld, plane) of a per-step scores buffer: bf16 [G, >= rows, V] planes with unit inner stride (``scores_buffer``)."""
+    if scores.dtype != bf16 or scores.dim() != 3 or scores.shape[1] < rows or scores.shape[2] != V or scores.stride(2) != 1 or \
+            not scores.is_cuda:
+        raise ValueError(f"{name}: scores bf16 [G, >= {rows}, {V}] with unit inner stride expected (got {scores.dtype} "
+                         f"{tuple(scores.shape)})")
+    if step is not None and (step.dtype != torch.int32 or step.numel() < step_numel or not step.is_cuda):
+        raise ValueError(f"{name}: step int32 [>= {step_numel}] on the device expected")
+    return ptr(scores), i64(scores.stride(1)), i64(scores.stride(0))
+
+
+def scores_buffer(planes: int, rows: int, V: int, device) -> torch.Tensor:
+    """Uninitialised bf16 [planes, rows, V] per-step scores whose rows start 16-byte aligned (``logits_buffer``'s stride)."""
+    return torch.empty((planes, rows, (V + 63) // 64 * 64), dtype=bf16, device=device)[:, :, :V]
+
+
+def scores_store(src, special, scores, step):
+    """Rows of bf16 ``src`` [R, V] to plane ``step[0]`` (int32 on the device, read at run time) of ``scores`` [G, >= R, V], the
+    special ids -inf (nv_scores_store)."""
+    R, V = src.shape
+    if src.dtype != bf16 or src.stride(1) != 1:
+        raise ValueError(f"scores_store: bf16 src with unit inner stride expected (got {src.dtype})")
+    args = _scores_io("scores_store", scores, R, V, step)
+    check(_lib.load().nv_scores_store(ptr(src), i64(src.stride(0)), i32(V), ptr(special), i32(special.numel()), *args, ptr(step),
+                                      i32(R), stream_ptr()), "nv_scores_store")
+
+
+def lookup_scores(logits, special, n_prev, n_out, W, scores):
+    """After ``lookup_accept``: logits row b * W + j of each token prompt b emitted in the step goes to plane n_prev[b] + j,
+    row b of ``scores`` [G, >= B, V], special ids -inf (nv_lookup_scores)."""
+    B = n_out.numel()
+    V = logits.shape[1]
+    for name, t in (("n_prev", n_prev), ("n_out", n_out)):
+        if t.dtype != torch.int32 or t.numel() != B or not t.is_cuda:
+            raise ValueError(f"lookup_scores: {name} int32 [{B}] on the device expected")
+    args = _scores_io("lookup_scores", scores, B, V)
+    check(_lib.load().nv_lookup_scores(ptr(logits), i64(logits.stride(0)), i32(V), ptr(special), i32(special.numel()), ptr(n_prev),
+                                       ptr(n_out), i32(W), *args, i32(B), stream_ptr()), "nv_lookup_scores")
+
+
+def beam_topk(logits, special, beam_score, K, cand_score, cand_tok, cand_parent, *, first_step=False, scores=None,
+              prompt_state=None):
     """The 2K best next-token candidates of each prompt (nv_beam_topk): logits bf16 [B * K, V] (beam k of prompt b in row
     b * K + k), or with ``first_step`` [>= B, V] holding one prefill row per prompt that all K beams read.  beam_score fp32
-    [B * K].  Writes cand_score fp32, cand_tok and cand_parent int32 [B, 2K], best first."""
+    [B * K].  Writes cand_score fp32, cand_tok and cand_parent int32 [B, 2K], best first.  With ``scores`` (bf16 [G, B * K, V])
+    each beam's bf16 log-probs also go to plane prompt_state[b, 0] (nv_beam_topk_scores)."""
     B = cand_score.shape[0]
     V = logits.shape[1]
     if logits.dtype != bf16 or logits.stride(1) != 1 or logits.shape[0] < (B if first_step else B * K):
         raise ValueError(f"beam_topk: bf16 logits with {B if first_step else B * K} rows expected (got {logits.dtype} {tuple(logits.shape)})")
     _beam_io("beam_topk", B, K, 1, cand_score=cand_score, cand_tok=cand_tok, cand_parent=cand_parent, beam_score=beam_score)
     ld = logits.stride(0)
+    if scores is not None:
+        check(_lib.load().nv_beam_topk_scores(ptr(logits), i64(ld if first_step else K * ld), i64(0 if first_step else ld), i32(V),
+                                              ptr(special), i32(special.numel()), ptr(beam_score), ptr(cand_score), ptr(cand_tok),
+                                              ptr(cand_parent), ptr(prompt_state),
+                                              *_beam_scores_io("beam_topk", scores, prompt_state, B, K, V), i32(B), i32(K),
+                                              stream_ptr()), "nv_beam_topk_scores")
+        return
     check(_lib.load().nv_beam_topk(ptr(logits), i64(ld if first_step else K * ld), i64(0 if first_step else ld), i32(V), ptr(special),
                                    i32(special.numel()), ptr(beam_score), ptr(cand_score), ptr(cand_tok), ptr(cand_parent), i32(B),
                                    i32(K), stream_ptr()), "nv_beam_topk")
+
+
+def _beam_scores_io(name, scores, prompt_state, B, K, V):
+    if prompt_state is None:
+        raise ValueError(f"{name}: scores= needs prompt_state (the plane of beam b is prompt_state[b, 0])")
+    _beam_io(name, B, K, 1, prompt_state=prompt_state)
+    return _scores_io(name, scores, B * K, V)
 
 
 def _proc_io(name, V, prompt_ids, prompt_width, hist, proc):
@@ -892,9 +948,10 @@ def logits_process_(logits, prompt_ids, prompt_width, hist, hist_len, append, pr
 
 
 def beam_topk_processed(logits, special, beam_score, K, cand_score, cand_tok, cand_parent, prompt_ids, prompt_width, hist,
-                        prompt_state, proc, *, first_step=False):
+                        prompt_state, proc, *, first_step=False, scores=None):
     """``beam_topk`` with the processors of ``logits_process_`` applied to each bf16 log-prob before the beam-score add
-    (nv_beam_topk_processed); beam k of prompt b has the history prompt_ids[b, :S] ++ hist[b * K + k, :prompt_state[b, 0]]."""
+    (nv_beam_topk_processed); beam k of prompt b has the history prompt_ids[b, :S] ++ hist[b * K + k, :prompt_state[b, 0]].
+    ``scores``: as in ``beam_topk`` (nv_beam_topk_processed_scores)."""
     B = cand_score.shape[0]
     V = logits.shape[1]
     if logits.dtype != bf16 or logits.stride(1) != 1 or logits.shape[0] < (B if first_step else B * K):
@@ -904,6 +961,14 @@ def beam_topk_processed(logits, special, beam_score, K, cand_score, cand_tok, ca
              beam_score=beam_score, hist=hist, prompt_state=prompt_state)
     args = _proc_io("beam_topk_processed", V, prompt_ids, prompt_width, hist, proc)
     ld = logits.stride(0)
+    if scores is not None:
+        check(_lib.load().nv_beam_topk_processed_scores(ptr(logits), i64(ld if first_step else K * ld), i64(0 if first_step else ld),
+                                                        i32(V), ptr(special), i32(special.numel()), ptr(beam_score), ptr(cand_score),
+                                                        ptr(cand_tok), ptr(cand_parent), ptr(prompt_ids), i64(prompt_ids.stride(0)),
+                                                        ptr(prompt_width), ptr(hist), i32(hist.shape[1]), ptr(prompt_state), *args,
+                                                        *_beam_scores_io("beam_topk_processed", scores, prompt_state, B, K, V), i32(B),
+                                                        i32(K), stream_ptr()), "nv_beam_topk_processed_scores")
+        return
     check(_lib.load().nv_beam_topk_processed(ptr(logits), i64(ld if first_step else K * ld), i64(0 if first_step else ld), i32(V),
                                              ptr(special), i32(special.numel()), ptr(beam_score), ptr(cand_score), ptr(cand_tok),
                                              ptr(cand_parent), ptr(prompt_ids), i64(prompt_ids.stride(0)), ptr(prompt_width),
@@ -915,11 +980,12 @@ PROC_OFF = (1.0, 0, 0, 0, -1)  # the processors' off values: beam_topk_trie with
 
 
 def beam_topk_trie(logits, special, beam_score, K, cand_score, cand_tok, cand_parent, prompt_ids, prompt_width, hist, prompt_state,
-                   proc, node_ptr, child_tok, child_node, n_nodes, leaf_tok, *, first_step=False):
+                   proc, node_ptr, child_tok, child_node, n_nodes, leaf_tok, *, first_step=False, scores=None):
     """``beam_topk_processed`` followed by the trie mask (nv_beam_topk_trie): every log-prob the trie does not allow at the beam's
     node becomes -inf.  Beam k of prompt b walks its generated tokens hist[b * K + k, :prompt_state[b, 0]] from the root;
     node_ptr / child_tok / child_node: the CSR trie of ``trie_mask`` with n_nodes real nodes plus the dead node n_nodes, leaf_tok
-    the token a childless node allows.  ``proc`` = None (or ``PROC_OFF``) runs the trie mask alone."""
+    the token a childless node allows.  ``proc`` = None (or ``PROC_OFF``) runs the trie mask alone.  ``scores``: as in
+    ``beam_topk`` (nv_beam_topk_trie_scores)."""
     B = cand_score.shape[0]
     V = logits.shape[1]
     if logits.dtype != bf16 or logits.stride(1) != 1 or logits.shape[0] < (B if first_step else B * K):
@@ -936,6 +1002,15 @@ def beam_topk_trie(logits, special, beam_score, K, cand_score, cand_tok, cand_pa
     if child_tok.numel() != child_node.numel():
         raise ValueError(f"beam_topk_trie: child_tok [{child_tok.numel()}] and child_node [{child_node.numel()}] differ in length")
     ld = logits.stride(0)
+    if scores is not None:
+        check(_lib.load().nv_beam_topk_trie_scores(ptr(logits), i64(ld if first_step else K * ld), i64(0 if first_step else ld), i32(V),
+                                                   ptr(special), i32(special.numel()), ptr(beam_score), ptr(cand_score), ptr(cand_tok),
+                                                   ptr(cand_parent), ptr(prompt_ids), i64(prompt_ids.stride(0)), ptr(prompt_width),
+                                                   ptr(hist), i32(hist.shape[1]), ptr(prompt_state), *args, ptr(node_ptr),
+                                                   ptr(child_tok), ptr(child_node), i32(n_nodes), i32(leaf_tok),
+                                                   *_beam_scores_io("beam_topk_trie", scores, prompt_state, B, K, V), i32(B), i32(K),
+                                                   stream_ptr()), "nv_beam_topk_trie_scores")
+        return
     check(_lib.load().nv_beam_topk_trie(ptr(logits), i64(ld if first_step else K * ld), i64(0 if first_step else ld), i32(V),
                                         ptr(special), i32(special.numel()), ptr(beam_score), ptr(cand_score), ptr(cand_tok),
                                         ptr(cand_parent), ptr(prompt_ids), i64(prompt_ids.stride(0)), ptr(prompt_width), ptr(hist),
@@ -944,14 +1019,24 @@ def beam_topk_trie(logits, special, beam_score, K, cand_score, cand_tok, cand_pa
 
 
 def beam_select(cand_score, cand_tok, cand_parent, beam_score, hist, src, hyp_score, hyp_meta, hyp_tok, prompt_state, next_ids, lens,
-                norm, eos_id, pad_id, early_stopping):
+                norm, eos_id, pad_id, early_stopping, *, trace=None):
     """One BeamSearchScorer.process step on the device (nv_beam_select); norm fp64 [G]: (S + t) ** length_penalty for S padded
-    prompt columns (``beam_norm``)."""
+    prompt columns (``beam_norm``).  ``trace`` = (par_hist int32 [B * K, G], hyp_par int32 [B, K, G], done_step int32 [B]) also
+    keeps 4.28's beam_indices (nv_beam_select_scores)."""
     B, K2 = cand_score.shape
     K, G = K2 // 2, hist.shape[1]
     _beam_io("beam_select", B, K, G, cand_score=cand_score, cand_tok=cand_tok, cand_parent=cand_parent, beam_score=beam_score,
              hist=hist, src=src, hyp_score=hyp_score, hyp_meta=hyp_meta, hyp_tok=hyp_tok, prompt_state=prompt_state,
              next_ids=next_ids, lens=lens, norm=norm)
+    if trace is not None:
+        par_hist, hyp_par, done_step = trace
+        _beam_io("beam_select", B, K, G, hist=par_hist, hyp_tok=hyp_par, plens=done_step)
+        check(_lib.load().nv_beam_select_scores(ptr(cand_score), ptr(cand_tok), ptr(cand_parent), ptr(beam_score), ptr(hist), ptr(src),
+                                                ptr(hyp_score), ptr(hyp_meta), ptr(hyp_tok), ptr(prompt_state), ptr(next_ids),
+                                                ptr(lens), ptr(norm), ptr(par_hist), ptr(hyp_par), ptr(done_step), i32(B), i32(K),
+                                                i32(G), i32(eos_id), i32(pad_id), i32(1 if early_stopping else 0), stream_ptr()),
+              "nv_beam_select_scores")
+        return
     check(_lib.load().nv_beam_select(ptr(cand_score), ptr(cand_tok), ptr(cand_parent), ptr(beam_score), ptr(hist), ptr(src),
                                      ptr(hyp_score), ptr(hyp_meta), ptr(hyp_tok), ptr(prompt_state), ptr(next_ids), ptr(lens), ptr(norm),
                                      i32(B), i32(K), i32(G), i32(eos_id), i32(pad_id), i32(1 if early_stopping else 0), stream_ptr()),
@@ -1062,13 +1147,22 @@ def sample_topk(logits, special, finished, eos_id, pad_id, stop_on_eos, temperat
     return next_ids
 
 
-def sample(logits, special, finished, eos_id, pad_id, stop_on_eos, temperature, top_k, top_p, u, next_ids, probs_out=None):
-    """``sample_topk`` with top-p filtering after top-k (nv_sample); ``top_p`` in [0, 1], 1 is off."""
+def sample(logits, special, finished, eos_id, pad_id, stop_on_eos, temperature, top_k, top_p, u, next_ids, probs_out=None, *,
+           scores=None, step=None):
+    """``sample_topk`` with top-p filtering after top-k (nv_sample); ``top_p`` in [0, 1], 1 is off.  With ``scores`` (bf16
+    [G, >= B, V]) the warped bf16 scores (-inf outside the kept set) also go to plane ``step[0]`` (nv_sample_scores)."""
     B, V = logits.shape
     assert logits.dtype == bf16 and logits.stride(1) == 1 and u.dtype == torch.float32 and u.numel() == B
     assert next_ids.dtype == torch.int32 and finished.dtype == torch.int32
     if probs_out is not None:
         assert probs_out.dtype == torch.float32 and probs_out.shape == (B, V) and probs_out.is_contiguous()
+    if scores is not None:
+        args = _scores_io("sample", scores, B, V, step)
+        check(_lib.load().nv_sample_scores(ptr(logits), i64(logits.stride(0)), i32(V), ptr(special), i32(special.numel()),
+                                           ptr(finished), i32(eos_id), i32(pad_id), i32(1 if stop_on_eos else 0), f32(temperature),
+                                           i32(top_k), f32(top_p), ptr(u), ptr(next_ids), ptr(probs_out), *args, ptr(step), i32(B),
+                                           stream_ptr()), "nv_sample_scores")
+        return next_ids
     check(_lib.load().nv_sample(ptr(logits), i64(logits.stride(0)), i32(V), ptr(special), i32(special.numel()), ptr(finished),
                                 i32(eos_id), i32(pad_id), i32(1 if stop_on_eos else 0), f32(temperature), i32(top_k), f32(top_p),
                                 ptr(u), ptr(next_ids), ptr(probs_out), i32(B), stream_ptr()), "nv_sample")
