@@ -507,6 +507,42 @@ int nv_beam_select_scores(const float* cand_score, const int* cand_tok, const in
                           double* hyp_score, int* hyp_meta, int* hyp_tok, int* prompt_state, int* next_ids, int* lens,
                           const double* norm, int* par_hist, int* hyp_par, int* done_step, int B, int K, int G, int eos_id, int pad_id,
                           int early_stopping, void* stream);
+/* Diverse (group) beam search: transformers 4.28's group_beam_search with num_beam_groups = n_groups and the
+ * HammingDiversityLogitsProcessor.  The K beams of a prompt form n_groups groups of Kg = K / n_groups (K in 2..8, n_groups
+ * dividing K); a step runs, for group = 0 .. n_groups - 1 in order, one top-k and one select launch.
+ * nv_beam_topk_group[_processed][_scores]: nv_beam_topk[_processed][_scores] over beams group * Kg + [0, Kg) of each prompt
+ * only, writing that group's 2Kg best to cand_* [B, 2Kg] (parents local to the group).  Before the processors, each bf16
+ * log-prob of token c is lowered to bf16(lp - diversity_penalty * freq[c]) in fp32, freq[c] counting c among next_ids[b * K +
+ * 0 .. group * Kg) (the earlier groups' tokens of this step, which their selects have written).  diversity_penalty > 0.
+ * nv_beam_select_group[_scores]: nv_beam_select[_scores] over those candidates with group_size Kg against the prompt's one set
+ * of K hypotheses; it reorders and writes only the group's rows (parents and beam_indices as global rows b * K + k), pads a
+ * prompt that is already done (an earlier group of this step included), and only the last group advances prompt_state[b, 0]. */
+int nv_beam_topk_group(const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, const int* special, int n_special,
+                       const float* beam_score, float* cand_score, int* cand_tok, int* cand_parent, const int* next_ids,
+                       float diversity_penalty, int group, int n_groups, int B, int K, void* stream);
+int nv_beam_topk_group_scores(const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, const int* special, int n_special,
+                              const float* beam_score, float* cand_score, int* cand_tok, int* cand_parent, const int* prompt_state,
+                              void* scores, int64_t ld_scores, int64_t plane, const int* next_ids, float diversity_penalty, int group,
+                              int n_groups, int B, int K, void* stream);
+int nv_beam_topk_group_processed(const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, const int* special, int n_special,
+                                 const float* beam_score, float* cand_score, int* cand_tok, int* cand_parent, const int* prompt_ids,
+                                 int64_t ld_ids, const int* prompt_width, const int* hist, int G, const int* prompt_state,
+                                 float penalty, int ngram, int min_length, int min_new_tokens, int eos_id, const int* next_ids,
+                                 float diversity_penalty, int group, int n_groups, int B, int K, void* stream);
+int nv_beam_topk_group_processed_scores(const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, const int* special,
+                                        int n_special, const float* beam_score, float* cand_score, int* cand_tok, int* cand_parent,
+                                        const int* prompt_ids, int64_t ld_ids, const int* prompt_width, const int* hist, int G,
+                                        const int* prompt_state, float penalty, int ngram, int min_length, int min_new_tokens,
+                                        int eos_id, void* scores, int64_t ld_scores, int64_t plane, const int* next_ids,
+                                        float diversity_penalty, int group, int n_groups, int B, int K, void* stream);
+int nv_beam_select_group(const float* cand_score, const int* cand_tok, const int* cand_parent, float* beam_score, int* hist, int* src,
+                         double* hyp_score, int* hyp_meta, int* hyp_tok, int* prompt_state, int* next_ids, int* lens,
+                         const double* norm, int group, int n_groups, int B, int K, int G, int eos_id, int pad_id, int early_stopping,
+                         void* stream);
+int nv_beam_select_group_scores(const float* cand_score, const int* cand_tok, const int* cand_parent, float* beam_score, int* hist,
+                                int* src, double* hyp_score, int* hyp_meta, int* hyp_tok, int* prompt_state, int* next_ids, int* lens,
+                                const double* norm, int* par_hist, int* hyp_par, int* done_step, int group, int n_groups, int B, int K,
+                                int G, int eos_id, int pad_id, int early_stopping, void* stream);
 
 /* ---- fused clip + AdamW over flat buffers (csrc/optim.cu) ------------------------------------------------------
  * torch.nn.utils.clip_grad_norm_(model.parameters(), 40.) + torch.optim.AdamW.step() of the reference

@@ -1517,13 +1517,25 @@ __device__ __forceinline__ int trie_walk(const BeamTrie& tr, const int* __restri
 
 // SCORES (nv_beam_topk*_scores): each beam's processed bf16 log-probs before the beam-score add (4.28's
 // next_token_scores_processed; special ids -inf) also go to so.row(b, b * K + k), the plane of step t = prompt_state[b, 0].
-template <bool PROC, bool TRIE = false, bool SCORES = false>
+// GROUP (nv_beam_topk_group*, diverse beam search): the CTA scans only the Kg = K / n_groups beams k0 + [0, Kg) of group g
+// (k0 = g * Kg) and writes that group's 2Kg best to cand_* [B, 2Kg], the parent local to the group.  Before the processors, each
+// bf16 log-prob of token c becomes bf16(lp - fp32(penalty) * freq[c]) in fp32, 4.28's HammingDiversityLogitsProcessor
+// (scores -= diversity_penalty * bincount): freq counts c among next_ids of rows b * K + [0, k0), the tokens the earlier groups'
+// selects of this step have already written there (at most BEAM_MAX - 1 of them).
+struct BeamGroup {
+  const int* next_ids;                       // [B * K]
+  float penalty;                             // diversity_penalty
+  int g, Kg;
+};
+
+template <bool PROC, bool TRIE = false, bool SCORES = false, bool GROUP = false>
 __device__ __forceinline__ void beam_topk_body(const __nv_bfloat16* __restrict__ logits, int64_t ld_prompt, int64_t ld_beam, int V,
                                                const int* __restrict__ special, int n_special, const float* __restrict__ beam_score,
                                                 int K, float* __restrict__ cand_score, int* __restrict__ cand_tok,
                                                int* __restrict__ cand_par, const BeamProc& bp, const BeamTrie& tr = BeamTrie{},
-                                               const ScoresOut& so = ScoresOut{}) {
+                                               const ScoresOut& so = ScoresOut{}, const BeamGroup& gr = BeamGroup{}) {
   static_assert(PROC || !TRIE, "the trie mask runs inside the processed scan");
+  static_assert(!(GROUP && TRIE), "group beams have no trie form");
   __shared__ int s_special[MAX_SPECIAL];
   __shared__ float s_m[BEAM_MAX], s_ls[BEAM_MAX], s_bs[BEAM_MAX];
   __shared__ float redf[32];
@@ -1534,16 +1546,32 @@ __device__ __forceinline__ void beam_topk_body(const __nv_bfloat16* __restrict__
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   constexpr int NW = BT_THREADS / 32;
   const int ns = n_special;
+  const int nb = GROUP ? gr.Kg : K;                              // beams scanned, from beam k0 of the prompt
+  const int k0 = GROUP ? gr.g * gr.Kg : 0;
   if (tid < ns) s_special[tid] = special[tid];
-  if (tid < K) s_bs[tid] = beam_score[b * K + tid];
+  if (tid < nb) s_bs[tid] = beam_score[b * K + k0 + tid];
+  int* s_div = nullptr;                                          // GROUP: the earlier groups' tokens of this step
+  if constexpr (GROUP) {
+    __shared__ int s_div_tok[BEAM_MAX];
+    s_div = s_div_tok;
+    if (tid < k0) s_div[tid] = gr.next_ids[b * K + tid];
+  }
   __syncthreads();
   auto is_special = [&](int c) {
     bool sp = false;
     for (int s = 0; s < ns; ++s) sp |= (s_special[s] == c);
     return sp;
   };
-  for (int k = 0; k < K; ++k) {
-    const __nv_bfloat16* row = logits + (int64_t)b * ld_prompt + (int64_t)k * ld_beam;
+  auto diversity = [&](float lp, int c) {                        // the Hamming penalty on a bf16 log-prob
+    if constexpr (GROUP) {
+      int f = 0;
+      for (int i = 0; i < k0; ++i) f += (s_div[i] == c);
+      if (f) lp = bf16_round(__fsub_rn(lp, __fmul_rn(gr.penalty, (float)f)));
+    }
+    return lp;
+  };
+  for (int k = 0; k < nb; ++k) {
+    const __nv_bfloat16* row = logits + (int64_t)b * ld_prompt + (int64_t)(k0 + k) * ld_beam;
     float mx = -INFINITY;
     for (int c = tid; c < V; c += BT_THREADS)
       if (!is_special(c)) mx = fmaxf(mx, __bfloat162float(row[c]));
@@ -1573,11 +1601,11 @@ __device__ __forceinline__ void beam_topk_body(const __nv_bfloat16* __restrict__
   unsigned long long L[BT_LIST];                                 // this thread's best keys, descending; 0 = empty
 #pragma unroll
   for (int i = 0; i < BT_LIST; ++i) L[i] = 0ull;
-  for (int k = 0; k < K; ++k) {
-    const __nv_bfloat16* row = logits + (int64_t)b * ld_prompt + (int64_t)k * ld_beam;
+  for (int k = 0; k < nb; ++k) {
+    const __nv_bfloat16* row = logits + (int64_t)b * ld_prompt + (int64_t)(k0 + k) * ld_beam;
     const float m = s_m[k], ls = s_ls[k], bs = s_bs[k];
     __nv_bfloat16* srow = nullptr;
-    if constexpr (SCORES) srow = so.row(b, b * K + k);
+    if constexpr (SCORES) srow = so.row(b, b * K + k0 + k);
     uint32_t* seen = nullptr;
     uint32_t* banned = nullptr;
     uint32_t* allowed = nullptr;
@@ -1591,7 +1619,7 @@ __device__ __forceinline__ void beam_topk_body(const __nv_bfloat16* __restrict__
       for (int i = tid; i < NMAPS * nw; i += BT_THREADS) bt_bits[i] = 0u;
       __syncthreads();
       const int S = *bp.prompt_width, t = bp.prompt_state[b * 5], L = S + t;
-      const ProcHist h{bp.prompt + (int64_t)b * bp.ld_prompt, bp.hist + (int64_t)(b * K + k) * bp.G, S};
+      const ProcHist h{bp.prompt + (int64_t)b * bp.ld_prompt, bp.hist + (int64_t)(b * K + k0 + k) * bp.G, S};
       __shared__ int s_node;                                     // TRIE: the beam's node
       if constexpr (TRIE)
         if (tid == 0) s_node = trie_walk(tr, bp.hist + (int64_t)(b * K + k) * bp.G, t);
@@ -1621,7 +1649,7 @@ __device__ __forceinline__ void beam_topk_body(const __nv_bfloat16* __restrict__
       float sc = -INFINITY;
       if constexpr (PROC) {
         if (!is_special(c)) {
-          float lp = bf16_round((__bfloat162float(row[c]) - m) - ls);
+          float lp = diversity(bf16_round((__bfloat162float(row[c]) - m) - ls), c);
           const uint32_t bit = 1u << (c & 31);
           if (seen[c >> 5] & bit) lp = rep_penalize(lp, bp.p.penalty);
           if (banned[c >> 5] & bit) lp = -INFINITY;
@@ -1635,14 +1663,14 @@ __device__ __forceinline__ void beam_topk_body(const __nv_bfloat16* __restrict__
       } else {
         if constexpr (SCORES) {
           if (!is_special(c)) {
-            const float lp = bf16_round((__bfloat162float(row[c]) - m) - ls);
+            const float lp = diversity(bf16_round((__bfloat162float(row[c]) - m) - ls), c);
             srow[c] = __float2bfloat16_rn(lp);
             sc = lp + bs;
           } else {
             srow[c] = __float2bfloat16_rn(-INFINITY);
           }
         } else {
-          if (!is_special(c)) sc = bf16_round((__bfloat162float(row[c]) - m) - ls) + bs;
+          if (!is_special(c)) sc = diversity(bf16_round((__bfloat162float(row[c]) - m) - ls), c) + bs;
         }
       }
       if (sc != sc) sc = -INFINITY;
@@ -1659,7 +1687,7 @@ __device__ __forceinline__ void beam_topk_body(const __nv_bfloat16* __restrict__
     }
   }
   // 2K rounds: the CTA-wide largest head wins and its owner pops it
-  for (int r = 0; r < 2 * K; ++r) {
+  for (int r = 0; r < 2 * nb; ++r) {
     unsigned long long best = L[0];
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
@@ -1681,9 +1709,9 @@ __device__ __forceinline__ void beam_topk_body(const __nv_bfloat16* __restrict__
     }
     if (tid == 0) {
       const uint32_t flat = 0xffffffffu - (uint32_t)(best & 0xffffffffull);
-      cand_score[b * 2 * K + r] = f32_unorder((uint32_t)(best >> 32));
-      cand_tok[b * 2 * K + r] = (int)(flat % (uint32_t)V);
-      cand_par[b * 2 * K + r] = (int)(flat / (uint32_t)V);
+      cand_score[b * 2 * nb + r] = f32_unorder((uint32_t)(best >> 32));
+      cand_tok[b * 2 * nb + r] = (int)(flat % (uint32_t)V);
+      cand_par[b * 2 * nb + r] = (int)(flat / (uint32_t)V);
     }
     __syncthreads();                                             // redk is reused by the next round
   }
@@ -1744,6 +1772,46 @@ __global__ void __launch_bounds__(BT_THREADS, 1) beam_topk_trie_scores_kernel(co
                                                                               ScoresOut so) {
   beam_topk_body<true, true, true>(logits, ld_prompt, ld_beam, V, special, n_special, beam_score, K, cand_score, cand_tok, cand_par,
                                    bp, tr, so);
+}
+
+// the group top-k kernels (nv_beam_topk_group[_processed][_scores]); bounds as above
+__global__ void __launch_bounds__(BT_THREADS) beam_topk_group_kernel(const __nv_bfloat16* __restrict__ logits, int64_t ld_prompt,
+                                                                     int64_t ld_beam, int V, const int* __restrict__ special,
+                                                                     int n_special, const float* __restrict__ beam_score, int K,
+                                                                     float* __restrict__ cand_score, int* __restrict__ cand_tok,
+                                                                     int* __restrict__ cand_par, BeamGroup gr) {
+  beam_topk_body<false, false, false, true>(logits, ld_prompt, ld_beam, V, special, n_special, beam_score, K, cand_score, cand_tok,
+                                            cand_par, BeamProc{}, BeamTrie{}, ScoresOut{}, gr);
+}
+
+__global__ void __launch_bounds__(BT_THREADS, 1) beam_topk_group_proc_kernel(const __nv_bfloat16* __restrict__ logits,
+                                                                             int64_t ld_prompt, int64_t ld_beam, int V,
+                                                                             const int* __restrict__ special, int n_special,
+                                                                             const float* __restrict__ beam_score, int K,
+                                                                             float* __restrict__ cand_score, int* __restrict__ cand_tok,
+                                                                             int* __restrict__ cand_par, BeamProc bp, BeamGroup gr) {
+  beam_topk_body<true, false, false, true>(logits, ld_prompt, ld_beam, V, special, n_special, beam_score, K, cand_score, cand_tok,
+                                           cand_par, bp, BeamTrie{}, ScoresOut{}, gr);
+}
+
+__global__ void __launch_bounds__(BT_THREADS) beam_topk_group_scores_kernel(const __nv_bfloat16* __restrict__ logits, int64_t ld_prompt,
+                                                                            int64_t ld_beam, int V, const int* __restrict__ special,
+                                                                            int n_special, const float* __restrict__ beam_score, int K,
+                                                                            float* __restrict__ cand_score, int* __restrict__ cand_tok,
+                                                                            int* __restrict__ cand_par, ScoresOut so, BeamGroup gr) {
+  beam_topk_body<false, false, true, true>(logits, ld_prompt, ld_beam, V, special, n_special, beam_score, K, cand_score, cand_tok,
+                                           cand_par, BeamProc{}, BeamTrie{}, so, gr);
+}
+
+__global__ void __launch_bounds__(BT_THREADS, 1) beam_topk_group_proc_scores_kernel(const __nv_bfloat16* __restrict__ logits,
+                                                                                    int64_t ld_prompt, int64_t ld_beam, int V,
+                                                                                    const int* __restrict__ special, int n_special,
+                                                                                    const float* __restrict__ beam_score, int K,
+                                                                                    float* __restrict__ cand_score,
+                                                                                    int* __restrict__ cand_tok, int* __restrict__ cand_par,
+                                                                                    BeamProc bp, ScoresOut so, BeamGroup gr) {
+  beam_topk_body<true, false, true, true>(logits, ld_prompt, ld_beam, V, special, n_special, beam_score, K, cand_score, cand_tok,
+                                          cand_par, bp, BeamTrie{}, so, gr);
 }
 
 // ---- answer scoring (nv_trie_score): every answer of a trie teacher-forced over one tree-masked forward ----
@@ -1853,13 +1921,24 @@ struct BeamTrace {
   int* done_step;
 };
 
-template <bool SCORES>
+// GROUP (nv_beam_select_group*, diverse beam search): process over group g's 2Kg candidates of nv_beam_topk_group (cand_*
+// [B, 2Kg], parents local to the group) with group_size Kg, against the prompt's one set of K hypotheses (4.28's
+// BeamSearchScorer with num_beam_groups: EOS at rank >= Kg is skipped, Kg survivors).  It reads the current done flag, so a
+// prompt an earlier group finished in this step pads, and it reorders and writes only the group's rows b * K + k0 + [0, Kg)
+// (k0 = g * Kg; parents, par_hist and hyp_par in global rows).  Only the last group's launch (``last``) advances BS_STEP, so
+// the scans of later groups still see step t.
+struct BeamSelGroup {
+  int g, Kg, last;
+};
+
+template <bool SCORES, bool GROUP = false>
 __device__ __forceinline__ void beam_select_body(const float* __restrict__ cand_score, const int* __restrict__ cand_tok,
                                                  const int* __restrict__ cand_par, float* __restrict__ beam_score,
                                                  int* __restrict__ hist, int* __restrict__ src, double* __restrict__ hyp_score,
                                                  int* __restrict__ hyp_meta, int* __restrict__ hyp_tok, int* __restrict__ pstate,
                                                  int* __restrict__ next_ids, int* __restrict__ lens, const double* __restrict__ norm,
-                                                 int K, int G, int eos_id, int pad_id, int early_stopping, const BeamTrace& tr) {
+                                                 int K, int G, int eos_id, int pad_id, int early_stopping, const BeamTrace& tr,
+                                                 const BeamSelGroup& gr = BeamSelGroup{}) {
   __shared__ int s_tok[BEAM_MAX], s_par[BEAM_MAX];
   __shared__ float s_sc[BEAM_MAX];
   __shared__ int s_op_slot[BEAM_MAX], s_op_par[BEAM_MAX], s_nops;
@@ -1870,10 +1949,12 @@ __device__ __forceinline__ void beam_select_body(const float* __restrict__ cand_
   int* ps = pstate + b * BS_FIELDS;
   const int t = ps[BS_STEP];
   if (t >= G) return;                                            // the host sizes G to the call's max_new_tokens
+  const int nb = GROUP ? gr.Kg : K;                              // beams selected: rows b * K + k0 + [0, nb)
+  const int k0 = GROUP ? gr.g * gr.Kg : 0;
   if (tid == 0) {
     int nops = 0;
     if (ps[BS_DONE]) {                                           // a done prompt's beams emit pad with score 0
-      for (int j = 0; j < K; ++j) { s_tok[j] = pad_id; s_par[j] = j; s_sc[j] = 0.f; }
+      for (int j = 0; j < nb; ++j) { s_tok[j] = pad_id; s_par[j] = j; s_sc[j] = 0.f; }
     } else {
       double* hs = hyp_score + b * (K + 1);
       int* hm = hyp_meta + b * K * 2;
@@ -1881,11 +1962,11 @@ __device__ __forceinline__ void beam_select_body(const float* __restrict__ cand_
       int cnt = ps[BS_COUNT], seq = ps[BS_SEQ];
       const double nt = norm[t];
       int j = 0;
-      for (int rank = 0; rank < 2 * K; ++rank) {
-        const int tok = cand_tok[b * 2 * K + rank], par = cand_par[b * 2 * K + rank];
-        const float sc = cand_score[b * 2 * K + rank];
+      for (int rank = 0; rank < 2 * nb; ++rank) {
+        const int tok = cand_tok[b * 2 * nb + rank], par = cand_par[b * 2 * nb + rank];
+        const float sc = cand_score[b * 2 * nb + rank];
         if (tok == eos_id) {
-          if (rank >= K) continue;                               // EOS below the top K is not a hypothesis
+          if (rank >= nb) continue;                              // EOS below the top K is not a hypothesis
           const double score = (double)sc / nt;
           if (cnt < K || score > worst) {
             int slot;
@@ -1912,10 +1993,10 @@ __device__ __forceinline__ void beam_select_body(const float* __restrict__ cand_
           s_tok[j] = tok; s_par[j] = par; s_sc[j] = sc;
           ++j;
         }
-        if (j == K) break;
+        if (j == nb) break;
       }
       int done = 0;
-      if (cnt >= K) done = early_stopping ? 1 : (worst >= (double)cand_score[b * 2 * K] / nt);
+      if (cnt >= K) done = early_stopping ? 1 : (worst >= (double)cand_score[b * 2 * nb] / nt);
       if constexpr (SCORES)
         if (done) tr.done_step[b] = t + 1;
       hs[K] = worst;
@@ -1927,31 +2008,31 @@ __device__ __forceinline__ void beam_select_body(const float* __restrict__ cand_
   }
   __syncthreads();
   for (int o = 0; o < s_nops; ++o) {                             // in order: a later hypothesis may take an earlier one's slot
-    const int* from = hist + (int64_t)(b * K + s_op_par[o]) * G;
+    const int* from = hist + (int64_t)(b * K + k0 + s_op_par[o]) * G;
     int* to = hyp_tok + (int64_t)(b * K + s_op_slot[o]) * G;
     for (int i = tid; i < t; i += BS_THREADS) to[i] = from[i];
     if constexpr (SCORES) {
-      const int* pf = tr.par_hist + (int64_t)(b * K + s_op_par[o]) * G;
+      const int* pf = tr.par_hist + (int64_t)(b * K + k0 + s_op_par[o]) * G;
       int* pt = tr.hyp_par + (int64_t)(b * K + s_op_slot[o]) * G;
       for (int i = tid; i < t; i += BS_THREADS) pt[i] = pf[i];
-      if (tid == 0) pt[t] = b * K + s_op_par[o];
+      if (tid == 0) pt[t] = b * K + k0 + s_op_par[o];
     }
   }
   for (int c0 = 0; c0 < t; c0 += BS_CHUNK) {                     // rows of the new beams = rows of their parents
     const int n = min(BS_CHUNK, t - c0);
-    for (int idx = tid; idx < K * BS_CHUNK; idx += BS_THREADS) {
+    for (int idx = tid; idx < nb * BS_CHUNK; idx += BS_THREADS) {
       const int j = idx / BS_CHUNK, i = idx % BS_CHUNK;
       if (i < n) {
-        const int64_t from = (int64_t)(b * K + s_par[j]) * G + c0 + i;
+        const int64_t from = (int64_t)(b * K + k0 + s_par[j]) * G + c0 + i;
         s_h[j][i] = hist[from];
         s_s[j][i] = src[from];
       }
     }
     __syncthreads();
-    for (int idx = tid; idx < K * BS_CHUNK; idx += BS_THREADS) {
+    for (int idx = tid; idx < nb * BS_CHUNK; idx += BS_THREADS) {
       const int j = idx / BS_CHUNK, i = idx % BS_CHUNK;
       if (i < n) {
-        const int64_t to = (int64_t)(b * K + j) * G + c0 + i;
+        const int64_t to = (int64_t)(b * K + k0 + j) * G + c0 + i;
         hist[to] = s_h[j][i];
         src[to] = s_s[j][i];
       }
@@ -1961,21 +2042,21 @@ __device__ __forceinline__ void beam_select_body(const float* __restrict__ cand_
   if constexpr (SCORES) {
     for (int c0 = 0; c0 < t; c0 += BS_CHUNK) {                   // par_hist by parent, through s_h
       const int n = min(BS_CHUNK, t - c0);
-      for (int idx = tid; idx < K * BS_CHUNK; idx += BS_THREADS) {
+      for (int idx = tid; idx < nb * BS_CHUNK; idx += BS_THREADS) {
         const int j = idx / BS_CHUNK, i = idx % BS_CHUNK;
-        if (i < n) s_h[j][i] = tr.par_hist[(int64_t)(b * K + s_par[j]) * G + c0 + i];
+        if (i < n) s_h[j][i] = tr.par_hist[(int64_t)(b * K + k0 + s_par[j]) * G + c0 + i];
       }
       __syncthreads();
-      for (int idx = tid; idx < K * BS_CHUNK; idx += BS_THREADS) {
+      for (int idx = tid; idx < nb * BS_CHUNK; idx += BS_THREADS) {
         const int j = idx / BS_CHUNK, i = idx % BS_CHUNK;
-        if (i < n) tr.par_hist[(int64_t)(b * K + j) * G + c0 + i] = s_h[j][i];
+        if (i < n) tr.par_hist[(int64_t)(b * K + k0 + j) * G + c0 + i] = s_h[j][i];
       }
       __syncthreads();
     }
   }
-  if (tid < K) {
-    const int r = b * K + tid;
-    if constexpr (SCORES) tr.par_hist[(int64_t)r * G + t] = b * K + s_par[tid];
+  if (tid < nb) {
+    const int r = b * K + k0 + tid;
+    if constexpr (SCORES) tr.par_hist[(int64_t)r * G + t] = b * K + k0 + s_par[tid];
     hist[(int64_t)r * G + t] = s_tok[tid];
     src[(int64_t)r * G + t] = r;                                 // the next step writes generated key t of row r at (r, t)
     next_ids[r] = s_tok[tid];
@@ -1983,7 +2064,7 @@ __device__ __forceinline__ void beam_select_body(const float* __restrict__ cand_
     beam_score[r] = s_sc[tid];
   }
   __syncthreads();
-  if (tid == 0) ps[BS_STEP] = t + 1;
+  if (tid == 0 && (!GROUP || gr.last)) ps[BS_STEP] = t + 1;
 }
 
 __global__ void __launch_bounds__(BS_THREADS) beam_select_kernel(const float* __restrict__ cand_score, const int* __restrict__ cand_tok,
@@ -2008,6 +2089,32 @@ __global__ void __launch_bounds__(BS_THREADS) beam_select_scores_kernel(const fl
                                                                         int G, int eos_id, int pad_id, int early_stopping, BeamTrace tr) {
   beam_select_body<true>(cand_score, cand_tok, cand_par, beam_score, hist, src, hyp_score, hyp_meta, hyp_tok, pstate, next_ids, lens,
                          norm, K, G, eos_id, pad_id, early_stopping, tr);
+}
+
+__global__ void __launch_bounds__(BS_THREADS, 1) beam_select_group_kernel(const float* __restrict__ cand_score,
+                                                                       const int* __restrict__ cand_tok, const int* __restrict__ cand_par,
+                                                                       float* __restrict__ beam_score, int* __restrict__ hist,
+                                                                       int* __restrict__ src, double* __restrict__ hyp_score,
+                                                                       int* __restrict__ hyp_meta, int* __restrict__ hyp_tok,
+                                                                       int* __restrict__ pstate, int* __restrict__ next_ids,
+                                                                       int* __restrict__ lens, const double* __restrict__ norm, int K,
+                                                                       int G, int eos_id, int pad_id, int early_stopping, BeamSelGroup gr) {
+  beam_select_body<false, true>(cand_score, cand_tok, cand_par, beam_score, hist, src, hyp_score, hyp_meta, hyp_tok, pstate, next_ids,
+                                lens, norm, K, G, eos_id, pad_id, early_stopping, BeamTrace{}, gr);
+}
+
+__global__ void __launch_bounds__(BS_THREADS, 1) beam_select_group_scores_kernel(const float* __restrict__ cand_score,
+                                                                              const int* __restrict__ cand_tok,
+                                                                              const int* __restrict__ cand_par, float* __restrict__ beam_score,
+                                                                              int* __restrict__ hist, int* __restrict__ src,
+                                                                              double* __restrict__ hyp_score, int* __restrict__ hyp_meta,
+                                                                              int* __restrict__ hyp_tok, int* __restrict__ pstate,
+                                                                              int* __restrict__ next_ids, int* __restrict__ lens,
+                                                                              const double* __restrict__ norm, int K, int G, int eos_id,
+                                                                              int pad_id, int early_stopping, BeamTrace tr,
+                                                                              BeamSelGroup gr) {
+  beam_select_body<true, true>(cand_score, cand_tok, cand_par, beam_score, hist, src, hyp_score, hyp_meta, hyp_tok, pstate, next_ids,
+                               lens, norm, K, G, eos_id, pad_id, early_stopping, tr, gr);
 }
 
 // ---- contrastive search (GenerationMixin.contrastive_search / _ranking_fast of transformers 4.28) ----
@@ -2799,6 +2906,139 @@ int nv_beam_select_scores(const float* cand_score, const int* cand_tok, const in
                      beam_score, hist, src, hyp_score, hyp_meta, hyp_tok, prompt_state, next_ids, lens, norm, K, G, eos_id, pad_id,
                      early_stopping, BeamTrace{par_hist, hyp_par, done_step}));
   return NV_OK;
+}
+
+// Diverse (group) beam search: group g of n_groups (see beam_topk_body / beam_select_body with GROUP).  One static entry for the
+// four top-k forms: prompt_ids null = no processors, scores null = no scores output.
+static int beam_topk_group(const char* name, const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, const int* special,
+                           int n_special, const float* beam_score, float* cand_score, int* cand_tok, int* cand_parent,
+                           const int* prompt_ids, int64_t ld_ids, const int* prompt_width, const int* hist, int G,
+                           const int* prompt_state, float penalty, int ngram, int min_length, int min_new_tokens, int eos_id,
+                           void* scores, int64_t ld_scores, int64_t plane, const int* next_ids, float diversity_penalty, int group,
+                           int n_groups, int B, int K, void* stream) {
+  NV_REQUIRE(logits && beam_score && cand_score && cand_tok && cand_parent && next_ids && V > 0 && B >= 0,
+             "%s: bad arguments (V=%d B=%d)", name, V, B);
+  NV_REQUIRE(K >= 2 && K <= BEAM_MAX && n_groups >= 2 && n_groups <= K && K % n_groups == 0 && group >= 0 && group < n_groups &&
+             2 * (K / n_groups) <= V, "%s: K=%d beams in %d groups (group %d): 2..%d beams, 2..K groups dividing K", name, K,
+             n_groups, group, BEAM_MAX);
+  NV_REQUIRE((int64_t)K * V < 0xffffffffll, "%s: K * V = %lld does not fit the 32-bit candidate index", name, (long long)K * V);
+  NV_REQUIRE(n_special >= 0 && n_special <= MAX_SPECIAL && (n_special == 0 || special), "%s: n_special=%d out of range (max %d)",
+             name, n_special, MAX_SPECIAL);
+  NV_REQUIRE(diversity_penalty > 0.f, "%s: diversity_penalty=%g must be > 0", name, (double)diversity_penalty);
+  if (prompt_ids) {
+    NV_REQUIRE(prompt_width && hist && prompt_state && G > 0, "%s: processors need prompt_width, hist and prompt_state", name);
+    const int st = check_proc(name, V, penalty, ngram, min_length, min_new_tokens);
+    if (st != NV_OK) return st;
+  }
+  if (scores) {
+    const int st = check_scores(name, scores, ld_scores, plane, prompt_state, V, B * K);
+    if (st != NV_OK) return st;
+  }
+  if (B == 0) return NV_OK;
+  const int Kg = K / n_groups;
+  const BeamGroup gr{next_ids, diversity_penalty, group, Kg};
+  const ScoresOut so{BF(scores), ld_scores, plane, prompt_state, BS_FIELDS};
+  if (prompt_ids) {
+    const BeamProc bp{prompt_ids, ld_ids, prompt_width, hist, G, prompt_state, ProcParams{penalty, ngram, min_length, min_new_tokens, eos_id}};
+    const size_t smem = (size_t)((V + 31) / 32) * 4 * 2;
+    if (scores)
+      NV_CUDA(launch_pdl(beam_topk_group_proc_scores_kernel, dim3(B), dim3(BT_THREADS), smem, S_(stream), CBF(logits), ld_prompt,
+                         ld_beam, V, special, n_special, beam_score, K, cand_score, cand_tok, cand_parent, bp, so, gr));
+    else
+      NV_CUDA(launch_pdl(beam_topk_group_proc_kernel, dim3(B), dim3(BT_THREADS), smem, S_(stream), CBF(logits), ld_prompt, ld_beam,
+                         V, special, n_special, beam_score, K, cand_score, cand_tok, cand_parent, bp, gr));
+  } else if (scores) {
+    NV_CUDA(launch_pdl(beam_topk_group_scores_kernel, dim3(B), dim3(BT_THREADS), 0, S_(stream), CBF(logits), ld_prompt, ld_beam, V,
+                       special, n_special, beam_score, K, cand_score, cand_tok, cand_parent, so, gr));
+  } else {
+    NV_CUDA(launch_pdl(beam_topk_group_kernel, dim3(B), dim3(BT_THREADS), 0, S_(stream), CBF(logits), ld_prompt, ld_beam, V, special,
+                       n_special, beam_score, K, cand_score, cand_tok, cand_parent, gr));
+  }
+  return NV_OK;
+}
+
+int nv_beam_topk_group(const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, const int* special, int n_special,
+                       const float* beam_score, float* cand_score, int* cand_tok, int* cand_parent, const int* next_ids,
+                       float diversity_penalty, int group, int n_groups, int B, int K, void* stream) {
+  return beam_topk_group("nv_beam_topk_group", logits, ld_prompt, ld_beam, V, special, n_special, beam_score, cand_score, cand_tok,
+                         cand_parent, nullptr, 0, nullptr, nullptr, 0, nullptr, 1.f, 0, 0, 0, -1, nullptr, 0, 0, next_ids,
+                         diversity_penalty, group, n_groups, B, K, stream);
+}
+
+int nv_beam_topk_group_scores(const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, const int* special, int n_special,
+                              const float* beam_score, float* cand_score, int* cand_tok, int* cand_parent, const int* prompt_state,
+                              void* scores, int64_t ld_scores, int64_t plane, const int* next_ids, float diversity_penalty, int group,
+                              int n_groups, int B, int K, void* stream) {
+  NV_REQUIRE(scores && prompt_state, "nv_beam_topk_group_scores: null scores or prompt_state");
+  return beam_topk_group("nv_beam_topk_group_scores", logits, ld_prompt, ld_beam, V, special, n_special, beam_score, cand_score,
+                         cand_tok, cand_parent, nullptr, 0, nullptr, nullptr, 0, prompt_state, 1.f, 0, 0, 0, -1, scores, ld_scores,
+                         plane, next_ids, diversity_penalty, group, n_groups, B, K, stream);
+}
+
+int nv_beam_topk_group_processed(const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, const int* special, int n_special,
+                                 const float* beam_score, float* cand_score, int* cand_tok, int* cand_parent, const int* prompt_ids,
+                                 int64_t ld_ids, const int* prompt_width, const int* hist, int G, const int* prompt_state,
+                                 float penalty, int ngram, int min_length, int min_new_tokens, int eos_id, const int* next_ids,
+                                 float diversity_penalty, int group, int n_groups, int B, int K, void* stream) {
+  NV_REQUIRE(prompt_ids, "nv_beam_topk_group_processed: null prompt_ids");
+  return beam_topk_group("nv_beam_topk_group_processed", logits, ld_prompt, ld_beam, V, special, n_special, beam_score, cand_score,
+                         cand_tok, cand_parent, prompt_ids, ld_ids, prompt_width, hist, G, prompt_state, penalty, ngram, min_length,
+                         min_new_tokens, eos_id, nullptr, 0, 0, next_ids, diversity_penalty, group, n_groups, B, K, stream);
+}
+
+int nv_beam_topk_group_processed_scores(const void* logits, int64_t ld_prompt, int64_t ld_beam, int V, const int* special,
+                                        int n_special, const float* beam_score, float* cand_score, int* cand_tok, int* cand_parent,
+                                        const int* prompt_ids, int64_t ld_ids, const int* prompt_width, const int* hist, int G,
+                                        const int* prompt_state, float penalty, int ngram, int min_length, int min_new_tokens,
+                                        int eos_id, void* scores, int64_t ld_scores, int64_t plane, const int* next_ids,
+                                        float diversity_penalty, int group, int n_groups, int B, int K, void* stream) {
+  NV_REQUIRE(prompt_ids && scores, "nv_beam_topk_group_processed_scores: null prompt_ids or scores");
+  return beam_topk_group("nv_beam_topk_group_processed_scores", logits, ld_prompt, ld_beam, V, special, n_special, beam_score,
+                         cand_score, cand_tok, cand_parent, prompt_ids, ld_ids, prompt_width, hist, G, prompt_state, penalty, ngram,
+                         min_length, min_new_tokens, eos_id, scores, ld_scores, plane, next_ids, diversity_penalty, group, n_groups,
+                         B, K, stream);
+}
+
+// nv_beam_select over group g's candidates [B, 2 * (K / n_groups)] (see beam_select_body<..., true>); trace pointers all null
+// or all set (nv_beam_select_scores' beam_indices).
+static int beam_select_group(const char* name, const float* cand_score, const int* cand_tok, const int* cand_parent, float* beam_score,
+                             int* hist, int* src, double* hyp_score, int* hyp_meta, int* hyp_tok, int* prompt_state, int* next_ids,
+                             int* lens, const double* norm, int* par_hist, int* hyp_par, int* done_step, int group, int n_groups, int B,
+                             int K, int G, int eos_id, int pad_id, int early_stopping, void* stream) {
+  NV_REQUIRE(cand_score && cand_tok && cand_parent && beam_score && hist && src && hyp_score && hyp_meta && hyp_tok &&
+             prompt_state && next_ids && lens && norm, "%s: null argument", name);
+  NV_REQUIRE(K >= 2 && K <= BEAM_MAX && n_groups >= 2 && n_groups <= K && K % n_groups == 0 && group >= 0 && group < n_groups &&
+             G > 0 && B >= 0, "%s: bad sizes (B=%d K=%d groups=%d group=%d G=%d)", name, B, K, n_groups, group, G);
+  if (B == 0) return NV_OK;
+  const BeamSelGroup gr{group, K / n_groups, group == n_groups - 1 ? 1 : 0};
+  if (par_hist)
+    NV_CUDA(launch_pdl(beam_select_group_scores_kernel, dim3(B), dim3(BS_THREADS), 0, S_(stream), cand_score, cand_tok, cand_parent,
+                       beam_score, hist, src, hyp_score, hyp_meta, hyp_tok, prompt_state, next_ids, lens, norm, K, G, eos_id, pad_id,
+                       early_stopping, BeamTrace{par_hist, hyp_par, done_step}, gr));
+  else
+    NV_CUDA(launch_pdl(beam_select_group_kernel, dim3(B), dim3(BS_THREADS), 0, S_(stream), cand_score, cand_tok, cand_parent,
+                       beam_score, hist, src, hyp_score, hyp_meta, hyp_tok, prompt_state, next_ids, lens, norm, K, G, eos_id, pad_id,
+                       early_stopping, gr));
+  return NV_OK;
+}
+
+int nv_beam_select_group(const float* cand_score, const int* cand_tok, const int* cand_parent, float* beam_score, int* hist, int* src,
+                         double* hyp_score, int* hyp_meta, int* hyp_tok, int* prompt_state, int* next_ids, int* lens,
+                         const double* norm, int group, int n_groups, int B, int K, int G, int eos_id, int pad_id, int early_stopping,
+                         void* stream) {
+  return beam_select_group("nv_beam_select_group", cand_score, cand_tok, cand_parent, beam_score, hist, src, hyp_score, hyp_meta,
+                           hyp_tok, prompt_state, next_ids, lens, norm, nullptr, nullptr, nullptr, group, n_groups, B, K, G, eos_id,
+                           pad_id, early_stopping, stream);
+}
+
+int nv_beam_select_group_scores(const float* cand_score, const int* cand_tok, const int* cand_parent, float* beam_score, int* hist,
+                                int* src, double* hyp_score, int* hyp_meta, int* hyp_tok, int* prompt_state, int* next_ids, int* lens,
+                                const double* norm, int* par_hist, int* hyp_par, int* done_step, int group, int n_groups, int B, int K,
+                                int G, int eos_id, int pad_id, int early_stopping, void* stream) {
+  NV_REQUIRE(par_hist && hyp_par && done_step, "nv_beam_select_group_scores: null argument");
+  return beam_select_group("nv_beam_select_group_scores", cand_score, cand_tok, cand_parent, beam_score, hist, src, hyp_score,
+                           hyp_meta, hyp_tok, prompt_state, next_ids, lens, norm, par_hist, hyp_par, done_step, group, n_groups, B, K,
+                           G, eos_id, pad_id, early_stopping, stream);
 }
 
 // nv_decode_attn_rope for R = B * K beam rows over a prompt cache shared by the K beams of a prompt and a generated cache

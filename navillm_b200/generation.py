@@ -40,6 +40,8 @@ class Decoding:
     lookup_k: Optional[int] = None           # prompt-lookup decoding: drafts per step (the window is lookup_k + 1 rows)
     lookup_ngram: Optional[int] = None       # prompt-lookup decoding: max_matching_ngram_size
     scores: bool = False                     # return_dict_in_generate + output_scores: the step stores HF's per-step scores
+    groups: int = 1                          # beams: num_beam_groups (diverse beam search when > 1)
+    diversity_penalty: Optional[float] = None    # diverse beam search: the Hamming diversity penalty
 
     @property
     def sampled(self) -> bool:
@@ -48,7 +50,8 @@ class Decoding:
     def key(self) -> tuple:
         """The graph key: every field a captured step bakes in (not ``n_return`` or ``length_penalty``), the format last."""
         return (self.eos, self.pad, self.stop_on_eos, self.mode, self.temperature, self.top_k, self.top_p, self.trie_eos, self.n,
-                self.early_stopping, self.proc, self.penalty_alpha, self.lookup_k, self.lookup_ngram, self.scores, self.kv)
+                self.early_stopping, self.proc, self.penalty_alpha, self.lookup_k, self.lookup_ngram, self.scores, self.groups,
+                self.diversity_penalty, self.kv)
 
 
 def processors(repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens, eos: int) -> Optional[tuple]:
@@ -206,8 +209,9 @@ def prefill(lm, dec: Decoding, input_ids, attention_mask, vis, max_new_tokens: i
         st = SimpleNamespace(kc=cache(R, G), vc=cache(R, G), logits=logits_buffer(P * W, V, dev), next_ids=i32(P), lens=i32(R),
                              Sp=Sp, G=G, graph=None)
         if dec.mode == "beam":
-            st.beam_score, st.cand_score, st.cand_tok = zeros(torch.float32, R), zeros(torch.float32, B, 2 * n), i32(B, 2 * n)
-            st.cand_par, st.hist, st.src, st.hyp_score = i32(B, 2 * n), i32(R, G), i32(R, G), zeros(torch.float64, B, n + 1)
+            c = 2 * n // dec.groups                                         # candidates per prompt (and group) and step
+            st.beam_score, st.cand_score, st.cand_tok = zeros(torch.float32, R), zeros(torch.float32, B, c), i32(B, c)
+            st.cand_par, st.hist, st.src, st.hyp_score = i32(B, c), i32(R, G), i32(R, G), zeros(torch.float64, B, n + 1)
             st.hyp_meta, st.hyp_tok, st.pstate, st.norm = i32(B, n, 2), i32(B, n, G), i32(B, 5), zeros(torch.float64, G)
             if dec.scores:                                                  # 4.28's beam_indices (ops.beam_select trace=)
                 st.par_hist, st.hyp_par, st.done_step = i32(R, G), i32(B, n, G), i32(B)
@@ -686,12 +690,19 @@ def beam_search(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_gra
     root, and the log-probs its node does not allow become -inf after the processors, as 4.28's PrefixConstrainedLogitsProcessor
     masks log_softmax's output; the trie is loaded as in ``decode``, and one that outgrows the buffers is recaptured.
 
+    Diverse beam search (``dec.groups`` = G > 1, transformers 4.28's group_beam_search): the K beams of a prompt form G groups
+    of Kg = K / G, and only the first beam of each group starts with score 0.  The decode step runs over all B * K rows as
+    above; then, for g = 0 .. G - 1 in order, ``nv_beam_topk_group`` takes group g's 2Kg best candidates (each log-prob first
+    lowered by ``dec.diversity_penalty`` times the count of its token among the tokens groups 0 .. g - 1 chose in this step,
+    which their selects have just written to ``next_ids``) and ``nv_beam_select_group`` runs process for the group against the
+    prompt's one set of K hypotheses and reorders the group's rows.  All 2G launches are in the captured step.
+
     ``out_fields`` (return_dict_in_generate) gets ``sequences_scores`` fp32 [B * n], the returned hypotheses' scores from the host
     finalisation.  ``dec.scores`` (and output_scores) adds ``scores``: the top-k kernel of step t writes each beam's processed
     log-probs to plane t (``prompt_state[:, 0]``), one entry per step 4.28 runs (until every prompt is done, not the extra steps
     of the every-8-steps check); and ``beam_indices`` int64 [B * n, L]: ``nv_beam_select_scores`` keeps each beam's rows
     (``par_hist``) and each hypothesis' rows (``hyp_par``), padded with -1."""
-    K, eos, pad, proc, special = dec.n, dec.eos, dec.pad, dec.proc, lm.special_ids_dev
+    K, eos, pad, proc, special, n_groups = dec.n, dec.eos, dec.pad, dec.proc, lm.special_ids_dev, dec.groups
     if K > BEAM_MAX:
         raise NotImplementedError(f"generate(num_beams={K}): at most {BEAM_MAX} beams are built")
     if max_new_tokens < 1:
@@ -703,7 +714,7 @@ def beam_search(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_gra
         load_proc(st, input_ids, 0, G)
     if table is not None:
         trie_csr = load_trie(st, table)
-    st.beam_score.view(B, K).fill_(-1e9)[:, 0] = 0.0             # only beam 0 of a prompt expands at the first step
+    st.beam_score.view(B, K).fill_(-1e9)[:, ::K // n_groups] = 0.0   # only beam 0 of a prompt (of each group) expands first
     st.hyp_score.zero_()
     st.hyp_score[:, K] = 1e9                                      # BeamHypotheses.worst_score starts at 1e9
     st.hyp_meta.zero_()
@@ -720,6 +731,16 @@ def beam_search(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_gra
                                   st.hyp_meta, st.hyp_tok, st.pstate, st.next_ids, st.lens, st.norm, eos, pad,
                                   dec.early_stopping, trace=trace)
 
+    def group_step(first_step=False):
+        for g in range(n_groups):
+            ops.beam_topk_group(st.logits, special, st.beam_score, K, n_groups, g, st.cand_score, st.cand_tok, st.cand_par,
+                                st.next_ids, dec.diversity_penalty, first_step=first_step, proc=proc, prompt_ids=st.proc_ids
+                                if proc is not None else None, prompt_width=st.proc_width if proc is not None else None,
+                                hist=st.hist, prompt_state=st.pstate, scores=sc.get("scores"))
+            ops.beam_select_group(st.cand_score, st.cand_tok, st.cand_par, st.beam_score, st.hist, st.src, st.hyp_score, st.hyp_meta,
+                                  st.hyp_tok, st.pstate, st.next_ids, st.lens, st.norm, eos, pad, dec.early_stopping, n_groups, g,
+                                  trace=trace)
+
     def topk(first_step=False):
         if table is not None:
             ops.beam_topk_trie(st.logits, special, st.beam_score, K, st.cand_score, st.cand_tok, st.cand_par, st.proc_ids,
@@ -731,8 +752,11 @@ def beam_search(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_gra
             ops.beam_topk_processed(st.logits, special, st.beam_score, K, st.cand_score, st.cand_tok, st.cand_par, st.proc_ids,
                                     st.proc_width, st.hist, st.pstate, proc, first_step=first_step, scores=sc.get("scores"))
 
-    topk(first_step=True)
-    sel()
+    if n_groups > 1:
+        group_step(first_step=True)
+    else:
+        topk(first_step=True)
+        sel()
     timer.mark()
 
     def step():
@@ -740,8 +764,11 @@ def beam_search(lm, input_ids, attention_mask, vis, max_new_tokens, use_cuda_gra
             xt = ops.embed_fwd(st.next_ids, lm.model.embed_tokens.weight.data)
             h = lm.core.decode_step(xt, st.lens, st.kc, st.vc, beam=st.beam)
             decode_head(lm, h, st.logits)
-            topk()
-            sel()
+            if n_groups > 1:
+                group_step()
+            else:
+                topk()
+                sel()
 
     # like the greedy loop, ask the device whether every prompt is done only every few steps: a done prompt's steps leave
     # its hypotheses unchanged, so the extra steps change no output

@@ -17,6 +17,7 @@ from __future__ import annotations
 import contextlib
 import dataclasses
 import math
+import numbers
 import time
 import weakref
 from types import SimpleNamespace
@@ -110,6 +111,35 @@ def _lookup_k(k, ngram) -> tuple:
     if isinstance(ngram, bool) or not isinstance(ngram, int) or ngram < 1:
         raise ValueError(f"generate(max_matching_ngram_size={ngram!r}): a positive int expected")
     return k, ngram
+
+
+def _beam_groups(num_beams, num_beam_groups, diversity_penalty, do_sample: bool, other_processors: bool) -> int:
+    """``generate(num_beam_groups=G, diversity_penalty=d)`` validated as transformers 4.28 does (``ValueError``), before any
+    device work; returns G (1: no groups).  Groups without a penalty (None or 0), with sampling, or with ``trie=`` /
+    ``logits_processor=`` are not built (``NotImplementedError`` naming "group").  ``d`` without groups is ignored."""
+    if num_beam_groups is None or num_beam_groups <= 1:                  # as before: no groups (1, 1.0, np.int64(1), ...)
+        return 1
+    if isinstance(num_beam_groups, bool) or not isinstance(num_beam_groups, numbers.Integral):
+        raise ValueError(f"generate(num_beam_groups={num_beam_groups!r}): `num_beam_groups` has to be an integer")
+    groups = int(num_beam_groups)
+    if groups > num_beams:
+        raise ValueError(f"generate(num_beam_groups={groups}, num_beams={num_beams}): `num_beam_groups` has to be smaller or "
+                         "equal to `num_beams`")
+    if num_beams % groups:
+        raise ValueError(f"generate(num_beam_groups={groups}, num_beams={num_beams}): `num_beams` has to be divisible by "
+                         "`num_beam_groups`")
+    if do_sample:
+        raise NotImplementedError("generate(num_beam_groups > 1, do_sample=True): group (diverse) beam sampling is not built")
+    if diversity_penalty is None or (not isinstance(diversity_penalty, bool) and diversity_penalty == 0):
+        raise NotImplementedError("generate(num_beam_groups > 1) without diversity_penalty > 0: group beam search without a "
+                                  "penalty is G copies of one search and is not built")
+    if isinstance(diversity_penalty, bool) or not isinstance(diversity_penalty, float) or not diversity_penalty > 0:
+        raise ValueError(f"generate(diversity_penalty={diversity_penalty!r}): `diversity_penalty` should be a float strictly "
+                         "larger than 0")
+    if other_processors:
+        raise NotImplementedError("generate(num_beam_groups > 1) with trie= / logits_processor=: group (diverse) beam search "
+                                  "runs the device processors only")
+    return groups
 
 
 class PackedPrompt:
@@ -1025,7 +1055,8 @@ class ModifiedLlamaForCausalLM(nn.Module):
                  no_repeat_ngram_size: Optional[int] = None, min_length: Optional[int] = None,
                  min_new_tokens: Optional[int] = None, penalty_alpha: Optional[float] = None,
                  prompt_lookup_num_tokens: Optional[int] = None, max_matching_ngram_size: Optional[int] = 2,
-                 return_dict_in_generate: bool = False, output_scores: bool = False, **unused):
+                 return_dict_in_generate: bool = False, output_scores: bool = False,
+                 diversity_penalty: Optional[float] = None, **unused):
         """Prefill on the packed kernels (positions = cumsum(mask)-1 like HF generate; visual tokens injected only
         here, as in models/modified_lm.py:195-197), then one token per step over a pre-allocated KV cache.  The
         decode step of the greedy, sampled and trie-constrained modes has static shapes and is replayed as a CUDA graph
@@ -1051,8 +1082,19 @@ class ModifiedLlamaForCausalLM(nn.Module):
 
         ``num_beams > 1`` is HF beam search as transformers 4.28 (the reference's pin) runs it, ``length_penalty``,
         ``early_stopping`` and ``num_return_sequences`` included; see ``generation.beam_search``.  Returns [B * num_return_sequences,
-        L] ids.  Beam sampling, group beam search, ``logits_processor=`` with beams and more return sequences than beams raise
+        L] ids.  Beam sampling, ``logits_processor=`` with beams and more return sequences than beams raise
         ``NotImplementedError``.
+
+        ``num_beam_groups=G > 1`` with ``diversity_penalty > 0`` is 4.28's diverse (group) beam search: the K beams of a prompt
+        form G groups of K / G that take their steps in order, and each group's log-probs are lowered by ``diversity_penalty``
+        times the number of times the earlier groups chose the token in the same step (HammingDiversityLogitsProcessor, before
+        the device processors).  All groups share the prompt's K hypotheses, as in 4.28.  It runs on the device in the captured
+        step (``nv_beam_topk_group`` / ``nv_beam_select_group``, see ``generation.beam_search``); ``length_penalty``,
+        ``early_stopping``, ``num_return_sequences``, the device processors, per-step scores (``beam_indices`` hold global rows
+        b * K + k), the fp8 / int4 weight copies and the fp8 KV cache all apply.  ``num_beam_groups`` above ``num_beams`` or not
+        dividing it, and a ``diversity_penalty`` that is not a float > 0, raise ``ValueError``; groups without a penalty (None or
+        0: G identical copies of one search), with ``do_sample``, ``trie=`` or ``logits_processor=`` raise
+        ``NotImplementedError``.  ``diversity_penalty`` without groups is ignored.
 
         ``trie=`` with ``num_beams > 1`` is 4.28's beam search with a PrefixConstrainedLogitsProcessor whose allowed tokens come
         from walking the trie: each beam walks its own generated tokens from ``trie.root`` (a node without children stays; a token
@@ -1129,8 +1171,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
             if top_k > ops.CONTRASTIVE_KMAX:
                 raise NotImplementedError(f"generate(penalty_alpha > 0, top_k={top_k}): at most {ops.CONTRASTIVE_KMAX} candidates "
                                           "per prompt are built")
-        if num_beam_groups is not None and num_beam_groups > 1:
-            raise NotImplementedError("generate(num_beam_groups > 1): group (diverse) beam search is not built")
+        groups = _beam_groups(num_beams, num_beam_groups, diversity_penalty, do_sample, trie is not None or bool(logits_processor))
         top_p = 1.0 if top_p is None else float(top_p)
         if not 0.0 <= top_p <= 1.0:
             raise ValueError(f"generate(top_p={top_p}): top_p must lie in [0, 1]")
@@ -1186,7 +1227,8 @@ class ModifiedLlamaForCausalLM(nn.Module):
                                               "processors keep per-row state that reordering the beams would scramble")
             dec = generation.Decoding(int(eos), int(pad), None, "beam", self.kv_cache_dtype, n=int(num_beams), n_return=n_seq,
                                       length_penalty=float(length_penalty), early_stopping=bool(early_stopping), proc=proc,
-                                      trie_eos=None if table is None else table.eos, scores=scores)
+                                      trie_eos=None if table is None else table.eos, scores=scores, groups=groups,
+                                      diversity_penalty=float(diversity_penalty) if groups > 1 else None)
             out = generation.beam_search(*call, dec, table=table, out_fields=fields)
             if stats is not None and table is not None:
                 stats.update({"trie_path": "device", "trie_flatten_ms": flatten_ms})

@@ -525,6 +525,10 @@ class NavModel(nn.Module):
         # beam search over the answer trie: the beam kwargs (and output_scores) reach generate() only when the caller passes them
         beams = {k: kwargs[k] for k in ("num_beams", "num_return_sequences", "length_penalty", "early_stopping", "output_scores")
                  if k in kwargs}
+        # diverse beam search: num_beam_groups reaches generate() only together with diversity_penalty (num_beam_groups alone
+        # has always been dropped here, and a call that passes it keeps running plain beams)
+        if "diversity_penalty" in kwargs:
+            beams.update({k: kwargs[k] for k in ("num_beam_groups", "diversity_penalty") if k in kwargs})
         return self._generate_sentences(text, input_ids=text["input_ids"], attention_mask=text["attention_mask"], cand_vis=cand_vis,
                                         hist_vis=hist_vis_input, eos_token_id=self.lang_model.tokenizer.eos_token_id,
                                         pad_token_id=self.lang_model.tokenizer.unk_token_id, max_new_tokens=50, do_sample=False,

@@ -1043,6 +1043,67 @@ def beam_select(cand_score, cand_tok, cand_parent, beam_score, hist, src, hyp_sc
           "nv_beam_select")
 
 
+def beam_topk_group(logits, special, beam_score, K, groups, group, cand_score, cand_tok, cand_parent, next_ids, diversity_penalty, *,
+                    first_step=False, proc=None, prompt_ids=None, prompt_width=None, hist=None, prompt_state=None, scores=None):
+    """Diverse beam search's top-k for group ``group`` of ``groups`` (nv_beam_topk_group[_processed][_scores]): ``beam_topk`` over
+    the Kg = K / groups beams group * Kg + [0, Kg) of each prompt, each bf16 log-prob first lowered by diversity_penalty times the
+    count of its token among next_ids[b * K + 0 .. group * Kg) (4.28's Hamming diversity).  cand_* [B, 2Kg], parents local to the
+    group.  ``proc``: the processors of ``beam_topk_processed`` (prompt_ids, prompt_width, hist, prompt_state); ``scores``: the
+    group's rows of plane prompt_state[b, 0], as in ``beam_topk``."""
+    B = cand_score.shape[0]
+    V = logits.shape[1]
+    if not (isinstance(groups, int) and 2 <= groups <= K and K % groups == 0 and 0 <= group < groups):
+        raise ValueError(f"beam_topk_group: {K} beams in {groups} groups (group {group}) not supported")
+    Kg = K // groups
+    if logits.dtype != bf16 or logits.stride(1) != 1 or logits.shape[0] < (B if first_step else B * K):
+        raise ValueError(f"beam_topk_group: bf16 logits with {B if first_step else B * K} rows expected "
+                         f"(got {logits.dtype} {tuple(logits.shape)})")
+    _beam_io("beam_topk_group", B, Kg, 1, cand_score=cand_score, cand_tok=cand_tok, cand_parent=cand_parent)
+    _beam_io("beam_topk_group", B, K, 1, beam_score=beam_score, next_ids=next_ids)
+    ld = logits.stride(0)
+    head = (ptr(logits), i64(ld if first_step else K * ld), i64(0 if first_step else ld), i32(V), ptr(special), i32(special.numel()),
+            ptr(beam_score), ptr(cand_score), ptr(cand_tok), ptr(cand_parent))
+    tail = (ptr(next_ids), f32(diversity_penalty), i32(group), i32(groups), i32(B), i32(K), stream_ptr())
+    sc = () if scores is None else _beam_scores_io("beam_topk_group", scores, prompt_state, B, K, V)
+    lib = _lib.load()
+    if proc is not None:
+        _beam_io("beam_topk_group", B, K, hist.shape[1], hist=hist, prompt_state=prompt_state)
+        args = _proc_io("beam_topk_group", V, prompt_ids, prompt_width, hist, proc)
+        pa = (ptr(prompt_ids), i64(prompt_ids.stride(0)), ptr(prompt_width), ptr(hist), i32(hist.shape[1]), ptr(prompt_state), *args)
+        if scores is not None:
+            check(lib.nv_beam_topk_group_processed_scores(*head, *pa, *sc, *tail), "nv_beam_topk_group_processed_scores")
+        else:
+            check(lib.nv_beam_topk_group_processed(*head, *pa, *tail), "nv_beam_topk_group_processed")
+    elif scores is not None:
+        check(lib.nv_beam_topk_group_scores(*head, ptr(prompt_state), *sc, *tail), "nv_beam_topk_group_scores")
+    else:
+        check(lib.nv_beam_topk_group(*head, *tail), "nv_beam_topk_group")
+
+
+def beam_select_group(cand_score, cand_tok, cand_parent, beam_score, hist, src, hyp_score, hyp_meta, hyp_tok, prompt_state, next_ids,
+                      lens, norm, eos_id, pad_id, early_stopping, groups, group, *, trace=None):
+    """``beam_select`` over group ``group``'s candidates [B, 2Kg] of ``beam_topk_group`` (nv_beam_select_group[_scores]): process
+    with group_size Kg against the prompt's K hypotheses; only the group's rows are reordered and written, and only the last
+    group advances prompt_state[:, 0].  ``trace``: as in ``beam_select``, with global rows."""
+    B, K = hyp_score.shape[0], hyp_score.shape[1] - 1
+    G = hist.shape[1]
+    if not (isinstance(groups, int) and 2 <= groups <= K and K % groups == 0 and 0 <= group < groups):
+        raise ValueError(f"beam_select_group: {K} beams in {groups} groups (group {group}) not supported")
+    _beam_io("beam_select_group", B, K // groups, G, cand_score=cand_score, cand_tok=cand_tok, cand_parent=cand_parent)
+    _beam_io("beam_select_group", B, K, G, beam_score=beam_score, hist=hist, src=src, hyp_score=hyp_score, hyp_meta=hyp_meta,
+             hyp_tok=hyp_tok, prompt_state=prompt_state, next_ids=next_ids, lens=lens, norm=norm)
+    head = (ptr(cand_score), ptr(cand_tok), ptr(cand_parent), ptr(beam_score), ptr(hist), ptr(src), ptr(hyp_score), ptr(hyp_meta),
+            ptr(hyp_tok), ptr(prompt_state), ptr(next_ids), ptr(lens), ptr(norm))
+    tail = (i32(group), i32(groups), i32(B), i32(K), i32(G), i32(eos_id), i32(pad_id), i32(1 if early_stopping else 0), stream_ptr())
+    if trace is not None:
+        par_hist, hyp_par, done_step = trace
+        _beam_io("beam_select_group", B, K, G, hist=par_hist, hyp_tok=hyp_par, plens=done_step)
+        check(_lib.load().nv_beam_select_group_scores(*head, ptr(par_hist), ptr(hyp_par), ptr(done_step), *tail),
+              "nv_beam_select_group_scores")
+        return
+    check(_lib.load().nv_beam_select_group(*head, *tail), "nv_beam_select_group")
+
+
 def beam_norm(S: int, G: int, length_penalty: float) -> torch.Tensor:
     """The hypothesis normalisers (S + t) ** length_penalty, t < G, in the Python float arithmetic of transformers 4.28's
     BeamHypotheses.add (host fp64 [G]; copy it to the device for ``beam_select``)."""
