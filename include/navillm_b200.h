@@ -41,6 +41,12 @@ int nv_abi_version(void);
  * cudaLaunchAttributeProgrammaticStreamSerialization so a kernel's prologue (and the skinny GEMM's first weight tiles)
  * overlaps the tail of its predecessor.  Returns the previous setting.  Process-wide; default off. */
 int nv_set_pdl(int on);
+/* Batch-invariant split-K for the panorama encoder GEMMs nv_sgemm / nv_gemm_tf32 (NavModel.set_batch_invariant; reference
+ * image_embedding.py's nn.Linear / nn.TransformerEncoder layers): when on, the K split count is the largest power of two
+ * <= 8 that leaves every split at least 256 k (K alone decides), instead of following the tile count -- the number of
+ * views in the batch -- and sm_count().  The splits are added in rank order either way, so an element's bits then depend
+ * on its own row alone.  Returns the previous setting.  Process-wide; default off. */
+int nv_set_fixed_splits(int on);
 int nv_device_check(void); /* NV_OK iff the current device is sm_90 (Hopper) */
 int nv_sm_count(void);
 
@@ -66,6 +72,20 @@ int nv_gemm_skinny_bf16(const void* X, int64_t ldx, const void* W, int64_t ldw, 
 /* ... with the SwiGLU of HF LlamaMLP fused: h[M,F] = bf16(bf16(silu(g)) * u), [g|u] = bf16(X Wgu^T), Wgu [2F,K] */
 int nv_gemm_skinny_swiglu_bf16(const void* X, int64_t ldx, const void* Wgu, int64_t ldw, void* H, int64_t ldh, int M, int F,
                                int K, void* stream);
+/* Batch-invariant inference GEMMs (ModifiedLlamaForCausalLM.set_batch_invariant; csrc/gemm_bi.cu).  The invariant
+ * arithmetic of an element C[m, n]: acc = 0, then for every 64-deep k-block in k order the four m64nNk16 bf16 wgmma steps
+ * (fp32 accumulation, no split-K), then C = bf16(acc) | bf16(bf16(acc) + addend[m, n]) | for SwiGLU
+ * h = bf16(bf16(silu(g)) * u) from g = bf16(acc_g), u = bf16(acc_u).  nv_gemm_bf16 computes every element that way with
+ * any of its tiles, so a row's bits depend on that row alone.  These kernels give the same bits while streaming the
+ * weights over narrow 32-column tiles (64-row activation blocks, rows padded by TMA zero fill), so the decode steps keep
+ * weight-streaming rates at every batch size.  X [M,K], W [N,K] (nn.Linear layout), any M.
+ * nv_gemm_bi_bf16: the decode step's q|k|v, o_proj (+ residual) and down_proj (+ residual) (LlamaCore.decode_step) and
+ *   every inference lm_head (generation.lm_head_rows, the no-grad logits of ModifiedLlamaForCausalLM), each in the mode.
+ * nv_gemm_bi_swiglu_bf16: the decode step's gate|up projection with the SwiGLU of HF LlamaMLP fused, Wgu [2F,K], F % 16 == 0. */
+int nv_gemm_bi_bf16(const void* X, int64_t ldx, const void* W, int64_t ldw, void* C, int64_t ldc, const void* addend,
+                    int64_t ld_add, int M, int N, int K, void* stream);
+int nv_gemm_bi_swiglu_bf16(const void* X, int64_t ldx, const void* Wgu, int64_t ldw, void* H, int64_t ldh, int M, int F,
+                           int K, void* stream);
 /* Opt-in fp8 weight streaming of the same decode-step GEMMs (HF generate through models/modified_lm.py:184-199; no
  * reference counterpart for the number format).  nv_quantize_fp8_rows (csrc/quant.cu) rounds a bf16 weight W [N,K] to
  * e4m3 with one power-of-two scale per row: exps[n] = e_n (int8, the smallest e with max|W[n,:]| / 2^e <= 448, clamped

@@ -196,9 +196,10 @@ static int launch_tf32(const float* A, int64_t lda, const float* B, int64_t ldb,
   const uint32_t num_m = ceil_div_u32(M, T32_BM), num_n = ceil_div_u32(N, T32_BN);
   const uint32_t tiles = num_m * num_n, total_kb = ceil_div_u32(K, T32_BK);
   // split K until about two CTAs per SM are in flight, keeping at least 8 k-blocks (256 k) per split; the splits of
-  // a tile are one cluster (at most 8 CTAs)
+  // a tile are one cluster (at most 8 CTAs); with g_fixed_splits as far as K allows, whatever the tile count
   uint32_t splits = 1;
-  while (splits < 8 && tiles * splits * 2 <= 2u * (uint32_t)sm_count() && total_kb / (splits * 2) >= 8) splits *= 2;
+  while (splits < 8 && (g_fixed_splits || tiles * splits * 2 <= 2u * (uint32_t)sm_count()) && total_kb / (splits * 2) >= 8)
+    splits *= 2;
   const uint32_t kb_per_split = ceil_div_u32(total_kb, splits);
   splits = ceil_div_u32(total_kb, kb_per_split);
   cudaLaunchConfig_t cfg = {};

@@ -28,6 +28,7 @@ int cuda_fail(cudaError_t e, const char* what, const char* file, int line) {
 }
 
 int g_pdl = 0;
+int g_fixed_splits = 0;
 
 int sm_count() {
   static int n = -1;
@@ -107,6 +108,12 @@ int nv_abi_version(void) { return 1; }
 int nv_set_pdl(int on) {
   const int prev = nv::g_pdl;
   nv::g_pdl = on ? 1 : 0;
+  return prev;
+}
+
+int nv_set_fixed_splits(int on) {
+  const int prev = nv::g_fixed_splits;
+  nv::g_fixed_splits = on ? 1 : 0;
   return prev;
 }
 

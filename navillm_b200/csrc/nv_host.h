@@ -42,6 +42,10 @@ int sm_count();
 // cudaLaunchAttributeProgrammaticStreamSerialization (see griddep_wait / griddep_launch in nv_common.cuh).
 extern int g_pdl;
 
+// Batch-invariant split-K (nv_set_fixed_splits): when on, the panorama encoder GEMMs (nv_sgemm, nv_gemm_tf32) take a K split
+// count that depends on K alone, not on the tile count (the batch) or sm_count().
+extern int g_fixed_splits;
+
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args... args) {
   cudaLaunchConfig_t cfg = {};

@@ -448,10 +448,11 @@ int nv_sgemm(const float* A, int64_t lda, int ta, const float* B, int64_t ldb, i
   if (M == 0 || N == 0) return NV_OK;
   NV_REQUIRE(M > 0 && N > 0 && K > 0 && A && B && C, "nv_sgemm: bad arguments M=%d N=%d K=%d", M, N, K);
   dim3 grid((N + SG_BN - 1) / SG_BN, (M + SG_BM - 1) / SG_BM, 1);
-  // Encoder GEMMs are small (<= a few hundred tiles, K up to 4096): split K until ~3 CTAs per SM are in flight.
+  // Encoder GEMMs are small (<= a few hundred tiles, K up to 4096): split K until ~3 CTAs per SM are in flight (with
+  // g_fixed_splits: as far as K allows, whatever the tile count).
   const int tiles = grid.x * grid.y;
   int splits = 1;
-  while (splits < 8 && tiles * splits < 3 * sm_count() && K / (splits * 2) >= 256) splits *= 2;
+  while (splits < 8 && (g_fixed_splits || tiles * splits < 3 * sm_count()) && K / (splits * 2) >= 256) splits *= 2;
   int k_per_split = ((K + splits - 1) / splits + SG_BK - 1) / SG_BK * SG_BK;
   grid.z = (K + k_per_split - 1) / k_per_split;
   cudaLaunchConfig_t cfg = {};

@@ -42,6 +42,7 @@ class Decoding:
     scores: bool = False                     # return_dict_in_generate + output_scores: the step stores HF's per-step scores
     groups: int = 1                          # beams: num_beam_groups (diverse beam search when > 1)
     diversity_penalty: Optional[float] = None    # diverse beam search: the Hamming diversity penalty
+    batch_invariant: bool = False            # ModifiedLlamaForCausalLM.set_batch_invariant: the step runs other kernels
 
     @property
     def sampled(self) -> bool:
@@ -51,7 +52,7 @@ class Decoding:
         """The graph key: every field a captured step bakes in (not ``n_return`` or ``length_penalty``), the format last."""
         return (self.eos, self.pad, self.stop_on_eos, self.mode, self.temperature, self.top_k, self.top_p, self.trie_eos, self.n,
                 self.early_stopping, self.proc, self.penalty_alpha, self.lookup_k, self.lookup_ngram, self.scores, self.groups,
-                self.diversity_penalty, self.kv)
+                self.diversity_penalty, self.batch_invariant, self.kv)
 
 
 def processors(repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens, eos: int) -> Optional[tuple]:
@@ -252,7 +253,9 @@ def lm_head_rows(lm, hn: torch.Tensor, out: torch.Tensor) -> None:
     """lm_head of final-norm rows ``hn`` into ``out`` [rows, V] bf16 (the fp8 weight copy when there is one)."""
     B = hn.shape[0]
     fp8_head = lm._fp8.view([lm.lm_head.weight], tuple(lm.lm_head.weight.shape)) if lm.core.fp8 is not None else None
-    if B <= 16 and fp8_head is not None:
+    if lm.core.batch_invariant:
+        ops.gemm_bi(hn, lm.lm_head.weight.data, out=out)
+    elif B <= 16 and fp8_head is not None:
         ops.gemm_skinny_fp8(hn, *fp8_head, out=out)
     elif B <= llama_mod.FP8_MAX_ROWS and fp8_head is not None:
         ops.gemm_fp8w(hn, *fp8_head, out=out)

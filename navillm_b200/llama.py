@@ -610,6 +610,7 @@ class LlamaCore:
         self.int4 = None              # per-layer int4 weight triples (set_int4)
         self.int4_src = None
         self.act_fp8 = False          # W8A8 in the no-grad forwards (ModifiedLlamaForCausalLM.set_activation_dtype)
+        self.batch_invariant = False  # ModifiedLlamaForCausalLM.set_batch_invariant
         self.wgrad_stash: Optional[WgradStash] = None   # deferred linear weight gradients (defer_weight_grads)
         self.calibration: Optional[Int4Calibration] = None   # open GPTQ calibration: the forwards record their linear inputs
 
@@ -728,11 +729,14 @@ class LlamaCore:
     # its workspace.
     LAYER_CALL = True
 
-    def _fused(self, T: int, a8) -> bool:
+    def _fused(self, T: int, a8, save: bool = True) -> bool:
         """Whether a forward of T rows runs the fused-epilogue kernels (RoPE / SwiGLU in the 128 x 256-tile GEMM's epilogue).
         They need F % 128 == 0, D % 256 == 0 and at least one wave of tiles; W8A8 runs the plain GEMM and the RoPE / SwiGLU
-        row kernels instead."""
+        row kernels instead.  So does a no-grad forward (``save`` False) in batch-invariant mode, at every T: one form of
+        the layer whatever the batch."""
         d = self.d
+        if self.batch_invariant and not save:
+            return False
         return a8 is None and T >= 1024 and d.inter % 128 == 0 and d.hidden % 256 == 0
 
     def _layer_calls(self, x, pos, cu, seqlens, out_rows, a8, kc, vc, mode, Smax, Tkv=0, cached=None, kv_start=None,
@@ -825,7 +829,7 @@ class LlamaCore:
         exponents [B, Smax, H])`` pairs (``is_fp8_kv``); the prompt's own attention reads the unrounded K, V either way."""
         B, T, H = len(seqlens), x.shape[0], self.d.n_heads
         a8 = None if save else self.act_fp8_weights()       # W8A8 (set_activation_dtype("fp8")): no-grad forwards only
-        fused = self._fused(T, a8)
+        fused = self._fused(T, a8, save)
         kc, vc = kv_store if kv_store is not None else (None, None)
         fp8_kv = kc is not None and is_fp8_kv(kc)
         if self.LAYER_CALL and not save and not fused and self.calibration is None:
@@ -874,7 +878,7 @@ class LlamaCore:
         H, D = d.n_heads, d.hidden
         B, T = len(q_lens), x.shape[0]
         a8 = None if save else self.act_fp8_weights()       # W8A8 (set_activation_dtype("fp8")): no-grad forwards only
-        fused = self._fused(T, a8)
+        fused = self._fused(T, a8, save)
         fp8_kv = is_fp8_kv(kc)
         if save and (fp8_kv or acc is None or kv_lens is None):
             raise ValueError("forward_suffix(save=True) needs bf16 caches, the gradient accumulators and the host kv_lens")
@@ -1007,11 +1011,17 @@ class LlamaCore:
         # With an fp8 copy of the weights (set_fp8), the skinny GEMMs and, up to FP8_MAX_ROWS rows, nv_gemm_fp8w_bf16 stream
         # it instead: same bits as bf16 on W'.  With an int4 copy (set_int4), the skinny GEMMs stream it, and up to
         # INT4_MAX_ROWS rows nv_gemm_int4w_bf16 does for q|k|v; again the same bits.  generate() refuses a stale copy before it gets here.
-        skinny = x.shape[0] <= 16
+        # Batch-invariant mode (set_batch_invariant) streams every weight through nv_gemm_bi_bf16 at every batch size: one
+        # accumulation chain per element, no split-K, the SwiGLU fused (gemm_bi.cu).
+        inv = self.batch_invariant
+        skinny = x.shape[0] <= 16 and not inv
         fuse_mlp = skinny and d.inter % 64 == 0
-        f8 = self.fp8 if x.shape[0] <= FP8_MAX_ROWS else None
-        q4 = self.int4 if x.shape[0] <= INT4_MAX_ROWS else None
-        if q4 is not None and skinny:
+        f8 = self.fp8 if x.shape[0] <= FP8_MAX_ROWS and not inv else None
+        q4 = self.int4 if x.shape[0] <= INT4_MAX_ROWS and not inv else None
+        if inv:
+            wqkv, wo, wgu, wd = self.wqkv, self.wo, self.wgu, self.wd
+            lin = lambda a, w, addend=None: ops.gemm_bi(a, w, addend=addend)
+        elif q4 is not None and skinny:
             lin = lambda a, w, addend=None: ops.gemm_skinny_int4(a, *w, addend=addend)
             wqkv, wo, wgu, wd = q4.wqkv, q4.wo, q4.wgu, q4.wd
         elif q4 is not None:                                  # q|k|v from the int4 copy, the others bf16 (INT4_MAX_ROWS)
@@ -1050,7 +1060,9 @@ class LlamaCore:
                 ao = ops.decode_attn_rope(qkv, lens, self.cos, self.sin, kc[l], vc[l], H)   # RoPE + cache append + attention
             xm = lin(ao, wo[l], x)
             xn2, _ = ops.rmsnorm_fwd(xm, lyr.post_attention_layernorm.weight.data, d.rms_eps)
-            if q4 is not None and skinny:                                                # Int4Weights: F % 64 == 0
+            if inv:
+                h = ops.gemm_bi_swiglu(xn2, wgu[l])
+            elif q4 is not None and skinny:                                              # Int4Weights: F % 64 == 0
                 h = ops.gemm_skinny_swiglu_int4(xn2, *wgu[l])
             elif fuse_mlp and f8 is not None:
                 h = ops.gemm_skinny_swiglu_fp8(xn2, *wgu[l])

@@ -18,6 +18,7 @@ import contextlib
 import dataclasses
 import math
 import numbers
+import os
 import time
 import weakref
 from types import SimpleNamespace
@@ -156,7 +157,10 @@ class PackedPrompt:
         flat_rows = np.flatnonzero(msk.reshape(-1))                       # packed order == row-major order
         self.T = int(flat_rows.size)
         tok = ids.reshape(-1)[flat_rows]
-        if generate_positions:                                            # HF generate: cumsum(mask) - 1
+        # batch-invariant no-grad forwards take generate's positions too: arange(S) would move a left-padded prompt's rotary
+        # positions with the batch's longest prompt (the same attention up to the rounding of the cos/sin tables)
+        invariant = callable(getattr(lm, "invariant_inference", None)) and lm.invariant_inference()
+        if generate_positions or invariant:                               # HF generate: cumsum(mask) - 1
             pos = (np.cumsum(msk, axis=1) - 1).reshape(-1)[flat_rows]
         else:                                                             # plain forward: arange(S), pads included
             pos = np.tile(np.arange(S), B)[flat_rows]
@@ -403,8 +407,9 @@ def _reusable_prefix(old: np.ndarray, toks: np.ndarray, cand_id: int) -> int:
 
 
 def plan_prefix_reuse(ids: np.ndarray, msk: np.ndarray, cache: "PrefixKVCache", hist_counts, n_cand_total: int, cand_id: int,
-                      hist_id: int, cls_id: int):
-    """Host-side plan of one cached navigation step (pure numpy; updates ``cache.ids`` / ``cache.off``).
+                      hist_id: int, cls_id: int, invariant: bool = False):
+    """Host-side plan of one cached navigation step (pure numpy; updates ``cache.ids`` / ``cache.off``).  ``invariant``
+    (batch-invariant mode): a new row's rotary offset is 0 instead of its left padding.
 
     For every left-padded row: the reusable prefix = longest common token prefix with what the cache holds for the row, cut
     before the first <cand> token (candidates change every step) and at most L - 1 (the last token is always encoded).
@@ -423,8 +428,9 @@ def plan_prefix_reuse(ids: np.ndarray, msk: np.ndarray, cache: "PrefixKVCache", 
             raise ValueError("prefix reuse needs left-padded prompts with at least one token")
         if L > cache.max_len:
             raise ValueError(f"prompt of {L} tokens exceeds the prefix cache length {cache.max_len}")
-        if cache.off[b] is None:
-            cache.off[b] = S - L                               # the row keeps this rotary offset for the rollout
+        if cache.off[b] is None:                               # the row keeps this rotary offset for the rollout; in
+            # batch-invariant mode 0 (generate's positions), else the reference's S - L, which follows the longest prompt
+            cache.off[b] = 0 if invariant else S - L
         n = _reusable_prefix(cache.ids[b], toks, cand_id)
         new = toks[n:]
         is_h, is_c = new == hist_id, new == cand_id
@@ -484,7 +490,8 @@ class _LMFn(torch.autograd.Function):
         # ---- LM loss on the label rows only ----
         V = lm.lm_head.weight.shape[0]
         logits = generation.logits_buffer(g.shape[0], V, g.device)
-        ops.gemm(hn, lm.lm_head.weight.data, out=logits)                 # [Nl, V] bf16
+        head = ops.gemm_bi if lm.invariant_inference() else ops.gemm
+        head(hn, lm.lm_head.weight.data, out=logits)                     # [Nl, V] bf16
         row_loss, dlogits = ops.ce_fwd_bwd(logits, pp.loss_tgt, lm.special_ids_dev,
                                            grad_scale=(1.0 / max(pp.n_loss, 1)) if train else None)
         loss = row_loss.sum() / max(pp.n_loss, 1)
@@ -553,6 +560,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
         self.grad_sync.before_exchange = self.complete_pending_grads
         self._prefix_caches = weakref.WeakSet()      # PrefixKVCache(train=True) instances built on this model
         self._decode_states = generation.DecodeStates()  # generate()'s KV caches and captured decode graphs
+        self.batch_invariant = os.environ.get("NAVILLM_BATCH_INVARIANT", "") == "1"   # set_batch_invariant
         if tokenizer is not None:
             self._set_tokenizer(tokenizer)
 
@@ -626,6 +634,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
         self._lm_head_grad_clean = False             # unknown until the next zero_grad
         self.core = LlamaCore(self.dims, self.model, self.flat)
         self.core.act_fp8 = self.activation_dtype == "fp8"
+        self.core.batch_invariant = self.batch_invariant
         if self._wgrad_stash is not None:
             self._wgrad_stash.core = self.core
             self.core.wgrad_stash = self._wgrad_stash
@@ -723,7 +732,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
         if cache.train:
             cache._flush_shrinking(ids, msk, self.cand_token_id[0])
         plan = plan_prefix_reuse(ids, msk, cache, hist_counts, n_cand_total, self.cand_token_id[0], self.hist_token_id[0],
-                                 self.cls_token_id[0])
+                                 self.cls_token_id[0], invariant=self.invariant_inference())
         tok_new, pos_new, vis_new, q_lens, cached, kv_len, cls_rows = plan
         cu = np.concatenate([[0], np.cumsum(q_lens)])
         kv_start = np.arange(B, dtype=np.int64) * cache.max_len
@@ -804,7 +813,8 @@ class ModifiedLlamaForCausalLM(nn.Module):
             hidden = torch.zeros((pp.B * pp.S, self.dims.hidden), dtype=bf16, device=dev).index_copy(0, flat, hn)
             hidden = hidden.view(pp.B, pp.S, -1)
             if return_logits:
-                lg = ops.gemm(hn.detach().contiguous(), self.lm_head.weight.data)
+                head = ops.gemm_bi if self.invariant_inference() else ops.gemm
+                lg = head(hn.detach().contiguous(), self.lm_head.weight.data)
                 lg[:, self.special_token_ids] = float("-inf")
                 logits = torch.zeros((pp.B * pp.S, lg.shape[1]), dtype=bf16, device=dev).index_copy(0, flat, lg).view(pp.B, pp.S, -1)
         return LMOutput(loss=loss, logits=logits, past_key_values=None, hidden_states=hidden, attentions=None)
@@ -833,6 +843,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
         until this is called again (or ``drop_fp8_weights``); the no-grad forwards then run bf16 on the current weights.
         Returns the size of the copy in bytes.  Drops the int4 copy (``quantize_weights_int4``) if there is one; quantizing
         after that rounds its W' further."""
+        self._refuse_in_batch_invariant("quantize_weights_fp8()")
         self._ensure()
         self.drop_int4_weights()
         self.drop_fp8_weights()
@@ -919,6 +930,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
         The fp8 and int4 copies exclude each other: this drops the fp8 copy (``quantize_weights_fp8``), and quantizing to
         fp8 drops this one.  The roundings compose: after ``quantize_weights_fp8()`` the weights are the fp8 W', and this
         rounds that W' to 4 bits (and the other way round).  Returns the size of the copy in bytes."""
+        self._refuse_in_batch_invariant("quantize_weights_int4()")
         self._ensure()
         if calibration is not None:
             calibration.check(self.flat, damp)
@@ -968,10 +980,50 @@ class ModifiedLlamaForCausalLM(nn.Module):
         falls back to bf16.  Its effect on task metrics has not been measured."""
         if dtype not in ("bf16", "fp8"):
             raise ValueError(f"set_activation_dtype: 'bf16' or 'fp8' expected, got {dtype!r}")
+        if dtype == "fp8" and self.batch_invariant:
+            raise ValueError("set_activation_dtype('fp8'): batch-invariant mode is on, and W8A8 is not part of its "
+                             "arithmetic; call set_batch_invariant(False) first")
         prev, self.activation_dtype = self.activation_dtype, dtype
         if self.core is not None:
             self.core.act_fp8 = dtype == "fp8"
         return prev
+
+    # ---- opt-in batch-invariant inference ----
+    def set_batch_invariant(self, on: bool) -> bool:
+        """Batch-invariant inference: while on, a prompt's no-grad LM outputs -- hidden states and logits, ``generate()`` ids
+        and scores in the greedy, beam, group-beam, contrastive and prompt-lookup modes, ``score_answers`` -- are bitwise a
+        function of that prompt alone, not of the batch size, the other prompts, its position among them or padding.
+        Sampled modes keep HF's one RNG stream for the whole batch, so only their logits and scores are covered; a beam's
+        ``sequences_scores`` keep HF's normalisation by the padded length (exact at ``length_penalty=0``).  No-grad forwards
+        take generate's rotary positions (cumsum(mask) - 1) instead of arange(S), which moved with the longest prompt.
+        Every inference GEMM then accumulates each element in one fp32 chain over 64-deep k-blocks, in order, without split-K
+        (include/navillm_b200.h): decode steps and lm_head stream the weights through nv_gemm_bi_bf16 at every batch size,
+        and the no-grad forwards run the plain GEMM with the RoPE / SwiGLU row kernels at every row count.  Training is
+        unchanged.  Prefill need not equal decode, nor eager a graph replay.  The fp8 and int4 weight copies and fp8
+        activations are refused while it is on.  Returns the previous value; ``NAVILLM_BATCH_INVARIANT=1`` in the
+        environment makes it the default."""
+        on = bool(on)
+        if on and (self.fp8_weights is not None or self.int4_weights is not None or self.activation_dtype == "fp8"):
+            what = ("the fp8 weight copy (drop_fp8_weights())" if self.fp8_weights is not None else
+                    "the int4 weight copy (drop_int4_weights())" if self.int4_weights is not None else
+                    "fp8 activations (set_activation_dtype('bf16'))")
+            raise ValueError(f"set_batch_invariant(True): batch-invariant mode does not combine with {what}")
+        prev, self.batch_invariant = self.batch_invariant, on
+        if self.core is not None:
+            self.core.batch_invariant = on
+        return prev
+
+    def invariant_inference(self) -> bool:
+        """Whether batch-invariant mode governs the call being made: the mode is on and the call does not train (the
+        forwards' ``train = torch.is_grad_enabled() and self.training_enabled``).  The one predicate for the positions, the
+        heads, the prefix cache's offsets and the encoder's splits; inside the decoder stack the same decision arrives as
+        ``save`` (a forward saves its activations exactly when it trains)."""
+        return self.batch_invariant and not (torch.is_grad_enabled() and self.training_enabled)
+
+    def _refuse_in_batch_invariant(self, what: str) -> None:
+        if self.batch_invariant:
+            raise ValueError(f"{what}: batch-invariant mode is on, and the quantized weight copies are not part of its "
+                             f"arithmetic; call set_batch_invariant(False) first")
 
     # ---- opt-in deferred weight gradients of the decoder linears (WgradStash) ----
     _wgrad_stash: Optional[WgradStash] = None
@@ -1209,12 +1261,13 @@ class ModifiedLlamaForCausalLM(nn.Module):
         def result(cls, ids):
             return ids if not rd else cls(sequences=ids, **fields)
         if lookup:
-            dec = generation.Decoding(int(eos), int(pad), bool(stop_on_eos), "lookup", self.kv_cache_dtype, lookup_k=lookup,
+            dec = generation.Decoding(int(eos), int(pad), bool(stop_on_eos), "lookup", self.kv_cache_dtype,
+                                      batch_invariant=self.batch_invariant, lookup_k=lookup,
                                       lookup_ngram=ngram, scores=scores)
             return result(GreedySearchDecoderOnlyOutput, generation.lookup_decode(*call, dec, out_fields=fields))
         if contrastive:
-            dec = generation.Decoding(int(eos), int(pad), bool(stop_on_eos), "contrastive", self.kv_cache_dtype, top_k=int(top_k),
-                                      n=int(top_k), proc=proc, penalty_alpha=float(penalty_alpha), scores=scores)
+            dec = generation.Decoding(int(eos), int(pad), bool(stop_on_eos), "contrastive", self.kv_cache_dtype,
+                                      batch_invariant=self.batch_invariant, top_k=int(top_k), n=int(top_k), proc=proc, penalty_alpha=float(penalty_alpha), scores=scores)
             return result(ContrastiveSearchDecoderOnlyOutput, generation.contrastive_search(*call, dec, out_fields=fields))
         if num_beams > 1:
             table = None
@@ -1225,7 +1278,8 @@ class ModifiedLlamaForCausalLM(nn.Module):
                 if table is None:
                     raise NotImplementedError("generate(num_beams > 1) with a trie= that flatten_trie cannot represent: the host "
                                               "processors keep per-row state that reordering the beams would scramble")
-            dec = generation.Decoding(int(eos), int(pad), None, "beam", self.kv_cache_dtype, n=int(num_beams), n_return=n_seq,
+            dec = generation.Decoding(int(eos), int(pad), None, "beam", self.kv_cache_dtype,
+                                      batch_invariant=self.batch_invariant, n=int(num_beams), n_return=n_seq,
                                       length_penalty=float(length_penalty), early_stopping=bool(early_stopping), proc=proc,
                                       trie_eos=None if table is None else table.eos, scores=scores, groups=groups,
                                       diversity_penalty=float(diversity_penalty) if groups > 1 else None)
@@ -1241,7 +1295,7 @@ class ModifiedLlamaForCausalLM(nn.Module):
             flatten_ms = 1e3 * (time.perf_counter() - t0)
         sampling = dict(temperature=float(temperature), top_k=int(top_k), top_p=top_p) if do_sample else {}
         dec = generation.Decoding(int(eos), int(pad), bool(stop_on_eos), "sample" if do_sample else "greedy", self.kv_cache_dtype,
-                                  n=max(1, n_seq), proc=proc, scores=scores, **sampling)
+                                  batch_invariant=self.batch_invariant, n=max(1, n_seq), proc=proc, scores=scores, **sampling)
         if table is not None:
             rng = torch.cuda.get_rng_state(dev) if do_sample else None
             trie_dec = dataclasses.replace(dec, mode="trie+sample" if do_sample else "trie", trie_eos=table.eos)
@@ -1303,5 +1357,5 @@ class ModifiedLlamaForCausalLM(nn.Module):
             raise NotImplementedError("score_answers: the trie shares a node between two parents; answer scoring needs a tree")
         eos = self.tokenizer.eos_token_id
         dec = generation.Decoding(int(eos), int(self.tokenizer.unk_token_id), True, "trie_score", self.kv_cache_dtype,
-                                  trie_eos=table.eos)
+                                  batch_invariant=self.batch_invariant, trie_eos=table.eos)
         return generation.score_answers(self, input_ids, attention_mask, (cand_vis, hist_vis, obj_vis), rows, lp, stats, dec)

@@ -275,6 +275,15 @@ class NavModel(nn.Module):
         (default) or ``"fp8"``; see ``ModifiedLlamaForCausalLM.set_kv_cache_dtype``.  Returns the previous format."""
         return self.lang_model.set_kv_cache_dtype(dtype)
 
+    def set_batch_invariant(self, on: bool) -> bool:
+        """Batch-invariant inference (``ModifiedLlamaForCausalLM.set_batch_invariant``): while on, an episode's outputs of a
+        call that does not train -- the panorama encoder's, ``fuse_logits`` / ``obj_logits`` of the navigation and grounding
+        modes with or without a ``PrefixKVCache``, generation and answer scores -- are bitwise a function of that episode
+        alone.  The encoder GEMMs then split K by K alone (``ops.fixed_splits``).  The navigation mode's candidate shuffle
+        draws one CPU randperm per episode from one RNG stream, as the reference does; the mode keeps that stream, so an
+        episode's candidate order, like a sampled token, follows its row.  Returns the previous value."""
+        return self.lang_model.set_batch_invariant(on)
+
     def set_activation_dtype(self, dtype: str) -> str:
         """Number format of the language model's decoder-layer GEMM inputs in no-grad forwards: ``"bf16"`` (default) or
         ``"fp8"`` (W8A8 after ``quantize_weights_fp8()``); see ``ModifiedLlamaForCausalLM.set_activation_dtype``.  Returns the
@@ -366,6 +375,12 @@ class NavModel(nn.Module):
     # ---------------------------------------------------------------------------------------------------
     def forward(self, mode: str, batch: Dict[str, Any], **kwargs) -> Dict[str, Any]:
         self._ensure()
+        if self.lang_model.invariant_inference():
+            with ops.fixed_splits():                 # the encoder's split-K by K alone (set_batch_invariant)
+                return self._forward(mode, batch, **kwargs)
+        return self._forward(mode, batch, **kwargs)
+
+    def _forward(self, mode: str, batch: Dict[str, Any], **kwargs) -> Dict[str, Any]:
         batch = collections.defaultdict(lambda: None, batch)
         if mode == "panorama":                       # models/nav_model.py:99-111
             batch["view_img_fts"] = self.drop_env(batch["view_img_fts"])

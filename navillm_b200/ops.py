@@ -1392,6 +1392,21 @@ class LayerRunner:
         return y
 
 
+class fixed_splits:
+    """Context: the panorama encoder GEMMs (``sgemm``) split K by K alone (nv_set_fixed_splits), so that a row's bits do not
+    depend on the batch; used by ``NavModel`` in batch-invariant mode."""
+
+    def __init__(self, on: bool = True):
+        self.on = on
+
+    def __enter__(self):
+        self.prev = _lib.load().nv_set_fixed_splits(i32(1 if self.on else 0))
+        return self
+
+    def __exit__(self, *a):
+        _lib.load().nv_set_fixed_splits(i32(self.prev))
+
+
 class pdl:
     """Context: launch the decode-chain kernels with programmatic dependent launch (nv_set_pdl)."""
 
@@ -1498,6 +1513,52 @@ def gemm_skinny_swiglu(x: torch.Tensor, wgu: torch.Tensor, *, out: torch.Tensor 
         out = torch.empty((M, F), dtype=bf16, device=x.device)
     check(_lib.load().nv_gemm_skinny_swiglu_bf16(ptr(x), i64(x.stride(0)), ptr(wgu), i64(wgu.stride(0)), ptr(out), i64(out.stride(0)),
                                                  i32(M), i32(F), i32(K), stream_ptr()), "nv_gemm_skinny_swiglu_bf16")
+    return out
+
+
+BI_MAX_ROWS = 128           # batch-invariant linears: the weight-streaming kernel up to here, nv_gemm_bf16 above
+
+
+def gemm_bi(x: torch.Tensor, w: torch.Tensor, *, addend: torch.Tensor | None = None,
+            out: torch.Tensor | None = None) -> torch.Tensor:
+    """Batch-invariant linear: x [M, K] bf16, w [N, K] bf16 (nn.Linear weight) -> bf16 [M, N] (+ addend), each row's bits a
+    function of that row alone.  Up to ``BI_MAX_ROWS`` rows the weight-streaming kernel nv_gemm_bi_bf16 (csrc/gemm_bi.cu),
+    above it ``gemm``: the same accumulation chain per element (include/navillm_b200.h)."""
+    _rowmajor(x, "x"); _rowmajor(w, "w")
+    M, K = x.shape
+    N = w.shape[0]
+    if x.dtype != bf16 or w.dtype != bf16 or w.shape[1] != K or M == 0:
+        raise ValueError(f"gemm_bi: x {x.dtype} {tuple(x.shape)} w {w.dtype} {tuple(w.shape)} (bf16, M > 0, matching K)")
+    if M > BI_MAX_ROWS:
+        return gemm(x, w, addend=addend, out=out)
+    if out is None:
+        out = torch.empty((M, N), dtype=bf16, device=x.device)
+    _rowmajor(out, "out")
+    if out.shape != (M, N) or out.dtype != bf16:
+        raise ValueError(f"gemm_bi: out bf16 [{M}, {N}] expected (got {out.dtype} {tuple(out.shape)})")
+    if addend is not None:
+        _rowmajor(addend, "addend")
+        if addend.shape != (M, N) or addend.dtype != bf16:
+            raise ValueError(f"gemm_bi: addend bf16 [{M}, {N}] expected (got {addend.dtype} {tuple(addend.shape)})")
+    check(_lib.load().nv_gemm_bi_bf16(ptr(x), i64(x.stride(0)), ptr(w), i64(w.stride(0)), ptr(out), i64(out.stride(0)),
+                                      ptr(addend), i64(addend.stride(0) if addend is not None else 0),
+                                      i32(M), i32(N), i32(K), stream_ptr()), "nv_gemm_bi_bf16")
+    return out
+
+
+def gemm_bi_swiglu(x: torch.Tensor, wgu: torch.Tensor) -> torch.Tensor:
+    """Batch-invariant gate|up projection + SwiGLU: x [M, K], wgu [2F, K] -> h [M, F] bf16, bit for bit
+    ``swiglu_fwd(gemm_bi(x, wgu))``.  Up to ``BI_MAX_ROWS`` rows with F % 16 == 0 one kernel (gate|up never materialised)."""
+    _rowmajor(x, "x"); _rowmajor(wgu, "wgu")
+    M, K = x.shape
+    F = wgu.shape[0] // 2
+    if x.dtype != bf16 or wgu.dtype != bf16 or wgu.shape[1] != K or wgu.shape[0] % 2 or M == 0:
+        raise ValueError(f"gemm_bi_swiglu: x {x.dtype} {tuple(x.shape)} wgu {wgu.dtype} {tuple(wgu.shape)}")
+    if M > BI_MAX_ROWS or F % 16:
+        return swiglu_fwd(gemm_bi(x, wgu))
+    out = torch.empty((M, F), dtype=bf16, device=x.device)
+    check(_lib.load().nv_gemm_bi_swiglu_bf16(ptr(x), i64(x.stride(0)), ptr(wgu), i64(wgu.stride(0)), ptr(out), i64(out.stride(0)),
+                                             i32(M), i32(F), i32(K), stream_ptr()), "nv_gemm_bi_swiglu_bf16")
     return out
 
 
